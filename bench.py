@@ -67,6 +67,9 @@ def parse_args():
     ap.add_argument("--expert-dtype", choices=["bf16", "fp8"], default="bf16",
                     help="fp8 = forward expert GEMMs on block-scaled FP8 tensor cores (MXFP8)")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (its loss, the loss of every timed "
+                         "step, a fixed sample of the updated parameters) as DIR/<name>.npy, float32")
     return ap.parse_args()
 
 
@@ -351,6 +354,7 @@ def _measure_ours(args, rank, world, local_rank, B, path="auto", tag="named", st
                      tokens_per_rank=B, capacity_factor=capacity, failure_rate=args.failure_rate,
                      gate_mode=args.gate, shadow_experts=args.shadow_experts, shadow_tol=args.shadow_tol,
                      expert_dtype=args.expert_dtype, expert_path=path)
+    torch.manual_seed(4321 + rank)   # same weights on every run: outputs of two builds can be compared one to one
     trainer = DMoETrainer(cfg, use_graph=False if args.no_graph else None)
     n_batches = 4
     xs_host, ys_host = synthetic_mnist(B, n_batches, seed=1234 + rank, in_features=cfg.in_features)
@@ -411,6 +415,8 @@ def _measure_ours(args, rank, world, local_rank, B, path="auto", tag="named", st
     exposed_ranks = gather_ranks(exposed_local, world)   # the rank with the SMALLEST wait is the step's straggler
     clocks = sampler.stop()
     check_all_ranks()
+    if args.dump_outputs and tag == "named":
+        dump_outputs(args.dump_outputs, trainer, dev_losses[-steps:], rank)
     global_batch = B * world
     value = global_batch * steps / (ms / 1e3)
     loss_curve = [float(t) for t in torch.cat(dev_losses).cpu()]
@@ -450,7 +456,7 @@ def _measure_ours(args, rank, world, local_rank, B, path="auto", tag="named", st
     # step roofline in the weight-streaming regime: every ACTIVE expert streams its bf16 weights twice (forward, dgrad) and
     # its fp32 optimizer state once (34 B / parameter with the fused wgrad+AMSGrad kernel); rank 0's share
     per_expert = sum(int(torch.tensor(s).prod()) for s in cfg.seg_shapes().values())
-    hbm = float(_peaks().get("hbm_gbs", 6650.0))
+    hbm = float(_peaks().get("hbm_gbs", 3350.0))   # H100 SXM data sheet
     ideal_ms = active_total * per_expert * (2 + 2 + 34) / (hbm * 1e9) * 1e3
     out = None
     result = {
@@ -463,20 +469,20 @@ def _measure_ours(args, rank, world, local_rank, B, path="auto", tag="named", st
                    "global_batch": global_batch, "batch_per_gpu": B, "trainers_x_batch": "64 x 4 per GPU" if B == 256 else None,
                    "seq_len": 1, "parallelism": f"ep{world}+dp{world}",
                    "expert_path": "small (swap-AB weight streaming, fused wgrad+AMSGrad, CUDA graph)" if trainer.ctx.small
-                   else "big (CTA-pair 256x256 tiles)",
+                   else "big (128x256 wgmma tiles)",
                    "cuda_graph": bool(trainer.use_graph),
                    "capacity_factor": capacity, "shadow_experts": trainer.ctx.S, "shadow_tol": cfg.shadow_tol,
                    "expert_gemm_dtype": cfg.expert_dtype + (" forward, bf16 dgrad/wgrad" if cfg.expert_dtype == "fp8" else ""),
                    "experts_total": cfg.num_experts * cfg.num_layers, "failure_rate": cfg.failure_rate,
                    "gate": cfg.gate_mode + (" (LayerNorm(x) @ normalize(keys); gate params not trained, exactly like the reference's EmulatedDMoE)" if cfg.gate_mode == "emulator" else " (trainable product-key proj, lib.GatingFunction)"),
-                   "l2_policy": "working set per step (optimizer state + weights of the active experts, >10 GB) exceeds the 126 MB L2; no explicit flush"},
+                   "l2_policy": "working set per step (optimizer state + weights of the active experts, >10 GB) exceeds the 50 MB L2; no explicit flush"},
         "clocks": clocks, "gpu_launches": launches, "e2e": e2e, "routing_rank0": routing,
         "exposed_comm_wait_ms_per_step": exposed_ms, "exposed_comm_wait_ms_per_rank": exposed_ranks,
         "hottest_expert_rows_per_layer": hottest, "stage_ms_rank0": stage_ms,
         "loss_first_last": [loss_curve[0], loss_curve[-1]] if loss_curve else None,
         "roofline": {"active_experts_rank0": active_total, "ideal_ms_hbm_bound_rank0": round(ideal_ms, 3),
                      "frac_of_measured_copy": round(ideal_ms / (ms / steps), 3) if trainer.ctx.small else None,
-                     "note": "38 B per parameter of every active expert at the MEASURED copy bandwidth"},
+                     "note": "38 B per parameter of every active expert at hbm_gbs of MEASURED_PEAKS.json if present, else the 3.35 TB/s data sheet"},
         "baseline_note": "vs_baseline = value / 16.8 samples/s (reference notebook dmoe64x4, BASELINE.md)",
     }
     trainer.close()
@@ -484,6 +490,29 @@ def _measure_ours(args, rank, world, local_rank, B, path="auto", tag="named", st
     gc.collect()
     torch.cuda.empty_cache()
     return result
+
+
+def dump_outputs(out_dir, trainer, step_losses, rank):
+    """What the timed path handed back and left behind in its last step, as float32 .npy files (a few MB in all):
+    loss (the last step's loss), losses (every timed step), and a fixed, seeded sample of 65536 entries of every updated
+    parameter group (each expert layer's fp32 master weights, the trainer's dense parameters)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    suffix = f"_rank{rank}" if rank else ""
+    losses = torch.cat(step_losses).float().cpu().numpy()
+    arrays = {"loss": losses[-1:], "losses": losses}
+    gen = torch.Generator().manual_seed(99)
+    for i, block in enumerate(trainer.model.blocks):
+        p = block.shard.p.detach().float().flatten()
+        idx = torch.randint(0, p.numel(), (min(65536, p.numel()),), generator=gen).to(p.device)
+        arrays[f"layer{i}_expert_params_sample"] = p[idx].cpu().numpy()
+    for name in ("stem", "norm", "head"):
+        mod = getattr(trainer.model, name, None)
+        if mod is not None:
+            for pname, t in mod.named_parameters():
+                arrays[f"{name}_{pname}"] = t.detach().float().cpu().numpy()
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + suffix + ".npy"), a.astype(np.float32))
 
 
 DATA_STR = "synthetic (MNIST-shaped 784-d fp32 rows: 10 Gaussian class prototypes + noise, learnable; random-init weights)"

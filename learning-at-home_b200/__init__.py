@@ -1,11 +1,11 @@
 """
-lah_b200 — a Blackwell-native Decentralized Mixture-of-Experts engine with the public API of mryab/learning-at-home.
+lah_b200 — a Hopper-native Decentralized Mixture-of-Experts engine with the public API of mryab/learning-at-home.
 
     import lah_b200 as lib                      # or `import lib` (compat alias at the repository root)
     lib.RemoteExpert, lib.GatingFunction        # trainer side           (client/)
     lib.TesseractServer, lib.ExpertBackend      # expert server          (server/, runtime/)
     lib.TesseractNetwork, lib.InBoxNetwork      # discovery              (network/)
-    lib.DMoETrainer, lib.DMoEConfig, lib.FusedDMoE   # sm_100a in-box engine (parallel/)
+    lib.DMoETrainer, lib.DMoEConfig, lib.FusedDMoE   # sm_90a in-box engine (parallel/)
 
 See README.md and DESIGN.md.
 """

@@ -1,7 +1,7 @@
 """
 Builds the native parts of the framework IN-TREE (so the shared objects travel with a repo snapshot):
 
-  _C/liblah_cuda.so   every .cu under csrc/  -> nvcc -gencode arch=compute_100a,code=sm_100a (sm_100a ONLY)
+  _C/liblah_cuda.so   every .cu under csrc/  -> nvcc -gencode arch=compute_90a,code=sm_90a (sm_90a ONLY)
   _C/liblah_host.so   every .cpp under csrc/ -> g++ (C++ host runtime: batching queue, framing, DHT routing table)
 
 Both expose a plain C ABI and are loaded with ctypes (see ops/native.py); there is deliberately no dependency on
@@ -19,7 +19,7 @@ CSRC = ROOT / "csrc"
 OUT = ROOT / "_C"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--use_fast_math", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default",
 ]
 GXX_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-shared", "-pthread", "-Wall"]

@@ -7,7 +7,7 @@ Two execution paths behind one module:
 
 * **fused in-box path** — when ``network`` is bound to an in-box engine layer (``network.fused_layer``, see
   ``lah_b200.parallel.engine.FusedDMoE``) and the input lives on that GPU, the whole layer (top-k, dispatch, expert FFN,
-  combine; and their backward + expert optimizer) runs in the sm_100a kernels; ``self.proj`` is the gate in both paths.
+  combine; and their backward + expert optimizer) runs in the sm_90a kernels; ``self.proj`` is the gate in both paths.
 * **generic path** — any ``TesseractNetwork``-like object + ``RemoteExpert`` RPCs.  Same results as the reference, but
   rows are grouped PER EXPERT: one forward RPC per chosen expert carrying all of its rows (the reference issues one RPC
   per (sample, expert) with a single row and relies on the server to re-batch).  Fault tolerance is unchanged: experts
@@ -63,7 +63,7 @@ class GatingFunction(nn.Module):
         fused = getattr(self.network, "fused_layer", None)
         if fused is not None and input.is_cuda and not args and not kwargs:
             # in-box fast path (InBoxNetwork.bind_engine): liveness comes from the device-resident heartbeat table, the whole
-            # layer runs in the sm_100a kernels; k_min / timeout_after_k_min map to DMoEConfig.peer_timeout_ms
+            # layer runs in the sm_90a kernels; k_min / timeout_after_k_min map to DMoEConfig.peer_timeout_ms
             self.network.sync_alive(force=False)
             return fused.forward_with_gate(input, self.proj)
 

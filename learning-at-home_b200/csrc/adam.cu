@@ -11,7 +11,7 @@
 // Replicated (trainer-side) parameters: `peer_grad_off >= 0` makes the kernel read the gradient of every rank from the
 // symmetric heap (P2P loads over NVLink) and average them before the update, so the data-parallel gradient reduce and
 // the optimizer are one kernel; every rank computes the bit-identical sum in the same order.
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace lah {
 
@@ -193,7 +193,7 @@ int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_b
     const long long span = a.num_ranges ? a.r_cum[a.num_ranges] : a.total;
     if (span <= 0) return 0;
     long long blocks = (span / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     adam_kernel<<<(int)blocks, 256, 0, st>>>(a);
     return -(int)cudaGetLastError();
 }
@@ -207,7 +207,7 @@ int lah_cast_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
     if (n % 4) return -2;
     if (n <= 0) return 0;
     long long blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     cast_bf16_kernel<<<(int)blocks, 256, 0, st>>>(src, (bf16*)dst, n);
     return -(int)cudaGetLastError();
 }

@@ -1,17 +1,16 @@
-// attention.cu — tcgen05 self-attention for the transformer expert (d_model 1024, 16 heads x 64, seq 512;
-// reference: nn.MultiheadAttention inside /root/reference/experiments/throughput/layers.py:22-51).
+// attention.cu — wgmma self-attention for the transformer expert (d_model 1024, 16 heads x 64, seq 512;
+// reference: nn.MultiheadAttention inside experiments/throughput/layers.py:22-51).
 //
-// FORWARD (this file): ping-pong flash attention.  One CTA owns a PAIR of 128-query tiles of one (batch, head); K / V stream
-// through a 2-stage TMA pipeline in 128-key blocks shared by both tiles; warps 0-3 / 4-7 are the softmax groups of the two
-// tiles (thread = query row: the 128 scores of a block are read from TMEM once and stay in registers), warp 8 issues
-// tcgen05.mma, warp 9 drives TMA; while one group turns S_j into P_j the tensor core works for the other; online softmax
-// with the running output O in TMEM, rescaled in place (tcgen05.ld -> mul -> tcgen05.st) only when the row maximum grew by
-// more than 2^8 (lazy rescale).  S and P never touch HBM.  The kernel also emits the row log-sum-exp (base 2) that the
+// FORWARD (this file): flash attention.  One CTA owns one 128-query tile of one (batch, head); two consumer warpgroups own
+// 64 query rows each.  K / V stream through a 2-stage TMA pipeline in 128-key blocks; per block S = Q K^T is computed by
+// wgmma into registers, the online softmax runs on those registers (a row is spread over the 4 lanes of a quad), and the
+// bf16 probabilities are fed straight from registers as the A operand of O += P V (their accumulator layout IS the A
+// fragment layout).  S and P never touch shared memory or HBM.  The kernel also emits the row log-sum-exp (base 2) that the
 // BACKWARD kernel (attention_bwd.cu) needs to recompute P without a second softmax pass.
 //
 // Input : qkv [T = batch*512, 3*D] bf16 (output of the fused in_proj GEMM: [q | k | v] per token, heads contiguous)
 // Output: out [T, D] bf16 (heads concatenated, ready for out_proj); lse2 [T, heads] fp32 (optional)
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include <stdlib.h>
 
 namespace lah {
@@ -25,32 +24,15 @@ namespace v2 {
 
 constexpr int KB = 128;                       // keys per block
 constexpr int NUM_KB = S_LEN / KB;            // 4
-constexpr int NUM_THREADS2 = 320;
+constexpr int NUM_THREADS2 = 256;             // two consumer warpgroups; thread 0 also drives TMA
 constexpr int TILE_BYTES = 128 * HEAD_DIM * 2;            // 16 KB: a 128 x 64 bf16 tile (Q tile, K block, V block)
-constexpr int P_BYTES = Q_TILE * KB * 2;                  // 32 KB per query tile
-constexpr int OFF_Q2 = 0;                                 // Q_A, Q_B
-constexpr int OFF_K2 = OFF_Q2 + 2 * TILE_BYTES;           // 2 stages
-constexpr int OFF_V2 = OFF_K2 + 2 * TILE_BYTES;
-constexpr int OFF_P2 = OFF_V2 + 2 * TILE_BYTES;           // P_A, P_B
-constexpr int OFF_BAR2 = OFF_P2 + 2 * P_BYTES;
-constexpr int NUM_BARS = 1 + 8 + 8;
+constexpr int OFF_Q2 = 0;
+constexpr int OFF_K2 = OFF_Q2 + TILE_BYTES;               // 2 stages
+constexpr int OFF_V2 = OFF_K2 + 2 * TILE_BYTES;           // 2 stages
+constexpr int OFF_BAR2 = OFF_V2 + 2 * TILE_BYTES;
+constexpr int NUM_BARS = 1 + 2;
 constexpr int SMEM_TOTAL2 = OFF_BAR2 + NUM_BARS * 8 + 16 + 1024;
-constexpr int COL_S = 0, COL_O = 256;
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// (320 threads x 200 registers did not launch (cudaErrorLaunchOutOfResources); the launch-bounds build uses 168)
 __global__ void __launch_bounds__(NUM_THREADS2, 1)
 attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, float* __restrict__ lse2,
                         int d_model, int num_heads, float scale_log2e) {
@@ -58,218 +40,107 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR2);
     uint64_t* bar_q = bars;
-    uint64_t* k_full = bars + 1;    // [2]
-    uint64_t* k_empty = bars + 3;   // [2]
-    uint64_t* v_full = bars + 5;    // [2]
-    uint64_t* v_empty = bars + 7;   // [2]
-    uint64_t* s_full = bars + 9;    // [2 tiles]  MMA -> softmax
-    uint64_t* s_free = bars + 11;   // [2 tiles]  softmax (128 threads) -> MMA
-    uint64_t* p_full = bars + 13;   // [2 tiles]  softmax (128 threads) -> MMA
-    uint64_t* pv_done = bars + 15;  // [2 tiles]  MMA -> softmax
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + NUM_BARS);
+    uint64_t* kv_full = bars + 1;   // [2]
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int qpair = blockIdx.x & 1;
-    const int head = (blockIdx.x >> 1) % num_heads;
-    const int batch = (blockIdx.x >> 1) / num_heads;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+    const int qt = blockIdx.x & 3;
+    const int head = (blockIdx.x >> 2) % num_heads;
+    const int batch = (blockIdx.x >> 2) / num_heads;
     const int seq_row0 = batch * S_LEN;
 
-    if (warp == 9 && lane == 0) {
+    auto load_kv = [&](int j) {   // thread 0 only; stage j & 1 must be free
+        const int st = j & 1;
+        mbar_arrive_expect_tx(&kv_full[st], 2 * TILE_BYTES);
+        tma_load_2d(smem + OFF_K2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], d_model + head * HEAD_DIM, seq_row0 + j * KB);
+        tma_load_2d(smem + OFF_V2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], 2 * d_model + head * HEAD_DIM, seq_row0 + j * KB);
+    };
+    if (tid == 0) {
         tma_prefetch_desc(&tm_qkv);
         mbar_init(bar_q, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&k_full[i], 1);
-            mbar_init(&k_empty[i], 1);
-            mbar_init(&v_full[i], 1);
-            mbar_init(&v_empty[i], 1);
-            mbar_init(&s_full[i], 1);
-            mbar_init(&s_free[i], 128);
-            mbar_init(&p_full[i], 128);
-            mbar_init(&pv_done[i], 1);
-        }
+        mbar_init(&kv_full[0], 1);
+        mbar_init(&kv_full[1], 1);
         fence_mbar_init();
+        mbar_arrive_expect_tx(bar_q, TILE_BYTES);
+        tma_load_2d(smem + OFF_Q2, &tm_qkv, bar_q, head * HEAD_DIM, seq_row0 + qt * Q_TILE);
+        load_kv(0);
+        load_kv(1);
     }
-    if (warp == 8) tmem_alloc(tmem_ptr, 512);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 9) {
-        if (lane == 0) {
-            // ------------------------------------------------------------------ TMA producer
-            mbar_arrive_expect_tx(bar_q, 2 * TILE_BYTES);
-            tma_load_2d(smem + OFF_Q2, &tm_qkv, bar_q, head * HEAD_DIM, seq_row0 + (2 * qpair) * Q_TILE);
-            tma_load_2d(smem + OFF_Q2 + TILE_BYTES, &tm_qkv, bar_q, head * HEAD_DIM, seq_row0 + (2 * qpair + 1) * Q_TILE);
-            for (int j = 0; j < NUM_KB; ++j) {
-                const int st = j & 1;
-                const uint32_t par = ((j >> 1) & 1) ^ 1;
-                mbar_wait(&k_empty[st], par);
-                mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
-                tma_load_2d(smem + OFF_K2 + st * TILE_BYTES, &tm_qkv, &k_full[st], d_model + head * HEAD_DIM, seq_row0 + j * KB);
-                mbar_wait(&v_empty[st], par);
-                mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
-                tma_load_2d(smem + OFF_V2 + st * TILE_BYTES, &tm_qkv, &v_full[st], 2 * d_model + head * HEAD_DIM, seq_row0 + j * KB);
-            }
-        }
-    } else if (warp == 8) {
-        if (lane == 0) {
-            // ------------------------------------------------------------------ MMA issuer
-            constexpr uint32_t idesc_s = make_idesc_bf16_f32(Q_TILE, KB, 0u, 0u);
-            constexpr uint32_t idesc_o = make_idesc_bf16_f32(Q_TILE, HEAD_DIM, 0u, 1u);
-            const uint32_t sq = smem_u32(smem + OFF_Q2), sk = smem_u32(smem + OFF_K2), sv = smem_u32(smem + OFF_V2),
-                           sp = smem_u32(smem + OFF_P2);
-            auto issue_s = [&](int t, int j) {
-                const uint32_t a = sq + t * TILE_BYTES, b = sk + (j & 1) * TILE_BYTES;
+    const uint32_t sq = smem_u32(smem + OFF_Q2) + wg * (64 * 128);   // this warpgroup's 64 query rows
+    float o[HEAD_DIM / 2];
 #pragma unroll
-                for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
-                    umma_bf16_ss(tmem_base + COL_S + t * KB, make_smem_desc_sw128(a + ks * 32, 0, 1024),
-                                 make_smem_desc_sw128(b + ks * 32, 0, 1024), idesc_s, ks > 0 ? 1u : 0u);
-                umma_commit(&s_full[t]);
-            };
-            mbar_wait(bar_q, 0);
-            mbar_wait(&k_full[0], 0);
-            tcgen05_fence_after();
-            issue_s(0, 0);
-            issue_s(1, 0);
-            umma_commit(&k_empty[0]);
-            for (int j = 0; j < NUM_KB; ++j) {
-                const int st = j & 1;
-                for (int t = 0; t < 2; ++t) {
-                    if (j + 1 < NUM_KB) {   // S of the NEXT block first: the softmax warps hold S_t(j) in registers already
-                        if (t == 0) mbar_wait(&k_full[(j + 1) & 1], ((j + 1) >> 1) & 1);
-                        mbar_wait(&s_free[t], j & 1);
-                        tcgen05_fence_after();
-                        issue_s(t, j + 1);
-                        if (t == 1) umma_commit(&k_empty[(j + 1) & 1]);
-                    }
-                    mbar_wait(&p_full[t], j & 1);
-                    if (t == 0) mbar_wait(&v_full[st], (j >> 1) & 1);
-                    tcgen05_fence_after();
-                    const uint32_t a = sp + t * P_BYTES, b = sv + st * TILE_BYTES;
-#pragma unroll
-                    for (int kb = 0; kb < KB / 64; ++kb) {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks)
-                            umma_bf16_ss(tmem_base + COL_O + t * HEAD_DIM,
-                                         make_smem_desc_sw128(a + kb * (Q_TILE * 128) + ks * 32, 0, 1024),
-                                         make_smem_desc_sw128(b + (kb * 64 + ks * 16) * 128, 0, 1024), idesc_o,
-                                         (j | kb | ks) ? 1u : 0u);
-                    }
-                    umma_commit(&pv_done[t]);
-                    if (t == 1) umma_commit(&v_empty[st]);
-                }
-            }
-        }
-    } else {
-        // ---------------------------------------------------------------------- softmax + epilogue: thread = query row
-        const int t = warp >> 2;                 // query tile of the pair
-        const int row = (warp & 3) * 32 + lane;  // row inside the tile == TMEM lane
-        const uint32_t lane_base = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-        const uint32_t ts = lane_base + COL_S + t * KB, to = lane_base + COL_O + t * HEAD_DIM;
-        uint8_t* pbase = smem + OFF_P2 + t * P_BYTES;
-        // m = the reference maximum the probabilities are currently expressed against (raw score units).  LAZY rescale:
-        // m only moves when the row maximum grew by more than 8 / scale_log2e, i.e. probabilities stay below 2^8 — exact
-        // after the final division by l, and the TMEM round trip of O (ld -> mul -> st) is skipped for most blocks.
-        float m = -INFINITY, l = 0.f;
-        const float lazy_margin = 8.f / scale_log2e;
+    for (int i = 0; i < HEAD_DIM / 2; ++i) o[i] = 0.f;
+    // m = running row maximum (raw score units), l = this thread's share of the row sum (reduced over the quad at the end)
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    mbar_wait(bar_q, 0);
 #pragma unroll 1
-        for (int j = 0; j < NUM_KB; ++j) {
-            mbar_wait(&s_full[t], j & 1);
-            tcgen05_fence_after();
-            uint32_t r[KB / 32][32];   // the whole 128-score row of this block: one pass over TMEM
+    for (int j = 0; j < NUM_KB; ++j) {
+        const int st = j & 1;
+        mbar_wait(&kv_full[st], (j >> 1) & 1);
+        const uint32_t sk = smem_u32(smem + OFF_K2 + st * TILE_BYTES), sv = smem_u32(smem + OFF_V2 + st * TILE_BYTES);
+        float s[KB / 2];
+        wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < KB / 32; ++c) tmem_ld_32x32(ts + c * 32, r[c]);
-            tmem_ld_wait();
-            tcgen05_fence_before();
-            mbar_arrive(&s_free[t]);   // S_t is in registers: the issuer may already compute the next block's S_t
-            // 8 independent max chains (a single 128-deep fmaxf chain is 128 x the ALU latency on the critical path)
-            float mxs8[8];
+        for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
+            wgmma_bf16_n128<0, 0>(s, make_smem_desc_sw128(sq + ks * 32, 0, 1024), make_smem_desc_sw128(sk + ks * 32, 0, 1024),
+                                  ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        uint32_t pa[KB / 16][4];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) mxs8[i] = -INFINITY;
+        for (int h = 0; h < 2; ++h) {
+            float mx = -INFINITY;
 #pragma unroll
-            for (int c = 0; c < KB / 32; ++c)
+            for (int jj = 0; jj < KB / 8; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m[h], mx);
+            const float alpha = exp2f((m[h] - m_new) * scale_log2e);   // j == 0: m = -inf -> 0 (O and l are 0 then)
+            m[h] = m_new;
+            const float ms = m_new * scale_log2e;
+            float sum = 0.f;
 #pragma unroll
-                for (int i = 0; i < 32; ++i) mxs8[i & 7] = fmaxf(mxs8[i & 7], __uint_as_float(r[c][i]));
-            const float mx = fmaxf(fmaxf(fmaxf(mxs8[0], mxs8[1]), fmaxf(mxs8[2], mxs8[3])),
-                                   fmaxf(fmaxf(mxs8[4], mxs8[5]), fmaxf(mxs8[6], mxs8[7])));
-            float alpha = 1.f;
-            if (mx > m + lazy_margin || j == 0) {
-                alpha = exp2f((m - mx) * scale_log2e);   // j == 0: m = -inf -> 0 (O is not read then)
-                m = mx;
+            for (int jj = 0; jj < KB / 8; ++jj) {
+                const uint32_t pk = pack_bf16x2(exp2f(s[4 * jj + 2 * h] * scale_log2e - ms),
+                                                exp2f(s[4 * jj + 2 * h + 1] * scale_log2e - ms));
+                const float2 back = unpack_bf16x2(pk);   // sum what the tensor core will actually see
+                sum += back.x + back.y;
+                // A fragment of key chunk jj/2: regs {row g, keys 0-7 | row g+8, keys 0-7 | row g, keys 8-15 | row g+8, ...}
+                pa[jj >> 1][(jj & 1) * 2 + h] = pk;
             }
-            const float ms = m * scale_log2e;
-            if (j > 0) {   // P buffer free and O_t stable once PV_t(j-1) completed
-                mbar_wait(&pv_done[t], (j - 1) & 1);
-                tcgen05_fence_after();
-                if (__any_sync(0xffffffffu, alpha != 1.f)) {   // rescale the running output in place (warp-collective)
-#pragma unroll 1
-                    for (int c = 0; c < HEAD_DIM / 32; ++c) {
-                        uint32_t o[32];
-                        tmem_ld_32x32(to + c * 32, o);
-                        tmem_ld_wait();
+            l[h] = l[h] * alpha + sum;
 #pragma unroll
-                        for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                        tmem_st_32x32(to + c * 32, o);
-                    }
-                    tmem_st_wait();
-                }
+            for (int jj = 0; jj < HEAD_DIM / 8; ++jj) {
+                o[4 * jj + 2 * h] *= alpha;
+                o[4 * jj + 2 * h + 1] *= alpha;
             }
-            float sum4[4] = {0.f, 0.f, 0.f, 0.f};   // independent partial sums: short dependency chains
-#pragma unroll
-            for (int c = 0; c < KB / 32; ++c) {
-                uint32_t packed[16];
-#pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float p0 = exp2f(__uint_as_float(r[c][2 * i]) * scale_log2e - ms);
-                    const float p1 = exp2f(__uint_as_float(r[c][2 * i + 1]) * scale_log2e - ms);
-                    const uint32_t pk = pack_bf16x2(p0, p1);
-                    const float2 back = unpack_bf16x2(pk);   // sum what the tensor core will actually see
-                    sum4[i & 3] += back.x + back.y;
-                    packed[i] = pk;
-                }
-                // keys [c*32, c*32+32) of the block live in P tile kb = c/2 (64 keys), 16B chunks (c%2)*4 .. +3 of the row
-                uint8_t* tile_row = pbase + (c >> 1) * (Q_TILE * 128) + row * 128;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int chunk = (c & 1) * 4 + q;
-                    int4 v;
-                    v.x = packed[4 * q + 0]; v.y = packed[4 * q + 1]; v.z = packed[4 * q + 2]; v.w = packed[4 * q + 3];
-                    *reinterpret_cast<int4*>(tile_row + ((chunk ^ (row & 7)) << 4)) = v;
-                }
-            }
-            l = l * alpha + ((sum4[0] + sum4[1]) + (sum4[2] + sum4[3]));
-            tcgen05_fence_before();
-            fence_proxy_async_smem();       // generic-proxy smem writes (P) -> visible to the tensor core
-            mbar_arrive(&p_full[t]);
         }
-        mbar_wait(&pv_done[t], (NUM_KB - 1) & 1);
-        tcgen05_fence_after();
-        const float inv = 1.f / l;
-        const long long token = seq_row0 + (2 * qpair + t) * Q_TILE + row;
-        if (lse2) lse2[token * num_heads + head] = m * scale_log2e + log2f(l);   // log2 sum_j exp2(s_j * scale_log2e)
-        bf16* op = out + token * d_model + head * HEAD_DIM;
+        wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-            uint32_t r[32];
-            tmem_ld_32x32(to + c * 32, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                int4 v;
-                v.x = pack_bf16x2(__uint_as_float(r[8 * i + 0]) * inv, __uint_as_float(r[8 * i + 1]) * inv);
-                v.y = pack_bf16x2(__uint_as_float(r[8 * i + 2]) * inv, __uint_as_float(r[8 * i + 3]) * inv);
-                v.z = pack_bf16x2(__uint_as_float(r[8 * i + 4]) * inv, __uint_as_float(r[8 * i + 5]) * inv);
-                v.w = pack_bf16x2(__uint_as_float(r[8 * i + 6]) * inv, __uint_as_float(r[8 * i + 7]) * inv);
-                *reinterpret_cast<int4*>(op + c * 32 + 8 * i) = v;
-            }
+        for (int kc = 0; kc < KB / 16; ++kc)   // V block as an MN-major B operand: 16 keys = 16 rows of 128 B per step
+            wgmma_bf16_rs_n64<1>(o, pa[kc], make_smem_desc_sw128(sv + kc * 2048, 0, 1024), 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        if (j + 2 < NUM_KB) {
+            named_bar_sync(1, NUM_THREADS2);   // both warpgroups are done with stage st
+            if (tid == 0) load_kv(j + 2);
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 512);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float lt = l[h];
+        lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+        lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+        const float inv = 1.f / lt;
+        const long long token = seq_row0 + qt * Q_TILE + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        if (lse2 && (lane & 3) == 0) lse2[token * num_heads + head] = m[h] * scale_log2e + log2f(lt);
+        bf16* op = out + token * d_model + head * HEAD_DIM + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < HEAD_DIM / 8; ++jj)
+            *reinterpret_cast<uint32_t*>(op + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
     }
 }
 
@@ -315,7 +186,7 @@ int lah_attention_fwd(const void* qkv, void* out, float* lse2, int batch, int nu
     }
     if (batch <= 0) return 0;
     const float scale_log2e = 1.4426950408889634f / sqrtf((float)HEAD_DIM);
-    v2::attention_fwd_v2_kernel<<<batch * num_heads * 2, v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
+    v2::attention_fwd_v2_kernel<<<batch * num_heads * (S_LEN / Q_TILE), v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
         tm, (bf16*)out, lse2, d_model, num_heads, scale_log2e);
     return -(int)cudaGetLastError();
 }

@@ -1,22 +1,21 @@
-// attention_bwd.cu — tcgen05 self-attention BACKWARD for the transformer expert (d_model 1024, 16 heads x 64, seq 512).
+// attention_bwd.cu — wgmma self-attention BACKWARD for the transformer expert (d_model 1024, 16 heads x 64, seq 512).
 // The reference's transformer expert cannot be trained at all (in-place transpose of a leaf, SURVEY.md §0.3); this kernel is
-// what makes the sm_100a transformer expert trainable without falling back to eager PyTorch.
+// what makes the sm_90a transformer expert trainable without falling back to eager PyTorch.
 //
-// One CTA = one (batch, head, 128-key block j).  K_j / V_j stay in shared memory; the four 128-query blocks i stream through
-// a 2-stage TMA pipeline (Q_i and dO_i).  Per query block, all on tensor cores with accumulators in TMEM:
+// One CTA = one (batch, head, 128-key block j); consumer warpgroup w owns keys [64w, 64w + 64) of the block.  K_j / V_j stay
+// in shared memory; the four 128-query blocks i stream through a 2-stage TMA pipeline (Q_i and dO_i).  Per query block, all
+// on tensor cores with accumulators in registers (transposed problem: keys are the MMA rows):
 //
-//     S   = Q_i K_j^T                 (128 x 128)        dP  = dO_i V_j^T              (128 x 128)
-//     P   = exp2(S * scale*log2e - LSE_i)   [recomputed from the forward's row log-sum-exp: no second softmax pass]
-//     dS  = P o (dP - Delta_i) * scale      [Delta = rowsum(dO o O)]
-//     dV_j += P^T dO_i   (128 x 64)    dK_j += dS^T Q_i  (128 x 64)    dQ_i^(j) = dS K_j  (128 x 64, one partial per key block j)
+//     S^T = K_j Q_i^T               (64 x 128 per warpgroup)     dP^T = V_j dO_i^T            (64 x 128)
+//     P^T = exp2(S^T * scale*log2e - LSE_i)   [recomputed from the forward's row log-sum-exp: no second softmax pass]
+//     dS^T = P^T o (dP^T - Delta_i) * scale   [Delta = rowsum(dO o O)]
+//     dV_j += P^T dO_i   (64 x 64)   dK_j += dS^T Q_i  (64 x 64)   dQ_i^(j) = dS K_j  (128 x 64, one partial per key block j)
 //
-// P and dS are written ONCE to shared memory (bf16, 128B-swizzled [query rows][64 keys] atoms) and consumed three ways by
-// tcgen05.mma without any transpose: as an MN-major A operand (P^T, dS^T) and as a K-major A operand (dS); Q_i, dO_i, K_j are
-// consumed both K-major (S, dP) and MN-major (dV, dK, dQ) straight from their TMA tiles.  Nothing of size S x S touches HBM.
-//
-// Roles: warp 0 = TMA producer, warp 1 = MMA issuer (one thread), warps 2-5 = one thread per query row (tcgen05.ld of the S and
-// dP rows, exp2, dS, smem stores, dQ reduction, final dK / dV epilogue).
-#include "sm100.cuh"
+// P^T and dS^T are fed to dV / dK straight from registers (the accumulator layout IS the wgmma A fragment layout); dS^T is
+// also stored once to shared memory (bf16, 128B-swizzled [key rows][64 queries] atoms), where it is the MN-major A operand
+// of dQ.  Q_i, dO_i, K_j are consumed both K-major (S, dP) and MN-major (dV, dK, dQ) straight from their TMA tiles.
+// Nothing of size S x S touches HBM.  Thread 0 also drives TMA.
+#include "sm90.cuh"
 
 namespace lah {
 namespace attnb {
@@ -25,20 +24,18 @@ constexpr int S_LEN = 512;
 constexpr int HEAD_DIM = 64;
 constexpr int BLK = 128;                       // query block == key block
 constexpr int NUM_QB = S_LEN / BLK;            // 4
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 256;
 constexpr int TILE = BLK * HEAD_DIM * 2;       // 16 KB: 128 x 64 bf16
-constexpr int PS_BYTES = BLK * BLK * 2;        // 32 KB: P / dS (two [128 rows][64 keys] atoms)
-constexpr int ATOM = BLK * 128;                // bytes between the two 64-wide atoms of P / dS
+constexpr int ATOM = BLK * 128;                // 16 KB: one [128 key rows][64 queries] atom of dS^T
 constexpr int OFF_K = 0;
 constexpr int OFF_V = OFF_K + TILE;
 constexpr int OFF_Q = OFF_V + TILE;            // 2 stages
 constexpr int OFF_DO = OFF_Q + 2 * TILE;       // 2 stages
-constexpr int OFF_P = OFF_DO + 2 * TILE;
-constexpr int OFF_DS = OFF_P + PS_BYTES;
-constexpr int OFF_BAR = OFF_DS + PS_BYTES;
-constexpr int NUM_BARS = 1 + 2 + 2 + 1 + 1 + 1;
+constexpr int OFF_DS = OFF_DO + 2 * TILE;      // dS^T: two atoms (queries 0-63, 64-127)
+constexpr int OFF_LSE = OFF_DS + 2 * ATOM;     // lse2 / delta of the current query block: 2 x 128 fp32
+constexpr int OFF_BAR = OFF_LSE + 2 * BLK * 4;
+constexpr int NUM_BARS = 1 + 2;
 constexpr int SMEM_TOTAL = OFF_BAR + NUM_BARS * 8 + 16 + 1024;
-constexpr int COL_S = 0, COL_DP = 128, COL_DV = 256, COL_DK = 320, COL_DQ = 384;
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
@@ -50,185 +47,133 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
     uint64_t* kv_full = bars;
     uint64_t* q_full = bars + 1;     // [2]
-    uint64_t* q_empty = bars + 3;    // [2]
-    uint64_t* s_full = bars + 5;     // MMA -> row threads: S and dP of block i are in TMEM
-    uint64_t* p_full = bars + 6;     // row threads (128) -> MMA: P and dS of block i are in shared memory
-    uint64_t* dq_full = bars + 7;    // MMA -> row threads: dQ_i complete (and P / dS / Q_i / dO_i no longer read)
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + NUM_BARS);
+    float* s_lse = reinterpret_cast<float*>(smem + OFF_LSE);
+    float* s_delta = s_lse + BLK;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
     const int j = blockIdx.x & 3;
     const int head = (blockIdx.x >> 2) % num_heads;
     const int batch = (blockIdx.x >> 2) / num_heads;
     const int seq0 = batch * S_LEN;
 
-    if (warp == 0 && lane == 0) {
+    auto load_q = [&](int i) {   // thread 0 only; stage i & 1 must be free
+        const int st = i & 1;
+        mbar_arrive_expect_tx(&q_full[st], 2 * TILE);
+        tma_load_2d(smem + OFF_Q + st * TILE, &tm_qkv, &q_full[st], head * HEAD_DIM, seq0 + i * BLK);
+        tma_load_2d(smem + OFF_DO + st * TILE, &tm_do, &q_full[st], head * HEAD_DIM, seq0 + i * BLK);
+    };
+    if (tid == 0) {
         tma_prefetch_desc(&tm_qkv);
         tma_prefetch_desc(&tm_do);
         mbar_init(kv_full, 1);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 1);
-        }
-        mbar_init(s_full, 1);
-        mbar_init(p_full, 128);
-        mbar_init(dq_full, 1);
+        mbar_init(&q_full[0], 1);
+        mbar_init(&q_full[1], 1);
         fence_mbar_init();
+        mbar_arrive_expect_tx(kv_full, 2 * TILE);
+        tma_load_2d(smem + OFF_K, &tm_qkv, kv_full, d_model + head * HEAD_DIM, seq0 + j * BLK);
+        tma_load_2d(smem + OFF_V, &tm_qkv, kv_full, 2 * d_model + head * HEAD_DIM, seq0 + j * BLK);
+        load_q(0);
+        load_q(1);
     }
-    if (warp == 1) tmem_alloc(tmem_ptr, 512);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp == 0) {
-        if (lane == 0) {
-            // ------------------------------------------------------------------ TMA producer
-            mbar_arrive_expect_tx(kv_full, 2 * TILE);
-            tma_load_2d(smem + OFF_K, &tm_qkv, kv_full, d_model + head * HEAD_DIM, seq0 + j * BLK);
-            tma_load_2d(smem + OFF_V, &tm_qkv, kv_full, 2 * d_model + head * HEAD_DIM, seq0 + j * BLK);
-            for (int i = 0; i < NUM_QB; ++i) {
-                const int st = i & 1;
-                mbar_wait(&q_empty[st], ((i >> 1) & 1) ^ 1);
-                mbar_arrive_expect_tx(&q_full[st], 2 * TILE);
-                tma_load_2d(smem + OFF_Q + st * TILE, &tm_qkv, &q_full[st], head * HEAD_DIM, seq0 + i * BLK);
-                tma_load_2d(smem + OFF_DO + st * TILE, &tm_do, &q_full[st], head * HEAD_DIM, seq0 + i * BLK);
+    const uint32_t sk = smem_u32(smem + OFF_K), sv = smem_u32(smem + OFF_V), sds = smem_u32(smem + OFF_DS);
+    const int key_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // row of the block (+ 8 for h = 1)
+    const int qcol = 2 * (lane & 3);                               // query column (+ 8 jj, + 1)
+    float dv[HEAD_DIM / 2], dk[HEAD_DIM / 2];
+#pragma unroll
+    for (int e = 0; e < HEAD_DIM / 2; ++e) dv[e] = dk[e] = 0.f;
+    mbar_wait(kv_full, 0);
+#pragma unroll 1
+    for (int i = 0; i < NUM_QB; ++i) {
+        const int st = i & 1;
+        const long long tok0 = seq0 + i * BLK;
+        if (tid < BLK) s_lse[tid] = __ldg(lse2 + (tok0 + tid) * num_heads + head);
+        else s_delta[tid - BLK] = __ldg(delta + (tok0 + tid - BLK) * num_heads + head);
+        mbar_wait(&q_full[st], (i >> 1) & 1);
+        const uint32_t sq = smem_u32(smem + OFF_Q + st * TILE), sdo = smem_u32(smem + OFF_DO + st * TILE);
+        float sacc[BLK / 2], dpacc[BLK / 2];
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
+            wgmma_bf16_n128<0, 0>(sacc, make_smem_desc_sw128(sk + wg * 8192 + ks * 32, 0, 1024),
+                                  make_smem_desc_sw128(sq + ks * 32, 0, 1024), ks > 0 ? 1u : 0u);
+#pragma unroll
+        for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
+            wgmma_bf16_n128<0, 0>(dpacc, make_smem_desc_sw128(sv + wg * 8192 + ks * 32, 0, 1024),
+                                  make_smem_desc_sw128(sdo + ks * 32, 0, 1024), ks > 0 ? 1u : 0u);
+        wgmma_commit();
+        named_bar_sync(1, NUM_THREADS);   // lse / delta of this block are in shared memory
+        wgmma_wait<0>();
+        wgmma_fence_regs(sacc);
+        wgmma_fence_regs(dpacc);
+        uint32_t pa[BLK / 16][4], da[BLK / 16][4];
+#pragma unroll
+        for (int jj = 0; jj < BLK / 8; ++jj) {
+            const int q = 8 * jj + qcol;
+            const float l0 = s_lse[q], l1 = s_lse[q + 1], d0 = s_delta[q], d1 = s_delta[q + 1];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const float p0 = exp2f(sacc[4 * jj + 2 * h] * scale_log2e - l0);
+                const float p1 = exp2f(sacc[4 * jj + 2 * h + 1] * scale_log2e - l1);
+                const uint32_t pp = pack_bf16x2(p0, p1);
+                const uint32_t dd = pack_bf16x2(p0 * (dpacc[4 * jj + 2 * h] - d0) * scale,
+                                                p1 * (dpacc[4 * jj + 2 * h + 1] - d1) * scale);
+                pa[jj >> 1][(jj & 1) * 2 + h] = pp;
+                da[jj >> 1][(jj & 1) * 2 + h] = dd;
+                // dS^T[key][q]: atom q / 64, 16 B chunk (q % 64) / 8 swizzled with key & 7
+                const int key = key_row + 8 * h;
+                *reinterpret_cast<uint32_t*>(smem + OFF_DS + (jj >> 3) * ATOM + key * 128 + (((jj & 7) ^ (key & 7)) << 4) +
+                                             4 * (lane & 3)) = dd;
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ------------------------------------------------------------------ MMA issuer
-            constexpr uint32_t idesc_s = make_idesc_bf16_f32(BLK, BLK, 0u, 0u);          // S, dP: both operands K-major
-            constexpr uint32_t idesc_t = make_idesc_bf16_f32(BLK, HEAD_DIM, 1u, 1u);     // dV, dK: A^T (MN-major) x MN-major B
-            constexpr uint32_t idesc_q = make_idesc_bf16_f32(BLK, HEAD_DIM, 0u, 1u);     // dQ: K-major A x MN-major B
-            const uint32_t sk = smem_u32(smem + OFF_K), sv = smem_u32(smem + OFF_V), sp = smem_u32(smem + OFF_P),
-                           sds = smem_u32(smem + OFF_DS);
-            mbar_wait(kv_full, 0);
-            for (int i = 0; i < NUM_QB; ++i) {
-                const int st = i & 1;
-                const uint32_t sq = smem_u32(smem + OFF_Q + st * TILE), sdo = smem_u32(smem + OFF_DO + st * TILE);
-                mbar_wait(&q_full[st], (i >> 1) & 1);
-                tcgen05_fence_after();
+        // dV += P^T dO, dK += dS^T Q: reduction over the 128 queries of the block, B operands MN-major (16 rows per step)
+        wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
-                    umma_bf16_ss(tmem_base + COL_S, make_smem_desc_sw128(sq + ks * 32, 0, 1024),
-                                 make_smem_desc_sw128(sk + ks * 32, 0, 1024), idesc_s, ks > 0 ? 1u : 0u);
+        for (int kc = 0; kc < BLK / 16; ++kc)
+            wgmma_bf16_rs_n64<1>(dv, pa[kc], make_smem_desc_sw128(sdo + kc * 2048, 0, 1024), 1u);
 #pragma unroll
-                for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
-                    umma_bf16_ss(tmem_base + COL_DP, make_smem_desc_sw128(sdo + ks * 32, 0, 1024),
-                                 make_smem_desc_sw128(sv + ks * 32, 0, 1024), idesc_s, ks > 0 ? 1u : 0u);
-                umma_commit(s_full);
-                mbar_wait(p_full, i & 1);
-                tcgen05_fence_after();
+        for (int kc = 0; kc < BLK / 16; ++kc)
+            wgmma_bf16_rs_n64<1>(dk, da[kc], make_smem_desc_sw128(sq + kc * 2048, 0, 1024), 1u);
+        wgmma_commit();
+        fence_proxy_async_smem();          // generic-proxy smem writes (dS^T) -> visible to the tensor core
+        named_bar_sync(1, NUM_THREADS);    // dS^T of both warpgroups is in shared memory
+        // dQ (this warpgroup's 64 queries) = dS K_j: A = dS^T atom wg (MN-major), B = K_j (MN-major), 8 steps of 16 keys
+        float dq[HEAD_DIM / 2];
+        wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < BLK / 16; ++ks) {   // reduction over the 128 queries of the block, 16 rows per step
-                    umma_bf16_ss(tmem_base + COL_DV, make_smem_desc_sw128(sp + ks * 2048, ATOM, 1024),
-                                 make_smem_desc_sw128(sdo + ks * 2048, ATOM, 1024), idesc_t, (i | ks) ? 1u : 0u);
-                }
+        for (int kc = 0; kc < BLK / 16; ++kc)
+            wgmma_bf16_n64<1, 1>(dq, make_smem_desc_sw128(sds + wg * ATOM + kc * 2048, ATOM, 1024),
+                                 make_smem_desc_sw128(sk + kc * 2048, 0, 1024), kc > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(dq);
+        wgmma_fence_regs(dv);
+        wgmma_fence_regs(dk);
+        // partial dQ of THIS key block into slice j of dq_part ([4, T, D] bf16; attn_dq_reduce_kernel sums the four slices in
+        // fp32) — no atomics, half the bytes of fp32 partials
 #pragma unroll
-                for (int ks = 0; ks < BLK / 16; ++ks) {
-                    umma_bf16_ss(tmem_base + COL_DK, make_smem_desc_sw128(sds + ks * 2048, ATOM, 1024),
-                                 make_smem_desc_sw128(sq + ks * 2048, ATOM, 1024), idesc_t, (i | ks) ? 1u : 0u);
-                }
+        for (int h = 0; h < 2; ++h) {
+            const long long token = tok0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+            bf16* dqp = dq_part + (static_cast<long long>(j) * total_tokens + token) * d_model + head * HEAD_DIM + qcol;
 #pragma unroll
-                for (int ks = 0; ks < BLK / 16; ++ks) {   // reduction over the 128 keys: atom ks / 4, 32 B per step inside the row
-                    umma_bf16_ss(tmem_base + COL_DQ, make_smem_desc_sw128(sds + (ks >> 2) * ATOM + (ks & 3) * 32, 0, 1024),
-                                 make_smem_desc_sw128(sk + ks * 2048, ATOM, 1024), idesc_q, ks ? 1u : 0u);
-                }
-                umma_commit(&q_empty[st]);
-                umma_commit(dq_full);
-            }
+            for (int jj = 0; jj < HEAD_DIM / 8; ++jj)
+                *reinterpret_cast<uint32_t*>(dqp + 8 * jj) = pack_bf16x2(dq[4 * jj + 2 * h], dq[4 * jj + 2 * h + 1]);
         }
-    } else {
-        // ---------------------------------------------------------------------- one thread per query row (TMEM lane)
-        const int row = (warp & 3) * 32 + lane;
-        const uint32_t lane_base = tmem_base + (static_cast<uint32_t>((warp & 3) * 32) << 16);
-        uint8_t* p_row = smem + OFF_P + row * 128;
-        uint8_t* ds_row = smem + OFF_DS + row * 128;
-#pragma unroll 1
-        for (int i = 0; i < NUM_QB; ++i) {
-            const long long token = seq0 + i * BLK + row;
-            const float lse = __ldg(lse2 + token * num_heads + head);
-            const float dl = __ldg(delta + token * num_heads + head);
-            mbar_wait(s_full, i & 1);
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < BLK / 32; ++c) {
-                uint32_t rs[32], rd[32];
-                tmem_ld_32x32(lane_base + COL_S + c * 32, rs);
-                tmem_ld_32x32(lane_base + COL_DP + c * 32, rd);
-                tmem_ld_wait();
-                uint32_t pp[16], dd[16];
-#pragma unroll
-                for (int e = 0; e < 16; ++e) {
-                    const float p0 = exp2f(__uint_as_float(rs[2 * e]) * scale_log2e - lse);
-                    const float p1 = exp2f(__uint_as_float(rs[2 * e + 1]) * scale_log2e - lse);
-                    pp[e] = pack_bf16x2(p0, p1);
-                    dd[e] = pack_bf16x2(p0 * (__uint_as_float(rd[2 * e]) - dl) * scale,
-                                        p1 * (__uint_as_float(rd[2 * e + 1]) - dl) * scale);
-                }
-                // keys [c*32, c*32+32) live in atom c/2, 16 B chunks (c%2)*4 .. +3 of the 128 B row (swizzled with row & 7)
-                const int atom_off = (c >> 1) * ATOM;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int chunk = (((c & 1) * 4 + q) ^ (row & 7)) << 4;
-                    *reinterpret_cast<int4*>(p_row + atom_off + chunk) = make_int4(pp[4 * q], pp[4 * q + 1], pp[4 * q + 2], pp[4 * q + 3]);
-                    *reinterpret_cast<int4*>(ds_row + atom_off + chunk) = make_int4(dd[4 * q], dd[4 * q + 1], dd[4 * q + 2], dd[4 * q + 3]);
-                }
-            }
-            tcgen05_fence_before();
-            fence_proxy_async_smem();
-            mbar_arrive(p_full);
-            mbar_wait(dq_full, i & 1);
-            tcgen05_fence_after();
-            // partial dQ of THIS key block: plain 16 B stores of the thread's 128 contiguous bytes into slice j of dq_part
-            // ([4, T, D] bf16; attn_dq_reduce_kernel sums the four slices in fp32) — no atomics, half the bytes of fp32 partials
-            int4* dq = reinterpret_cast<int4*>(dq_part + (static_cast<long long>(j) * total_tokens + token) * d_model + head * HEAD_DIM);
-#pragma unroll 1
-            for (int c = 0; c < HEAD_DIM / 32; ++c) {
-                uint32_t r[32];
-                tmem_ld_32x32(lane_base + COL_DQ + c * 32, r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int e = 0; e < 4; ++e)
-                    dq[c * 4 + e] = make_int4(pack_bf16x2(__uint_as_float(r[8 * e]), __uint_as_float(r[8 * e + 1])),
-                                              pack_bf16x2(__uint_as_float(r[8 * e + 2]), __uint_as_float(r[8 * e + 3])),
-                                              pack_bf16x2(__uint_as_float(r[8 * e + 4]), __uint_as_float(r[8 * e + 5])),
-                                              pack_bf16x2(__uint_as_float(r[8 * e + 6]), __uint_as_float(r[8 * e + 7])));
-            }
-            tcgen05_fence_before();
-        }
-        // dK_j / dV_j: complete after the last dq_full (the commit covers every MMA issued before it)
-        const long long key = seq0 + j * BLK + row;
-        bf16* dk = dqkv + key * (3ll * d_model) + d_model + head * HEAD_DIM;
-        bf16* dv = dqkv + key * (3ll * d_model) + 2 * d_model + head * HEAD_DIM;
-#pragma unroll 1
-        for (int c = 0; c < HEAD_DIM / 32; ++c) {
-            uint32_t rk[32], rv[32];
-            tmem_ld_32x32(lane_base + COL_DK + c * 32, rk);
-            tmem_ld_32x32(lane_base + COL_DV + c * 32, rv);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                int4 a, b;
-                a.x = pack_bf16x2(__uint_as_float(rk[8 * q + 0]), __uint_as_float(rk[8 * q + 1]));
-                a.y = pack_bf16x2(__uint_as_float(rk[8 * q + 2]), __uint_as_float(rk[8 * q + 3]));
-                a.z = pack_bf16x2(__uint_as_float(rk[8 * q + 4]), __uint_as_float(rk[8 * q + 5]));
-                a.w = pack_bf16x2(__uint_as_float(rk[8 * q + 6]), __uint_as_float(rk[8 * q + 7]));
-                b.x = pack_bf16x2(__uint_as_float(rv[8 * q + 0]), __uint_as_float(rv[8 * q + 1]));
-                b.y = pack_bf16x2(__uint_as_float(rv[8 * q + 2]), __uint_as_float(rv[8 * q + 3]));
-                b.z = pack_bf16x2(__uint_as_float(rv[8 * q + 4]), __uint_as_float(rv[8 * q + 5]));
-                b.w = pack_bf16x2(__uint_as_float(rv[8 * q + 6]), __uint_as_float(rv[8 * q + 7]));
-                *reinterpret_cast<int4*>(dk + c * 32 + 8 * q) = a;
-                *reinterpret_cast<int4*>(dv + c * 32 + 8 * q) = b;
-            }
-        }
+        named_bar_sync(1, NUM_THREADS);    // dS^T, Q_i, dO_i, lse / delta of this block are no longer read
+        if (tid == 0 && i + 2 < NUM_QB) load_q(i + 2);
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    // dK_j / dV_j
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const long long key = seq0 + j * BLK + key_row + 8 * h;
+        bf16* dkp = dqkv + key * (3ll * d_model) + d_model + head * HEAD_DIM + qcol;
+        bf16* dvp = dqkv + key * (3ll * d_model) + 2 * d_model + head * HEAD_DIM + qcol;
+#pragma unroll
+        for (int jj = 0; jj < HEAD_DIM / 8; ++jj) {
+            *reinterpret_cast<uint32_t*>(dkp + 8 * jj) = pack_bf16x2(dk[4 * jj + 2 * h], dk[4 * jj + 2 * h + 1]);
+            *reinterpret_cast<uint32_t*>(dvp + 8 * jj) = pack_bf16x2(dv[4 * jj + 2 * h], dv[4 * jj + 2 * h + 1]);
+        }
     }
 }
 

@@ -1,29 +1,30 @@
-// grouped_gemm.cu — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// grouped_gemm.cu — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
 // One kernel template covers every GEMM-shaped op of the DMoE expert path
 // (reference hot loops: experiments/throughput/layers.py:8-19 forward, lib/runtime/expert_backend.py:73-93 backward):
 //
-//   MODE_MGROUP  C[rows, N] = A[rows, K] * B[g(rows)]^T (+bias[g]) (+residual)
+//   MODE_MGROUP  C[rows, N] = act(A[rows, K] * B[g(rows)]^T (+bias[g])) (+residual)
 //                rows are grouped by expert, every group padded to a multiple of 128 rows; the group of a
 //                128-row tile comes from a device-side table written by the dispatch kernel (no host sync).
 //                B is either K-major  ([G, N, K], forward:  x @ W^T)
 //                      or MN-major    ([G, K, N], dgrad:    dy @ W  with W stored [K=out, N=in]).
-//   MODE_KGROUP  C[g][M, N] = A_g^T * B_g   (wgrad: dW = dY^T X, reduction over the tokens of expert g)
+//   MODE_KGROUP  C[g][M, N] (+)= A_g^T * B_g   (wgrad: dW = dY^T X, reduction over the tokens of expert g)
 //                A = dY [tokens, M], B = X [tokens, N], both "MN-major" operands; fp32 output per group.
 //
-// Structure (one CTA per SM, 192 threads):
-//   warp 0 (one lane)  TMA producer: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx
-//   warp 1 (one lane)  MMA issuer:   tcgen05.mma cta_group::1 kind::f16, 128 x BLOCK_N x 16, accumulators in TMEM
-//                      (2 accumulator stages => epilogue of tile i overlaps the MMAs of tile i+1)
-//   warps 2..5         epilogue:     tcgen05.ld 32x32b -> registers -> bias/residual -> bf16|fp32 -> global
-#include "sm100.cuh"
+// Structure (one CTA per SM, 288 threads):
+//   warps 0-7  two consumer warpgroups: warpgroup w owns rows [64w, 64w + 64) of the 128 x BLOCK_N tile, issues
+//              wgmma.m64nBLOCK_Nk16 from the shared-memory ring (accumulator in registers) and runs the epilogue
+//              (bias / activation / residual / accumulate -> bf16 | fp32 -> global) straight from its registers
+//   warp 8     TMA producer (one lane): cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx; it runs
+//              ahead into the next tile while the consumers drain the previous one
+#include "sm90.cuh"
 
 namespace lah {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 bytes = one swizzle-128B row
-constexpr int UMMA_K = 16;
-constexpr int NUM_THREADS = 192;
+constexpr int MMA_K = 16;
+constexpr int NUM_THREADS = 288;
 constexpr int MODE_MGROUP = 0;
 constexpr int MODE_KGROUP = 1;
 
@@ -46,6 +47,8 @@ struct GemmParams {
     int wait_count, wait_epoch;
     const int* epoch_base;   // device-side epoch base added to wait_epoch (nullptr: 0), see moe.cu Peers::step_ctr
     int* status;
+    int act;                 // MGROUP epilogue activation after the bias: 0 none, 1 ReLU, 2 GELU (erf)
+    int accumulate;          // KGROUP: C += result (gradient accumulation across steps, update_every_*)
 };
 
 template <int BLOCK_N, int STAGES>
@@ -54,8 +57,26 @@ struct SmemLayout {
     static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-    static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 4) * 8 + 16 + 1024;  // + alignment slack
+    static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024;  // + alignment slack
+    static_assert(TOTAL <= 227 * 1024, "shared memory budget");
 };
+
+template <int BLOCK_N, bool A_MN, bool B_MN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa, uint32_t sb, int wg, bool first) {
+    // A: this warpgroup's 64 rows. K-major: rows 64wg.. (8 KB in). MN-major: the wg-th 64-wide atom (BLOCK_K*128 B).
+    const uint32_t a0 = sa + wg * (A_MN ? BLOCK_K * 128 : 64 * 128);
+    constexpr uint32_t A_KSTEP = A_MN ? MMA_K * 128 : MMA_K * 2, B_KSTEP = B_MN ? MMA_K * 128 : MMA_K * 2;
+    constexpr uint32_t LBO = BLOCK_K * 128;
+#pragma unroll
+    for (int k = 0; k < BLOCK_K / MMA_K; ++k) {
+        const uint64_t da = make_smem_desc_sw128(a0 + k * A_KSTEP, LBO, 1024);
+        const uint64_t db = make_smem_desc_sw128(sb + k * B_KSTEP, LBO, 1024);
+        const uint32_t accum = (first && k == 0) ? 0u : 1u;
+        if constexpr (BLOCK_N == 256) wgmma_bf16_n256<A_MN, B_MN>(acc, da, db, accum);
+        if constexpr (BLOCK_N == 128) wgmma_bf16_n128<A_MN, B_MN>(acc, da, db, accum);
+        if constexpr (BLOCK_N == 64) wgmma_bf16_n64<A_MN, B_MN>(acc, da, db, accum);
+    }
+}
 
 template <int BLOCK_N, int STAGES, int MODE, bool A_MN, bool B_MN, bool OUT_F32>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -65,33 +86,20 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const _
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full = empty_bar + STAGES;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full[i], 1);
-            mbar_init(&tmem_empty[i], 4);  // one arrive per epilogue warp
+            mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
         }
         fence_mbar_init();
     }
-    constexpr uint32_t TMEM_COLS = (2 * BLOCK_N <= 32) ? 32 : (2 * BLOCK_N <= 64) ? 64 : (2 * BLOCK_N <= 128) ? 128
-                                   : (2 * BLOCK_N <= 256) ? 256 : 512;
-    if (warp == 1) tmem_alloc(tmem_ptr, TMEM_COLS);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     // ------------------------------------------------------------------ tile enumeration
     const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
@@ -127,7 +135,8 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const _
         }
     };
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8) {
+        if (lane != 0) return;
         // =============================================================== TMA producer
         if (p.wait_flags) {  // rows pushed by peer GPUs over NVLink must have landed before the first TMA load
             const unsigned long long t_wait = globaltimer_ns();
@@ -181,129 +190,88 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const _
                 }
             }
         }
-    } else if (warp == 1 && lane == 0) {
-        // =============================================================== MMA issuer
-        constexpr uint32_t idesc = make_idesc_bf16_f32(BLOCK_M, BLOCK_N, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-        // K-major:  SBO = 8 rows * 128B = 1024, LBO unused; advance 32 B per UMMA_K inside the swizzle row
-        // MN-major: SBO = 1024 (8 k-rows), LBO = BLOCK_K * 128 B (next 64-wide MN atom); advance 16 k-rows = 2048 B
-        constexpr uint32_t A_LBO = A_MN ? BLOCK_K * 128 : 0, B_LBO = B_MN ? BLOCK_K * 128 : 0;
-        constexpr uint32_t A_KSTEP = A_MN ? UMMA_K * 128 : UMMA_K * 2, B_KSTEP = B_MN ? UMMA_K * 128 : UMMA_K * 2;
-        int stage = 0;
-        uint32_t phase = 0;
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            int m_row, n_col, g, k_begin, num_kb;
-            if (!decode(tile, m_row, n_col, g, k_begin, num_kb)) continue;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_empty[as], aphase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BLOCK_N;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tcgen05_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
-                const uint32_t sb = sa + L::A_BYTES;
-#pragma unroll
-                for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                    const uint64_t da = make_smem_desc_sw128(sa + k * A_KSTEP, A_LBO, 1024);
-                    const uint64_t db = make_smem_desc_sw128(sb + k * B_KSTEP, B_LBO, 1024);
-                    umma_bf16_ss(tmem_d, da, db, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&empty_bar[stage]);  // smem slot is free once these MMAs have read it
-                if (kb == num_kb - 1) umma_commit(&tmem_full[as]);
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
+        return;
+    }
+
+    // =================================================================== consumers (two warpgroups)
+    const int wg = warp >> 2;
+    const int row_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // and + 8
+    const int col_in_tile = 2 * (lane & 3);                             // + 8 j (+ 1)
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[BLOCK_N / 2];
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        int m_row, n_col, g, k_begin, num_kb;
+        if (!decode(tile, m_row, n_col, g, k_begin, num_kb)) continue;
+        int prev_stage = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * L::STAGE_BYTES);
+            wgmma_fence();
+            mma_kblock<BLOCK_N, A_MN, B_MN>(acc, sa, sa + L::A_BYTES, wg, kb == 0);
+            wgmma_commit();
+            wgmma_wait<1>();   // the k-block before this one is done: release its stage
+            if (prev_stage >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
             }
-            ++iter;
+            prev_stage = stage;
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
         }
-    } else if (warp >= 2) {
-        // =============================================================== epilogue (4 warps, one row per thread)
-        const int lane_group = warp & 3;  // TMEM lane quarter this warp may access
-        int iter = 0;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            int m_row, n_col, g, k_begin, num_kb;
-            if (!decode(tile, m_row, n_col, g, k_begin, num_kb)) continue;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_full[as], aphase);
-            tcgen05_fence_after();
-            const int row = m_row + lane_group * 32 + lane;
-            const bool row_ok = (MODE == MODE_KGROUP) ? true : (row < p.M);
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_group * 32) << 16) + as * BLOCK_N;
-#pragma unroll 1
-            for (int c = 0; c < BLOCK_N / 32; ++c) {
-                uint32_t r[32];
-                tmem_ld_32x32(taddr + c * 32, r);
-                tmem_ld_wait();
-                const int col = n_col + c * 32;
-                if (col >= p.N || !row_ok) continue;
-                float v[32];
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+        // ------------------------------------------------------------ epilogue from registers
 #pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
+        for (int h = 0; h < 2; ++h) {
+            const int row = m_row + row_in_tile + 8 * h;
+            const bool row_ok = (MODE == MODE_KGROUP) ? true : (row < p.M);
+            if (!row_ok) continue;
+            const long long gbase = (MODE == MODE_KGROUP ? static_cast<long long>(g) * p.c_group_stride : 0ll) +
+                                    static_cast<long long>(row) * p.ldc;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int col = n_col + 8 * j + col_in_tile;
+                if (col >= p.N) continue;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
                 if (MODE == MODE_MGROUP) {
                     if (p.bias) {
-                        const float4* bp = reinterpret_cast<const float4*>(p.bias + static_cast<long long>(g) * p.N + col);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float4 b = __ldg(bp + j);
-                            v[4 * j + 0] += b.x;
-                            v[4 * j + 1] += b.y;
-                            v[4 * j + 2] += b.z;
-                            v[4 * j + 3] += b.w;
-                        }
+                        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + static_cast<long long>(g) * p.N + col));
+                        v0 += b.x;
+                        v1 += b.y;
+                    }
+                    if (p.act == 1) {
+                        v0 = fmaxf(v0, 0.f);
+                        v1 = fmaxf(v1, 0.f);
+                    } else if (p.act == 2) {
+                        v0 = 0.5f * v0 * (1.f + erff(v0 * 0.70710678118654752f));
+                        v1 = 0.5f * v1 * (1.f + erff(v1 * 0.70710678118654752f));
                     }
                     if (p.residual) {
-                        const int4* rp = reinterpret_cast<const int4*>(p.residual + static_cast<long long>(row) * p.ldr + col);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const int4 q = __ldg(rp + j);
-                            const uint32_t w[4] = {(uint32_t)q.x, (uint32_t)q.y, (uint32_t)q.z, (uint32_t)q.w};
-#pragma unroll
-                            for (int t = 0; t < 4; ++t) {
-                                const float2 f = unpack_bf16x2(w[t]);
-                                v[8 * j + 2 * t] += f.x;
-                                v[8 * j + 2 * t + 1] += f.y;
-                            }
-                        }
+                        const float2 r = unpack_bf16x2(
+                            __ldg(reinterpret_cast<const unsigned int*>(p.residual + static_cast<long long>(row) * p.ldr + col)));
+                        v0 += r.x;
+                        v1 += r.y;
                     }
                 }
                 if (OUT_F32) {
-                    float* cp = reinterpret_cast<float*>(p.C) +
-                                (MODE == MODE_KGROUP ? static_cast<long long>(g) * p.c_group_stride : 0ll) +
-                                static_cast<long long>(row) * p.ldc + col;
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        *reinterpret_cast<float4*>(cp + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                } else {
-                    bf16* cp = reinterpret_cast<bf16*>(p.C) +
-                               (MODE == MODE_KGROUP ? static_cast<long long>(g) * p.c_group_stride : 0ll) +
-                               static_cast<long long>(row) * p.ldc + col;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        int4 q;
-                        q.x = pack_bf16x2(v[8 * j + 0], v[8 * j + 1]);
-                        q.y = pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
-                        q.z = pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
-                        q.w = pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
-                        *reinterpret_cast<int4*>(cp + 8 * j) = q;
+                    float2* cp = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + gbase + col);
+                    if (MODE == MODE_KGROUP && p.accumulate) {
+                        const float2 o = *cp;
+                        v0 += o.x;
+                        v1 += o.y;
                     }
+                    *cp = make_float2(v0, v1);
+                } else {
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.C) + gbase + col) = pack_bf16x2(v0, v1);
                 }
             }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[as]);
-            ++iter;
         }
-    }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
     }
 }
 
@@ -377,26 +345,12 @@ static int launch(const GemmParams& p, const CUtensorMap& tmA, const CUtensorMap
     return e == cudaSuccess ? 0 : -static_cast<int>(e);
 }
 
-}  // namespace lah
-
-using namespace lah;
-
-// ------------------------------------------------------------------------------------------------
-// C ABI (called from python via ctypes; see ops/native.py)
-// ------------------------------------------------------------------------------------------------
-extern "C" const int* lah_get_epoch_base();
-
-extern "C" {
-
-// C[rows, N] = A[rows, K] @ B[g]^T (+bias) (+residual)
-//   b_mn == 0: B is [G, N, K] (K contiguous);  b_mn == 1: B is [G, K, N] (N contiguous)
-//   a_rows: rows of the A buffer (TMA bound); m_valid: rows of C that may be written
-//   tile_group: device int[num_m_tiles] or null; out_f32: 0 => bf16 C, 1 => fp32 C
-int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
-                    long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group,
-                    const float* bias, const void* residual, long long ldr, int block_n, int max_ctas,
-                    const int* wait_flags, int wait_count, int wait_epoch, int* status, cudaStream_t stream) {
+static int gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
+                       long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group, const float* bias,
+                       const void* residual, long long ldr, int block_n, int max_ctas, const int* wait_flags,
+                       int wait_count, int wait_epoch, int* status, int act, const int* epoch_base, cudaStream_t stream) {
     if ((K % 8) || (N % 32) || (lda % 8)) return -2;
+    if (block_n != 256 && block_n != 128 && block_n != 64) return -3;
     CUtensorMap tmA, tmB;
     {
         uint64_t dims[2] = {(uint64_t)K, (uint64_t)a_rows};
@@ -422,7 +376,8 @@ int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int
     p.N = N; p.K = K; p.M = m_valid; p.num_groups = G; p.num_m_tiles = num_m_tiles; p.tile_group = tile_group;
     p.group_off = nullptr; p.C = C; p.ldc = ldc; p.c_group_stride = 0; p.bias = bias;
     p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr;
-    p.wait_flags = wait_flags; p.wait_count = wait_count; p.wait_epoch = wait_epoch; p.epoch_base = lah_get_epoch_base(); p.status = status;
+    p.wait_flags = wait_flags; p.wait_count = wait_count; p.wait_epoch = wait_epoch; p.epoch_base = epoch_base; p.status = status;
+    p.act = act; p.accumulate = 0;
 #define LAH_LAUNCH_M(BN, ST)                                                                                   \
     if (!b_mn && !out_f32) return launch<BN, ST, MODE_MGROUP, false, false, false>(p, tmA, tmB, max_ctas, stream); \
     if (b_mn && !out_f32) return launch<BN, ST, MODE_MGROUP, false, true, false>(p, tmA, tmB, max_ctas, stream);   \
@@ -430,15 +385,13 @@ int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int
     return launch<BN, ST, MODE_MGROUP, false, true, true>(p, tmA, tmB, max_ctas, stream);
     if (block_n == 256) { LAH_LAUNCH_M(256, 4) }
     if (block_n == 128) { LAH_LAUNCH_M(128, 6) }
-    if (block_n == 64) { LAH_LAUNCH_M(64, 8) }
+    LAH_LAUNCH_M(64, 8)
 #undef LAH_LAUNCH_M
-    return -3;
 }
 
-// C[g][M, N] (fp32) = A[off[g]:off[g+1], :M]^T @ B[off[g]:off[g+1], :N]   (A, B row-major token matrices)
-int lah_gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
-                    const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n,
-                    int max_ctas, cudaStream_t stream) {
+static int gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
+                       const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n, int max_ctas,
+                       int accumulate, cudaStream_t stream) {
     if ((M % 128) || (N % 32) || (lda % 8) || (ldb % 8)) return -2;
     CUtensorMap tmA, tmB;
     {
@@ -459,10 +412,61 @@ int lah_gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, 
     p.N = N; p.K = 0; p.M = M; p.num_groups = G; p.num_m_tiles = 0; p.tile_group = nullptr; p.group_off = group_off;
     p.C = C; p.ldc = ldc; p.c_group_stride = c_group_stride; p.bias = nullptr; p.residual = nullptr; p.ldr = 0;
     p.wait_flags = nullptr; p.wait_count = 0; p.wait_epoch = 0; p.epoch_base = nullptr; p.status = nullptr;
+    p.act = 0; p.accumulate = accumulate;
     if (block_n == 256) return launch<256, 4, MODE_KGROUP, true, true, true>(p, tmA, tmB, max_ctas, stream);
     if (block_n == 128) return launch<128, 6, MODE_KGROUP, true, true, true>(p, tmA, tmB, max_ctas, stream);
     if (block_n == 64) return launch<64, 8, MODE_KGROUP, true, true, true>(p, tmA, tmB, max_ctas, stream);
     return -3;
+}
+
+}  // namespace lah
+
+using namespace lah;
+
+// ------------------------------------------------------------------------------------------------
+// C ABI (called from python via ctypes; see ops/native.py)
+// ------------------------------------------------------------------------------------------------
+extern "C" const int* lah_get_epoch_base();
+
+extern "C" {
+
+// C[rows, N] = A[rows, K] @ B[g]^T (+bias) (+residual)
+//   b_mn == 0: B is [G, N, K] (K contiguous);  b_mn == 1: B is [G, K, N] (N contiguous)
+//   a_rows: rows of the A buffer (TMA bound); m_valid: rows of C that may be written
+//   tile_group: device int[num_m_tiles] or null; out_f32: 0 => bf16 C, 1 => fp32 C
+int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
+                    long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group,
+                    const float* bias, const void* residual, long long ldr, int block_n, int max_ctas,
+                    const int* wait_flags, int wait_count, int wait_epoch, int* status, cudaStream_t stream) {
+    return gemm_mgroup(A, lda, a_rows, B, G, N, K, b_mn, C, ldc, out_f32, m_valid, num_m_tiles, tile_group, bias, residual,
+                       ldr, block_n, max_ctas, wait_flags, wait_count, wait_epoch, status, 0, lah_get_epoch_base(), stream);
+}
+
+// C[g][M, N] (fp32) = A[off[g]:off[g+1], :M]^T @ B[off[g]:off[g+1], :N]   (A, B row-major token matrices)
+int lah_gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
+                    const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n,
+                    int max_ctas, cudaStream_t stream) {
+    return gemm_kgroup(A, lda, B, ldb, total_rows, G, M, N, group_off, C, ldc, c_group_stride, block_n, max_ctas, 0, stream);
+}
+
+// Wide-tile entry points of the big-batch expert path (expert groups padded to 256 rows, N a multiple of 256):
+// 128 x 256 tiles with the fused epilogue activation (act: 0 none, 1 ReLU, 2 GELU) and, for the weight gradient,
+// accumulation into C across steps.  tile_group has one entry per 128 rows.
+int lah_gemm_mgroup2(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
+                     long long ldc, int out_f32, int m_valid, int num_m_tiles128, const int* tile_group,
+                     const float* bias, const void* residual, long long ldr, int max_ctas, const int* wait_flags,
+                     int wait_count, int wait_epoch, int* status, int act, cudaStream_t stream) {
+    return gemm_mgroup(A, lda, a_rows, B, G, N, K, b_mn, C, ldc, out_f32, m_valid, num_m_tiles128, tile_group, bias,
+                       residual, ldr, 256, max_ctas, wait_flags, wait_count, wait_epoch, status, act, lah_get_epoch_base(),
+                       stream);
+}
+
+int lah_gemm_kgroup2(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
+                     const int* group_off, float* C, long long ldc, long long c_group_stride, int max_ctas,
+                     int accumulate, cudaStream_t stream) {
+    if (N % 256) return -2;
+    return gemm_kgroup(A, lda, B, ldb, total_rows, G, M, N, group_off, C, ldc, c_group_stride, 256, max_ctas, accumulate,
+                       stream);
 }
 
 }  // extern "C"

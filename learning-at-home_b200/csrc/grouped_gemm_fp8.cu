@@ -1,48 +1,36 @@
 // grouped_gemm_fp8.cu — block-scaled FP8 (MXFP8: E4M3 data, one UE8M0 scale per 1x32 block along K) grouped GEMM on
-// tcgen05.mma.cta_group::2.kind::mxf8f6f4.block_scale, plus the quantisation kernels that produce its operands.
+// Hopper FP8 tensor cores (wgmma ... e4m3.e4m3), plus the quantisation kernels that produce its operands.
 //
 //   C[r, :] = (A_q[r, :] * 2^sfa) @ (W_q[g(r)] * 2^sfb)^T (+ bias) (+ act) (+ residual)       bf16 / fp32 out
 //
-// Same CTA-pair protocol as grouped_gemm_2cta.cu (two TMA producers, one MMA thread in the leader, multicast commits,
-// two TMEM accumulator stages, smem-transposed coalesced epilogue).  Differences:
-//   * 8-bit operands: BLOCK_K = 128 elements (one 128 B swizzle row), UMMA_K = 32 -> twice the math per smem byte;
-//   * scale factors travel with every K block: TMA -> smem (512 B per 128 rows x 4 k-steps, already in the UTCCP
-//     "32 x 128 bit" order, see sf_word_index) -> TMEM with tcgen05.cp.32x128b.warpx4 issued by the MMA thread right
-//     before the four MMAs of the block (tcgen05.cp and tcgen05.mma execute in issue order, so ONE scale buffer in
-//     TMEM is enough); the a_sf_id/b_sf_id fields of the instruction descriptor select the byte (k-step) of each word;
-//   * TMEM budget: 2 accumulator stages + 12 scale columns must fit in 512 columns -> TILE_N = 192 (2*192 + 4 + 8).
+// Same structure as grouped_gemm.cu (one TMA producer warp, two consumer warpgroups of 64 rows, 128 x 128 tiles, epilogue
+// from registers).  Differences:
+//   * 8-bit operands: BLOCK_K = 128 elements (one 128 B swizzle row), MMA K = 32 -> twice the math per smem byte;
+//   * the tensor core has no block scaling here, so every 32-element K block is one wgmma into a scratch accumulator that
+//     is added to the running accumulator times 2^sfa[row] * 2^sfb[col] (exact: powers of two); the scale words come
+//     straight from the quantiser's layout (sf_word) through the read-only cache.
 //
 // Used for the expert FFN forward GEMMs (BASELINE.json config "fp8 expert GEMM"); dgrad / wgrad stay in bf16.
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include <cuda_fp8.h>
 
 namespace lah {
 namespace f8 {
 
-constexpr int TILE_M = 256;   // per pair
-constexpr int CTA_M = 128;    // per CTA
-constexpr int TILE_N = 192;   // per pair
-constexpr int CTA_N = 96;     // B rows loaded per CTA
+constexpr int TILE_M = 128;
+constexpr int TILE_N = 128;
 constexpr int BLOCK_K = 128;  // elements == bytes
-constexpr int UMMA_K = 32;
+constexpr int MMA_K = 32;
 constexpr int STAGES = 6;
-constexpr int NUM_THREADS = 320;   // TMA warp, MMA warp, up to 8 epilogue warps
+constexpr int NUM_THREADS = 288;     // two consumer warpgroups + one TMA producer warp
+constexpr int A_TILE_ROWS = 128;     // scale-factor tiling of activations / weights (see the storage layout below)
+constexpr int W_TILE_ROWS = 192;
 
-constexpr int A_BYTES = CTA_M * BLOCK_K;        // 16 KB
-constexpr int B_BYTES = CTA_N * BLOCK_K;        // 12 KB
-constexpr int SFA_BYTES = 512;                  // 128 rows x 4 k-steps
-constexpr int SFB_BYTES = 1024;                 // 2 atoms of 128 rows (192 used)
-constexpr int STAGE_TX = A_BYTES + B_BYTES + SFA_BYTES + SFB_BYTES;
-constexpr int STAGE_BYTES = 30 * 1024;          // padded to a multiple of 1024 (swizzle atom alignment)
-constexpr int SFA_OFF = A_BYTES + B_BYTES;
-constexpr int SFB_OFF = SFA_OFF + SFA_BYTES;
-constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;
-constexpr int EPI_BYTES = 8 * 32 * 80;          // max(8 warps x 32 rows x 80 B (bf16), 4 warps x 32 rows x 144 B (fp32))
-constexpr int BAR_OFFSET = EPI_OFFSET + EPI_BYTES;
-constexpr int SMEM_TOTAL = BAR_OFFSET + (2 * STAGES + 4) * 8 + 16 + 1024;
-constexpr int TMEM_SFA_COL = 2 * TILE_N;        // 384
-constexpr int TMEM_SFB_COL = TMEM_SFA_COL + 4;  // 388 .. 395
-static_assert(STAGE_TX <= STAGE_BYTES, "stage layout");
+constexpr int A_BYTES = TILE_M * BLOCK_K;       // 16 KB
+constexpr int B_BYTES = TILE_N * BLOCK_K;       // 16 KB
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+constexpr int SMEM_TOTAL = BAR_OFFSET + 2 * STAGES * 8 + 1024;
 static_assert(SMEM_TOTAL <= 227 * 1024, "shared memory budget");
 
 struct Params {
@@ -58,283 +46,179 @@ struct Params {
     const int* epoch_base;   // device-side epoch base added to wait_epoch (nullptr: 0), see moe.cu Peers::step_ctr
     int* status;
     int act;
+    const uint32_t* sfa;   // activation scales (tile_rows = 128)
+    const uint32_t* sfb;   // weight scales (tile_rows = 192)
 };
 
-// Instruction descriptor of kind::mxf8f6f4.block_scale (cute/arch/mma_sm100_desc.hpp, InstrDescriptorBlockScaled):
-//   [4,6) b_sf_id  [7,10) a_format (0 = E4M3)  [10,13) b_format  [15] a_major  [16] b_major  [17,23) N>>3
-//   [23] scale_format (1 = UE8M0)  [24,29) M>>4  [29,31) a_sf_id  [31] k_size (0 = K32)
-__host__ __device__ constexpr uint32_t make_idesc_mxf8(uint32_t M, uint32_t N, uint32_t sf_id) {
-    return (sf_id << 4) | ((N >> 3) << 17) | (1u << 23) | ((M >> 4) << 24) | (sf_id << 29);
+// D (64 x 128 per warpgroup) = A * B for one 32-element K block, E4M3 inputs (both K-major), fp32 accumulate, D overwritten
+__device__ __forceinline__ void wgmma_e4m3_n128(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 0, 1, 1;\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db));
 }
 
-// smem descriptor of a scale-factor chunk for tcgen05.cp: no swizzle, 8-row x 16 B core matrices 128 B apart
-__device__ __forceinline__ uint64_t make_sf_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
-    d |= static_cast<uint64_t>((128u >> 4) & 0x3FFFu) << 32;  // SBO = 128 B
-    d |= static_cast<uint64_t>(1) << 46;
-    return d;
+// the four UE8M0 scale bytes (k-steps of 32 elements) of row r of a 128-element K block, see the storage layout below
+__device__ __forceinline__ uint32_t sf_word(const uint32_t* __restrict__ sf, int g, int r, int tiles_per_group, int tile_rows,
+                                            int num_kb, int kb) {
+    const int tile = r / tile_rows, rt = r - tile * tile_rows;
+    const int atoms = (tile_rows + 127) >> 7, atom = rt >> 7, ra = rt & 127;
+    const long long chunk = ((static_cast<long long>(g) * tiles_per_group + tile) * num_kb + kb) * atoms + atom;
+    return __ldg(sf + chunk * 128 + (ra & 31) * 4 + (ra >> 5));
 }
-// smem (32 rows x 128 bit) -> TMEM (32 lanes x 4 columns, replicated into the 4 lane quadrants) in BOTH CTAs of the pair
-__device__ __forceinline__ void utccp_32x128b_2sm(uint32_t taddr, uint64_t sdesc) {
-    asm volatile("tcgen05.cp.cta_group::2.32x128b.warpx4 [%0], %1;" ::"r"(taddr), "l"(sdesc) : "memory");
-}
-__device__ __forceinline__ void umma_mxf8_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t tmem_sfa, uint32_t tmem_sfb, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(tmem_sfa), "r"(tmem_sfb)
-        : "memory");
-}
+__device__ __forceinline__ float e8m0_scale(uint32_t word, int ks) { return __uint_as_float(((word >> (8 * ks)) & 0xFFu) << 23); }
 
 template <bool OUT_F32>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS, 1)
-gemm_fp8_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                const __grid_constant__ CUtensorMap tmSFA, const __grid_constant__ CUtensorMap tmSFB) {
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_fp8_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full = empty_bar + STAGES;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-    // epilogue geometry: 32-column chunks; a chunk row is 64 B (bf16) or 128 B (fp32) + 16 B pad in the staging slab
-    constexpr int EPI_WARPS = OUT_F32 ? 4 : 8;
-    constexpr int EPI_ROW_BYTES = OUT_F32 ? 144 : 80;
-    constexpr int EPI_WARP_BYTES = 32 * EPI_ROW_BYTES;
-    static_assert(EPI_WARPS * EPI_WARP_BYTES <= EPI_BYTES, "epilogue staging");
-
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    const uint32_t cta_rank = cluster_ctarank();
-    const bool leader = cta_rank == 0;
-
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-        tma_prefetch_desc(&tmSFA);
-        tma_prefetch_desc(&tmSFB);
         for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full_bar[i], 2);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full[i], 1);
-            mbar_init(&tmem_empty[i], 2 * EPI_WARPS);   // every epilogue warp of both CTAs
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
         }
         fence_mbar_init();
     }
-    cluster_sync_all();
-    if (warp == 1) tmem_alloc_2sm(tmem_ptr, 512);
-    tcgen05_fence_before();
-    cluster_sync_all();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
+    __syncthreads();
+    const int total_tiles = p.num_m_tiles * p.n_tiles;
 
-    const int n_tiles = p.n_tiles;
-    const int num_kb = p.num_kb;
-    const int total_tiles = p.num_m_tiles * n_tiles;
-    const int pair_id = blockIdx.x >> 1;
-    const int num_pairs = gridDim.x >> 1;
-
-    auto decode = [&](int tile, int& m_tile, int& n_tile, int& group) -> bool {
-        m_tile = tile / n_tiles;
-        n_tile = tile - m_tile * n_tiles;
-        group = p.tile_group ? __ldg(p.tile_group + 2 * m_tile) : 0;
-        return group >= 0;
-    };
-
-    if (warp == 0 && lane == 0) {
-        // =============================================================== TMA producer (both CTAs)
-        if (p.wait_flags) {
+    if (warp == 8) {
+        if (lane != 0) return;
+        // =============================================================== TMA producer
+        if (p.wait_flags) {   // rows pushed by peer GPUs over NVLink must have landed before the first TMA load
             const unsigned long long t_wait = globaltimer_ns();
             for (int sidx = 0; sidx < p.wait_count; ++sidx)
                 spin_flag_ft(p.wait_flags + sidx, p.wait_epoch + (p.epoch_base ? p.epoch_base[0] : 0), p.status, sidx,
                              p.epoch_base ? p.epoch_base[1] : 0);
-            // exposed communication wait (ns) of this rank: status[2..3] is a 64-bit counter (EngineContext.wait_ns)
             if (blockIdx.x == 0) atomicAdd(reinterpret_cast<unsigned long long*>(p.status + 2), globaltimer_ns() - t_wait);
             fence_proxy_async_global();
         }
         int stage = 0;
         uint32_t phase = 0;
-        for (int tile = pair_id; tile < total_tiles; tile += num_pairs) {
-            int m_tile, n_tile, g;
-            if (!decode(tile, m_tile, n_tile, g)) continue;
-            const int my_m = m_tile * TILE_M + cta_rank * CTA_M;
-            const int my_n = n_tile * TILE_N + cta_rank * CTA_N;
-            const int sfa_row = (my_m >> 7) * num_kb;                      // [row tile of 128][kb] chunks of 512 B
-            const int sfb_row = ((g * n_tiles + n_tile) * num_kb) * 2;     // [g][n tile][kb][2 atoms]
-            for (int kb = 0; kb < num_kb; ++kb) {
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
+            const int g = p.tile_group ? __ldg(p.tile_group + m_tile) : 0;
+            if (g < 0) continue;
+            for (int kb = 0; kb < p.num_kb; ++kb) {
                 mbar_wait(&empty_bar[stage], phase ^ 1);
                 uint8_t* sa = smem + stage * STAGE_BYTES;
-                if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * STAGE_TX);
-                tma_load_2d_2sm(sa, &tmA, &full_bar[stage], kb * BLOCK_K, my_m);
-                tma_load_3d_2sm(sa + A_BYTES, &tmB, &full_bar[stage], kb * BLOCK_K, my_n, g);
-                tma_load_2d_2sm(sa + SFA_OFF, &tmSFA, &full_bar[stage], 0, sfa_row + kb);
-                tma_load_2d_2sm(sa + SFB_OFF, &tmSFB, &full_bar[stage], 0, sfb_row + 2 * kb);
-                if (!leader) mbar_arrive_cluster(&full_bar[stage], 0);
+                mbar_arrive_expect_tx(&full_bar[stage], STAGE_BYTES);
+                tma_load_2d(sa, &tmA, &full_bar[stage], kb * BLOCK_K, m_tile * TILE_M);
+                tma_load_3d(sa + A_BYTES, &tmB, &full_bar[stage], kb * BLOCK_K, n_tile * TILE_N, g);
                 if (++stage == STAGES) {
                     stage = 0;
                     phase ^= 1;
                 }
             }
         }
-    } else if (warp == 1 && lane == 0 && leader) {
-        // =============================================================== MMA issuer (leader CTA only)
-        int stage = 0;
-        uint32_t phase = 0;
-        int iter = 0;
-        const uint32_t tsfa = tmem_base + TMEM_SFA_COL;
-        const uint32_t tsfb = tmem_base + TMEM_SFB_COL;
-        for (int tile = pair_id; tile < total_tiles; tile += num_pairs) {
-            int m_tile, n_tile, g;
-            if (!decode(tile, m_tile, n_tile, g)) continue;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_empty[as], aphase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t tmem_d = tmem_base + as * TILE_N;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tcgen05_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-                const uint32_t sb = sa + A_BYTES;
-                utccp_32x128b_2sm(tsfa, make_sf_desc(sa + SFA_OFF));
-                utccp_32x128b_2sm(tsfb, make_sf_desc(sa + SFB_OFF));
-                utccp_32x128b_2sm(tsfb + 4, make_sf_desc(sa + SFB_OFF + 512));
-#pragma unroll
-                for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                    const uint64_t da = make_smem_desc_sw128(sa + k * UMMA_K, 0, 1024);
-                    const uint64_t db = make_smem_desc_sw128(sb + k * UMMA_K, 0, 1024);
-                    umma_mxf8_ss_2sm(tmem_d, da, db, make_idesc_mxf8(TILE_M, TILE_N, k), tsfa, tsfb,
-                                     (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit_2sm(&empty_bar[stage], 0b11);
-                if (kb == num_kb - 1) umma_commit_2sm(&tmem_full[as], 0b11);
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            ++iter;
-        }
-    } else if (warp >= 2 && warp < 2 + EPI_WARPS) {
-        // =============================================================== epilogue (both CTAs; own 128 rows)
-        // bf16 output: EIGHT warps — two per TMEM lane quadrant, interleaved over the 32-column chunks.  With four warps
-        // one warp per SM sub-partition walked a ~100-instruction dependent chain per chunk (tcgen05.ld -> bias ->
-        // pack -> smem transpose -> stores) and the drain of a tile took longer than its MMAs (ncu: tensor pipe 46 %).
-        const int lane_group = warp & 3;
-        const int chunk_first = (warp - 2) >> 2;             // 0 or 1 (always 0 with four warps)
-        constexpr int CHUNK_STEP = EPI_WARPS / 4;
-        int iter = 0;
-        for (int tile = pair_id; tile < total_tiles; tile += num_pairs) {
-            int m_tile, n_tile, g;
-            if (!decode(tile, m_tile, n_tile, g)) continue;
-            const int n_col = n_tile * TILE_N;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_full[as], aphase);
-            tcgen05_fence_after();
-            const int row_base = m_tile * TILE_M + cta_rank * CTA_M + lane_group * 32;
-            const int row = row_base + lane;
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_group * 32) << 16) + as * TILE_N;
-            uint8_t* slab = smem + EPI_OFFSET + (warp - 2) * EPI_WARP_BYTES;
-#pragma unroll 1
-            for (int c0 = chunk_first * 32; c0 < TILE_N; c0 += CHUNK_STEP * 32) {
-                const int col = n_col + c0;
-                if (col >= p.N) break;  // tail tile (N % 192 != 0): columns past N are never stored
-                uint32_t r[32];
-                tmem_ld_32x32(taddr + c0, r);
-                tmem_ld_wait();
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-                if (p.bias) {
-                    const float4* bp = reinterpret_cast<const float4*>(p.bias + static_cast<long long>(g) * p.N + col);
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 b = __ldg(bp + j);
-                        v[4 * j + 0] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
-                    }
-                }
-                if (p.act == 1) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-                } else if (p.act == 2) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 0.5f * v[j] * (1.f + erff(v[j] * 0.70710678118654752f));
-                }
-                if (p.residual && row < p.M) {
-                    const int4* rp = reinterpret_cast<const int4*>(p.residual + static_cast<long long>(row) * p.ldr + col);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int4 q = __ldg(rp + j);
-                        const uint32_t w[4] = {(uint32_t)q.x, (uint32_t)q.y, (uint32_t)q.z, (uint32_t)q.w};
-#pragma unroll
-                        for (int t = 0; t < 4; ++t) {
-                            const float2 f = unpack_bf16x2(w[t]);
-                            v[8 * j + 2 * t] += f.x;
-                            v[8 * j + 2 * t + 1] += f.y;
-                        }
-                    }
-                }
-                // transpose through a padded smem slab so that the global stores are row-contiguous
-                uint8_t* my = slab + lane * EPI_ROW_BYTES;
-                if (OUT_F32) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        *reinterpret_cast<float4*>(my + 16 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        int4 q;
-                        q.x = pack_bf16x2(v[8 * j + 0], v[8 * j + 1]);
-                        q.y = pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
-                        q.z = pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
-                        q.w = pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
-                        *reinterpret_cast<int4*>(my + 16 * j) = q;
-                    }
-                }
-                __syncwarp();
-                constexpr int ELEM = OUT_F32 ? 4 : 2;
-                constexpr int LANES_PER_ROW = 32 * ELEM / 16;        // 16 B pieces of a 32-column row segment: 8 / 4
-                constexpr int ROWS_PER_INSTR = 32 / LANES_PER_ROW;   // 4 / 8
-                const int piece = lane % LANES_PER_ROW;
-                uint8_t* cbase = reinterpret_cast<uint8_t*>(p.C) + (static_cast<long long>(col) * ELEM + piece * 16);
-                const long long row_bytes = p.ldc * ELEM;
-#pragma unroll
-                for (int i = 0; i < 32 / ROWS_PER_INSTR; ++i) {
-                    const int rl = i * ROWS_PER_INSTR + lane / LANES_PER_ROW;
-                    const int grow = row_base + rl;
-                    const int4 q = *reinterpret_cast<const int4*>(slab + rl * EPI_ROW_BYTES + piece * 16);
-                    if (grow < p.M) *reinterpret_cast<int4*>(cbase + static_cast<long long>(grow) * row_bytes) = q;
-                }
-                __syncwarp();
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(&tmem_empty[as], 0);
-            ++iter;
-        }
+        return;
     }
 
-    tcgen05_fence_before();
-    cluster_sync_all();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc_2sm(tmem_base, 512);
+    // =================================================================== consumers (two warpgroups of 64 rows)
+    const int wg = warp >> 2;
+    const int row_in_tile = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // and + 8
+    const int col_in_tile = 2 * (lane & 3);                             // + 8 j (+ 1)
+    const int w_tiles_per_group = (p.N + W_TILE_ROWS - 1) / W_TILE_ROWS;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[TILE_N / 2], part[TILE_N / 2];
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int m_tile = tile / p.n_tiles, n_tile = tile - m_tile * p.n_tiles;
+        const int g = p.tile_group ? __ldg(p.tile_group + m_tile) : 0;
+        if (g < 0) continue;
+        const int m_row = m_tile * TILE_M, n_col = n_tile * TILE_N;
+#pragma unroll
+        for (int i = 0; i < TILE_N / 2; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+            // block scales of this thread's 2 rows and 32 columns (one 32-bit word = the 4 k-steps of the K block)
+            uint32_t wa[2], wb[TILE_N / 8][2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) wa[h] = sf_word(p.sfa, 0, m_row + row_in_tile + 8 * h, 0, A_TILE_ROWS, p.num_kb, kb);
+#pragma unroll
+            for (int j = 0; j < TILE_N / 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int n = min(n_col + 8 * j + col_in_tile + e, p.N - 1);
+                    wb[j][e] = sf_word(p.sfb, g, n, w_tiles_per_group, W_TILE_ROWS, p.num_kb, kb);
+                }
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * (64 * 128);
+            const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES + A_BYTES);
+#pragma unroll
+            for (int ks = 0; ks < BLOCK_K / MMA_K; ++ks) {
+                wgmma_fence();
+                wgmma_e4m3_n128(part, make_smem_desc_sw128(sa + ks * 32, 0, 1024), make_smem_desc_sw128(sb + ks * 32, 0, 1024));
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs(part);
+                // the 1x32 block scales are powers of two: scaling the block's partial product is exact
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float sa_h = e8m0_scale(wa[h], ks);
+#pragma unroll
+                    for (int j = 0; j < TILE_N / 8; ++j)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e)
+                            acc[4 * j + 2 * h + e] = fmaf(part[4 * j + 2 * h + e] * sa_h, e8m0_scale(wb[j][e], ks),
+                                                          acc[4 * j + 2 * h + e]);
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+        // ------------------------------------------------------------ epilogue from registers
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = m_row + row_in_tile + 8 * h;
+            if (row >= p.M) continue;
+#pragma unroll
+            for (int j = 0; j < TILE_N / 8; ++j) {
+                const int col = n_col + 8 * j + col_in_tile;
+                if (col >= p.N) continue;
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (p.bias) {
+                    const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + static_cast<long long>(g) * p.N + col));
+                    v0 += b.x;
+                    v1 += b.y;
+                }
+                if (p.act == 1) {
+                    v0 = fmaxf(v0, 0.f);
+                    v1 = fmaxf(v1, 0.f);
+                } else if (p.act == 2) {
+                    v0 = 0.5f * v0 * (1.f + erff(v0 * 0.70710678118654752f));
+                    v1 = 0.5f * v1 * (1.f + erff(v1 * 0.70710678118654752f));
+                }
+                if (p.residual) {
+                    const float2 r = unpack_bf16x2(
+                        __ldg(reinterpret_cast<const unsigned int*>(p.residual + static_cast<long long>(row) * p.ldr + col)));
+                    v0 += r.x;
+                    v1 += r.y;
+                }
+                if (OUT_F32)
+                    *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.C) + static_cast<long long>(row) * p.ldc + col) =
+                        make_float2(v0, v1);
+                else
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<bf16*>(p.C) + static_cast<long long>(row) * p.ldc + col) =
+                        pack_bf16x2(v0, v1);
+            }
+        }
     }
 }
 
 // ------------------------------------------------------------------------------------------------ quantisation
-// Scale-factor storage.  Rows are split into tiles of `tile_rows` rows (128 for activations = one CTA's share of an M
-// tile; 192 for weights = one N tile), every tile into atoms of 128 rows, K into blocks of 128 elements.  One
-// (atom, K block) chunk is 128 32-bit words = 512 B, ordered the way tcgen05.cp.32x128b.warpx4 wants them:
+// Scale-factor storage.  Rows are split into tiles of `tile_rows` rows (128 for activations, 192 for weights), every
+// tile into atoms of 128 rows, K into blocks of 128 elements.  One (atom, K block) chunk is 128 32-bit words = 512 B:
 //   word (r % 32) * 4 + (r / 32)  holds the four UE8M0 bytes (k-steps of 32 elements) of row r of the atom.
 // Chunk index = ((tile * num_kb + kb) * atoms_per_tile + atom).
 __host__ __device__ inline long long sf_chunks(long long rows, int tile_rows, int num_kb) {
@@ -453,8 +337,7 @@ static int tmap(CUtensorMap* tm, CUtensorMapDataType dt, int elem_bytes, const v
 }
 
 template <bool OUT_F32>
-static int launch_fp8(const Params& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmSFA,
-                      const CUtensorMap& tmSFB, int max_ctas, cudaStream_t st) {
+static int launch_fp8(const Params& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int max_ctas, cudaStream_t st) {
     auto kern = gemm_fp8_kernel<OUT_F32>;
     static bool configured = false;
     if (!configured) {
@@ -470,10 +353,10 @@ static int launch_fp8(const Params& p, const CUtensorMap& tmA, const CUtensorMap
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     }
-    int pairs = sms / 2;
-    if (max_ctas > 0 && max_ctas / 2 < pairs) pairs = max_ctas / 2 > 0 ? max_ctas / 2 : 1;
-    if (total < pairs) pairs = static_cast<int>(total);
-    kern<<<pairs * 2, NUM_THREADS, SMEM_TOTAL, st>>>(p, tmA, tmB, tmSFA, tmSFB);
+    int grid = sms;
+    if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
+    if (total < grid) grid = static_cast<int>(total);
+    kern<<<grid, NUM_THREADS, SMEM_TOTAL, st>>>(p, tmA, tmB);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : -static_cast<int>(e);
 }
@@ -516,7 +399,7 @@ int lah_quant_mxfp8(const void* in, long long ld_in, int in_f32, void* out, long
 }
 
 // A: e4m3 [a_rows, K] (lda bytes), sfa: activation scales (tile_rows = 128); B: e4m3 [G, N, K], sfb: weight scales
-// (tile_rows = 192).  Expert groups padded to 256 rows; tile_group has one entry per 128 rows (like lah_gemm_mgroup2).
+// (tile_rows = 192).  tile_group has one entry per 128 rows.
 int lah_gemm_mgroup_fp8(const void* A, long long lda, int a_rows, const void* sfa, const void* B, const void* sfb, int G,
                         int N, int K, void* C, long long ldc, int out_f32, int m_valid, int num_m_tiles128,
                         const int* tile_group, const float* bias, const void* residual, long long ldr, int max_ctas,
@@ -524,44 +407,29 @@ int lah_gemm_mgroup_fp8(const void* A, long long lda, int a_rows, const void* sf
     if ((K % 128) || (N % 64) || (lda % 16)) return -2;
     const int num_kb = K / 128;
     const int n_tiles = (N + TILE_N - 1) / TILE_N;
-    CUtensorMap tmA, tmB, tmSFA, tmSFB;
+    CUtensorMap tmA, tmB;
     {
         uint64_t dims[2] = {(uint64_t)K, (uint64_t)a_rows};
         uint64_t str[1] = {(uint64_t)lda};
-        uint32_t box[2] = {BLOCK_K, CTA_M};
+        uint32_t box[2] = {BLOCK_K, TILE_M};
         int r = tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, A, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
         if (r) return r;
     }
     {
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)G};
         uint64_t str[2] = {(uint64_t)K, (uint64_t)N * K};
-        uint32_t box[3] = {BLOCK_K, CTA_N, 1};
+        uint32_t box[3] = {BLOCK_K, TILE_N, 1};
         int r = tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, B, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
         if (r) return r;
     }
-    {
-        const uint64_t chunks = (uint64_t)((a_rows + 127) / 128) * num_kb;
-        uint64_t dims[2] = {128, chunks};
-        uint64_t str[1] = {512};
-        uint32_t box[2] = {128, 1};
-        int r = tmap(&tmSFA, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4, sfa, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (r) return r;
-    }
-    {
-        const uint64_t chunks = (uint64_t)G * n_tiles * num_kb * 2;
-        uint64_t dims[2] = {128, chunks};
-        uint64_t str[1] = {512};
-        uint32_t box[2] = {128, 2};
-        int r = tmap(&tmSFB, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4, sfb, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE);
-        if (r) return r;
-    }
     Params p;
-    p.N = N; p.K = K; p.M = m_valid; p.num_groups = G; p.num_m_tiles = (num_m_tiles128 + 1) / 2; p.n_tiles = n_tiles;
+    p.N = N; p.K = K; p.M = m_valid; p.num_groups = G; p.num_m_tiles = num_m_tiles128; p.n_tiles = n_tiles;
     p.num_kb = num_kb; p.tile_group = tile_group; p.C = C; p.ldc = ldc; p.bias = bias;
     p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr;
     p.wait_flags = wait_flags; p.wait_count = wait_count; p.wait_epoch = wait_epoch; p.epoch_base = lah_get_epoch_base(); p.status = status; p.act = act;
-    return out_f32 ? launch_fp8<true>(p, tmA, tmB, tmSFA, tmSFB, max_ctas, stream)
-                   : launch_fp8<false>(p, tmA, tmB, tmSFA, tmSFB, max_ctas, stream);
+    p.sfa = reinterpret_cast<const uint32_t*>(sfa); p.sfb = reinterpret_cast<const uint32_t*>(sfb);
+    return out_f32 ? launch_fp8<true>(p, tmA, tmB, max_ctas, stream)
+                   : launch_fp8<false>(p, tmA, tmB, max_ctas, stream);
 }
 
 }  // extern "C"

@@ -5,7 +5,7 @@
 // (/root/reference/experiments/throughput/layers.py:9-15); per-expert affine parameters gamma/beta are stacked [G, C].
 //
 // Rows are grouped by expert in 128-row tiles; tile_group[t] gives the expert (or -1: tile unused, skipped).
-#include "sm100.cuh"
+#include "sm90.cuh"
 #include <cuda_fp8.h>
 #include <stdlib.h>
 
@@ -154,7 +154,9 @@ __global__ void __launch_bounds__(256, 2) ln_relu_fwd_kernel(
 
 // ------------------------------------------------------------------------------------------------
 // backward: one CTA (C/8 threads) per 128-row tile; thread owns 8 consecutive columns, keeps fp32 column
-// accumulators (dgamma, dbeta, dbias) in registers for the whole tile, block-reduces the two row statistics.
+// accumulators (dgamma, dbeta, dbias) in registers for the whole tile, block-reduces the two row statistics.  The
+// tile's column sums go to part[tile][0..2][C]; group_tile_sum_kernel adds them to the group's gradients in tile order, so
+// the result does not depend on the order in which the CTAs finish.
 //   y    = xhat*gamma + beta            (recomputed; relu mask = y > 0)
 //   g    = da * mask                    dbeta += g        dgamma += g * xhat
 //   dxh  = g * gamma
@@ -166,8 +168,7 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
                                                             const float* __restrict__ rstd_in,
                                                             const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, bf16* __restrict__ dh,
-                                                            float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                                            float* __restrict__ dbias,
+                                                            float* __restrict__ part,
                                                             const int* __restrict__ tile_group, int rows, int relu, int tile_rows) {
     constexpr int THREADS = C / 8;
     constexpr int WARPS = THREADS / 32;
@@ -293,23 +294,22 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
         // `tot` is rewritten only after the next batch's first __syncthreads, which every thread reaches
         // after it finished reading tot above -> no extra barrier needed.
     }
-    float* pg = dgamma + static_cast<long long>(g) * C + col;
-    float* pb = dbeta + static_cast<long long>(g) * C + col;
-    float* pbi = dbias + static_cast<long long>(g) * C + col;
+    float* pg = part + static_cast<long long>(tile) * 3 * C + col;
 #pragma unroll
     for (int t = 0; t < 8; ++t) {
-        atomicAdd(pg + t, acc_dg[t]);
-        atomicAdd(pb + t, acc_db[t]);
-        atomicAdd(pbi + t, acc_dbias[t]);
+        pg[t] = acc_dg[t];
+        pg[C + t] = acc_db[t];
+        pg[2 * C + t] = acc_dbias[t];
     }
 }
 
 // ------------------------------------------------------------------------------------------------
 // grouped column sum: out[g, c] += sum over the rows of every 128-row tile of group g of x[row, c]
-// CTA = (tile, 256-column slab); thread owns one column pair, 4 row phases
+// CTA = (tile, 256-column slab); thread owns one column pair, 4 row phases; the tile's sums go to part[tile][C] and are
+// added to out by group_tile_sum_kernel
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(512) grouped_colsum_kernel(const bf16* __restrict__ x, long long ldx,
-                                                             float* __restrict__ out, int C,
+                                                             float* __restrict__ part, int C,
                                                              const int* __restrict__ tile_group, int rows, int tile_rows) {
     __shared__ float2 sm[4][128];
     const int tile = blockIdx.x;
@@ -336,9 +336,32 @@ __global__ void __launch_bounds__(512) grouped_colsum_kernel(const bf16* __restr
             s.x += sm[p][cp].x;
             s.y += sm[p][cp].y;
         }
-        atomicAdd(out + static_cast<long long>(g) * C + col, s.x);
-        atomicAdd(out + static_cast<long long>(g) * C + col + 1, s.y);
+        *reinterpret_cast<float2*>(part + static_cast<long long>(tile) * C + col) = s;
     }
+}
+
+// out_v[g, c] += sum over the tiles t of group g (in increasing t) of part[t][v][c], v < V: a fixed summation order, so
+// the per-group gradients are the same in every run.  Thread = (v, c); tiles with group -1 are skipped.
+__global__ void __launch_bounds__(256) group_tile_sum_kernel(const float* __restrict__ part, int num_tiles, int V, int C,
+                                                             const int* __restrict__ tile_group, float* out0, float* out1,
+                                                             float* out2) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= V * C) return;
+    const int v = i / C, c = i - v * C;
+    float* out = v == 0 ? out0 : (v == 1 ? out1 : out2);
+    int cur = -1;
+    float acc = 0.f;
+    for (int t = 0; t < num_tiles; ++t) {
+        const int g = tile_group ? __ldg(tile_group + t) : 0;
+        if (g < 0) continue;
+        if (g != cur) {
+            if (cur >= 0) out[static_cast<long long>(cur) * C + c] += acc;
+            cur = g;
+            acc = 0.f;
+        }
+        acc += __ldg(part + (static_cast<long long>(t) * V + v) * C + c);
+    }
+    if (cur >= 0) out[static_cast<long long>(cur) * C + c] += acc;
 }
 
 }  // namespace lah
@@ -400,17 +423,20 @@ int lah_ln_relu_fwd_q(const void* h, void* a, float* mean, float* rstd, const fl
     return -2;
 }
 
+// part: scratch of [ceil(rows / tile_rows), 3, C] fp32 (per-tile column sums, reduced in tile order)
 int lah_ln_relu_bwd_t(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
-                      const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, const int* tile_group,
-                      int rows, int C, int relu, int tile_rows, cudaStream_t st) {
+                      const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
+                      const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
     if (shift_of(tile_rows) < 0) return -2;
     const int grid = (rows + tile_rows - 1) / tile_rows;
 #define LAH_LN_BWD(CC)                                                                                          \
     if (C == CC) {                                                                                              \
         ln_relu_bwd_kernel<CC><<<grid, CC / 8, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd, gamma,    \
-                                                        beta, (bf16*)dh, dgamma, dbeta, dbias, tile_group,     \
-                                                        rows, relu, tile_rows);                                 \
+                                                        beta, (bf16*)dh, part, tile_group, rows, relu,         \
+                                                        tile_rows);                                             \
+        group_tile_sum_kernel<<<(3 * CC + 255) / 256, 256, 0, st>>>(part, grid, 3, CC, tile_group, dgamma,     \
+                                                                     dbeta, dbias);                            \
         return -(int)cudaGetLastError();                                                                        \
     }
     LAH_LN_BWD(256) LAH_LN_BWD(512) LAH_LN_BWD(1024) LAH_LN_BWD(2048) LAH_LN_BWD(4096)
@@ -419,23 +445,27 @@ int lah_ln_relu_bwd_t(const void* da, const void* h, const float* mean, const fl
 }
 
 int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
-                    const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, const int* tile_group,
-                    int rows, int C, int relu, cudaStream_t st) {
-    return lah_ln_relu_bwd_t(da, h, mean, rstd, gamma, beta, dh, dgamma, dbeta, dbias, tile_group, rows, C, relu, 128, st);
+                    const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
+                    const int* tile_group, int rows, int C, int relu, cudaStream_t st) {
+    return lah_ln_relu_bwd_t(da, h, mean, rstd, gamma, beta, dh, dgamma, dbeta, dbias, part, tile_group, rows, C, relu, 128,
+                             st);
 }
 
-int lah_grouped_colsum_t(const void* x, long long ldx, float* out, int C, const int* tile_group, int rows, int tile_rows,
-                         cudaStream_t st) {
+// part: scratch of [ceil(rows / tile_rows), C] fp32 (per-tile column sums, reduced in tile order)
+int lah_grouped_colsum_t(const void* x, long long ldx, float* out, float* part, int C, const int* tile_group, int rows,
+                         int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
     if (C % 256 || shift_of(tile_rows) < 0) return -2;
-    dim3 grid((rows + tile_rows - 1) / tile_rows, (C + 255) / 256);
-    grouped_colsum_kernel<<<grid, 512, 0, st>>>((const bf16*)x, ldx, out, C, tile_group, rows, tile_rows);
+    const int tiles = (rows + tile_rows - 1) / tile_rows;
+    dim3 grid(tiles, (C + 255) / 256);
+    grouped_colsum_kernel<<<grid, 512, 0, st>>>((const bf16*)x, ldx, part, C, tile_group, rows, tile_rows);
+    group_tile_sum_kernel<<<(C + 255) / 256, 256, 0, st>>>(part, tiles, 1, C, tile_group, out, nullptr, nullptr);
     return -(int)cudaGetLastError();
 }
 
-int lah_grouped_colsum(const void* x, long long ldx, float* out, int C, const int* tile_group, int rows,
+int lah_grouped_colsum(const void* x, long long ldx, float* out, float* part, int C, const int* tile_group, int rows,
                        cudaStream_t st) {
-    return lah_grouped_colsum_t(x, ldx, out, C, tile_group, rows, 128, st);
+    return lah_grouped_colsum_t(x, ldx, out, part, C, tile_group, rows, 128, st);
 }
 
 }  // extern "C"

@@ -6,7 +6,7 @@
 // GPU, every GPU's heap mapped into every peer):
 //
 //   gate_topk        product-key scores + liveness table + Bernoulli failure injection -> exact top-k, softmax over the
-//                    survivors, per-expert slot allocation (the TaskPool "batch assembly" becomes an atomic counter)
+//                    survivors, per-expert slot allocation (the TaskPool "batch assembly" becomes a per-expert rank in token order)
 //   layout_exchange  every rank stores its per-expert counts into every peer (P2P st), release/acquire flags, then each
 //                    rank derives the SAME global layout: rows grouped by expert, groups padded to 128 rows
 //   scatter_rows     fused permute + P2P store of token rows into the owner GPU's receive buffer (+ zero padding rows)
@@ -17,7 +17,7 @@
 // Memory ordering protocol (SURVEY.md §5.2): data is written with plain stores, then `__threadfence_system()` +
 // `st.release.sys` of a monotonically increasing epoch into the consumer's flag word; consumers poll with
 // `ld.acquire.sys`.  Flags never need resetting.  Every poll loop has a clock64() timeout that raises status[0].
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace lah {
 
@@ -230,8 +230,42 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
         const long long o = static_cast<long long>(b) * k + lane;
         idx_out[o] = id;
         w_out[o] = id >= 0 ? __expf(v - mx) / denom : 0.f;
-        pos_out[o] = id >= 0 ? atomicAdd(counts + id, 1) : 0;
+        if (id < 0) pos_out[o] = 0;   // slots of the routed pairs: rank_slots_kernel
     }
+}
+
+// slot of every routed (token, choice) pair inside its expert = the number of EARLIER pairs (token-major order) routed to
+// the same expert; counts[e] += pairs routed to e.  One CTA per expert: the row order inside every expert group, and with
+// it every reduction over an expert's rows, is the same in every run (an atomic slot counter would order rows by arrival).
+__global__ void __launch_bounds__(1024) rank_slots_kernel(const int* __restrict__ idx, int n, int* __restrict__ pos,
+                                                          int* __restrict__ counts) {
+    __shared__ int warp_off[32];
+    __shared__ int s_total;
+    const int e = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    int base = 0;
+    for (int start = 0; start < n; start += 1024) {
+        const int i = start + tid;
+        const bool hit = i < n && __ldg(idx + i) == e;
+        const unsigned m = __ballot_sync(0xffffffffu, hit);
+        if (lane == 0) warp_off[warp] = __popc(m);
+        __syncthreads();
+        if (warp == 0) {
+            const int v = warp_off[lane];
+            int incl = v;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, incl, d);
+                if (lane >= d) incl += y;
+            }
+            warp_off[lane] = incl - v;
+            if (lane == 31) s_total = incl;
+        }
+        __syncthreads();
+        if (hit) pos[i] = base + warp_off[warp] + __popc(m & ((1u << lane) - 1u));
+        base += s_total;
+        __syncthreads();   // warp_off / s_total are rewritten by the next chunk
+    }
+    if (tid == 0 && base) counts[e] += base;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -245,7 +279,7 @@ struct LayoutArgs {
     int E, E_loc;
     int max_rows;            // capacity of the receive buffers (rows)
     int max_tiles;           // max_rows / tile_rows
-    int align;               // group padding in rows: 128 (1-CTA GEMM), 256 (CTA-pair GEMM) or 16 (small-M swap-AB path)
+    int align;               // group padding in rows: 128 (1-CTA GEMM), 256 (wide-tile GEMM) or 16 (small-M swap-AB path)
     int tile_rows;           // rows per tile_group entry: min(align, 128)
     int* counts;             // [E] local counts (zeroed on exit)
     int* dst_row;            // [E]  row (in route_owner[e]'s buffer) where MY first row for expert e goes
@@ -934,7 +968,7 @@ int lah_nvls_allreduce(long long off, long long n, float scale, cudaStream_t st)
     if (n % 4 || off % 16) return -2;
     long long blocks = (n / 4 / g_peers.world + 255) / 256;
     if (blocks < 1) blocks = 1;
-    if (blocks > 148 * 4) blocks = 148 * 4;
+    if (blocks > 132 * 4) blocks = 132 * 4;
     nvls_allreduce_kernel<<<(int)blocks, 256, 0, st>>>(g_peers, off, n, scale);
     return -(int)cudaGetLastError();
 }
@@ -991,6 +1025,7 @@ int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, 
     gate_topk_kernel<<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(logits, B, gs, k, alive, failure_rate, seed,
                                                                            token_offset, idx, w, pos, counts,
                                                                            g_peers.step_ctr);
+    rank_slots_kernel<<<gs.num_experts, 1024, 0, st>>>(idx, B * k, pos, counts);
     return -(int)cudaGetLastError();
 }
 

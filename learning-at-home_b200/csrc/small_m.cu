@@ -1,34 +1,35 @@
 // small_m.cu — the "many small requests" regime of the reference (64 trainers x batch 4 -> O(1..64) rows per expert and
-// step; /root/reference/experiments/convergence notebooks, lib/runtime/task_pool.py:105-125) on sm_100a.
+// step; reference: experiments/convergence notebooks, lib/runtime/task_pool.py:105-125) on sm_90a.
 //
 // With a handful of rows per expert every expert GEMM is a WEIGHT-STREAMING problem (12.6 MB of bf16 weights per
 // active expert and forward at hid 512) and the optimizer is a STATE-STREAMING problem (fp32 p, m, v, vmax).  Two
-// kernels, both persistent / warp-specialised / TMA-fed with accumulators in TMEM:
+// kernels, both persistent / warp-specialised / TMA-fed, with wgmma accumulators in registers (two consumer warpgroups of
+// 64 MMA rows each, one TMA producer warp):
 //
 //   swapab_kernel      D^T[out_features, tokens] = W[out_features, K] * X^T[K, tokens]   ("swap-AB": the weights sit on
 //                      the 128-wide MMA-M side, the expert's 16..128 tokens on the MMA-N side, so a group of 16 rows
-//                      costs one N=16 instruction instead of a 256-row padded tile).  A tile = (expert, 128-token
+//                      costs N=16 instructions instead of a 128-row padded tile).  A tile = (expert, 128-token
 //                      chunk, 128-row slice of the weight matrix) streamed through a 6-stage TMA ring; experts with
 //                      more than 128 rows are spread over several CTAs (hot experts).  A_MN selects dgrad
 //                      (W^T read straight from the same [out, in] tensor as an MN-major operand).
-//   wgrad_adam_kernel  dW tile = dY^T X on tcgen05 (both operands MN-major, two 32-token stages, reduction over the
+//   wgrad_adam_kernel  dW tile = dY^T X with wgmma (both operands MN-major, two 32-token stages, reduction over the
 //                      expert's tokens = the gradient reduction over all trainers that routed to it) with the per-expert AMSGrad step FUSED
-//                      INTO THE EPILOGUE: p / m / v / vmax tiles arrive through TMA (128B-swizzled smem, per-warp
-//                      3-slot ring), are updated in place from the TMEM accumulator and leave through TMA stores; the
-//                      bf16 mirror is written from registers.  The weight gradient never exists in HBM: 34 B / parameter
+//                      INTO THE EPILOGUE: every thread reads p / m / v / vmax at the positions of its accumulator
+//                      registers (four 8-column groups at a time, so 32 loads are in flight per thread), updates them
+//                      and writes them back together with the bf16 mirror.  The weight gradient never exists in HBM: 34 B / parameter
 //                      instead of 46 (wgrad write 4 + Adam 38 + re-read 4).
 //                      Reference semantics: one torch.optim.Adam(amsgrad=True) step per expert right after its backward
 //                      (/root/reference/lib/runtime/expert_backend.py:90-97).
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace lah {
 namespace smallm {
 
 constexpr int BM = 128;      // MMA M: weight rows (swapab) / dY features (wgrad)
 constexpr int BK = 64;       // k elements per stage row (128 B of bf16 = one swizzle row)
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int BN_MAX = 128;  // max tokens per MMA (swapab) / X features per tile (wgrad)
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 288;   // two consumer warpgroups + one producer warp
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -87,7 +88,7 @@ constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
 constexpr int QD = 4;                         // depth of the tile queue (dynamic scheduler)
 constexpr int MAX_G = 1023;                   // groups per launch (prefix table of 128-token chunks lives in smem)
-constexpr int CUM_OFFSET = BAR_OFFSET + (2 * STAGES + 4 + 2 * QD) * 8 + QD * 4 + 16;
+constexpr int CUM_OFFSET = BAR_OFFSET + (2 * STAGES + 2 * QD) * 8 + QD * 4 + 16;
 constexpr int SMEM_TOTAL = CUM_OFFSET + (MAX_G + 1) * 4 + 1024;
 static_assert(SMEM_TOTAL <= 232448, "shared memory budget");
 
@@ -109,9 +110,9 @@ struct Params {
 
 __device__ __forceinline__ int box_rows_of(int nn) { return nn <= 16 ? 16 : (nn <= 32 ? 32 : (nn <= 64 ? 64 : 128)); }
 
-// Tiles are handed out DYNAMICALLY: SMs do not get equal shares of HBM bandwidth (ncu on the static version: SMs idle 15-20 %
-// of the kernel waiting for the slowest one), so the TMA-producer thread of every CTA draws the next tile from a global
-// counter and publishes it to the other roles of its CTA through a small smem queue.
+// Tiles are handed out DYNAMICALLY: SMs do not get equal shares of HBM bandwidth (a static split leaves the fast SMs idle
+// while they wait for the slowest one), so the TMA-producer thread of every CTA draws the next tile from a global
+// counter and publishes it to the consumer warps of its CTA through a small smem queue.
 // A tile is (group, 128-token chunk, 128-feature slice): a HOT expert (routing collapses while training; with 8 experts per
 // rank one of them can hold > 1000 of the rank's rows) is split over as many CTAs as it has chunks instead of one CTA
 // walking all of its chunks back to back - the slowest rank of a step is the one that owns the hottest expert, and every
@@ -125,6 +126,70 @@ __device__ __forceinline__ int find_group(const int* cum, int G, int gc) {   // 
     return lo;
 }
 
+// mainloop + epilogue of one tile for a token box of NB rows (MMA N = NB); warpgroup wg owns weight rows [64wg, 64wg + 64)
+template <int NB, bool A_MN>
+__device__ __forceinline__ void sab_tile(const Params& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& stage,
+                                         uint32_t& phase, int num_kb, int wg, int warp, int lane, int g, int ms, int row0,
+                                         int nn) {
+    float acc[NB / 2];
+    constexpr uint32_t A_KSTEP = A_MN ? MMA_K * 128 : MMA_K * 2;
+    int prev_stage = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + wg * (A_MN ? BK * 128 : 64 * 128);
+        const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES + A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k) {
+            const uint64_t da = make_smem_desc_sw128(sa + k * A_KSTEP, BK * 128, 1024);
+            const uint64_t db = make_smem_desc_sw128(sb + k * (MMA_K * 2), 0, 1024);
+            const uint32_t accum = (kb > 0 || k > 0) ? 1u : 0u;
+            if constexpr (NB == 16) wgmma_bf16_n16<A_MN, 0>(acc, da, db, accum);
+            if constexpr (NB == 32) wgmma_bf16_n32<A_MN, 0>(acc, da, db, accum);
+            if constexpr (NB == 64) wgmma_bf16_n64<A_MN, 0>(acc, da, db, accum);
+            if constexpr (NB == 128) wgmma_bf16_n128<A_MN, 0>(acc, da, db, accum);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_stage >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        }
+        prev_stage = stage;
+        if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+        }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    __syncwarp();
+    if (lane == 0 && prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    // epilogue: accumulator row = output feature, column = token.  The padding rows of the group's last 16-row block are
+    // WRITTEN too (their inputs are zero rows, so they get bias / zero): every later kernel may then read whole 16-row
+    // blocks without meeting stale memory, and the k-step masked wgrad sees exact zeros there
+    const int n16 = (nn + 15) & ~15;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int feat = ms * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        const float bias = p.bias ? __ldg(p.bias + static_cast<long long>(g) * p.M_out + feat) : 0.f;
+#pragma unroll
+        for (int j = 0; j < NB / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = 8 * j + 2 * (lane & 3) + e;
+                if (n < n16) {
+                    const long long row = row0 + n;
+                    float v = acc[4 * j + 2 * h + e] + bias;
+                    if (p.residual) v += __bfloat162float(p.residual[row * p.ldr + feat]);
+                    p.out[row * p.ldo + feat] = __float2bfloat16(v);
+                }
+            }
+        }
+    }
+}
+
 template <bool A_MN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB16,
@@ -134,18 +199,15 @@ swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __g
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full = empty_bar + STAGES;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint64_t* q_full = tmem_empty + 2;
+    uint64_t* q_full = empty_bar + STAGES;
     uint64_t* q_empty = q_full + QD;
     volatile int* q_tile = reinterpret_cast<volatile int*>(q_empty + QD);
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(const_cast<int*>(q_tile) + QD);
     int* cum = reinterpret_cast<int*>(smem + CUM_OFFSET);   // cum[g] = 128-token chunks of the groups before g
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
 
-    if (warp == 2) {   // prefix table of chunks (warp scan, 32 groups per round)
+    if (warp == 0) {   // prefix table of chunks (warp scan, 32 groups per round)
         int carry = 0;
         for (int base = 0; base < p.G; base += 32) {
             const int g = base + lane;
@@ -160,7 +222,7 @@ swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __g
         }
         if (lane == 0) cum[0] = 0;
     }
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB16);
         tma_prefetch_desc(&tmB32);
@@ -168,29 +230,22 @@ swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __g
         tma_prefetch_desc(&tmB128);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full[i], 1);
-            mbar_init(&tmem_empty[i], 4);
+            mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
         }
         for (int i = 0; i < QD; ++i) {
             mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 5);   // MMA thread + 4 epilogue warps
+            mbar_init(&q_empty[i], 8);
         }
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(tmem_ptr, 2 * BN_MAX);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     const int m_slices = p.M_out / BM;
     const int total = cum[p.G] * m_slices;
     const int num_kb = p.K / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8) {
+        if (lane != 0) return;
         // =============================================================== scheduler + TMA producer
         if (p.wait_flags) {
             const int epoch = p.wait_epoch + (p.epoch_base ? *p.epoch_base : 0);
@@ -239,110 +294,34 @@ swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __g
                 }
             }
         }
-    } else if (warp == 1 && lane == 0) {
-        // =============================================================== MMA issuer
-        constexpr uint32_t A_LBO = A_MN ? BK * 128 : 0;
-        constexpr uint32_t A_KSTEP = A_MN ? UMMA_K * 128 : UMMA_K * 2;
-        int stage = 0, qi = 0;
-        uint32_t phase = 0, qphase = 0;
-        int iter = 0;
-        while (true) {
-            mbar_wait(&q_full[qi], qphase);
-            const int tile = q_tile[qi];
-            mbar_arrive(&q_empty[qi]);
-            if (++qi == QD) {
-                qi = 0;
-                qphase ^= 1;
-            }
-            if (tile >= total) break;
-            const int gc = tile / m_slices;
-            const int g = find_group(cum, p.G, gc);
-            const int nn = min(__ldg(p.group_rows + g) - (gc - cum[g]) * BN_MAX, BN_MAX);
-            const uint32_t n16 = static_cast<uint32_t>((nn + 15) & ~15);
-            const uint32_t idesc = make_idesc_bf16_f32(BM, n16, A_MN ? 1u : 0u, 0u);
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_empty[as], aphase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BN_MAX;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                tcgen05_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-                const uint32_t sb = sa + A_BYTES;
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k) {
-                    const uint64_t da = make_smem_desc_sw128(sa + k * A_KSTEP, A_LBO, 1024);
-                    const uint64_t db = make_smem_desc_sw128(sb + k * (UMMA_K * 2), 0, 1024);
-                    umma_bf16_ss(tmem_d, da, db, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&empty_bar[stage]);
-                if (kb == num_kb - 1) umma_commit(&tmem_full[as]);
-                if (++stage == STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            ++iter;
-        }
-    } else if (warp >= 2) {
-        // =============================================================== epilogue: thread = output feature, column = token
-        const int lane_group = warp & 3;
-        int iter = 0, qi = 0;
-        uint32_t qphase = 0;
-        while (true) {
-            mbar_wait(&q_full[qi], qphase);
-            const int tile = q_tile[qi];
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&q_empty[qi]);
-            if (++qi == QD) {
-                qi = 0;
-                qphase ^= 1;
-            }
-            if (tile >= total) break;
-            const int gc = tile / m_slices, ms = tile - gc * m_slices;
-            const int g = find_group(cum, p.G, gc);
-            const int n0 = (gc - cum[g]) * BN_MAX;
-            const int nn = min(__ldg(p.group_rows + g) - n0, BN_MAX);
-            const int off = __ldg(p.group_off + g);
-            const int feat = ms * BM + lane_group * 32 + lane;
-            const float bias = p.bias ? __ldg(p.bias + static_cast<long long>(g) * p.M_out + feat) : 0.f;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_full[as], aphase);
-            tcgen05_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lane_group * 32) << 16) + as * BN_MAX;
-            // the padding rows of the group's last 16-row block are WRITTEN too (their inputs are zero rows, so they get
-            // bias / zero): every later kernel may then read whole 16-row blocks without meeting stale memory, and the
-            // k-step masked wgrad sees exact zeros there
-            const int n16 = (nn + 15) & ~15;
-#pragma unroll 1
-            for (int c0 = 0; c0 < n16; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld_32x32(taddr + c0, r);
-                tmem_ld_wait();
-                const int cn = min(32, n16 - c0);
-                const long long row0 = off + n0 + c0;
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    if (j < cn) {
-                        float v = __uint_as_float(r[j]) + bias;
-                        if (p.residual) v += __bfloat162float(p.residual[(row0 + j) * p.ldr + feat]);
-                        p.out[(row0 + j) * p.ldo + feat] = __float2bfloat16(v);   // warp: 32 consecutive features = 64 B
-                    }
-                }
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[as]);
-            ++iter;
-        }
+        return;
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 2 * BN_MAX);
+
+    // =================================================================== consumers (two warpgroups)
+    const int wg = warp >> 2;
+    int stage = 0, qi = 0;
+    uint32_t phase = 0, qphase = 0;
+    while (true) {
+        mbar_wait(&q_full[qi], qphase);
+        const int tile = q_tile[qi];
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&q_empty[qi]);
+        if (++qi == QD) {
+            qi = 0;
+            qphase ^= 1;
+        }
+        if (tile >= total) break;
+        const int gc = tile / m_slices, ms = tile - gc * m_slices;
+        const int g = find_group(cum, p.G, gc);
+        const int n0 = (gc - cum[g]) * BN_MAX;
+        const int nn = min(__ldg(p.group_rows + g) - n0, BN_MAX);
+        const int row0 = __ldg(p.group_off + g) + n0;
+        switch (box_rows_of(nn)) {
+            case 16: sab_tile<16, A_MN>(p, smem, full_bar, empty_bar, stage, phase, num_kb, wg, warp, lane, g, ms, row0, nn); break;
+            case 32: sab_tile<32, A_MN>(p, smem, full_bar, empty_bar, stage, phase, num_kb, wg, warp, lane, g, ms, row0, nn); break;
+            case 64: sab_tile<64, A_MN>(p, smem, full_bar, empty_bar, stage, phase, num_kb, wg, warp, lane, g, ms, row0, nn); break;
+            default: sab_tile<128, A_MN>(p, smem, full_bar, empty_bar, stage, phase, num_kb, wg, warp, lane, g, ms, row0, nn); break;
+        }
     }
 }
 
@@ -354,17 +333,13 @@ swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __g
 namespace wa {
 
 constexpr int WBK = 32;                                  // tokens per operand stage
-constexpr int OP_STAGES = 2;                             // a hot expert has tens of k-blocks: loads run ahead of the MMAs
+constexpr int OP_STAGES = 4;                             // a hot expert has tens of k-blocks: loads run ahead of the MMAs
 constexpr int OP_STAGE_BYTES = 2 * (WBK * BM * 2);       // A [32 t][128 n] + B [32 t][128 k] (two 64-wide MN atoms each)
 constexpr int OP_BYTES = OP_STAGES * OP_STAGE_BYTES;
-constexpr int SLOTS = 3;                                 // state ring per epilogue warp
-constexpr int STATE_TILE = 32 * 128;                     // 32 rows x 32 fp32 (one swizzle-128B atom group)
-constexpr int SLOT_BYTES = 4 * STATE_TILE;               // p, m, v, vmax
-constexpr int STATE_OFFSET = OP_BYTES;
-constexpr int BAR_OFFSET = STATE_OFFSET + 4 * SLOTS * SLOT_BYTES;
+constexpr int BAR_OFFSET = OP_BYTES;
 constexpr int QD = 4;                                    // depth of the tile queue (dynamic scheduler)
-constexpr int CHUNKS = BN_MAX / 32;                      // 32-column chunks per tile
-constexpr int SMEM_TOTAL = BAR_OFFSET + (2 * OP_STAGES + 4 + 4 * SLOTS + 2 * QD) * 8 + QD * 4 + 16 + 1024;
+constexpr int SMEM_TOTAL = BAR_OFFSET + (2 * OP_STAGES + 2 * QD) * 8 + QD * 4 + 16 + 1024;
+constexpr int JB = 4;                                    // 8-column groups whose state is loaded together
 static_assert(SMEM_TOTAL <= 232448, "shared memory budget");
 
 struct Params {
@@ -373,6 +348,10 @@ struct Params {
     const int* group_rows;    // [G] valid rows (0: the expert is not stepped)
     const int* skip;          // optional [G, 2]: skip[2g] >= 0 -> handled by the unfused path (shadowed experts)
     const int* step;          // [G] per-expert step count AFTER this update
+    float* p;                 // [G, N, K] fp32 master weights and AMSGrad state
+    float* m;
+    float* v;
+    float* vmax;
     bf16* p_bf16;             // [G, N, K] bf16 mirror consumed by the GEMMs
     float lr, beta1, beta2, eps;
     int amsgrad;
@@ -385,55 +364,33 @@ struct Tile {
 };
 
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX,
-                  const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmM,
-                  const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmVM) {
+wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* op_full = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
     uint64_t* op_empty = op_full + OP_STAGES;
-    uint64_t* tmem_full = op_empty + OP_STAGES;   // [2]
-    uint64_t* tmem_empty = tmem_full + 2;   // [2]
-    uint64_t* st_full = tmem_empty + 2;     // [4 warps][SLOTS]
-    uint64_t* q_full = st_full + 4 * SLOTS;
+    uint64_t* q_full = op_empty + OP_STAGES;
     uint64_t* q_empty = q_full + QD;
     volatile int* q_tile = reinterpret_cast<volatile int*>(q_empty + QD);
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(const_cast<int*>(q_tile) + QD);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     if (p.poison && (*p.poison & 1)) return;   // degraded step (a peer timed out): no optimizer step from partial data
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmDY);
         tma_prefetch_desc(&tmX);
-        tma_prefetch_desc(&tmP);
-        tma_prefetch_desc(&tmM);
-        tma_prefetch_desc(&tmV);
-        tma_prefetch_desc(&tmVM);
         for (int i = 0; i < OP_STAGES; ++i) {
             mbar_init(&op_full[i], 1);
-            mbar_init(&op_empty[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full[i], 1);
-            mbar_init(&tmem_empty[i], 4);
+            mbar_init(&op_empty[i], 8);
         }
         for (int i = 0; i < QD; ++i) {
             mbar_init(&q_full[i], 1);
-            mbar_init(&q_empty[i], 5);   // MMA thread + 4 epilogue warps
+            mbar_init(&q_empty[i], 8);
         }
         fence_mbar_init();
     }
-    if (warp >= 2 && lane == 0) {   // every epilogue warp owns (initialises, arms, waits on) the barriers of its state ring
-        for (int i = 0; i < SLOTS; ++i) mbar_init(&st_full[(warp - 2) * SLOTS + i], 1);
-        fence_mbar_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_ptr, 2 * BN_MAX);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     const int n_tiles = p.K / BN_MAX;
     const int tiles_per_group = (p.N / BM) * n_tiles;
@@ -447,10 +404,11 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
         return t;
     };
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8) {
+        if (lane != 0) return;
         // =============================================================== scheduler + operand producer (dY^T / X^T k-blocks)
         // tiles are drawn from a global counter (work stealing: SMs see different HBM bandwidth, a static split leaves the
-        // fast ones idle for ~15 % of the kernel) and published to the MMA thread and the epilogue warps through a queue
+        // fast ones idle) and published to the consumer warps through a queue
         uint32_t phase = 0, qphase = 0;
         int qi = 0, stage = 0;
         while (true) {
@@ -489,177 +447,102 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                 }
             }
         }
-    } else if (warp == 1 && lane == 0) {
-        // =============================================================== MMA issuer: only ceil(rows/16) k-steps of a block
-        constexpr uint32_t idesc = make_idesc_bf16_f32(BM, BN_MAX, 1u, 1u);
-        uint32_t phase = 0, qphase = 0;
-        int iter = 0, qi = 0, stage = 0;
-        while (true) {
-            mbar_wait(&q_full[qi], qphase);
-            const int tile = q_tile[qi];
-            mbar_arrive(&q_empty[qi]);
-            if (++qi == QD) {
-                qi = 0;
-                qphase ^= 1;
-            }
-            if (tile >= total) break;
-            const Tile t = decode(tile);
-            const int rows = __ldg(p.group_rows + t.g);
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            mbar_wait(&tmem_empty[as], aphase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t tmem_d = tmem_base + as * BN_MAX;
-            for (int t0 = 0; t0 < rows; t0 += WBK) {
-                mbar_wait(&op_full[stage], phase);
-                tcgen05_fence_after();
-                const uint32_t sa = smem_u32(smem + stage * OP_STAGE_BYTES);
-                const uint32_t sb = sa + WBK * BM * 2;
-                const int ksteps = min(WBK / UMMA_K, (rows - t0 + UMMA_K - 1) / UMMA_K);
-                for (int k = 0; k < ksteps; ++k) {
-                    const uint64_t da = make_smem_desc_sw128(sa + k * (UMMA_K * 128), WBK * 128, 1024);
-                    const uint64_t db = make_smem_desc_sw128(sb + k * (UMMA_K * 128), WBK * 128, 1024);
-                    umma_bf16_ss(tmem_d, da, db, idesc, (t0 > 0 || k > 0) ? 1u : 0u);
-                }
-                umma_commit(&op_empty[stage]);
-                if (t0 + WBK >= rows) umma_commit(&tmem_full[as]);
-                if (++stage == OP_STAGES) {
-                    stage = 0;
-                    phase ^= 1;
-                }
-            }
-            ++iter;
-        }
-    } else if (warp >= 2) {
-        // =============================================================== epilogue: state streaming + AMSGrad
-        const int q = warp & 3;                     // TMEM lane quadrant = rows [32q, 32q+32) of the tile
-        uint8_t* ring = smem + STATE_OFFSET + (warp - 2) * SLOTS * SLOT_BYTES;
-        uint64_t* full = st_full + (warp - 2) * SLOTS;
-        const int n_state = p.amsgrad ? 4 : 3;
-        // chunk n of this CTA = 32-column chunk (n % CHUNKS) of the (n / CHUNKS)-th tile drawn from the queue; the loads run
-        // two chunks ahead of the update, so at most two tiles are live: fifo[(n / CHUNKS) & 1]
-        Tile fifo[2];
-        int fetched = 0, qi = 0;
-        uint32_t qphase = 0;
-        bool drained = false;
-        auto have_chunk = [&](int n) -> bool {
-            while (!drained && n / CHUNKS >= fetched) {
-                mbar_wait(&q_full[qi], qphase);
-                const int tile = q_tile[qi];
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&q_empty[qi]);
-                if (++qi == QD) {
-                    qi = 0;
-                    qphase ^= 1;
-                }
-                if (tile >= total) {
-                    drained = true;
-                } else {
-                    fifo[fetched & 1] = decode(tile);
-                    ++fetched;
-                }
-            }
-            return n / CHUNKS < fetched;
-        };
-        auto issue_load = [&](int n) {   // lane 0 only
-            const Tile& t = fifo[(n / CHUNKS) & 1];
-            const int cc = n % CHUNKS, slot = n % SLOTS;
-            uint8_t* s = ring + slot * SLOT_BYTES;
-            const int col = t.nt * BN_MAX + cc * 32;
-            const int row = t.g * p.N + t.mt * BM + q * 32;
-            mbar_arrive_expect_tx(&full[slot], n_state * STATE_TILE);
-            tma_load_2d(s, &tmP, &full[slot], col, row);
-            tma_load_2d(s + STATE_TILE, &tmM, &full[slot], col, row);
-            tma_load_2d(s + 2 * STATE_TILE, &tmV, &full[slot], col, row);
-            if (p.amsgrad) tma_load_2d(s + 3 * STATE_TILE, &tmVM, &full[slot], col, row);
-        };
-        for (int n = 0; n < SLOTS - 1; ++n)
-            if (have_chunk(n) && lane == 0) issue_load(n);
-        float step_size = 0.f, inv_sqrt_bc2 = 0.f;
-        for (int c = 0; have_chunk(c); ++c) {
-            const Tile t = fifo[(c / CHUNKS) & 1];
-            const int cc = c % CHUNKS, slot = c % SLOTS, iter = c / CHUNKS, as = iter & 1;
-            const uint32_t sphase = (c / SLOTS) & 1;
-            if (cc == 0) {
-                const float st = static_cast<float>(__ldg(p.step + t.g));
-                step_size = p.lr / (1.f - powf(p.beta1, st));
-                inv_sqrt_bc2 = rsqrtf(1.f - powf(p.beta2, st));
-                mbar_wait(&tmem_full[as], (iter >> 1) & 1);
-                tcgen05_fence_after();
-            }
-            // slot (c-1) % SLOTS is refilled with chunk c + SLOTS - 1: its previous contents (chunk c-1) must have been read by
-            // the TMA store engine
-            if (have_chunk(c + SLOTS - 1) && lane == 0) {
-                tma_store_wait_read<0>();
-                issue_load(c + SLOTS - 1);
-            }
-            mbar_wait(&full[slot], sphase);
-            uint32_t r[32];
-            tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * BN_MAX + cc * 32, r);
-            tmem_ld_wait();
-            uint8_t* s = ring + slot * SLOT_BYTES + lane * 128;
-            uint32_t packed[16];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int o = (j ^ (lane & 7)) << 4;
-                float4 pw = *reinterpret_cast<float4*>(s + o);
-                float4 m = *reinterpret_cast<float4*>(s + STATE_TILE + o);
-                float4 v = *reinterpret_cast<float4*>(s + 2 * STATE_TILE + o);
-                float4 vm = p.amsgrad ? *reinterpret_cast<float4*>(s + 3 * STATE_TILE + o) : make_float4(0.f, 0.f, 0.f, 0.f);
-                float* pp = &pw.x; float* mp = &m.x; float* vp = &v.x; float* vmp = &vm.x;
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const float grad = __uint_as_float(r[4 * j + e]);
-                    mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
-                    vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
-                    float denom;
-                    if (p.amsgrad) {
-                        vmp[e] = fmaxf(vmp[e], vp[e]);
-                        denom = sqrtf(vmp[e]) * inv_sqrt_bc2 + p.eps;
-                    } else {
-                        denom = sqrtf(vp[e]) * inv_sqrt_bc2 + p.eps;
-                    }
-                    pp[e] -= step_size * (mp[e] / denom);
-                }
-                *reinterpret_cast<float4*>(s + o) = pw;
-                *reinterpret_cast<float4*>(s + STATE_TILE + o) = m;
-                *reinterpret_cast<float4*>(s + 2 * STATE_TILE + o) = v;
-                if (p.amsgrad) *reinterpret_cast<float4*>(s + 3 * STATE_TILE + o) = vm;
-                packed[2 * j] = pack_bf16x2(pw.x, pw.y);
-                packed[2 * j + 1] = pack_bf16x2(pw.z, pw.w);
-            }
-            {   // bf16 mirror: 64 B per thread straight from registers
-                const long long row = static_cast<long long>(t.g) * p.N + t.mt * BM + q * 32 + lane;
-                int4* dst = reinterpret_cast<int4*>(p.p_bf16 + row * p.K + t.nt * BN_MAX + cc * 32);
-#pragma unroll
-                for (int j = 0; j < 4; ++j)
-                    dst[j] = make_int4(packed[4 * j], packed[4 * j + 1], packed[4 * j + 2], packed[4 * j + 3]);
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-                uint8_t* sb = ring + slot * SLOT_BYTES;
-                const int col = t.nt * BN_MAX + cc * 32;
-                const int row = t.g * p.N + t.mt * BM + q * 32;
-                tma_store_2d(&tmP, sb, col, row);
-                tma_store_2d(&tmM, sb + STATE_TILE, col, row);
-                tma_store_2d(&tmV, sb + 2 * STATE_TILE, col, row);
-                if (p.amsgrad) tma_store_2d(&tmVM, sb + 3 * STATE_TILE, col, row);
-                tma_store_commit();
-            }
-            if (cc == CHUNKS - 1) {   // accumulator fully drained
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tmem_empty[as]);
-            }
-        }
-        if (lane == 0) tma_store_wait<0>();   // all state tiles are in global memory before the CTA exits
+        return;
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc(tmem_base, 2 * BN_MAX);
+
+    // =================================================================== consumers: wgrad tile (MMA) + AMSGrad epilogue
+    const int wg = warp >> 2;
+    int qi = 0, stage = 0;
+    uint32_t phase = 0, qphase = 0;
+    float acc[BN_MAX / 2];
+    while (true) {
+        mbar_wait(&q_full[qi], qphase);
+        const int tile = q_tile[qi];
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&q_empty[qi]);
+        if (++qi == QD) {
+            qi = 0;
+            qphase ^= 1;
+        }
+        if (tile >= total) break;
+        const Tile t = decode(tile);
+        const int rows = __ldg(p.group_rows + t.g);
+        // ---- dW tile: only ceil(rows/16) k-steps of the last block (the group's padding rows up to 16 are zero)
+        int prev_stage = -1;
+        for (int t0 = 0; t0 < rows; t0 += WBK) {
+            mbar_wait(&op_full[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * OP_STAGE_BYTES) + wg * (WBK * 128);
+            const uint32_t sb = smem_u32(smem + stage * OP_STAGE_BYTES + WBK * BM * 2);
+            const int ksteps = min(WBK / MMA_K, (rows - t0 + MMA_K - 1) / MMA_K);
+            wgmma_fence();
+            for (int k = 0; k < ksteps; ++k) {
+                const uint64_t da = make_smem_desc_sw128(sa + k * (MMA_K * 128), WBK * 128, 1024);
+                const uint64_t db = make_smem_desc_sw128(sb + k * (MMA_K * 128), WBK * 128, 1024);
+                wgmma_bf16_n128<1, 1>(acc, da, db, (t0 > 0 || k > 0) ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev_stage >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&op_empty[prev_stage]);
+            }
+            prev_stage = stage;
+            if (++stage == OP_STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs(acc);
+        __syncwarp();
+        if (lane == 0 && prev_stage >= 0) mbar_arrive(&op_empty[prev_stage]);
+
+        // ---- AMSGrad on the accumulator positions: rows r (+8), columns 8j + 2(lane%4) (+1)
+        const float st = static_cast<float>(__ldg(p.step + t.g));
+        const float step_size = p.lr / (1.f - powf(p.beta1, st));
+        const float inv_sqrt_bc2 = rsqrtf(1.f - powf(p.beta2, st));
+        const long long row_base = static_cast<long long>(t.g) * p.N + t.mt * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int col_base = t.nt * BN_MAX + 2 * (lane & 3);
+#pragma unroll
+        for (int j0 = 0; j0 < BN_MAX / 8; j0 += JB) {
+            float2 pw[JB][2], m[JB][2], v[JB][2], vm[JB][2];
+#pragma unroll
+            for (int jj = 0; jj < JB; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const long long o = (row_base + 8 * h) * p.K + col_base + 8 * (j0 + jj);
+                    pw[jj][h] = *reinterpret_cast<const float2*>(p.p + o);
+                    m[jj][h] = *reinterpret_cast<const float2*>(p.m + o);
+                    v[jj][h] = *reinterpret_cast<const float2*>(p.v + o);
+                    vm[jj][h] = p.amsgrad ? *reinterpret_cast<const float2*>(p.vmax + o) : make_float2(0.f, 0.f);
+                }
+#pragma unroll
+            for (int jj = 0; jj < JB; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float* pp = &pw[jj][h].x; float* mp = &m[jj][h].x; float* vp = &v[jj][h].x; float* vmp = &vm[jj][h].x;
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float grad = acc[4 * (j0 + jj) + 2 * h + e];
+                        mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
+                        vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
+                        float denom;
+                        if (p.amsgrad) {
+                            vmp[e] = fmaxf(vmp[e], vp[e]);
+                            denom = sqrtf(vmp[e]) * inv_sqrt_bc2 + p.eps;
+                        } else {
+                            denom = sqrtf(vp[e]) * inv_sqrt_bc2 + p.eps;
+                        }
+                        pp[e] -= step_size * (mp[e] / denom);
+                    }
+                    const long long o = (row_base + 8 * h) * p.K + col_base + 8 * (j0 + jj);
+                    *reinterpret_cast<float2*>(p.p + o) = pw[jj][h];
+                    *reinterpret_cast<float2*>(p.m + o) = m[jj][h];
+                    *reinterpret_cast<float2*>(p.v + o) = v[jj][h];
+                    if (p.amsgrad) *reinterpret_cast<float2*>(p.vmax + o) = vm[jj][h];
+                    *reinterpret_cast<uint32_t*>(p.p_bf16 + o) = pack_bf16x2(pw[jj][h].x, pw[jj][h].y);
+                }
+        }
     }
 }
 
@@ -760,7 +643,7 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
                    float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
                    int max_ctas, cudaStream_t st) {
     if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8)) return -2;
-    CUtensorMap tmDY, tmX, tmS[4];
+    CUtensorMap tmDY, tmX;
     {
         uint64_t dims[2] = {(uint64_t)N, (uint64_t)total_rows};
         uint64_t str[1] = {(uint64_t)lddy * 2};
@@ -775,17 +658,9 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
         int r = make_tmap(&tmX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, 2, dims, str, box);
         if (r) return r;
     }
-    float* states[4] = {p, m, v, amsgrad ? vmax : p};
-    for (int i = 0; i < 4; ++i) {
-        uint64_t dims[2] = {(uint64_t)K, (uint64_t)G * N};
-        uint64_t str[1] = {(uint64_t)K * 4};
-        uint32_t box[2] = {32, 32};
-        int r = make_tmap(&tmS[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, states[i], 2, dims, str, box);
-        if (r) return r;
-    }
     wa::Params a;
     a.G = G; a.N = N; a.K = K; a.group_off = group_off; a.group_rows = group_rows; a.skip = skip; a.step = step;
-    a.p_bf16 = (bf16*)p_bf16; a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.amsgrad = amsgrad;
+    a.p = p; a.m = m; a.v = v; a.vmax = vmax; a.p_bf16 = (bf16*)p_bf16; a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.amsgrad = amsgrad;
     a.tile_counter = tile_counter() ? tile_counter() + 16 : nullptr;   // own word (64 B apart from the GEMM's)
     a.poison = g_poison;
     if (!a.tile_counter) return -3;
@@ -801,7 +676,7 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
         if (e != cudaSuccess) return -(int)e;
         configured = true;
     }
-    wa::wgrad_adam_kernel<<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS[0], tmS[1], tmS[2], tmS[3]);
+    wa::wgrad_adam_kernel<<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX);
     return -(int)cudaGetLastError();
 }
 

@@ -10,7 +10,7 @@ Setups (README.md:51-65 grid):  --setup dmoe | faulty | largeffn
 
 Data: MNIST is not available offline, so a synthetic MNIST-shaped task is used (784-d inputs, 10 classes, class
 prototypes + noise; deterministic per seed).  Works on CPU (BASELINE config #1: 16 experts x 4 layers, 2 trainers) and
-on a GPU (`--device cuda`).  `--backend engine` trains the same model on the sm_100a engine (synchronous trainers).
+on a GPU (`--device cuda`).  `--backend engine` trains the same model on the sm_90a engine (synchronous trainers).
 """
 import os
 import pickle

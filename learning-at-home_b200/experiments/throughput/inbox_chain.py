@@ -1,11 +1,11 @@
 """
 In-box version of the throughput experiment (BASELINE.json config "throughput_client transformer-block 56 layers/GPU,
-64 trainers, experts sharded over 8xB200"; reference: /root/reference/experiments/throughput/throughput_client.py:40-68
+64 trainers, experts sharded over 8xH100"; reference: experiments/throughput/throughput_client.py:40-68
 + throughput_server.py:13-33).
 
 The reference chains 56 x H remote layers, interleaved across the H servers, and keeps them busy with 64 concurrent
-trainer processes, each forward pass being one 8 MiB TCP RPC per layer.  Here every rank (one process per B200) hosts
-``layers_per_gpu`` experts executed by the sm_100a kernels (NativeTransformerLayer / NativeFFNLayer); layer i of the
+trainer processes, each forward pass being one 8 MiB TCP RPC per layer.  Here every rank (one process per H100) hosts
+``layers_per_gpu`` experts executed by the sm_90a kernels (NativeTransformerLayer / NativeFFNLayer); layer i of the
 chain lives on rank i % W exactly like the reference's interleaving; the 64 trainers' batches travel in W waves, one per
 rank per pipeline tick, and the LAST kernel of every layer writes its output straight into the NEXT rank's input buffer
 over NVLink (plain stores to peer memory from the LayerNorm / GEMM epilogue — no copy kernel, no NCCL), followed by a

@@ -1,6 +1,6 @@
 """
-sm_100a forward of the FFN expert (``FeedforwardBlock``, /root/reference/experiments/throughput/layers.py:5-19) for the
-forward-only throughput experiment: three tcgen05 GEMMs with fused bias (+ residual) epilogues and the fused
+sm_90a forward of the FFN expert (``FeedforwardBlock``, the reference's experiments/throughput/layers.py:5-19) for the
+forward-only throughput experiment: three wgmma GEMMs with fused bias (+ residual) epilogues and the fused
 LayerNorm+ReLU kernel in between.  ``dtype="fp8"`` runs the GEMMs on block-scaled FP8 tensor cores (MXFP8); LayerNorm
 then emits the next GEMM's FP8 operand directly and no bf16 activation is written at all.
 """

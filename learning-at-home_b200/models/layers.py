@@ -10,8 +10,8 @@ Expert architectures (the L1 "ops/models" layer of SURVEY.md).
   ``ExpertBackend.backward`` (the reference's block raises there; SURVEY.md §0.3).  Parameter names are identical
   (``self_attn.in_proj_weight`` ..., ``linear1``, ``linear2``, ``norm1``, ``norm2``).
 
-These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_100a execution of the same
-maths lives in ``lah_b200.parallel.engine`` (grouped tcgen05 GEMMs + fused LN/ReLU/Adam kernels).
+These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_90a execution of the same
+maths lives in ``lah_b200.parallel.engine`` (grouped wgmma GEMMs + fused LN/ReLU/Adam kernels).
 """
 import torch
 from torch import nn

@@ -1,6 +1,6 @@
 """
-sm_100a execution of the transformer expert (post-LN encoder layer, GELU; architecture of
-/root/reference/experiments/throughput/layers.py:22-51): QKV / out / MLP projections on the CTA-pair tcgen05 GEMM with
+sm_90a execution of the transformer expert (post-LN encoder layer, GELU; architecture of
+the reference's experiments/throughput/layers.py:22-51): QKV / out / MLP projections on the wide-tile wgmma GEMM with
 fused bias / GELU / residual epilogues, attention on csrc/attention.cu (S and P never leave the SM), LayerNorm on
 csrc/layernorm.cu.  Forward (inference / throughput experiment) only; training of transformer experts goes through the
 PyTorch module (``TransformerEncoderLayer`` + ``ExpertBackend``), which — unlike the reference's — is trainable.

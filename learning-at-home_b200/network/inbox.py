@@ -30,7 +30,7 @@ class InBoxNetwork:
         self._endpoints: Dict[str, Tuple[str, int]] = {}
         self._lock = threading.Lock()
         self._alive = bool(start)
-        self.fused_layer = None      # set by bind_engine(): GatingFunction then runs the sm_100a layer for CUDA inputs
+        self.fused_layer = None      # set by bind_engine(): GatingFunction then runs the sm_90a layer for CUDA inputs
         self._engine = None          # (ctx, cfg) of the bound in-box engine
         self._last_sync = 0.0
         self._ages_cache = (0.0, None)
@@ -40,7 +40,7 @@ class InBoxNetwork:
         """Attach a ``lah_b200.parallel.engine.FusedDMoE`` layer (or a ``DMoETrainer`` -> its first DMoE layer).
 
         * ``lib.GatingFunction(network=this, ...)`` called on a CUDA tensor then runs the fused layer (product-key gate with
-          the GatingFunction's own ``proj``, P2P dispatch, tcgen05 expert FFN, combine; backward + expert AMSGrad);
+          the GatingFunction's own ``proj``, P2P dispatch, wgmma expert FFN, combine; backward + expert AMSGrad);
         * ``declare_experts`` of uids that belong to the engine's grid and live on THIS rank stamps their heartbeat into the
           device-resident table of EVERY rank (multimem.st over NVSwitch), and the gate kernel's liveness mask is refreshed
           from that table at most every ``sync_period`` seconds — heartbeats reach the kernel without a host-side table;

@@ -1,14 +1,14 @@
 """
 Block-scaled FP8 (MXFP8) operands and the grouped GEMM that consumes them (csrc/grouped_gemm_fp8.cu):
-E4M3 data + one UE8M0 (power-of-two) scale per 1x32 block along K, tcgen05.mma.kind::mxf8f6f4.block_scale.
+E4M3 data + one UE8M0 (power-of-two) scale per 1x32 block along K, applied per 32-element K block to FP8 wgmma partials.
 
 BASELINE.json config "DMoE 4096 experts ... fp8 expert GEMM": the expert FFN forward GEMMs
 (/root/reference/experiments/throughput/layers.py:8-19 — nn.Linear in the reference, fp32 cuBLAS) run on FP8 tensor
 cores; dgrad / wgrad stay bf16 (see DESIGN.md §5).
 
 Scale-factor storage (shared with the kernel): rows are split into tiles of ``tile_rows`` rows (128 for activations,
-192 = the GEMM's N tile for weights), tiles into atoms of 128 rows, K into blocks of 128; one (atom, K-block) chunk is
-512 bytes in the order tcgen05.cp.32x128b.warpx4 expects (byte ``((r % 32) * 4 + r // 32) * 4 + kstep``).
+192 for weights), tiles into atoms of 128 rows, K into blocks of 128; one (atom, K-block) chunk is
+512 bytes (byte ``((r % 32) * 4 + r // 32) * 4 + kstep``).
 """
 import ctypes
 

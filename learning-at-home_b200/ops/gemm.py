@@ -1,5 +1,5 @@
 """
-Grouped GEMMs of the expert path (tcgen05/TMEM/TMA kernel in csrc/grouped_gemm.cu) + plain PyTorch oracles.
+Grouped GEMMs of the expert path (wgmma/TMA kernel in csrc/grouped_gemm.cu) + plain PyTorch oracles.
 
 Layout contract shared with the dispatch kernel (ops/dispatch.py):
   * token rows are grouped by expert, every group is padded with ZERO rows to a multiple of 128,
@@ -60,7 +60,7 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
     :param w: [G, N, K] bf16 (w_is_kn=False, y = x W^T)   or   [G, K, N] bf16 (w_is_kn=True, y = x W: dgrad)
     :param tile_group: int32 [ceil(rows/128)] expert of every 128-row tile (-1 skips the tile); None => expert 0
     :param bias: fp32 [G, N] or None;  residual: bf16 [rows, N] or None
-    :param act: activation fused after the bias (CTA-pair kernel only): 0 none, 1 ReLU, 2 GELU(erf)
+    :param act: activation fused after the bias (wide-tile kernel only): 0 none, 1 ReLU, 2 GELU(erf)
     :param wait: (flags int32 tensor [count], epoch, status tensor) — receive-side fusion: the kernel's TMA producer
         polls the peers' dispatch flags (ld.acquire.sys) before its first load instead of a separate wait kernel
     """
@@ -86,7 +86,7 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
     if residual is not None:
         assert residual.dtype == torch.bfloat16 and residual.stride(1) == 1
     if two_cta and N % 256 == 0:
-        # CTA-pair kernel (cta_group::2, 256x256 tiles): expert groups must be padded to 256 rows
+        # wide-tile kernel (128x256 tiles): expert groups must be padded to 256 rows
         code = _lib().lah_gemm_mgroup2(
             ptr(a), a.stride(0), rows, ptr(w), G, N, K, int(w_is_kn), ptr(out), out.stride(0),
             int(out.dtype == torch.float32), rows if m_valid is None else m_valid, num_m_tiles, ptr(tile_group),
@@ -95,7 +95,7 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
         native.check(code, "lah_gemm_mgroup2")
         native.count_launch()
         return out
-    assert act == 0, "epilogue activations are implemented in the CTA-pair kernel (two_cta=True, N % 256 == 0)"
+    assert act == 0, "epilogue activations are implemented in the wide-tile kernel (two_cta=True, N % 256 == 0)"
     bn = block_n or _pick_block_n(N)
     code = _lib().lah_gemm_mgroup(
         ptr(a), a.stride(0), rows, ptr(w), G, N, K, int(w_is_kn), ptr(out), out.stride(0),
@@ -126,7 +126,7 @@ def grouped_wgrad(dy, x, group_off, num_groups, *, out=None, block_n=None, max_c
         native.check(code, "lah_gemm_kgroup2")
         native.count_launch()
         return out
-    assert not accumulate, "gradient accumulation is implemented in the CTA-pair kernel (two_cta=True)"
+    assert not accumulate, "gradient accumulation is implemented in the wide-tile kernel (two_cta=True)"
     bn = block_n or _pick_block_n(N)
     code = _lib().lah_gemm_kgroup(ptr(dy), dy.stride(0), ptr(x), x.stride(0), rows, num_groups, M, N, ptr(group_off),
                                   ptr(out), N, M * N, bn, max_ctas, stream_ptr())

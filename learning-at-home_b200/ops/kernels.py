@@ -1,5 +1,5 @@
 """
-Python entry points for the non-GEMM sm_100a kernels (csrc/layernorm.cu, csrc/moe.cu, csrc/adam.cu) and their PyTorch
+Python entry points for the non-GEMM sm_90a kernels (csrc/layernorm.cu, csrc/moe.cu, csrc/adam.cu) and their PyTorch
 oracles.  All wrappers launch on the current CUDA stream, never synchronise, and are CUDA-graph capturable.
 """
 import ctypes
@@ -28,8 +28,8 @@ def _lib():
     sigs = {
         "lah_ln_relu_fwd": [P, P, P, P, P, P, P, I, I, I, P],
         "lah_ln_relu_fwd_t": [P, P, P, P, P, P, P, I, I, I, I, P],
-        "lah_ln_relu_bwd_t": [P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
-        "lah_grouped_colsum_t": [P, L, P, I, P, I, I, P],
+        "lah_ln_relu_bwd_t": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
+        "lah_grouped_colsum_t": [P, L, P, P, I, P, I, I, P],
         "lah_set_step_counters": [P],
         "lah_set_multicast": [c_ull],
         "lah_set_poison_word": [P],
@@ -41,8 +41,8 @@ def _lib():
         "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, P, I, P],
         "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, I, P],
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
-        "lah_ln_relu_bwd": [P, P, P, P, P, P, P, P, P, P, P, I, I, I, P],
-        "lah_grouped_colsum": [P, L, P, I, P, I, P],
+        "lah_ln_relu_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, P],
+        "lah_grouped_colsum": [P, L, P, P, I, P, I, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
         "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P],
@@ -99,20 +99,24 @@ def ln_relu_fwd(h, gamma, beta, tile_group, *, out, mean, rstd, relu=True, quant
 
 
 def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta, dbias, relu=True, tile_rows=128):
+    """dgamma / dbeta / dbias (+)= the column sums of every group's rows, summed in a fixed order (run-to-run identical)"""
     rows, C = h.shape
     assert da.is_contiguous() and h.is_contiguous() and dh.is_contiguous()
+    part = torch.empty((rows + tile_rows - 1) // tile_rows, 3, C, device=h.device, dtype=torch.float32)
     native.check(_lib().lah_ln_relu_bwd_t(ptr(da), ptr(h), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(dh),
-                                          ptr(dgamma), ptr(dbeta), ptr(dbias), ptr(tile_group), rows, C, int(relu),
-                                          int(tile_rows), stream_ptr()), "lah_ln_relu_bwd")
-    native.count_launch()
+                                          ptr(dgamma), ptr(dbeta), ptr(dbias), ptr(part), ptr(tile_group), rows, C,
+                                          int(relu), int(tile_rows), stream_ptr()), "lah_ln_relu_bwd")
+    native.count_launch(2)
     return dh
 
 
 def grouped_colsum(x, tile_group, *, out, tile_rows=128):
+    """out[g] += the column sums of group g's rows, summed in a fixed order (run-to-run identical)"""
     rows, C = x.shape
-    native.check(_lib().lah_grouped_colsum_t(ptr(x), x.stride(0), ptr(out), C, ptr(tile_group), rows, int(tile_rows),
-                                             stream_ptr()), "lah_grouped_colsum")
-    native.count_launch()
+    part = torch.empty((rows + tile_rows - 1) // tile_rows, C, device=x.device, dtype=torch.float32)
+    native.check(_lib().lah_grouped_colsum_t(ptr(x), x.stride(0), ptr(out), ptr(part), C, ptr(tile_group), rows,
+                                             int(tile_rows), stream_ptr()), "lah_grouped_colsum")
+    native.count_launch(2)
     return out
 
 
@@ -181,7 +185,7 @@ def gate_topk(logits, grid_size, k, *, alive=None, failure_rate=0.0, seed=0, tok
     native.check(_lib().lah_gate_topk(ptr(logits), B, ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), k,
                                       ptr(alive), float(failure_rate), int(seed) & (2 ** 64 - 1), int(token_offset),
                                       ptr(idx), ptr(w), ptr(pos), ptr(counts), stream_ptr()), "lah_gate_topk")
-    native.count_launch()
+    native.count_launch(2)
 
 
 def layout_exchange(cnt_all_off, flags_off, slot, epoch, E, E_loc, max_rows, *, align=128, tile_rows=None, counts, dst_row, group_off, group_rows,
@@ -260,7 +264,7 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
 # ---------------------------------------------------------------------------------------------------------
 def attention_fwd(qkv, num_heads, *, out=None, lse=None):
     """
-    Self-attention over 512-token sequences on tcgen05 (csrc/attention.cu).
+    Self-attention over 512-token sequences on wgmma (csrc/attention.cu).
     :param qkv: [batch*512, 3*d_model] bf16 = in_proj output, [q | k | v] per token; head_dim must be 64
     :param lse: optional fp32 [batch*512, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd)
     :returns: [batch*512, d_model] bf16, heads concatenated (input of out_proj)
@@ -280,7 +284,7 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None):
 
 def attention_bwd(qkv, out, dout, lse, num_heads):
     """
-    Backward of ``attention_fwd`` on tcgen05 (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
+    Backward of ``attention_fwd`` on wgmma (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
     dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.
     """
     tokens, three_d = qkv.shape
@@ -292,7 +296,7 @@ def attention_bwd(qkv, out, dout, lse, num_heads):
     dq_part = torch.empty(4, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
     native.check(_lib().lah_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
                                           tokens // 512, num_heads, d_model, stream_ptr()), "lah_attention_bwd")
-    native.count_launch(3)   # delta prologue, tcgen05 backward, dQ partial reduction
+    native.count_launch(3)   # delta prologue, wgmma backward, dQ partial reduction
     return dqkv
 
 
@@ -339,7 +343,7 @@ def adam_step(p, g, m, v, vmax, p_bf16, seg_sizes, G, *, step=None, group_rows=N
 
 def swapab_linear(x, w, group_off, group_rows, *, out, bias=None, residual=None, w_is_kn=False, wait=None, max_ctas=0):
     """
-    Small-M grouped linear on swap-AB tcgen05 tiles (csrc/small_m.cu): for the rows [group_off[g], +group_rows[g]) of every
+    Small-M grouped linear on swap-AB wgmma tiles (csrc/small_m.cu): for the rows [group_off[g], +group_rows[g]) of every
     group, out = x @ W[g]^T (+bias[g]) (+residual)   (w_is_kn: out = x @ W[g], the dgrad of a Linear whose weight is W).
     Weights are streamed exactly once per 128 tokens; a group of r rows costs MMAs of N = ceil16(r).
     :param x: [rows, K] bf16;  w: [G, M_out, K] (or [G, K, M_out] with w_is_kn) bf16;  out: [rows, M_out] bf16
@@ -380,7 +384,7 @@ def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, ski
                eps=1e-8, amsgrad=True, max_ctas=0):
     """
     Fused weight gradient + per-expert AMSGrad (csrc/small_m.cu): for every group g with rows > 0,
-    dW[g] = dy_g^T x_g is formed in TMEM and applied to p / m / v / vmax ([G, N, K] fp32) and the bf16 mirror in the same
+    dW[g] = dy_g^T x_g is formed in registers and applied to p / m / v / vmax ([G, N, K] fp32) and the bf16 mirror in the same
     kernel; the gradient never reaches HBM.  ``step`` holds the per-expert step counts AFTER this update.
     """
     G, N, Kd = p.shape

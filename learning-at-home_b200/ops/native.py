@@ -1,7 +1,7 @@
 """
 ctypes bindings for the in-tree native libraries (built by ``build_native.py``):
 
-* ``liblah_cuda.so`` — hand-written sm_100a kernels (tcgen05 grouped GEMM, LayerNorm/ReLU, gate/top-k, P2P dispatch /
+* ``liblah_cuda.so`` — hand-written sm_90a kernels (wgmma grouped GEMM, LayerNorm/ReLU, gate/top-k, P2P dispatch /
   combine, fused Adam, symmetric-heap helpers).  Loading it REQUIRES a CUDA device at call time; on a GPU box a missing
   library is a hard error (``cuda_lib()`` raises) — there is no silent PyTorch fallback on the GPU hot path.
 * ``liblah_host.so`` — C++ host runtime (batch former, wire framing, DHT routing table); usable on CPU-only machines.
@@ -54,7 +54,7 @@ def host_lib():
 
 
 def have_cuda_kernels() -> bool:
-    """True when the sm_100a kernels can actually run here (GPU present).  On a GPU box this also loads the library,
+    """True when the sm_90a kernels can actually run here (GPU present).  On a GPU box this also loads the library,
     so a broken build fails loudly instead of silently taking a PyTorch path."""
     if not torch.cuda.is_available():
         return False

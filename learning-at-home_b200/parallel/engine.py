@@ -1,12 +1,12 @@
 """
-The in-box DMoE engine: every rank (one process per B200) is BOTH a trainer and the host of a shard of experts.
+The in-box DMoE engine: every rank (one process per H100) is BOTH a trainer and the host of a shard of experts.
 
 Mapping to the reference (SURVEY.md §7.0):
   * ``GatingFunction.forward``  (/root/reference/lib/client/gating_function.py:25-66)   -> ``FusedDMoE.forward``
   * ``RemoteExpert`` fwd/bwd RPCs (/root/reference/lib/client/remote_expert.py:53-76)   -> P2P scatter / combine kernels
   * ``TaskPool`` batching (/root/reference/lib/runtime/task_pool.py:105-172)            -> expert-grouped row layout
   * ``ExpertBackend.forward/backward/apply_gradients`` (lib/runtime/expert_backend.py:64-97)
-                                                            -> grouped tcgen05 GEMMs, fused LN/ReLU, fused Adam(AMSGrad)
+                                                            -> grouped wgmma GEMMs, fused LN/ReLU, fused Adam(AMSGrad)
   * DHT liveness (/root/reference/lib/network/__init__.py:88-129)                       -> ``alive`` table read by the gate
 
 Activations of the experts stay resident on the expert's GPU between forward and backward (the reference recomputes
@@ -52,7 +52,7 @@ class DMoEConfig:
     amsgrad: bool = True
     seed: int = 1337
     uid_prefix: str = "expert"
-    two_cta: bool = True                 # CTA-pair (cta_group::2, 256x256 tiles) GEMMs; expert groups padded to 256 rows
+    two_cta: bool = True                 # wide 128x256 GEMM tiles with fused activation; expert groups padded to 256 rows
     # gate of the fused layer:
     #   "product_key": lib.GatingFunction semantics — trainable proj = Linear(hidden, sum(grid)), score = sum of per-dim logits
     #   "emulator":    EmulatedDMoE semantics (dmoe_emulator.py:47) — logits = LayerNorm(x) @ F.normalize(expert_keys, -1);
@@ -69,20 +69,19 @@ class DMoEConfig:
     # E4M3 + UE8M0 scale per 1x32 block, csrc/grouped_gemm_fp8.cu); dgrad / wgrad / optimizer are unchanged (bf16 / fp32)
     expert_dtype: str = "bf16"
     # which expert kernels run (csrc/):
-    #   "big":   rows grouped per expert and padded to 256-row CTA-pair tiles (grouped_gemm_2cta.cu) — compute-bound regime
-    #   "small": the reference's operating point (64 trainers x batch 4 => O(16) rows per expert): swap-AB tcgen05 tiles
+    #   "big":   rows grouped per expert and padded to 256 rows, 128x256 wgmma tiles (grouped_gemm.cu) — compute-bound regime
+    #   "small": the reference's operating point (64 trainers x batch 4 => O(16) rows per expert): swap-AB wgmma tiles
     #            that stream every weight once (small_m.cu), groups padded to 16 rows, weight gradient + AMSGrad fused in
     #            one kernel (the gradient never reaches HBM)
     #   "auto":  "small" when a step brings fewer than 512 rows per expert on average (up to there streaming the weights
     #            through 128-token swap-AB tiles, with the fused optimizer and the step in one CUDA graph, beats padding every
-    #            expert to 256-row CTA-pair tiles; beyond, the 2x more efficient pair tiles win)
+    #            expert to 256 rows; beyond, the wide tiles of the big path win)
     expert_path: str = "auto"
     # small path: run the fused weight-gradient + AMSGrad kernels (bandwidth-bound, ~75 % of the step) on a SECOND stream,
     # concurrently with the latency-bound chain of the backward pass (dgrads, LayerNorm backward, combine, the next layer's
     # dispatch).  `optimizer_ctas` SMs stream optimizer state, the chain keeps the remaining ones (persistent kernels of both
     # sides are launched with matching CTA limits so that neither starves the other).  0 disables the overlap, -1 = automatic:
-    # 116 of 148 on one GPU, 96 when the experts are sharded (measured: 1 GPU 10.96 -> 10.06 ms, 2 GPUs 7.08 -> 6.54 ms,
-    # 4 GPUs 5.16 -> 4.32 ms per step; 64 and >= 132 are slower than no overlap — profiles/overlap_sweep_r2.md)
+    # 11/14 of the SMs on one GPU, 9/14 when the experts are sharded (the sharded chain waits on peers and needs more SMs)
     optimizer_ctas: int = -1
     # asynchronous expert updates (reference: EmulatedDMoE.update_every_inputs / update_every_steps,
     # experiments/convergence/dmoe_emulator.py:70-77): an expert accumulates weight gradients and steps once it has seen
@@ -210,9 +209,9 @@ class EngineContext:
         self.dead_mask = 0                            # ranks excluded from every flag wait / reduce (host-decided)
         import os as _os
         octas = int(_os.environ.get("LAH_OPTIMIZER_CTAS", cfg.optimizer_ctas))
-        if octas < 0:
-            octas = 116 if self.world == 1 else 96
         sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        if octas < 0:
+            octas = sms * (11 if self.world == 1 else 9) // 14
         self.opt_ctas = octas if (self.small and 0 < octas < sms - 8) else 0     # CTAs of the optimizer stream (0: no overlap)
         self.chain_ctas = sms - self.opt_ctas if self.opt_ctas else 0            # CTA limit of the persistent chain kernels
         self.opt_stream = torch.cuda.Stream(self.device) if self.opt_ctas else None
@@ -641,7 +640,7 @@ class FusedDMoE(nn.Module):
         if self.ws is not None:
             self.ws.outstanding = False
 
-    # ------------------------------------------------------------------ sm_100a path
+    # ------------------------------------------------------------------ sm_90a path
     def _forward_cuda(self, x, logits):
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         B, k = x.shape[0], cfg.k
@@ -700,7 +699,7 @@ class FusedDMoE(nn.Module):
         """forward GEMMs on block-scaled FP8 tensor cores; LayerNorm emits the next GEMM's MXFP8 operand directly (and the
         bf16 copy the bf16 wgrad needs)"""
         c, ws, sh = self.ctx, self.ws, self.shard
-        assert c.two_cta, "the FP8 GEMM is a CTA-pair kernel (hidden and 4*hidden must be multiples of 256)"
+        assert c.two_cta, "the FP8 path needs the 256-row expert groups of the wide-tile layout (hidden and 4*hidden multiples of 256)"
         tg = ws.tile_group
         if wait is not None:  # the quantiser is the first consumer of the rows pushed by the peers
             K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
@@ -753,9 +752,6 @@ class FusedDMoE(nn.Module):
                             two_cta=c.two_cta)
         c.timer.mark("expert_ffn_bwd(wgrad+dgrad+ln)")
         # ---- expert-side optimizer step (reference: ExpertBackend.apply_gradients right after backward)
-        # (measured: moving this AMSGrad to a second stream with a bounded grid buys nothing in the saturated regime — the GPU
-        # sits at its power cap there, 705 W / 1665 MHz, and the next layer's bandwidth-bound stages slow down by what the
-        # optimizer gains: 62.1 vs 62.2 ms on 1 GPU, 61.3 vs 62.3 ms on 2; gpurun calls 19 / 20)
         if c.S:  # the owners read every rank's partial gradients of the shadowed experts: all ranks must be done
             K.signal_wait(c.flags_off, K.SLOT_SHADOW, epoch, c.status, signal=True, wait=True)
         self.apply_expert_gradients()
@@ -778,7 +774,7 @@ class FusedDMoE(nn.Module):
         side, chain_ctas = c.opt_stream, c.chain_ctas
 
         def wgrad(name, dy, x):
-            """dW never reaches HBM: TMEM accumulator -> AMSGrad epilogue -> TMA stores of p / m / v / vmax.  With the overlap
+            """dW never reaches HBM: register accumulator -> AMSGrad epilogue -> p / m / v / vmax updated in place.  With the overlap
             enabled the kernel goes to the optimizer stream, ordered after everything the main stream has launched so far (in
             particular the dgrad that still reads the OLD weights); its inputs live in per-layer buffers."""
             kw = dict(p=sh.views[name][:self.E_loc], m=sh.m_views[name][:self.E_loc], v=sh.v_views[name][:self.E_loc],

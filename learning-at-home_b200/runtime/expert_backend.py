@@ -28,8 +28,8 @@ class ExpertBackend(nn.Module):
                  args_schema: Tuple[BatchTensorProto, ...] = None, kwargs_schema: Dict[str, BatchTensorProto] = None,
                  outputs_schema: Union[BatchTensorProto, Tuple[BatchTensorProto, ...]] = None, native: bool = True,
                  **kwargs):
-        """:param native: run FeedforwardBlock experts that live on a CUDA device through the sm_100a kernels
-        (runtime/native_executor.py: swap-AB tcgen05 GEMMs, fused LayerNorm, fused weight-gradient + AMSGrad) instead of
+        """:param native: run FeedforwardBlock experts that live on a CUDA device through the sm_90a kernels
+        (runtime/native_executor.py: swap-AB wgmma GEMMs, fused LayerNorm, fused weight-gradient + AMSGrad) instead of
         eager PyTorch; anything the executor does not support falls back to the module itself"""
         super().__init__()
         self.expert, self.opt, self.name = expert, opt, name
@@ -58,7 +58,7 @@ class ExpertBackend(nn.Module):
 
     # ------------------------------------------------------------------ tasks
     def native_executor(self, inputs):
-        """the sm_100a executor of this expert, or None (CPU tensors, unsupported expert / optimizer, no GPU)"""
+        """the sm_90a executor of this expert, or None (CPU tensors, unsupported expert / optimizer, no GPU)"""
         if not self.native or len(inputs) < 1 or not inputs[0].is_cuda or self.kwargs_schema or len(self.args_schema) != 1:
             return None
         first = next(self.expert.parameters(), None)

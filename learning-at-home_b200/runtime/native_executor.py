@@ -1,7 +1,7 @@
 """
 NativeFFNExecutor — runs ``ExpertBackend.forward`` / ``ExpertBackend.backward`` of a ``FeedforwardBlock`` expert on the
-hand-written sm_100a kernels instead of eager PyTorch, so that a ``TesseractServer``'s runtime loop
-(/root/reference/lib/runtime/__init__.py:42-47 -> lib/runtime/expert_backend.py:64-97) executes tcgen05 code:
+hand-written sm_90a kernels instead of eager PyTorch, so that a ``TesseractServer``'s runtime loop
+(the reference's lib/runtime/__init__.py:42-47 -> lib/runtime/expert_backend.py:64-97) executes wgmma code:
 
   forward   swap-AB grouped linear (weights streamed once per 128 rows, csrc/small_m.cu) x 3 + fused LayerNorm+ReLU x 2
   backward  the reference semantics — recompute the forward from the inputs the client re-sent, back-propagate, step the
@@ -175,13 +175,13 @@ class NativeFFNExecutor:
 
 class NativeTransformerExecutor:
     """
-    Trainable sm_100a transformer expert (post-LN encoder layer of /root/reference/experiments/throughput/layers.py:22-51,
+    Trainable sm_90a transformer expert (post-LN encoder layer of the reference's experiments/throughput/layers.py:22-51,
     batch-first [B, 512, d], head_dim 64, dropout must be 0 for training — the reference's block cannot be trained at all).
 
-      forward   in_proj GEMM -> tcgen05 flash attention (emits the row log-sum-exp) -> out_proj GEMM (+bias +residual) ->
+      forward   in_proj GEMM -> wgmma flash attention (emits the row log-sum-exp) -> out_proj GEMM (+bias +residual) ->
                 LayerNorm -> linear1 GEMM -> GELU -> linear2 GEMM (+bias +residual) -> LayerNorm
-      backward  LayerNorm backward kernels (they also produce the bias gradients of the preceding Linear), CTA-pair tcgen05
-                dgrad / wgrad GEMMs for the four projections, the tcgen05 ATTENTION BACKWARD kernel (csrc/attention_bwd.cu),
+      backward  LayerNorm backward kernels (they also produce the bias gradients of the preceding Linear), wide-tile wgmma
+                dgrad / wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel (csrc/attention_bwd.cu),
                 GELU backward (aten elementwise), one fused AMSGrad/Adam step over the flat parameter buffer
 
     Like the FFN executor, module parameters and optimizer state are views of flat fp32 buffers (state_dict / checkpoints

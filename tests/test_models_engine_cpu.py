@@ -349,7 +349,7 @@ def test_update_every_on_cpu_matches_the_emulator_schedule_and_resumes():
 
 
 def test_expert_path_selection():
-    """"small" (swap-AB weight streaming, fused wgrad+AMSGrad) below 512 rows per expert and step, "big" (CTA-pair tiles) above;
+    """"small" (swap-AB weight streaming, fused wgrad+AMSGrad) below 512 rows per expert and step, "big" (wide-tile tiles) above;
     gradient accumulation and FP8 forward GEMMs live on the big path"""
     named = E.DMoEConfig(hidden=512, grid_size=(64,), k=4, tokens_per_rank=256)
     assert named.resolved_path(1) == "small" and named.resolved_path(8) == "small"      # 16 .. 128 rows per expert

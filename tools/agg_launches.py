@@ -4,7 +4,7 @@ import csv
 import re
 import sys
 
-path = sys.argv[1] if len(sys.argv) > 1 else "gpurun_out/launches.csv"
+path = sys.argv[1] if len(sys.argv) > 1 else "check_out/launches.csv"
 steps = float(sys.argv[2]) if len(sys.argv) > 2 else 1.0
 rows = list(csv.reader(open(path)))
 hi = [i for i, r in enumerate(rows) if r and r[0] == "ID"][0]

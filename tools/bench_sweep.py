@@ -1,7 +1,7 @@
 """
 Sweep of the named-config step over expert paths / optimizer-stream CTA partitions inside ONE torchrun job (one rendezvous,
 one import, a fresh engine per point): `torchrun --nproc-per-node N tools/bench_sweep.py --gpus N --points small:0 small:64 big`
-Prints one JSON line per point (rank 0) and writes gpurun_out/sweep_n{N}.jsonl.  Used for profiles/overlap_sweep_r2.md.
+Prints one JSON line per point (rank 0) and writes check_out/sweep_n{N}.jsonl.
 """
 import json
 import os
@@ -9,6 +9,7 @@ import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench  # noqa: E402
+from tools import output_path  # noqa: E402
 
 
 def main():
@@ -41,8 +42,7 @@ def main():
         if rank == 0:
             print(json.dumps(line), flush=True)
     if rank == 0:
-        os.makedirs("gpurun_out", exist_ok=True)
-        with open(f"gpurun_out/sweep_n{world}.jsonl", "w") as f:
+        with open(output_path(f"sweep_n{world}.jsonl"), "w") as f:
             for line in lines:
                 f.write(json.dumps(line) + "\n")
     if world > 1:

@@ -1,4 +1,4 @@
-"""GPU check: tcgen05 attention kernel and the native transformer layer vs PyTorch oracles (run via gpurun)."""
+"""GPU check: wgmma attention kernel and the native transformer layer vs PyTorch oracles (writes check_out/native_layers_check.json)."""
 import os
 import sys
 
@@ -6,6 +6,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 import lah_b200  # noqa
+from tools import output_path
 from lah_b200.models.layers import TransformerEncoderLayer
 from lah_b200.models.transformer_native import NativeTransformerLayer
 from lah_b200.ops import kernels as K
@@ -54,7 +55,7 @@ def check_attention():
 
 
 def check_attention_bwd():
-    """tcgen05 attention backward (csrc/attention_bwd.cu) vs autograd through the fp32 reference attention"""
+    """wgmma attention backward (csrc/attention_bwd.cu) vs autograd through the fp32 reference attention"""
     torch.manual_seed(3)
     for batch, heads in [(1, 2), (2, 16)]:
         d = heads * 64
@@ -92,7 +93,7 @@ def check_attention_bwd():
 
 
 def check_transformer_train():
-    """the TRAINABLE sm_100a transformer expert (ExpertBackend + NativeTransformerExecutor): forward, input gradients and three
+    """the TRAINABLE sm_90a transformer expert (ExpertBackend + NativeTransformerExecutor): forward, input gradients and three
     AMSGrad steps against the fp32 nn.Module + torch.optim.Adam"""
     import copy
     import lah_b200 as lib
@@ -171,7 +172,7 @@ def check_layer():
 
 
 def check_ffn_native():
-    """sm_100a forward of the FFN expert (bf16 and MXFP8) vs the fp32 nn.Module; throughput of the fwd-only chain layer"""
+    """sm_90a forward of the FFN expert (bf16 and MXFP8) vs the fp32 nn.Module; throughput of the fwd-only chain layer"""
     from lah_b200.models.layers import FeedforwardBlock
     from lah_b200.models.ffn_native import NativeFFNLayer
     torch.manual_seed(2)
@@ -219,6 +220,5 @@ if __name__ == "__main__":
             traceback.print_exc()
             results[fn.__name__] = dict(ok=False, error=repr(e))
     import json
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(results, open("gpurun_out/native_layers_check.json", "w"), indent=1)
+    json.dump(results, open(output_path("native_layers_check.json"), "w"), indent=1)
     print("ALL_OK" if all(v.get("ok") for v in results.values()) else "SOME_FAILED")

@@ -1,4 +1,4 @@
-"""GPU check: MXFP8 quantisation kernel + block-scaled tcgen05 grouped GEMM vs PyTorch oracles (run via gpurun)."""
+"""GPU check: MXFP8 quantisation kernel + block-scaled wgmma grouped GEMM vs PyTorch oracles (writes check_out/fp8_check.json)."""
 import json
 import os
 import sys
@@ -7,6 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 import lah_b200  # noqa
+from tools import output_path
 from lah_b200.ops import fp8, gemm
 
 results = {}
@@ -139,6 +140,5 @@ if __name__ == "__main__":
             import traceback
             traceback.print_exc()
             results[fn.__name__] = dict(ok=False, error=repr(e))
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(results, open("gpurun_out/fp8_check.json", "w"), indent=1)
+    json.dump(results, open(output_path("fp8_check.json"), "w"), indent=1)
     print("ALL_OK" if all(v.get("ok") for v in results.values()) else "SOME_FAILED")

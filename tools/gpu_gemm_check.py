@@ -1,4 +1,4 @@
-"""GPU sanity + perf check for the tcgen05 grouped GEMM (run via gpurun). Prints one line per case."""
+"""GPU sanity + perf check for the wgmma grouped GEMM (writes check_out/gemm_check.json). Prints one line per case."""
 import json
 import os
 import sys
@@ -8,6 +8,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 import lah_b200  # noqa
+from tools import output_path
 from lah_b200.ops import gemm
 
 
@@ -170,8 +171,7 @@ def main():
         results["perf_error"] = repr(e)
         print("perf_error", repr(e), flush=True)
 
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/gemm_check.json", "w") as f:
+    with open(output_path("gemm_check.json"), "w") as f:
         json.dump(results, f, indent=1)
     print("ALL_OK" if all(v.get("ok", True) for v in results.values() if isinstance(v, dict)) else "SOME_FAILED")
 

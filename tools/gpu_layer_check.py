@@ -1,4 +1,4 @@
-"""GPU check of the non-GEMM kernels and of one full FusedDMoE layer against PyTorch oracles (run via gpurun)."""
+"""GPU check of the non-GEMM kernels and of one full FusedDMoE layer against PyTorch oracles (writes check_out/layer_check.json)."""
 import json
 import os
 import sys
@@ -9,6 +9,7 @@ import torch
 import torch.nn.functional as F
 
 import lah_b200  # noqa
+from tools import output_path
 from lah_b200.ops import kernels as K
 from lah_b200.models.layers import FeedforwardBlock
 from lah_b200.parallel import engine as E
@@ -227,8 +228,7 @@ def main():
             import traceback
             traceback.print_exc()
             record(fn.__name__ + "_exception", ok=False, error=repr(e))
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/layer_check.json", "w") as f:
+    with open(output_path("layer_check.json"), "w") as f:
         json.dump(results, f, indent=1, default=str)
     print("ALL_OK" if all(v.get("ok") for v in results.values()) else "SOME_FAILED")
 

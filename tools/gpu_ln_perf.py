@@ -1,4 +1,4 @@
-"""GPU perf probe for the LayerNorm+ReLU kernels at the bench shapes (run via gpurun; LAH_LN_ROWS=1 = one row per warp)."""
+"""GPU perf probe for the LayerNorm+ReLU kernels at the bench shapes (run on the GPU; LAH_LN_ROWS=1 = one row per warp)."""
 import json
 import os
 import sys

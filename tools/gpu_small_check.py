@@ -3,7 +3,7 @@
   swapab_linear   forward (K-major weights) and dgrad (MN-major weights) over ragged groups of 0..300 rows
   wgrad_adam      fused weight gradient + AMSGrad vs (dy^T x in fp32) + torch.optim.Adam(amsgrad=True) semantics
 
-Run via gpurun: python tools/gpu_small_check.py [--perf]; writes gpurun_out/small_check.json"""
+Run on the GPU: python tools/gpu_small_check.py [--perf]; writes check_out/small_check.json"""
 import json
 import os
 import sys
@@ -12,6 +12,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
 import lah_b200  # noqa
+from tools import output_path
 from lah_b200.ops import kernels as K
 
 results = {}
@@ -217,8 +218,7 @@ def main():
             import traceback
             traceback.print_exc()
             record(fn.__name__ + "_exception", ok=False, error=repr(e))
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/small_check.json", "w") as f:
+    with open(output_path("small_check.json"), "w") as f:
         json.dump(results, f, indent=1, default=str)
     print("ALL_OK" if all(v.get("ok") for v in results.values()) else "SOME_FAILED")
 

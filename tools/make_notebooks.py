@@ -1,7 +1,7 @@
 """Generates the three convergence notebooks (experiments/convergence/*.ipynb) — same names, configurations and metric
 files as the reference notebooks (/root/reference/experiments/convergence/*.ipynb, cells 1-4), written against this package:
 config cell -> data / model -> asynchronous trainer threads with stale gradients -> evaluation curve + metrics pickle ->
-the same experiment on the sm_100a engine.  `LAH_NB_SMOKE=1` shrinks every size so that tests can execute the cells on CPU.
+the same experiment on the sm_90a engine.  `LAH_NB_SMOKE=1` shrinks every size so that tests can execute the cells on CPU.
 
     python tools/make_notebooks.py
 """
@@ -48,7 +48,7 @@ Counterpart of `/root/reference/experiments/convergence/{name}` ({s['ref_lines']
 lock, sleeps `delay_ms * Weibull(1)` (emulated network latency) and then applies its — by now stale — gradients; experts
 update themselves inside the emulated DMoE layer once they have seen `update_every_inputs` inputs or `update_every_steps`
 steps.  MNIST is not available offline: the data is a synthetic MNIST-shaped task (784-d inputs, 10 classes, class
-prototypes + noise).  The last section trains the same model on the sm_100a engine (`DMoETrainer`, stale trainer gradients
+prototypes + noise).  The last section trains the same model on the sm_90a engine (`DMoETrainer`, stale trainer gradients
 through `DMoEConfig.trainer_staleness`).  `LAH_NB_SMOKE=1` runs a tiny version of every cell.""")]
     cells.append(code(f"""
 import os, sys, time, pickle, random, threading
@@ -155,7 +155,7 @@ mean_delay = float(np.mean([h['delay_steps'] for h in train_history]))
 print('final val acc', val_history[-1]['acc'], '| mean staleness', round(mean_delay, 1), 'updates')
 """))
     if s["setup"] != "largeffn":
-        cells.append(md("""## The same experiment on the sm_100a engine
+        cells.append(md("""## The same experiment on the sm_90a engine
 
 One `DMoETrainer` per GPU: the 64 trainers x batch become ONE fused step of `num_trainers * batch_size` samples, experts step
 themselves after every backward (fused wgrad + AMSGrad kernel), the trainer-side optimizer applies gradients that are

@@ -1,5 +1,5 @@
-"""Summarise an .ncu-rep (read on the CPU box with `ncu -i`) into a small JSON for profiles/.
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/ncu_<name>.json"""
+"""Summarise an .ncu-rep (read on the CPU box with `ncu -i`) into a small JSON.
+    python tools/ncu_summary.py prof.ncu-rep ncu_<name>.json"""
 import csv
 import io
 import json

@@ -1,4 +1,4 @@
-"""GPU probe: how does expert routing evolve while the flagship model trains on synthetic data?  (run via gpurun)
+"""GPU probe: how does expert routing evolve while the flagship model trains on synthetic data?  (run on the GPU)
 
 Prints, per step and DMoE layer: active experts, share of the hottest expert, and the per-rank load imbalance
 (max / mean padded rows) that an 8-way expert-parallel placement would see.  `--labels teacher` draws labels from a fixed
