@@ -14,13 +14,15 @@
 //                      (W^T read straight from the same [out, in] tensor as an MN-major operand).
 //   wgrad_adam_kernel  dW tile = dY^T X with wgmma (both operands MN-major, two 32-token stages, reduction over the
 //                      expert's tokens = the gradient reduction over all trainers that routed to it) with the per-expert AMSGrad step FUSED
-//                      INTO THE EPILOGUE: every thread reads p / m / v / vmax at the positions of its accumulator
-//                      registers (four 8-column groups at a time, so 32 loads are in flight per thread), updates them
-//                      and writes them back together with the bf16 mirror.  The weight gradient never exists in HBM: 34 B / parameter
+//                      INTO THE EPILOGUE: p / m / v / vmax stream through a TMA ring of 32-column chunks of the tile
+//                      (loaded while the MMAs run), every thread updates them in shared memory at the positions of its
+//                      accumulator registers and writes the bf16 mirror, and the chunk goes back to HBM by TMA store.
+//                      The weight gradient never exists in HBM: 34 B / parameter
 //                      instead of 46 (wgrad write 4 + Adam 38 + re-read 4).
 //                      Reference semantics: one torch.optim.Adam(amsgrad=True) step per expert right after its backward
 //                      (/root/reference/lib/runtime/expert_backend.py:90-97).
 #include "sm90.cuh"
+#include <climits>
 
 namespace lah {
 namespace smallm {
@@ -333,13 +335,22 @@ swapab_kernel(const Params p, const __grid_constant__ CUtensorMap tmA, const __g
 namespace wa {
 
 constexpr int WBK = 32;                                  // tokens per operand stage
-constexpr int OP_STAGES = 4;                             // a hot expert has tens of k-blocks: loads run ahead of the MMAs
+constexpr int OP_STAGES = 2;                             // a hot expert has tens of k-blocks: loads run ahead of the MMAs
 constexpr int OP_STAGE_BYTES = 2 * (WBK * BM * 2);       // A [32 t][128 n] + B [32 t][128 k] (two 64-wide MN atoms each)
 constexpr int OP_BYTES = OP_STAGES * OP_STAGE_BYTES;
-constexpr int BAR_OFFSET = OP_BYTES;
+// optimizer state streams through its own ring: a chunk is one 32-column slice of the tile (= 4 accumulator column groups)
+// of p, m, v and vmax, each a [128 rows][32 fp32] TMA box with 128-B swizzle
+constexpr int CH_COLS = 32;
+constexpr int CHUNKS = BN_MAX / CH_COLS;                 // chunks per tile
+constexpr int ARR_BYTES = BM * CH_COLS * 4;              // 16 KB: one state array of a chunk
+constexpr int ST_STAGES = 3;
+constexpr int ST_STAGE_BYTES = 4 * ARR_BYTES;
+constexpr int ST_OFFSET = OP_BYTES;
+constexpr int BAR_OFFSET = ST_OFFSET + ST_STAGES * ST_STAGE_BYTES;
 constexpr int QD = 4;                                    // depth of the tile queue (dynamic scheduler)
-constexpr int SMEM_TOTAL = BAR_OFFSET + (2 * OP_STAGES + 2 * QD) * 8 + QD * 4 + 16 + 1024;
-constexpr int JB = 4;                                    // 8-column groups whose state is loaded together
+constexpr int SMEM_TOTAL = BAR_OFFSET + (2 * OP_STAGES + 2 * ST_STAGES + 2 * QD) * 8 + QD * 4 + 16 + 1024;
+static_assert(ST_STAGES <= CHUNKS, "the producer issues a tile's first ST_STAGES chunks before its remaining k-blocks");
+static_assert(OP_STAGE_BYTES % 1024 == 0 && ARR_BYTES % 1024 == 0, "128-B swizzle atoms need 1 KB alignment");
 static_assert(SMEM_TOTAL <= 232448, "shared memory budget");
 
 struct Params {
@@ -363,26 +374,41 @@ struct Tile {
     int g, mt, nt;
 };
 
+// state tensor maps: p, m, v, vmax viewed as [G * N, K] fp32 (vmax only read when amsgrad)
+struct StateMaps {
+    CUtensorMap a[4];
+};
+
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX) {
+wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX,
+                  const __grid_constant__ StateMaps tmS) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* st_smem = smem + ST_OFFSET;
     uint64_t* op_full = reinterpret_cast<uint64_t*>(smem + BAR_OFFSET);
     uint64_t* op_empty = op_full + OP_STAGES;
-    uint64_t* q_full = op_empty + OP_STAGES;
+    uint64_t* st_full = op_empty + OP_STAGES;
+    uint64_t* st_empty = st_full + ST_STAGES;
+    uint64_t* q_full = st_empty + ST_STAGES;
     uint64_t* q_empty = q_full + QD;
     volatile int* q_tile = reinterpret_cast<volatile int*>(q_empty + QD);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     if (p.poison && (*p.poison & 1)) return;   // degraded step (a peer timed out): no optimizer step from partial data
+    const int n_arr = p.amsgrad ? 4 : 3;
 
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmDY);
         tma_prefetch_desc(&tmX);
+        for (int a = 0; a < n_arr; ++a) tma_prefetch_desc(&tmS.a[a]);
         for (int i = 0; i < OP_STAGES; ++i) {
             mbar_init(&op_full[i], 1);
             mbar_init(&op_empty[i], 8);
+        }
+        for (int i = 0; i < ST_STAGES; ++i) {
+            mbar_init(&st_full[i], 1);
+            mbar_init(&st_empty[i], 1);   // released by the thread that stored the chunk back
         }
         for (int i = 0; i < QD; ++i) {
             mbar_init(&q_full[i], 1);
@@ -406,11 +432,14 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
 
     if (warp == 8) {
         if (lane != 0) return;
-        // =============================================================== scheduler + operand producer (dY^T / X^T k-blocks)
+        // =============================================================== scheduler + operand / state producer
         // tiles are drawn from a global counter (work stealing: SMs see different HBM bandwidth, a static split leaves the
-        // fast ones idle) and published to the consumer warps through a queue
-        uint32_t phase = 0, qphase = 0;
-        int qi = 0, stage = 0;
+        // fast ones idle) and published to the consumer warps through a queue.  Per tile: the dY^T / X^T k-blocks and the
+        // state chunks.  The state does not depend on the gradient, so the first ST_STAGES chunks go out right after the
+        // first k-block (their slots are freed by the previous tile's epilogue) and stream in during the MMA; the rest
+        // follow the last k-block.  The consumers take the same order, so no wait of the producer can deadlock.
+        uint32_t phase = 0, qphase = 0, sphase = 0;
+        int qi = 0, stage = 0, sstage = 0;
         while (true) {
             int tile;
             while (true) {
@@ -430,6 +459,18 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
             if (tile >= total) break;
             const Tile t = decode(tile);
             const int off = __ldg(p.group_off + t.g), rows = __ldg(p.group_rows + t.g);
+            const int srow = t.g * p.N + t.mt * BM;
+            auto load_chunk = [&](int c) {
+                mbar_wait(&st_empty[sstage], sphase ^ 1);
+                mbar_arrive_expect_tx(&st_full[sstage], n_arr * ARR_BYTES);
+                uint8_t* ss = st_smem + sstage * ST_STAGE_BYTES;
+                for (int a = 0; a < n_arr; ++a)
+                    tma_load_2d(ss + a * ARR_BYTES, &tmS.a[a], &st_full[sstage], t.nt * BN_MAX + c * CH_COLS, srow);
+                if (++sstage == ST_STAGES) {
+                    sstage = 0;
+                    sphase ^= 1;
+                }
+            };
             for (int t0 = 0; t0 < rows; t0 += WBK) {
                 mbar_wait(&op_empty[stage], phase ^ 1);
                 mbar_arrive_expect_tx(&op_full[stage], OP_STAGE_BYTES);
@@ -445,16 +486,22 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                     stage = 0;
                     phase ^= 1;
                 }
+                if (t0 == 0)
+                    for (int c = 0; c < ST_STAGES; ++c) load_chunk(c);
             }
+            for (int c = ST_STAGES; c < CHUNKS; ++c) load_chunk(c);
         }
         return;
     }
 
     // =================================================================== consumers: wgrad tile (MMA) + AMSGrad epilogue
     const int wg = warp >> 2;
-    int qi = 0, stage = 0;
-    uint32_t phase = 0, qphase = 0;
+    int qi = 0, stage = 0, sstage = 0;
+    uint32_t phase = 0, qphase = 0, sphase = 0;
     float acc[BN_MAX / 2];
+    // this thread's first accumulator row inside the chunk box, and the 128-B swizzle key of its rows (lrow and lrow + 8)
+    const int lrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int sw = lrow & 7;
     while (true) {
         mbar_wait(&q_full[qi], qphase);
         const int tile = q_tile[qi];
@@ -497,33 +544,33 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
         __syncwarp();
         if (lane == 0 && prev_stage >= 0) mbar_arrive(&op_empty[prev_stage]);
 
-        // ---- AMSGrad on the accumulator positions: rows r (+8), columns 8j + 2(lane%4) (+1)
+        // ---- AMSGrad on the accumulator positions: rows r (+8), columns 8j + 2(lane%4) (+1), state from the chunk ring
         const float st = static_cast<float>(__ldg(p.step + t.g));
         const float step_size = p.lr / (1.f - powf(p.beta1, st));
         const float inv_sqrt_bc2 = rsqrtf(1.f - powf(p.beta2, st));
-        const long long row_base = static_cast<long long>(t.g) * p.N + t.mt * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int srow = t.g * p.N + t.mt * BM;
+        const long long row_base = static_cast<long long>(srow) + lrow;
         const int col_base = t.nt * BN_MAX + 2 * (lane & 3);
 #pragma unroll
-        for (int j0 = 0; j0 < BN_MAX / 8; j0 += JB) {
-            float2 pw[JB][2], m[JB][2], v[JB][2], vm[JB][2];
+        for (int c = 0; c < CHUNKS; ++c) {
+            mbar_wait(&st_full[sstage], sphase);
+            uint8_t* ss = st_smem + sstage * ST_STAGE_BYTES;
 #pragma unroll
-            for (int jj = 0; jj < JB; ++jj)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const long long o = (row_base + 8 * h) * p.K + col_base + 8 * (j0 + jj);
-                    pw[jj][h] = *reinterpret_cast<const float2*>(p.p + o);
-                    m[jj][h] = *reinterpret_cast<const float2*>(p.m + o);
-                    v[jj][h] = *reinterpret_cast<const float2*>(p.v + o);
-                    vm[jj][h] = p.amsgrad ? *reinterpret_cast<const float2*>(p.vmax + o) : make_float2(0.f, 0.f);
-                }
-#pragma unroll
-            for (int jj = 0; jj < JB; ++jj)
+            for (int jj = 0; jj < CH_COLS / 8; ++jj)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                    float* pp = &pw[jj][h].x; float* mp = &m[jj][h].x; float* vp = &v[jj][h].x; float* vmp = &vm[jj][h].x;
+                    // 16-B unit (2 jj + lane%4 / 2) of row lrow + 8h, XOR-swizzled by the row (8h leaves the pattern alone)
+                    const int so = (lrow + 8 * h) * 128 + (((2 * jj + ((lane & 3) >> 1)) ^ sw) << 4) + 8 * (lane & 1);
+                    float2* sp = reinterpret_cast<float2*>(ss + so);
+                    float2* sm = reinterpret_cast<float2*>(ss + ARR_BYTES + so);
+                    float2* sv = reinterpret_cast<float2*>(ss + 2 * ARR_BYTES + so);
+                    float2* svm = reinterpret_cast<float2*>(ss + 3 * ARR_BYTES + so);
+                    float2 pw = *sp, m = *sm, v = *sv;
+                    float2 vm = p.amsgrad ? *svm : make_float2(0.f, 0.f);
+                    float* pp = &pw.x; float* mp = &m.x; float* vp = &v.x; float* vmp = &vm.x;
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        const float grad = acc[4 * (j0 + jj) + 2 * h + e];
+                        const float grad = acc[4 * jj + 2 * h + e];
                         mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
                         vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
                         float denom;
@@ -535,15 +582,34 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                         }
                         pp[e] -= step_size * (mp[e] / denom);
                     }
-                    const long long o = (row_base + 8 * h) * p.K + col_base + 8 * (j0 + jj);
-                    *reinterpret_cast<float2*>(p.p + o) = pw[jj][h];
-                    *reinterpret_cast<float2*>(p.m + o) = m[jj][h];
-                    *reinterpret_cast<float2*>(p.v + o) = v[jj][h];
-                    if (p.amsgrad) *reinterpret_cast<float2*>(p.vmax + o) = vm[jj][h];
-                    *reinterpret_cast<uint32_t*>(p.p_bf16 + o) = pack_bf16x2(pw[jj][h].x, pw[jj][h].y);
+                    *sp = pw;
+                    *sm = m;
+                    *sv = v;
+                    if (p.amsgrad) *svm = vm;
+                    const long long o = (row_base + 8 * h) * p.K + col_base + CH_COLS * c + 8 * jj;
+                    *reinterpret_cast<uint32_t*>(p.p_bf16 + o) = pack_bf16x2(pw.x, pw.y);
                 }
+            // the updated chunk goes back to HBM by TMA; its slot returns to the producer once the store has read it
+            fence_proxy_async_smem();
+            named_bar_sync(1, 256);
+            if (threadIdx.x == 0) {
+                for (int a = 0; a < n_arr; ++a)
+                    tma_store_2d(&tmS.a[a], ss + a * ARR_BYTES, t.nt * BN_MAX + c * CH_COLS, srow);
+                tma_store_commit();
+                tma_store_wait_read<0>();
+                mbar_arrive(&st_empty[sstage]);
+            }
+            if (++sstage == ST_STAGES) {
+                sstage = 0;
+                sphase ^= 1;
+            }
+            // the next chunk's gradient moves to acc[0, 16): the chunk loop is not unrolled, and a run-time index into
+            // the accumulator would put it in local memory
+#pragma unroll
+            for (int i = 0; i < BN_MAX / 2 - 16; ++i) acc[i] = acc[i + 16];
         }
     }
+    if (threadIdx.x == 0) tma_store_wait<0>();
 }
 
 }  // namespace wa
@@ -642,8 +708,19 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
                    const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
                    float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
                    int max_ctas, cudaStream_t st) {
-    if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8)) return -2;
+    if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8) || 1ll * G * N > INT_MAX) return -2;
     CUtensorMap tmDY, tmX;
+    wa::StateMaps tmS;
+    {
+        float* arrs[4] = {p, m, v, amsgrad ? vmax : p};   // without amsgrad the vmax map is never used
+        uint64_t dims[2] = {(uint64_t)K, (uint64_t)G * N};
+        uint64_t str[1] = {(uint64_t)K * 4};
+        uint32_t box[2] = {wa::CH_COLS, BM};
+        for (int a = 0; a < 4; ++a) {
+            int r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, arrs[a], 2, dims, str, box);
+            if (r) return r;
+        }
+    }
     {
         uint64_t dims[2] = {(uint64_t)N, (uint64_t)total_rows};
         uint64_t str[1] = {(uint64_t)lddy * 2};
@@ -676,7 +753,7 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
         if (e != cudaSuccess) return -(int)e;
         configured = true;
     }
-    wa::wgrad_adam_kernel<<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX);
+    wa::wgrad_adam_kernel<<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
     return -(int)cudaGetLastError();
 }
 

@@ -81,7 +81,8 @@ class DMoEConfig:
     # concurrently with the latency-bound chain of the backward pass (dgrads, LayerNorm backward, combine, the next layer's
     # dispatch).  `optimizer_ctas` SMs stream optimizer state, the chain keeps the remaining ones (persistent kernels of both
     # sides are launched with matching CTA limits so that neither starves the other).  0 disables the overlap, -1 = automatic:
-    # 11/14 of the SMs on one GPU, 9/14 when the experts are sharded (the sharded chain waits on peers and needs more SMs)
+    # 17/28 of the SMs on one GPU (80 of an H100's 132: the state stream already runs near copy bandwidth there, and the
+    # chain gains from the rest), 9/14 when the experts are sharded (the sharded chain waits on peers and needs more SMs)
     optimizer_ctas: int = -1
     # asynchronous expert updates (reference: EmulatedDMoE.update_every_inputs / update_every_steps,
     # experiments/convergence/dmoe_emulator.py:70-77): an expert accumulates weight gradients and steps once it has seen
@@ -211,7 +212,7 @@ class EngineContext:
         octas = int(_os.environ.get("LAH_OPTIMIZER_CTAS", cfg.optimizer_ctas))
         sms = torch.cuda.get_device_properties(self.device).multi_processor_count
         if octas < 0:
-            octas = sms * (11 if self.world == 1 else 9) // 14
+            octas = sms * (17 if self.world == 1 else 18) // 28
         self.opt_ctas = octas if (self.small and 0 < octas < sms - 8) else 0     # CTAs of the optimizer stream (0: no overlap)
         self.chain_ctas = sms - self.opt_ctas if self.opt_ctas else 0            # CTA limit of the persistent chain kernels
         self.opt_stream = torch.cuda.Stream(self.device) if self.opt_ctas else None

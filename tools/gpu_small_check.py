@@ -21,7 +21,7 @@ try:
     PEAKS = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
 except Exception:
     pass
-HBM = float(PEAKS.get("hbm_gbs", 6650.0))
+HBM = float(PEAKS.get("hbm_gbs", 3350.0))   # H100 SXM data sheet (HBM3)
 
 
 def rel(got, ref):
@@ -161,10 +161,20 @@ def perf():
     pb = torch.zeros(G, I, I, device="cuda", dtype=torch.bfloat16)
     step = torch.ones(G, dtype=torch.int32, device="cuda")
     dy = (torch.randn(total, I, device="cuda") * 0.1).to(torch.bfloat16)
-    ms = timeit(lambda: K.wgrad_adam(dy, a, off, rows, p=p, m=m, v=v, vmax=vmax, p_bf16=pb, step=step), flush=flush)
+    # device-to-device copy of a buffer far larger than L2: the bandwidth this card actually reaches (read + write)
+    src = torch.empty(1 << 30, dtype=torch.uint8, device="cuda")
+    dst = torch.empty_like(src)
+    ms_copy = timeit(lambda: dst.copy_(src))
+    copy_gbs = 2 * src.numel() / ms_copy / 1e6
+    del src, dst
+    record("perf_copy_1GiB", ok=True, ms=ms_copy, GBps=copy_gbs, frac_of_hbm=copy_gbs / HBM)
     nbytes = p.numel() * 34
-    record("perf_wgrad_adam_w2", ok=True, ms=ms, state_GB=nbytes / 1e9, TBps=nbytes / ms / 1e9,
-           frac_of_measured_copy=nbytes / ms / 1e6 / HBM)
+    # all SMs, and the optimizer stream's share of a 132-SM H100 in the training step (EngineContext, one GPU)
+    for tag, ctas in [("", 0), ("_opt_share", 132 * 17 // 28)]:
+        ms = timeit(lambda: K.wgrad_adam(dy, a, off, rows, p=p, m=m, v=v, vmax=vmax, p_bf16=pb, step=step, max_ctas=ctas),
+                    flush=flush)
+        record("perf_wgrad_adam_w2" + tag, ok=True, ms=ms, ctas=ctas or "all", state_GB=nbytes / 1e9,
+               TBps=nbytes / ms / 1e9, frac_of_hbm=nbytes / ms / 1e6 / HBM, frac_of_copy=nbytes / ms / 1e6 / copy_gbs)
     # the unfused pair it replaces: fp32 gradient written by a wgrad GEMM + the stand-alone AMSGrad kernel (38 B / param)
     g = torch.randn_like(p)
     rows_all = torch.full((G,), 16, dtype=torch.int32, device="cuda")
