@@ -11,6 +11,7 @@
 // Input : qkv [T = batch*512, 3*D] bf16 (output of the fused in_proj GEMM: [q | k | v] per token, heads contiguous)
 // Output: out [T, D] bf16 (heads concatenated, ready for out_proj); lse2 [T, heads] fp32 (optional)
 #include "sm90.cuh"
+#include "dropout.cuh"
 #include <stdlib.h>
 
 namespace lah {
@@ -33,9 +34,13 @@ constexpr int OFF_BAR2 = OFF_V2 + 2 * TILE_BYTES;
 constexpr int NUM_BARS = 1 + 2;
 constexpr int SMEM_TOTAL2 = OFF_BAR2 + NUM_BARS * 8 + 16 + 1024;
 
+// DROP: attention dropout (dropout.cuh, site 0).  The kept bf16 probabilities feed O += P V; the row sum l (and so the LSE)
+// keeps summing ALL of them, and 1 / (1 - p) is folded into the final 1 / l.
+template <bool DROP>
 __global__ void __launch_bounds__(NUM_THREADS2, 1)
 attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, float* __restrict__ lse2,
-                        int d_model, int num_heads, float scale_log2e) {
+                        int d_model, int num_heads, float scale_log2e, unsigned long long seed, uint32_t thr,
+                        float rescale) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR2);
@@ -86,6 +91,21 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
             wgmma_bf16_n128<0, 0>(s, make_smem_desc_sw128(sq + ks * 32, 0, 1024), make_smem_desc_sw128(sk + ks * 32, 0, 1024),
                                   ks > 0 ? 1u : 0u);
         wgmma_commit();
+        // keep bits of this thread's 64 scores, bit i <-> s[i], generated while the S MMA runs: one Philox granule per
+        // 16-key chunk kc covers rows {g, g+8} x keys {2c, 2c+1, 2c+8, 2c+9} = s[8kc .. 8kc+7]
+        uint32_t km[2] = {0u, 0u};
+        if constexpr (DROP) {
+            const uint32_t q = qt * Q_TILE + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+            for (int kc = 0; kc < KB / 16; ++kc) {
+                const uint4 bits = drop::attn_bits(seed, batch, head, drop::granule_attn(q), (8 * j + kc) * 4 + (lane & 3), q & 1u);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {   // lane e = h * 4 + jl * 2 + i  <->  s[4 (2kc + jl) + 2h + i]
+                    const int idx = 8 * kc + 4 * ((e >> 1) & 1) + 2 * (e >> 2) + (e & 1);
+                    km[idx >> 5] |= static_cast<uint32_t>(drop::keep(bits, e, thr)) << (idx & 31);
+                }
+            }
+        }
         wgmma_wait<0>();
         wgmma_fence_regs(s);
         uint32_t pa[KB / 16][4];
@@ -103,10 +123,15 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
             float sum = 0.f;
 #pragma unroll
             for (int jj = 0; jj < KB / 8; ++jj) {
-                const uint32_t pk = pack_bf16x2(exp2f(s[4 * jj + 2 * h] * scale_log2e - ms),
-                                                exp2f(s[4 * jj + 2 * h + 1] * scale_log2e - ms));
+                uint32_t pk = pack_bf16x2(exp2f(s[4 * jj + 2 * h] * scale_log2e - ms),
+                                          exp2f(s[4 * jj + 2 * h + 1] * scale_log2e - ms));
                 const float2 back = unpack_bf16x2(pk);   // sum what the tensor core will actually see
                 sum += back.x + back.y;
+                if constexpr (DROP) {
+                    const int idx = 4 * jj + 2 * h;
+                    const uint32_t b2 = (km[idx >> 5] >> (idx & 31)) & 3u;
+                    pk &= ((b2 & 1u) ? 0x0000ffffu : 0u) | ((b2 & 2u) ? 0xffff0000u : 0u);
+                }
                 // A fragment of key chunk jj/2: regs {row g, keys 0-7 | row g+8, keys 0-7 | row g, keys 8-15 | row g+8, ...}
                 pa[jj >> 1][(jj & 1) * 2 + h] = pk;
             }
@@ -134,7 +159,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         float lt = l[h];
         lt += __shfl_xor_sync(0xffffffffu, lt, 1);
         lt += __shfl_xor_sync(0xffffffffu, lt, 2);
-        const float inv = 1.f / lt;
+        const float inv = DROP ? rescale / lt : 1.f / lt;
         const long long token = seq_row0 + qt * Q_TILE + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
         if (lse2 && (lane & 3) == 0) lse2[token * num_heads + head] = m[h] * scale_log2e + log2f(lt);
         bf16* op = out + token * d_model + head * HEAD_DIM + 2 * (lane & 3);
@@ -159,8 +184,10 @@ using namespace lah::attn;
 extern "C" {
 
 // qkv: [tokens, 3*d_model] bf16, tokens = batch * 512; out: [tokens, d_model] bf16; lse2: [tokens, heads] fp32 or NULL
-int lah_attention_fwd(const void* qkv, void* out, float* lse2, int batch, int num_heads, int d_model, cudaStream_t st) {
-    if (d_model != num_heads * HEAD_DIM) return -2;
+// drop_thr < 0: no dropout; otherwise attention dropout with threshold drop_thr (dropout.cuh), seed, rescale = 1 / (1 - p)
+int lah_attention_fwd(const void* qkv, void* out, float* lse2, int batch, int num_heads, int d_model,
+                      unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
+    if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
     static PFN_encodeTiled fn = nullptr;
     if (!fn) {
         void* ptr = nullptr;
@@ -180,14 +207,17 @@ int lah_attention_fwd(const void* qkv, void* out, float* lse2, int batch, int nu
     if (r != CUDA_SUCCESS) return -1000 - (int)r;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(v2::attention_fwd_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, v2::SMEM_TOTAL2);
-        if (e != cudaSuccess) return -(int)e;
+        for (auto kern : {v2::attention_fwd_v2_kernel<false>, v2::attention_fwd_v2_kernel<true>}) {
+            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, v2::SMEM_TOTAL2);
+            if (e != cudaSuccess) return -(int)e;
+        }
         configured = true;
     }
     if (batch <= 0) return 0;
     const float scale_log2e = 1.4426950408889634f / sqrtf((float)HEAD_DIM);
-    v2::attention_fwd_v2_kernel<<<batch * num_heads * (S_LEN / Q_TILE), v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
-        tm, (bf16*)out, lse2, d_model, num_heads, scale_log2e);
+    auto kern = drop_thr < 0 ? v2::attention_fwd_v2_kernel<false> : v2::attention_fwd_v2_kernel<true>;
+    kern<<<batch * num_heads * (S_LEN / Q_TILE), v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
+        tm, (bf16*)out, lse2, d_model, num_heads, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale);
     return -(int)cudaGetLastError();
 }
 

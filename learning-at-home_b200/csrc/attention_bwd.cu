@@ -15,7 +15,13 @@
 // also stored once to shared memory (bf16, 128B-swizzled [key rows][64 queries] atoms), where it is the MN-major A operand
 // of dQ.  Q_i, dO_i, K_j are consumed both K-major (S, dP) and MN-major (dV, dK, dQ) straight from their TMA tiles.
 // Nothing of size S x S touches HBM.  Thread 0 also drives TMA.
+//
+// DROP (attention dropout, dropout.cuh site 0): the keep mask M is regenerated from the seed, never stored.  With
+// Pd = M o P / (1 - p):  dV += Pd^T dO,  dS = P o (M o dP / (1 - p) - Delta) * scale, Delta = rowsum(dO o O) of the DROPPED
+// output O (attn_delta_kernel, unchanged); LSE is that of the undropped softmax.  P^T is masked but not scaled in the dV
+// MMA; 1 / (1 - p) is applied to dV once at the end.
 #include "sm90.cuh"
+#include "dropout.cuh"
 
 namespace lah {
 namespace attnb {
@@ -37,11 +43,12 @@ constexpr int OFF_BAR = OFF_LSE + 2 * BLK * 4;
 constexpr int NUM_BARS = 1 + 2;
 constexpr int SMEM_TOTAL = OFF_BAR + NUM_BARS * 8 + 16 + 1024;
 
+template <bool DROP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
                      bf16* __restrict__ dq_part, long long total_tokens, int d_model, int num_heads, float scale,
-                     float scale_log2e) {
+                     float scale_log2e, unsigned long long seed, uint32_t thr, float rescale) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
@@ -107,18 +114,46 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         wgmma_wait<0>();
         wgmma_fence_regs(sacc);
         wgmma_fence_regs(dpacc);
+        const uint32_t kk = j * BLK + key_row;   // this thread's keys: kk, kk + 8
+        uint32_t km = 0u;
         uint32_t pa[BLK / 16][4], da[BLK / 16][4];
 #pragma unroll
         for (int jj = 0; jj < BLK / 8; ++jj) {
+            if constexpr (DROP) {
+                // keep bits of the 16-query chunk jp = jj / 2, bit 4 jl + 2h + par <-> sacc[4 (2jp + jl) + 2h + par]
+                // (keys kk + 8h x queries 16jp + qcol + 8jl + par): the granules of query parity 0 / 1 each hold 4 of them
+                if ((jj & 1) == 0) {
+                    km = 0u;
+#pragma unroll
+                    for (int par = 0; par < 2; ++par) {
+                        const uint4 bits = drop::attn_bits(seed, batch, head, (8 * i + (jj >> 1)) * 4 + (lane & 3),
+                                                           drop::granule_attn(kk), par);
+#pragma unroll
+                        for (int jl = 0; jl < 2; ++jl)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h)   // lane = query bit 3 * 4 + (key bit 0 | key bit 3 << 1)
+                                km |= static_cast<uint32_t>(drop::keep(bits, jl * 4 + static_cast<int>(kk & 1u) + 2 * h, thr))
+                                      << (4 * jl + 2 * h + par);
+                    }
+                }
+            }
             const int q = 8 * jj + qcol;
             const float l0 = s_lse[q], l1 = s_lse[q + 1], d0 = s_delta[q], d1 = s_delta[q + 1];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const float p0 = exp2f(sacc[4 * jj + 2 * h] * scale_log2e - l0);
                 const float p1 = exp2f(sacc[4 * jj + 2 * h + 1] * scale_log2e - l1);
-                const uint32_t pp = pack_bf16x2(p0, p1);
-                const uint32_t dd = pack_bf16x2(p0 * (dpacc[4 * jj + 2 * h] - d0) * scale,
-                                                p1 * (dpacc[4 * jj + 2 * h + 1] - d1) * scale);
+                uint32_t pp, dd;
+                if constexpr (DROP) {
+                    const int idx = 4 * (jj & 1) + 2 * h;
+                    const bool k0 = (km >> idx) & 1u, k1 = (km >> (idx + 1)) & 1u;
+                    pp = pack_bf16x2(k0 ? p0 : 0.f, k1 ? p1 : 0.f);
+                    dd = pack_bf16x2(p0 * ((k0 ? dpacc[4 * jj + 2 * h] * rescale : 0.f) - d0) * scale,
+                                     p1 * ((k1 ? dpacc[4 * jj + 2 * h + 1] * rescale : 0.f) - d1) * scale);
+                } else {
+                    pp = pack_bf16x2(p0, p1);
+                    dd = pack_bf16x2(p0 * (dpacc[4 * jj + 2 * h] - d0) * scale, p1 * (dpacc[4 * jj + 2 * h + 1] - d1) * scale);
+                }
                 pa[jj >> 1][(jj & 1) * 2 + h] = pp;
                 da[jj >> 1][(jj & 1) * 2 + h] = dd;
                 // dS^T[key][q]: atom q / 64, 16 B chunk (q % 64) / 8 swizzled with key & 7
@@ -172,7 +207,10 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
 #pragma unroll
         for (int jj = 0; jj < HEAD_DIM / 8; ++jj) {
             *reinterpret_cast<uint32_t*>(dkp + 8 * jj) = pack_bf16x2(dk[4 * jj + 2 * h], dk[4 * jj + 2 * h + 1]);
-            *reinterpret_cast<uint32_t*>(dvp + 8 * jj) = pack_bf16x2(dv[4 * jj + 2 * h], dv[4 * jj + 2 * h + 1]);
+            if constexpr (DROP)
+                *reinterpret_cast<uint32_t*>(dvp + 8 * jj) = pack_bf16x2(dv[4 * jj + 2 * h] * rescale, dv[4 * jj + 2 * h + 1] * rescale);
+            else
+                *reinterpret_cast<uint32_t*>(dvp + 8 * jj) = pack_bf16x2(dv[4 * jj + 2 * h], dv[4 * jj + 2 * h + 1]);
         }
     }
 }
@@ -230,9 +268,11 @@ extern "C" {
 // qkv [T, 3D] bf16 (forward input), out [T, D] bf16 (forward output), dout [T, D] bf16, lse2 [T, H] fp32 (forward output)
 // -> dqkv [T, 3D] bf16.  Scratch: delta [T, H] fp32 (rowsum(dout o out), computed here), dq_part [4, T, D] bf16 (the four
 // per-key-block partials of dQ, reduced into the Q third of dqkv here).  Three launches, no PyTorch ops around them.
+// drop_thr < 0: the forward ran without dropout; otherwise the same (seed, drop_thr, rescale) as lah_attention_fwd.
 int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
-                      void* dq_part, int batch, int num_heads, int d_model, cudaStream_t st) {
-    if (d_model != num_heads * HEAD_DIM) return -2;
+                      void* dq_part, int batch, int num_heads, int d_model, unsigned long long seed, int drop_thr,
+                      float rescale, cudaStream_t st) {
+    if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
     static PFN_encodeTiled fn = nullptr;
     if (!fn) {
         void* ptr = nullptr;
@@ -262,17 +302,20 @@ int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const 
     }
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(attention_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
-        if (e != cudaSuccess) return -(int)e;
+        for (auto kern : {attention_bwd_kernel<false>, attention_bwd_kernel<true>}) {
+            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
+            if (e != cudaSuccess) return -(int)e;
+        }
         configured = true;
     }
     if (batch <= 0) return 0;
     const float scale = 1.f / sqrtf((float)HEAD_DIM);
     const long long tokens = (long long)batch * S_LEN, pairs = tokens * num_heads;
     attn_delta_kernel<<<(unsigned)((pairs * 32 + 255) / 256), 256, 0, st>>>((const bf16*)dout, (const bf16*)out, delta, pairs);
-    attention_bwd_kernel<<<batch * num_heads * (S_LEN / BLK), NUM_THREADS, SMEM_TOTAL, st>>>(
+    auto kern = drop_thr < 0 ? attention_bwd_kernel<false> : attention_bwd_kernel<true>;
+    kern<<<batch * num_heads * (S_LEN / BLK), NUM_THREADS, SMEM_TOTAL, st>>>(
         tm_qkv, tm_do, lse2, delta, (bf16*)dqkv, (bf16*)dq_part, tokens, d_model, num_heads, scale,
-        scale * 1.4426950408889634f);
+        scale * 1.4426950408889634f, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale);
     attn_dq_reduce_kernel<<<(unsigned)((tokens * d_model / 8 + 255) / 256), 256, 0, st>>>((const bf16*)dq_part, (bf16*)dqkv, tokens, d_model,
                                                                                          S_LEN / BLK);
     return -(int)cudaGetLastError();

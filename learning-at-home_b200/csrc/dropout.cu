@@ -1,0 +1,112 @@
+// dropout.cu — elementwise dropout kernels of the transformer expert and the mask materialiser (masks: dropout.cuh).
+//
+//   op 0  out = M o x / (1 - p)                            backward of dropout1 / dropout2 (the branch side of the residual)
+//   op 1  out = M o gelu(x) / (1 - p)                      forward of linear1's activation + dropout
+//   op 2  out = gelu'(f) o M o x / (1 - p)   (x = dg)      backward of the same
+//
+// One thread owns one mask granule ({r, r+8} x {b, b+1, b+8, b+9}): one Philox call, eight elements, 4-byte accesses that a
+// quad of threads turns into 32 contiguous bytes per row.  GELU is the erf form, as nn.GELU().
+#include "sm90.cuh"
+#include "dropout.cuh"
+
+namespace lah {
+namespace drop {
+
+constexpr int OP_APPLY = 0, OP_GELU_FWD = 1, OP_GELU_BWD = 2;
+
+__device__ __forceinline__ float gelu_f(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752f)); }
+__device__ __forceinline__ float gelu_grad(float v) {
+    return 0.5f * (1.f + erff(v * 0.70710678118654752f)) + v * 0.39894228040143268f * __expf(-0.5f * v * v);
+}
+
+template <int OP>
+__global__ void __launch_bounds__(256) dropout_ew_kernel(const bf16* __restrict__ x, const bf16* __restrict__ f,
+                                                         bf16* __restrict__ out, long long granules, int cols,
+                                                         unsigned long long seed, int site, uint32_t thr, float scale) {
+    const long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (t >= granules) return;
+    const int col_granules = cols >> 2;
+    const uint32_t gr = static_cast<uint32_t>(t / col_granules), gn = static_cast<uint32_t>(t % col_granules);
+    const uint4 bits = rc_bits(seed, site, gr, gn);
+    const long long r0 = static_cast<long long>(gr >> 3) * 16 + (gr & 7);
+    const int n0 = static_cast<int>(gn >> 2) * 16 + 2 * static_cast<int>(gn & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int jl = 0; jl < 2; ++jl) {
+            const long long off = (r0 + 8 * h) * cols + n0 + 8 * jl;
+            const float2 xv = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(x + off)));
+            float v[2] = {xv.x, xv.y};
+            float fv[2] = {0.f, 0.f};
+            if (OP == OP_GELU_BWD) {
+                const float2 t2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(f + off)));
+                fv[0] = t2.x;
+                fv[1] = t2.y;
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const float s = keep(bits, h * 4 + jl * 2 + i, thr) ? scale : 0.f;
+                if (OP == OP_APPLY) v[i] = v[i] * s;
+                if (OP == OP_GELU_FWD) v[i] = gelu_f(v[i]) * s;
+                if (OP == OP_GELU_BWD) v[i] = gelu_grad(fv[i]) * (v[i] * s);
+            }
+            *reinterpret_cast<uint32_t*>(out + off) = pack_bf16x2(v[0], v[1]);
+        }
+    }
+}
+
+// mask[b, h, r, c] (uint8 0 / 1): site 0 -> keep_attn(b, h, query r, key c); sites 1-3 -> keep_rc(r, c) (b = h = 0)
+__global__ void __launch_bounds__(256) dropout_mask_kernel(uint8_t* __restrict__ out, int site, int heads, int rows,
+                                                           int cols, long long total, unsigned long long seed, uint32_t thr) {
+    const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const uint32_t c = static_cast<uint32_t>(i % cols);
+    const long long br = i / cols;
+    const uint32_t r = static_cast<uint32_t>(br % rows);
+    const long long bh = br / rows;
+    const bool k = site == SITE_ATTN ? keep_attn(seed, static_cast<int>(bh / heads), static_cast<int>(bh % heads), r, c, thr)
+                                     : keep_rc(seed, site, r, c, thr);
+    out[i] = k ? 1 : 0;
+}
+
+}  // namespace drop
+}  // namespace lah
+
+using namespace lah;
+using namespace lah::drop;
+
+extern "C" {
+
+// out[batch, heads, rows, cols] uint8 keep mask of `site` (sites 1-3: batch = heads = 1)
+int lah_dropout_mask(void* out, int site, int batch, int heads, int rows, int cols, unsigned long long seed, int thr,
+                     cudaStream_t st) {
+    if (site < 0 || site > 3 || batch < 0 || heads < 1 || rows < 0 || cols < 1 || thr < 0 || thr > 65535) return -2;
+    if (site != SITE_ATTN && (batch != 1 || heads != 1)) return -2;
+    const long long total = static_cast<long long>(batch) * heads * rows * cols;
+    if (total == 0) return 0;
+    dropout_mask_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((uint8_t*)out, site, heads, rows, cols, total, seed,
+                                                                       static_cast<uint32_t>(thr));
+    return -(int)cudaGetLastError();
+}
+
+// elementwise dropout op (see the top of this file) over contiguous [rows, cols] bf16 tensors; rows, cols multiples of 16
+int lah_dropout_ew(int op, const void* x, const void* f, void* out, long long rows, int cols, unsigned long long seed,
+                   int site, int thr, float scale, cudaStream_t st) {
+    if ((rows % 16) || (cols % 16) || cols <= 0 || site < 1 || site > 3 || thr < 0 || thr > 65535) return -2;
+    const long long granules = rows * cols / 8;
+    if (granules == 0) return 0;
+    const unsigned grid = (unsigned)((granules + 255) / 256);
+    const uint32_t t = static_cast<uint32_t>(thr);
+    if (op == OP_APPLY)
+        dropout_ew_kernel<OP_APPLY><<<grid, 256, 0, st>>>((const bf16*)x, nullptr, (bf16*)out, granules, cols, seed, site, t, scale);
+    else if (op == OP_GELU_FWD)
+        dropout_ew_kernel<OP_GELU_FWD><<<grid, 256, 0, st>>>((const bf16*)x, nullptr, (bf16*)out, granules, cols, seed, site, t, scale);
+    else if (op == OP_GELU_BWD)
+        dropout_ew_kernel<OP_GELU_BWD><<<grid, 256, 0, st>>>((const bf16*)x, (const bf16*)f, (bf16*)out, granules, cols, seed, site, t,
+                                                            scale);
+    else
+        return -3;
+    return -(int)cudaGetLastError();
+}
+
+}  // extern "C"

@@ -17,7 +17,13 @@
 //              (bias / activation / residual / accumulate -> bf16 | fp32 -> global) straight from its registers
 //   warp 8     TMA producer (one lane): cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier complete_tx; it runs
 //              ahead into the next tile while the consumers drain the previous one
+//
+// DROP (MGROUP, 128 x 256 tiles, K-major B, bf16 C only; the transformer expert's dropout1 / dropout2): after the bias and
+// the activation, before the residual, v = M o v / (1 - p) with the (token row, column) mask of dropout.cuh.  Every other
+// instantiation has DROP = false and is unchanged.
 #include "sm90.cuh"
+#include "dropout.cuh"
+#include <type_traits>
 
 namespace lah {
 
@@ -51,6 +57,14 @@ struct GemmParams {
     int accumulate;          // KGROUP: C += result (gradient accumulation across steps, update_every_*)
 };
 
+// parameters of the DROP instantiation: mask of dropout.cuh site `drop_site`, threshold drop_thr, kept values * drop_scale
+struct GemmDropParams : GemmParams {
+    unsigned long long drop_seed;
+    uint32_t drop_thr;
+    float drop_scale;
+    int drop_site;
+};
+
 template <int BLOCK_N, int STAGES>
 struct SmemLayout {
     static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
@@ -78,9 +92,11 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t s
     }
 }
 
-template <int BLOCK_N, int STAGES, int MODE, bool A_MN, bool B_MN, bool OUT_F32>
+template <int BLOCK_N, int STAGES, int MODE, bool A_MN, bool B_MN, bool OUT_F32, bool DROP = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB) {
+gemm_kernel(const typename std::conditional<DROP, GemmDropParams, GemmParams>::type p, const __grid_constant__ CUtensorMap tmA,
+            const __grid_constant__ CUtensorMap tmB) {
+    static_assert(!DROP || (BLOCK_N == 256 && MODE == MODE_MGROUP), "dropout epilogue: 128 x 256 MGROUP tiles only");
     using L = SmemLayout<BLOCK_N, STAGES>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -227,6 +243,23 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const _
         if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
         // ------------------------------------------------------------ epilogue from registers
+        // DROP: keep bits of this thread's accumulator, bit i of km[i / 64] <-> acc[i]; the granule of 16-column chunk J
+        // covers rows {row, row + 8} x columns {2c, 2c+1, 2c+8, 2c+9} = acc[8J .. 8J+7].  The loop is not unrolled so that
+        // the Philox rounds do not compete with the live accumulator for registers.
+        uint64_t km[2] = {0ull, 0ull};
+        if constexpr (DROP) {
+            const uint32_t gr = drop::granule_row(static_cast<uint32_t>(m_row + row_in_tile));
+#pragma unroll 1
+            for (int J = 0; J < BLOCK_N / 16; ++J) {
+                const uint4 bits = drop::rc_bits(p.drop_seed, p.drop_site, gr, ((n_col >> 4) + J) * 4 + (lane & 3));
+                uint64_t b8 = 0;
+#pragma unroll
+                for (int e = 0; e < 8; ++e)   // lane e = h * 4 + jl * 2 + i  <->  acc[4 (2J + jl) + 2h + i]
+                    b8 |= static_cast<uint64_t>(drop::keep(bits, e, p.drop_thr)) << (4 * ((e >> 1) & 1) + 2 * (e >> 2) + (e & 1));
+                if (J < 8) km[0] |= b8 << (8 * J);
+                else km[1] |= b8 << (8 * (J - 8));
+            }
+        }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = m_row + row_in_tile + 8 * h;
@@ -251,6 +284,11 @@ gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmA, const _
                     } else if (p.act == 2) {
                         v0 = 0.5f * v0 * (1.f + erff(v0 * 0.70710678118654752f));
                         v1 = 0.5f * v1 * (1.f + erff(v1 * 0.70710678118654752f));
+                    }
+                    if constexpr (DROP) {
+                        const int idx = 4 * j + 2 * h;
+                        v0 = ((km[idx >> 6] >> (idx & 63)) & 1u) ? v0 * p.drop_scale : 0.f;
+                        v1 = ((km[idx >> 6] >> ((idx & 63) + 1)) & 1u) ? v1 * p.drop_scale : 0.f;
                     }
                     if (p.residual) {
                         const float2 r = unpack_bf16x2(
@@ -324,10 +362,10 @@ static int num_sms() {
     return g_num_sms;
 }
 
-template <int BLOCK_N, int STAGES, int MODE, bool A_MN, bool B_MN, bool OUT_F32>
-static int launch(const GemmParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int max_ctas, cudaStream_t st) {
+template <int BLOCK_N, int STAGES, int MODE, bool A_MN, bool B_MN, bool OUT_F32, bool DROP = false, typename P>
+static int launch(const P& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int max_ctas, cudaStream_t st) {
     using L = SmemLayout<BLOCK_N, STAGES>;
-    auto kern = gemm_kernel<BLOCK_N, STAGES, MODE, A_MN, B_MN, OUT_F32>;
+    auto kern = gemm_kernel<BLOCK_N, STAGES, MODE, A_MN, B_MN, OUT_F32, DROP>;
     static bool configured = false;
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
@@ -348,8 +386,10 @@ static int launch(const GemmParams& p, const CUtensorMap& tmA, const CUtensorMap
 static int gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
                        long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group, const float* bias,
                        const void* residual, long long ldr, int block_n, int max_ctas, const int* wait_flags,
-                       int wait_count, int wait_epoch, int* status, int act, const int* epoch_base, cudaStream_t stream) {
+                       int wait_count, int wait_epoch, int* status, int act, const int* epoch_base, cudaStream_t stream,
+                       unsigned long long drop_seed = 0, int drop_thr = -1, float drop_scale = 1.f, int drop_site = 0) {
     if ((K % 8) || (N % 32) || (lda % 8)) return -2;
+    if (drop_thr >= 0 && (block_n != 256 || b_mn || out_f32 || drop_thr > 65535)) return -4;
     if (block_n != 256 && block_n != 128 && block_n != 64) return -3;
     CUtensorMap tmA, tmB;
     {
@@ -378,6 +418,13 @@ static int gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, 
     p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr;
     p.wait_flags = wait_flags; p.wait_count = wait_count; p.wait_epoch = wait_epoch; p.epoch_base = epoch_base; p.status = status;
     p.act = act; p.accumulate = 0;
+    if (drop_thr >= 0) {
+        GemmDropParams pd;
+        static_cast<GemmParams&>(pd) = p;
+        pd.drop_seed = drop_seed; pd.drop_thr = static_cast<uint32_t>(drop_thr); pd.drop_scale = drop_scale;
+        pd.drop_site = drop_site;
+        return launch<256, 4, MODE_MGROUP, false, false, false, true>(pd, tmA, tmB, max_ctas, stream);
+    }
 #define LAH_LAUNCH_M(BN, ST)                                                                                   \
     if (!b_mn && !out_f32) return launch<BN, ST, MODE_MGROUP, false, false, false>(p, tmA, tmB, max_ctas, stream); \
     if (b_mn && !out_f32) return launch<BN, ST, MODE_MGROUP, false, true, false>(p, tmA, tmB, max_ctas, stream);   \
@@ -459,6 +506,18 @@ int lah_gemm_mgroup2(const void* A, long long lda, int a_rows, const void* B, in
     return gemm_mgroup(A, lda, a_rows, B, G, N, K, b_mn, C, ldc, out_f32, m_valid, num_m_tiles128, tile_group, bias,
                        residual, ldr, 256, max_ctas, wait_flags, wait_count, wait_epoch, status, act, lah_get_epoch_base(),
                        stream);
+}
+
+// lah_gemm_mgroup2 with K-major B and bf16 C, plus dropout after the bias / activation and before the residual
+// (grouped_gemm.cu DROP, dropout.cuh): kept values are multiplied by drop_scale = 1 / (1 - p), drop_thr in [0, 65535]
+int lah_gemm_mgroup2_drop(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, void* C, long long ldc,
+                          int m_valid, int num_m_tiles128, const int* tile_group, const float* bias, const void* residual,
+                          long long ldr, int max_ctas, int act, unsigned long long drop_seed, int drop_thr, float drop_scale,
+                          int drop_site, cudaStream_t stream) {
+    if (drop_thr < 0 || drop_site < 1 || drop_site > 3) return -2;
+    return gemm_mgroup(A, lda, a_rows, B, G, N, K, 0, C, ldc, 0, m_valid, num_m_tiles128, tile_group, bias, residual, ldr, 256,
+                       max_ctas, nullptr, 0, 0, nullptr, act, lah_get_epoch_base(), stream, drop_seed, drop_thr, drop_scale,
+                       drop_site);
 }
 
 int lah_gemm_kgroup2(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,

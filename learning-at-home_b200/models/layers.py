@@ -8,7 +8,10 @@ Expert architectures (the L1 "ops/models" layer of SURVEY.md).
   batch-first input ``[B, S, d]`` (/root/reference/experiments/throughput/layers.py:22-51).  Unlike the reference it
   does NOT transpose its input in place, so it does not mutate the caller's tensor and it is trainable through
   ``ExpertBackend.backward`` (the reference's block raises there; SURVEY.md §0.3).  Parameter names are identical
-  (``self_attn.in_proj_weight`` ..., ``linear1``, ``linear2``, ``norm1``, ``norm2``).
+  (``self_attn.in_proj_weight`` ..., ``linear1``, ``linear2``, ``norm1``, ``norm2``).  Its four dropouts (attention
+  probabilities, ``dropout1``, ``dropout`` after the GELU, ``dropout2``) act in training mode, which is the mode
+  ``ExpertBackend`` runs it in; the sm_90a executor (``runtime/native_executor.py``) implements them with in-kernel
+  Philox masks (DESIGN.md §9), so the reference's default ``name_to_block["transformer"]`` trains natively.
 
 These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_90a execution of the same
 maths lives in ``lah_b200.parallel.engine`` (grouped wgmma GEMMs + fused LN/ReLU/Adam kernels).

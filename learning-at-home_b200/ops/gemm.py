@@ -36,6 +36,10 @@ def _lib():
         lib.lah_gemm_mgroup2.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_ll,
                                          c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_void_p,
                                          c_int, c_void_p]
+        lib.lah_gemm_mgroup2_drop.restype = c_int
+        lib.lah_gemm_mgroup2_drop.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_ll, c_int, c_int,
+                                              c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, ctypes.c_ulonglong, c_int,
+                                              ctypes.c_float, c_int, c_void_p]
         lib.lah_gemm_kgroup2.restype = c_int
         lib.lah_gemm_kgroup2.argtypes = [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p,
                                          c_void_p, c_ll, c_ll, c_int, c_int, c_void_p]
@@ -52,7 +56,8 @@ def _pick_block_n(n: int) -> int:
 
 
 def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=False, out=None,
-                   out_dtype=torch.bfloat16, m_valid=None, block_n=None, max_ctas=0, two_cta=False, wait=None, act=0):
+                   out_dtype=torch.bfloat16, m_valid=None, block_n=None, max_ctas=0, two_cta=False, wait=None, act=0,
+                   dropout=None):
     """
     out[r, :] = a[r, :] @ W[g(r)]^T (+ bias[g(r)]) (+ residual[r, :])
 
@@ -63,6 +68,8 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
     :param act: activation fused after the bias (wide-tile kernel only): 0 none, 1 ReLU, 2 GELU(erf)
     :param wait: (flags int32 tensor [count], epoch, status tensor) — receive-side fusion: the kernel's TMA producer
         polls the peers' dispatch flags (ld.acquire.sys) before its first load instead of a separate wait kernel
+    :param dropout: (p, seed, site): out = M o act(a W^T + bias) / (1 - p) (+ residual), M the (row, column) mask of
+        ``kernels.dropout_mask`` site 1-3; wide-tile kernel, y = x W^T, bf16 output.  p = 0 or None: no dropout
     """
     wait_flags, wait_count, wait_epoch, wait_status = (wait[0], wait[0].numel(), wait[1], wait[2]) if wait else (None, 0, 0, None)
     assert a.is_cuda and a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and a.dim() == 2 and w.dim() == 3
@@ -85,6 +92,17 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
         assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == G * N
     if residual is not None:
         assert residual.dtype == torch.bfloat16 and residual.stride(1) == 1
+    if dropout is not None and dropout[0] > 0:
+        from .kernels import _dropout_args
+        assert two_cta and N % 256 == 0 and not w_is_kn and out.dtype == torch.bfloat16 and wait is None
+        seed, thr, scale = _dropout_args(dropout[:2])
+        code = _lib().lah_gemm_mgroup2_drop(
+            ptr(a), a.stride(0), rows, ptr(w), G, N, K, ptr(out), out.stride(0), rows if m_valid is None else m_valid,
+            num_m_tiles, ptr(tile_group), ptr(bias), ptr(residual), residual.stride(0) if residual is not None else 0,
+            max_ctas, int(act), seed, thr, scale, int(dropout[2]), stream_ptr())
+        native.check(code, "lah_gemm_mgroup2_drop")
+        native.count_launch()
+        return out
     if two_cta and N % 256 == 0:
         # wide-tile kernel (128x256 tiles): expert groups must be padded to 256 rows
         code = _lib().lah_gemm_mgroup2(

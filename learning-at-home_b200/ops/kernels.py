@@ -3,6 +3,7 @@ Python entry points for the non-GEMM sm_90a kernels (csrc/layernorm.cu, csrc/moe
 oracles.  All wrappers launch on the current CUDA stream, never synchronise, and are CUDA-graph capturable.
 """
 import ctypes
+import math
 
 import torch
 import torch.nn.functional as F
@@ -56,8 +57,10 @@ def _lib():
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, P],
         "lah_bump_steps": [P, P, I, P],
         "lah_cast_bf16": [P, P, L, P],
-        "lah_attention_fwd": [P, P, P, I, I, I, P],
-        "lah_attention_bwd": [P, P, P, P, P, P, P, I, I, I, P],
+        "lah_attention_fwd": [P, P, P, I, I, I, c_ull, I, Fl, P],
+        "lah_attention_bwd": [P, P, P, P, P, P, P, I, I, I, c_ull, I, Fl, P],
+        "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
+        "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
         "lah_symm_alloc": [c_ull, ctypes.POINTER(c_void_p)],
         "lah_symm_free": [P],
         "lah_symm_get_handle": [P, ctypes.c_char_p],
@@ -262,11 +265,14 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
 # ---------------------------------------------------------------------------------------------------------
 # attention (transformer expert)
 # ---------------------------------------------------------------------------------------------------------
-def attention_fwd(qkv, num_heads, *, out=None, lse=None):
+def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None):
     """
     Self-attention over 512-token sequences on wgmma (csrc/attention.cu).
     :param qkv: [batch*512, 3*d_model] bf16 = in_proj output, [q | k | v] per token; head_dim must be 64
-    :param lse: optional fp32 [batch*512, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd)
+    :param lse: optional fp32 [batch*512, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd); with
+        dropout it is still that of the undropped softmax
+    :param dropout: (p, seed): O = (M o P) V / (1 - p) with the site-0 mask of ``dropout_mask``; p = 0 or None launches the
+        kernel without dropout
     :returns: [batch*512, d_model] bf16, heads concatenated (input of out_proj)
     """
     tokens, three_d = qkv.shape
@@ -276,16 +282,18 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None):
         out = torch.empty(tokens, d_model, dtype=torch.bfloat16, device=qkv.device)
     if lse is not None:
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == tokens * num_heads
-    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens // 512, num_heads, d_model, stream_ptr()),
-                 "lah_attention_fwd")
+    seed, thr, rescale = _dropout_args(dropout)
+    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens // 512, num_heads, d_model, seed, thr, rescale,
+                                          stream_ptr()), "lah_attention_fwd")
     native.count_launch()
     return out
 
 
-def attention_bwd(qkv, out, dout, lse, num_heads):
+def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None):
     """
     Backward of ``attention_fwd`` on wgmma (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
     dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.
+    :param dropout: the (p, seed) of the forward that produced ``out``; the mask is regenerated, not read
     """
     tokens, three_d = qkv.shape
     d_model = three_d // 3
@@ -295,7 +303,8 @@ def attention_bwd(qkv, out, dout, lse, num_heads):
     dqkv = torch.empty_like(qkv)
     dq_part = torch.empty(4, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
     native.check(_lib().lah_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
-                                          tokens // 512, num_heads, d_model, stream_ptr()), "lah_attention_bwd")
+                                          tokens // 512, num_heads, d_model, *_dropout_args(dropout), stream_ptr()),
+                 "lah_attention_bwd")
     native.count_launch(3)   # delta prologue, wgmma backward, dQ partial reduction
     return dqkv
 
@@ -308,6 +317,124 @@ def attention_ref(qkv, num_heads, seq_len=512):
     q, k, v = (t.transpose(1, 2) for t in (q, k, v))  # [B, H, S, hd]
     att = torch.softmax(q @ k.transpose(-1, -2) / (d // num_heads) ** 0.5, dim=-1) @ v
     return att.transpose(1, 2).reshape(tokens, d)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# dropout of the transformer expert (csrc/dropout.cuh: counter-based Philox4x32-10 masks, csrc/dropout.cu)
+#   site 0 = attention probabilities, position (batch, head, query, key)
+#   sites 1, 2, 3 = dropout1 (after out_proj), dropout (after linear1's GELU), dropout2 (after linear2), position (row, col)
+# ---------------------------------------------------------------------------------------------------------
+SITE_ATTN, SITE_OUT_PROJ, SITE_FF, SITE_LINEAR2 = range(4)
+
+
+def dropout_threshold(p):
+    """an element is kept iff its 16-bit Philox lane >= this; the realised drop probability is threshold / 65536"""
+    assert 0.0 <= p < 1.0, p
+    return min(65535, int(math.floor(p * 65536 + 0.5)))
+
+
+def _dropout_args(dropout):
+    """(seed, threshold, 1 / (1 - p)) for the C entry points; threshold -1 = no dropout"""
+    if dropout is None or dropout[0] == 0:
+        return 0, -1, 1.0
+    p, seed = dropout[0], dropout[1]
+    return int(seed) & (2 ** 64 - 1), dropout_threshold(p), 1.0 / (1.0 - p)
+
+
+def dropout_mask(shape, p, seed, site, device=None):
+    """
+    Materialised keep mask (bool) from the same device functions the fused kernels use: ``shape`` is (batch, heads, queries,
+    keys) for site 0 and (rows, cols) for sites 1-3.  For tests and oracles; the training path never stores a mask.
+    """
+    if site == SITE_ATTN:
+        batch, heads, rows, cols = shape
+    else:
+        (rows, cols), batch, heads = shape, 1, 1
+    out = torch.empty(*shape, dtype=torch.uint8, device=device or "cuda")
+    native.check(_lib().lah_dropout_mask(ptr(out), int(site), batch, heads, rows, cols, int(seed) & (2 ** 64 - 1),
+                                         dropout_threshold(p), stream_ptr()), "lah_dropout_mask")
+    native.count_launch()
+    return out.bool()
+
+
+def _dropout_ew(op, x, f, p, seed, site, out):
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.dim() == 2 and 1 <= site <= 3
+    assert f is None or (f.shape == x.shape and f.dtype == torch.bfloat16 and f.is_contiguous())
+    out = torch.empty_like(x) if out is None else out
+    assert out.shape == x.shape and out.is_contiguous()
+    rows, cols = x.shape
+    native.check(_lib().lah_dropout_ew(op, ptr(x), ptr(f), ptr(out), rows, cols, int(seed) & (2 ** 64 - 1), int(site),
+                                       dropout_threshold(p), 1.0 / (1.0 - p), stream_ptr()), "lah_dropout_ew")
+    native.count_launch()
+    return out
+
+
+def dropout_apply(x, p, seed, site, *, out=None):
+    """out = M o x / (1 - p) (bf16 [rows, cols], rows and cols multiples of 16): the gradient of a dropout site's branch"""
+    return _dropout_ew(0, x, None, p, seed, site, out)
+
+
+def gelu_dropout(f, p, seed, site, *, out=None):
+    """out = M o gelu(f) / (1 - p) (erf GELU)"""
+    return _dropout_ew(1, f, None, p, seed, site, out)
+
+
+def gelu_dropout_bwd(dg, f, p, seed, site, *, out=None):
+    """out = gelu'(f) o M o dg / (1 - p): backward of ``gelu_dropout``"""
+    return _dropout_ew(2, dg, f, p, seed, site, out)
+
+
+_PHILOX_M0, _PHILOX_M1, _PHILOX_W0, _PHILOX_W1 = 0xD2511F53, 0xCD9E8D57, 0x9E3779B9, 0xBB67AE85
+_U32 = 0xFFFFFFFF
+
+
+def _mulhilo32(a, m):
+    """(a * m) >> 32 and (a * m) & 0xffffffff for int64 tensors holding uint32 values, without 64-bit overflow"""
+    t1, t2 = (a & 0xFFFF) * m, (a >> 16) * m
+    return (t2 + (t1 >> 16)) >> 16, (((t2 & 0xFFFF) << 16) + t1) & _U32
+
+
+def philox4x32_10_ref(ctr, key):
+    """CPU Philox4x32-10 (Salmon et al., SC'11) on int64 tensors holding uint32 values; ctr: 4 words, key: 2 words"""
+    c = [torch.as_tensor(w, dtype=torch.int64) for w in ctr]
+    c = list(torch.broadcast_tensors(*c))
+    k0, k1 = int(key[0]) & _U32, int(key[1]) & _U32
+    for _ in range(10):
+        hi0, lo0 = _mulhilo32(c[0], _PHILOX_M0)
+        hi1, lo1 = _mulhilo32(c[2], _PHILOX_M1)
+        c = [hi1 ^ c[1] ^ k0, lo1, hi0 ^ c[3] ^ k1, lo0]
+        k0, k1 = (k0 + _PHILOX_W0) & _U32, (k1 + _PHILOX_W1) & _U32
+    return c
+
+
+def dropout_keep_ref(p, seed, site, *index):
+    """
+    Independent CPU definition of the keep decision (the mask definition of csrc/dropout.cuh): ``index`` are broadcastable
+    integer tensors, (batch, head, query, key) for site 0 and (row, col) for sites 1-3.  Returns a bool tensor.
+    """
+    idx = torch.broadcast_tensors(*[torch.as_tensor(t, dtype=torch.int64) for t in index])
+    seed = int(seed) & (2 ** 64 - 1)
+    zero = torch.zeros_like(idx[0])
+    if site == SITE_ATTN:
+        b, h, q, k = idx
+        gq, gk = (q >> 4) * 4 + ((q >> 1) & 3), (k >> 4) * 4 + ((k >> 1) & 3)
+        ctr = ((gq * 128 + gk) | ((q & 1) << 14), h, b, zero)
+        lane = ((q >> 3) & 1) * 4 + ((k & 1) | (((k >> 3) & 1) << 1))
+    else:
+        r, n = idx
+        gr, gn = (r >> 4) * 8 + (r & 7), (n >> 4) * 4 + ((n >> 1) & 3)
+        ctr = (gn, gr, zero, zero + site)
+        lane = ((r >> 3) & 1) * 4 + ((n & 1) | (((n >> 3) & 1) << 1))
+    words = torch.stack(philox4x32_10_ref(ctr, (seed & _U32, seed >> 32)), dim=-1)
+    w = words.gather(-1, (lane >> 1).unsqueeze(-1)).squeeze(-1)
+    u16 = torch.where((lane & 1) == 1, w >> 16, w & 0xFFFF)
+    return u16 >= dropout_threshold(p)
+
+
+def dropout_mask_ref(shape, p, seed, site):
+    """CPU counterpart of ``dropout_mask`` (same shape convention)"""
+    grids = [torch.arange(n).view(*([1] * i), n, *([1] * (len(shape) - i - 1))) for i, n in enumerate(shape)]
+    return dropout_keep_ref(p, seed, site, *grids)
 
 
 # ---------------------------------------------------------------------------------------------------------

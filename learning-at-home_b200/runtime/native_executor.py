@@ -173,16 +173,32 @@ class NativeFFNExecutor:
         return self.dxd[:rows].to(x.dtype)
 
 
+def draw_dropout_seed() -> int:
+    """the 64-bit seed of one dropout executor call, drawn from torch's default CPU generator (no device read, no sync;
+    ``torch.manual_seed`` makes it reproducible)"""
+    lo, hi = torch.randint(0, 2 ** 32, (2,), dtype=torch.int64).tolist()
+    return (hi << 32) | lo
+
+
 class NativeTransformerExecutor:
     """
     Trainable sm_90a transformer expert (post-LN encoder layer of the reference's experiments/throughput/layers.py:22-51,
-    batch-first [B, 512, d], head_dim 64, dropout must be 0 for training — the reference's block cannot be trained at all).
+    batch-first [B, 512, d], head_dim 64, every dropout probability in [0, 1) — the reference's block cannot be trained).
 
-      forward   in_proj GEMM -> wgmma flash attention (emits the row log-sum-exp) -> out_proj GEMM (+bias +residual) ->
-                LayerNorm -> linear1 GEMM -> GELU -> linear2 GEMM (+bias +residual) -> LayerNorm
-      backward  LayerNorm backward kernels (they also produce the bias gradients of the preceding Linear), wide-tile wgmma
-                dgrad / wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel (csrc/attention_bwd.cu),
-                GELU backward (aten elementwise), one fused AMSGrad/Adam step over the flat parameter buffer
+      forward   in_proj GEMM -> wgmma flash attention (emits the row log-sum-exp; attention dropout in-kernel) -> out_proj
+                GEMM (+bias, dropout1, +residual) -> LayerNorm -> linear1 GEMM -> GELU (+dropout: csrc/dropout.cu) ->
+                linear2 GEMM (+bias, dropout2, +residual) -> LayerNorm
+      backward  LayerNorm backward kernels (they also produce the bias gradients of the preceding Linear when its dropout is
+                off), wide-tile wgmma dgrad / wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel
+                (csrc/attention_bwd.cu), GELU backward (aten elementwise, or the fused GELU + dropout backward kernel), one
+                fused AMSGrad/Adam step over the flat parameter buffer
+
+    Dropout (the reference's default layer has p = 0.1 at all four sites) applies iff ``expert.training``, like nn.Dropout.
+    Every call with dropout draws one seed (``draw_dropout_seed``); a backward call uses it for its forward recompute and
+    its backward, so a backward task re-runs the forward with a fresh mask, as the reference's ExpertBackend does.  Masks
+    are regenerated from (seed, site, position) inside the kernels (csrc/dropout.cuh) and never stored.  With dropout
+    applied to a Linear's output, the branch gradient M o dh / (1 - p) is formed by a masking kernel and its bias gradient
+    by the grouped column sum; the residual still receives dh unmasked.
 
     Like the FFN executor, module parameters and optimizer state are views of flat fp32 buffers (state_dict / checkpoints
     keep the reference key names: self_attn.in_proj_weight, linear1.weight, norm1.weight, ...).
@@ -200,8 +216,8 @@ class NativeTransformerExecutor:
         params = list(expert.parameters())
         if d // attn.num_heads != 64 or d % 256 or ff % 256 or not params[0].is_cuda or params[0].dtype != torch.float32:
             return False
-        if expert.dropout.p or expert.dropout1.p or expert.dropout2.p or attn.dropout:
-            return False   # dropout masks are not implemented in the kernels: eager PyTorch handles that configuration
+        if not all(0.0 <= p < 1.0 for p in NativeTransformerExecutor._dropout_ps(expert)):
+            return False   # p = 1 zeroes a whole branch: eager PyTorch handles that configuration
         if type(opt) is not torch.optim.Adam or len(opt.param_groups) != 1:
             return False
         g = opt.param_groups[0]
@@ -210,6 +226,18 @@ class NativeTransformerExecutor:
         if {id(p) for p in g["params"]} != {id(p) for p in params}:
             return False
         return native.have_cuda_kernels()
+
+    @staticmethod
+    def _dropout_ps(expert):
+        """drop probabilities of the kernels' sites 0-3: attention, dropout1, dropout (after GELU), dropout2"""
+        return (float(expert.self_attn.dropout), float(expert.dropout1.p), float(expert.dropout.p), float(expert.dropout2.p))
+
+    def _dropout(self):
+        """(seed, (p_attn, p_1, p_ff, p_2)) for one call, or None in eval mode / without dropout"""
+        ps = self._dropout_ps(self.expert)
+        if not self.expert.training or not any(ps):
+            return None
+        return draw_dropout_seed(), ps
 
     def __init__(self, expert, opt):
         self.expert, self.opt = expert, opt
@@ -277,52 +305,80 @@ class NativeTransformerExecutor:
             self._ws = {T: ws}
         return ws
 
-    def _forward(self, src):
+    @staticmethod
+    def _site(drop, site):
+        """kernel dropout argument of one site: (p, seed) for attention, (p, seed, site) for the others; None when off"""
+        if drop is None or not drop[1][site]:
+            return None
+        return (drop[1][site], drop[0]) if site == K.SITE_ATTN else (drop[1][site], drop[0], site)
+
+    def _forward(self, src, drop=None):
         from ..ops import gemm
         batch, seq, d = src.shape
         assert seq == 512 and d == self.d
         T = batch * seq
         ws = self._workspace(T)
         ws["x"].copy_(src.reshape(T, d))
-        x, bv, pv = ws["x"], self.bv, self.pv
+        x, bv, pv, site = ws["x"], self.bv, self.pv, self._site
         gemm.grouped_linear(x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"], two_cta=True)
-        K.attention_fwd(ws["qkv"], self.heads, out=ws["att"], lse=ws["lse"])
-        gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"], two_cta=True)
+        K.attention_fwd(ws["qkv"], self.heads, out=ws["att"], lse=ws["lse"], dropout=site(drop, K.SITE_ATTN))
+        gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"], two_cta=True,
+                            dropout=site(drop, K.SITE_OUT_PROJ))
         K.ln_relu_fwd(ws["h"], pv["g1"], pv["be1"], None, out=ws["x1"], mean=ws["stats"][0], rstd=ws["stats"][1], relu=False)
         gemm.grouped_linear(ws["x1"], bv["w1"], bias=pv["b1"], out=ws["f"], two_cta=True)       # pre-activation kept for backward
-        ws["gact"] = torch.nn.functional.gelu(ws["f"])
-        gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["x1"], out=ws["y"], two_cta=True)
+        ff = site(drop, K.SITE_FF)
+        ws["gact"] = K.gelu_dropout(ws["f"], *ff) if ff else torch.nn.functional.gelu(ws["f"])
+        gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["x1"], out=ws["y"], two_cta=True,
+                            dropout=site(drop, K.SITE_LINEAR2))
         K.ln_relu_fwd(ws["y"], pv["g2"], pv["be2"], None, out=ws["out"], mean=ws["stats"][2], rstd=ws["stats"][3], relu=False)
         return ws, T
 
     @torch.no_grad()
     def forward(self, src: torch.Tensor) -> torch.Tensor:
-        ws, T = self._forward(src)
+        ws, T = self._forward(src, self._dropout())
         return ws["out"].view(src.shape).to(src.dtype)
 
     @torch.no_grad()
     def backward(self, src: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
         from ..ops import gemm
-        ws, T = self._forward(src)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
-        d, bv, pv, gv = self.d, self.bv, self.pv, self.gv
+        drop = self._dropout()
+        ws, T = self._forward(src, drop)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
+        d, bv, pv, gv, site = self.d, self.bv, self.pv, self.gv, self._site
         go = ws["group_off"]
         bf = dict(dtype=torch.bfloat16, device=self.device)
         dout = grad_out.reshape(T, d).to(torch.bfloat16).contiguous()
+
+        def branch_grad(dres, drop_site, bias_grad):
+            """gradient of a Linear whose output went through dropout `drop_site` into a residual sum: M o dres / (1 - p)
+            and its bias gradient (without dropout the LayerNorm backward already produced the bias gradient)"""
+            s = site(drop, drop_site)
+            if s is None:
+                return dres
+            dbr = K.dropout_apply(dres, *s)
+            K.grouped_colsum(dbr, None, out=bias_grad)
+            return dbr
+
+        # with dropout at site 3 / 1 the bias gradient comes from the masked branch gradient, so the LayerNorm backward's
+        # column sum goes to a scratch row
+        scratch = torch.empty(1, d, dtype=torch.float32, device=self.device) if drop is not None else None
         dy = torch.empty(T, d, **bf)
         K.ln_relu_bwd(dout, ws["y"], ws["stats"][2], ws["stats"][3], pv["g2"], pv["be2"], None, dh=dy, dgamma=gv["g2"],
-                      dbeta=gv["be2"], dbias=gv["b2"], relu=False)
-        gemm.grouped_wgrad(dy, ws["gact"], go, 1, out=gv["w2"], two_cta=True)
-        dg = gemm.grouped_linear(dy, bv["w2"], w_is_kn=True, two_cta=True)
-        df = torch.ops.aten.gelu_backward(dg, ws["f"])
+                      dbeta=gv["be2"], dbias=scratch if site(drop, K.SITE_LINEAR2) else gv["b2"], relu=False)
+        dff = branch_grad(dy, K.SITE_LINEAR2, gv["b2"])
+        gemm.grouped_wgrad(dff, ws["gact"], go, 1, out=gv["w2"], two_cta=True)
+        dg = gemm.grouped_linear(dff, bv["w2"], w_is_kn=True, two_cta=True)
+        ff = site(drop, K.SITE_FF)
+        df = K.gelu_dropout_bwd(dg, ws["f"], *ff) if ff else torch.ops.aten.gelu_backward(dg, ws["f"])
         K.grouped_colsum(df, None, out=gv["b1"])
         gemm.grouped_wgrad(df, ws["x1"], go, 1, out=gv["w1"], two_cta=True)
         dx1 = gemm.grouped_linear(df, bv["w1"], w_is_kn=True, residual=dy, two_cta=True)
         dh = torch.empty(T, d, **bf)
         K.ln_relu_bwd(dx1, ws["h"], ws["stats"][0], ws["stats"][1], pv["g1"], pv["be1"], None, dh=dh, dgamma=gv["g1"],
-                      dbeta=gv["be1"], dbias=gv["b_out"], relu=False)
-        gemm.grouped_wgrad(dh, ws["att"], go, 1, out=gv["w_out"], two_cta=True)
-        datt = gemm.grouped_linear(dh, bv["w_out"], w_is_kn=True, two_cta=True)
-        dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads)
+                      dbeta=gv["be1"], dbias=scratch if site(drop, K.SITE_OUT_PROJ) else gv["b_out"], relu=False)
+        dhb = branch_grad(dh, K.SITE_OUT_PROJ, gv["b_out"])
+        gemm.grouped_wgrad(dhb, ws["att"], go, 1, out=gv["w_out"], two_cta=True)
+        datt = gemm.grouped_linear(dhb, bv["w_out"], w_is_kn=True, two_cta=True)
+        dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN))
         K.grouped_colsum(dqkv, None, out=gv["b_in"])
         gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"], two_cta=True)
         dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh, two_cta=True)
