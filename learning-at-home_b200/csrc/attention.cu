@@ -171,10 +171,6 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
 
 }  // namespace v2
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 }  // namespace attn
 }  // namespace lah
 
@@ -188,31 +184,16 @@ extern "C" {
 int lah_attention_fwd(const void* qkv, void* out, float* lse2, int batch, int num_heads, int d_model,
                       unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
     if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || !ptr)
-            return -100;
-        fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-    }
     CUtensorMap tm;
-    cuuint64_t dims[2] = {(cuuint64_t)3 * d_model, (cuuint64_t)batch * S_LEN};
-    cuuint64_t strides[1] = {(cuuint64_t)3 * d_model * 2};
-    cuuint32_t box[2] = {HEAD_DIM, 128};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(qkv), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return -1000 - (int)r;
-    static bool configured = false;
-    if (!configured) {
-        for (auto kern : {v2::attention_fwd_v2_kernel<false>, v2::attention_fwd_v2_kernel<true>}) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, v2::SMEM_TOTAL2);
-            if (e != cudaSuccess) return -(int)e;
-        }
-        configured = true;
+    {
+        uint64_t dims[2] = {(uint64_t)3 * d_model, (uint64_t)batch * S_LEN};
+        uint64_t str[1] = {(uint64_t)3 * d_model * 2};
+        uint32_t box[2] = {HEAD_DIM, 128};
+        int r = make_tmap(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, qkv, dims, str, box);
+        if (r) return r;
     }
+    if (int e = set_max_dynamic_smem<v2::attention_fwd_v2_kernel<false>>(v2::SMEM_TOTAL2)) return e;
+    if (int e = set_max_dynamic_smem<v2::attention_fwd_v2_kernel<true>>(v2::SMEM_TOTAL2)) return e;
     if (batch <= 0) return 0;
     const float scale_log2e = 1.4426950408889634f / sqrtf((float)HEAD_DIM);
     auto kern = drop_thr < 0 ? v2::attention_fwd_v2_kernel<false> : v2::attention_fwd_v2_kernel<true>;

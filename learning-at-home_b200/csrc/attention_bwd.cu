@@ -215,10 +215,6 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     }
 }
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 // prologue: delta[t, h] = sum_d dO[t, h, d] * O[t, h, d]  (one warp per (token, head): 64 bf16 = one 128 B row segment each)
 __global__ void __launch_bounds__(256) attn_delta_kernel(const bf16* __restrict__ dout, const bf16* __restrict__ out,
                                                          float* __restrict__ delta, long long pairs) {
@@ -273,41 +269,22 @@ int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const 
                       void* dq_part, int batch, int num_heads, int d_model, unsigned long long seed, int drop_thr,
                       float rescale, cudaStream_t st) {
     if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || !ptr)
-            return -100;
-        fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-    }
     CUtensorMap tm_qkv, tm_do;
-    cuuint32_t box[2] = {HEAD_DIM, BLK};
-    cuuint32_t estr[2] = {1, 1};
+    const uint32_t box[2] = {HEAD_DIM, BLK};
     {
-        cuuint64_t dims[2] = {(cuuint64_t)3 * d_model, (cuuint64_t)batch * S_LEN};
-        cuuint64_t strides[1] = {(cuuint64_t)3 * d_model * 2};
-        CUresult r = fn(&tm_qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(qkv), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return -1000 - (int)r;
+        uint64_t dims[2] = {(uint64_t)3 * d_model, (uint64_t)batch * S_LEN};
+        uint64_t str[1] = {(uint64_t)3 * d_model * 2};
+        int r = make_tmap(&tm_qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, qkv, dims, str, box);
+        if (r) return r;
     }
     {
-        cuuint64_t dims[2] = {(cuuint64_t)d_model, (cuuint64_t)batch * S_LEN};
-        cuuint64_t strides[1] = {(cuuint64_t)d_model * 2};
-        CUresult r = fn(&tm_do, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(dout), dims, strides, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) return -1000 - (int)r;
+        uint64_t dims[2] = {(uint64_t)d_model, (uint64_t)batch * S_LEN};
+        uint64_t str[1] = {(uint64_t)d_model * 2};
+        int r = make_tmap(&tm_do, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dout, dims, str, box);
+        if (r) return r;
     }
-    static bool configured = false;
-    if (!configured) {
-        for (auto kern : {attention_bwd_kernel<false>, attention_bwd_kernel<true>}) {
-            cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
-            if (e != cudaSuccess) return -(int)e;
-        }
-        configured = true;
-    }
+    if (int e = set_max_dynamic_smem<attention_bwd_kernel<false>>(SMEM_TOTAL)) return e;
+    if (int e = set_max_dynamic_smem<attention_bwd_kernel<true>>(SMEM_TOTAL)) return e;
     if (batch <= 0) return 0;
     const float scale = 1.f / sqrtf((float)HEAD_DIM);
     const long long tokens = (long long)batch * S_LEN, pairs = tokens * num_heads;

@@ -316,79 +316,44 @@ gemm_kernel(const typename std::conditional<DROP, GemmDropParams, GemmParams>::t
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode_fn() {
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || !ptr)
-            return nullptr;
-        fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-    }
-    return fn;
-}
-
-// bf16 tensor map, up to 3 dims (dim0 = contiguous), 128B swizzle, zero OOB fill.
-static int make_tmap_bf16(CUtensorMap* tm, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                          const uint32_t* box) {
-    PFN_encodeTiled fn = get_encode_fn();
-    if (!fn) return -100;
-    cuuint64_t gdims[3];
-    cuuint64_t gstr[2];
-    cuuint32_t gbox[3];
-    cuuint32_t estr[3] = {1, 1, 1};
-    for (int i = 0; i < rank; ++i) {
-        gdims[i] = dims[i];
-        gbox[i] = box[i];
-    }
-    for (int i = 0; i < rank - 1; ++i) gstr[i] = strides_bytes[i];
-    CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdims, gstr, gbox, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 1000;
-}
-
-static int g_num_sms = 0;
-static int num_sms() {
-    if (!g_num_sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    return g_num_sms;
-}
-
 template <int BLOCK_N, int STAGES, int MODE, bool A_MN, bool B_MN, bool OUT_F32, bool DROP = false, typename P>
 static int launch(const P& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int max_ctas, cudaStream_t st) {
     using L = SmemLayout<BLOCK_N, STAGES>;
-    auto kern = gemm_kernel<BLOCK_N, STAGES, MODE, A_MN, B_MN, OUT_F32, DROP>;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
-        if (e != cudaSuccess) return -static_cast<int>(e);
-        configured = true;
-    }
+    constexpr auto kern = gemm_kernel<BLOCK_N, STAGES, MODE, A_MN, B_MN, OUT_F32, DROP>;
+    if (const int e = set_max_dynamic_smem<kern>(L::TOTAL)) return e;
     const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
     long long total = (MODE == MODE_MGROUP) ? 1ll * p.num_m_tiles * n_tiles : 1ll * p.num_groups * (p.M / BLOCK_M) * n_tiles;
     if (total <= 0) return 0;
-    int grid = num_sms();
-    if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
-    if (total < grid) grid = static_cast<int>(total);
-    kern<<<grid, NUM_THREADS, L::TOTAL, st>>>(p, tmA, tmB);
+    kern<<<persistent_grid(total, max_ctas), NUM_THREADS, L::TOTAL, st>>>(p, tmA, tmB);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : -static_cast<int>(e);
 }
 
-static int gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
-                       long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group, const float* bias,
-                       const void* residual, long long ldr, int block_n, int max_ctas, const int* wait_flags,
-                       int wait_count, int wait_epoch, int* status, int act, const int* epoch_base, cudaStream_t stream,
-                       unsigned long long drop_seed = 0, int drop_thr = -1, float drop_scale = 1.f, int drop_site = 0) {
+}  // namespace lah
+
+using namespace lah;
+
+// ------------------------------------------------------------------------------------------------
+// C ABI (called from python via ctypes; see ops/native.py)
+// ------------------------------------------------------------------------------------------------
+extern "C" const int* lah_get_epoch_base();
+
+extern "C" {
+
+// C[rows, N] = act(A[rows, K] @ B[g]^T (+bias)) (+residual) on 128 x block_n tiles (block_n: 256, 128 or 64)
+//   b_mn == 0: B is [G, N, K] (K contiguous);  b_mn == 1: B is [G, K, N] (N contiguous)
+//   a_rows: rows of the A buffer (TMA bound); m_valid: rows of C that may be written
+//   tile_group: device int[num_m_tiles] (one entry per 128 rows) or null; out_f32: 0 => bf16 C, 1 => fp32 C
+//   act: epilogue activation after the bias: 0 none, 1 ReLU, 2 GELU (erf)
+//   drop_thr < 0: no dropout.  Otherwise dropout site drop_site (1-3) of dropout.cuh after the activation and before the
+//   residual, kept values * drop_scale = 1 / (1 - p), drop_thr in [0, 65535]; needs block_n = 256, b_mn = 0 and bf16 C
+int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
+                    long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group,
+                    const float* bias, const void* residual, long long ldr, int block_n, int max_ctas,
+                    const int* wait_flags, int wait_count, int wait_epoch, int* status, int act,
+                    unsigned long long drop_seed, int drop_thr, float drop_scale, int drop_site, cudaStream_t stream) {
     if ((K % 8) || (N % 32) || (lda % 8)) return -2;
+    if (drop_thr >= 0 && (drop_site < 1 || drop_site > 3)) return -2;
     if (drop_thr >= 0 && (block_n != 256 || b_mn || out_f32 || drop_thr > 65535)) return -4;
     if (block_n != 256 && block_n != 128 && block_n != 64) return -3;
     CUtensorMap tmA, tmB;
@@ -396,28 +361,28 @@ static int gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, 
         uint64_t dims[2] = {(uint64_t)K, (uint64_t)a_rows};
         uint64_t str[1] = {(uint64_t)lda * 2};
         uint32_t box[2] = {BLOCK_K, BLOCK_M};
-        int r = make_tmap_bf16(&tmA, A, 2, dims, str, box);
+        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, A, dims, str, box);
         if (r) return r;
     }
     if (!b_mn) {
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)G};
         uint64_t str[2] = {(uint64_t)K * 2, (uint64_t)N * K * 2};
         uint32_t box[3] = {BLOCK_K, (uint32_t)block_n, 1};
-        int r = make_tmap_bf16(&tmB, B, 3, dims, str, box);
+        int r = make_tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, B, dims, str, box);
         if (r) return r;
     } else {
         uint64_t dims[3] = {(uint64_t)N, (uint64_t)K, (uint64_t)G};
         uint64_t str[2] = {(uint64_t)N * 2, (uint64_t)N * K * 2};
         uint32_t box[3] = {64, BLOCK_K, 1};
-        int r = make_tmap_bf16(&tmB, B, 3, dims, str, box);
+        int r = make_tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, B, dims, str, box);
         if (r) return r;
     }
     GemmParams p;
     p.N = N; p.K = K; p.M = m_valid; p.num_groups = G; p.num_m_tiles = num_m_tiles; p.tile_group = tile_group;
     p.group_off = nullptr; p.C = C; p.ldc = ldc; p.c_group_stride = 0; p.bias = bias;
     p.residual = reinterpret_cast<const bf16*>(residual); p.ldr = ldr;
-    p.wait_flags = wait_flags; p.wait_count = wait_count; p.wait_epoch = wait_epoch; p.epoch_base = epoch_base; p.status = status;
-    p.act = act; p.accumulate = 0;
+    p.wait_flags = wait_flags; p.wait_count = wait_count; p.wait_epoch = wait_epoch; p.epoch_base = lah_get_epoch_base();
+    p.status = status; p.act = act; p.accumulate = 0;
     if (drop_thr >= 0) {
         GemmDropParams pd;
         static_cast<GemmParams&>(pd) = p;
@@ -436,23 +401,25 @@ static int gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, 
 #undef LAH_LAUNCH_M
 }
 
-static int gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
-                       const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n, int max_ctas,
-                       int accumulate, cudaStream_t stream) {
+// C[g][M, N] (fp32) (+)= A[off[g]:off[g+1], :M]^T @ B[off[g]:off[g+1], :N]   (A, B row-major token matrices)
+//   accumulate != 0: C += the product (gradient accumulation across steps)
+int lah_gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
+                    const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n,
+                    int max_ctas, int accumulate, cudaStream_t stream) {
     if ((M % 128) || (N % 32) || (lda % 8) || (ldb % 8)) return -2;
     CUtensorMap tmA, tmB;
     {
         uint64_t dims[2] = {(uint64_t)M, (uint64_t)total_rows};
         uint64_t str[1] = {(uint64_t)lda * 2};
         uint32_t box[2] = {64, BLOCK_K};
-        int r = make_tmap_bf16(&tmA, A, 2, dims, str, box);
+        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, A, dims, str, box);
         if (r) return r;
     }
     {
         uint64_t dims[2] = {(uint64_t)N, (uint64_t)total_rows};
         uint64_t str[1] = {(uint64_t)ldb * 2};
         uint32_t box[2] = {64, BLOCK_K};
-        int r = make_tmap_bf16(&tmB, B, 2, dims, str, box);
+        int r = make_tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, B, dims, str, box);
         if (r) return r;
     }
     GemmParams p;
@@ -464,68 +431,6 @@ static int gemm_kgroup(const void* A, long long lda, const void* B, long long ld
     if (block_n == 128) return launch<128, 6, MODE_KGROUP, true, true, true>(p, tmA, tmB, max_ctas, stream);
     if (block_n == 64) return launch<64, 8, MODE_KGROUP, true, true, true>(p, tmA, tmB, max_ctas, stream);
     return -3;
-}
-
-}  // namespace lah
-
-using namespace lah;
-
-// ------------------------------------------------------------------------------------------------
-// C ABI (called from python via ctypes; see ops/native.py)
-// ------------------------------------------------------------------------------------------------
-extern "C" const int* lah_get_epoch_base();
-
-extern "C" {
-
-// C[rows, N] = A[rows, K] @ B[g]^T (+bias) (+residual)
-//   b_mn == 0: B is [G, N, K] (K contiguous);  b_mn == 1: B is [G, K, N] (N contiguous)
-//   a_rows: rows of the A buffer (TMA bound); m_valid: rows of C that may be written
-//   tile_group: device int[num_m_tiles] or null; out_f32: 0 => bf16 C, 1 => fp32 C
-int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
-                    long long ldc, int out_f32, int m_valid, int num_m_tiles, const int* tile_group,
-                    const float* bias, const void* residual, long long ldr, int block_n, int max_ctas,
-                    const int* wait_flags, int wait_count, int wait_epoch, int* status, cudaStream_t stream) {
-    return gemm_mgroup(A, lda, a_rows, B, G, N, K, b_mn, C, ldc, out_f32, m_valid, num_m_tiles, tile_group, bias, residual,
-                       ldr, block_n, max_ctas, wait_flags, wait_count, wait_epoch, status, 0, lah_get_epoch_base(), stream);
-}
-
-// C[g][M, N] (fp32) = A[off[g]:off[g+1], :M]^T @ B[off[g]:off[g+1], :N]   (A, B row-major token matrices)
-int lah_gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
-                    const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n,
-                    int max_ctas, cudaStream_t stream) {
-    return gemm_kgroup(A, lda, B, ldb, total_rows, G, M, N, group_off, C, ldc, c_group_stride, block_n, max_ctas, 0, stream);
-}
-
-// Wide-tile entry points of the big-batch expert path (expert groups padded to 256 rows, N a multiple of 256):
-// 128 x 256 tiles with the fused epilogue activation (act: 0 none, 1 ReLU, 2 GELU) and, for the weight gradient,
-// accumulation into C across steps.  tile_group has one entry per 128 rows.
-int lah_gemm_mgroup2(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, int b_mn, void* C,
-                     long long ldc, int out_f32, int m_valid, int num_m_tiles128, const int* tile_group,
-                     const float* bias, const void* residual, long long ldr, int max_ctas, const int* wait_flags,
-                     int wait_count, int wait_epoch, int* status, int act, cudaStream_t stream) {
-    return gemm_mgroup(A, lda, a_rows, B, G, N, K, b_mn, C, ldc, out_f32, m_valid, num_m_tiles128, tile_group, bias,
-                       residual, ldr, 256, max_ctas, wait_flags, wait_count, wait_epoch, status, act, lah_get_epoch_base(),
-                       stream);
-}
-
-// lah_gemm_mgroup2 with K-major B and bf16 C, plus dropout after the bias / activation and before the residual
-// (grouped_gemm.cu DROP, dropout.cuh): kept values are multiplied by drop_scale = 1 / (1 - p), drop_thr in [0, 65535]
-int lah_gemm_mgroup2_drop(const void* A, long long lda, int a_rows, const void* B, int G, int N, int K, void* C, long long ldc,
-                          int m_valid, int num_m_tiles128, const int* tile_group, const float* bias, const void* residual,
-                          long long ldr, int max_ctas, int act, unsigned long long drop_seed, int drop_thr, float drop_scale,
-                          int drop_site, cudaStream_t stream) {
-    if (drop_thr < 0 || drop_site < 1 || drop_site > 3) return -2;
-    return gemm_mgroup(A, lda, a_rows, B, G, N, K, 0, C, ldc, 0, m_valid, num_m_tiles128, tile_group, bias, residual, ldr, 256,
-                       max_ctas, nullptr, 0, 0, nullptr, act, lah_get_epoch_base(), stream, drop_seed, drop_thr, drop_scale,
-                       drop_site);
-}
-
-int lah_gemm_kgroup2(const void* A, long long lda, const void* B, long long ldb, int total_rows, int G, int M, int N,
-                     const int* group_off, float* C, long long ldc, long long c_group_stride, int max_ctas,
-                     int accumulate, cudaStream_t stream) {
-    if (N % 256) return -2;
-    return gemm_kgroup(A, lda, B, ldb, total_rows, G, M, N, group_off, C, ldc, c_group_stride, 256, max_ctas, accumulate,
-                       stream);
 }
 
 }  // extern "C"

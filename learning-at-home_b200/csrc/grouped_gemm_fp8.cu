@@ -301,62 +301,12 @@ __global__ void __launch_bounds__(256) quant_mxfp8_kernel(const T* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------------ host
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled encode_fn() {
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || !ptr)
-            return nullptr;
-        fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-    }
-    return fn;
-}
-
-static int tmap(CUtensorMap* tm, CUtensorMapDataType dt, int elem_bytes, const void* ptr, int rank, const uint64_t* dims,
-                const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle sw) {
-    PFN_encodeTiled fn = encode_fn();
-    if (!fn) return -100;
-    cuuint64_t gdims[3];
-    cuuint64_t gstr[2];
-    cuuint32_t gbox[3];
-    cuuint32_t estr[3] = {1, 1, 1};
-    for (int i = 0; i < rank; ++i) {
-        gdims[i] = dims[i];
-        gbox[i] = box[i];
-    }
-    for (int i = 0; i < rank - 1; ++i) gstr[i] = strides_bytes[i];
-    (void)elem_bytes;
-    CUresult r = fn(tm, dt, rank, const_cast<void*>(ptr), gdims, gstr, gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 1000;
-}
-
 template <bool OUT_F32>
 static int launch_fp8(const Params& p, const CUtensorMap& tmA, const CUtensorMap& tmB, int max_ctas, cudaStream_t st) {
-    auto kern = gemm_fp8_kernel<OUT_F32>;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
-        if (e != cudaSuccess) return -static_cast<int>(e);
-        configured = true;
-    }
+    if (const int e = set_max_dynamic_smem<gemm_fp8_kernel<OUT_F32>>(SMEM_TOTAL)) return e;
     const long long total = 1ll * p.num_m_tiles * p.n_tiles;
     if (total <= 0) return 0;
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    int grid = sms;
-    if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
-    if (total < grid) grid = static_cast<int>(total);
-    kern<<<grid, NUM_THREADS, SMEM_TOTAL, st>>>(p, tmA, tmB);
+    gemm_fp8_kernel<OUT_F32><<<persistent_grid(total, max_ctas), NUM_THREADS, SMEM_TOTAL, st>>>(p, tmA, tmB);
     cudaError_t e = cudaGetLastError();
     return e == cudaSuccess ? 0 : -static_cast<int>(e);
 }
@@ -412,14 +362,14 @@ int lah_gemm_mgroup_fp8(const void* A, long long lda, int a_rows, const void* sf
         uint64_t dims[2] = {(uint64_t)K, (uint64_t)a_rows};
         uint64_t str[1] = {(uint64_t)lda};
         uint32_t box[2] = {BLOCK_K, TILE_M};
-        int r = tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, A, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, A, dims, str, box);
         if (r) return r;
     }
     {
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)N, (uint64_t)G};
         uint64_t str[2] = {(uint64_t)K, (uint64_t)N * K};
         uint32_t box[3] = {BLOCK_K, TILE_N, 1};
-        int r = tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, B, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B);
+        int r = make_tmap(&tmB, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, B, dims, str, box);
         if (r) return r;
     }
     Params p;

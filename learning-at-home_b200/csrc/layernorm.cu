@@ -377,8 +377,8 @@ static int shift_of(int tile_rows) {
 }
 
 // tile_rows: rows per tile_group entry (power of two >= 8; 128 for the padded big-batch layout, 16 for the small-M layout)
-int lah_ln_relu_fwd_t(const void* h, void* a, float* mean, float* rstd, const float* gamma, const float* beta,
-                      const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
+int lah_ln_relu_fwd(const void* h, void* a, float* mean, float* rstd, const float* gamma, const float* beta,
+                    const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
     const int tile_shift = shift_of(tile_rows);
     if (tile_shift < 0) return -2;
@@ -396,11 +396,6 @@ int lah_ln_relu_fwd_t(const void* h, void* a, float* mean, float* rstd, const fl
     LAH_LN_FWD(256) LAH_LN_FWD(512) LAH_LN_FWD(1024) LAH_LN_FWD(2048) LAH_LN_FWD(4096)
 #undef LAH_LN_FWD
     return -2;
-}
-
-int lah_ln_relu_fwd(const void* h, void* a, float* mean, float* rstd, const float* gamma, const float* beta,
-                    const int* tile_group, int rows, int C, int relu, cudaStream_t st) {
-    return lah_ln_relu_fwd_t(h, a, mean, rstd, gamma, beta, tile_group, rows, C, relu, 128, st);
 }
 
 // same + MXFP8 copy of the output (aq: e4m3 [rows, C]; sf: activation scale layout, tile_rows = 128); a may be NULL
@@ -424,9 +419,9 @@ int lah_ln_relu_fwd_q(const void* h, void* a, float* mean, float* rstd, const fl
 }
 
 // part: scratch of [ceil(rows / tile_rows), 3, C] fp32 (per-tile column sums, reduced in tile order)
-int lah_ln_relu_bwd_t(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
-                      const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
-                      const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
+int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
+                    const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
+                    const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
     if (shift_of(tile_rows) < 0) return -2;
     const int grid = (rows + tile_rows - 1) / tile_rows;
@@ -444,16 +439,9 @@ int lah_ln_relu_bwd_t(const void* da, const void* h, const float* mean, const fl
     return -2;
 }
 
-int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
-                    const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
-                    const int* tile_group, int rows, int C, int relu, cudaStream_t st) {
-    return lah_ln_relu_bwd_t(da, h, mean, rstd, gamma, beta, dh, dgamma, dbeta, dbias, part, tile_group, rows, C, relu, 128,
-                             st);
-}
-
 // part: scratch of [ceil(rows / tile_rows), C] fp32 (per-tile column sums, reduced in tile order)
-int lah_grouped_colsum_t(const void* x, long long ldx, float* out, float* part, int C, const int* tile_group, int rows,
-                         int tile_rows, cudaStream_t st) {
+int lah_grouped_colsum(const void* x, long long ldx, float* out, float* part, int C, const int* tile_group, int rows,
+                       int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
     if (C % 256 || shift_of(tile_rows) < 0) return -2;
     const int tiles = (rows + tile_rows - 1) / tile_rows;
@@ -461,11 +449,6 @@ int lah_grouped_colsum_t(const void* x, long long ldx, float* out, float* part, 
     grouped_colsum_kernel<<<grid, 512, 0, st>>>((const bf16*)x, ldx, part, C, tile_group, rows, tile_rows);
     group_tile_sum_kernel<<<(C + 255) / 256, 256, 0, st>>>(part, tiles, 1, C, tile_group, out, nullptr, nullptr);
     return -(int)cudaGetLastError();
-}
-
-int lah_grouped_colsum(const void* x, long long ldx, float* out, float* part, int C, const int* tile_group, int rows,
-                       cudaStream_t st) {
-    return lah_grouped_colsum_t(x, ldx, out, part, C, tile_group, rows, 128, st);
 }
 
 }  // extern "C"

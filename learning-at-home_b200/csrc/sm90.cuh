@@ -1,5 +1,6 @@
 // sm90.cuh — thin inline-PTX layer for Hopper (sm_90a): mbarrier, TMA, wgmma, descriptors,
-// system-scope acquire/release used by the peer-to-peer (NVLink) kernels.
+// system-scope acquire/release used by the peer-to-peer (NVLink) kernels; and the host-side tensor-map / launch helpers
+// shared by the TMA kernel files.
 //
 // Everything here is written for sm_90a only (no fallbacks, no multi-arch dispatch).
 #pragma once
@@ -299,6 +300,69 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
+}
+
+// ----------------------------------------------------------------------------------------------
+// host side: tensor maps and launch geometry of the TMA kernels
+// ----------------------------------------------------------------------------------------------
+// Tiled tensor map over `rank` (<= 3) dims, dim 0 contiguous, zero OOB fill.  Returns 0, -100 when the driver has no
+// cuTensorMapEncodeTiled, or -1000 - CUresult when the encode fails.
+inline int make_tmap(CUtensorMap* tm, CUtensorMapDataType dtype, int rank, const void* ptr, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box,
+                     CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
+    typedef CUresult (*EncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    static const EncodeTiled encode = [] {
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess) fn = nullptr;
+        return reinterpret_cast<EncodeTiled>(fn);
+    }();
+    if (!encode) return -100;
+    cuuint64_t gdims[3], gstr[2];
+    cuuint32_t gbox[3], estr[3] = {1, 1, 1};
+    for (int i = 0; i < rank; ++i) {
+        gdims[i] = dims[i];
+        gbox[i] = box[i];
+    }
+    for (int i = 0; i < rank - 1; ++i) gstr[i] = strides_bytes[i];
+    const CUresult r = encode(tm, dtype, rank, const_cast<void*>(ptr), gdims, gstr, gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                              swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS ? 0 : -1000 - static_cast<int>(r);
+}
+
+// SM count of the device current at the first call
+inline int num_sms() {
+    static const int sms = [] {
+        int dev = 0, n = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+        return n;
+    }();
+    return sms;
+}
+
+// grid of a persistent kernel: one CTA per SM, capped by max_ctas (> 0) and by the number of tiles
+inline int persistent_grid(long long total_tiles, int max_ctas) {
+    int grid = num_sms();
+    if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
+    if (total_tiles < grid) grid = static_cast<int>(total_tiles);
+    return grid;
+}
+
+// Raises Kernel's dynamic shared-memory limit to `bytes` on its first call; a launch above 48 KB fails without it.  The
+// kernel itself is the template argument because all instantiations of a kernel template share one function type, and
+// each of them needs its own attribute.  Returns 0 or -cudaError_t.
+template <auto Kernel>
+inline int set_max_dynamic_smem(int bytes) {
+    static bool done = false;
+    if (!done) {
+        const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+        if (e != cudaSuccess) return -static_cast<int>(e);
+        done = true;
+    }
+    return 0;
 }
 
 }  // namespace lah

@@ -33,51 +33,6 @@ constexpr int MMA_K = 16;
 constexpr int BN_MAX = 128;  // max tokens per MMA (swapab) / X features per tile (wgrad)
 constexpr int NUM_THREADS = 288;   // two consumer warpgroups + one producer warp
 
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled encode_fn() {
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess || !ptr)
-            return nullptr;
-        fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-    }
-    return fn;
-}
-
-static int make_tmap(CUtensorMap* tm, CUtensorMapDataType dt, int esize, const void* ptr, int rank, const uint64_t* dims,
-                     const uint64_t* strides_bytes, const uint32_t* box) {
-    PFN_encodeTiled fn = encode_fn();
-    if (!fn) return -100;
-    cuuint64_t gdims[3];
-    cuuint64_t gstr[2];
-    cuuint32_t gbox[3];
-    cuuint32_t estr[3] = {1, 1, 1};
-    for (int i = 0; i < rank; ++i) {
-        gdims[i] = dims[i];
-        gbox[i] = box[i];
-    }
-    for (int i = 0; i < rank - 1; ++i) gstr[i] = strides_bytes[i];
-    (void)esize;
-    CUresult r = fn(tm, dt, rank, const_cast<void*>(ptr), gdims, gstr, gbox, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 1000;
-}
-
-static int num_sms() {
-    static int sms = 0;
-    if (!sms) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    }
-    return sms;
-}
-
 // =====================================================================================================================
 // swap-AB grouped linear
 // =====================================================================================================================
@@ -653,13 +608,13 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
         uint64_t dims[3] = {(uint64_t)K, (uint64_t)M_out, (uint64_t)G};
         uint64_t str[2] = {(uint64_t)K * 2, (uint64_t)M_out * K * 2};
         uint32_t box[3] = {BK, BM, 1};
-        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, W, 3, dims, str, box);
+        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, W, dims, str, box);
         if (r) return r;
     } else {
         uint64_t dims[3] = {(uint64_t)M_out, (uint64_t)K, (uint64_t)G};
         uint64_t str[2] = {(uint64_t)M_out * 2, (uint64_t)M_out * K * 2};
         uint32_t box[3] = {64, BK, 1};
-        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, W, 3, dims, str, box);
+        int r = make_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, W, dims, str, box);
         if (r) return r;
     }
     const uint32_t boxes[4] = {16, 32, 64, 128};
@@ -667,7 +622,7 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
         uint64_t dims[2] = {(uint64_t)K, (uint64_t)x_rows};
         uint64_t str[1] = {(uint64_t)ldx * 2};
         uint32_t box[2] = {BK, boxes[i]};
-        int r = make_tmap(&tmB[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, 2, dims, str, box);
+        int r = make_tmap(&tmB[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, dims, str, box);
         if (r) return r;
     }
     sab::Params p;
@@ -681,23 +636,12 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
     const long long total = 1ll * (M_out / BM) * (G + x_rows / BN_MAX);
     if (total <= 0 || G <= 0) return 0;
     if (cudaMemsetAsync(p.tile_counter, 0, sizeof(int), st) != cudaSuccess) return -4;
-    int ctas = num_sms();
-    if (max_ctas > 0 && max_ctas < ctas) ctas = max_ctas;
-    if (total < ctas) ctas = static_cast<int>(total);
-    static bool configured[2] = {false, false};
+    const int ctas = persistent_grid(total, max_ctas);
     if (!a_mn) {
-        if (!configured[0]) {
-            cudaError_t e = cudaFuncSetAttribute(sab::swapab_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, sab::SMEM_TOTAL);
-            if (e != cudaSuccess) return -(int)e;
-            configured[0] = true;
-        }
+        if (int e = set_max_dynamic_smem<sab::swapab_kernel<false>>(sab::SMEM_TOTAL)) return e;
         sab::swapab_kernel<false><<<ctas, NUM_THREADS, sab::SMEM_TOTAL, st>>>(p, tmA, tmB[0], tmB[1], tmB[2], tmB[3]);
     } else {
-        if (!configured[1]) {
-            cudaError_t e = cudaFuncSetAttribute(sab::swapab_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, sab::SMEM_TOTAL);
-            if (e != cudaSuccess) return -(int)e;
-            configured[1] = true;
-        }
+        if (int e = set_max_dynamic_smem<sab::swapab_kernel<true>>(sab::SMEM_TOTAL)) return e;
         sab::swapab_kernel<true><<<ctas, NUM_THREADS, sab::SMEM_TOTAL, st>>>(p, tmA, tmB[0], tmB[1], tmB[2], tmB[3]);
     }
     return -(int)cudaGetLastError();
@@ -717,7 +661,7 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
         uint64_t str[1] = {(uint64_t)K * 4};
         uint32_t box[2] = {wa::CH_COLS, BM};
         for (int a = 0; a < 4; ++a) {
-            int r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, arrs[a], 2, dims, str, box);
+            int r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, arrs[a], dims, str, box);
             if (r) return r;
         }
     }
@@ -725,14 +669,14 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
         uint64_t dims[2] = {(uint64_t)N, (uint64_t)total_rows};
         uint64_t str[1] = {(uint64_t)lddy * 2};
         uint32_t box[2] = {64, wa::WBK};
-        int r = make_tmap(&tmDY, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dy, 2, dims, str, box);
+        int r = make_tmap(&tmDY, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dy, dims, str, box);
         if (r) return r;
     }
     {
         uint64_t dims[2] = {(uint64_t)K, (uint64_t)total_rows};
         uint64_t str[1] = {(uint64_t)ldx * 2};
         uint32_t box[2] = {64, wa::WBK};
-        int r = make_tmap(&tmX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, 2, dims, str, box);
+        int r = make_tmap(&tmX, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, x, dims, str, box);
         if (r) return r;
     }
     wa::Params a;
@@ -744,16 +688,8 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
     const long long total = 1ll * G * (N / BM) * (K / BN_MAX);
     if (total <= 0) return 0;
     if (cudaMemsetAsync(a.tile_counter, 0, sizeof(int), st) != cudaSuccess) return -4;
-    int ctas = num_sms();
-    if (max_ctas > 0 && max_ctas < ctas) ctas = max_ctas;
-    if (total < ctas) ctas = (int)total;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(wa::wgrad_adam_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wa::SMEM_TOTAL);
-        if (e != cudaSuccess) return -(int)e;
-        configured = true;
-    }
-    wa::wgrad_adam_kernel<<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
+    if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel>(wa::SMEM_TOTAL)) return e;
+    wa::wgrad_adam_kernel<<<persistent_grid(total, max_ctas), NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
     return -(int)cudaGetLastError();
 }
 

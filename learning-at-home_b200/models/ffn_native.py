@@ -63,9 +63,9 @@ class NativeFFNLayer(nn.Module):
             fp8.grouped_linear_fp8(ws["aq"], self.w[2], bias=self.b[2], residual=x, out=out)
         else:
             mean = rstd = ws.setdefault("stat", torch.empty(rows, device=x.device))
-            gemm.grouped_linear(x, self.w[0], bias=self.b[0], out=ws["h"], two_cta=True)
+            gemm.grouped_linear(x, self.w[0], bias=self.b[0], out=ws["h"])
             K.ln_relu_fwd(ws["h"], g1, be1, None, out=ws["a"], mean=mean, rstd=rstd)
-            gemm.grouped_linear(ws["a"], self.w[1], bias=self.b[1], out=ws["h"], two_cta=True)
+            gemm.grouped_linear(ws["a"], self.w[1], bias=self.b[1], out=ws["h"])
             K.ln_relu_fwd(ws["h"], g2, be2, None, out=ws["a"], mean=mean, rstd=rstd)
-            gemm.grouped_linear(ws["a"], self.w[2], bias=self.b[2], residual=x, out=out, two_cta=True)
+            gemm.grouped_linear(ws["a"], self.w[2], bias=self.b[2], residual=x, out=out)
         return out

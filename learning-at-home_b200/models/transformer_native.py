@@ -1,6 +1,6 @@
 """
 sm_90a execution of the transformer expert (post-LN encoder layer, GELU; architecture of
-the reference's experiments/throughput/layers.py:22-51): QKV / out / MLP projections on the wide-tile wgmma GEMM with
+the reference's experiments/throughput/layers.py:22-51): QKV / out / MLP projections on the 128 x 256-tile wgmma GEMM with
 fused bias / GELU / residual epilogues, attention on csrc/attention.cu (S and P never leave the SM), LayerNorm on
 csrc/layernorm.cu.  Forward (inference / throughput experiment) only; training of transformer experts goes through the
 PyTorch module (``TransformerEncoderLayer`` + ``ExpertBackend``), which — unlike the reference's — is trainable.
@@ -55,12 +55,12 @@ class NativeTransformerLayer(nn.Module):
         if x.dtype != torch.bfloat16 or not x.is_contiguous():
             x = x.to(torch.bfloat16).contiguous()
         ws = self._workspace(batch * seq, x.device)
-        gemm.grouped_linear(x, self.w_in, bias=self.b_in, out=ws["qkv"], two_cta=True)
+        gemm.grouped_linear(x, self.w_in, bias=self.b_in, out=ws["qkv"])
         K.attention_fwd(ws["qkv"], self.num_heads, out=ws["att"])
-        gemm.grouped_linear(ws["att"], self.w_out, bias=self.b_out, residual=x, out=ws["h"], two_cta=True)
+        gemm.grouped_linear(ws["att"], self.w_out, bias=self.b_out, residual=x, out=ws["h"])
         K.ln_relu_fwd(ws["h"], self.g1, self.be1, None, out=ws["x1"], mean=ws["mean"], rstd=ws["rstd"], relu=False)
-        gemm.grouped_linear(ws["x1"], self.w1, bias=self.b1, out=ws["f"], two_cta=True, act=2)
-        gemm.grouped_linear(ws["f"], self.w2, bias=self.b2, residual=ws["x1"], out=ws["y"], two_cta=True)
+        gemm.grouped_linear(ws["x1"], self.w1, bias=self.b1, out=ws["f"], act=2)
+        gemm.grouped_linear(ws["f"], self.w2, bias=self.b2, residual=ws["x1"], out=ws["y"])
         out = torch.empty(batch * seq, d, dtype=torch.bfloat16, device=x.device) if out is None else out.view(batch * seq, d)
         K.ln_relu_fwd(ws["y"], self.g2, self.be2, None, out=out, mean=ws["mean"], rstd=ws["rstd"], relu=False)
         return out.view(batch, seq, d)

@@ -15,6 +15,7 @@ import ctypes
 import torch
 
 from . import native
+from .kernels import _dropout_args
 from .native import c_void_p, c_int, c_ll, ptr, stream_ptr
 
 TILE_M = 128
@@ -28,21 +29,10 @@ def _lib():
         lib.lah_gemm_mgroup.restype = c_int
         lib.lah_gemm_mgroup.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_ll,
                                         c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p, c_int, c_int,
-                                        c_void_p, c_void_p]
+                                        c_void_p, c_int, ctypes.c_ulonglong, c_int, ctypes.c_float, c_int, c_void_p]
         lib.lah_gemm_kgroup.restype = c_int
         lib.lah_gemm_kgroup.argtypes = [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p,
-                                        c_void_p, c_ll, c_ll, c_int, c_int, c_void_p]
-        lib.lah_gemm_mgroup2.restype = c_int
-        lib.lah_gemm_mgroup2.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_ll,
-                                         c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_void_p,
-                                         c_int, c_void_p]
-        lib.lah_gemm_mgroup2_drop.restype = c_int
-        lib.lah_gemm_mgroup2_drop.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_ll, c_int, c_int,
-                                              c_void_p, c_void_p, c_void_p, c_ll, c_int, c_int, ctypes.c_ulonglong, c_int,
-                                              ctypes.c_float, c_int, c_void_p]
-        lib.lah_gemm_kgroup2.restype = c_int
-        lib.lah_gemm_kgroup2.argtypes = [c_void_p, c_ll, c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p,
-                                         c_void_p, c_ll, c_ll, c_int, c_int, c_void_p]
+                                        c_void_p, c_ll, c_ll, c_int, c_int, c_int, c_void_p]
         _configured = True
     return lib
 
@@ -56,20 +46,20 @@ def _pick_block_n(n: int) -> int:
 
 
 def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=False, out=None,
-                   out_dtype=torch.bfloat16, m_valid=None, block_n=None, max_ctas=0, two_cta=False, wait=None, act=0,
-                   dropout=None):
+                   out_dtype=torch.bfloat16, m_valid=None, block_n=None, max_ctas=0, wait=None, act=0, dropout=None):
     """
-    out[r, :] = a[r, :] @ W[g(r)]^T (+ bias[g(r)]) (+ residual[r, :])
+    out[r, :] = act(a[r, :] @ W[g(r)]^T (+ bias[g(r)])) (+ residual[r, :])   on 128 x block_n tiles
 
     :param a: [rows, K] bf16, rows grouped by expert & padded to 128 (see module docstring)
     :param w: [G, N, K] bf16 (w_is_kn=False, y = x W^T)   or   [G, K, N] bf16 (w_is_kn=True, y = x W: dgrad)
     :param tile_group: int32 [ceil(rows/128)] expert of every 128-row tile (-1 skips the tile); None => expert 0
     :param bias: fp32 [G, N] or None;  residual: bf16 [rows, N] or None
-    :param act: activation fused after the bias (wide-tile kernel only): 0 none, 1 ReLU, 2 GELU(erf)
+    :param block_n: tile width 256, 128 or 64; None picks it from N (256 whenever N is a multiple of 256)
+    :param act: activation fused after the bias: 0 none, 1 ReLU, 2 GELU(erf)
     :param wait: (flags int32 tensor [count], epoch, status tensor) — receive-side fusion: the kernel's TMA producer
         polls the peers' dispatch flags (ld.acquire.sys) before its first load instead of a separate wait kernel
     :param dropout: (p, seed, site): out = M o act(a W^T + bias) / (1 - p) (+ residual), M the (row, column) mask of
-        ``kernels.dropout_mask`` site 1-3; wide-tile kernel, y = x W^T, bf16 output.  p = 0 or None: no dropout
+        ``kernels.dropout_mask`` site 1-3; needs 128 x 256 tiles, y = x W^T, bf16 output.  p = 0 or None: no dropout
     """
     wait_flags, wait_count, wait_epoch, wait_status = (wait[0], wait[0].numel(), wait[1], wait[2]) if wait else (None, 0, 0, None)
     assert a.is_cuda and a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and a.dim() == 2 and w.dim() == 3
@@ -92,43 +82,28 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
         assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == G * N
     if residual is not None:
         assert residual.dtype == torch.bfloat16 and residual.stride(1) == 1
-    if dropout is not None and dropout[0] > 0:
-        from .kernels import _dropout_args
-        assert two_cta and N % 256 == 0 and not w_is_kn and out.dtype == torch.bfloat16 and wait is None
-        seed, thr, scale = _dropout_args(dropout[:2])
-        code = _lib().lah_gemm_mgroup2_drop(
-            ptr(a), a.stride(0), rows, ptr(w), G, N, K, ptr(out), out.stride(0), rows if m_valid is None else m_valid,
-            num_m_tiles, ptr(tile_group), ptr(bias), ptr(residual), residual.stride(0) if residual is not None else 0,
-            max_ctas, int(act), seed, thr, scale, int(dropout[2]), stream_ptr())
-        native.check(code, "lah_gemm_mgroup2_drop")
-        native.count_launch()
-        return out
-    if two_cta and N % 256 == 0:
-        # wide-tile kernel (128x256 tiles): expert groups must be padded to 256 rows
-        code = _lib().lah_gemm_mgroup2(
-            ptr(a), a.stride(0), rows, ptr(w), G, N, K, int(w_is_kn), ptr(out), out.stride(0),
-            int(out.dtype == torch.float32), rows if m_valid is None else m_valid, num_m_tiles, ptr(tile_group),
-            ptr(bias), ptr(residual), residual.stride(0) if residual is not None else 0, max_ctas, ptr(wait_flags),
-            wait_count, wait_epoch, ptr(wait_status), int(act), stream_ptr())
-        native.check(code, "lah_gemm_mgroup2")
-        native.count_launch()
-        return out
-    assert act == 0, "epilogue activations are implemented in the wide-tile kernel (two_cta=True, N % 256 == 0)"
     bn = block_n or _pick_block_n(N)
+    seed, thr, scale = _dropout_args(dropout)
+    site = 0
+    if thr >= 0:
+        assert bn == 256 and not w_is_kn and out.dtype == torch.bfloat16 and wait is None, \
+            "the dropout epilogue needs 128 x 256 tiles, y = x W^T and a bf16 output"
+        site = int(dropout[2])
     code = _lib().lah_gemm_mgroup(
         ptr(a), a.stride(0), rows, ptr(w), G, N, K, int(w_is_kn), ptr(out), out.stride(0),
         int(out.dtype == torch.float32), rows if m_valid is None else m_valid, num_m_tiles, ptr(tile_group),
         ptr(bias), ptr(residual), residual.stride(0) if residual is not None else 0, bn, max_ctas, ptr(wait_flags),
-        wait_count, wait_epoch, ptr(wait_status), stream_ptr())
+        wait_count, wait_epoch, ptr(wait_status), int(act), seed, thr, scale, site, stream_ptr())
     native.check(code, "lah_gemm_mgroup")
     native.count_launch()
     return out
 
 
-def grouped_wgrad(dy, x, group_off, num_groups, *, out=None, block_n=None, max_ctas=0, two_cta=False, accumulate=False):
+def grouped_wgrad(dy, x, group_off, num_groups, *, out=None, block_n=None, max_ctas=0, accumulate=False):
     """
-    out[g] = dy[off[g]:off[g+1]]^T @ x[off[g]:off[g+1]]   (fp32 [G, M, N]); groups with no rows are left untouched.
+    out[g] (+)= dy[off[g]:off[g+1]]^T @ x[off[g]:off[g+1]]   (fp32 [G, M, N]); groups with no rows are left untouched.
     The reduction over an expert's rows IS the gradient reduction over all trainers that routed tokens to it.
+    :param accumulate: add to ``out`` instead of overwriting it (gradient accumulation across steps)
     """
     assert dy.is_cuda and dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16
     assert dy.stride(1) == 1 and x.stride(1) == 1 and dy.shape[0] == x.shape[0]
@@ -138,16 +113,9 @@ def grouped_wgrad(dy, x, group_off, num_groups, *, out=None, block_n=None, max_c
     if out is None:
         out = torch.zeros(num_groups, M, N, device=dy.device, dtype=torch.float32)
     assert out.dtype == torch.float32 and out.is_contiguous()
-    if two_cta and M % 256 == 0 and N % 256 == 0:
-        code = _lib().lah_gemm_kgroup2(ptr(dy), dy.stride(0), ptr(x), x.stride(0), rows, num_groups, M, N,
-                                       ptr(group_off), ptr(out), N, M * N, max_ctas, int(accumulate), stream_ptr())
-        native.check(code, "lah_gemm_kgroup2")
-        native.count_launch()
-        return out
-    assert not accumulate, "gradient accumulation is implemented in the wide-tile kernel (two_cta=True)"
     bn = block_n or _pick_block_n(N)
     code = _lib().lah_gemm_kgroup(ptr(dy), dy.stride(0), ptr(x), x.stride(0), rows, num_groups, M, N, ptr(group_off),
-                                  ptr(out), N, M * N, bn, max_ctas, stream_ptr())
+                                  ptr(out), N, M * N, bn, max_ctas, int(accumulate), stream_ptr())
     native.check(code, "lah_gemm_kgroup")
     native.count_launch()
     return out

@@ -27,10 +27,9 @@ def _lib():
         return lib
     P, I, L, Fl = c_void_p, c_int, c_ll, c_float
     sigs = {
-        "lah_ln_relu_fwd": [P, P, P, P, P, P, P, I, I, I, P],
-        "lah_ln_relu_fwd_t": [P, P, P, P, P, P, P, I, I, I, I, P],
-        "lah_ln_relu_bwd_t": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
-        "lah_grouped_colsum_t": [P, L, P, P, I, P, I, I, P],
+        "lah_ln_relu_fwd": [P, P, P, P, P, P, P, I, I, I, I, P],
+        "lah_ln_relu_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
+        "lah_grouped_colsum": [P, L, P, P, I, P, I, I, P],
         "lah_set_step_counters": [P],
         "lah_set_multicast": [c_ull],
         "lah_set_poison_word": [P],
@@ -42,8 +41,6 @@ def _lib():
         "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, P, I, P],
         "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, I, P],
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
-        "lah_ln_relu_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, P],
-        "lah_grouped_colsum": [P, L, P, P, I, P, I, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
         "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P],
@@ -94,8 +91,8 @@ def ln_relu_fwd(h, gamma, beta, tile_group, *, out, mean, rstd, relu=True, quant
                                               ptr(tile_group), rows, C, int(relu), ptr(quant.q), ptr(quant.sf),
                                               stream_ptr()), "lah_ln_relu_fwd_q")
     else:
-        native.check(_lib().lah_ln_relu_fwd_t(ptr(h), ptr(out), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta),
-                                              ptr(tile_group), rows, C, int(relu), int(tile_rows), stream_ptr()),
+        native.check(_lib().lah_ln_relu_fwd(ptr(h), ptr(out), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta),
+                                            ptr(tile_group), rows, C, int(relu), int(tile_rows), stream_ptr()),
                      "lah_ln_relu_fwd")
     native.count_launch()
     return out
@@ -106,9 +103,9 @@ def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta
     rows, C = h.shape
     assert da.is_contiguous() and h.is_contiguous() and dh.is_contiguous()
     part = torch.empty((rows + tile_rows - 1) // tile_rows, 3, C, device=h.device, dtype=torch.float32)
-    native.check(_lib().lah_ln_relu_bwd_t(ptr(da), ptr(h), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(dh),
-                                          ptr(dgamma), ptr(dbeta), ptr(dbias), ptr(part), ptr(tile_group), rows, C,
-                                          int(relu), int(tile_rows), stream_ptr()), "lah_ln_relu_bwd")
+    native.check(_lib().lah_ln_relu_bwd(ptr(da), ptr(h), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(dh),
+                                        ptr(dgamma), ptr(dbeta), ptr(dbias), ptr(part), ptr(tile_group), rows, C,
+                                        int(relu), int(tile_rows), stream_ptr()), "lah_ln_relu_bwd")
     native.count_launch(2)
     return dh
 
@@ -117,8 +114,8 @@ def grouped_colsum(x, tile_group, *, out, tile_rows=128):
     """out[g] += the column sums of group g's rows, summed in a fixed order (run-to-run identical)"""
     rows, C = x.shape
     part = torch.empty((rows + tile_rows - 1) // tile_rows, C, device=x.device, dtype=torch.float32)
-    native.check(_lib().lah_grouped_colsum_t(ptr(x), x.stride(0), ptr(out), ptr(part), C, ptr(tile_group), rows,
-                                             int(tile_rows), stream_ptr()), "lah_grouped_colsum")
+    native.check(_lib().lah_grouped_colsum(ptr(x), x.stride(0), ptr(out), ptr(part), C, ptr(tile_group), rows,
+                                           int(tile_rows), stream_ptr()), "lah_grouped_colsum")
     native.count_launch(2)
     return out
 

@@ -52,7 +52,6 @@ class DMoEConfig:
     amsgrad: bool = True
     seed: int = 1337
     uid_prefix: str = "expert"
-    two_cta: bool = True                 # wide 128x256 GEMM tiles with fused activation; expert groups padded to 256 rows
     # gate of the fused layer:
     #   "product_key": lib.GatingFunction semantics — trainable proj = Linear(hidden, sum(grid)), score = sum of per-dim logits
     #   "emulator":    EmulatedDMoE semantics (dmoe_emulator.py:47) — logits = LayerNorm(x) @ F.normalize(expert_keys, -1);
@@ -166,17 +165,14 @@ class EngineContext:
         self.E_loc = self.E // self.world
         pairs = cfg.tokens_per_rank * cfg.k
         cap = pairs if self.world == 1 else int(math.ceil(pairs * cfg.capacity_factor))
-        import os
         self.small = cfg.resolved_path(self.world) == "small"
         if self.small:
             # weight-streaming regime: hot-expert replicas would move 12.6 MB of weights to save a few rows -> static placement
-            self.two_cta = False
             self.align = self.tile_rows = 16
             self.S = 0
         else:
-            self.two_cta = cfg.two_cta and os.environ.get("LAH_TWO_CTA", "1") != "0" and cfg.inner % 256 == 0 \
-                and cfg.hidden % 256 == 0
-            self.align = 256 if self.two_cta else 128   # expert groups are padded to this many rows
+            # expert groups are padded to this many rows: 256 when every GEMM of the expert runs on 128 x 256 tiles
+            self.align = 256 if cfg.hidden % 256 == 0 and cfg.inner % 256 == 0 else 128
             self.tile_rows = 128
             self.S = min(int(cfg.shadow_experts), 2 * K.MAX_WORLD) if self.world > 1 else 0   # shadow slots per rank / layer
         self.G_tot = self.E_loc + self.S
@@ -682,13 +678,11 @@ class FusedDMoE(nn.Module):
         elif cfg.expert_dtype == "fp8":
             self._expert_ffn_fp8(wait, epoch)
         else:
-            gemm.grouped_linear(ws.xd, sh.bf16["w1"], tile_group=tg, bias=sh.views["b1"], out=ws.h1, two_cta=c.two_cta,
-                                wait=wait)
+            gemm.grouped_linear(ws.xd, sh.bf16["w1"], tile_group=tg, bias=sh.views["b1"], out=ws.h1, wait=wait)
             K.ln_relu_fwd(ws.h1, sh.views["g1"], sh.views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1)
-            gemm.grouped_linear(ws.a1, sh.bf16["w2"], tile_group=tg, bias=sh.views["b2"], out=ws.h2, two_cta=c.two_cta)
+            gemm.grouped_linear(ws.a1, sh.bf16["w2"], tile_group=tg, bias=sh.views["b2"], out=ws.h2)
             K.ln_relu_fwd(ws.h2, sh.views["g2"], sh.views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2)
-            gemm.grouped_linear(ws.a2, sh.bf16["w3"], tile_group=tg, bias=sh.views["b3"], residual=ws.xd, out=ws.yo,
-                                two_cta=c.two_cta)
+            gemm.grouped_linear(ws.a2, sh.bf16["w3"], tile_group=tg, bias=sh.views["b3"], residual=ws.xd, out=ws.yo)
         c.timer.mark("expert_ffn_fwd")
         y = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=x.device)
         K.combine_rows(ws.yo_off, idx, pair_row, w, y, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_OUTPUT, epoch=epoch,
@@ -700,7 +694,7 @@ class FusedDMoE(nn.Module):
         """forward GEMMs on block-scaled FP8 tensor cores; LayerNorm emits the next GEMM's MXFP8 operand directly (and the
         bf16 copy the bf16 wgrad needs)"""
         c, ws, sh = self.ctx, self.ws, self.shard
-        assert c.two_cta, "the FP8 path needs the 256-row expert groups of the wide-tile layout (hidden and 4*hidden multiples of 256)"
+        assert c.align == 256, "the FP8 path needs 256-row expert groups (hidden and 4*hidden multiples of 256)"
         tg = ws.tile_group
         if wait is not None:  # the quantiser is the first consumer of the rows pushed by the peers
             K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
@@ -740,17 +734,16 @@ class FusedDMoE(nn.Module):
             c.timer.mark("bwd_combine")
             return dx, dlogits
         K.grouped_colsum(c.gyd, tg, out=gr["b3"])
-        gemm.grouped_wgrad(c.gyd, ws.a2, go, G, out=gr["w3"], two_cta=c.two_cta, accumulate=cfg.accumulate)
-        gemm.grouped_linear(c.gyd, sh.bf16["w3"], tile_group=tg, w_is_kn=True, out=c.da, two_cta=c.two_cta)
+        gemm.grouped_wgrad(c.gyd, ws.a2, go, G, out=gr["w3"], accumulate=cfg.accumulate)
+        gemm.grouped_linear(c.gyd, sh.bf16["w3"], tile_group=tg, w_is_kn=True, out=c.da)
         K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=c.dh, dgamma=gr["g2"],
                       dbeta=gr["be2"], dbias=gr["b2"])
-        gemm.grouped_wgrad(c.dh, ws.a1, go, G, out=gr["w2"], two_cta=c.two_cta, accumulate=cfg.accumulate)
-        gemm.grouped_linear(c.dh, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da, two_cta=c.two_cta)
+        gemm.grouped_wgrad(c.dh, ws.a1, go, G, out=gr["w2"], accumulate=cfg.accumulate)
+        gemm.grouped_linear(c.dh, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
         K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=c.dh, dgamma=gr["g1"],
                       dbeta=gr["be1"], dbias=gr["b1"])
-        gemm.grouped_wgrad(c.dh, ws.xd, go, G, out=gr["w1"], two_cta=c.two_cta, accumulate=cfg.accumulate)
-        gemm.grouped_linear(c.dh, sh.bf16["w1"], tile_group=tg, w_is_kn=True, residual=c.gyd, out=c.dxd,
-                            two_cta=c.two_cta)
+        gemm.grouped_wgrad(c.dh, ws.xd, go, G, out=gr["w1"], accumulate=cfg.accumulate)
+        gemm.grouped_linear(c.dh, sh.bf16["w1"], tile_group=tg, w_is_kn=True, residual=c.gyd, out=c.dxd)
         c.timer.mark("expert_ffn_bwd(wgrad+dgrad+ln)")
         # ---- expert-side optimizer step (reference: ExpertBackend.apply_gradients right after backward)
         if c.S:  # the owners read every rank's partial gradients of the shadowed experts: all ranks must be done

@@ -189,7 +189,7 @@ class NativeTransformerExecutor:
                 GEMM (+bias, dropout1, +residual) -> LayerNorm -> linear1 GEMM -> GELU (+dropout: csrc/dropout.cu) ->
                 linear2 GEMM (+bias, dropout2, +residual) -> LayerNorm
       backward  LayerNorm backward kernels (they also produce the bias gradients of the preceding Linear when its dropout is
-                off), wide-tile wgmma dgrad / wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel
+                off), 128 x 256-tile wgmma dgrad / wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel
                 (csrc/attention_bwd.cu), GELU backward (aten elementwise, or the fused GELU + dropout backward kernel), one
                 fused AMSGrad/Adam step over the flat parameter buffer
 
@@ -320,15 +320,15 @@ class NativeTransformerExecutor:
         ws = self._workspace(T)
         ws["x"].copy_(src.reshape(T, d))
         x, bv, pv, site = ws["x"], self.bv, self.pv, self._site
-        gemm.grouped_linear(x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"], two_cta=True)
+        gemm.grouped_linear(x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
         K.attention_fwd(ws["qkv"], self.heads, out=ws["att"], lse=ws["lse"], dropout=site(drop, K.SITE_ATTN))
-        gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"], two_cta=True,
+        gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"],
                             dropout=site(drop, K.SITE_OUT_PROJ))
         K.ln_relu_fwd(ws["h"], pv["g1"], pv["be1"], None, out=ws["x1"], mean=ws["stats"][0], rstd=ws["stats"][1], relu=False)
-        gemm.grouped_linear(ws["x1"], bv["w1"], bias=pv["b1"], out=ws["f"], two_cta=True)       # pre-activation kept for backward
+        gemm.grouped_linear(ws["x1"], bv["w1"], bias=pv["b1"], out=ws["f"])       # pre-activation kept for backward
         ff = site(drop, K.SITE_FF)
         ws["gact"] = K.gelu_dropout(ws["f"], *ff) if ff else torch.nn.functional.gelu(ws["f"])
-        gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["x1"], out=ws["y"], two_cta=True,
+        gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["x1"], out=ws["y"],
                             dropout=site(drop, K.SITE_LINEAR2))
         K.ln_relu_fwd(ws["y"], pv["g2"], pv["be2"], None, out=ws["out"], mean=ws["stats"][2], rstd=ws["stats"][3], relu=False)
         return ws, T
@@ -365,23 +365,23 @@ class NativeTransformerExecutor:
         K.ln_relu_bwd(dout, ws["y"], ws["stats"][2], ws["stats"][3], pv["g2"], pv["be2"], None, dh=dy, dgamma=gv["g2"],
                       dbeta=gv["be2"], dbias=scratch if site(drop, K.SITE_LINEAR2) else gv["b2"], relu=False)
         dff = branch_grad(dy, K.SITE_LINEAR2, gv["b2"])
-        gemm.grouped_wgrad(dff, ws["gact"], go, 1, out=gv["w2"], two_cta=True)
-        dg = gemm.grouped_linear(dff, bv["w2"], w_is_kn=True, two_cta=True)
+        gemm.grouped_wgrad(dff, ws["gact"], go, 1, out=gv["w2"])
+        dg = gemm.grouped_linear(dff, bv["w2"], w_is_kn=True)
         ff = site(drop, K.SITE_FF)
         df = K.gelu_dropout_bwd(dg, ws["f"], *ff) if ff else torch.ops.aten.gelu_backward(dg, ws["f"])
         K.grouped_colsum(df, None, out=gv["b1"])
-        gemm.grouped_wgrad(df, ws["x1"], go, 1, out=gv["w1"], two_cta=True)
-        dx1 = gemm.grouped_linear(df, bv["w1"], w_is_kn=True, residual=dy, two_cta=True)
+        gemm.grouped_wgrad(df, ws["x1"], go, 1, out=gv["w1"])
+        dx1 = gemm.grouped_linear(df, bv["w1"], w_is_kn=True, residual=dy)
         dh = torch.empty(T, d, **bf)
         K.ln_relu_bwd(dx1, ws["h"], ws["stats"][0], ws["stats"][1], pv["g1"], pv["be1"], None, dh=dh, dgamma=gv["g1"],
                       dbeta=gv["be1"], dbias=scratch if site(drop, K.SITE_OUT_PROJ) else gv["b_out"], relu=False)
         dhb = branch_grad(dh, K.SITE_OUT_PROJ, gv["b_out"])
-        gemm.grouped_wgrad(dhb, ws["att"], go, 1, out=gv["w_out"], two_cta=True)
-        datt = gemm.grouped_linear(dhb, bv["w_out"], w_is_kn=True, two_cta=True)
+        gemm.grouped_wgrad(dhb, ws["att"], go, 1, out=gv["w_out"])
+        datt = gemm.grouped_linear(dhb, bv["w_out"], w_is_kn=True)
         dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN))
         K.grouped_colsum(dqkv, None, out=gv["b_in"])
-        gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"], two_cta=True)
-        dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh, two_cta=True)
+        gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"])
+        dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh)
         g = self.opt.param_groups[0]
         K.bump_steps(self.step, self.one)
         K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step, lr=float(g["lr"]),

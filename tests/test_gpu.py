@@ -50,9 +50,9 @@ def test_grouped_gemm_wgrad(gemm_check, args):
     dict(rows_per_group=[1000, 24, 2048], N=2048, K=512, w_is_kn=False, block_n=256),
     dict(rows_per_group=[700, 1, 513], N=2048, K=2048, w_is_kn=True, block_n=256, bias=False),
 ])
-def test_cta_pair_gemm_forward_and_dgrad(gemm_check, args):
-    """the PRODUCTION entry point of the big path (lah_gemm_mgroup2: 128x256 tiles, 256-row expert groups)"""
-    err, untouched = gemm_check.case_mgroup(two_cta=True, **args)
+def test_grouped_gemm_256row_groups_forward_and_dgrad(gemm_check, args):
+    """the big expert path's layout: 128 x 256 tiles over expert groups padded to 256 rows"""
+    err, untouched = gemm_check.case_mgroup(align=256, **args)
     assert err < 1e-2 and untouched
 
 
@@ -62,9 +62,10 @@ def test_cta_pair_gemm_forward_and_dgrad(gemm_check, args):
     dict(rows_per_group=[2048, 0, 640], M=2048, N=2048, block_n=256),
     dict(rows_per_group=[1000, 64], M=2048, N=512, block_n=256),
 ])
-def test_cta_pair_gemm_wgrad_values(gemm_check, args):
-    """wgrad of the production kernel compared by VALUE (rel. L2 error vs the fp32 matmul of the same bf16 operands)"""
-    assert gemm_check.case_kgroup(two_cta=True, **args) < 1e-3
+def test_grouped_gemm_256row_groups_wgrad(gemm_check, args):
+    """wgrad over expert groups padded to 256 rows on 128 x 256 tiles, compared by VALUE (rel. L2 error vs the fp32 matmul
+    of the same bf16 operands)"""
+    assert gemm_check.case_kgroup(align=256, **args) < 1e-3
 
 
 @pytest.mark.parametrize("check", ["check_swapab", "check_wgrad_adam"])

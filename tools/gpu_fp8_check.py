@@ -123,7 +123,7 @@ def check_perf():
         wq = fp8.quantize(w, tile_rows=fp8.WEIGHT_TILE, groups=G)
         out = torch.empty(rows, N, device="cuda", dtype=torch.bfloat16)
         ms8 = timeit(lambda: fp8.grouped_linear_fp8(aq, wq, tile_group=tg, bias=b, out=out))
-        ms16 = timeit(lambda: gemm.grouped_linear(a, wb, tile_group=tg, bias=b, out=out, two_cta=True))
+        ms16 = timeit(lambda: gemm.grouped_linear(a, wb, tile_group=tg, bias=b, out=out))
         msq = timeit(lambda: fp8.quantize(a, out=aq))
         flops = 2.0 * rows * N * K
         results[f"perf_{name}"] = dict(ok=True, fp8_ms=ms8, fp8_tflops=flops / ms8 / 1e9, bf16_ms=ms16,

@@ -29,10 +29,10 @@ def timeit(fn, iters=20, warmup=3):
     return s.elapsed_time(e) / iters
 
 
-def case_mgroup(rows_per_group, N, K, w_is_kn, block_n, bias=True, residual=False, out_f32=False, seed=0, two_cta=False):
+def case_mgroup(rows_per_group, N, K, w_is_kn, block_n, bias=True, residual=False, out_f32=False, seed=0, align=128):
+    """expert groups padded to `align` rows (128, or 256 as on the big expert path)"""
     torch.manual_seed(seed)
     G = len(rows_per_group)
-    align = 256 if two_cta else 128
     tiles = []
     for g, r in enumerate(rows_per_group):
         tiles += [g] * (((r + align - 1) // align) * (align // 128))
@@ -48,8 +48,7 @@ def case_mgroup(rows_per_group, N, K, w_is_kn, block_n, bias=True, residual=Fals
     res = torch.randn(rows, N, device="cuda").to(torch.bfloat16) if residual else None
     tg = torch.tensor(tiles, device="cuda", dtype=torch.int32)
     out = torch.full((rows, N), 7.0, device="cuda", dtype=torch.float32 if out_f32 else torch.bfloat16)
-    gemm.grouped_linear(a, w, tile_group=tg, bias=b, residual=res, w_is_kn=w_is_kn, out=out, block_n=block_n,
-                        two_cta=two_cta)
+    gemm.grouped_linear(a, w, tile_group=tg, bias=b, residual=res, w_is_kn=w_is_kn, out=out, block_n=block_n)
     torch.cuda.synchronize()
     ref = gemm.grouped_linear_ref(a, w, tile_group=tg, bias=b, residual=res, w_is_kn=w_is_kn)
     valid = (tg >= 0).repeat_interleave(128)
@@ -58,12 +57,13 @@ def case_mgroup(rows_per_group, N, K, w_is_kn, block_n, bias=True, residual=Fals
     return err, untouched
 
 
-def case_kgroup(rows_per_group, M, N, block_n, seed=0, two_cta=False):
+def case_kgroup(rows_per_group, M, N, block_n, seed=0, align=128):
+    """expert groups padded to `align` rows (128, or 256 as on the big expert path)"""
     torch.manual_seed(seed)
     G = len(rows_per_group)
     off = [0]
     for r in rows_per_group:
-        off.append(off[-1] + ((r + 127) // 128) * 128)
+        off.append(off[-1] + ((r + align - 1) // align) * align)
     rows = off[-1] + 128
     dy = torch.zeros(rows, M, device="cuda", dtype=torch.bfloat16)
     x = torch.zeros(rows, N, device="cuda", dtype=torch.bfloat16)
@@ -71,7 +71,7 @@ def case_kgroup(rows_per_group, M, N, block_n, seed=0, two_cta=False):
         dy[off[g]: off[g] + r] = torch.randn(r, M, device="cuda").to(torch.bfloat16)
         x[off[g]: off[g] + r] = torch.randn(r, N, device="cuda").to(torch.bfloat16)
     go = torch.tensor(off, device="cuda", dtype=torch.int32)
-    out = gemm.grouped_wgrad(dy, x, go, G, block_n=block_n, two_cta=two_cta)
+    out = gemm.grouped_wgrad(dy, x, go, G, block_n=block_n)
     torch.cuda.synchronize()
     ref = gemm.grouped_wgrad_ref(dy, x, go, G)
     return rel_err(out, ref)
@@ -97,10 +97,10 @@ def main():
             results[name] = dict(error=repr(e), ok=False)
         print(name, results[name], flush=True)
     for (name, args) in [
-        ("mg2_kmajor", dict(rows_per_group=[128, 300, 0, 77, 1000], N=512, K=512, w_is_kn=False, block_n=256, two_cta=True)),
-        ("mg2_kmajor_res_f32", dict(rows_per_group=[200, 530], N=512, K=2048, w_is_kn=False, block_n=256, residual=True, out_f32=True, two_cta=True)),
-        ("mg2_kn", dict(rows_per_group=[128, 300, 0, 77], N=2048, K=512, w_is_kn=True, block_n=256, bias=False, two_cta=True)),
-        ("mg2_kn_res", dict(rows_per_group=[640, 5], N=512, K=2048, w_is_kn=True, block_n=256, bias=False, residual=True, two_cta=True)),
+        ("mg_align256_kmajor", dict(rows_per_group=[128, 300, 0, 77, 1000], N=512, K=512, w_is_kn=False, block_n=256, align=256)),
+        ("mg_align256_kmajor_res_f32", dict(rows_per_group=[200, 530], N=512, K=2048, w_is_kn=False, block_n=256, residual=True, out_f32=True, align=256)),
+        ("mg_align256_kn", dict(rows_per_group=[128, 300, 0, 77], N=2048, K=512, w_is_kn=True, block_n=256, bias=False, align=256)),
+        ("mg_align256_kn_res", dict(rows_per_group=[640, 5], N=512, K=2048, w_is_kn=True, block_n=256, bias=False, residual=True, align=256)),
     ]:
         try:
             err, untouched = case_mgroup(**args)
@@ -109,8 +109,8 @@ def main():
             results[name] = dict(error=repr(e), ok=False)
         print(name, results[name], flush=True)
     for (name, args) in [
-        ("kg2_a", dict(rows_per_group=[128, 300, 0, 77], M=256, N=512, block_n=256, two_cta=True)),
-        ("kg2_b", dict(rows_per_group=[2048, 640], M=2048, N=2048, block_n=256, two_cta=True)),
+        ("kg_align256_a", dict(rows_per_group=[128, 300, 0, 77], M=256, N=512, block_n=256, align=256)),
+        ("kg_align256_b", dict(rows_per_group=[2048, 640], M=2048, N=2048, block_n=256, align=256)),
         ("kg_bn256", dict(rows_per_group=[128, 300, 0, 77], M=256, N=512, block_n=256)),
         ("kg_bn128", dict(rows_per_group=[1000, 64], M=128, N=384, block_n=128)),
         ("kg_bn64", dict(rows_per_group=[512, 512], M=512, N=64, block_n=64)),
@@ -141,13 +141,6 @@ def main():
             ms = timeit(lambda: gemm.grouped_linear(a, wkn, tile_group=tg, out=out, w_is_kn=True, block_n=256))
             results[f"perf_{nm}_kn_bn256"] = dict(ms=ms, tflops=fl / ms / 1e9)
             print(f"perf_{nm}_kn_bn256", results[f"perf_{nm}_kn_bn256"], flush=True)
-            if N % 256 == 0:
-                ms = timeit(lambda: gemm.grouped_linear(a, w, tile_group=tg, out=out, two_cta=True))
-                results[f"perf_{nm}_kmajor_2cta"] = dict(ms=ms, tflops=fl / ms / 1e9)
-                print(f"perf_{nm}_kmajor_2cta", results[f"perf_{nm}_kmajor_2cta"], flush=True)
-                ms = timeit(lambda: gemm.grouped_linear(a, wkn, tile_group=tg, out=out, w_is_kn=True, two_cta=True))
-                results[f"perf_{nm}_kn_2cta"] = dict(ms=ms, tflops=fl / ms / 1e9)
-                print(f"perf_{nm}_kn_2cta", results[f"perf_{nm}_kn_2cta"], flush=True)
             # cuBLAS reference: bmm over groups
             a3 = a.view(G, R, K)
             ms = timeit(lambda: torch.bmm(a3, w.transpose(1, 2)))
@@ -161,9 +154,6 @@ def main():
             ms = timeit(lambda: gemm.grouped_wgrad(dy, x, go, G, out=out, block_n=256))
             results[f"perf_{nm}"] = dict(ms=ms, tflops=fl / ms / 1e9)
             print(f"perf_{nm}", results[f"perf_{nm}"], flush=True)
-            ms = timeit(lambda: gemm.grouped_wgrad(dy, x, go, G, out=out, two_cta=True))
-            results[f"perf_{nm}_2cta"] = dict(ms=ms, tflops=fl / ms / 1e9)
-            print(f"perf_{nm}_2cta", results[f"perf_{nm}_2cta"], flush=True)
             ms = timeit(lambda: torch.bmm(dy.view(G, R, M).transpose(1, 2), x.view(G, R, N)))
             results[f"perf_{nm}_cublas_bmm"] = dict(ms=ms, tflops=fl / ms / 1e9)
             print(f"perf_{nm}_cublas_bmm", results[f"perf_{nm}_cublas_bmm"], flush=True)

@@ -204,7 +204,7 @@ def perf_skew():
         out["fwd2_ms"] = timeit(lambda: K.swapab_linear(a, w2, off, rows, out=h), flush=flush)
         out["dgrad2_ms"] = timeit(lambda: K.swapab_linear(a, w2, off, rows, out=h, w_is_kn=True), flush=flush)
         out["dgrad1_ms"] = timeit(lambda: K.swapab_linear(a, w1, off, rows, out=y, w_is_kn=True), flush=flush)
-        out["fwd2_52ctas_ms"] = timeit(lambda: K.swapab_linear(a, w2, off, rows, out=h, max_ctas=52), flush=flush)
+        out["fwd2_52_ctas_ms"] =timeit(lambda: K.swapab_linear(a, w2, off, rows, out=h, max_ctas=52), flush=flush)
         p = torch.randn(G, I, I, device="cuda")
         m, v, vmax = torch.zeros_like(p), torch.zeros_like(p), torch.zeros_like(p)
         pb = torch.zeros(G, I, I, device="cuda", dtype=torch.bfloat16)

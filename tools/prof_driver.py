@@ -26,7 +26,7 @@ if "fp8" in which or "bf16" in which:
     if "bf16" in which:
         wb = w.view(G, N, Kd).to(torch.bfloat16)
         for _ in range(2):
-            gemm.grouped_linear(a, wb, tile_group=tg, bias=b, out=out, two_cta=True)
+            gemm.grouped_linear(a, wb, tile_group=tg, bias=b, out=out)
 if "attn" in which:
     qkv = torch.randn(32 * 512, 3 * 1024, device="cuda").to(torch.bfloat16)
     o = torch.empty(32 * 512, 1024, device="cuda", dtype=torch.bfloat16)
