@@ -786,7 +786,8 @@ __global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineA
 
 // ------------------------------------------------------------------------------------------------
 // backward of combine (gate side): dw[b,j] = <g[b], y_j>;  dlogit_j = w_j (dw_j - sum_i w_i dw_i)
-// scattered into the gradient of the grid logits [B, gs.total]
+// scattered into the gradient of the grid logits [B, gs.total].  A selected pair that scatter_rows dropped (pair_row -1)
+// has y_j = 0, so dw_j = 0, but its weight still took softmax mass from the others: its logit gets -w_j sum_i w_i dw_i
 // ------------------------------------------------------------------------------------------------
 struct GateBwdArgs {
     long long yo_off;         // symmetric expert outputs [max_rows, H]
@@ -829,6 +830,10 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
             const long long p = static_cast<long long>(b) * a.k + j;
             const int e = a.idx[p];
             const int row = a.pair_row[p];
+            if (e >= 0) {   // a pair dropped by scatter_rows (row -1) added nothing to y but keeps its softmax weight
+                wj[j] = a.w[p];
+                ej[j] = e;
+            }
             if (e >= 0 && row >= 0) {
                 const int4* sp = reinterpret_cast<const int4*>(peers.base[a.route_owner ? a.route_owner[e] : e / a.E_loc] + a.yo_off) +
                                  static_cast<long long>(row) * (a.H / 8);
@@ -845,8 +850,6 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
                 }
                 d = warp_sum(d);
                 dw[j] = d;
-                wj[j] = a.w[p];
-                ej[j] = e;
                 dot_sum += wj[j] * d;
             }
         }
@@ -1021,6 +1024,10 @@ int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, 
     GridSpec gs;
     if (make_grid_spec(&gs, grid, ndim)) return -2;
     if (k < 1 || k > MAX_K) return -3;
+    // each of the 8 warps stages its token's grid logits in shared memory: 4096 of them (a dense gate over as many experts
+    // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in
+    if (gs.total > LAYOUT_MAX_E) return -2;
+    if (int e = set_max_dynamic_smem<gate_topk_kernel>(8 * sizeof(float) * LAYOUT_MAX_E)) return e;
     if (B <= 0) return 0;
     gate_topk_kernel<<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(logits, B, gs, k, alive, failure_rate, seed,
                                                                            token_offset, idx, w, pos, counts,

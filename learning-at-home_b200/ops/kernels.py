@@ -545,7 +545,10 @@ def product_key_scores(logits, grid_size):
 
 
 def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None):
-    """returns idx [B,k] (-1 for missing), weights [B,k] (softmax over alive selected)"""
+    """returns idx [B,k] (-1 for missing), weights [B,k] (softmax over alive selected).  Equal scores select the smaller
+    expert id first, like gate_topk_kernel (torch.topk leaves the order of ties unspecified, so it sorts stably instead).
+    The scores are summed first grid dimension first and the kernel last dimension first: on 3-d and 4-d grids they can
+    differ in the last bit unless the logits are exact in any order (e.g. small multiples of a power of two)."""
     scores = product_key_scores(logits.float(), grid_size)
     dead = torch.zeros_like(scores, dtype=torch.bool)
     if alive is not None:
@@ -553,11 +556,40 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None):
     if fail_mask is not None:
         dead |= fail_mask
     scores = scores.masked_fill(dead, float("-inf"))
-    top_v, top_i = torch.topk(scores, k, dim=-1)
+    if scores.shape[-1] < k:
+        scores = F.pad(scores, (0, k - scores.shape[-1]), value=float("-inf"))
+    top_v, top_i = torch.sort(scores, dim=-1, descending=True, stable=True)
+    top_v, top_i = top_v[..., :k], top_i[..., :k]
     valid = torch.isfinite(top_v)
     w = torch.softmax(top_v.masked_fill(~valid, float("-inf")), dim=-1)
     w = torch.where(valid, w, torch.zeros_like(w)).nan_to_num(0.0)
     return torch.where(valid, top_i, torch.full_like(top_i, -1)), w
+
+
+_SPLITMIX_GAMMA = 0x9E3779B97F4A7C15
+
+
+def splitmix64_ref(x):
+    """splitmix64 finaliser of csrc/moe.cu hash_uniform, x + gamma included (= the output of a splitmix64 generator whose
+    state was x); numpy uint64 arrays wrap modulo 2**64 like the kernel's unsigned long long"""
+    import numpy as np
+    x = np.array(x, dtype=np.uint64, ndmin=1) + np.uint64(_SPLITMIX_GAMMA)
+    x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return x ^ (x >> np.uint64(31))
+
+
+def gate_fail_mask_ref(B, E, rate, seed, token_offset):
+    """[B, E] bool: the (token, expert) pairs that gate_topk's failure injection drops.  Token b of a call draws
+    u = (splitmix64(seed ^ ((token_offset + b) * 0x100000001B3 + e)) >> 40) / 2**24 for expert e and fails iff u < rate, with
+    rate rounded to float32 as the kernel receives it.  u has 24 bits, so this is exact, not a statistical twin.
+    ``token_offset`` is the kernel argument plus the device token base (step counters [2:4]) at the launch."""
+    import numpy as np
+    mask64 = 2 ** 64 - 1
+    tok = (np.arange(B, dtype=np.uint64) + np.uint64(int(token_offset) & mask64)) * np.uint64(0x100000001B3)
+    key = np.uint64(int(seed) & mask64) ^ (tok[:, None] + np.arange(E, dtype=np.uint64)[None, :])
+    u = (splitmix64_ref(key) >> np.uint64(40)).astype(np.float64) / 2.0 ** 24
+    return torch.from_numpy(u < float(np.float32(rate)))
 
 
 def ln_relu_ref(h, gamma, beta, relu=True):
