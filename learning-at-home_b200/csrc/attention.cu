@@ -1,4 +1,4 @@
-// attention.cu — wgmma self-attention for the transformer expert (d_model 1024, 16 heads x 64, seq 512;
+// attention.cu — wgmma self-attention for the transformer expert (head_dim 64, any sequence length S in 1..MAX_SEQ;
 // reference: nn.MultiheadAttention inside experiments/throughput/layers.py:22-51).
 //
 // FORWARD (this file): flash attention.  One CTA owns one 128-query tile of one (batch, head); two consumer warpgroups own
@@ -8,8 +8,14 @@
 // fragment layout).  S and P never touch shared memory or HBM.  The kernel also emits the row log-sum-exp (base 2) that the
 // BACKWARD kernel (attention_bwd.cu) needs to recompute P without a second softmax pass.
 //
-// Input : qkv [T = batch*512, 3*D] bf16 (output of the fused in_proj GEMM: [q | k | v] per token, heads contiguous)
+// Input : qkv [T = batch*S, 3*D] bf16 (output of the fused in_proj GEMM: [q | k | v] per token, heads contiguous)
 // Output: out [T, D] bf16 (heads concatenated, ready for out_proj); lse2 [T, heads] fp32 (optional)
+//
+// Sequence length: ceil(S / 128) query tiles and key blocks per sequence.  The tensor map is 3-D {3*D, S, batch}, so TMA
+// zero-fills the rows past the end of a sequence and no tile reads the next one.  In the last key block of a partial
+// sequence (S % 128 != 0) the scores of keys >= S are set to -inf before the row maximum, so they enter neither l nor the
+// LSE; rows of queries >= S are computed on zeros and not stored.  Full blocks take exactly the arithmetic of the
+// 512-token kernel: the tail test is one uniform branch per key block.
 #include "sm90.cuh"
 #include "dropout.cuh"
 #include <stdlib.h>
@@ -17,14 +23,12 @@
 namespace lah {
 namespace attn {
 
-constexpr int S_LEN = 512;      // keys per sequence
 constexpr int HEAD_DIM = 64;
 constexpr int Q_TILE = 128;
 
 namespace v2 {
 
 constexpr int KB = 128;                       // keys per block
-constexpr int NUM_KB = S_LEN / KB;            // 4
 constexpr int NUM_THREADS2 = 256;             // two consumer warpgroups; thread 0 also drives TMA
 constexpr int TILE_BYTES = 128 * HEAD_DIM * 2;            // 16 KB: a 128 x 64 bf16 tile (Q tile, K block, V block)
 constexpr int OFF_Q2 = 0;
@@ -39,7 +43,7 @@ constexpr int SMEM_TOTAL2 = OFF_BAR2 + NUM_BARS * 8 + 16 + 1024;
 template <bool DROP>
 __global__ void __launch_bounds__(NUM_THREADS2, 1)
 attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, float* __restrict__ lse2,
-                        int d_model, int num_heads, float scale_log2e, unsigned long long seed, uint32_t thr,
+                        int d_model, int num_heads, int seq_len, float scale_log2e, unsigned long long seed, uint32_t thr,
                         float rescale) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -48,16 +52,16 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     uint64_t* kv_full = bars + 1;   // [2]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-    const int qt = blockIdx.x & 3;
-    const int head = (blockIdx.x >> 2) % num_heads;
-    const int batch = (blockIdx.x >> 2) / num_heads;
-    const int seq_row0 = batch * S_LEN;
+    const int num_kb = (seq_len + KB - 1) / KB;   // key blocks = query tiles per sequence
+    const int qt = blockIdx.x % num_kb;
+    const int head = (blockIdx.x / num_kb) % num_heads;
+    const int batch = (blockIdx.x / num_kb) / num_heads;
 
     auto load_kv = [&](int j) {   // thread 0 only; stage j & 1 must be free
         const int st = j & 1;
         mbar_arrive_expect_tx(&kv_full[st], 2 * TILE_BYTES);
-        tma_load_2d(smem + OFF_K2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], d_model + head * HEAD_DIM, seq_row0 + j * KB);
-        tma_load_2d(smem + OFF_V2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], 2 * d_model + head * HEAD_DIM, seq_row0 + j * KB);
+        tma_load_3d(smem + OFF_K2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], d_model + head * HEAD_DIM, j * KB, batch);
+        tma_load_3d(smem + OFF_V2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], 2 * d_model + head * HEAD_DIM, j * KB, batch);
     };
     if (tid == 0) {
         tma_prefetch_desc(&tm_qkv);
@@ -66,9 +70,9 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         mbar_init(&kv_full[1], 1);
         fence_mbar_init();
         mbar_arrive_expect_tx(bar_q, TILE_BYTES);
-        tma_load_2d(smem + OFF_Q2, &tm_qkv, bar_q, head * HEAD_DIM, seq_row0 + qt * Q_TILE);
+        tma_load_3d(smem + OFF_Q2, &tm_qkv, bar_q, head * HEAD_DIM, qt * Q_TILE, batch);
         load_kv(0);
-        load_kv(1);
+        if (num_kb > 1) load_kv(1);
     }
     __syncthreads();
 
@@ -80,7 +84,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(bar_q, 0);
 #pragma unroll 1
-    for (int j = 0; j < NUM_KB; ++j) {
+    for (int j = 0; j < num_kb; ++j) {
         const int st = j & 1;
         mbar_wait(&kv_full[st], (j >> 1) & 1);
         const uint32_t sk = smem_u32(smem + OFF_K2 + st * TILE_BYTES), sv = smem_u32(smem + OFF_V2 + st * TILE_BYTES);
@@ -108,6 +112,13 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         }
         wgmma_wait<0>();
         wgmma_fence_regs(s);
+        if (j * KB + KB > seq_len) {   // last block of a partial sequence: s[4 jj + 2 h + i] is key 8 jj + 2 (lane & 3) + i
+#pragma unroll
+            for (int jj = 0; jj < KB / 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (j * KB + 8 * jj + 2 * (lane & 3) + i >= seq_len) s[4 * jj + i] = s[4 * jj + 2 + i] = -INFINITY;
+        }
         uint32_t pa[KB / 16][4];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -149,7 +160,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(o);
-        if (j + 2 < NUM_KB) {
+        if (j + 2 < num_kb) {
             named_bar_sync(1, NUM_THREADS2);   // both warpgroups are done with stage st
             if (tid == 0) load_kv(j + 2);
         }
@@ -160,7 +171,9 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         lt += __shfl_xor_sync(0xffffffffu, lt, 1);
         lt += __shfl_xor_sync(0xffffffffu, lt, 2);
         const float inv = DROP ? rescale / lt : 1.f / lt;
-        const long long token = seq_row0 + qt * Q_TILE + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        const int q = qt * Q_TILE + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        if (q >= seq_len) continue;
+        const long long token = static_cast<long long>(batch) * seq_len + q;
         if (lse2 && (lane & 3) == 0) lse2[token * num_heads + head] = m[h] * scale_log2e + log2f(lt);
         bf16* op = out + token * d_model + head * HEAD_DIM + 2 * (lane & 3);
 #pragma unroll
@@ -179,26 +192,32 @@ using namespace lah::attn;
 
 extern "C" {
 
-// qkv: [tokens, 3*d_model] bf16, tokens = batch * 512; out: [tokens, d_model] bf16; lse2: [tokens, heads] fp32 or NULL
+// qkv: [tokens, 3*d_model] bf16, tokens = batch * seq_len, 1 <= seq_len <= MAX_SEQ; out: [tokens, d_model] bf16;
+// lse2: [tokens, heads] fp32 or NULL.  Returns -2 for a sequence length out of range or one that does not divide tokens.
 // drop_thr < 0: no dropout; otherwise attention dropout with threshold drop_thr (dropout.cuh), seed, rescale = 1 / (1 - p)
-int lah_attention_fwd(const void* qkv, void* out, float* lse2, int batch, int num_heads, int d_model,
+int lah_attention_fwd(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
                       unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
     if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
     CUtensorMap tm;
-    {
-        uint64_t dims[2] = {(uint64_t)3 * d_model, (uint64_t)batch * S_LEN};
-        uint64_t str[1] = {(uint64_t)3 * d_model * 2};
-        uint32_t box[2] = {HEAD_DIM, 128};
-        int r = make_tmap(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, qkv, dims, str, box);
+    {   // 3-D {columns, position in sequence, sequence}: a tile never crosses into the next sequence
+        uint64_t dims[3] = {(uint64_t)3 * d_model, (uint64_t)seq_len, (uint64_t)batch};
+        uint64_t str[2] = {(uint64_t)3 * d_model * 2, (uint64_t)seq_len * 3 * d_model * 2};
+        uint32_t box[3] = {HEAD_DIM, 128, 1};
+        int r = make_tmap(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, qkv, dims, str, box);
         if (r) return r;
     }
     if (int e = set_max_dynamic_smem<v2::attention_fwd_v2_kernel<false>>(v2::SMEM_TOTAL2)) return e;
     if (int e = set_max_dynamic_smem<v2::attention_fwd_v2_kernel<true>>(v2::SMEM_TOTAL2)) return e;
-    if (batch <= 0) return 0;
     const float scale_log2e = 1.4426950408889634f / sqrtf((float)HEAD_DIM);
+    const long long ctas = batch * num_heads * ((seq_len + Q_TILE - 1) / Q_TILE);
+    if (ctas > 0x7fffffffll) return -2;
     auto kern = drop_thr < 0 ? v2::attention_fwd_v2_kernel<false> : v2::attention_fwd_v2_kernel<true>;
-    kern<<<batch * num_heads * (S_LEN / Q_TILE), v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
-        tm, (bf16*)out, lse2, d_model, num_heads, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale);
+    kern<<<(unsigned)ctas, v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
+        tm, (bf16*)out, lse2, d_model, num_heads, seq_len, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr),
+        rescale);
     return -(int)cudaGetLastError();
 }
 

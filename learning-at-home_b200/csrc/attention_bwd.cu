@@ -1,9 +1,10 @@
-// attention_bwd.cu — wgmma self-attention BACKWARD for the transformer expert (d_model 1024, 16 heads x 64, seq 512).
+// attention_bwd.cu — wgmma self-attention BACKWARD for the transformer expert (head_dim 64, any sequence length S in
+// 1..MAX_SEQ).
 // The reference's transformer expert cannot be trained at all (in-place transpose of a leaf, SURVEY.md §0.3); this kernel is
 // what makes the sm_90a transformer expert trainable without falling back to eager PyTorch.
 //
 // One CTA = one (batch, head, 128-key block j); consumer warpgroup w owns keys [64w, 64w + 64) of the block.  K_j / V_j stay
-// in shared memory; the four 128-query blocks i stream through a 2-stage TMA pipeline (Q_i and dO_i).  Per query block, all
+// in shared memory; the ceil(S / 128) query blocks i stream through a 2-stage TMA pipeline (Q_i and dO_i).  Per query block, all
 // on tensor cores with accumulators in registers (transposed problem: keys are the MMA rows):
 //
 //     S^T = K_j Q_i^T               (64 x 128 per warpgroup)     dP^T = V_j dO_i^T            (64 x 128)
@@ -20,16 +21,20 @@
 // Pd = M o P / (1 - p):  dV += Pd^T dO,  dS = P o (M o dP / (1 - p) - Delta) * scale, Delta = rowsum(dO o O) of the DROPPED
 // output O (attn_delta_kernel, unchanged); LSE is that of the undropped softmax.  P^T is masked but not scaled in the dV
 // MMA; 1 / (1 - p) is applied to dV once at the end.
+//
+// Sequence length: the tensor maps are 3-D {columns, S, batch}, so rows past the end of a sequence arrive as zeros.  Zeros
+// alone do not make P vanish (exp2(0 - LSE) is not 0, and a garbage LSE can make it inf, and inf * 0 is NaN), so in a
+// partial block P^T and dS^T are forced to exactly 0: queries >= S get LSE = +inf and Delta = 0 (LSE and Delta are only
+// read for valid queries), keys >= S get S^T = -inf.  No dK / dV row is stored for keys >= S and no dQ-partial row for
+// queries >= S.  Full blocks run exactly the arithmetic of the 512-token kernel.
 #include "sm90.cuh"
 #include "dropout.cuh"
 
 namespace lah {
 namespace attnb {
 
-constexpr int S_LEN = 512;
 constexpr int HEAD_DIM = 64;
 constexpr int BLK = 128;                       // query block == key block
-constexpr int NUM_QB = S_LEN / BLK;            // 4
 constexpr int NUM_THREADS = 256;
 constexpr int TILE = BLK * HEAD_DIM * 2;       // 16 KB: 128 x 64 bf16
 constexpr int ATOM = BLK * 128;                // 16 KB: one [128 key rows][64 queries] atom of dS^T
@@ -47,7 +52,7 @@ template <bool DROP>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
-                     bf16* __restrict__ dq_part, long long total_tokens, int d_model, int num_heads, float scale,
+                     bf16* __restrict__ dq_part, long long total_tokens, int d_model, int num_heads, int seq_len, float scale,
                      float scale_log2e, unsigned long long seed, uint32_t thr, float rescale) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -58,16 +63,17 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     float* s_delta = s_lse + BLK;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-    const int j = blockIdx.x & 3;
-    const int head = (blockIdx.x >> 2) % num_heads;
-    const int batch = (blockIdx.x >> 2) / num_heads;
-    const int seq0 = batch * S_LEN;
+    const int num_qb = (seq_len + BLK - 1) / BLK;   // query blocks = key blocks per sequence
+    const int j = blockIdx.x % num_qb;
+    const int head = (blockIdx.x / num_qb) % num_heads;
+    const int batch = (blockIdx.x / num_qb) / num_heads;
+    const long long seq0 = static_cast<long long>(batch) * seq_len;
 
     auto load_q = [&](int i) {   // thread 0 only; stage i & 1 must be free
         const int st = i & 1;
         mbar_arrive_expect_tx(&q_full[st], 2 * TILE);
-        tma_load_2d(smem + OFF_Q + st * TILE, &tm_qkv, &q_full[st], head * HEAD_DIM, seq0 + i * BLK);
-        tma_load_2d(smem + OFF_DO + st * TILE, &tm_do, &q_full[st], head * HEAD_DIM, seq0 + i * BLK);
+        tma_load_3d(smem + OFF_Q + st * TILE, &tm_qkv, &q_full[st], head * HEAD_DIM, i * BLK, batch);
+        tma_load_3d(smem + OFF_DO + st * TILE, &tm_do, &q_full[st], head * HEAD_DIM, i * BLK, batch);
     };
     if (tid == 0) {
         tma_prefetch_desc(&tm_qkv);
@@ -77,10 +83,10 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         mbar_init(&q_full[1], 1);
         fence_mbar_init();
         mbar_arrive_expect_tx(kv_full, 2 * TILE);
-        tma_load_2d(smem + OFF_K, &tm_qkv, kv_full, d_model + head * HEAD_DIM, seq0 + j * BLK);
-        tma_load_2d(smem + OFF_V, &tm_qkv, kv_full, 2 * d_model + head * HEAD_DIM, seq0 + j * BLK);
+        tma_load_3d(smem + OFF_K, &tm_qkv, kv_full, d_model + head * HEAD_DIM, j * BLK, batch);
+        tma_load_3d(smem + OFF_V, &tm_qkv, kv_full, 2 * d_model + head * HEAD_DIM, j * BLK, batch);
         load_q(0);
-        load_q(1);
+        if (num_qb > 1) load_q(1);
     }
     __syncthreads();
 
@@ -92,11 +98,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     for (int e = 0; e < HEAD_DIM / 2; ++e) dv[e] = dk[e] = 0.f;
     mbar_wait(kv_full, 0);
 #pragma unroll 1
-    for (int i = 0; i < NUM_QB; ++i) {
+    for (int i = 0; i < num_qb; ++i) {
         const int st = i & 1;
         const long long tok0 = seq0 + i * BLK;
-        if (tid < BLK) s_lse[tid] = __ldg(lse2 + (tok0 + tid) * num_heads + head);
-        else s_delta[tid - BLK] = __ldg(delta + (tok0 + tid - BLK) * num_heads + head);
+        const int qr = tid & (BLK - 1);   // query row of the block whose LSE (tid < 128) or Delta this thread loads
+        const bool qvalid = i * BLK + qr < seq_len;
+        if (tid < BLK) s_lse[qr] = qvalid ? __ldg(lse2 + (tok0 + qr) * num_heads + head) : INFINITY;
+        else s_delta[qr] = qvalid ? __ldg(delta + (tok0 + qr) * num_heads + head) : 0.f;
         mbar_wait(&q_full[st], (i >> 1) & 1);
         const uint32_t sq = smem_u32(smem + OFF_Q + st * TILE), sdo = smem_u32(smem + OFF_DO + st * TILE);
         float sacc[BLK / 2], dpacc[BLK / 2];
@@ -114,6 +122,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         wgmma_wait<0>();
         wgmma_fence_regs(sacc);
         wgmma_fence_regs(dpacc);
+        if (j * BLK + BLK > seq_len) {   // last key block of a partial sequence: sacc[4 jj + 2 h + par] is key key_row + 8 h
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (j * BLK + key_row + 8 * h >= seq_len)
+#pragma unroll
+                    for (int jj = 0; jj < BLK / 8; ++jj) sacc[4 * jj + 2 * h] = sacc[4 * jj + 2 * h + 1] = -INFINITY;
+        }
         const uint32_t kk = j * BLK + key_row;   // this thread's keys: kk, kk + 8
         uint32_t km = 0u;
         uint32_t pa[BLK / 16][4], da[BLK / 16][4];
@@ -185,22 +200,25 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         wgmma_fence_regs(dq);
         wgmma_fence_regs(dv);
         wgmma_fence_regs(dk);
-        // partial dQ of THIS key block into slice j of dq_part ([4, T, D] bf16; attn_dq_reduce_kernel sums the four slices in
-        // fp32) — no atomics, half the bytes of fp32 partials
+        // partial dQ of THIS key block into slice j of dq_part ([ceil(S / 128), T, D] bf16; attn_dq_reduce_kernel sums the
+        // slices in fp32) — no atomics, half the bytes of fp32 partials
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            const long long token = tok0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+            const int q = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+            if (i * BLK + q >= seq_len) continue;
+            const long long token = tok0 + q;
             bf16* dqp = dq_part + (static_cast<long long>(j) * total_tokens + token) * d_model + head * HEAD_DIM + qcol;
 #pragma unroll
             for (int jj = 0; jj < HEAD_DIM / 8; ++jj)
                 *reinterpret_cast<uint32_t*>(dqp + 8 * jj) = pack_bf16x2(dq[4 * jj + 2 * h], dq[4 * jj + 2 * h + 1]);
         }
         named_bar_sync(1, NUM_THREADS);    // dS^T, Q_i, dO_i, lse / delta of this block are no longer read
-        if (tid == 0 && i + 2 < NUM_QB) load_q(i + 2);
+        if (tid == 0 && i + 2 < num_qb) load_q(i + 2);
     }
     // dK_j / dV_j
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
+        if (j * BLK + key_row + 8 * h >= seq_len) continue;
         const long long key = seq0 + j * BLK + key_row + 8 * h;
         bf16* dkp = dqkv + key * (3ll * d_model) + d_model + head * HEAD_DIM + qcol;
         bf16* dvp = dqkv + key * (3ll * d_model) + 2 * d_model + head * HEAD_DIM + qcol;
@@ -229,7 +247,7 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const bf16* __restrict_
     if (lane == 0) delta[w] = acc;
 }
 
-// epilogue: dQ = sum of the per-key-block partials, written as bf16 into the Q third of dqkv
+// epilogue: dQ = sum of the per-key-block partials in key-block order (deterministic), written as bf16 into the Q third of dqkv
 __global__ void __launch_bounds__(256) attn_dq_reduce_kernel(const bf16* __restrict__ dq_part, bf16* __restrict__ dqkv,
                                                              long long tokens, int d_model, int parts) {
     const long long i8 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;   // 8-element (16 B) index inside [T, D]
@@ -262,39 +280,44 @@ using namespace lah::attnb;
 extern "C" {
 
 // qkv [T, 3D] bf16 (forward input), out [T, D] bf16 (forward output), dout [T, D] bf16, lse2 [T, H] fp32 (forward output)
-// -> dqkv [T, 3D] bf16.  Scratch: delta [T, H] fp32 (rowsum(dout o out), computed here), dq_part [4, T, D] bf16 (the four
-// per-key-block partials of dQ, reduced into the Q third of dqkv here).  Three launches, no PyTorch ops around them.
+// -> dqkv [T, 3D] bf16, T = batch * seq_len, 1 <= seq_len <= MAX_SEQ (-2 otherwise, or when seq_len does not divide T).
+// Scratch: delta [T, H] fp32 (rowsum(dout o out), computed here), dq_part [ceil(seq_len / 128), T, D] bf16 (one partial
+// of dQ per key block, reduced into the Q third of dqkv here).  Three launches, no PyTorch ops around them.
 // drop_thr < 0: the forward ran without dropout; otherwise the same (seed, drop_thr, rescale) as lah_attention_fwd.
 int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
-                      void* dq_part, int batch, int num_heads, int d_model, unsigned long long seed, int drop_thr,
-                      float rescale, cudaStream_t st) {
+                      void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
+                      int drop_thr, float rescale, cudaStream_t st) {
     if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
     CUtensorMap tm_qkv, tm_do;
-    const uint32_t box[2] = {HEAD_DIM, BLK};
-    {
-        uint64_t dims[2] = {(uint64_t)3 * d_model, (uint64_t)batch * S_LEN};
-        uint64_t str[1] = {(uint64_t)3 * d_model * 2};
-        int r = make_tmap(&tm_qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, qkv, dims, str, box);
+    const uint32_t box[3] = {HEAD_DIM, BLK, 1};
+    {   // 3-D {columns, position in sequence, sequence}: a tile never crosses into the next sequence
+        uint64_t dims[3] = {(uint64_t)3 * d_model, (uint64_t)seq_len, (uint64_t)batch};
+        uint64_t str[2] = {(uint64_t)3 * d_model * 2, (uint64_t)seq_len * 3 * d_model * 2};
+        int r = make_tmap(&tm_qkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, qkv, dims, str, box);
         if (r) return r;
     }
     {
-        uint64_t dims[2] = {(uint64_t)d_model, (uint64_t)batch * S_LEN};
-        uint64_t str[1] = {(uint64_t)d_model * 2};
-        int r = make_tmap(&tm_do, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dout, dims, str, box);
+        uint64_t dims[3] = {(uint64_t)d_model, (uint64_t)seq_len, (uint64_t)batch};
+        uint64_t str[2] = {(uint64_t)d_model * 2, (uint64_t)seq_len * d_model * 2};
+        int r = make_tmap(&tm_do, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dout, dims, str, box);
         if (r) return r;
     }
     if (int e = set_max_dynamic_smem<attention_bwd_kernel<false>>(SMEM_TOTAL)) return e;
     if (int e = set_max_dynamic_smem<attention_bwd_kernel<true>>(SMEM_TOTAL)) return e;
-    if (batch <= 0) return 0;
     const float scale = 1.f / sqrtf((float)HEAD_DIM);
-    const long long tokens = (long long)batch * S_LEN, pairs = tokens * num_heads;
+    const int blocks = (seq_len + BLK - 1) / BLK;
+    const long long pairs = tokens * num_heads, ctas = batch * num_heads * blocks;
+    if (ctas > 0x7fffffffll) return -2;
     attn_delta_kernel<<<(unsigned)((pairs * 32 + 255) / 256), 256, 0, st>>>((const bf16*)dout, (const bf16*)out, delta, pairs);
     auto kern = drop_thr < 0 ? attention_bwd_kernel<false> : attention_bwd_kernel<true>;
-    kern<<<batch * num_heads * (S_LEN / BLK), NUM_THREADS, SMEM_TOTAL, st>>>(
-        tm_qkv, tm_do, lse2, delta, (bf16*)dqkv, (bf16*)dq_part, tokens, d_model, num_heads, scale,
+    kern<<<(unsigned)ctas, NUM_THREADS, SMEM_TOTAL, st>>>(
+        tm_qkv, tm_do, lse2, delta, (bf16*)dqkv, (bf16*)dq_part, tokens, d_model, num_heads, seq_len, scale,
         scale * 1.4426950408889634f, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale);
     attn_dq_reduce_kernel<<<(unsigned)((tokens * d_model / 8 + 255) / 256), 256, 0, st>>>((const bf16*)dq_part, (bf16*)dqkv, tokens, d_model,
-                                                                                         S_LEN / BLK);
+                                                                                         blocks);
     return -(int)cudaGetLastError();
 }
 

@@ -11,7 +11,8 @@ Expert architectures (the L1 "ops/models" layer of SURVEY.md).
   (``self_attn.in_proj_weight`` ..., ``linear1``, ``linear2``, ``norm1``, ``norm2``).  Its four dropouts (attention
   probabilities, ``dropout1``, ``dropout`` after the GELU, ``dropout2``) act in training mode, which is the mode
   ``ExpertBackend`` runs it in; the sm_90a executor (``runtime/native_executor.py``) implements them with in-kernel
-  Philox masks (DESIGN.md §9), so the reference's default ``name_to_block["transformer"]`` trains natively.
+  Philox masks (DESIGN.md §9), so the reference's default ``name_to_block["transformer"]`` trains natively.  Like
+  ``nn.MultiheadAttention`` it takes any sequence length; the sm_90a executor runs 1 <= S <= ``kernels.MAX_SEQ`` (65536).
 
 These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_90a execution of the same
 maths lives in ``lah_b200.parallel.engine`` (grouped wgmma GEMMs + fused LN/ReLU/Adam kernels).
@@ -62,7 +63,7 @@ class TransformerEncoderLayer(nn.Module):
         return x.transpose(0, 1)
 
 
-SEQ_LEN = 512  # the throughput experiment hard-codes 512-token sequences (reference layers.py:57)
+SEQ_LEN = 512  # input shape of the throughput experiment (reference layers.py:57); the layer itself takes any length
 
 name_to_block = {
     "ffn": lambda hid_dim: FeedforwardBlock(hid_dim),

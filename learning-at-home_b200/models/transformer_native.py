@@ -2,15 +2,16 @@
 sm_90a execution of the transformer expert (post-LN encoder layer, GELU; architecture of
 the reference's experiments/throughput/layers.py:22-51): QKV / out / MLP projections on the 128 x 256-tile wgmma GEMM with
 fused bias / GELU / residual epilogues, attention on csrc/attention.cu (S and P never leave the SM), LayerNorm on
-csrc/layernorm.cu.  Forward (inference / throughput experiment) only; training of transformer experts goes through the
-PyTorch module (``TransformerEncoderLayer`` + ``ExpertBackend``), which — unlike the reference's — is trainable.
-Dropout is the identity here (the throughput experiment is forward-only; see DESIGN.md).
+csrc/layernorm.cu.  Forward (inference / throughput experiment) only; training of transformer experts goes through
+``ExpertBackend``, whose sm_90a executor (runtime/native_executor.py) trains the same layer.  Dropout is the identity here
+(the throughput experiment is forward-only; see DESIGN.md).  Any sequence length 1 <= S <= kernels.MAX_SEQ: the token rows
+are padded with zeros to a multiple of 128 for the GEMM and LayerNorm kernels, and attention sees only the real rows.
 """
 import torch
 import torch.nn as nn
 
 from ..ops import gemm, kernels as K
-from .layers import TransformerEncoderLayer, SEQ_LEN
+from .layers import TransformerEncoderLayer
 
 
 class NativeTransformerLayer(nn.Module):
@@ -40,7 +41,8 @@ class NativeTransformerLayer(nn.Module):
         if ws is None:
             bf = dict(dtype=torch.bfloat16, device=device)
             d, ff = self.d_model, self.w1.shape[1]
-            ws = dict(qkv=torch.empty(tokens, 3 * d, **bf), att=torch.empty(tokens, d, **bf), h=torch.empty(tokens, d, **bf),
+            ws = dict(x=torch.empty(tokens, d, **bf), qkv=torch.empty(tokens, 3 * d, **bf), att=torch.empty(tokens, d, **bf),
+                      h=torch.empty(tokens, d, **bf),
                       x1=torch.empty(tokens, d, **bf), f=torch.empty(tokens, ff, **bf), y=torch.empty(tokens, d, **bf),
                       mean=torch.empty(tokens, device=device), rstd=torch.empty(tokens, device=device))
             self._ws = {tokens: ws}
@@ -48,19 +50,32 @@ class NativeTransformerLayer(nn.Module):
 
     @torch.no_grad()
     def forward(self, src, out=None):
-        """src: [batch, 512, d_model] (bf16 preferred); returns a bf16 tensor of the same shape"""
+        """src: [batch, S, d_model] (bf16 preferred), 1 <= S <= kernels.MAX_SEQ; returns a bf16 tensor of the same shape"""
         batch, seq, d = src.shape
-        assert seq == SEQ_LEN and d == self.d_model
-        x = src.reshape(batch * seq, d)
-        if x.dtype != torch.bfloat16 or not x.is_contiguous():
+        assert 1 <= seq <= K.MAX_SEQ and d == self.d_model, (tuple(src.shape), self.d_model)
+        rows = batch * seq
+        tokens = (rows + 127) // 128 * 128
+        x = src.reshape(rows, d)
+        ws = self._workspace(tokens, x.device)
+        if tokens > rows:   # zero padding rows; attention writes only the real rows of att
+            ws["x"][:rows].copy_(x)
+            ws["x"][rows:].zero_()
+            ws["att"][rows:].zero_()
+            x = ws["x"]
+        elif x.dtype != torch.bfloat16 or not x.is_contiguous():
             x = x.to(torch.bfloat16).contiguous()
-        ws = self._workspace(batch * seq, x.device)
         gemm.grouped_linear(x, self.w_in, bias=self.b_in, out=ws["qkv"])
-        K.attention_fwd(ws["qkv"], self.num_heads, out=ws["att"])
+        K.attention_fwd(ws["qkv"][:rows], self.num_heads, out=ws["att"][:rows], seq_len=seq)
         gemm.grouped_linear(ws["att"], self.w_out, bias=self.b_out, residual=x, out=ws["h"])
         K.ln_relu_fwd(ws["h"], self.g1, self.be1, None, out=ws["x1"], mean=ws["mean"], rstd=ws["rstd"], relu=False)
         gemm.grouped_linear(ws["x1"], self.w1, bias=self.b1, out=ws["f"], act=2)
         gemm.grouped_linear(ws["f"], self.w2, bias=self.b2, residual=ws["x1"], out=ws["y"])
-        out = torch.empty(batch * seq, d, dtype=torch.bfloat16, device=x.device) if out is None else out.view(batch * seq, d)
+        if tokens > rows:
+            res = torch.empty(tokens, d, dtype=torch.bfloat16, device=x.device)
+            K.ln_relu_fwd(ws["y"], self.g2, self.be2, None, out=res, mean=ws["mean"], rstd=ws["rstd"], relu=False)
+            res = res[:rows]
+            out = res if out is None else out.view(rows, d).copy_(res)
+            return out.view(batch, seq, d)
+        out = torch.empty(rows, d, dtype=torch.bfloat16, device=x.device) if out is None else out.view(rows, d)
         K.ln_relu_fwd(ws["y"], self.g2, self.be2, None, out=out, mean=ws["mean"], rstd=ws["rstd"], relu=False)
         return out.view(batch, seq, d)

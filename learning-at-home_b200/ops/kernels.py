@@ -54,8 +54,8 @@ def _lib():
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, P],
         "lah_bump_steps": [P, P, I, P],
         "lah_cast_bf16": [P, P, L, P],
-        "lah_attention_fwd": [P, P, P, I, I, I, c_ull, I, Fl, P],
-        "lah_attention_bwd": [P, P, P, P, P, P, P, I, I, I, c_ull, I, Fl, P],
+        "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
+        "lah_attention_bwd": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P],
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
         "lah_symm_alloc": [c_ull, ctypes.POINTER(c_void_p)],
@@ -262,45 +262,58 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
 # ---------------------------------------------------------------------------------------------------------
 # attention (transformer expert)
 # ---------------------------------------------------------------------------------------------------------
-def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None):
+MAX_SEQ = 65536   # longest sequence of the attention kernels (csrc/dropout.cuh MAX_SEQ)
+
+
+def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=512):
     """
-    Self-attention over 512-token sequences on wgmma (csrc/attention.cu).
-    :param qkv: [batch*512, 3*d_model] bf16 = in_proj output, [q | k | v] per token; head_dim must be 64
-    :param lse: optional fp32 [batch*512, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd); with
+    Self-attention over sequences of ``seq_len`` tokens (1 <= seq_len <= MAX_SEQ) on wgmma (csrc/attention.cu).
+    :param qkv: [batch*seq_len, 3*d_model] bf16 = in_proj output, [q | k | v] per token; head_dim must be 64
+    :param out: optional [batch*seq_len, d_model] bf16 destination (may be the leading rows of a larger buffer)
+    :param lse: optional fp32 [batch*seq_len, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd); with
         dropout it is still that of the undropped softmax
     :param dropout: (p, seed): O = (M o P) V / (1 - p) with the site-0 mask of ``dropout_mask``; p = 0 or None launches the
         kernel without dropout
-    :returns: [batch*512, d_model] bf16, heads concatenated (input of out_proj)
+    :returns: [batch*seq_len, d_model] bf16, heads concatenated (input of out_proj)
     """
     tokens, three_d = qkv.shape
     d_model = three_d // 3
-    assert qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and tokens % 512 == 0
+    assert qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.is_contiguous()
+    assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
     if out is None:
         out = torch.empty(tokens, d_model, dtype=torch.bfloat16, device=qkv.device)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (tokens, d_model)
     if lse is not None:
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == tokens * num_heads
     seed, thr, rescale = _dropout_args(dropout)
-    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens // 512, num_heads, d_model, seed, thr, rescale,
-                                          stream_ptr()), "lah_attention_fwd")
+    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed, thr,
+                                          rescale, stream_ptr()), "lah_attention_fwd")
     native.count_launch()
     return out
 
 
-def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None):
+def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, dqkv=None):
     """
     Backward of ``attention_fwd`` on wgmma (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
     dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.
+    Scratch: the per-key-block dQ partials, 2 * ceil(seq_len / 128) * tokens * d_model bytes (4x the bytes of dQ at 512
+    tokens, 32x at 4096), and the fp32 [tokens, num_heads] row sums Delta.
     :param dropout: the (p, seed) of the forward that produced ``out``; the mask is regenerated, not read
+    :param dqkv: optional contiguous [tokens, 3*d_model] bf16 destination
     """
     tokens, three_d = qkv.shape
     d_model = three_d // 3
     assert dout.dtype == torch.bfloat16 and dout.is_contiguous() and out.is_contiguous() and lse.dtype == torch.float32
     assert out.dtype == torch.bfloat16 and qkv.is_contiguous()
+    assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
     delta = torch.empty(tokens, num_heads, dtype=torch.float32, device=qkv.device)      # rowsum(dout o out), filled by the prologue kernel
-    dqkv = torch.empty_like(qkv)
-    dq_part = torch.empty(4, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
+    if dqkv is None:
+        dqkv = torch.empty_like(qkv)
+    assert dqkv.dtype == torch.bfloat16 and dqkv.is_contiguous() and dqkv.shape == qkv.shape
+    blocks = (seq_len + 127) // 128
+    dq_part = torch.empty(blocks, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
     native.check(_lib().lah_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
-                                          tokens // 512, num_heads, d_model, *_dropout_args(dropout), stream_ptr()),
+                                          tokens, int(seq_len), num_heads, d_model, *_dropout_args(dropout), stream_ptr()),
                  "lah_attention_bwd")
     native.count_launch(3)   # delta prologue, wgmma backward, dQ partial reduction
     return dqkv
@@ -404,24 +417,34 @@ def philox4x32_10_ref(ctr, key):
     return c
 
 
-def dropout_keep_ref(p, seed, site, *index):
+def dropout_counter_ref(site, *index):
     """
-    Independent CPU definition of the keep decision (the mask definition of csrc/dropout.cuh): ``index`` are broadcastable
-    integer tensors, (batch, head, query, key) for site 0 and (row, col) for sites 1-3.  Returns a bool tensor.
+    The Philox counter (four int64 tensors holding uint32 words) and the lane (0..7) of the keep decision at ``index``
+    (csrc/dropout.cuh): ``index`` are broadcastable integer tensors, (batch, head, query, key) for site 0 and (row, col)
+    for sites 1-3.
     """
     idx = torch.broadcast_tensors(*[torch.as_tensor(t, dtype=torch.int64) for t in index])
-    seed = int(seed) & (2 ** 64 - 1)
     zero = torch.zeros_like(idx[0])
     if site == SITE_ATTN:
         b, h, q, k = idx
         gq, gk = (q >> 4) * 4 + ((q >> 1) & 3), (k >> 4) * 4 + ((k >> 1) & 3)
-        ctr = ((gq * 128 + gk) | ((q & 1) << 14), h, b, zero)
+        ctr = ((((gq & 127) * 128) + (gk & 127)) | ((q & 1) << 14), h, b, ((gq >> 7) << 8) | ((gk >> 7) << 20) | SITE_ATTN)
         lane = ((q >> 3) & 1) * 4 + ((k & 1) | (((k >> 3) & 1) << 1))
     else:
         r, n = idx
         gr, gn = (r >> 4) * 8 + (r & 7), (n >> 4) * 4 + ((n >> 1) & 3)
         ctr = (gn, gr, zero, zero + site)
         lane = ((r >> 3) & 1) * 4 + ((n & 1) | (((n >> 3) & 1) << 1))
+    return ctr, lane
+
+
+def dropout_keep_ref(p, seed, site, *index):
+    """
+    Independent CPU definition of the keep decision (the mask definition of csrc/dropout.cuh): ``index`` are broadcastable
+    integer tensors, (batch, head, query, key) for site 0 and (row, col) for sites 1-3.  Returns a bool tensor.
+    """
+    ctr, lane = dropout_counter_ref(site, *index)
+    seed = int(seed) & (2 ** 64 - 1)
     words = torch.stack(philox4x32_10_ref(ctr, (seed & _U32, seed >> 32)), dim=-1)
     w = words.gather(-1, (lane >> 1).unsqueeze(-1)).squeeze(-1)
     u16 = torch.where((lane & 1) == 1, w >> 16, w & 0xFFFF)

@@ -58,7 +58,8 @@ class ExpertBackend(nn.Module):
 
     # ------------------------------------------------------------------ tasks
     def native_executor(self, inputs):
-        """the sm_90a executor of this expert, or None (CPU tensors, unsupported expert / optimizer, no GPU)"""
+        """the sm_90a executor of this expert, or None (CPU tensors, unsupported expert / optimizer, no GPU).  Inputs the
+        executor does not accept (``executor.accepts``: rank, feature size, sequence length) run on the module itself."""
         if not self.native or len(inputs) < 1 or not inputs[0].is_cuda or self.kwargs_schema or len(self.args_schema) != 1:
             return None
         first = next(self.expert.parameters(), None)
@@ -72,7 +73,7 @@ class ExpertBackend(nn.Module):
 
     def forward(self, *inputs: torch.Tensor) -> Tuple[torch.Tensor, ...]:
         executor = self.native_executor(inputs)
-        if executor is not None and inputs[0].dim() == executor.INPUT_DIMS:
+        if executor is not None and executor.accepts(inputs[0]):
             return (executor.forward(inputs[0]),)
         args, kwargs = nested_pack(inputs, structure=self.forward_schema)
         with torch.no_grad():
@@ -81,7 +82,7 @@ class ExpertBackend(nn.Module):
 
     def backward(self, *inputs: torch.Tensor) -> Tuple[torch.Tensor, ...]:
         executor = self.native_executor(inputs)
-        if executor is not None and len(inputs) == 2 and inputs[0].dim() == executor.INPUT_DIMS:
+        if executor is not None and len(inputs) == 2 and executor.accepts(inputs[0]):
             grad_x = executor.backward(inputs[0], inputs[1].to(inputs[0].device))   # dgrad + fused wgrad/AMSGrad: one update
             self.update_count += 1
             return (grad_x,)

@@ -27,6 +27,10 @@ ALIGN = 16
 class NativeFFNExecutor:
     INPUT_DIMS = 2   # [rows, hid]
 
+    def accepts(self, x) -> bool:
+        """True when ``x`` is an input this executor runs: [rows, hid]"""
+        return x.dim() == self.INPUT_DIMS and x.shape[1] == self.hid
+
     @staticmethod
     def supports(expert, opt) -> bool:
         if not isinstance(expert, FeedforwardBlock) or not torch.cuda.is_available():
@@ -183,7 +187,14 @@ def draw_dropout_seed() -> int:
 class NativeTransformerExecutor:
     """
     Trainable sm_90a transformer expert (post-LN encoder layer of the reference's experiments/throughput/layers.py:22-51,
-    batch-first [B, 512, d], head_dim 64, every dropout probability in [0, 1) — the reference's block cannot be trained).
+    batch-first [B, S, d] with any sequence length 1 <= S <= K.MAX_SEQ, head_dim 64, every dropout probability in [0, 1) —
+    the reference's block cannot be trained).
+
+    Sequences: the token dimension B*S is padded with zero rows to a multiple of 128 for the GEMM, LayerNorm and dropout
+    kernels; attention sees only the B*S real rows and is told S.  Padding rows contribute exactly zero to every parameter
+    gradient: their output gradient is zero, so every gradient row the backward forms for them is zero, except the rows of
+    dqkv, which attention_bwd does not write and which are zeroed before the in_proj bias and weight gradients.  Dropout
+    sites 1-3 index token row b*S + s, as an unpadded layer would.
 
       forward   in_proj GEMM -> wgmma flash attention (emits the row log-sum-exp; attention dropout in-kernel) -> out_proj
                 GEMM (+bias, dropout1, +residual) -> LayerNorm -> linear1 GEMM -> GELU (+dropout: csrc/dropout.cu) ->
@@ -204,11 +215,15 @@ class NativeTransformerExecutor:
     keep the reference key names: self_attn.in_proj_weight, linear1.weight, norm1.weight, ...).
     """
     NAMES = ("w_in", "b_in", "w_out", "b_out", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
-    INPUT_DIMS = 3   # [batch, 512, d_model]
+    INPUT_DIMS = 3   # [batch, seq, d_model]
+
+    def accepts(self, x) -> bool:
+        """True when ``x`` is an input this executor runs: [batch, S, d_model] with 1 <= S <= K.MAX_SEQ"""
+        return x.dim() == self.INPUT_DIMS and x.shape[2] == self.d and 1 <= x.shape[1] <= K.MAX_SEQ
 
     @staticmethod
     def supports(expert, opt) -> bool:
-        from ..models.layers import TransformerEncoderLayer, SEQ_LEN  # noqa
+        from ..models.layers import TransformerEncoderLayer
         if not isinstance(expert, TransformerEncoderLayer) or not torch.cuda.is_available():
             return False
         attn = expert.self_attn
@@ -293,6 +308,7 @@ class NativeTransformerExecutor:
         K.cast_bf16(self.p, self.p_bf16)
 
     def _workspace(self, T):
+        """buffers for T padded token rows (T a multiple of 128)"""
         ws = self._ws.get(T)
         if ws is None:
             bf = dict(dtype=torch.bfloat16, device=self.device)
@@ -313,15 +329,21 @@ class NativeTransformerExecutor:
         return (drop[1][site], drop[0]) if site == K.SITE_ATTN else (drop[1][site], drop[0], site)
 
     def _forward(self, src, drop=None):
+        """returns the workspace, the real token rows Tr = batch * seq and the padded rows T (a multiple of 128)"""
         from ..ops import gemm
+        assert self.accepts(src), (tuple(src.shape), self.d)
         batch, seq, d = src.shape
-        assert seq == 512 and d == self.d
-        T = batch * seq
+        Tr = batch * seq
+        T = (Tr + 127) // 128 * 128
         ws = self._workspace(T)
-        ws["x"].copy_(src.reshape(T, d))
+        ws["x"][:Tr].copy_(src.reshape(Tr, d))
+        if T > Tr:
+            ws["x"][Tr:].zero_()
+            ws["att"][Tr:].zero_()   # attention writes only the real rows
         x, bv, pv, site = ws["x"], self.bv, self.pv, self._site
         gemm.grouped_linear(x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
-        K.attention_fwd(ws["qkv"], self.heads, out=ws["att"], lse=ws["lse"], dropout=site(drop, K.SITE_ATTN))
+        K.attention_fwd(ws["qkv"][:Tr], self.heads, out=ws["att"][:Tr], lse=ws["lse"][:Tr], dropout=site(drop, K.SITE_ATTN),
+                        seq_len=seq)
         gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"],
                             dropout=site(drop, K.SITE_OUT_PROJ))
         K.ln_relu_fwd(ws["h"], pv["g1"], pv["be1"], None, out=ws["x1"], mean=ws["stats"][0], rstd=ws["stats"][1], relu=False)
@@ -331,22 +353,27 @@ class NativeTransformerExecutor:
         gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["x1"], out=ws["y"],
                             dropout=site(drop, K.SITE_LINEAR2))
         K.ln_relu_fwd(ws["y"], pv["g2"], pv["be2"], None, out=ws["out"], mean=ws["stats"][2], rstd=ws["stats"][3], relu=False)
-        return ws, T
+        return ws, Tr, T
 
     @torch.no_grad()
     def forward(self, src: torch.Tensor) -> torch.Tensor:
-        ws, T = self._forward(src, self._dropout())
-        return ws["out"].view(src.shape).to(src.dtype)
+        ws, Tr, T = self._forward(src, self._dropout())
+        return ws["out"][:Tr].view(src.shape).to(src.dtype)
 
     @torch.no_grad()
     def backward(self, src: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
         from ..ops import gemm
         drop = self._dropout()
-        ws, T = self._forward(src, drop)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
+        ws, Tr, T = self._forward(src, drop)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
         d, bv, pv, gv, site = self.d, self.bv, self.pv, self.gv, self._site
         go = ws["group_off"]
         bf = dict(dtype=torch.bfloat16, device=self.device)
-        dout = grad_out.reshape(T, d).to(torch.bfloat16).contiguous()
+        seq = src.shape[1]
+        if T > Tr:   # zero gradient on the padding rows
+            dout = torch.zeros(T, d, **bf)
+            dout[:Tr].copy_(grad_out.reshape(Tr, d))
+        else:
+            dout = grad_out.reshape(T, d).to(torch.bfloat16).contiguous()
 
         def branch_grad(dres, drop_site, bias_grad):
             """gradient of a Linear whose output went through dropout `drop_site` into a residual sum: M o dres / (1 - p)
@@ -378,7 +405,13 @@ class NativeTransformerExecutor:
         dhb = branch_grad(dh, K.SITE_OUT_PROJ, gv["b_out"])
         gemm.grouped_wgrad(dhb, ws["att"], go, 1, out=gv["w_out"])
         datt = gemm.grouped_linear(dhb, bv["w_out"], w_is_kn=True)
-        dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN))
+        if T > Tr:   # attention_bwd does not write the padding rows
+            dqkv = torch.empty(T, 3 * d, **bf)
+            dqkv[Tr:].zero_()
+            K.attention_bwd(ws["qkv"][:Tr], ws["att"][:Tr], datt[:Tr], ws["lse"][:Tr], self.heads, dropout=site(drop, K.SITE_ATTN),
+                            seq_len=seq, dqkv=dqkv[:Tr])
+        else:
+            dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN), seq_len=seq)
         K.grouped_colsum(dqkv, None, out=gv["b_in"])
         gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"])
         dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh)
@@ -391,7 +424,7 @@ class NativeTransformerExecutor:
         step_t = torch.tensor(float(self.steps_host))
         for param in self.params:
             self.opt.state[param]["step"] = step_t
-        return dx.view(src.shape).to(src.dtype)
+        return dx[:Tr].view(src.shape).to(src.dtype)
 
 
 def make_executor(expert, opt):
