@@ -1,5 +1,5 @@
-// attention.cu — wgmma self-attention for the transformer expert (head_dim 64, any sequence length S in 1..MAX_SEQ;
-// reference: nn.MultiheadAttention inside experiments/throughput/layers.py:22-51).
+// attention.cu — wgmma self-attention for the transformer expert (head_dim HD = 32, 64 or 128, any sequence length S in
+// 1..MAX_SEQ; reference: nn.MultiheadAttention inside experiments/throughput/layers.py:22-51).
 //
 // FORWARD (this file): flash attention.  One CTA owns one 128-query tile of one (batch, head); two consumer warpgroups own
 // 64 query rows each.  K / V stream through a 2-stage TMA pipeline in 128-key blocks; per block S = Q K^T is computed by
@@ -10,6 +10,13 @@
 //
 // Input : qkv [T = batch*S, 3*D] bf16 (output of the fused in_proj GEMM: [q | k | v] per token, heads contiguous)
 // Output: out [T, D] bf16 (heads concatenated, ready for out_proj); lse2 [T, heads] fp32 (optional)
+//
+// Head dim: HD is a template parameter; the entry point dispatches on D / heads.  A tile row of a head is stored as swizzle
+// atoms of 64 columns (128 B, 128B swizzle) or, at HD = 32, one atom of 32 columns (64 B, 64B swizzle: the head is never
+// padded, since 64 columns would reach into the next head).  HD = 128 loads each 128-row tile as two 64-column atoms (two TMA
+// boxes), runs the S MMA in 8 k16 steps across them and P V as m64n128 with V MN-major across the two atoms (LBO = one
+// atom).  Shared memory: Q + 2 stages of K and V = 5 tiles of 128 x HD bf16 (40 / 80 / 160 KB).  Registers per thread: S 64,
+// O HD / 2, P 32.
 //
 // Sequence length: ceil(S / 128) query tiles and key blocks per sequence.  The tensor map is 3-D {3*D, S, batch}, so TMA
 // zero-fills the rows past the end of a sequence and no tile reads the next one.  In the last key block of a partial
@@ -23,31 +30,44 @@
 namespace lah {
 namespace attn {
 
-constexpr int HEAD_DIM = 64;
 constexpr int Q_TILE = 128;
 
 namespace v2 {
 
 constexpr int KB = 128;                       // keys per block
 constexpr int NUM_THREADS2 = 256;             // two consumer warpgroups; thread 0 also drives TMA
-constexpr int TILE_BYTES = 128 * HEAD_DIM * 2;            // 16 KB: a 128 x 64 bf16 tile (Q tile, K block, V block)
-constexpr int OFF_Q2 = 0;
-constexpr int OFF_K2 = OFF_Q2 + TILE_BYTES;               // 2 stages
-constexpr int OFF_V2 = OFF_K2 + 2 * TILE_BYTES;           // 2 stages
-constexpr int OFF_BAR2 = OFF_V2 + 2 * TILE_BYTES;
 constexpr int NUM_BARS = 1 + 2;
-constexpr int SMEM_TOTAL2 = OFF_BAR2 + NUM_BARS * 8 + 16 + 1024;
+
+// shared-memory layout of one head dim: a 128 x HD bf16 tile (Q tile, K block, V block) is HD / ATOM_COLS atoms of
+// [128 rows][ATOM_COLS columns], each loaded by one TMA box
+template <int HD>
+struct Fwd {
+    static_assert(HD == 32 || HD == 64 || HD == 128, "head_dim 32, 64 or 128");
+    static constexpr int ATOM_COLS = HD < 64 ? HD : 64;
+    static constexpr int ATOMS = HD / ATOM_COLS;
+    static constexpr int ROW_BYTES = ATOM_COLS * 2;
+    static constexpr int ATOM_BYTES = 128 * ROW_BYTES;
+    static constexpr int TILE_BYTES = 128 * HD * 2;           // 8 / 16 / 32 KB
+    static constexpr int OFF_Q2 = 0;
+    static constexpr int OFF_K2 = OFF_Q2 + TILE_BYTES;        // 2 stages
+    static constexpr int OFF_V2 = OFF_K2 + 2 * TILE_BYTES;    // 2 stages
+    static constexpr int OFF_BAR2 = OFF_V2 + 2 * TILE_BYTES;
+    static constexpr int SMEM_TOTAL2 = OFF_BAR2 + NUM_BARS * 8 + 16 + 1024;
+};
 
 // DROP: attention dropout (dropout.cuh, site 0).  The kept bf16 probabilities feed O += P V; the row sum l (and so the LSE)
 // keeps summing ALL of them, and 1 / (1 - p) is folded into the final 1 / l.
-template <bool DROP>
+template <int HD, bool DROP>
 __global__ void __launch_bounds__(NUM_THREADS2, 1)
 attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, float* __restrict__ lse2,
                         int d_model, int num_heads, int seq_len, float scale_log2e, unsigned long long seed, uint32_t thr,
                         float rescale) {
+    using C = Fwd<HD>;
+    constexpr int TILE_BYTES = C::TILE_BYTES, OFF_Q2 = C::OFF_Q2, OFF_K2 = C::OFF_K2, OFF_V2 = C::OFF_V2;
+    constexpr int KSTEPS_PER_ATOM = C::ATOM_COLS / 16;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR2);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR2);
     uint64_t* bar_q = bars;
     uint64_t* kv_full = bars + 1;   // [2]
 
@@ -57,11 +77,16 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     const int head = (blockIdx.x / num_kb) % num_heads;
     const int batch = (blockIdx.x / num_kb) / num_heads;
 
+    // one 128-row tile of HD columns starting at column c0: one TMA box per atom
+    auto load_tile = [&](uint8_t* dst, uint64_t* bar, int c0, int row) {
+        tma_load_3d(dst, &tm_qkv, bar, c0, row, batch);
+        if constexpr (C::ATOMS == 2) tma_load_3d(dst + C::ATOM_BYTES, &tm_qkv, bar, c0 + 64, row, batch);
+    };
     auto load_kv = [&](int j) {   // thread 0 only; stage j & 1 must be free
         const int st = j & 1;
         mbar_arrive_expect_tx(&kv_full[st], 2 * TILE_BYTES);
-        tma_load_3d(smem + OFF_K2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], d_model + head * HEAD_DIM, j * KB, batch);
-        tma_load_3d(smem + OFF_V2 + st * TILE_BYTES, &tm_qkv, &kv_full[st], 2 * d_model + head * HEAD_DIM, j * KB, batch);
+        load_tile(smem + OFF_K2 + st * TILE_BYTES, &kv_full[st], d_model + head * HD, j * KB);
+        load_tile(smem + OFF_V2 + st * TILE_BYTES, &kv_full[st], 2 * d_model + head * HD, j * KB);
     };
     if (tid == 0) {
         tma_prefetch_desc(&tm_qkv);
@@ -70,16 +95,16 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         mbar_init(&kv_full[1], 1);
         fence_mbar_init();
         mbar_arrive_expect_tx(bar_q, TILE_BYTES);
-        tma_load_3d(smem + OFF_Q2, &tm_qkv, bar_q, head * HEAD_DIM, qt * Q_TILE, batch);
+        load_tile(smem + OFF_Q2, bar_q, head * HD, qt * Q_TILE);
         load_kv(0);
         if (num_kb > 1) load_kv(1);
     }
     __syncthreads();
 
-    const uint32_t sq = smem_u32(smem + OFF_Q2) + wg * (64 * 128);   // this warpgroup's 64 query rows
-    float o[HEAD_DIM / 2];
+    const uint32_t sq = smem_u32(smem + OFF_Q2) + wg * (64 * C::ROW_BYTES);   // this warpgroup's 64 query rows
+    float o[HD / 2];
 #pragma unroll
-    for (int i = 0; i < HEAD_DIM / 2; ++i) o[i] = 0.f;
+    for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
     // m = running row maximum (raw score units), l = this thread's share of the row sum (reduced over the quad at the end)
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(bar_q, 0);
@@ -91,9 +116,11 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         float s[KB / 2];
         wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < HEAD_DIM / 16; ++ks)
-            wgmma_bf16_n128<0, 0>(s, make_smem_desc_sw128(sq + ks * 32, 0, 1024), make_smem_desc_sw128(sk + ks * 32, 0, 1024),
-                                  ks > 0 ? 1u : 0u);
+        for (int ks = 0; ks < HD / 16; ++ks) {   // k16 step ks: atom ks / KSTEPS_PER_ATOM, 32 B into its swizzle row
+            const uint32_t koff = (ks / KSTEPS_PER_ATOM) * C::ATOM_BYTES + (ks % KSTEPS_PER_ATOM) * 32;
+            wgmma_bf16_n128<0, 0>(s, make_smem_desc_cols<C::ATOM_COLS>(sq + koff, 0),
+                                  make_smem_desc_cols<C::ATOM_COLS>(sk + koff, 0), ks > 0 ? 1u : 0u);
+        }
         wgmma_commit();
         // keep bits of this thread's 64 scores, bit i <-> s[i], generated while the S MMA runs: one Philox granule per
         // 16-key chunk kc covers rows {g, g+8} x keys {2c, 2c+1, 2c+8, 2c+9} = s[8kc .. 8kc+7]
@@ -148,15 +175,16 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
             }
             l[h] = l[h] * alpha + sum;
 #pragma unroll
-            for (int jj = 0; jj < HEAD_DIM / 8; ++jj) {
+            for (int jj = 0; jj < HD / 8; ++jj) {
                 o[4 * jj + 2 * h] *= alpha;
                 o[4 * jj + 2 * h + 1] *= alpha;
             }
         }
         wgmma_fence();
 #pragma unroll
-        for (int kc = 0; kc < KB / 16; ++kc)   // V block as an MN-major B operand: 16 keys = 16 rows of 128 B per step
-            wgmma_bf16_rs_n64<1>(o, pa[kc], make_smem_desc_sw128(sv + kc * 2048, 0, 1024), 1u);
+        for (int kc = 0; kc < KB / 16; ++kc)   // V block as an MN-major B operand: 16 keys = 16 rows per step, atoms ATOM_BYTES apart
+            wgmma_bf16_rs<HD, 1>(o, pa[kc],
+                                 make_smem_desc_cols<C::ATOM_COLS>(sv + kc * 16 * C::ROW_BYTES, C::ATOMS > 1 ? C::ATOM_BYTES : 0), 1u);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(o);
@@ -175,11 +203,36 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         if (q >= seq_len) continue;
         const long long token = static_cast<long long>(batch) * seq_len + q;
         if (lse2 && (lane & 3) == 0) lse2[token * num_heads + head] = m[h] * scale_log2e + log2f(lt);
-        bf16* op = out + token * d_model + head * HEAD_DIM + 2 * (lane & 3);
+        bf16* op = out + token * d_model + head * HD + 2 * (lane & 3);
 #pragma unroll
-        for (int jj = 0; jj < HEAD_DIM / 8; ++jj)
+        for (int jj = 0; jj < HD / 8; ++jj)
             *reinterpret_cast<uint32_t*>(op + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
     }
+}
+
+template <int HD>
+int launch_fwd(const void* qkv, void* out, float* lse2, long long batch, int seq_len, int num_heads, int d_model,
+               unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
+    using C = Fwd<HD>;
+    CUtensorMap tm;
+    {   // 3-D {columns, position in sequence, sequence}: a tile never crosses into the next sequence
+        uint64_t dims[3] = {(uint64_t)3 * d_model, (uint64_t)seq_len, (uint64_t)batch};
+        uint64_t str[2] = {(uint64_t)3 * d_model * 2, (uint64_t)seq_len * 3 * d_model * 2};
+        uint32_t box[3] = {C::ATOM_COLS, 128, 1};
+        int r = make_tmap(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, qkv, dims, str, box,
+                          C::ATOM_COLS == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
+        if (r) return r;
+    }
+    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false>>(C::SMEM_TOTAL2)) return e;
+    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true>>(C::SMEM_TOTAL2)) return e;
+    const float scale_log2e = 1.4426950408889634f / sqrtf((float)HD);
+    const long long ctas = batch * num_heads * ((seq_len + Q_TILE - 1) / Q_TILE);
+    if (ctas > 0x7fffffffll) return -2;
+    auto kern = drop_thr < 0 ? attention_fwd_v2_kernel<HD, false> : attention_fwd_v2_kernel<HD, true>;
+    kern<<<(unsigned)ctas, NUM_THREADS2, C::SMEM_TOTAL2, st>>>(
+        tm, (bf16*)out, lse2, d_model, num_heads, seq_len, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr),
+        rescale);
+    return -(int)cudaGetLastError();
 }
 
 }  // namespace v2
@@ -193,32 +246,20 @@ using namespace lah::attn;
 extern "C" {
 
 // qkv: [tokens, 3*d_model] bf16, tokens = batch * seq_len, 1 <= seq_len <= MAX_SEQ; out: [tokens, d_model] bf16;
-// lse2: [tokens, heads] fp32 or NULL.  Returns -2 for a sequence length out of range or one that does not divide tokens.
+// lse2: [tokens, heads] fp32 or NULL.  Returns -2 for a head dim d_model / num_heads other than 32, 64 or 128 (or heads that
+// do not divide d_model), a sequence length out of range or one that does not divide tokens.
 // drop_thr < 0: no dropout; otherwise attention dropout with threshold drop_thr (dropout.cuh), seed, rescale = 1 / (1 - p)
 int lah_attention_fwd(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
                       unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
-    if (d_model != num_heads * HEAD_DIM || drop_thr > 65535) return -2;
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
     if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
     const long long batch = tokens / seq_len;
     if (batch == 0) return 0;
-    CUtensorMap tm;
-    {   // 3-D {columns, position in sequence, sequence}: a tile never crosses into the next sequence
-        uint64_t dims[3] = {(uint64_t)3 * d_model, (uint64_t)seq_len, (uint64_t)batch};
-        uint64_t str[2] = {(uint64_t)3 * d_model * 2, (uint64_t)seq_len * 3 * d_model * 2};
-        uint32_t box[3] = {HEAD_DIM, 128, 1};
-        int r = make_tmap(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, qkv, dims, str, box);
-        if (r) return r;
-    }
-    if (int e = set_max_dynamic_smem<v2::attention_fwd_v2_kernel<false>>(v2::SMEM_TOTAL2)) return e;
-    if (int e = set_max_dynamic_smem<v2::attention_fwd_v2_kernel<true>>(v2::SMEM_TOTAL2)) return e;
-    const float scale_log2e = 1.4426950408889634f / sqrtf((float)HEAD_DIM);
-    const long long ctas = batch * num_heads * ((seq_len + Q_TILE - 1) / Q_TILE);
-    if (ctas > 0x7fffffffll) return -2;
-    auto kern = drop_thr < 0 ? v2::attention_fwd_v2_kernel<false> : v2::attention_fwd_v2_kernel<true>;
-    kern<<<(unsigned)ctas, v2::NUM_THREADS2, v2::SMEM_TOTAL2, st>>>(
-        tm, (bf16*)out, lse2, d_model, num_heads, seq_len, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr),
-        rescale);
-    return -(int)cudaGetLastError();
+    if (hd == 32) return v2::launch_fwd<32>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st);
+    if (hd == 64) return v2::launch_fwd<64>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st);
+    return v2::launch_fwd<128>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st);
 }
 
 }  // extern "C"

@@ -171,6 +171,15 @@ __device__ __forceinline__ void wgmma_bf16_n256(float (&d)[128], uint64_t da, ui
 }
 
 template <int TB>
+__device__ __forceinline__ void wgmma_bf16_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB));
+}
+
+template <int TB>
 __device__ __forceinline__ void wgmma_bf16_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
     asm volatile(
         "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
@@ -188,6 +197,22 @@ __device__ __forceinline__ void wgmma_bf16_rs_n128(float (&d)[64], const uint32_
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB));
 }
 
+// the m64nNk16 forms above picked by N (32, 64 or 128; d holds N / 2 accumulators): A from shared memory / from registers
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 128, "N");
+    if constexpr (N == 32) wgmma_bf16_n32<TA, TB>(d, da, db, accumulate);
+    else if constexpr (N == 64) wgmma_bf16_n64<TA, TB>(d, da, db, accumulate);
+    else wgmma_bf16_n128<TA, TB>(d, da, db, accumulate);
+}
+template <int N, int TB>
+__device__ __forceinline__ void wgmma_bf16_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 128, "N");
+    if constexpr (N == 32) wgmma_bf16_rs_n32<TB>(d, a, db, accumulate);
+    else if constexpr (N == 64) wgmma_bf16_rs_n64<TB>(d, a, db, accumulate);
+    else wgmma_bf16_rs_n128<TB>(d, a, db, accumulate);
+}
+
 // ----------------------------------------------------------------------------------------------
 // shared-memory matrix descriptor (sm_90 layout), 128B swizzle
 //   [0,14) addr>>4   [16,30) LBO>>4   [32,46) SBO>>4   [62,64) layout=1 (SWIZZLE_128B)
@@ -201,6 +226,27 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
     d |= static_cast<uint64_t>(1) << 62;
     return d;
+}
+
+// 64B swizzle (layout type 2): the atom is 8 rows of 64 B, i.e. 32 bf16 columns (tensor maps with CU_TENSOR_MAP_SWIZZLE_64B)
+// K-major: SBO = 512 (8 rows x 64 B), LBO unused, advance 32 B per k16 step inside the swizzle row.
+// MN-major: SBO = 512 (8 k-rows), LBO = bytes between 32-wide MN atoms, advance 16 k-rows = 1024 B per k16 step.
+__device__ __forceinline__ uint64_t make_smem_desc_sw64(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
+    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
+    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
+    d |= static_cast<uint64_t>(2) << 62;
+    return d;
+}
+
+// descriptor of a bf16 tile stored as atoms COLS (32 or 64) columns wide, i.e. rows of 64 B (64B swizzle) or 128 B (128B
+// swizzle); SBO is the dense 8-row stride of that swizzle
+template <int COLS>
+__device__ __forceinline__ uint64_t make_smem_desc_cols(uint32_t saddr, uint32_t lbo_bytes) {
+    static_assert(COLS == 32 || COLS == 64, "atoms are 32 or 64 bf16 columns wide");
+    if constexpr (COLS == 32) return make_smem_desc_sw64(saddr, lbo_bytes, 512);
+    else return make_smem_desc_sw128(saddr, lbo_bytes, 1024);
 }
 
 // named barrier over a subset of the CTA's warps (id 0 is __syncthreads)

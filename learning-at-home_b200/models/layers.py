@@ -12,7 +12,9 @@ Expert architectures (the L1 "ops/models" layer of SURVEY.md).
   probabilities, ``dropout1``, ``dropout`` after the GELU, ``dropout2``) act in training mode, which is the mode
   ``ExpertBackend`` runs it in; the sm_90a executor (``runtime/native_executor.py``) implements them with in-kernel
   Philox masks (DESIGN.md §9), so the reference's default ``name_to_block["transformer"]`` trains natively.  Like
-  ``nn.MultiheadAttention`` it takes any sequence length; the sm_90a executor runs 1 <= S <= ``kernels.MAX_SEQ`` (65536).
+  ``nn.MultiheadAttention`` it takes any sequence length; the sm_90a executor runs 1 <= S <= ``kernels.MAX_SEQ`` (65536)
+  and head dims ``d_model / nhead`` in ``kernels.HEAD_DIMS`` = (32, 64, 128), so ``name_to_block["transformer"](hid_dim)``
+  (nhead 16) trains natively at hid_dim 512, 1024 and 2048.
 
 These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_90a execution of the same
 maths lives in ``lah_b200.parallel.engine`` (grouped wgmma GEMMs + fused LN/ReLU/Adam kernels).

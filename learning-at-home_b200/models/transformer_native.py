@@ -20,7 +20,8 @@ class NativeTransformerLayer(nn.Module):
         device = device or torch.device("cuda", torch.cuda.current_device())
         attn = layer.self_attn
         self.d_model, self.num_heads = attn.embed_dim, attn.num_heads
-        assert self.d_model // self.num_heads == 64, "the attention kernel is specialised for head_dim = 64"
+        assert self.d_model % self.num_heads == 0 and self.d_model // self.num_heads in K.HEAD_DIMS, \
+            f"the attention kernels run head_dim {K.HEAD_DIMS}, not {self.d_model} / {self.num_heads}"
 
         def w(t):  # [1, N, K] bf16: the grouped GEMM with a single group
             return t.detach().to(device=device, dtype=torch.bfloat16).unsqueeze(0).contiguous()

@@ -263,12 +263,14 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
 # attention (transformer expert)
 # ---------------------------------------------------------------------------------------------------------
 MAX_SEQ = 65536   # longest sequence of the attention kernels (csrc/dropout.cuh MAX_SEQ)
+HEAD_DIMS = (32, 64, 128)   # head dims d_model / num_heads of the attention kernels (csrc/attention.cu, attention_bwd.cu)
 
 
 def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=512):
     """
     Self-attention over sequences of ``seq_len`` tokens (1 <= seq_len <= MAX_SEQ) on wgmma (csrc/attention.cu).
-    :param qkv: [batch*seq_len, 3*d_model] bf16 = in_proj output, [q | k | v] per token; head_dim must be 64
+    :param qkv: [batch*seq_len, 3*d_model] bf16 = in_proj output, [q | k | v] per token; num_heads must divide d_model and
+        the head dim d_model / num_heads must be in HEAD_DIMS
     :param out: optional [batch*seq_len, d_model] bf16 destination (may be the leading rows of a larger buffer)
     :param lse: optional fp32 [batch*seq_len, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd); with
         dropout it is still that of the undropped softmax
@@ -280,6 +282,7 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=5
     d_model = three_d // 3
     assert qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.is_contiguous()
     assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
+    assert num_heads > 0 and d_model % num_heads == 0 and d_model // num_heads in HEAD_DIMS, (d_model, num_heads)
     if out is None:
         out = torch.empty(tokens, d_model, dtype=torch.bfloat16, device=qkv.device)
     assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (tokens, d_model)
@@ -295,7 +298,8 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=5
 def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, dqkv=None):
     """
     Backward of ``attention_fwd`` on wgmma (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
-    dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.
+    dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.  Same head dims as
+    ``attention_fwd``.
     Scratch: the per-key-block dQ partials, 2 * ceil(seq_len / 128) * tokens * d_model bytes (4x the bytes of dQ at 512
     tokens, 32x at 4096), and the fp32 [tokens, num_heads] row sums Delta.
     :param dropout: the (p, seed) of the forward that produced ``out``; the mask is regenerated, not read
@@ -306,6 +310,7 @@ def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, 
     assert dout.dtype == torch.bfloat16 and dout.is_contiguous() and out.is_contiguous() and lse.dtype == torch.float32
     assert out.dtype == torch.bfloat16 and qkv.is_contiguous()
     assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
+    assert num_heads > 0 and d_model % num_heads == 0 and d_model // num_heads in HEAD_DIMS, (d_model, num_heads)
     delta = torch.empty(tokens, num_heads, dtype=torch.float32, device=qkv.device)      # rowsum(dout o out), filled by the prologue kernel
     if dqkv is None:
         dqkv = torch.empty_like(qkv)

@@ -187,8 +187,9 @@ def draw_dropout_seed() -> int:
 class NativeTransformerExecutor:
     """
     Trainable sm_90a transformer expert (post-LN encoder layer of the reference's experiments/throughput/layers.py:22-51,
-    batch-first [B, S, d] with any sequence length 1 <= S <= K.MAX_SEQ, head_dim 64, every dropout probability in [0, 1) —
-    the reference's block cannot be trained).
+    batch-first [B, S, d] with any sequence length 1 <= S <= K.MAX_SEQ, head_dim d / nhead in K.HEAD_DIMS = (32, 64, 128),
+    d and dim_feedforward multiples of 256, every dropout probability in [0, 1) — the reference's block cannot be trained).
+    With the reference's nhead = 16 that is d = 512, 1024 and 2048; any other layer stays on the module.
 
     Sequences: the token dimension B*S is padded with zero rows to a multiple of 128 for the GEMM, LayerNorm and dropout
     kernels; attention sees only the B*S real rows and is told S.  Padding rows contribute exactly zero to every parameter
@@ -229,7 +230,8 @@ class NativeTransformerExecutor:
         attn = expert.self_attn
         d, ff = attn.embed_dim, expert.linear1.out_features
         params = list(expert.parameters())
-        if d // attn.num_heads != 64 or d % 256 or ff % 256 or not params[0].is_cuda or params[0].dtype != torch.float32:
+        if (d % attn.num_heads or d // attn.num_heads not in K.HEAD_DIMS or d % 256 or ff % 256 or not params[0].is_cuda
+                or params[0].dtype != torch.float32):
             return False
         if not all(0.0 <= p < 1.0 for p in NativeTransformerExecutor._dropout_ps(expert)):
             return False   # p = 1 zeroes a whole branch: eager PyTorch handles that configuration
