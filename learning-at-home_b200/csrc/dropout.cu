@@ -3,6 +3,8 @@
 //   op 0  out = M o x / (1 - p)                            backward of dropout1 / dropout2 (the branch side of the residual)
 //   op 1  out = M o gelu(x) / (1 - p)                      forward of linear1's activation + dropout
 //   op 2  out = gelu'(f) o M o x / (1 - p)   (x = dg)      backward of the same
+//   op 3  out = M o relu(x) / (1 - p)                      the same pair for a ReLU activation
+//   op 4  out = [f > 0] o M o x / (1 - p)    (x = dg)
 //
 // One thread owns one mask granule ({r, r+8} x {b, b+1, b+8, b+9}): one Philox call, eight elements, 4-byte accesses that a
 // quad of threads turns into 32 contiguous bytes per row.  GELU is the erf form, as nn.GELU().
@@ -12,7 +14,7 @@
 namespace lah {
 namespace drop {
 
-constexpr int OP_APPLY = 0, OP_GELU_FWD = 1, OP_GELU_BWD = 2;
+constexpr int OP_APPLY = 0, OP_GELU_FWD = 1, OP_GELU_BWD = 2, OP_RELU_FWD = 3, OP_RELU_BWD = 4;
 
 __device__ __forceinline__ float gelu_f(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752f)); }
 __device__ __forceinline__ float gelu_grad(float v) {
@@ -38,7 +40,7 @@ __global__ void __launch_bounds__(256) dropout_ew_kernel(const bf16* __restrict_
             const float2 xv = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(x + off)));
             float v[2] = {xv.x, xv.y};
             float fv[2] = {0.f, 0.f};
-            if (OP == OP_GELU_BWD) {
+            if (OP == OP_GELU_BWD || OP == OP_RELU_BWD) {
                 const float2 t2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(f + off)));
                 fv[0] = t2.x;
                 fv[1] = t2.y;
@@ -49,6 +51,8 @@ __global__ void __launch_bounds__(256) dropout_ew_kernel(const bf16* __restrict_
                 if (OP == OP_APPLY) v[i] = v[i] * s;
                 if (OP == OP_GELU_FWD) v[i] = gelu_f(v[i]) * s;
                 if (OP == OP_GELU_BWD) v[i] = gelu_grad(fv[i]) * (v[i] * s);
+                if (OP == OP_RELU_FWD) v[i] = v[i] > 0.f ? v[i] * s : 0.f;
+                if (OP == OP_RELU_BWD) v[i] = fv[i] > 0.f ? v[i] * s : 0.f;
             }
             *reinterpret_cast<uint32_t*>(out + off) = pack_bf16x2(v[0], v[1]);
         }
@@ -103,6 +107,11 @@ int lah_dropout_ew(int op, const void* x, const void* f, void* out, long long ro
         dropout_ew_kernel<OP_GELU_FWD><<<grid, 256, 0, st>>>((const bf16*)x, nullptr, (bf16*)out, granules, cols, seed, site, t, scale);
     else if (op == OP_GELU_BWD)
         dropout_ew_kernel<OP_GELU_BWD><<<grid, 256, 0, st>>>((const bf16*)x, (const bf16*)f, (bf16*)out, granules, cols, seed, site, t,
+                                                            scale);
+    else if (op == OP_RELU_FWD)
+        dropout_ew_kernel<OP_RELU_FWD><<<grid, 256, 0, st>>>((const bf16*)x, nullptr, (bf16*)out, granules, cols, seed, site, t, scale);
+    else if (op == OP_RELU_BWD)
+        dropout_ew_kernel<OP_RELU_BWD><<<grid, 256, 0, st>>>((const bf16*)x, (const bf16*)f, (bf16*)out, granules, cols, seed, site, t,
                                                             scale);
     else
         return -3;

@@ -161,15 +161,19 @@ __global__ void __launch_bounds__(256, 2) ln_relu_fwd_kernel(
 //   g    = da * mask                    dbeta += g        dgamma += g * xhat
 //   dxh  = g * gamma
 //   dh   = rstd * (dxh - mean_c(dxh) - xhat * mean_c(dxh * xhat))     dbias += dh
+// With RES the LayerNorm sits on a residual branch (pre-LN encoder layer: h = x + f(LN(x))): the gradient that bypasses it,
+// dres, is added to dh before it is stored, and dbias is the column sum of that total.  dres is the LAST parameter so
+// that the RES = false kernels keep the parameter layout, and the code, they had before it existed.
 // ------------------------------------------------------------------------------------------------
-template <int C>
+template <int C, bool RES>
 __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel(const bf16* __restrict__ da, const bf16* __restrict__ h,
                                                             const float* __restrict__ mean_in,
                                                             const float* __restrict__ rstd_in,
                                                             const float* __restrict__ gamma,
                                                             const float* __restrict__ beta, bf16* __restrict__ dh,
                                                             float* __restrict__ part,
-                                                            const int* __restrict__ tile_group, int rows, int relu, int tile_rows) {
+                                                            const int* __restrict__ tile_group, int rows, int relu, int tile_rows,
+                                                            const bf16* __restrict__ dres) {
     constexpr int THREADS = C / 8;
     constexpr int WARPS = THREADS / 32;
     constexpr int RB = (C >= 4096) ? 2 : 4;  // rows per batch (register blocking)
@@ -276,10 +280,21 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
             float gvv[8], xhh[8];
             slice(r, true, gvv, xhh);
             const float m1 = tot[2 * r], m2 = tot[2 * r + 1];
-            float o[8];
+            float o[8], res[8];
+            if (RES) {
+                const int4 qr = ld_nc_v4(reinterpret_cast<const int4*>(dres + static_cast<long long>(row) * C + col));
+                const uint32_t wr[4] = {(uint32_t)qr.x, (uint32_t)qr.y, (uint32_t)qr.z, (uint32_t)qr.w};
+#pragma unroll
+                for (int t = 0; t < 4; ++t) {
+                    const float2 fr = unpack_bf16x2(wr[t]);
+                    res[2 * t] = fr.x;
+                    res[2 * t + 1] = fr.y;
+                }
+            }
 #pragma unroll
             for (int t = 0; t < 8; ++t) {
                 o[t] = rs[r] * (gvv[t] * gam[t] - m1 - xhh[t] * m2);
+                if (RES) o[t] += res[t];
                 acc_db[t] += gvv[t];
                 acc_dg[t] += gvv[t] * xhh[t];
                 acc_dbias[t] += o[t];
@@ -419,17 +434,23 @@ int lah_ln_relu_fwd_q(const void* h, void* a, float* mean, float* rstd, const fl
 }
 
 // part: scratch of [ceil(rows / tile_rows), 3, C] fp32 (per-tile column sums, reduced in tile order)
+// dres: optional [rows, C] bf16 residual gradient added to dh (and to dbias's column sum); NULL = none
 int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
                     const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
-                    const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
+                    const int* tile_group, int rows, int C, int relu, int tile_rows, const void* dres, cudaStream_t st) {
     if (rows <= 0) return 0;
     if (shift_of(tile_rows) < 0) return -2;
     const int grid = (rows + tile_rows - 1) / tile_rows;
 #define LAH_LN_BWD(CC)                                                                                          \
     if (C == CC) {                                                                                              \
-        ln_relu_bwd_kernel<CC><<<grid, CC / 8, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd, gamma,    \
-                                                        beta, (bf16*)dh, part, tile_group, rows, relu,         \
-                                                        tile_rows);                                             \
+        if (dres)                                                                                               \
+            ln_relu_bwd_kernel<CC, true><<<grid, CC / 8, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd,  \
+                                                                  gamma, beta, (bf16*)dh, part, tile_group,     \
+                                                                  rows, relu, tile_rows, (const bf16*)dres);    \
+        else                                                                                                    \
+            ln_relu_bwd_kernel<CC, false><<<grid, CC / 8, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd, \
+                                                                   gamma, beta, (bf16*)dh, part, tile_group,    \
+                                                                   rows, relu, tile_rows, nullptr);             \
         group_tile_sum_kernel<<<(3 * CC + 255) / 256, 256, 0, st>>>(part, grid, 3, CC, tile_group, dgamma,     \
                                                                      dbeta, dbias);                            \
         return -(int)cudaGetLastError();                                                                        \

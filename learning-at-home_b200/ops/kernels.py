@@ -28,7 +28,7 @@ def _lib():
     P, I, L, Fl = c_void_p, c_int, c_ll, c_float
     sigs = {
         "lah_ln_relu_fwd": [P, P, P, P, P, P, P, I, I, I, I, P],
-        "lah_ln_relu_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P],
+        "lah_ln_relu_bwd": [P, P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, P, P],
         "lah_grouped_colsum": [P, L, P, P, I, P, I, I, P],
         "lah_set_step_counters": [P],
         "lah_set_multicast": [c_ull],
@@ -98,14 +98,18 @@ def ln_relu_fwd(h, gamma, beta, tile_group, *, out, mean, rstd, relu=True, quant
     return out
 
 
-def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta, dbias, relu=True, tile_rows=128):
-    """dgamma / dbeta / dbias (+)= the column sums of every group's rows, summed in a fixed order (run-to-run identical)"""
+def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta, dbias, relu=True, tile_rows=128,
+                dres=None):
+    """dgamma / dbeta / dbias (+)= the column sums of every group's rows, summed in a fixed order (run-to-run identical)
+    :param dres: optional bf16 [rows, C] gradient of a residual that bypasses the LayerNorm: dh = dres + LN backward, and
+        dbias is the column sum of that total"""
     rows, C = h.shape
     assert da.is_contiguous() and h.is_contiguous() and dh.is_contiguous()
+    assert dres is None or (dres.shape == h.shape and dres.dtype == torch.bfloat16 and dres.is_contiguous())
     part = torch.empty((rows + tile_rows - 1) // tile_rows, 3, C, device=h.device, dtype=torch.float32)
     native.check(_lib().lah_ln_relu_bwd(ptr(da), ptr(h), ptr(mean), ptr(rstd), ptr(gamma), ptr(beta), ptr(dh),
                                         ptr(dgamma), ptr(dbeta), ptr(dbias), ptr(part), ptr(tile_group), rows, C,
-                                        int(relu), int(tile_rows), stream_ptr()), "lah_ln_relu_bwd")
+                                        int(relu), int(tile_rows), ptr(dres), stream_ptr()), "lah_ln_relu_bwd")
     native.count_launch(2)
     return dh
 
@@ -399,6 +403,26 @@ def gelu_dropout_bwd(dg, f, p, seed, site, *, out=None):
     return _dropout_ew(2, dg, f, p, seed, site, out)
 
 
+def relu_dropout(f, p, seed, site, *, out=None):
+    """out = M o relu(f) / (1 - p)"""
+    return _dropout_ew(3, f, None, p, seed, site, out)
+
+
+def relu_dropout_bwd(dg, f, p, seed, site, *, out=None):
+    """out = [f > 0] o M o dg / (1 - p): backward of ``relu_dropout``"""
+    return _dropout_ew(4, dg, f, p, seed, site, out)
+
+
+def relu_dropout_ref(f, mask, p):
+    """fp32 oracle of ``relu_dropout`` with a materialised keep mask"""
+    return mask.float() * F.relu(f.float()) / (1 - p)
+
+
+def relu_dropout_bwd_ref(dg, f, mask, p):
+    """fp32 oracle of ``relu_dropout_bwd``"""
+    return (f.float() > 0).float() * mask.float() * dg.float() / (1 - p)
+
+
 _PHILOX_M0, _PHILOX_M1, _PHILOX_W0, _PHILOX_W1 = 0xD2511F53, 0xCD9E8D57, 0x9E3779B9, 0xBB67AE85
 _U32 = 0xFFFFFFFF
 
@@ -623,6 +647,22 @@ def gate_fail_mask_ref(B, E, rate, seed, token_offset):
 def ln_relu_ref(h, gamma, beta, relu=True):
     y = F.layer_norm(h.float(), (h.shape[-1],), gamma.float(), beta.float(), 1e-5)
     return F.relu(y) if relu else y
+
+
+def ln_relu_bwd_ref(da, h, gamma, beta, relu=True, dres=None):
+    """fp32 closed-form oracle of ``ln_relu_bwd`` for one group: (dh, dgamma, dbeta, dbias), dbias = the column sum of dh"""
+    hf = h.float()
+    mu = hf.mean(-1, keepdim=True)
+    rstd = torch.rsqrt(hf.var(-1, unbiased=False, keepdim=True) + 1e-5)
+    xhat = (hf - mu) * rstd
+    g = da.float()
+    if relu:
+        g = g * (xhat * gamma.float() + beta.float() > 0)
+    dxh = g * gamma.float()
+    dh = rstd * (dxh - dxh.mean(-1, keepdim=True) - xhat * (dxh * xhat).mean(-1, keepdim=True))
+    if dres is not None:
+        dh = dh + dres.float()
+    return dh, (g * xhat).sum(0), g.sum(0), dh.sum(0)
 
 
 @torch.no_grad()

@@ -28,9 +28,16 @@ class ExpertBackend(nn.Module):
                  args_schema: Tuple[BatchTensorProto, ...] = None, kwargs_schema: Dict[str, BatchTensorProto] = None,
                  outputs_schema: Union[BatchTensorProto, Tuple[BatchTensorProto, ...]] = None, native: bool = True,
                  **kwargs):
-        """:param native: run FeedforwardBlock experts that live on a CUDA device through the sm_90a kernels
-        (runtime/native_executor.py: swap-AB wgmma GEMMs, fused LayerNorm, fused weight-gradient + AMSGrad) instead of
-        eager PyTorch; anything the executor does not support falls back to the module itself"""
+        """:param native: run experts that live on a CUDA device in fp32 with a single-group torch.optim.Adam through the
+        sm_90a kernels (runtime/native_executor.py) instead of eager PyTorch.  These run natively, plain or
+        ``torch.jit.script``-ed:
+          * ``FeedforwardBlock`` (swap-AB wgmma GEMMs, fused LayerNorm, fused weight-gradient + AMSGrad);
+          * this package's ``TransformerEncoderLayer`` and ``torch.nn.TransformerEncoderLayer`` with ReLU or erf GELU,
+            ``norm_first`` True or False, ``batch_first`` True or False, LayerNorm eps 1e-5 and all biases, head dim
+            d_model / nhead in (32, 64, 128), d_model and dim_feedforward multiples of 256, dropout p < 1 at every site,
+            sequence length 1 <= S <= 65536 (wgmma attention and GEMMs, in-kernel dropout, fused AMSGrad).
+        Anything else (another class, tanh GELU, kdim / vdim, bias=False, other widths or inputs, CPU tensors) runs on
+        the module itself"""
         super().__init__()
         self.expert, self.opt, self.name = expert, opt, name
         self.native, self._executor, self._executor_key = native, None, None

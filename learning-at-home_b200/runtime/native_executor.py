@@ -11,12 +11,98 @@ hand-written sm_90a kernels instead of eager PyTorch, so that a ``TesseractServe
 The module's parameters and the torch optimizer's state tensors are re-bound as VIEWS of the executor's flat fp32 buffers:
 ``expert.state_dict()``, ``opt.state_dict()`` and ``ExpertBackend.checkpoint()`` stay live and keep the reference layout.
 """
-from typing import Optional
+import re
+from typing import NamedTuple, Optional, Tuple
 
 import torch
+import torch.nn.functional as F
 
-from ..models.layers import FeedforwardBlock
+from ..models.layers import FeedforwardBlock, TransformerEncoderLayer
 from ..ops import kernels as K, native
+
+TORCH_ENCODER_LAYER = "torch.nn.modules.transformer.TransformerEncoderLayer"
+OWN_ENCODER_LAYER = "lah_b200.models.layers.TransformerEncoderLayer"
+OWN_FFN = "lah_b200.models.layers.FeedforwardBlock"
+LN_EPS = 1e-5   # the LayerNorm epsilon compiled into csrc/layernorm.cu
+
+
+def class_name(module) -> str:
+    """qualified name of the class a module was built from: for a ``torch.jit.script`` module that of its original class
+    (TorchScript's ``__torch__.`` prefix and ``___torch_mangle_N.`` parts removed).  Subclasses of this package's layers
+    report the layer they extend, as ``isinstance`` would; any other class reports itself, so a subclass of a torch layer
+    that overrides ``forward`` is not mistaken for it."""
+    if type(module) is torch.jit.RecursiveScriptModule:
+        name = module._c._type().qualified_name()
+        return re.sub(r"___torch_mangle_\d+\.", "", name[len("__torch__."):] if name.startswith("__torch__.") else name)
+    for own in (TransformerEncoderLayer, FeedforwardBlock):
+        if isinstance(module, own):
+            return f"{own.__module__}.{own.__qualname__}"
+    return f"{type(module).__module__}.{type(module).__qualname__}"
+
+
+class FFNSpec(NamedTuple):
+    hid: int
+    inner: int
+
+
+class EncoderLayerSpec(NamedTuple):
+    d: int
+    heads: int
+    ff: int
+    norm_first: bool         # pre-LN: h = x + attn(LN1(x)), y = h + ffn(LN2(h)); post-LN: LN2(x1 + ffn(x1)), x1 = LN1(x + attn(x))
+    activation: str          # "relu" or "gelu" (erf)
+    batch_first: bool        # interface layout: [B, S, d] or [S, B, d]
+    ps: Tuple[float, float, float, float]   # drop probabilities of sites 0-3: attention, dropout1, dropout, dropout2
+
+
+def ffn_spec(module) -> Optional[FFNSpec]:
+    """what NativeFFNExecutor needs of a FeedforwardBlock (plain or scripted), or None for any other module"""
+    if class_name(module) != OWN_FFN:
+        return None
+    return FFNSpec(module.layers[0].in_features, module.layers[0].out_features)
+
+
+def _activation(layer) -> Optional[str]:
+    """"relu" / "gelu" for the activations the executor implements, None for any other (tanh GELU included)"""
+    act = getattr(layer, "activation", None)
+    if act is None:   # a scripted layer does not keep a function activation as an attribute: F.relu -> 1, F.gelu -> 2
+        return {1: "relu", 2: "gelu"}.get(int(layer.activation_relu_or_gelu))
+    if act is F.relu or class_name(act) == "torch.nn.modules.activation.ReLU":
+        return "relu"
+    if act is F.gelu or (class_name(act) == "torch.nn.modules.activation.GELU" and act.approximate == "none"):
+        return "gelu"
+    return None
+
+
+def encoder_layer_spec(module) -> Optional[EncoderLayerSpec]:
+    """
+    What NativeTransformerExecutor needs of an encoder layer, or None when it cannot run it.  Accepted, plain or
+    ``torch.jit.script``-ed: this package's TransformerEncoderLayer (batch-first, post-LN, GELU) and
+    torch.nn.TransformerEncoderLayer with either ``norm_first`` and ``batch_first``, ReLU or erf GELU.  Refused: any other
+    activation (tanh GELU too), a LayerNorm eps other than 1e-5, missing biases or LayerNorm affine parameters, ``kdim`` /
+    ``vdim`` other than d_model, ``add_bias_kv``, ``add_zero_attn``, and every other class.
+    """
+    name = class_name(module)
+    if name == OWN_ENCODER_LAYER:
+        norm_first, activation, batch_first = False, "gelu", True
+    elif name == TORCH_ENCODER_LAYER:
+        norm_first, activation, batch_first = bool(module.norm_first), _activation(module), bool(module.self_attn.batch_first)
+        if activation is None:
+            return None
+    else:
+        return None
+    attn = module.self_attn
+    if not attn._qkv_same_embed_dim or attn.bias_k is not None or attn.add_zero_attn:
+        return None
+    linears = (attn.out_proj, module.linear1, module.linear2)
+    norms = (module.norm1, module.norm2)
+    if attn.in_proj_bias is None or any(m.bias is None for m in linears + norms) or any(n.weight is None for n in norms):
+        return None
+    if any(float(n.eps) != LN_EPS for n in norms):
+        return None
+    ps = (float(attn.dropout), float(module.dropout1.p), float(module.dropout.p), float(module.dropout2.p))
+    return EncoderLayerSpec(int(attn.embed_dim), int(attn.num_heads), int(module.linear1.out_features), norm_first,
+                            activation, batch_first, ps)
 
 SEGS = (("w1", 0, "weight"), ("b1", 0, "bias"), ("g1", 1, "weight"), ("be1", 1, "bias"), ("w2", 3, "weight"),
         ("b2", 3, "bias"), ("g2", 4, "weight"), ("be2", 4, "bias"), ("w3", 6, "weight"), ("b3", 6, "bias"))
@@ -33,9 +119,10 @@ class NativeFFNExecutor:
 
     @staticmethod
     def supports(expert, opt) -> bool:
-        if not isinstance(expert, FeedforwardBlock) or not torch.cuda.is_available():
+        spec = ffn_spec(expert)
+        if spec is None or not torch.cuda.is_available():
             return False
-        hid = expert.layers[0].in_features
+        hid = spec.hid
         params = list(expert.parameters())
         if hid % 128 or not params or not params[0].is_cuda or params[0].dtype != torch.float32:
             return False
@@ -48,7 +135,7 @@ class NativeFFNExecutor:
             return False
         return native.have_cuda_kernels()
 
-    def __init__(self, expert: FeedforwardBlock, opt: torch.optim.Adam):
+    def __init__(self, expert, opt: torch.optim.Adam):
         self.expert, self.opt = expert, opt
         dev = next(expert.parameters()).device
         self.device = dev
@@ -186,24 +273,31 @@ def draw_dropout_seed() -> int:
 
 class NativeTransformerExecutor:
     """
-    Trainable sm_90a transformer expert (post-LN encoder layer of the reference's experiments/throughput/layers.py:22-51,
-    batch-first [B, S, d] with any sequence length 1 <= S <= K.MAX_SEQ, head_dim d / nhead in K.HEAD_DIMS = (32, 64, 128),
-    d and dim_feedforward multiples of 256, every dropout probability in [0, 1) — the reference's block cannot be trained).
-    With the reference's nhead = 16 that is d = 512, 1024 and 2048; any other layer stays on the module.
+    Trainable sm_90a transformer expert: an encoder layer ``encoder_layer_spec`` accepts (this package's post-LN GELU layer,
+    the layer of the reference's experiments/throughput/layers.py:22-51, which the reference's block cannot train; and
+    torch.nn.TransformerEncoderLayer post- or pre-LN, ReLU or erf GELU, batch- or sequence-first; each plain or scripted)
+    with any sequence length 1 <= S <= K.MAX_SEQ, head_dim d / nhead in K.HEAD_DIMS = (32, 64, 128), d and
+    dim_feedforward multiples of 256 and every dropout probability in [0, 1).  With nhead = 16 that is d = 512, 1024 and
+    2048; any other layer stays on the module.
 
     Sequences: the token dimension B*S is padded with zero rows to a multiple of 128 for the GEMM, LayerNorm and dropout
     kernels; attention sees only the B*S real rows and is told S.  Padding rows contribute exactly zero to every parameter
     gradient: their output gradient is zero, so every gradient row the backward forms for them is zero, except the rows of
-    dqkv, which attention_bwd does not write and which are zeroed before the in_proj bias and weight gradients.  Dropout
-    sites 1-3 index token row b*S + s, as an unpadded layer would.
+    dqkv, which attention_bwd does not write and which are zeroed before the in_proj bias and weight gradients.  The
+    workspace is batch-major whatever the interface layout (a sequence-first input [S, B, d] is transposed on the copy in,
+    and the output and the input gradient on the copy out), so dropout sites 1-3 index token row b*S + s, as an unpadded
+    batch-first layer would.
 
       forward   in_proj GEMM -> wgmma flash attention (emits the row log-sum-exp; attention dropout in-kernel) -> out_proj
-                GEMM (+bias, dropout1, +residual) -> LayerNorm -> linear1 GEMM -> GELU (+dropout: csrc/dropout.cu) ->
-                linear2 GEMM (+bias, dropout2, +residual) -> LayerNorm
+                GEMM (+bias, dropout1, +residual) -> LayerNorm -> linear1 GEMM -> GELU / ReLU (+dropout: csrc/dropout.cu)
+                -> linear2 GEMM (+bias, dropout2, +residual) -> LayerNorm;  pre-LN moves each LayerNorm in front of its
+                branch (LN1 before in_proj, LN2 before linear1; the residuals are the un-normalised x and h) and has no
+                final LayerNorm
       backward  LayerNorm backward kernels (they also produce the bias gradients of the preceding Linear when its dropout is
-                off), 128 x 256-tile wgmma dgrad / wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel
-                (csrc/attention_bwd.cu), GELU backward (aten elementwise, or the fused GELU + dropout backward kernel), one
-                fused AMSGrad/Adam step over the flat parameter buffer
+                off; pre-LN: they add the residual gradient that bypasses the LayerNorm), 128 x 256-tile wgmma dgrad /
+                wgrad GEMMs for the four projections, the wgmma ATTENTION BACKWARD kernel (csrc/attention_bwd.cu), the
+                activation's backward (aten elementwise, or the fused activation + dropout backward kernel), one fused
+                AMSGrad/Adam step over the flat parameter buffer
 
     Dropout (the reference's default layer has p = 0.1 at all four sites) applies iff ``expert.training``, like nn.Dropout.
     Every call with dropout draws one seed (``draw_dropout_seed``); a backward call uses it for its forward recompute and
@@ -216,24 +310,25 @@ class NativeTransformerExecutor:
     keep the reference key names: self_attn.in_proj_weight, linear1.weight, norm1.weight, ...).
     """
     NAMES = ("w_in", "b_in", "w_out", "b_out", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
-    INPUT_DIMS = 3   # [batch, seq, d_model]
+    INPUT_DIMS = 3   # [batch, seq, d_model], or [seq, batch, d_model] for a sequence-first layer
 
     def accepts(self, x) -> bool:
-        """True when ``x`` is an input this executor runs: [batch, S, d_model] with 1 <= S <= K.MAX_SEQ"""
-        return x.dim() == self.INPUT_DIMS and x.shape[2] == self.d and 1 <= x.shape[1] <= K.MAX_SEQ
+        """True when ``x`` is an input this executor runs: [batch, S, d_model] (sequence-first: [S, batch, d_model]) with
+        1 <= S <= K.MAX_SEQ"""
+        seq = x.shape[1 if self.batch_first else 0] if x.dim() == self.INPUT_DIMS else 0
+        return x.dim() == self.INPUT_DIMS and x.shape[2] == self.d and 1 <= seq <= K.MAX_SEQ
 
     @staticmethod
     def supports(expert, opt) -> bool:
-        from ..models.layers import TransformerEncoderLayer
-        if not isinstance(expert, TransformerEncoderLayer) or not torch.cuda.is_available():
+        spec = encoder_layer_spec(expert)
+        if spec is None or not torch.cuda.is_available():
             return False
-        attn = expert.self_attn
-        d, ff = attn.embed_dim, expert.linear1.out_features
+        d, heads, ff = spec.d, spec.heads, spec.ff
         params = list(expert.parameters())
-        if (d % attn.num_heads or d // attn.num_heads not in K.HEAD_DIMS or d % 256 or ff % 256 or not params[0].is_cuda
+        if (d % heads or d // heads not in K.HEAD_DIMS or d % 256 or ff % 256 or not params[0].is_cuda
                 or params[0].dtype != torch.float32):
             return False
-        if not all(0.0 <= p < 1.0 for p in NativeTransformerExecutor._dropout_ps(expert)):
+        if not all(0.0 <= p < 1.0 for p in spec.ps):
             return False   # p = 1 zeroes a whole branch: eager PyTorch handles that configuration
         if type(opt) is not torch.optim.Adam or len(opt.param_groups) != 1:
             return False
@@ -246,8 +341,8 @@ class NativeTransformerExecutor:
 
     @staticmethod
     def _dropout_ps(expert):
-        """drop probabilities of the kernels' sites 0-3: attention, dropout1, dropout (after GELU), dropout2"""
-        return (float(expert.self_attn.dropout), float(expert.dropout1.p), float(expert.dropout.p), float(expert.dropout2.p))
+        """drop probabilities of the kernels' sites 0-3: attention, dropout1, dropout (after the activation), dropout2"""
+        return encoder_layer_spec(expert).ps
 
     def _dropout(self):
         """(seed, (p_attn, p_1, p_ff, p_2)) for one call, or None in eval mode / without dropout"""
@@ -258,8 +353,10 @@ class NativeTransformerExecutor:
 
     def __init__(self, expert, opt):
         self.expert, self.opt = expert, opt
+        spec = encoder_layer_spec(expert)
+        self.d, self.heads, self.ff = spec.d, spec.heads, spec.ff
+        self.norm_first, self.relu, self.batch_first = spec.norm_first, spec.activation == "relu", spec.batch_first
         attn = expert.self_attn
-        self.d, self.heads, self.ff = attn.embed_dim, attn.num_heads, expert.linear1.out_features
         self.params = [attn.in_proj_weight, attn.in_proj_bias, attn.out_proj.weight, attn.out_proj.bias, expert.linear1.weight,
                        expert.linear1.bias, expert.linear2.weight, expert.linear2.bias, expert.norm1.weight, expert.norm1.bias,
                        expert.norm2.weight, expert.norm2.bias]
@@ -320,8 +417,28 @@ class NativeTransformerExecutor:
                       x1=torch.empty(T, d, **bf), f=torch.empty(T, ff, **bf), y=torch.empty(T, d, **bf), out=torch.empty(T, d, **bf),
                       lse=torch.empty(T, self.heads, **f32), stats=torch.empty(4, T, **f32),
                       group_off=torch.tensor([0, T], dtype=torch.int32, device=self.device))
+            if self.norm_first:
+                ws["xa"] = torch.empty(T, d, **bf)   # LN1(x), the input of in_proj
             self._ws = {T: ws}
         return ws
+
+    def _batch_seq(self, t):
+        """(batch, seq) of an interface tensor"""
+        return (t.shape[0], t.shape[1]) if self.batch_first else (t.shape[1], t.shape[0])
+
+    def _to_rows(self, dst, t):
+        """copy the interface tensor ``t`` into the batch-major token rows ``dst`` [batch * seq, d]"""
+        if self.batch_first:
+            dst.copy_(t.reshape(dst.shape))
+        else:
+            dst.view(t.shape[1], t.shape[0], t.shape[2]).copy_(t.transpose(0, 1))
+
+    def _from_rows(self, rows, like):
+        """the batch-major token rows [batch * seq, d] as a tensor of the shape, layout and dtype of ``like``"""
+        if self.batch_first:
+            return rows.view(like.shape).to(like.dtype)
+        seq, batch, d = like.shape
+        return rows.view(batch, seq, d).transpose(0, 1).to(like.dtype, memory_format=torch.contiguous_format)
 
     @staticmethod
     def _site(drop, site):
@@ -334,46 +451,55 @@ class NativeTransformerExecutor:
         """returns the workspace, the real token rows Tr = batch * seq and the padded rows T (a multiple of 128)"""
         from ..ops import gemm
         assert self.accepts(src), (tuple(src.shape), self.d)
-        batch, seq, d = src.shape
+        batch, seq = self._batch_seq(src)
         Tr = batch * seq
         T = (Tr + 127) // 128 * 128
         ws = self._workspace(T)
-        ws["x"][:Tr].copy_(src.reshape(Tr, d))
+        self._to_rows(ws["x"][:Tr], src)
         if T > Tr:
             ws["x"][Tr:].zero_()
             ws["att"][Tr:].zero_()   # attention writes only the real rows
-        x, bv, pv, site = ws["x"], self.bv, self.pv, self._site
-        gemm.grouped_linear(x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
+        x, bv, pv, site, stats = ws["x"], self.bv, self.pv, self._site, ws["stats"]
+        if self.norm_first:
+            K.ln_relu_fwd(x, pv["g1"], pv["be1"], None, out=ws["xa"], mean=stats[0], rstd=stats[1], relu=False)
+        gemm.grouped_linear(ws["xa"] if self.norm_first else x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
         K.attention_fwd(ws["qkv"][:Tr], self.heads, out=ws["att"][:Tr], lse=ws["lse"][:Tr], dropout=site(drop, K.SITE_ATTN),
                         seq_len=seq)
         gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"],
                             dropout=site(drop, K.SITE_OUT_PROJ))
-        K.ln_relu_fwd(ws["h"], pv["g1"], pv["be1"], None, out=ws["x1"], mean=ws["stats"][0], rstd=ws["stats"][1], relu=False)
+        if self.norm_first:   # x1 = LN2(h) feeds the feed-forward branch, h is its residual
+            K.ln_relu_fwd(ws["h"], pv["g2"], pv["be2"], None, out=ws["x1"], mean=stats[2], rstd=stats[3], relu=False)
+        else:                 # x1 = LN1(h) is both
+            K.ln_relu_fwd(ws["h"], pv["g1"], pv["be1"], None, out=ws["x1"], mean=stats[0], rstd=stats[1], relu=False)
         gemm.grouped_linear(ws["x1"], bv["w1"], bias=pv["b1"], out=ws["f"])       # pre-activation kept for backward
         ff = site(drop, K.SITE_FF)
-        ws["gact"] = K.gelu_dropout(ws["f"], *ff) if ff else torch.nn.functional.gelu(ws["f"])
-        gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["x1"], out=ws["y"],
+        if self.relu:
+            ws["gact"] = K.relu_dropout(ws["f"], *ff) if ff else torch.relu(ws["f"])
+        else:
+            ws["gact"] = K.gelu_dropout(ws["f"], *ff) if ff else torch.nn.functional.gelu(ws["f"])
+        gemm.grouped_linear(ws["gact"], bv["w2"], bias=pv["b2"], residual=ws["h"] if self.norm_first else ws["x1"], out=ws["y"],
                             dropout=site(drop, K.SITE_LINEAR2))
-        K.ln_relu_fwd(ws["y"], pv["g2"], pv["be2"], None, out=ws["out"], mean=ws["stats"][2], rstd=ws["stats"][3], relu=False)
+        if not self.norm_first:
+            K.ln_relu_fwd(ws["y"], pv["g2"], pv["be2"], None, out=ws["out"], mean=stats[2], rstd=stats[3], relu=False)
         return ws, Tr, T
 
     @torch.no_grad()
     def forward(self, src: torch.Tensor) -> torch.Tensor:
         ws, Tr, T = self._forward(src, self._dropout())
-        return ws["out"][:Tr].view(src.shape).to(src.dtype)
+        return self._from_rows(ws["y" if self.norm_first else "out"][:Tr], src)
 
     @torch.no_grad()
     def backward(self, src: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
         from ..ops import gemm
         drop = self._dropout()
         ws, Tr, T = self._forward(src, drop)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
-        d, bv, pv, gv, site = self.d, self.bv, self.pv, self.gv, self._site
+        d, bv, pv, gv, site, stats = self.d, self.bv, self.pv, self.gv, self._site, ws["stats"]
         go = ws["group_off"]
         bf = dict(dtype=torch.bfloat16, device=self.device)
-        seq = src.shape[1]
-        if T > Tr:   # zero gradient on the padding rows
-            dout = torch.zeros(T, d, **bf)
-            dout[:Tr].copy_(grad_out.reshape(Tr, d))
+        seq = self._batch_seq(src)[1]
+        if T > Tr or not self.batch_first:   # zero gradient on the padding rows
+            dout = torch.zeros(T, d, **bf) if T > Tr else torch.empty(T, d, **bf)
+            self._to_rows(dout[:Tr], grad_out)
         else:
             dout = grad_out.reshape(T, d).to(torch.bfloat16).contiguous()
 
@@ -388,22 +514,36 @@ class NativeTransformerExecutor:
             return dbr
 
         # with dropout at site 3 / 1 the bias gradient comes from the masked branch gradient, so the LayerNorm backward's
-        # column sum goes to a scratch row
-        scratch = torch.empty(1, d, dtype=torch.float32, device=self.device) if drop is not None else None
-        dy = torch.empty(T, d, **bf)
-        K.ln_relu_bwd(dout, ws["y"], ws["stats"][2], ws["stats"][3], pv["g2"], pv["be2"], None, dh=dy, dgamma=gv["g2"],
-                      dbeta=gv["be2"], dbias=scratch if site(drop, K.SITE_LINEAR2) else gv["b2"], relu=False)
+        # column sum goes to a scratch row; pre-LN's LN1 backward has no bias to feed and always uses it
+        scratch = torch.empty(1, d, dtype=torch.float32, device=self.device) if drop is not None or self.norm_first else None
+        if self.norm_first:   # y = h + branch: no LayerNorm after it, the branch and the residual both receive dout
+            dy = dout
+            if site(drop, K.SITE_LINEAR2) is None:
+                K.grouped_colsum(dy, None, out=gv["b2"])
+        else:
+            dy = torch.empty(T, d, **bf)
+            K.ln_relu_bwd(dout, ws["y"], stats[2], stats[3], pv["g2"], pv["be2"], None, dh=dy, dgamma=gv["g2"],
+                          dbeta=gv["be2"], dbias=scratch if site(drop, K.SITE_LINEAR2) else gv["b2"], relu=False)
         dff = branch_grad(dy, K.SITE_LINEAR2, gv["b2"])
         gemm.grouped_wgrad(dff, ws["gact"], go, 1, out=gv["w2"])
         dg = gemm.grouped_linear(dff, bv["w2"], w_is_kn=True)
         ff = site(drop, K.SITE_FF)
-        df = K.gelu_dropout_bwd(dg, ws["f"], *ff) if ff else torch.ops.aten.gelu_backward(dg, ws["f"])
+        if self.relu:
+            df = K.relu_dropout_bwd(dg, ws["f"], *ff) if ff else torch.ops.aten.threshold_backward(dg, ws["f"], 0)
+        else:
+            df = K.gelu_dropout_bwd(dg, ws["f"], *ff) if ff else torch.ops.aten.gelu_backward(dg, ws["f"])
         K.grouped_colsum(df, None, out=gv["b1"])
         gemm.grouped_wgrad(df, ws["x1"], go, 1, out=gv["w1"])
-        dx1 = gemm.grouped_linear(df, bv["w1"], w_is_kn=True, residual=dy)
-        dh = torch.empty(T, d, **bf)
-        K.ln_relu_bwd(dx1, ws["h"], ws["stats"][0], ws["stats"][1], pv["g1"], pv["be1"], None, dh=dh, dgamma=gv["g1"],
-                      dbeta=gv["be1"], dbias=scratch if site(drop, K.SITE_OUT_PROJ) else gv["b_out"], relu=False)
+        if self.norm_first:   # dh = dy + LN2 backward(dx1): the residual gradient is added inside the LayerNorm backward
+            dx1 = gemm.grouped_linear(df, bv["w1"], w_is_kn=True)
+            dh = torch.empty(T, d, **bf)
+            K.ln_relu_bwd(dx1, ws["h"], stats[2], stats[3], pv["g2"], pv["be2"], None, dh=dh, dgamma=gv["g2"],
+                          dbeta=gv["be2"], dbias=scratch if site(drop, K.SITE_OUT_PROJ) else gv["b_out"], relu=False, dres=dy)
+        else:
+            dx1 = gemm.grouped_linear(df, bv["w1"], w_is_kn=True, residual=dy)
+            dh = torch.empty(T, d, **bf)
+            K.ln_relu_bwd(dx1, ws["h"], stats[0], stats[1], pv["g1"], pv["be1"], None, dh=dh, dgamma=gv["g1"],
+                          dbeta=gv["be1"], dbias=scratch if site(drop, K.SITE_OUT_PROJ) else gv["b_out"], relu=False)
         dhb = branch_grad(dh, K.SITE_OUT_PROJ, gv["b_out"])
         gemm.grouped_wgrad(dhb, ws["att"], go, 1, out=gv["w_out"])
         datt = gemm.grouped_linear(dhb, bv["w_out"], w_is_kn=True)
@@ -415,8 +555,15 @@ class NativeTransformerExecutor:
         else:
             dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN), seq_len=seq)
         K.grouped_colsum(dqkv, None, out=gv["b_in"])
-        gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"])
-        dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh)
+        if self.norm_first:   # dx = dh + LN1 backward(dxa)
+            gemm.grouped_wgrad(dqkv, ws["xa"], go, 1, out=gv["w_in"])
+            dxa = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True)
+            dx = torch.empty(T, d, **bf)
+            K.ln_relu_bwd(dxa, ws["x"], stats[0], stats[1], pv["g1"], pv["be1"], None, dh=dx, dgamma=gv["g1"], dbeta=gv["be1"],
+                          dbias=scratch, relu=False, dres=dh)
+        else:
+            gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"])
+            dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh)
         g = self.opt.param_groups[0]
         K.bump_steps(self.step, self.one)
         K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step, lr=float(g["lr"]),
@@ -426,7 +573,7 @@ class NativeTransformerExecutor:
         step_t = torch.tensor(float(self.steps_host))
         for param in self.params:
             self.opt.state[param]["step"] = step_t
-        return dx[:Tr].view(src.shape).to(src.dtype)
+        return self._from_rows(dx[:Tr], src)
 
 
 def make_executor(expert, opt):
