@@ -353,6 +353,11 @@ int lah_gemm_mgroup(const void* A, long long lda, int a_rows, const void* B, int
                     const int* wait_flags, int wait_count, int wait_epoch, int* status, int act,
                     unsigned long long drop_seed, int drop_thr, float drop_scale, int drop_site, cudaStream_t stream) {
     if ((K % 8) || (N % 32) || (lda % 8)) return -2;
+    // the epilogue reads the residual and writes a bf16 C as 4-byte pairs, writes an fp32 C as 8-byte pairs and reads the
+    // bias as float2: even row strides and bases aligned to those widths
+    if ((ldc % 2) || (reinterpret_cast<uintptr_t>(C) % (out_f32 ? 8 : 4))) return -2;
+    if (residual && ((ldr % 2) || (reinterpret_cast<uintptr_t>(residual) % 4))) return -2;
+    if (bias && (reinterpret_cast<uintptr_t>(bias) % 8)) return -2;
     if (drop_thr >= 0 && (drop_site < 1 || drop_site > 3)) return -2;
     if (drop_thr >= 0 && (block_n != 256 || b_mn || out_f32 || drop_thr > 65535)) return -4;
     if (block_n != 256 && block_n != 128 && block_n != 64) return -3;
@@ -407,6 +412,8 @@ int lah_gemm_kgroup(const void* A, long long lda, const void* B, long long ldb, 
                     const int* group_off, float* C, long long ldc, long long c_group_stride, int block_n,
                     int max_ctas, int accumulate, cudaStream_t stream) {
     if ((M % 128) || (N % 32) || (lda % 8) || (ldb % 8)) return -2;
+    // fp32 C is read (accumulate) and written as 8-byte pairs
+    if ((ldc % 2) || (c_group_stride % 2) || (reinterpret_cast<uintptr_t>(C) % 8)) return -2;
     CUtensorMap tmA, tmB;
     {
         uint64_t dims[2] = {(uint64_t)M, (uint64_t)total_rows};

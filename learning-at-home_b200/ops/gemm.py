@@ -45,6 +45,14 @@ def _pick_block_n(n: int) -> int:
     return 64
 
 
+def _check_pairs(t, what, align):
+    """the GEMM epilogue accesses ``t`` two elements at a time: its row stride must be even and its base ``align``-byte
+    aligned (a misaligned vector access faults on the device)"""
+    if (t.dim() > 1 and t.stride(0) % 2) or t.data_ptr() % align:
+        raise ValueError(f"{what}: the row stride must be even and the base {align}-byte aligned "
+                         f"(stride {t.stride(0)}, address {t.data_ptr():#x})")
+
+
 def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=False, out=None,
                    out_dtype=torch.bfloat16, m_valid=None, block_n=None, max_ctas=0, wait=None, act=0, dropout=None):
     """
@@ -78,10 +86,13 @@ def grouped_linear(a, w, *, tile_group=None, bias=None, residual=None, w_is_kn=F
     if out is None:
         out = torch.empty(rows, N, device=a.device, dtype=out_dtype)
     assert out.stride(1) == 1 and out.shape[0] >= rows and out.shape[1] == N
+    _check_pairs(out, "out", 2 * out.element_size())
     if bias is not None:
         assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == G * N
+        _check_pairs(bias, "bias", 8)
     if residual is not None:
         assert residual.dtype == torch.bfloat16 and residual.stride(1) == 1
+        _check_pairs(residual, "residual", 4)
     bn = block_n or _pick_block_n(N)
     seed, thr, scale = _dropout_args(dropout)
     site = 0
@@ -113,6 +124,7 @@ def grouped_wgrad(dy, x, group_off, num_groups, *, out=None, block_n=None, max_c
     if out is None:
         out = torch.zeros(num_groups, M, N, device=dy.device, dtype=torch.float32)
     assert out.dtype == torch.float32 and out.is_contiguous()
+    _check_pairs(out, "out", 8)
     bn = block_n or _pick_block_n(N)
     code = _lib().lah_gemm_kgroup(ptr(dy), dy.stride(0), ptr(x), x.stride(0), rows, num_groups, M, N, ptr(group_off),
                                   ptr(out), N, M * N, bn, max_ctas, int(accumulate), stream_ptr())
