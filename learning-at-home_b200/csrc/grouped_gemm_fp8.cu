@@ -331,6 +331,10 @@ int lah_quant_mxfp8(const void* in, long long ld_in, int in_f32, void* out, long
                     int groups, int K, int tile_rows, const int* tile_group128, const int* total_rows_dev,
                     cudaStream_t stream) {
     if ((K % 128) || (ld_out % 16) || (tile_rows != 128 && tile_rows != 192)) return -2;
+    // every thread reads its 32 input elements and writes its 32 payload bytes as 16-byte vectors: the input row stride
+    // (in bytes) and both bases must be multiples of 16
+    if (((ld_in * (in_f32 ? 4 : 2)) % 16) || (reinterpret_cast<uintptr_t>(in) % 16) || (reinterpret_cast<uintptr_t>(out) % 16))
+        return -2;
     const long long threads = static_cast<long long>(rows_per_group) * groups * (K / 32);
     if (threads == 0) return 0;
     const int blocks = static_cast<int>((threads + 255) / 256);
@@ -355,6 +359,11 @@ int lah_gemm_mgroup_fp8(const void* A, long long lda, int a_rows, const void* sf
                         const int* tile_group, const float* bias, const void* residual, long long ldr, int max_ctas,
                         const int* wait_flags, int wait_count, int wait_epoch, int* status, int act, cudaStream_t stream) {
     if ((K % 128) || (N % 64) || (lda % 16)) return -2;
+    // the epilogue reads the residual and writes a bf16 C as 4-byte pairs, writes an fp32 C as 8-byte pairs and reads the
+    // bias as float2: even row strides and bases aligned to those widths
+    if ((ldc % 2) || (reinterpret_cast<uintptr_t>(C) % (out_f32 ? 8 : 4))) return -2;
+    if (residual && ((ldr % 2) || (reinterpret_cast<uintptr_t>(residual) % 4))) return -2;
+    if (bias && (reinterpret_cast<uintptr_t>(bias) % 8)) return -2;
     const int num_kb = K / 128;
     const int n_tiles = (N + TILE_N - 1) / TILE_N;
     CUtensorMap tmA, tmB;

@@ -653,6 +653,7 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
                    float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
                    int max_ctas, cudaStream_t st) {
     if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8) || 1ll * G * N > INT_MAX) return -2;
+    if (amsgrad && !vmax) return -2;   // AMSGrad streams vmax through its own tensor map
     CUtensorMap tmDY, tmX;
     wa::StateMaps tmS;
     {

@@ -14,7 +14,7 @@ import ctypes
 
 import torch
 
-from . import native
+from . import gemm, native
 from .native import c_void_p, c_int, c_ll, ptr, stream_ptr
 
 ACT_TILE = 128      # tile_rows of activation scale factors
@@ -65,6 +65,10 @@ def quantize(x, *, tile_rows=ACT_TILE, groups=1, out: MXFP8Tensor = None, tile_g
     if out is None:
         out = MXFP8Tensor(rows // groups, groups, K, tile_rows, x.device)
     assert out.K == K and out.groups == groups and out.rows_per_group == rows // groups and out.tile_rows == tile_rows
+    # the kernel reads 32 input elements and writes 32 payload bytes per thread as 16-byte vectors
+    if (x.stride(0) * x.element_size()) % 16 or x.data_ptr() % 16 or out.q.data_ptr() % 16:
+        raise ValueError(f"quantize: the input row stride and both bases must be multiples of 16 bytes (input stride "
+                         f"{x.stride(0)}, address {x.data_ptr():#x}; payload address {out.q.data_ptr():#x})")
     code = _lib().lah_quant_mxfp8(ptr(x), x.stride(0), int(x.dtype == torch.float32), ptr(out.q), out.q.stride(0),
                                   ptr(out.sf), rows // groups, groups, K, tile_rows, ptr(tile_group), ptr(total_rows),
                                   stream_ptr())
@@ -83,12 +87,15 @@ def grouped_linear_fp8(a: MXFP8Tensor, w: MXFP8Tensor, *, tile_group=None, bias=
     if out is None:
         out = torch.empty(rows, N, device=a.q.device, dtype=out_dtype)
     assert out.stride(1) == 1 and out.dtype in (torch.bfloat16, torch.float32)
+    gemm._check_pairs(out, "out", 2 * out.element_size())
     if tile_group is not None:
         assert tile_group.dtype == torch.int32 and tile_group.numel() >= num_m_tiles
     if bias is not None:
         assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == G * N
+        gemm._check_pairs(bias, "bias", 8)
     if residual is not None:
         assert residual.dtype == torch.bfloat16 and residual.stride(1) == 1
+        gemm._check_pairs(residual, "residual", 4)
     wait_flags, wait_count, wait_epoch, wait_status = None, 0, 0, None
     if wait is not None:
         wait_flags, wait_epoch, wait_status = wait

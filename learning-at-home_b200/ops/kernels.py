@@ -566,6 +566,8 @@ def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, ski
     G, N, Kd = p.shape
     assert dy.shape[1] == N and x.shape[1] == Kd and dy.shape[0] == x.shape[0] and p.is_contiguous()
     assert dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16 and p.dtype == torch.float32
+    if amsgrad and vmax is None:
+        raise ValueError("wgrad_adam: amsgrad needs a vmax tensor (vmax=None only with amsgrad=False)")
     native.check(_lib().lah_wgrad_adam(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd, ptr(group_off),
                                        ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v), ptr(vmax),
                                        ptr(p_bf16), lr, betas[0], betas[1], eps, int(amsgrad), int(max_ctas),

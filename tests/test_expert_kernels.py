@@ -322,9 +322,12 @@ def cuda_randn(gen, *shape, scale=1.0, dtype=torch.float32):
     return (torch.randn(*shape, generator=gen) * scale).to(dtype).cuda()
 
 
-def gemm_epilogue64(pre, mag, K, *, bias=None, act=0, keep=None, p=0.0, residual=None, out_f32=False):
-    """float64 epilogue of the grouped GEMM over the product pre = A B and mag = |A| |B|: (ref, bound)"""
+def gemm_epilogue64(pre, mag, K, *, bias=None, act=0, keep=None, p=0.0, residual=None, out_f32=False, extra=None):
+    """float64 epilogue of the grouped GEMM over the product pre = A B and mag = |A| |B|: (ref, bound).  ``extra`` is an
+    error of the product that is not an fp32 summation (the FP8 tensor core's in-block accumulation)"""
     e = C_ACC * K * U * mag
+    if extra is not None:
+        e = e + extra
     if bias is not None:
         pre = pre + bias
         e = e + 2 * U * (pre.abs() + bias.abs())
