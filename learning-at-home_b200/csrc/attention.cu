@@ -23,6 +23,12 @@
 // sequence (S % 128 != 0) the scores of keys >= S are set to -inf before the row maximum, so they enter neither l nor the
 // LSE; rows of queries >= S are computed on zeros and not stored.  Full blocks take exactly the arithmetic of the
 // 512-token kernel: the tail test is one uniform branch per key block.
+//
+// Key padding mask (MASK instantiations): key_mask is [batch, ceil(S / 32)] uint32, bit k % 32 of word k / 32 set iff key k
+// is valid (attention_pack_key_mask_kernel; bits of keys >= S are clear, so the mask also covers the tail).  Producer and
+// consumers walk the same list of key blocks that hold a valid key: a block without one is neither loaded nor computed.  In
+// a partially valid block the scores of masked keys are set to -inf, as in the tail.  The mask is per key, so after the
+// first block every row maximum is finite.  A sequence without a valid key processes no block: out = 0, lse2 = +inf.
 #include "sm90.cuh"
 #include "dropout.cuh"
 #include <stdlib.h>
@@ -57,11 +63,12 @@ struct Fwd {
 
 // DROP: attention dropout (dropout.cuh, site 0).  The kept bf16 probabilities feed O += P V; the row sum l (and so the LSE)
 // keeps summing ALL of them, and 1 / (1 - p) is folded into the final 1 / l.
-template <int HD, bool DROP>
-__global__ void __launch_bounds__(NUM_THREADS2, 1)
+// MASK without DROP at HD <= 64 is held to 128 registers, as the unmasked kernel is: two CTAs per SM (129 would allow one)
+template <int HD, bool DROP, bool MASK>
+__global__ void __launch_bounds__(NUM_THREADS2, MASK && !DROP && HD <= 64 ? 2 : 1)
 attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, float* __restrict__ lse2,
                         int d_model, int num_heads, int seq_len, float scale_log2e, unsigned long long seed, uint32_t thr,
-                        float rescale) {
+                        float rescale, const uint32_t* __restrict__ key_mask) {
     using C = Fwd<HD>;
     constexpr int TILE_BYTES = C::TILE_BYTES, OFF_Q2 = C::OFF_Q2, OFF_K2 = C::OFF_K2, OFF_V2 = C::OFF_V2;
     constexpr int KSTEPS_PER_ATOM = C::ATOM_COLS / 16;
@@ -82,8 +89,24 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         tma_load_3d(dst, &tm_qkv, bar, c0, row, batch);
         if constexpr (C::ATOMS == 2) tma_load_3d(dst + C::ATOM_BYTES, &tm_qkv, bar, c0 + 64, row, batch);
     };
-    auto load_kv = [&](int j) {   // thread 0 only; stage j & 1 must be free
-        const int st = j & 1;
+    // this sequence's mask words; valid-key bits of block j: words 4j .. 4j + 3 (0 past the last word)
+    const int mask_words = (seq_len + 31) / 32;
+    const uint32_t* kmask = MASK ? key_mask + static_cast<long long>(batch) * mask_words : nullptr;
+    auto block_words = [&](int j, uint32_t (&w)[KB / 32]) {
+#pragma unroll
+        for (int i = 0; i < KB / 32; ++i) w[i] = j * (KB / 32) + i < mask_words ? __ldg(kmask + j * (KB / 32) + i) : 0u;
+    };
+    auto next_block = [&](int j) {   // first key block >= j holding a valid key, or num_kb
+        if constexpr (MASK) {
+            for (; j < num_kb; ++j) {
+                uint32_t w[KB / 32];
+                block_words(j, w);
+                if (w[0] | w[1] | w[2] | w[3]) break;
+            }
+        }
+        return j;
+    };
+    auto load_kv = [&](int st, int j) {   // thread 0 only; stage st must be free
         mbar_arrive_expect_tx(&kv_full[st], 2 * TILE_BYTES);
         load_tile(smem + OFF_K2 + st * TILE_BYTES, &kv_full[st], d_model + head * HD, j * KB);
         load_tile(smem + OFF_V2 + st * TILE_BYTES, &kv_full[st], 2 * d_model + head * HD, j * KB);
@@ -96,8 +119,21 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         fence_mbar_init();
         mbar_arrive_expect_tx(bar_q, TILE_BYTES);
         load_tile(smem + OFF_Q2, bar_q, head * HD, qt * Q_TILE);
-        load_kv(0);
-        if (num_kb > 1) load_kv(1);
+        if constexpr (!MASK) {
+            load_kv(0, 0);
+            if (num_kb > 1) load_kv(1, 1);
+        }
+    }
+    // j: the key block being processed, n: how many blocks were processed before it (its stage and phase); without MASK
+    // j = n.  j1 (MASK): the next block holding a valid key, already loaded into the other stage when < num_kb
+    int j = 0, j1 = 0;
+    if constexpr (MASK) {
+        j = next_block(0);
+        j1 = next_block(j + 1);
+        if (tid == 0) {
+            if (j < num_kb) load_kv(0, j);
+            if (j1 < num_kb) load_kv(1, j1);
+        }
     }
     __syncthreads();
 
@@ -109,9 +145,25 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(bar_q, 0);
 #pragma unroll 1
-    for (int j = 0; j < num_kb; ++j) {
-        const int st = j & 1;
-        mbar_wait(&kv_full[st], (j >> 1) & 1);
+    for (int n = 0; j < num_kb; ++n) {
+        const int st = (MASK ? n : j) & 1;
+        // MASK: bit 2 jj + i of kbits = key 8 jj + 2 (lane & 3) + i of block j is valid, i.e. bits 2c, 2c + 1 of every byte of
+        // the block's words, c = lane & 3; j2 = the block after j1, looked up before the MMAs so that its loads overlap them
+        uint32_t kbits = ~0u;
+        int j2 = 0;
+        if constexpr (MASK) {
+            uint32_t kw[KB / 32];
+            block_words(j, kw);
+            kbits = 0u;
+#pragma unroll
+            for (int w = 0; w < KB / 32; ++w) {
+                uint32_t x = (kw[w] >> (2 * (lane & 3))) & 0x03030303u;
+                x = (x | x >> 6) & 0x000F000Fu;
+                kbits |= ((x | x >> 12) & 0xFFu) << (8 * w);
+            }
+            j2 = next_block(j1 + 1);
+        }
+        mbar_wait(&kv_full[st], ((MASK ? n : j) >> 1) & 1);
         const uint32_t sk = smem_u32(smem + OFF_K2 + st * TILE_BYTES), sv = smem_u32(smem + OFF_V2 + st * TILE_BYTES);
         float s[KB / 2];
         wgmma_fence();
@@ -139,7 +191,15 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         }
         wgmma_wait<0>();
         wgmma_fence_regs(s);
-        if (j * KB + KB > seq_len) {   // last block of a partial sequence: s[4 jj + 2 h + i] is key 8 jj + 2 (lane & 3) + i
+        if constexpr (MASK) {   // masked keys and keys >= S (clear bits): s[4 jj + 2 h + i] is key 8 jj + 2 (lane & 3) + i
+            if (kbits != ~0u) {
+#pragma unroll
+                for (int jj = 0; jj < KB / 8; ++jj)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i)
+                        if (!((kbits >> (2 * jj + i)) & 1u)) s[4 * jj + i] = s[4 * jj + 2 + i] = -INFINITY;
+            }
+        } else if (j * KB + KB > seq_len) {   // last block of a partial sequence: s[4 jj + 2 h + i] is key 8 jj + 2 (lane & 3) + i
 #pragma unroll
             for (int jj = 0; jj < KB / 8; ++jj)
 #pragma unroll
@@ -188,21 +248,26 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_fence_regs(o);
-        if (j + 2 < num_kb) {
+        if constexpr (!MASK) j2 = j + 2;
+        if (j2 < num_kb) {
             named_bar_sync(1, NUM_THREADS2);   // both warpgroups are done with stage st
-            if (tid == 0) load_kv(j + 2);
+            if (tid == 0) load_kv((MASK ? n : j2) & 1, j2);
         }
+        j = MASK ? j1 : j + 1;
+        if constexpr (MASK) j1 = j2;
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         float lt = l[h];
         lt += __shfl_xor_sync(0xffffffffu, lt, 1);
         lt += __shfl_xor_sync(0xffffffffu, lt, 2);
-        const float inv = DROP ? rescale / lt : 1.f / lt;
+        // MASK: lt = 0 iff the sequence has no valid key (no block processed; otherwise the row maximum contributes 1)
+        const float inv = MASK && lt == 0.f ? 0.f : DROP ? rescale / lt : 1.f / lt;
         const int q = qt * Q_TILE + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
         if (q >= seq_len) continue;
         const long long token = static_cast<long long>(batch) * seq_len + q;
-        if (lse2 && (lane & 3) == 0) lse2[token * num_heads + head] = m[h] * scale_log2e + log2f(lt);
+        if (lse2 && (lane & 3) == 0)
+            lse2[token * num_heads + head] = MASK && lt == 0.f ? INFINITY : m[h] * scale_log2e + log2f(lt);
         bf16* op = out + token * d_model + head * HD + 2 * (lane & 3);
 #pragma unroll
         for (int jj = 0; jj < HD / 8; ++jj)
@@ -212,7 +277,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
 
 template <int HD>
 int launch_fwd(const void* qkv, void* out, float* lse2, long long batch, int seq_len, int num_heads, int d_model,
-               unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
+               unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
     using C = Fwd<HD>;
     CUtensorMap tm;
     {   // 3-D {columns, position in sequence, sequence}: a tile never crosses into the next sequence
@@ -223,19 +288,50 @@ int launch_fwd(const void* qkv, void* out, float* lse2, long long batch, int seq
                           C::ATOM_COLS == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
         if (r) return r;
     }
-    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false>>(C::SMEM_TOTAL2)) return e;
-    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true>>(C::SMEM_TOTAL2)) return e;
+    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, false>>(C::SMEM_TOTAL2)) return e;
+    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, false>>(C::SMEM_TOTAL2)) return e;
+    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, true>>(C::SMEM_TOTAL2)) return e;
+    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, true>>(C::SMEM_TOTAL2)) return e;
     const float scale_log2e = 1.4426950408889634f / sqrtf((float)HD);
     const long long ctas = batch * num_heads * ((seq_len + Q_TILE - 1) / Q_TILE);
     if (ctas > 0x7fffffffll) return -2;
-    auto kern = drop_thr < 0 ? attention_fwd_v2_kernel<HD, false> : attention_fwd_v2_kernel<HD, true>;
+    auto kern = key_mask ? (drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, true> : attention_fwd_v2_kernel<HD, true, true>)
+                         : (drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, false> : attention_fwd_v2_kernel<HD, true, false>);
     kern<<<(unsigned)ctas, NUM_THREADS2, C::SMEM_TOTAL2, st>>>(
         tm, (bf16*)out, lse2, d_model, num_heads, seq_len, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr),
-        rescale);
+        rescale, key_mask);
     return -(int)cudaGetLastError();
 }
 
 }  // namespace v2
+
+// words [batch, ceil(S / 32)]: bit k % 32 of word k / 32 = !pad[b, k] (key k valid), clear for k >= S; one thread per word
+__global__ void __launch_bounds__(256) attention_pack_key_mask_kernel(const uint8_t* __restrict__ pad, uint32_t* __restrict__ words,
+                                                                      long long batch, int seq_len) {
+    const int per_seq = (seq_len + 31) / 32;
+    const long long w = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (w >= batch * per_seq) return;
+    const long long b = w / per_seq;
+    const int k0 = static_cast<int>(w - b * per_seq) * 32;
+    const uint8_t* row = pad + b * seq_len;
+    uint32_t bits = 0u;
+    for (int i = 0; i < 32 && k0 + i < seq_len; ++i) bits |= static_cast<uint32_t>(row[k0 + i] == 0) << i;
+    words[w] = bits;
+}
+
+static int attention_fwd_entry(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads,
+                               int d_model, unsigned long long seed, int drop_thr, float rescale, cudaStream_t st,
+                               const uint32_t* key_mask) {
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
+    if (hd == 32) return v2::launch_fwd<32>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    if (hd == 64) return v2::launch_fwd<64>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    return v2::launch_fwd<128>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+}
 
 }  // namespace attn
 }  // namespace lah
@@ -251,15 +347,25 @@ extern "C" {
 // drop_thr < 0: no dropout; otherwise attention dropout with threshold drop_thr (dropout.cuh), seed, rescale = 1 / (1 - p)
 int lah_attention_fwd(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
                       unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
-    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
-    const int hd = d_model / num_heads;
-    if (hd != 32 && hd != 64 && hd != 128) return -2;
-    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
-    const long long batch = tokens / seq_len;
-    if (batch == 0) return 0;
-    if (hd == 32) return v2::launch_fwd<32>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st);
-    if (hd == 64) return v2::launch_fwd<64>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st);
-    return v2::launch_fwd<128>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st);
+    return attention_fwd_entry(qkv, out, lse2, tokens, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, nullptr);
+}
+
+// lah_attention_fwd with a key padding mask: key_mask [batch, ceil(seq_len / 32)] uint32 from lah_pack_key_mask (NULL: no
+// mask).  A sequence without a valid key gets out = 0 and lse2 = +inf.
+int lah_attention_fwd_masked(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads,
+                             int d_model, unsigned long long seed, int drop_thr, float rescale, cudaStream_t st,
+                             const uint32_t* key_mask) {
+    return attention_fwd_entry(qkv, out, lse2, tokens, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+}
+
+// pad: [batch, seq_len] bool (torch's src_key_padding_mask, true = ignored key) -> words [batch, ceil(seq_len / 32)] uint32
+// of valid-key bits.  Returns -2 for a sequence length out of range.
+int lah_pack_key_mask(const void* pad, void* words, long long batch, int seq_len, cudaStream_t st) {
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || batch < 0) return -2;
+    const long long n = batch * ((seq_len + 31) / 32);
+    if (n == 0) return 0;
+    attention_pack_key_mask_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const uint8_t*)pad, (uint32_t*)words, batch, seq_len);
+    return -(int)cudaGetLastError();
 }
 
 }  // extern "C"

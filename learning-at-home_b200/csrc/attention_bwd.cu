@@ -37,6 +37,11 @@
 // partial block P^T and dS^T are forced to exactly 0: queries >= S get LSE = +inf and Delta = 0 (LSE and Delta are only
 // read for valid queries), keys >= S get S^T = -inf.  No dK / dV row is stored for keys >= S and no dQ-partial row for
 // queries >= S.  Full blocks run exactly the arithmetic of the 512-token kernel.
+//
+// Key padding mask (MASK instantiations; format of attention.cu, bits of keys >= S clear): a CTA whose 128 keys hold no
+// valid key does no MMA and loads nothing; it writes exact zeros to its dK / dV rows and a zero dQ partial (slice j), so
+// attn_dq_reduce_kernel stays mask-blind.  In a partially valid block S^T of masked keys is set to -inf, as for keys >= S,
+// so P^T and dS^T are exactly 0 and so are those dK / dV rows.  A sequence without a valid key has LSE = +inf.
 #include "sm90.cuh"
 #include "dropout.cuh"
 
@@ -70,12 +75,13 @@ struct Bwd {
     static constexpr int SMEM_TOTAL = OFF_BAR + NUM_BARS * 8 + 16 + 1024;
 };
 
-template <int HD, bool DROP>
+template <int HD, bool DROP, bool MASK>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
                      bf16* __restrict__ dq_part, long long total_tokens, int d_model, int num_heads, int seq_len, float scale,
-                     float scale_log2e, unsigned long long seed, uint32_t thr, float rescale) {
+                     float scale_log2e, unsigned long long seed, uint32_t thr, float rescale,
+                     const uint32_t* __restrict__ key_mask) {
     using C = Bwd<HD>;
     constexpr int QB = C::QB, ACOLS = C::ATOM_COLS, ROW_BYTES = C::ROW_BYTES;
     constexpr int OFF_K = C::OFF_K, OFF_V = C::OFF_V, OFF_Q = C::OFF_Q, OFF_DO = C::OFF_DO, OFF_DS = C::OFF_DS;
@@ -95,6 +101,32 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     const int head = (blockIdx.x / num_kb) % num_heads;
     const int batch = (blockIdx.x / num_kb) / num_heads;
     const long long seq0 = static_cast<long long>(batch) * seq_len;
+    const int key_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // row of the block (+ 8 for h = 1)
+    uint32_t kvalid = 3u;   // MASK: bit h set iff key key_row + 8 h of this block is valid
+    if constexpr (MASK) {
+        const int mask_words = (seq_len + 31) / 32;
+        uint32_t w[BLK / 32];
+#pragma unroll
+        for (int i = 0; i < BLK / 32; ++i)
+            w[i] = j * (BLK / 32) + i < mask_words ? __ldg(key_mask + batch * mask_words + j * (BLK / 32) + i) : 0u;
+        if (!(w[0] | w[1] | w[2] | w[3])) {   // no valid key: zero dK_j / dV_j rows and dQ partial j, nothing else
+            constexpr int V8 = HD / 8;   // 16 B vectors per head row
+            const int keys = min(BLK, seq_len - j * BLK);
+            for (int e = tid; e < 2 * keys * V8; e += NUM_THREADS) {
+                const int t = e / (keys * V8), r = (e / V8) % keys, c = e % V8;
+                *reinterpret_cast<int4*>(dqkv + (seq0 + j * BLK + r) * (3ll * d_model) + (1 + t) * d_model + head * HD + 8 * c) =
+                    make_int4(0, 0, 0, 0);
+            }
+            for (int e = tid; e < seq_len * V8; e += NUM_THREADS)
+                *reinterpret_cast<int4*>(dq_part + (static_cast<long long>(j) * total_tokens + seq0 + e / V8) * d_model +
+                                         head * HD + 8 * (e % V8)) = make_int4(0, 0, 0, 0);
+            return;
+        }
+        const unsigned long long lo = w[0] | static_cast<unsigned long long>(w[1]) << 32,   // keys 0-63, 64-127
+                                 hi = w[2] | static_cast<unsigned long long>(w[3]) << 32;
+        const unsigned long long mine = (key_row < 64 ? lo : hi) >> (key_row & 63);   // key_row and key_row + 8: same half
+        kvalid = static_cast<uint32_t>(mine & 1u) | static_cast<uint32_t>((mine >> 8) & 1u) << 1;
+    }
 
     auto load_q = [&](int i) {   // thread 0 only; stage i & 1 must be free
         const int st = i & 1;
@@ -145,7 +177,6 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     __syncthreads();
 
     const uint32_t sk = smem_u32(smem + OFF_K), sv = smem_u32(smem + OFF_V), sds = smem_u32(smem + OFF_DS);
-    const int key_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // row of the block (+ 8 for h = 1)
     const int qcol = 2 * (lane & 3);                               // query column (+ 8 jj, + 1)
     float dv[HD / 2], dk[HD / 2];
 #pragma unroll
@@ -180,7 +211,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         wgmma_wait<0>();
         wgmma_fence_regs(sacc);
         wgmma_fence_regs(dpacc);
-        if (j * BLK + BLK > seq_len) {   // last key block of a partial sequence: sacc[4 jj + 2 h + par] is key key_row + 8 h
+        if constexpr (MASK) {   // masked keys and keys >= S: sacc[4 jj + 2 h + par] is key key_row + 8 h
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (!((kvalid >> h) & 1u))
+#pragma unroll
+                    for (int jj = 0; jj < QB / 8; ++jj) sacc[4 * jj + 2 * h] = sacc[4 * jj + 2 * h + 1] = -INFINITY;
+        } else if (j * BLK + BLK > seq_len) {   // last key block of a partial sequence: sacc[4 jj + 2 h + par] is key key_row + 8 h
 #pragma unroll
             for (int h = 0; h < 2; ++h)
                 if (j * BLK + key_row + 8 * h >= seq_len)
@@ -352,7 +389,7 @@ __global__ void __launch_bounds__(256) attn_dq_reduce_kernel(const bf16* __restr
 template <int HD>
 int launch_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv, void* dq_part,
                long long tokens, long long batch, int seq_len, int num_heads, int d_model, unsigned long long seed,
-               int drop_thr, float rescale, cudaStream_t st) {
+               int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
     using C = Bwd<HD>;
     CUtensorMap tm_qkv, tm_do;
     const uint32_t box[3] = {C::ATOM_COLS, C::QB, 1};
@@ -369,20 +406,42 @@ int launch_bwd(const void* qkv, const void* out, const void* dout, const float* 
         int r = make_tmap(&tm_do, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dout, dims, str, box, swz);
         if (r) return r;
     }
-    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false>>(C::SMEM_TOTAL)) return e;
-    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true>>(C::SMEM_TOTAL)) return e;
+    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, false>>(C::SMEM_TOTAL)) return e;
+    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, false>>(C::SMEM_TOTAL)) return e;
+    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, true>>(C::SMEM_TOTAL)) return e;
+    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, true>>(C::SMEM_TOTAL)) return e;
     const float scale = 1.f / sqrtf((float)HD);
     const int blocks = (seq_len + BLK - 1) / BLK;
     const long long pairs = tokens * num_heads, ctas = batch * num_heads * blocks;
     if (ctas > 0x7fffffffll) return -2;
     attn_delta_kernel<HD><<<(unsigned)((pairs * 32 + 255) / 256), 256, 0, st>>>((const bf16*)dout, (const bf16*)out, delta, pairs);
-    auto kern = drop_thr < 0 ? attention_bwd_kernel<HD, false> : attention_bwd_kernel<HD, true>;
+    auto kern = key_mask ? (drop_thr < 0 ? attention_bwd_kernel<HD, false, true> : attention_bwd_kernel<HD, true, true>)
+                         : (drop_thr < 0 ? attention_bwd_kernel<HD, false, false> : attention_bwd_kernel<HD, true, false>);
     kern<<<(unsigned)ctas, NUM_THREADS, C::SMEM_TOTAL, st>>>(
         tm_qkv, tm_do, lse2, delta, (bf16*)dqkv, (bf16*)dq_part, tokens, d_model, num_heads, seq_len, scale,
-        scale * 1.4426950408889634f, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale);
+        scale * 1.4426950408889634f, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale, key_mask);
     attn_dq_reduce_kernel<<<(unsigned)((tokens * d_model / 8 + 255) / 256), 256, 0, st>>>((const bf16*)dq_part, (bf16*)dqkv, tokens, d_model,
                                                                                          blocks);
     return -(int)cudaGetLastError();
+}
+
+static int attention_bwd_entry(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta,
+                               void* dqkv, void* dq_part, long long tokens, int seq_len, int num_heads, int d_model,
+                               unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
+    if (hd == 32)
+        return launch_bwd<32>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
+                              drop_thr, rescale, st, key_mask);
+    if (hd == 64)
+        return launch_bwd<64>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
+                              drop_thr, rescale, st, key_mask);
+    return launch_bwd<128>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
+                           drop_thr, rescale, st, key_mask);
 }
 
 }  // namespace attnb
@@ -402,20 +461,16 @@ extern "C" {
 int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
                       void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
                       int drop_thr, float rescale, cudaStream_t st) {
-    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
-    const int hd = d_model / num_heads;
-    if (hd != 32 && hd != 64 && hd != 128) return -2;
-    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
-    const long long batch = tokens / seq_len;
-    if (batch == 0) return 0;
-    if (hd == 32)
-        return launch_bwd<32>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                              drop_thr, rescale, st);
-    if (hd == 64)
-        return launch_bwd<64>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                              drop_thr, rescale, st);
-    return launch_bwd<128>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                           drop_thr, rescale, st);
+    return attention_bwd_entry(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, seq_len, num_heads, d_model, seed, drop_thr,
+                               rescale, st, nullptr);
+}
+
+// lah_attention_bwd with the key padding mask of lah_attention_fwd_masked (NULL: no mask)
+int lah_attention_bwd_masked(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
+                             void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
+                             int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
+    return attention_bwd_entry(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, seq_len, num_heads, d_model, seed, drop_thr,
+                               rescale, st, key_mask);
 }
 
 }  // extern "C"

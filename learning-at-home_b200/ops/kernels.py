@@ -56,6 +56,9 @@ def _lib():
         "lah_cast_bf16": [P, P, L, P],
         "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
         "lah_attention_bwd": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P],
+        "lah_attention_fwd_masked": [P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
+        "lah_attention_bwd_masked": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
+        "lah_pack_key_mask": [P, P, L, I, P],
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
         "lah_symm_alloc": [c_ull, ctypes.POINTER(c_void_p)],
@@ -270,16 +273,52 @@ MAX_SEQ = 65536   # longest sequence of the attention kernels (csrc/dropout.cuh 
 HEAD_DIMS = (32, 64, 128)   # head dims d_model / num_heads of the attention kernels (csrc/attention.cu, attention_bwd.cu)
 
 
-def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=512):
+def pack_key_mask(pad):
+    """
+    Packs a key padding mask for ``attention_fwd`` / ``attention_bwd`` (csrc/attention.cu, one launch).
+    :param pad: bool [batch, seq_len] CUDA tensor in torch's ``src_key_padding_mask`` convention: True = key ignored
+    :returns: int32 [batch, ceil(seq_len / 32)]: bit k % 32 of word k / 32 is set iff key k is valid (not padding); bits of
+        keys >= seq_len are clear
+    """
+    assert pad.is_cuda and pad.dtype == torch.bool and pad.dim() == 2 and pad.is_contiguous(), (pad.dtype, tuple(pad.shape))
+    batch, seq_len = pad.shape
+    assert 1 <= seq_len <= MAX_SEQ, seq_len
+    words = torch.empty(batch, (seq_len + 31) // 32, dtype=torch.int32, device=pad.device)
+    native.check(_lib().lah_pack_key_mask(ptr(pad), ptr(words), batch, seq_len, stream_ptr()), "lah_pack_key_mask")
+    native.count_launch()
+    return words
+
+
+def pack_key_mask_ref(pad):
+    """CPU oracle of ``pack_key_mask``"""
+    batch, seq_len = pad.shape
+    n = (seq_len + 31) // 32
+    valid = torch.zeros(batch, n * 32, dtype=torch.int64)
+    valid[:, :seq_len] = (~pad.cpu()).long()
+    bits = (valid.view(batch, n, 32) << torch.arange(32)).sum(-1)
+    return torch.where(bits >= 2 ** 31, bits - 2 ** 32, bits).to(torch.int32)
+
+
+def _check_key_mask(key_mask, tokens, seq_len, device):
+    if key_mask is not None:
+        assert key_mask.dtype == torch.int32 and key_mask.is_contiguous() and key_mask.device == device
+        assert key_mask.shape == (tokens // seq_len, (seq_len + 31) // 32), (tuple(key_mask.shape), tokens, seq_len)
+
+
+def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=512, key_mask=None):
     """
     Self-attention over sequences of ``seq_len`` tokens (1 <= seq_len <= MAX_SEQ) on wgmma (csrc/attention.cu).
     :param qkv: [batch*seq_len, 3*d_model] bf16 = in_proj output, [q | k | v] per token; num_heads must divide d_model and
         the head dim d_model / num_heads must be in HEAD_DIMS
     :param out: optional [batch*seq_len, d_model] bf16 destination (may be the leading rows of a larger buffer)
     :param lse: optional fp32 [batch*seq_len, num_heads]: receives the base-2 row log-sum-exp (needed by attention_bwd); with
-        dropout it is still that of the undropped softmax
+        dropout it is still that of the undropped softmax.  A row with no valid key gets lse = +inf, which attention_bwd
+        reads as "P is exactly 0"
     :param dropout: (p, seed): O = (M o P) V / (1 - p) with the site-0 mask of ``dropout_mask``; p = 0 or None launches the
         kernel without dropout
+    :param key_mask: optional key padding mask from ``pack_key_mask``: masked keys are ignored by every query of their
+        sequence (queries at padded positions are still computed); key blocks of 128 without a valid key are skipped.  A
+        sequence without a valid key gets out = 0.  None launches the unmasked kernel
     :returns: [batch*seq_len, d_model] bf16, heads concatenated (input of out_proj)
     """
     tokens, three_d = qkv.shape
@@ -292,14 +331,15 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=5
     assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (tokens, d_model)
     if lse is not None:
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == tokens * num_heads
+    _check_key_mask(key_mask, tokens, seq_len, qkv.device)
     seed, thr, rescale = _dropout_args(dropout)
-    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed, thr,
-                                          rescale, stream_ptr()), "lah_attention_fwd")
+    native.check(_lib().lah_attention_fwd_masked(ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed,
+                                                 thr, rescale, stream_ptr(), ptr(key_mask)), "lah_attention_fwd_masked")
     native.count_launch()
     return out
 
 
-def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, dqkv=None):
+def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, dqkv=None, key_mask=None):
     """
     Backward of ``attention_fwd`` on wgmma (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
     dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.  Same head dims as
@@ -308,6 +348,8 @@ def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, 
     tokens, 32x at 4096), and the fp32 [tokens, num_heads] row sums Delta.
     :param dropout: the (p, seed) of the forward that produced ``out``; the mask is regenerated, not read
     :param dqkv: optional contiguous [tokens, 3*d_model] bf16 destination
+    :param key_mask: the ``pack_key_mask`` words of the forward.  dK / dV rows of masked keys are exactly 0; a 128-key block
+        without a valid key does no MMA and writes a zero dQ partial
     """
     tokens, three_d = qkv.shape
     d_model = three_d // 3
@@ -321,20 +363,30 @@ def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, 
     assert dqkv.dtype == torch.bfloat16 and dqkv.is_contiguous() and dqkv.shape == qkv.shape
     blocks = (seq_len + 127) // 128
     dq_part = torch.empty(blocks, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
-    native.check(_lib().lah_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
-                                          tokens, int(seq_len), num_heads, d_model, *_dropout_args(dropout), stream_ptr()),
-                 "lah_attention_bwd")
+    _check_key_mask(key_mask, tokens, seq_len, qkv.device)
+    native.check(_lib().lah_attention_bwd_masked(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
+                                                 tokens, int(seq_len), num_heads, d_model, *_dropout_args(dropout), stream_ptr(),
+                                                 ptr(key_mask)),
+                 "lah_attention_bwd_masked")
     native.count_launch(3)   # delta prologue, wgmma backward, dQ partial reduction
     return dqkv
 
 
-def attention_ref(qkv, num_heads, seq_len=512):
-    """fp32 oracle: softmax(q k^T / sqrt(d)) v per head"""
+def attention_ref(qkv, num_heads, seq_len=512, key_mask=None):
+    """fp32 oracle (fp64 for a fp64 input): softmax(q k^T / sqrt(d)) v per head.
+    :param key_mask: optional bool [batch, seq_len], True = key ignored (torch's src_key_padding_mask): its scores are -inf;
+        rows without a valid key give 0 (``softmax(...).nan_to_num(0)``, which is what torch's layer computes in training mode)"""
     tokens, three_d = qkv.shape
     d = three_d // 3
-    q, k, v = qkv.float().view(tokens // seq_len, seq_len, 3, num_heads, d // num_heads).unbind(2)
+    x = qkv if qkv.dtype == torch.float64 else qkv.float()
+    q, k, v = x.view(tokens // seq_len, seq_len, 3, num_heads, d // num_heads).unbind(2)
     q, k, v = (t.transpose(1, 2) for t in (q, k, v))  # [B, H, S, hd]
-    att = torch.softmax(q @ k.transpose(-1, -2) / (d // num_heads) ** 0.5, dim=-1) @ v
+    s = q @ k.transpose(-1, -2) / (d // num_heads) ** 0.5
+    if key_mask is None:
+        att = torch.softmax(s, dim=-1) @ v
+    else:
+        s = s.masked_fill(key_mask.to(s.device).view(tokens // seq_len, 1, 1, seq_len), float("-inf"))
+        att = torch.softmax(s, dim=-1).nan_to_num(0.0) @ v
     return att.transpose(1, 2).reshape(tokens, d)
 
 

@@ -36,8 +36,14 @@ class ExpertBackend(nn.Module):
             ``norm_first`` True or False, ``batch_first`` True or False, LayerNorm eps 1e-5 and all biases, head dim
             d_model / nhead in (32, 64, 128), d_model and dim_feedforward multiples of 256, dropout p < 1 at every site,
             sequence length 1 <= S <= 65536 (wgmma attention and GEMMs, in-kernel dropout, fused AMSGrad).
-        Anything else (another class, tanh GELU, kdim / vdim, bias=False, other widths or inputs, CPU tensors) runs on
-        the module itself"""
+        ``torch.nn.TransformerEncoderLayer`` also runs natively with a key padding mask: one positional input and
+        ``kwargs_schema={"src_key_padding_mask": BatchTensorProto(S, dtype=torch.bool)}`` (True = padding key, [batch, S]
+        for sequence-first layers too).  The flat inputs are then (src, mask) for forward and (src, mask, grad_out) for
+        backward, which returns (dx, zeros_like(mask)), as on the module.  A sequence whose keys are all masked gets the
+        result of torch's layer in training mode (zero attention output) in eval mode too; torch's eval fast path returns
+        NaN for it.
+        Anything else (another class, tanh GELU, kdim / vdim, bias=False, other widths or inputs, float masks, other
+        keyword inputs, CPU tensors) runs on the module itself"""
         super().__init__()
         self.expert, self.opt, self.name = expert, opt, name
         self.native, self._executor, self._executor_key = native, None, None
@@ -64,10 +70,19 @@ class ExpertBackend(nn.Module):
         self.update_count = 0
 
     # ------------------------------------------------------------------ tasks
+    def _key_padding_schema(self) -> bool:
+        """True when the keyword inputs are exactly a bool key padding mask [batch, S]"""
+        proto = self.kwargs_schema.get("src_key_padding_mask")
+        return (len(self.kwargs_schema) == 1 and proto is not None and len(proto.size) == 2
+                and proto == BatchTensorProto(proto.size[1], dtype=torch.bool))
+
     def native_executor(self, inputs):
-        """the sm_90a executor of this expert, or None (CPU tensors, unsupported expert / optimizer, no GPU).  Inputs the
-        executor does not accept (``executor.accepts``: rank, feature size, sequence length) run on the module itself."""
-        if not self.native or len(inputs) < 1 or not inputs[0].is_cuda or self.kwargs_schema or len(self.args_schema) != 1:
+        """the sm_90a executor of this expert, or None (CPU tensors, unsupported expert / optimizer / keyword inputs, no
+        GPU).  Inputs the executor does not accept (``executor.accepts``: rank, feature size, sequence length, mask shape)
+        run on the module itself."""
+        if not self.native or len(inputs) < 1 or not inputs[0].is_cuda or len(self.args_schema) != 1:
+            return None
+        if self.kwargs_schema and not self._key_padding_schema():
             return None
         first = next(self.expert.parameters(), None)
         key = (id(first), first.device if first is not None else None)
@@ -76,12 +91,15 @@ class ExpertBackend(nn.Module):
             self._executor, self._executor_key = make_executor(self.expert, self.opt), key
             if self._executor is not None:
                 self._executor_key = (id(next(self.expert.parameters())), first.device)
+        if self.kwargs_schema and not getattr(self._executor, "takes_key_padding_mask", False):
+            return None
         return self._executor
 
     def forward(self, *inputs: torch.Tensor) -> Tuple[torch.Tensor, ...]:
         executor = self.native_executor(inputs)
-        if executor is not None and executor.accepts(inputs[0]):
-            return (executor.forward(inputs[0]),)
+        mask = inputs[1:2] if self.kwargs_schema else ()   # (src_key_padding_mask,) when the schema has it
+        if executor is not None and len(inputs) == 1 + len(mask) and executor.accepts(inputs[0], *mask):
+            return (executor.forward(inputs[0], *mask),)
         args, kwargs = nested_pack(inputs, structure=self.forward_schema)
         with torch.no_grad():
             outputs = self.expert(*args, **kwargs)
@@ -89,10 +107,13 @@ class ExpertBackend(nn.Module):
 
     def backward(self, *inputs: torch.Tensor) -> Tuple[torch.Tensor, ...]:
         executor = self.native_executor(inputs)
-        if executor is not None and len(inputs) == 2 and executor.accepts(inputs[0]):
-            grad_x = executor.backward(inputs[0], inputs[1].to(inputs[0].device))   # dgrad + fused wgrad/AMSGrad: one update
+        mask = inputs[1:2] if self.kwargs_schema else ()
+        n = 1 + len(mask)
+        if executor is not None and len(inputs) == n + 1 and executor.accepts(inputs[0], *mask):
+            # dgrad + fused wgrad/AMSGrad: one update
+            grad_x = executor.backward(inputs[0], inputs[n].to(inputs[0].device), *mask)
             self.update_count += 1
-            return (grad_x,)
+            return (grad_x, *(torch.zeros_like(m) for m in mask))
         (args, kwargs), grad_outputs = nested_pack(inputs, structure=self.backward_schema)
         with torch.enable_grad():
             args = [t.detach().clone().requires_grad_(t.is_floating_point()) for t in args]

@@ -308,15 +308,25 @@ class NativeTransformerExecutor:
 
     Like the FFN executor, module parameters and optimizer state are views of flat fp32 buffers (state_dict / checkpoints
     keep the reference key names: self_attn.in_proj_weight, linear1.weight, norm1.weight, ...).
+
+    Key padding mask (torch.nn.TransformerEncoderLayer only, ``takes_key_padding_mask``): ``forward`` / ``backward`` take
+    torch's bool ``src_key_padding_mask`` [batch, S] (sequence-first layers too; True = key ignored).  It is packed once per
+    call (``K.pack_key_mask``) and given to the attention forward, its backward recompute and the attention backward; every
+    other kernel is unchanged.  A sequence whose keys are all masked gets a zero attention output, as torch's layer in
+    training mode; torch's eval fast path returns NaN for it.
     """
     NAMES = ("w_in", "b_in", "w_out", "b_out", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
     INPUT_DIMS = 3   # [batch, seq, d_model], or [seq, batch, d_model] for a sequence-first layer
 
-    def accepts(self, x) -> bool:
+    def accepts(self, x, key_padding_mask=None) -> bool:
         """True when ``x`` is an input this executor runs: [batch, S, d_model] (sequence-first: [S, batch, d_model]) with
-        1 <= S <= K.MAX_SEQ"""
+        1 <= S <= K.MAX_SEQ, and ``key_padding_mask`` None or (torch's layer only) a bool [batch, S] tensor on x's device"""
         seq = x.shape[1 if self.batch_first else 0] if x.dim() == self.INPUT_DIMS else 0
-        return x.dim() == self.INPUT_DIMS and x.shape[2] == self.d and 1 <= seq <= K.MAX_SEQ
+        if not (x.dim() == self.INPUT_DIMS and x.shape[2] == self.d and 1 <= seq <= K.MAX_SEQ):
+            return False
+        m = key_padding_mask
+        return m is None or (self.takes_key_padding_mask and m.dtype == torch.bool and m.device == x.device
+                             and tuple(m.shape) == self._batch_seq(x))
 
     @staticmethod
     def supports(expert, opt) -> bool:
@@ -355,6 +365,7 @@ class NativeTransformerExecutor:
         self.expert, self.opt = expert, opt
         spec = encoder_layer_spec(expert)
         self.d, self.heads, self.ff = spec.d, spec.heads, spec.ff
+        self.takes_key_padding_mask = class_name(expert) == TORCH_ENCODER_LAYER   # this package's layer has no mask input
         self.norm_first, self.relu, self.batch_first = spec.norm_first, spec.activation == "relu", spec.batch_first
         attn = expert.self_attn
         self.params = [attn.in_proj_weight, attn.in_proj_bias, attn.out_proj.weight, attn.out_proj.bias, expert.linear1.weight,
@@ -447,8 +458,13 @@ class NativeTransformerExecutor:
             return None
         return (drop[1][site], drop[0]) if site == K.SITE_ATTN else (drop[1][site], drop[0], site)
 
-    def _forward(self, src, drop=None):
-        """returns the workspace, the real token rows Tr = batch * seq and the padded rows T (a multiple of 128)"""
+    @staticmethod
+    def _pack(key_padding_mask):
+        return None if key_padding_mask is None else K.pack_key_mask(key_padding_mask.contiguous())
+
+    def _forward(self, src, drop=None, key_mask=None):
+        """returns the workspace, the real token rows Tr = batch * seq and the padded rows T (a multiple of 128);
+        key_mask: packed key padding mask (``_pack``) or None"""
         from ..ops import gemm
         assert self.accepts(src), (tuple(src.shape), self.d)
         batch, seq = self._batch_seq(src)
@@ -464,7 +480,7 @@ class NativeTransformerExecutor:
             K.ln_relu_fwd(x, pv["g1"], pv["be1"], None, out=ws["xa"], mean=stats[0], rstd=stats[1], relu=False)
         gemm.grouped_linear(ws["xa"] if self.norm_first else x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
         K.attention_fwd(ws["qkv"][:Tr], self.heads, out=ws["att"][:Tr], lse=ws["lse"][:Tr], dropout=site(drop, K.SITE_ATTN),
-                        seq_len=seq)
+                        seq_len=seq, key_mask=key_mask)
         gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"],
                             dropout=site(drop, K.SITE_OUT_PROJ))
         if self.norm_first:   # x1 = LN2(h) feeds the feed-forward branch, h is its residual
@@ -484,15 +500,16 @@ class NativeTransformerExecutor:
         return ws, Tr, T
 
     @torch.no_grad()
-    def forward(self, src: torch.Tensor) -> torch.Tensor:
-        ws, Tr, T = self._forward(src, self._dropout())
+    def forward(self, src: torch.Tensor, key_padding_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        ws, Tr, T = self._forward(src, self._dropout(), self._pack(key_padding_mask))
         return self._from_rows(ws["y" if self.norm_first else "out"][:Tr], src)
 
     @torch.no_grad()
-    def backward(self, src: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
+    def backward(self, src: torch.Tensor, grad_out: torch.Tensor, key_padding_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
         from ..ops import gemm
         drop = self._dropout()
-        ws, Tr, T = self._forward(src, drop)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
+        key_mask = self._pack(key_padding_mask)
+        ws, Tr, T = self._forward(src, drop, key_mask)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
         d, bv, pv, gv, site, stats = self.d, self.bv, self.pv, self.gv, self._site, ws["stats"]
         go = ws["group_off"]
         bf = dict(dtype=torch.bfloat16, device=self.device)
@@ -551,9 +568,10 @@ class NativeTransformerExecutor:
             dqkv = torch.empty(T, 3 * d, **bf)
             dqkv[Tr:].zero_()
             K.attention_bwd(ws["qkv"][:Tr], ws["att"][:Tr], datt[:Tr], ws["lse"][:Tr], self.heads, dropout=site(drop, K.SITE_ATTN),
-                            seq_len=seq, dqkv=dqkv[:Tr])
+                            seq_len=seq, dqkv=dqkv[:Tr], key_mask=key_mask)
         else:
-            dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN), seq_len=seq)
+            dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN), seq_len=seq,
+                                   key_mask=key_mask)
         K.grouped_colsum(dqkv, None, out=gv["b_in"])
         if self.norm_first:   # dx = dh + LN1 backward(dxa)
             gemm.grouped_wgrad(dqkv, ws["xa"], go, 1, out=gv["w_in"])
