@@ -36,8 +36,13 @@ struct AdamArgs {
     int num_ranges; long long r_start[6]; long long r_cum[7];
     int dead_mask;       // ranks excluded from the peer gradient reduce (their buffers hold stale data)
     const int* poison;   // status word: bit 0 set (a peer-flag wait timed out in this step) -> no update from partial data
+    // decoupled weight decay (AdamW, Adam(decoupled_weight_decay=True)): p *= decay before the moments, decay = 1 - lr * wd
+    // computed in double by the caller and rounded to fp32 once, as torch's scalar multiply does.  Read only by the
+    // DECOUPLED instantiation; the other one keeps the L2 form (grad += weight_decay * p)
+    float decay;
 };
 
+template <bool DECOUPLED>
 __global__ void __launch_bounds__(256) adam_kernel(AdamArgs a) {
     if (a.poison && (*a.poison & 1)) return;
     const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
@@ -94,7 +99,8 @@ __global__ void __launch_bounds__(256) adam_kernel(AdamArgs a) {
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
             float grad = gp[t];
-            if (a.weight_decay != 0.f) grad += a.weight_decay * pp[t];
+            if constexpr (DECOUPLED) pp[t] = __fmul_rn(pp[t], a.decay);   // rounded on its own, as torch's p.mul_()
+            else if (a.weight_decay != 0.f) grad += a.weight_decay * pp[t];
             mp[t] = mp[t] + (1.f - a.beta1) * (grad - mp[t]);
             vp[t] = vp[t] * a.beta2 + (1.f - a.beta2) * grad * grad;
             float denom;
@@ -146,13 +152,16 @@ extern "C" const int* lah_get_poison_word();
 
 extern "C" {
 
-int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
-                  const long long* seg_n, int G,
-                  const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
-                  float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
-                  const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
-                  long long shadow_g_off, int me, int seg_mask, int dead_mask, cudaStream_t st) {
+// decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); weight_decay: the L2 coefficient.  At most one of the
+// two forms per launch.
+int lah_adam_step_wd(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
+                     const long long* seg_n, int G,
+                     const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
+                     float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
+                     const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
+                     long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay, cudaStream_t st) {
     if (num_segs < 1 || num_segs > 12) return -2;
+    if (decay != 1.f && weight_decay != 0.f) return -2;
     AdamArgs a;
     a.num_segs = num_segs;
     long long off = 0;
@@ -173,6 +182,7 @@ int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_b
     for (int i = 0; i < 8; ++i) a.peer_base[i] = (peer_bases && i < world) ? (char*)peer_bases[i] : nullptr;
     a.poison = lah_get_poison_word();
     a.dead_mask = dead_mask;
+    a.decay = decay;
     a.num_ranges = 0;
     a.r_cum[0] = 0;
     if (seg_mask) {   // adjacent selected segments merge into one range
@@ -194,8 +204,22 @@ int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_b
     if (span <= 0) return 0;
     long long blocks = (span / 4 + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    adam_kernel<<<(int)blocks, 256, 0, st>>>(a);
+    if (decay != 1.f)
+        adam_kernel<true><<<(int)blocks, 256, 0, st>>>(a);
+    else
+        adam_kernel<false><<<(int)blocks, 256, 0, st>>>(a);
     return -(int)cudaGetLastError();
+}
+
+int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
+                  const long long* seg_n, int G,
+                  const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
+                  float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
+                  const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
+                  long long shadow_g_off, int me, int seg_mask, int dead_mask, cudaStream_t st) {
+    return lah_adam_step_wd(p, g, m, v, vmax, p_bf16, num_segs, seg_n, G, step, group_rows, step_scalar, lr, beta1, beta2,
+                            eps, weight_decay, amsgrad, zero_mask, world, peer_grad_off, peer_bases, grad_scale, G_active,
+                            shadow_of, shadow_g_off, me, seg_mask, dead_mask, 1.f, st);
 }
 
 int lah_bump_steps(int* step, const int* group_rows, int G, cudaStream_t st) {

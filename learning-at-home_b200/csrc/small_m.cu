@@ -321,9 +321,14 @@ struct Params {
     bf16* p_bf16;             // [G, N, K] bf16 mirror consumed by the GEMMs
     float lr, beta1, beta2, eps;
     int amsgrad;
+    float wd;                 // WD_L2: grad += wd * p;  WD_DECOUPLED: p *= wd before the moments, wd = 1 - lr * weight_decay
+                              // rounded to fp32 by the caller (in the padding after amsgrad: the layout stays as it was)
     int* tile_counter;        // work-stealing tile counter (zeroed before the launch)
     const int* poison;        // optional status word: a step that timed out on a peer must not update anything
 };
+
+// weight-decay form of one launch (a template parameter: the WD_NONE instantiation is the kernel without decay)
+constexpr int WD_NONE = 0, WD_L2 = 1, WD_DECOUPLED = 2;
 
 struct Tile {
     int g, mt, nt;
@@ -334,6 +339,7 @@ struct StateMaps {
     CUtensorMap a[4];
 };
 
+template <int WD>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX,
                   const __grid_constant__ StateMaps tmS) {
@@ -525,7 +531,9 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                     float* pp = &pw.x; float* mp = &m.x; float* vp = &v.x; float* vmp = &vm.x;
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        const float grad = acc[4 * jj + 2 * h + e];
+                        float grad = acc[4 * jj + 2 * h + e];
+                        if constexpr (WD == WD_L2) grad += p.wd * pp[e];
+                        if constexpr (WD == WD_DECOUPLED) pp[e] = __fmul_rn(pp[e], p.wd);   // rounded alone, as p.mul_()
                         mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
                         vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
                         float denom;
@@ -647,12 +655,14 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
     return -(int)cudaGetLastError();
 }
 
-// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror
-int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                   const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                   float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
-                   int max_ctas, cudaStream_t st) {
+// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
+// weight_decay: the L2 coefficient; decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); at most one of the two
+int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                      const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                      float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
+                      float weight_decay, float decay, int max_ctas, cudaStream_t st) {
     if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8) || 1ll * G * N > INT_MAX) return -2;
+    if (decay != 1.f && weight_decay != 0.f) return -2;
     if (amsgrad && !vmax) return -2;   // AMSGrad streams vmax through its own tensor map
     CUtensorMap tmDY, tmX;
     wa::StateMaps tmS;
@@ -683,15 +693,33 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
     wa::Params a;
     a.G = G; a.N = N; a.K = K; a.group_off = group_off; a.group_rows = group_rows; a.skip = skip; a.step = step;
     a.p = p; a.m = m; a.v = v; a.vmax = vmax; a.p_bf16 = (bf16*)p_bf16; a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.amsgrad = amsgrad;
+    a.wd = decay != 1.f ? decay : weight_decay;
     a.tile_counter = tile_counter() ? tile_counter() + 16 : nullptr;   // own word (64 B apart from the GEMM's)
     a.poison = g_poison;
     if (!a.tile_counter) return -3;
     const long long total = 1ll * G * (N / BM) * (K / BN_MAX);
     if (total <= 0) return 0;
     if (cudaMemsetAsync(a.tile_counter, 0, sizeof(int), st) != cudaSuccess) return -4;
-    if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel>(wa::SMEM_TOTAL)) return e;
-    wa::wgrad_adam_kernel<<<persistent_grid(total, max_ctas), NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
+    const int ctas = persistent_grid(total, max_ctas);
+    if (decay != 1.f) {
+        if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<wa::WD_DECOUPLED>>(wa::SMEM_TOTAL)) return e;
+        wa::wgrad_adam_kernel<wa::WD_DECOUPLED><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
+    } else if (weight_decay != 0.f) {
+        if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<wa::WD_L2>>(wa::SMEM_TOTAL)) return e;
+        wa::wgrad_adam_kernel<wa::WD_L2><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
+    } else {
+        if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<wa::WD_NONE>>(wa::SMEM_TOTAL)) return e;
+        wa::wgrad_adam_kernel<wa::WD_NONE><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
+    }
     return -(int)cudaGetLastError();
+}
+
+int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                   const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                   float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
+                   int max_ctas, cudaStream_t st) {
+    return lah_wgrad_adam_wd(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, m, v, vmax, p_bf16,
+                             lr, beta1, beta2, eps, amsgrad, 0.f, 1.f, max_ctas, st);
 }
 
 }  // extern "C"

@@ -40,6 +40,7 @@ def _lib():
         "lah_step_begin": [I, L, P],
         "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, P, I, P],
         "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, I, P],
+        "lah_wgrad_adam_wd": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, Fl, Fl, I, P],
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
@@ -52,6 +53,8 @@ def _lib():
         "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P],
         "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P],
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, P],
+        "lah_adam_step_wd": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
+                             P],
         "lah_bump_steps": [P, P, I, P],
         "lah_cast_bf16": [P, P, L, P],
         "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
@@ -541,31 +544,42 @@ def dropout_mask_ref(shape, p, seed, site):
 # ---------------------------------------------------------------------------------------------------------
 # optimizer
 # ---------------------------------------------------------------------------------------------------------
+def weight_decay_args(lr, weight_decay, decoupled):
+    """(L2 coefficient, decoupled factor) the optimizer kernels take for torch's two weight-decay forms:
+    Adam(weight_decay=wd) adds wd * p to the gradient; AdamW (decoupled) multiplies p by 1 - lr * wd, computed in double and
+    rounded to fp32 once, as torch's ``p.mul_(1 - lr * wd)`` does.  A factor of 1 means no decoupled decay."""
+    if decoupled:
+        return 0.0, 1.0 - float(lr) * float(weight_decay)
+    return float(weight_decay), 1.0
+
+
 def adam_step(p, g, m, v, vmax, p_bf16, seg_sizes, G, *, step=None, group_rows=None, step_scalar=0, lr=1e-3,
-              betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=True, zero_mask=0, world=1,
+              betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, decoupled=False, amsgrad=True, zero_mask=0, world=1,
               peer_grad_off=-1, peer_bases=None, grad_scale=1.0, G_active=0, shadow_of=None, shadow_g_off=-1, me=0,
               seg_mask=0, dead_mask=0):
-    arr = None
-    if peer_bases is not None:
-        arr = (c_ull * len(peer_bases))(*[int(b) for b in peer_bases])
     """
     One fused Adam/AMSGrad step over a flat fp32 buffer laid out as consecutive segments [G, seg_sizes[s]].
     :param step: int32 [G] per-group step counts (already incremented) or None -> step_scalar for everything
     :param group_rows: int32 [G]; groups with 0 rows are skipped (experts that received no tokens are not stepped)
+    :param weight_decay: torch's ``weight_decay``: L2 (added to the gradient), or with ``decoupled`` AdamW's p *= 1 - lr wd
     :param G_active: only the first G_active of the G slots per segment are updated (the rest are shadow replicas)
     :param shadow_of: int32 [G_active, 2] (slot, rank mask): gradient of a shadowed expert = sum of the partial
         gradients in shadow slot ``slot`` of the ranks in ``mask`` (buffers at symmetric offset ``shadow_g_off``)
     """
+    arr = None
+    if peer_bases is not None:
+        arr = (c_ull * len(peer_bases))(*[int(b) for b in peer_bases])
     if isinstance(seg_sizes, int):
         seg_sizes = [seg_sizes]
     segs = (c_ll * len(seg_sizes))(*[int(s) for s in seg_sizes])
-    native.check(_lib().lah_adam_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
-                                      ctypes.cast(segs, c_void_p), G, ptr(step),
-                                      ptr(group_rows), int(step_scalar), lr, betas[0], betas[1], eps, weight_decay,
-                                      int(amsgrad), int(zero_mask), world, peer_grad_off,
-                                      ctypes.cast(arr, c_void_p) if arr is not None else c_void_p(0), grad_scale,
-                                      int(G_active), ptr(shadow_of), int(shadow_g_off), int(me), int(seg_mask),
-                                      int(dead_mask), stream_ptr()), "lah_adam_step")
+    l2, decay = weight_decay_args(lr, weight_decay, decoupled)
+    native.check(_lib().lah_adam_step_wd(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
+                                         ctypes.cast(segs, c_void_p), G, ptr(step),
+                                         ptr(group_rows), int(step_scalar), lr, betas[0], betas[1], eps, l2,
+                                         int(amsgrad), int(zero_mask), world, peer_grad_off,
+                                         ctypes.cast(arr, c_void_p) if arr is not None else c_void_p(0), grad_scale,
+                                         int(G_active), ptr(shadow_of), int(shadow_g_off), int(me), int(seg_mask),
+                                         int(dead_mask), decay, stream_ptr()), "lah_adam_step_wd")
     native.count_launch()
 
 
@@ -609,21 +623,23 @@ def swapab_linear_ref(x, w, group_off, group_rows, *, bias=None, residual=None, 
 
 
 def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, skip=None, lr=1e-3, betas=(0.9, 0.999),
-               eps=1e-8, amsgrad=True, max_ctas=0):
+               eps=1e-8, amsgrad=True, weight_decay=0.0, decoupled=False, max_ctas=0):
     """
     Fused weight gradient + per-expert AMSGrad (csrc/small_m.cu): for every group g with rows > 0,
     dW[g] = dy_g^T x_g is formed in registers and applied to p / m / v / vmax ([G, N, K] fp32) and the bf16 mirror in the same
     kernel; the gradient never reaches HBM.  ``step`` holds the per-expert step counts AFTER this update.
+    ``weight_decay`` / ``decoupled``: as in ``adam_step``.
     """
     G, N, Kd = p.shape
     assert dy.shape[1] == N and x.shape[1] == Kd and dy.shape[0] == x.shape[0] and p.is_contiguous()
     assert dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16 and p.dtype == torch.float32
     if amsgrad and vmax is None:
         raise ValueError("wgrad_adam: amsgrad needs a vmax tensor (vmax=None only with amsgrad=False)")
-    native.check(_lib().lah_wgrad_adam(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd, ptr(group_off),
-                                       ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v), ptr(vmax),
-                                       ptr(p_bf16), lr, betas[0], betas[1], eps, int(amsgrad), int(max_ctas),
-                                       stream_ptr()), "lah_wgrad_adam")
+    l2, decay = weight_decay_args(lr, weight_decay, decoupled)
+    native.check(_lib().lah_wgrad_adam_wd(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd,
+                                          ptr(group_off), ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v),
+                                          ptr(vmax), ptr(p_bf16), lr, betas[0], betas[1], eps, int(amsgrad), l2, decay,
+                                          int(max_ctas), stream_ptr()), "lah_wgrad_adam_wd")
     native.count_launch()
 
 
@@ -721,8 +737,9 @@ def ln_relu_bwd_ref(da, h, gamma, beta, relu=True, dres=None):
 
 @torch.no_grad()
 def adam_step_ref(p, g, m, v, vmax, seg_sizes, G, *, step, group_rows=None, lr=1e-3, betas=(0.9, 0.999), eps=1e-8,
-                  amsgrad=True, zero_mask=0):
-    """PyTorch implementation of csrc/adam.cu (flat segments [G, size]; per-group step; inactive groups skipped)."""
+                  amsgrad=True, zero_mask=0, weight_decay=0.0, decoupled=False):
+    """PyTorch implementation of csrc/adam.cu (flat segments [G, size]; per-group step; inactive groups skipped;
+    weight decay as torch.optim.Adam / AdamW apply it)."""
     if isinstance(seg_sizes, int):
         seg_sizes = [seg_sizes]
     off = 0
@@ -738,6 +755,10 @@ def adam_step_ref(p, g, m, v, vmax, seg_sizes, G, *, step, group_rows=None, lr=1
             continue
         P, Gr, M, V = p[sl].view(G, size), g[sl].view(G, size), m[sl].view(G, size), v[sl].view(G, size)
         grad = Gr[idx]
+        if weight_decay and decoupled:
+            P[idx] = P[idx] * (1 - lr * weight_decay)
+        elif weight_decay:
+            grad = grad + weight_decay * P[idx]
         m_new = M[idx] + (1 - betas[0]) * (grad - M[idx])
         v_new = V[idx] * betas[1] + (1 - betas[1]) * grad * grad
         if amsgrad:

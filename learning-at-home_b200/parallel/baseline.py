@@ -62,7 +62,9 @@ class BaselineDMoE(nn.Module):
         if device is not None:
             self.to(device)
         self.expert_optimizers = [torch.optim.Adam(e.parameters(), lr=cfg.lr, betas=cfg.betas, eps=cfg.eps,
-                                                   amsgrad=cfg.amsgrad) for e in self.experts]
+                                                   amsgrad=cfg.amsgrad, weight_decay=cfg.weight_decay,
+                                                   decoupled_weight_decay=cfg.decoupled_weight_decay)
+                                  for e in self.experts]
         self.fail_mask = None
 
     def load_from_shard(self, shard):
@@ -169,7 +171,8 @@ class BaselineTrainer:
         torch.manual_seed(cfg.seed)
         self.model = BaselineClassifier(cfg, group, self.device, dtype)
         self.params = self.model.non_expert_parameters()
-        self.opt = torch.optim.Adam(self.params, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad)
+        self.opt = torch.optim.Adam(self.params, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad,
+                                    weight_decay=cfg.weight_decay, decoupled_weight_decay=cfg.decoupled_weight_decay)
         self.autocast = dtype == torch.bfloat16
 
     def train_step_device(self, x, y):

@@ -139,7 +139,8 @@ class FastBaselineTrainer:
         self.trainer_params = list(self.stem.parameters()) + list(self.norm.parameters()) + list(self.head.parameters())
         for b in self.blocks:
             self.trainer_params += b.gate_parameters()
-        kw = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad)
+        kw = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad, weight_decay=cfg.weight_decay,
+                  decoupled_weight_decay=cfg.decoupled_weight_decay)
         fused = dict(fused=True) if dev.type == "cuda" else {}
         self.opt = torch.optim.Adam(self.trainer_params, **kw, **fused)
         self.expert_opt = torch.optim.Adam([p for b in self.blocks for p in b.expert_parameters()], **kw, **fused)

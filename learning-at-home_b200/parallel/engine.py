@@ -50,6 +50,11 @@ class DMoEConfig:
     betas: Tuple[float, float] = (0.9, 0.999)
     eps: float = 1e-8
     amsgrad: bool = True
+    # weight decay of every expert and trainer parameter, with torch's two forms: L2 (Adam(weight_decay=...): wd * p is added
+    # to the gradient) or decoupled (AdamW: p *= 1 - lr * wd before the update).  An expert that receives no rows in a step
+    # is not stepped and so not decayed, as with one torch optimizer per expert
+    weight_decay: float = 0.0
+    decoupled_weight_decay: bool = False
     seed: int = 1337
     uid_prefix: str = "expert"
     # gate of the fused layer:
@@ -130,6 +135,11 @@ class DMoEConfig:
     @property
     def inner(self) -> int:
         return 4 * self.hidden
+
+    def adam_kwargs(self) -> Dict:
+        """the optimizer settings as keywords of ``K.adam_step`` / ``K.wgrad_adam`` / ``K.adam_step_ref``"""
+        return dict(lr=self.lr, betas=self.betas, eps=self.eps, amsgrad=self.amsgrad, weight_decay=self.weight_decay,
+                    decoupled=self.decoupled_weight_decay)
 
     def seg_shapes(self) -> Dict[str, Tuple[int, ...]]:
         H, I = self.hidden, self.inner
@@ -461,8 +471,8 @@ class ExpertShard:
                 entry["max_exp_avg_sq"] = self.vmax[sl].view(shape).clone().cpu()
             state[i] = entry
         cfg = self.cfg
-        group = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, weight_decay=0, amsgrad=cfg.amsgrad,
-                     params=list(range(len(SEG_NAMES))))
+        group = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, weight_decay=cfg.weight_decay, amsgrad=cfg.amsgrad,
+                     decoupled_weight_decay=cfg.decoupled_weight_decay, params=list(range(len(SEG_NAMES))))
         return dict(state=state, param_groups=[group])
 
     def load_expert_state_dict(self, le: int, state: Dict[str, torch.Tensor], prefix: str = "expert."):
@@ -763,7 +773,7 @@ class FusedDMoE(nn.Module):
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         tg, go, rows, T = ws.tile_group, ws.group_off, ws.group_rows, c.tile_rows
         gr = sh.grads
-        opt = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad)
+        opt = cfg.adam_kwargs()
         main = torch.cuda.current_stream(c.device)
         side, chain_ctas = c.opt_stream, c.chain_ctas
 
@@ -815,8 +825,7 @@ class FusedDMoE(nn.Module):
             rows, zero_mask = sh.fire, (1 << len(SEG_NAMES)) - 1
         K.bump_steps(sh.step, rows)
         K.adam_step(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
-                    group_rows=rows, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad,
-                    zero_mask=zero_mask, G_active=self.E_loc, world=c.world,
+                    group_rows=rows, **cfg.adam_kwargs(), zero_mask=zero_mask, G_active=self.E_loc, world=c.world,
                     peer_bases=c.heap.peer_bases if c.S else None, shadow_of=ws.owned_shadow if c.S else None,
                     shadow_g_off=sh.g_off, me=c.rank)
         sh.w8_dirty = True
@@ -865,8 +874,7 @@ class FusedDMoE(nn.Module):
                 rows, zero_mask = due.to(rows.dtype), (1 << len(SEG_NAMES)) - 1
             sh.step += (rows > 0).to(sh.step.dtype)
             K.adam_step_ref(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.seg_sizes, self.E_loc, step=sh.step,
-                            group_rows=rows, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad,
-                            zero_mask=zero_mask)
+                            group_rows=rows, **cfg.adam_kwargs(), zero_mask=zero_mask)
         sh.sync_bf16()
         self._ref_rows = None
         self._ref_leaves = {}

@@ -135,8 +135,7 @@ class DMoETrainer:
             # so checkpoints taken on CPU carry the optimizer state
             with torch.no_grad():
                 K.adam_step_ref(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, [self._n_pad], 1,
-                                step=torch.tensor([self.step_count]), lr=cfg.lr, betas=cfg.betas, eps=cfg.eps,
-                                amsgrad=cfg.amsgrad, zero_mask=1)
+                                step=torch.tensor([self.step_count]), **cfg.adam_kwargs(), zero_mask=1)
             return
         c = self.ctx
         K.bump_steps(self.step_dev, self._one)
@@ -147,7 +146,7 @@ class DMoETrainer:
             epoch = c.next_epoch()
             K.signal_wait(c.flags_off, K.SLOT_TRAINER, epoch, c.status, signal=True, wait=True)
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad,
+                        step=self.step_dev, **cfg.adam_kwargs(),
                         world=c.world, peer_grad_off=self.flat_g_off, peer_bases=c.heap.peer_bases,
                         grad_scale=1.0 / alive, dead_mask=c.dead_mask)
             K.signal_wait(c.flags_off, K.SLOT_BARRIER, epoch, c.status, signal=True, wait=True)
@@ -160,12 +159,12 @@ class DMoETrainer:
             K.nvls_allreduce(self.flat_g_off, self._n_pad, 1.0 / c.world)
             K.signal_wait(c.flags_off, K.SLOT_BARRIER, epoch, c.status, signal=True, wait=True)
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad, zero_mask=1)
+                        step=self.step_dev, **cfg.adam_kwargs(), zero_mask=1)
         elif c.world > 1:
             epoch = c.next_epoch()
             K.signal_wait(c.flags_off, K.SLOT_TRAINER, epoch, c.status, signal=True, wait=True)
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad,
+                        step=self.step_dev, **cfg.adam_kwargs(),
                         world=c.world, peer_grad_off=self.flat_g_off, peer_bases=c.heap.peer_bases,
                         grad_scale=1.0 / c.world)
             # nobody may overwrite its gradient buffer before every peer has consumed it
@@ -173,8 +172,7 @@ class DMoETrainer:
             self.flat_g.zero_()
         else:
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, amsgrad=cfg.amsgrad,
-                        zero_mask=1)
+                        step=self.step_dev, **cfg.adam_kwargs(), zero_mask=1)
 
     # ------------------------------------------------------------------ steps
     def train_step_device(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:

@@ -28,9 +28,11 @@ class ExpertBackend(nn.Module):
                  args_schema: Tuple[BatchTensorProto, ...] = None, kwargs_schema: Dict[str, BatchTensorProto] = None,
                  outputs_schema: Union[BatchTensorProto, Tuple[BatchTensorProto, ...]] = None, native: bool = True,
                  **kwargs):
-        """:param native: run experts that live on a CUDA device in fp32 with a single-group torch.optim.Adam through the
-        sm_90a kernels (runtime/native_executor.py) instead of eager PyTorch.  These run natively, plain or
-        ``torch.jit.script``-ed:
+        """:param native: run experts that live on a CUDA device in fp32 through the sm_90a kernels
+        (runtime/native_executor.py) instead of eager PyTorch, with ``torch.optim.Adam`` or ``torch.optim.AdamW`` whose
+        param groups hold every parameter of the expert once (per group any lr, betas, eps, weight_decay, amsgrad and
+        decoupled_weight_decay; ``maximize``, ``capturable``, ``differentiable``, tensor lr / betas and other optimizers
+        run on the module).  These modules run natively, plain or ``torch.jit.script``-ed:
           * ``FeedforwardBlock`` (swap-AB wgmma GEMMs, fused LayerNorm, fused weight-gradient + AMSGrad);
           * this package's ``TransformerEncoderLayer`` and ``torch.nn.TransformerEncoderLayer`` with ReLU or erf GELU,
             ``norm_first`` True or False, ``batch_first`` True or False, LayerNorm eps 1e-5 and all biases, head dim

@@ -12,7 +12,7 @@ The module's parameters and the torch optimizer's state tensors are re-bound as 
 ``expert.state_dict()``, ``opt.state_dict()`` and ``ExpertBackend.checkpoint()`` stay live and keep the reference layout.
 """
 import re
-from typing import NamedTuple, Optional, Tuple
+from typing import List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -104,6 +104,71 @@ def encoder_layer_spec(module) -> Optional[EncoderLayerSpec]:
     return EncoderLayerSpec(int(attn.embed_dim), int(attn.num_heads), int(module.linear1.out_features), norm_first,
                             activation, batch_first, ps)
 
+def optimizer_groups(opt, params) -> Optional[List[int]]:
+    """
+    The executors' view of ``opt``: for each of its param groups the mask of the segments it holds (segment s is
+    ``params[s]``), or None when the optimizer must stay on the module.  Accepted: ``torch.optim.Adam`` and
+    ``torch.optim.AdamW`` whose groups together hold exactly ``params``, each once; per group any ``lr``, ``betas``,
+    ``eps``, ``weight_decay`` >= 0, ``amsgrad`` and ``decoupled_weight_decay`` (``foreach`` and ``fused`` do not change the
+    maths).  Refused: ``maximize``, ``capturable``, ``differentiable``, a tensor ``lr`` or ``betas``, a parameter missing
+    or present twice, any other optimizer class.
+    """
+    if type(opt) not in (torch.optim.Adam, torch.optim.AdamW):
+        return None
+    index = {id(p): s for s, p in enumerate(params)}
+    masks, seen = [], 0
+    for g in opt.param_groups:
+        if g.get("maximize", False) or g.get("capturable", False) or g.get("differentiable", False):
+            return None
+        if torch.is_tensor(g["lr"]) or any(torch.is_tensor(b) for b in g["betas"]) or not g["weight_decay"] >= 0:
+            return None
+        mask = 0
+        for p in g["params"]:
+            s = index.get(id(p))
+            if s is None or (seen >> s) & 1:
+                return None
+            mask |= 1 << s
+            seen |= 1 << s
+        masks.append(mask)
+    return masks if seen == (1 << len(params)) - 1 else None
+
+
+def group_hyper(group) -> dict:
+    """the optimizer keywords of ``K.adam_step`` / ``K.wgrad_adam`` for one param group, read at every call so that
+    learning-rate and weight-decay schedules take effect on the next step, as in torch"""
+    return dict(lr=float(group["lr"]), betas=(float(group["betas"][0]), float(group["betas"][1])), eps=float(group["eps"]),
+                weight_decay=float(group["weight_decay"]), decoupled=bool(group.get("decoupled_weight_decay", False)),
+                amsgrad=bool(group.get("amsgrad", False)))
+
+
+def bind_optimizer_state(opt, params, names, groups, pv, mv, vv, vmv):
+    """load the module's parameters and the optimizer's state into the flat buffers' views and re-bind both to them;
+    returns the step count (the largest of the parameters').  ``max_exp_avg_sq`` exists for the groups with amsgrad, as
+    in torch."""
+    amsgrad = {}
+    for g, mask in zip(opt.param_groups, groups):
+        for s in range(len(params)):
+            if (mask >> s) & 1:
+                amsgrad[s] = bool(g.get("amsgrad", False))
+    steps = 0
+    for s, (name, param) in enumerate(zip(names, params)):
+        pv[name][0].copy_(param.data)
+        param.data = pv[name][0]
+        param.grad = None
+        st = opt.state.get(param, {})
+        if st:
+            mv[name][0].copy_(st["exp_avg"])
+            vv[name][0].copy_(st["exp_avg_sq"])
+            if amsgrad[s] and "max_exp_avg_sq" in st:
+                vmv[name][0].copy_(st["max_exp_avg_sq"])
+            steps = max(steps, int(float(st["step"])))
+        new = dict(step=torch.tensor(float(steps)), exp_avg=mv[name][0], exp_avg_sq=vv[name][0])
+        if amsgrad[s]:
+            new["max_exp_avg_sq"] = vmv[name][0]
+        opt.state[param] = new
+    return steps
+
+
 SEGS = (("w1", 0, "weight"), ("b1", 0, "bias"), ("g1", 1, "weight"), ("be1", 1, "bias"), ("w2", 3, "weight"),
         ("b2", 3, "bias"), ("g2", 4, "weight"), ("be2", 4, "bias"), ("w3", 6, "weight"), ("b3", 6, "bias"))
 SMALL_MASK = sum(1 << i for i, (n, _, _) in enumerate(SEGS) if not n.startswith("w"))
@@ -126,21 +191,21 @@ class NativeFFNExecutor:
         params = list(expert.parameters())
         if hid % 128 or not params or not params[0].is_cuda or params[0].dtype != torch.float32:
             return False
-        if type(opt) is not torch.optim.Adam or len(opt.param_groups) != 1:
-            return False
-        g = opt.param_groups[0]
-        if g.get("weight_decay", 0) or g.get("maximize", False) or g.get("capturable", False) or g.get("differentiable", False):
-            return False
-        if {id(p) for p in g["params"]} != {id(p) for p in params}:
+        if optimizer_groups(opt, NativeFFNExecutor._segment_params(expert)) is None:
             return False
         return native.have_cuda_kernels()
 
-    def __init__(self, expert, opt: torch.optim.Adam):
+    @staticmethod
+    def _segment_params(expert):
+        return [getattr(expert.layers[li], attr) for _, li, attr in SEGS]
+
+    def __init__(self, expert, opt):
         self.expert, self.opt = expert, opt
         dev = next(expert.parameters()).device
         self.device = dev
         self.hid, self.inner = expert.layers[0].in_features, expert.layers[0].out_features
-        self.params = [getattr(expert.layers[li], attr) for _, li, attr in SEGS]
+        self.params = self._segment_params(expert)
+        self.groups = optimizer_groups(opt, self.params)
         self.sizes = [p.numel() for p in self.params]
         total = sum(self.sizes)
         f32 = dict(dtype=torch.float32, device=dev)
@@ -166,33 +231,13 @@ class NativeFFNExecutor:
     @torch.no_grad()
     def bind(self):
         """(re)load the module's parameters and the optimizer's state into the flat buffers and make them views of it"""
-        group = self.opt.param_groups[0]
-        amsgrad = bool(group.get("amsgrad", False))
         self.pv, self.gv = self._views(self.p), self._views(self.g)
         self.mv, self.vv, self.vmv, self.bv = self._views(self.m), self._views(self.v), self._views(self.vmax), self._views(self.p_bf16)
-        steps = 0
-        for (name, _, _), param in zip(SEGS, self.params):
-            self.pv[name][0].copy_(param.data)
-            param.data = self.pv[name][0]
-            param.grad = None
-            st = self.opt.state.get(param, {})
-            if st:
-                self.mv[name][0].copy_(st["exp_avg"])
-                self.vv[name][0].copy_(st["exp_avg_sq"])
-                if amsgrad and "max_exp_avg_sq" in st:
-                    self.vmv[name][0].copy_(st["max_exp_avg_sq"])
-                steps = max(steps, int(float(st["step"])))
-            new = dict(step=torch.tensor(float(steps)), exp_avg=self.mv[name][0], exp_avg_sq=self.vv[name][0])
-            if amsgrad:
-                new["max_exp_avg_sq"] = self.vmv[name][0]
-            self.opt.state[param] = new
+        steps = bind_optimizer_state(self.opt, self.params, [n for n, _, _ in SEGS], self.groups, self.pv, self.mv, self.vv,
+                                     self.vmv)
         self.steps_host = steps
         self.step.fill_(steps)
         K.cast_bf16(self.p, self.p_bf16)
-
-    def _hyper(self):
-        g = self.opt.param_groups[0]
-        return dict(lr=float(g["lr"]), betas=tuple(g["betas"]), eps=float(g["eps"]), amsgrad=bool(g.get("amsgrad", False)))
 
     def _workspace(self, rows: int):
         cap = (rows + ALIGN - 1) // ALIGN * ALIGN
@@ -237,10 +282,12 @@ class NativeFFNExecutor:
         if padded > rows:
             self.gyd[rows:padded].zero_()
         go, gr, pv, bv, gv = self.group_off, self.group_rows, self.pv, self.bv, self.gv
-        hyper = self._hyper()
+        hypers = [group_hyper(g) for g in self.opt.param_groups]
+        seg_hyper = {SEGS[s][0]: h for h, mask in zip(hypers, self.groups) for s in range(len(SEGS)) if (mask >> s) & 1}
         K.bump_steps(self.step, self.one)
 
-        def wgrad(name, dy, xin):
+        def wgrad(name, dy, xin):   # each weight matrix with the settings of its own group
+            hyper = seg_hyper[name]
             K.wgrad_adam(dy, xin, go, gr, p=pv[name], m=self.mv[name], v=self.vv[name],
                          vmax=self.vmv[name] if hyper["amsgrad"] else None, p_bf16=bv[name], step=self.step, **hyper)
 
@@ -255,12 +302,15 @@ class NativeFFNExecutor:
                       dh=self.dh[:padded], dgamma=gv["g1"], dbeta=gv["be1"], dbias=gv["b1"], tile_rows=ALIGN)
         K.swapab_linear(self.dh, bv["w1"], go, gr, out=self.dxd, w_is_kn=True, residual=self.gyd)
         wgrad("w1", self.dh, self.xd)
-        K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step, zero_mask=SMALL_MASK,
-                    seg_mask=SMALL_MASK, **hyper)
+        for hyper, mask in zip(hypers, self.groups):   # the small vectors: one launch per group that holds any
+            if mask & SMALL_MASK:
+                K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step,
+                            zero_mask=SMALL_MASK, seg_mask=mask & SMALL_MASK, **hyper)
         self.steps_host += 1
-        step_t = torch.tensor(float(self.steps_host))
+        # one step tensor per parameter, as torch keeps them: an eager optimizer that loads a shared one from a checkpoint
+        # increments it once per parameter
         for param in self.params:
-            self.opt.state[param]["step"] = step_t
+            self.opt.state[param]["step"] = torch.tensor(float(self.steps_host))
         return self.dxd[:rows].to(x.dtype)
 
 
@@ -340,14 +390,17 @@ class NativeTransformerExecutor:
             return False
         if not all(0.0 <= p < 1.0 for p in spec.ps):
             return False   # p = 1 zeroes a whole branch: eager PyTorch handles that configuration
-        if type(opt) is not torch.optim.Adam or len(opt.param_groups) != 1:
-            return False
-        g = opt.param_groups[0]
-        if g.get("weight_decay", 0) or g.get("maximize", False) or g.get("capturable", False) or g.get("differentiable", False):
-            return False
-        if {id(p) for p in g["params"]} != {id(p) for p in params}:
+        if optimizer_groups(opt, NativeTransformerExecutor._segment_params(expert)) is None:
             return False
         return native.have_cuda_kernels()
+
+    @staticmethod
+    def _segment_params(expert):
+        """the parameters in the order of NAMES (the segments of the flat buffers)"""
+        attn = expert.self_attn
+        return [attn.in_proj_weight, attn.in_proj_bias, attn.out_proj.weight, attn.out_proj.bias, expert.linear1.weight,
+                expert.linear1.bias, expert.linear2.weight, expert.linear2.bias, expert.norm1.weight, expert.norm1.bias,
+                expert.norm2.weight, expert.norm2.bias]
 
     @staticmethod
     def _dropout_ps(expert):
@@ -367,10 +420,8 @@ class NativeTransformerExecutor:
         self.d, self.heads, self.ff = spec.d, spec.heads, spec.ff
         self.takes_key_padding_mask = class_name(expert) == TORCH_ENCODER_LAYER   # this package's layer has no mask input
         self.norm_first, self.relu, self.batch_first = spec.norm_first, spec.activation == "relu", spec.batch_first
-        attn = expert.self_attn
-        self.params = [attn.in_proj_weight, attn.in_proj_bias, attn.out_proj.weight, attn.out_proj.bias, expert.linear1.weight,
-                       expert.linear1.bias, expert.linear2.weight, expert.linear2.bias, expert.norm1.weight, expert.norm1.bias,
-                       expert.norm2.weight, expert.norm2.bias]
+        self.params = self._segment_params(expert)
+        self.groups = optimizer_groups(opt, self.params)
         dev = self.params[0].device
         self.device = dev
         self.sizes = [p.numel() for p in self.params]
@@ -394,25 +445,9 @@ class NativeTransformerExecutor:
 
     @torch.no_grad()
     def bind(self):
-        amsgrad = bool(self.opt.param_groups[0].get("amsgrad", False))
         self.pv, self.gv, self.bv = self._views(self.p), self._views(self.g), self._views(self.p_bf16)
         mv, vv, vmv = self._views(self.m), self._views(self.v), self._views(self.vmax)
-        steps = 0
-        for name, param in zip(self.NAMES, self.params):
-            self.pv[name][0].copy_(param.data)
-            param.data = self.pv[name][0]
-            param.grad = None
-            st = self.opt.state.get(param, {})
-            if st:
-                mv[name][0].copy_(st["exp_avg"])
-                vv[name][0].copy_(st["exp_avg_sq"])
-                if amsgrad and "max_exp_avg_sq" in st:
-                    vmv[name][0].copy_(st["max_exp_avg_sq"])
-                steps = max(steps, int(float(st["step"])))
-            new = dict(step=torch.tensor(float(steps)), exp_avg=mv[name][0], exp_avg_sq=vv[name][0])
-            if amsgrad:
-                new["max_exp_avg_sq"] = vmv[name][0]
-            self.opt.state[param] = new
+        steps = bind_optimizer_state(self.opt, self.params, self.NAMES, self.groups, self.pv, mv, vv, vmv)
         self.steps_host = steps
         self.step.fill_(steps)
         K.cast_bf16(self.p, self.p_bf16)
@@ -582,15 +617,17 @@ class NativeTransformerExecutor:
         else:
             gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"])
             dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh)
-        g = self.opt.param_groups[0]
         K.bump_steps(self.step, self.one)
-        K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step, lr=float(g["lr"]),
-                    betas=tuple(g["betas"]), eps=float(g["eps"]), amsgrad=bool(g.get("amsgrad", False)),
-                    zero_mask=(1 << len(self.sizes)) - 1)
+        all_segs = (1 << len(self.sizes)) - 1
+        for g, mask in zip(self.opt.param_groups, self.groups):   # one launch per group, over its segments
+            if mask:
+                K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step,
+                            zero_mask=all_segs, seg_mask=0 if mask == all_segs else mask, **group_hyper(g))
         self.steps_host += 1
-        step_t = torch.tensor(float(self.steps_host))
+        # one step tensor per parameter, as torch keeps them: an eager optimizer that loads a shared one from a checkpoint
+        # increments it once per parameter
         for param in self.params:
-            self.opt.state[param]["step"] = step_t
+            self.opt.state[param]["step"] = torch.tensor(float(self.steps_host))
         return self._from_rows(dx[:Tr], src)
 
 
