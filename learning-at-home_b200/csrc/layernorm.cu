@@ -9,6 +9,9 @@
 #include <cuda_fp8.h>
 #include <stdlib.h>
 
+#include <array>
+#include <utility>
+
 namespace lah {
 
 constexpr float LN_EPS = 1e-5f;
@@ -24,9 +27,22 @@ constexpr float LN_EPS = 1e-5f;
 // With QUANT the kernel ALSO emits the MXFP8 operand of the next expert GEMM (csrc/grouped_gemm_fp8.cu): E4M3 payload +
 // one UE8M0 scale per 32 columns (4 adjacent lanes share a block: two shuffles), quantised from the fp32 value before it
 // is rounded to bf16.  The bf16 copy is optional (a == nullptr in forward-only runs).
+//
+// Widths: every multiple of 128 up to LN_MAX_C.  When C is an odd multiple of 128 the row ends in half a chunk
+// (128 columns), owned by lanes 0-15; lanes 16-31 hold zeros there, which leave the row sums unchanged.
+constexpr int LN_MAX_C = 4096;
+
 template <int C>
 struct LnFwdCfg {
-    static constexpr int R = (C >= 4096) ? 1 : ((C >= 2048) ? 2 : 4);   // rows per warp (64 packed registers)
+    static constexpr int NV = (C + 255) / 256;   // int4 chunks per lane and row, the half chunk counted whole
+    // The power-of-two widths keep the configuration they were tuned with: R = the largest power of two <= 4 with
+    // NV * R <= 16 (64 packed registers per lane; 1024, 2048 and 4096 spill a little under the 128-register cap).
+    // The other widths hold fewer rows, chosen so that no instantiation spills (-Xptxas -v; DESIGN.md §9, Widths):
+    // R = 4 up to NV = 2, R = 2 up to NV = 6, else 1; and above NV = 12 one row no longer fits in 128 registers, so
+    // those widths ask for one CTA per SM instead of two.
+    static constexpr bool TUNED = C >= 256 && (C & (C - 1)) == 0;
+    static constexpr int R = TUNED ? ((NV * 4 <= 16) ? 4 : ((NV * 2 <= 16) ? 2 : 1)) : (NV <= 2 ? 4 : (NV <= 6 ? 2 : 1));
+    static constexpr int MIN_BLOCKS = (TUNED || NV <= 12) ? 2 : 1;
 };
 
 static int ln_rows_per_warp(int dflt) {   // LAH_LN_ROWS=1 selects the one-row-per-warp variant (A/B measurements)
@@ -39,11 +55,13 @@ static int ln_rows_per_warp(int dflt) {   // LAH_LN_ROWS=1 selects the one-row-p
 }
 
 template <int C, bool QUANT, int R>
-__global__ void __launch_bounds__(256, 2) ln_relu_fwd_kernel(
+__global__ void __launch_bounds__(256, LnFwdCfg<C>::MIN_BLOCKS) ln_relu_fwd_kernel(
     const bf16* __restrict__ h, bf16* __restrict__ a, float* __restrict__ mean_out, float* __restrict__ rstd_out,
     const float* __restrict__ gamma, const float* __restrict__ beta, const int* __restrict__ tile_group, int rows,
     int relu, uint8_t* __restrict__ aq, uint8_t* __restrict__ sf, int tile_shift) {
-    constexpr int NV = C / 256;  // int4 (8 x bf16) chunks per lane
+    constexpr int NV = LnFwdCfg<C>::NV;  // int4 (8 x bf16) chunks per lane
+    constexpr bool HALF = C % 256 != 0;  // the last chunk is half a chunk: lanes 0-15 only
+    static_assert(C % 128 == 0 && C <= LN_MAX_C && !(QUANT && HALF), "unsupported LayerNorm width");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int row0 = (blockIdx.x * 8 + warp) * R;
     if (row0 >= rows) return;
@@ -55,7 +73,15 @@ __global__ void __launch_bounds__(256, 2) ln_relu_fwd_kernel(
     for (int r = 0; r < R; ++r) {
         const int4* hp = reinterpret_cast<const int4*>(h + static_cast<long long>(min(row0 + r, rows - 1)) * C);
 #pragma unroll
-        for (int j = 0; j < NV; ++j) q[r][j] = ld_nc_v4(hp + j * 32 + lane);
+        for (int j = 0; j < NV; ++j) {
+            if constexpr (HALF) {
+                if (j == NV - 1 && lane >= 16) {
+                    q[r][j] = make_int4(0, 0, 0, 0);
+                    continue;
+                }
+            }
+            q[r][j] = ld_nc_v4(hp + j * 32 + lane);
+        }
     }
     float mean[R], rstd[R];
 #pragma unroll
@@ -85,6 +111,9 @@ __global__ void __launch_bounds__(256, 2) ln_relu_fwd_kernel(
     const float* bp = beta + static_cast<long long>(g) * C;
 #pragma unroll
     for (int j = 0; j < NV; ++j) {
+        if constexpr (HALF) {
+            if (j == NV - 1 && lane >= 16) break;
+        }
         const int col = (j * 32 + lane) * 8;
         // volatile asm loads: ordered with the volatile asm stores below, so the compiler cannot hoist the parameter
         // loads of all later chunks to the top (16 registers per chunk -> spills)
@@ -164,9 +193,20 @@ __global__ void __launch_bounds__(256, 2) ln_relu_fwd_kernel(
 // With RES the LayerNorm sits on a residual branch (pre-LN encoder layer: h = x + f(LN(x))): the gradient that bypasses it,
 // dres, is added to dh before it is stored, and dbias is the column sum of that total.  dres is the LAST parameter so
 // that the RES = false kernels keep the parameter layout, and the code, they had before it existed.
+// When C is an odd multiple of 128, C/8 is not a whole number of warps: the CTA is rounded up to whole warps and the idle
+// threads (col >= C) hold zero inputs, so they add exact zeros to the row reductions and store nothing.
 // ------------------------------------------------------------------------------------------------
+template <int C>
+struct LnBwdCfg {
+    static constexpr int THREADS = (C / 8 + 31) / 32 * 32;
+    static constexpr int MIN_BLOCKS = (C <= 2048) ? 2 : 1;
+    // rows per batch: 4, or 2 where four or more warps share an SM sub-partition (a 128-register cap), as at 4096;
+    // 2048 keeps the 4 it was tuned with
+    static constexpr int RB = ((THREADS / 32 * MIN_BLOCKS + 3) / 4 >= 4 && C != 2048) ? 2 : 4;
+};
+
 template <int C, bool RES>
-__global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel(const bf16* __restrict__ da, const bf16* __restrict__ h,
+__global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS) ln_relu_bwd_kernel(const bf16* __restrict__ da, const bf16* __restrict__ h,
                                                             const float* __restrict__ mean_in,
                                                             const float* __restrict__ rstd_in,
                                                             const float* __restrict__ gamma,
@@ -174,9 +214,11 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
                                                             float* __restrict__ part,
                                                             const int* __restrict__ tile_group, int rows, int relu, int tile_rows,
                                                             const bf16* __restrict__ dres) {
-    constexpr int THREADS = C / 8;
+    constexpr int THREADS = LnBwdCfg<C>::THREADS;
     constexpr int WARPS = THREADS / 32;
-    constexpr int RB = (C >= 4096) ? 2 : 4;  // rows per batch (register blocking)
+    constexpr bool IDLE = THREADS * 8 != C;   // the last warp has threads past the last column
+    static_assert(C % 128 == 0 && C <= LN_MAX_C, "unsupported LayerNorm width");
+    constexpr int RB = LnBwdCfg<C>::RB;  // rows per batch (register blocking)
     __shared__ float red[WARPS][2 * RB];
     __shared__ float tot[2 * RB];
     const int tile = blockIdx.x;
@@ -184,8 +226,12 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
     if (g < 0) return;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int col = tid * 8;
+    const bool live = !IDLE || col < C;
     float gam[8], bet[8];
-    {
+    if (!live) {
+#pragma unroll
+        for (int t = 0; t < 8; ++t) gam[t] = bet[t] = 0.f;
+    } else {
         const float* gp = gamma + static_cast<long long>(g) * C + col;
         const float* bp = beta + static_cast<long long>(g) * C + col;
         const float4 g0 = __ldg(reinterpret_cast<const float4*>(gp)), g1 = __ldg(reinterpret_cast<const float4*>(gp + 4));
@@ -208,8 +254,12 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
             const int row = rb + r;
             const int rr = row < row_end ? row : row0;
             const long long off = static_cast<long long>(rr) * C + col;
-            nqa[r] = ld_nc_v4(reinterpret_cast<const int4*>(da + off));
-            nqh[r] = ld_nc_v4(reinterpret_cast<const int4*>(h + off));
+            if (live) {
+                nqa[r] = ld_nc_v4(reinterpret_cast<const int4*>(da + off));
+                nqh[r] = ld_nc_v4(reinterpret_cast<const int4*>(h + off));
+            } else {
+                nqa[r] = nqh[r] = make_int4(0, 0, 0, 0);
+            }
             nmu[r] = __ldg(mean_in + rr);
             nrs[r] = __ldg(rstd_in + rr);
         }
@@ -276,7 +326,7 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
 #pragma unroll
         for (int r = 0; r < RB; ++r) {
             const int row = rb + r;
-            if (row >= row_end) continue;
+            if (row >= row_end || !live) continue;
             float gvv[8], xhh[8];
             slice(r, true, gvv, xhh);
             const float m1 = tot[2 * r], m2 = tot[2 * r + 1];
@@ -309,6 +359,7 @@ __global__ void __launch_bounds__(C / 8, (C <= 2048) ? 2 : 1) ln_relu_bwd_kernel
         // `tot` is rewritten only after the next batch's first __syncthreads, which every thread reaches
         // after it finished reading tot above -> no extra barrier needed.
     }
+    if (!live) return;
     float* pg = part + static_cast<long long>(tile) * 3 * C + col;
 #pragma unroll
     for (int t = 0; t < 8; ++t) {
@@ -333,7 +384,7 @@ __global__ void __launch_bounds__(512) grouped_colsum_kernel(const bf16* __restr
     const int cp = threadIdx.x & 127;         // column pair inside the slab
     const int phase = threadIdx.x >> 7;       // 0..3
     const int col = blockIdx.y * 256 + cp * 2;
-    if (col >= C) return;                      // C is a multiple of 256 in practice; whole warps exit together
+    if (col >= C) return;                      // C is a multiple of 128: whole warps exit together
     const int row0 = tile * tile_rows, row_end = min(rows, row0 + tile_rows);
     float2 acc = make_float2(0.f, 0.f);
     for (int r = row0 + phase; r < row_end; r += 4) {
@@ -379,6 +430,60 @@ __global__ void __launch_bounds__(256) group_tile_sum_kernel(const float* __rest
     if (cur >= 0) out[static_cast<long long>(cur) * C + c] += acc;
 }
 
+// ------------------------------------------------------------------------------------------------
+// host launchers, one per width; the entry points below dispatch through tables indexed by C / 128 - 1
+// ------------------------------------------------------------------------------------------------
+using LnFwdLaunch = void (*)(const void*, void*, float*, float*, const float*, const float*, const int*, int, int, int,
+                             cudaStream_t);
+using LnBwdLaunch = void (*)(const void*, const void*, const float*, const float*, const float*, const float*, void*,
+                             float*, float*, float*, float*, const int*, int, int, int, const void*, cudaStream_t);
+
+template <int C>
+void ln_fwd_launch(const void* h, void* a, float* mean, float* rstd, const float* gamma, const float* beta,
+                   const int* tile_group, int rows, int relu, int tile_shift, cudaStream_t st) {
+    constexpr int RR = LnFwdCfg<C>::R;
+    // the one-row-per-warp variant (LAH_LN_ROWS=1) exists for the power-of-two widths only
+    if constexpr (LnFwdCfg<C>::TUNED) {
+        if (ln_rows_per_warp(RR) == 1) {
+            ln_relu_fwd_kernel<C, false, 1><<<(rows + 7) / 8, 256, 0, st>>>(
+                (const bf16*)h, (bf16*)a, mean, rstd, gamma, beta, tile_group, rows, relu, nullptr, nullptr, tile_shift);
+            return;
+        }
+    }
+    ln_relu_fwd_kernel<C, false, RR><<<(rows + 8 * RR - 1) / (8 * RR), 256, 0, st>>>(
+        (const bf16*)h, (bf16*)a, mean, rstd, gamma, beta, tile_group, rows, relu, nullptr, nullptr, tile_shift);
+}
+
+template <int C>
+void ln_bwd_launch(const void* da, const void* h, const float* mean, const float* rstd, const float* gamma,
+                   const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
+                   const int* tile_group, int rows, int relu, int tile_rows, const void* dres, cudaStream_t st) {
+    const int grid = (rows + tile_rows - 1) / tile_rows;
+    constexpr int T = LnBwdCfg<C>::THREADS;
+    if (dres)
+        ln_relu_bwd_kernel<C, true><<<grid, T, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd, gamma, beta,
+                                                        (bf16*)dh, part, tile_group, rows, relu, tile_rows,
+                                                        (const bf16*)dres);
+    else
+        ln_relu_bwd_kernel<C, false><<<grid, T, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd, gamma, beta,
+                                                         (bf16*)dh, part, tile_group, rows, relu, tile_rows, nullptr);
+    group_tile_sum_kernel<<<(3 * C + 255) / 256, 256, 0, st>>>(part, grid, 3, C, tile_group, dgamma, dbeta, dbias);
+}
+
+template <int... I>
+constexpr auto ln_fwd_table(std::integer_sequence<int, I...>) {
+    return std::array<LnFwdLaunch, sizeof...(I)>{ln_fwd_launch<(I + 1) * 128>...};
+}
+template <int... I>
+constexpr auto ln_bwd_table(std::integer_sequence<int, I...>) {
+    return std::array<LnBwdLaunch, sizeof...(I)>{ln_bwd_launch<(I + 1) * 128>...};
+}
+constexpr auto kLnFwd = ln_fwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
+constexpr auto kLnBwd = ln_bwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
+
+// widths the LayerNorm entry points run: multiples of 128 up to LN_MAX_C (the column sum has no upper limit)
+static bool ln_width_ok(int C) { return C > 0 && C % 128 == 0 && C <= LN_MAX_C; }
+
 }  // namespace lah
 
 using namespace lah;
@@ -396,21 +501,9 @@ int lah_ln_relu_fwd(const void* h, void* a, float* mean, float* rstd, const floa
                     const int* tile_group, int rows, int C, int relu, int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
     const int tile_shift = shift_of(tile_rows);
-    if (tile_shift < 0) return -2;
-#define LAH_LN_FWD(CC)                                                                                          \
-    if (C == CC) {                                                                                              \
-        constexpr int RR = LnFwdCfg<CC>::R;                                                                     \
-        if (ln_rows_per_warp(RR) == 1)                                                                          \
-            ln_relu_fwd_kernel<CC, false, 1><<<(rows + 7) / 8, 256, 0, st>>>(                                  \
-                (const bf16*)h, (bf16*)a, mean, rstd, gamma, beta, tile_group, rows, relu, nullptr, nullptr, tile_shift);   \
-        else                                                                                                    \
-            ln_relu_fwd_kernel<CC, false, RR><<<(rows + 8 * RR - 1) / (8 * RR), 256, 0, st>>>(                 \
-                (const bf16*)h, (bf16*)a, mean, rstd, gamma, beta, tile_group, rows, relu, nullptr, nullptr, tile_shift);   \
-        return -(int)cudaGetLastError();                                                                        \
-    }
-    LAH_LN_FWD(256) LAH_LN_FWD(512) LAH_LN_FWD(1024) LAH_LN_FWD(2048) LAH_LN_FWD(4096)
-#undef LAH_LN_FWD
-    return -2;
+    if (tile_shift < 0 || !ln_width_ok(C)) return -2;
+    kLnFwd[C / 128 - 1](h, a, mean, rstd, gamma, beta, tile_group, rows, relu, tile_shift, st);
+    return -(int)cudaGetLastError();
 }
 
 // same + MXFP8 copy of the output (aq: e4m3 [rows, C]; sf: activation scale layout, tile_rows = 128); a may be NULL
@@ -439,32 +532,17 @@ int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const floa
                     const float* beta, void* dh, float* dgamma, float* dbeta, float* dbias, float* part,
                     const int* tile_group, int rows, int C, int relu, int tile_rows, const void* dres, cudaStream_t st) {
     if (rows <= 0) return 0;
-    if (shift_of(tile_rows) < 0) return -2;
-    const int grid = (rows + tile_rows - 1) / tile_rows;
-#define LAH_LN_BWD(CC)                                                                                          \
-    if (C == CC) {                                                                                              \
-        if (dres)                                                                                               \
-            ln_relu_bwd_kernel<CC, true><<<grid, CC / 8, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd,  \
-                                                                  gamma, beta, (bf16*)dh, part, tile_group,     \
-                                                                  rows, relu, tile_rows, (const bf16*)dres);    \
-        else                                                                                                    \
-            ln_relu_bwd_kernel<CC, false><<<grid, CC / 8, 0, st>>>((const bf16*)da, (const bf16*)h, mean, rstd, \
-                                                                   gamma, beta, (bf16*)dh, part, tile_group,    \
-                                                                   rows, relu, tile_rows, nullptr);             \
-        group_tile_sum_kernel<<<(3 * CC + 255) / 256, 256, 0, st>>>(part, grid, 3, CC, tile_group, dgamma,     \
-                                                                     dbeta, dbias);                            \
-        return -(int)cudaGetLastError();                                                                        \
-    }
-    LAH_LN_BWD(256) LAH_LN_BWD(512) LAH_LN_BWD(1024) LAH_LN_BWD(2048) LAH_LN_BWD(4096)
-#undef LAH_LN_BWD
-    return -2;
+    if (shift_of(tile_rows) < 0 || !ln_width_ok(C)) return -2;
+    kLnBwd[C / 128 - 1](da, h, mean, rstd, gamma, beta, dh, dgamma, dbeta, dbias, part, tile_group, rows, relu,
+                        tile_rows, dres, st);
+    return -(int)cudaGetLastError();
 }
 
 // part: scratch of [ceil(rows / tile_rows), C] fp32 (per-tile column sums, reduced in tile order)
 int lah_grouped_colsum(const void* x, long long ldx, float* out, float* part, int C, const int* tile_group, int rows,
                        int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
-    if (C % 256 || shift_of(tile_rows) < 0) return -2;
+    if (C % 128 || shift_of(tile_rows) < 0) return -2;   // any multiple of 128: one CTA column per 256-column slab
     const int tiles = (rows + tile_rows - 1) / tile_rows;
     dim3 grid(tiles, (C + 255) / 256);
     grouped_colsum_kernel<<<grid, 512, 0, st>>>((const bf16*)x, ldx, part, C, tile_group, rows, tile_rows);

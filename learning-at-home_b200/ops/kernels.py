@@ -86,10 +86,21 @@ def _grid_array(grid_size):
 # ---------------------------------------------------------------------------------------------------------
 # LayerNorm + ReLU over expert-grouped rows
 # ---------------------------------------------------------------------------------------------------------
+def _check_ln_width(C, what, max_width=None):
+    """the LayerNorm kernels run the widths LN_WIDTHS, the grouped column sum any multiple of LN_WIDTH_STEP
+    (csrc/layernorm.cu); the C entry points return -2 for any other"""
+    if max_width is None and not ln_width_ok(C):
+        raise ValueError(f"{what}: width {C} is not a multiple of {LN_WIDTH_STEP} in [{LN_WIDTH_STEP}, {LN_MAX_WIDTH}]")
+    if max_width is not None and (C <= 0 or C % LN_WIDTH_STEP):
+        raise ValueError(f"{what}: width {C} is not a positive multiple of {LN_WIDTH_STEP}")
+
+
 def ln_relu_fwd(h, gamma, beta, tile_group, *, out, mean, rstd, relu=True, quant=None, tile_rows=128):
     """:param quant: optional ops.fp8.MXFP8Tensor that additionally receives the output as an MXFP8 GEMM operand
-    (``out`` may then be None: forward-only runs do not need the bf16 copy)"""
+    (``out`` may then be None: forward-only runs do not need the bf16 copy); the MXFP8 path runs C in 256, 512, 1024,
+    2048 and 4096 only"""
     rows, C = h.shape
+    _check_ln_width(C, "ln_relu_fwd")
     assert h.is_contiguous() and gamma.dtype == torch.float32 and (out is None or out.is_contiguous())
     if quant is not None:
         assert quant.K == C and quant.groups == 1 and quant.rows_per_group >= rows and quant.tile_rows == 128
@@ -110,6 +121,7 @@ def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta
     :param dres: optional bf16 [rows, C] gradient of a residual that bypasses the LayerNorm: dh = dres + LN backward, and
         dbias is the column sum of that total"""
     rows, C = h.shape
+    _check_ln_width(C, "ln_relu_bwd")
     assert da.is_contiguous() and h.is_contiguous() and dh.is_contiguous()
     assert dres is None or (dres.shape == h.shape and dres.dtype == torch.bfloat16 and dres.is_contiguous())
     part = torch.empty((rows + tile_rows - 1) // tile_rows, 3, C, device=h.device, dtype=torch.float32)
@@ -123,6 +135,7 @@ def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta
 def grouped_colsum(x, tile_group, *, out, tile_rows=128):
     """out[g] += the column sums of group g's rows, summed in a fixed order (run-to-run identical)"""
     rows, C = x.shape
+    _check_ln_width(C, "grouped_colsum", max_width=0)
     part = torch.empty((rows + tile_rows - 1) // tile_rows, C, device=x.device, dtype=torch.float32)
     native.check(_lib().lah_grouped_colsum(ptr(x), x.stride(0), ptr(out), ptr(part), C, ptr(tile_group), rows,
                                            int(tile_rows), stream_ptr()), "lah_grouped_colsum")
@@ -274,6 +287,16 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
 # ---------------------------------------------------------------------------------------------------------
 MAX_SEQ = 65536   # longest sequence of the attention kernels (csrc/dropout.cuh MAX_SEQ)
 HEAD_DIMS = (32, 64, 128)   # head dims d_model / num_heads of the attention kernels (csrc/attention.cu, attention_bwd.cu)
+# row widths of the LayerNorm kernels (csrc/layernorm.cu LN_MAX_C): every multiple of LN_WIDTH_STEP up to LN_MAX_WIDTH;
+# the grouped column sum runs any multiple of LN_WIDTH_STEP (the in_proj bias gradient sums 3 d_model columns)
+LN_WIDTH_STEP = 128
+LN_MAX_WIDTH = 4096
+LN_WIDTHS = tuple(range(LN_WIDTH_STEP, LN_MAX_WIDTH + 1, LN_WIDTH_STEP))
+
+
+def ln_width_ok(C) -> bool:
+    """True when ``C`` is a width the LayerNorm kernels run (LN_WIDTHS)"""
+    return 0 < C <= LN_MAX_WIDTH and C % LN_WIDTH_STEP == 0
 
 
 def pack_key_mask(pad):

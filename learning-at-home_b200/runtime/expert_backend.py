@@ -33,11 +33,13 @@ class ExpertBackend(nn.Module):
         param groups hold every parameter of the expert once (per group any lr, betas, eps, weight_decay, amsgrad and
         decoupled_weight_decay; ``maximize``, ``capturable``, ``differentiable``, tensor lr / betas and other optimizers
         run on the module).  These modules run natively, plain or ``torch.jit.script``-ed:
-          * ``FeedforwardBlock`` (swap-AB wgmma GEMMs, fused LayerNorm, fused weight-gradient + AMSGrad);
+          * ``FeedforwardBlock(hid)`` with hid a multiple of 128 up to 1024 (swap-AB wgmma GEMMs, fused LayerNorm, fused
+            weight-gradient + AMSGrad);
           * this package's ``TransformerEncoderLayer`` and ``torch.nn.TransformerEncoderLayer`` with ReLU or erf GELU,
             ``norm_first`` True or False, ``batch_first`` True or False, LayerNorm eps 1e-5 and all biases, head dim
-            d_model / nhead in (32, 64, 128), d_model and dim_feedforward multiples of 256, dropout p < 1 at every site,
-            sequence length 1 <= S <= 65536 (wgmma attention and GEMMs, in-kernel dropout, fused AMSGrad).
+            d_model / nhead in (32, 64, 128), d_model a multiple of 128 with 256 <= d_model <= 4096, dim_feedforward a
+            multiple of 128, dropout p < 1 at every site, sequence length 1 <= S <= 65536 (wgmma attention and GEMMs,
+            in-kernel dropout, fused AMSGrad).
         ``torch.nn.TransformerEncoderLayer`` also runs natively with a key padding mask: one positional input and
         ``kwargs_schema={"src_key_padding_mask": BatchTensorProto(S, dtype=torch.bool)}`` (True = padding key, [batch, S]
         for sequence-first layers too).  The flat inputs are then (src, mask) for forward and (src, mask, grad_out) for

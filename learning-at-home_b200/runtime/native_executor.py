@@ -176,6 +176,11 @@ ALIGN = 16
 
 
 class NativeFFNExecutor:
+    """
+    Trainable sm_90a ``FeedforwardBlock(hid)`` expert (the module docstring lists the kernels) for hid a multiple of 128
+    with 4 * hid <= K.LN_MAX_WIDTH = 4096, i.e. hid in 128, 256, ..., 1024: both LayerNorms run at 4 * hid columns.  Wider
+    blocks stay on the module.
+    """
     INPUT_DIMS = 2   # [rows, hid]
 
     def accepts(self, x) -> bool:
@@ -189,7 +194,9 @@ class NativeFFNExecutor:
             return False
         hid = spec.hid
         params = list(expert.parameters())
-        if hid % 128 or not params or not params[0].is_cuda or params[0].dtype != torch.float32:
+        # both LayerNorms run at 4 * hid columns
+        if (hid % 128 or 4 * hid > K.LN_MAX_WIDTH or not params or not params[0].is_cuda
+                or params[0].dtype != torch.float32):
             return False
         if optimizer_groups(opt, NativeFFNExecutor._segment_params(expert)) is None:
             return False
@@ -326,9 +333,10 @@ class NativeTransformerExecutor:
     Trainable sm_90a transformer expert: an encoder layer ``encoder_layer_spec`` accepts (this package's post-LN GELU layer,
     the layer of the reference's experiments/throughput/layers.py:22-51, which the reference's block cannot train; and
     torch.nn.TransformerEncoderLayer post- or pre-LN, ReLU or erf GELU, batch- or sequence-first; each plain or scripted)
-    with any sequence length 1 <= S <= K.MAX_SEQ, head_dim d / nhead in K.HEAD_DIMS = (32, 64, 128), d and
-    dim_feedforward multiples of 256 and every dropout probability in [0, 1).  With nhead = 16 that is d = 512, 1024 and
-    2048; any other layer stays on the module.
+    with any sequence length 1 <= S <= K.MAX_SEQ, head_dim d / nhead in K.HEAD_DIMS = (32, 64, 128), d a multiple of 128
+    with 256 <= d <= K.LN_MAX_WIDTH = 4096 (the LayerNorm kernels' widest row), dim_feedforward any multiple of 128 and
+    every dropout probability in [0, 1).  That includes d = 384 (6 heads), 768 (12 heads, BERT-base / ViT-B), 1280 and
+    1536; any other layer stays on the module.
 
     Sequences: the token dimension B*S is padded with zero rows to a multiple of 128 for the GEMM, LayerNorm and dropout
     kernels; attention sees only the B*S real rows and is told S.  Padding rows contribute exactly zero to every parameter
@@ -385,8 +393,9 @@ class NativeTransformerExecutor:
             return False
         d, heads, ff = spec.d, spec.heads, spec.ff
         params = list(expert.parameters())
-        if (d % heads or d // heads not in K.HEAD_DIMS or d % 256 or ff % 256 or not params[0].is_cuda
-                or params[0].dtype != torch.float32):
+        # d = 128 stays refused: its GEMMs would run 128-wide tiles, and the dropout epilogue runs 256-wide ones only
+        if (d % heads or d // heads not in K.HEAD_DIMS or d % 128 or not 256 <= d <= K.LN_MAX_WIDTH or ff % 128
+                or not params[0].is_cuda or params[0].dtype != torch.float32):
             return False
         if not all(0.0 <= p < 1.0 for p in spec.ps):
             return False   # p = 1 zeroes a whole branch: eager PyTorch handles that configuration
