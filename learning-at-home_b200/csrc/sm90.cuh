@@ -96,6 +96,12 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* 
                  "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                  : "memory");
 }
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                     reinterpret_cast<uint64_t>(tm)),
+                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {

@@ -14,7 +14,7 @@
 //                      (W^T read straight from the same [out, in] tensor as an MN-major operand).
 //   wgrad_adam_kernel  dW tile = dY^T X with wgmma (both operands MN-major, two 32-token stages, reduction over the
 //                      expert's tokens = the gradient reduction over all trainers that routed to it) with the per-expert AMSGrad step FUSED
-//                      INTO THE EPILOGUE: p / m / v / vmax stream through a TMA ring of 32-column chunks of the tile
+//                      INTO THE EPILOGUE: p / m / v / vmax stream through a TMA ring of 4-rows-per-band chunks of the tile
 //                      (loaded while the MMAs run), every thread updates them in shared memory at the positions of its
 //                      accumulator registers and writes the bf16 mirror, and the chunk goes back to HBM by TMA store.
 //                      The weight gradient never exists in HBM: 34 B / parameter
@@ -293,11 +293,14 @@ constexpr int WBK = 32;                                  // tokens per operand s
 constexpr int OP_STAGES = 2;                             // a hot expert has tens of k-blocks: loads run ahead of the MMAs
 constexpr int OP_STAGE_BYTES = 2 * (WBK * BM * 2);       // A [32 t][128 n] + B [32 t][128 k] (two 64-wide MN atoms each)
 constexpr int OP_BYTES = OP_STAGES * OP_STAGE_BYTES;
-// optimizer state streams through its own ring: a chunk is one 32-column slice of the tile (= 4 accumulator column groups)
-// of p, m, v and vmax, each a [128 rows][32 fp32] TMA box with 128-B swizzle
-constexpr int CH_COLS = 32;
-constexpr int CHUNKS = BN_MAX / CH_COLS;                 // chunks per tile
-constexpr int ARR_BYTES = BM * CH_COLS * 4;              // 16 KB: one state array of a chunk
+// optimizer state streams through its own ring.  Chunk c of a tile holds rows 4c .. 4c + 3 of each of the tile's eight
+// 16-row bands (one band per consumer warp) over all 128 columns, so every row is read and written as one 512-B run.  Per
+// array it is four [8 bands][4 rows][32 fp32] boxes of a 3-D view (K, 16, G*N / 16) with 128-B swizzle, side by side.
+constexpr int BAND_ROWS = 4;                             // rows of every 16-row band in one chunk
+constexpr int CHUNKS = 16 / BAND_ROWS;                   // chunks per tile
+constexpr int SUB_COLS = 32;                             // columns of one box (128 B: the swizzle row)
+constexpr int SUB_BYTES = BM / CHUNKS * SUB_COLS * 4;    // 4 KB: one box
+constexpr int ARR_BYTES = (BN_MAX / SUB_COLS) * SUB_BYTES;   // 16 KB: one state array of a chunk
 constexpr int ST_STAGES = 3;
 constexpr int ST_STAGE_BYTES = 4 * ARR_BYTES;
 constexpr int ST_OFFSET = OP_BYTES;
@@ -305,7 +308,7 @@ constexpr int BAR_OFFSET = ST_OFFSET + ST_STAGES * ST_STAGE_BYTES;
 constexpr int QD = 4;                                    // depth of the tile queue (dynamic scheduler)
 constexpr int SMEM_TOTAL = BAR_OFFSET + (2 * OP_STAGES + 2 * ST_STAGES + 2 * QD) * 8 + QD * 4 + 16 + 1024;
 static_assert(ST_STAGES <= CHUNKS, "the producer issues a tile's first ST_STAGES chunks before its remaining k-blocks");
-static_assert(OP_STAGE_BYTES % 1024 == 0 && ARR_BYTES % 1024 == 0, "128-B swizzle atoms need 1 KB alignment");
+static_assert(OP_STAGE_BYTES % 1024 == 0 && SUB_BYTES % 1024 == 0, "128-B swizzle atoms need 1 KB alignment");
 static_assert(SMEM_TOTAL <= 232448, "shared memory budget");
 
 struct Params {
@@ -334,10 +337,22 @@ struct Tile {
     int g, mt, nt;
 };
 
-// state tensor maps: p, m, v, vmax viewed as [G * N, K] fp32 (vmax only read when amsgrad)
+// state tensor maps: p, m, v, vmax viewed as [G * N / 16][16][K] fp32 (vmax only read when amsgrad)
 struct StateMaps {
     CUtensorMap a[4];
 };
+
+// TMA load (bar != nullptr) or store of chunk c of the tile whose rows start at srow and columns at col0, arrays [0, n_arr)
+__device__ __forceinline__ void state_chunk_tma(const StateMaps& tm, int n_arr, uint8_t* ss, uint64_t* bar, int col0, int srow,
+                                                int c) {
+    for (int a = 0; a < n_arr; ++a)
+#pragma unroll
+        for (int q = 0; q < BN_MAX / SUB_COLS; ++q) {
+            uint8_t* s = ss + a * ARR_BYTES + q * SUB_BYTES;
+            if (bar) tma_load_3d(s, &tm.a[a], bar, col0 + q * SUB_COLS, BAND_ROWS * c, srow / 16);
+            else tma_store_3d(&tm.a[a], s, col0 + q * SUB_COLS, BAND_ROWS * c, srow / 16);
+        }
+}
 
 template <int WD>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -424,9 +439,7 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
             auto load_chunk = [&](int c) {
                 mbar_wait(&st_empty[sstage], sphase ^ 1);
                 mbar_arrive_expect_tx(&st_full[sstage], n_arr * ARR_BYTES);
-                uint8_t* ss = st_smem + sstage * ST_STAGE_BYTES;
-                for (int a = 0; a < n_arr; ++a)
-                    tma_load_2d(ss + a * ARR_BYTES, &tmS.a[a], &st_full[sstage], t.nt * BN_MAX + c * CH_COLS, srow);
+                state_chunk_tma(tmS, n_arr, st_smem + sstage * ST_STAGE_BYTES, &st_full[sstage], t.nt * BN_MAX, srow, c);
                 if (++sstage == ST_STAGES) {
                     sstage = 0;
                     sphase ^= 1;
@@ -460,9 +473,16 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
     int qi = 0, stage = 0, sstage = 0;
     uint32_t phase = 0, qphase = 0, sphase = 0;
     float acc[BN_MAX / 2];
-    // this thread's first accumulator row inside the chunk box, and the 128-B swizzle key of its rows (lrow and lrow + 8)
+    float xg[BN_MAX / 8];   // gradient of the partner lane's row, columns 64 .. 127
+    // this thread's accumulator rows of the tile: lrow and lrow + 8, rows lane / 4 and lane / 4 + 8 of its warp's 16-row band
     const int lrow = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int sw = lrow & 7;
+    // Chunk c holds band rows 4c .. 4c + 3: row lrow + 8 (c / 2) of the lanes whose half (lane / 16) is c % 2, and the same
+    // row number of their partner lane ^ 16 in the other half.  Every lane works on every chunk: the row's owner on its
+    // columns 0 .. 63 (j < 8), the partner on columns 64 .. 127 with the owner's gradient fetched by a shuffle.  In a chunk's
+    // boxes both see the row as row R = 4 warp + (lane / 4) % 4 (128 B, 16-B unit u at u ^ (R % 8)).
+    const int brow = (lane >> 2) & 3;
+    const int R = warp * BAND_ROWS + brow;
+    const int jflip = 2 * (brow & 1);
     while (true) {
         mbar_wait(&q_full[qi], qphase);
         const int tile = q_tile[qi];
@@ -510,54 +530,61 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
         const float step_size = p.lr / (1.f - powf(p.beta1, st));
         const float inv_sqrt_bc2 = rsqrtf(1.f - powf(p.beta2, st));
         const int srow = t.g * p.N + t.mt * BM;
-        const long long row_base = static_cast<long long>(srow) + lrow;
         const int col_base = t.nt * BN_MAX + 2 * (lane & 3);
 #pragma unroll
         for (int c = 0; c < CHUNKS; ++c) {
             mbar_wait(&st_full[sstage], sphase);
             uint8_t* ss = st_smem + sstage * ST_STAGE_BYTES;
+            if ((c & 1) == 0) {   // the partner's gradient of columns 64 .. 127 in the current row pair (r, r ^ 4)
 #pragma unroll
-            for (int jj = 0; jj < CH_COLS / 8; ++jj)
+                for (int i = 0; i < BN_MAX / 8; ++i) xg[i] = __shfl_xor_sync(0xffffffffu, acc[4 * (BN_MAX / 16 + i / 2) + i % 2], 16);
+            }
+            const bool own = (lane >> 4) == (c & 1);
+            const long long o_row = (static_cast<long long>(srow) + (own ? lrow : lrow ^ 4) + 8 * (c >> 1)) * p.K + col_base;
+            const int jbase = own ? 0 : BN_MAX / 16;
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    // 16-B unit (2 jj + lane%4 / 2) of row lrow + 8h, XOR-swizzled by the row (8h leaves the pattern alone)
-                    const int so = (lrow + 8 * h) * 128 + (((2 * jj + ((lane & 3) >> 1)) ^ sw) << 4) + 8 * (lane & 1);
-                    float2* sp = reinterpret_cast<float2*>(ss + so);
-                    float2* sm = reinterpret_cast<float2*>(ss + ARR_BYTES + so);
-                    float2* sv = reinterpret_cast<float2*>(ss + 2 * ARR_BYTES + so);
-                    float2* svm = reinterpret_cast<float2*>(ss + 3 * ARR_BYTES + so);
-                    float2 pw = *sp, m = *sm, v = *sv;
-                    float2 vm = p.amsgrad ? *svm : make_float2(0.f, 0.f);
-                    float* pp = &pw.x; float* mp = &m.x; float* vp = &v.x; float* vmp = &vm.x;
+            for (int k = 0; k < BN_MAX / 16; ++k) {
+                // column group j = k of even rows, k ^ 2 of odd rows: rows R and R ^ 1 put the same j in the same two 16-B
+                // units, so this way the 16 lanes of each half cover eight distinct units, and the owners' columns
+                // (boxes 0, 1) and the partners' (boxes 2, 3) one wavefront each: no bank conflict
+                const int j = jbase + (k ^ jflip);
+                const int so = (j >> 2) * SUB_BYTES + R * 128 + (((2 * (j & 3) + ((lane & 3) >> 1)) ^ (R & 7)) << 4) +
+                               8 * (lane & 1);
+                float2* sp = reinterpret_cast<float2*>(ss + so);
+                float2* sm = reinterpret_cast<float2*>(ss + ARR_BYTES + so);
+                float2* sv = reinterpret_cast<float2*>(ss + 2 * ARR_BYTES + so);
+                float2* svm = reinterpret_cast<float2*>(ss + 3 * ARR_BYTES + so);
+                float2 pw = *sp, m = *sm, v = *sv;
+                float2 vm = p.amsgrad ? *svm : make_float2(0.f, 0.f);
+                float* pp = &pw.x; float* mp = &m.x; float* vp = &v.x; float* vmp = &vm.x;
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        float grad = acc[4 * jj + 2 * h + e];
-                        if constexpr (WD == WD_L2) grad += p.wd * pp[e];
-                        if constexpr (WD == WD_DECOUPLED) pp[e] = __fmul_rn(pp[e], p.wd);   // rounded alone, as p.mul_()
-                        mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
-                        vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
-                        float denom;
-                        if (p.amsgrad) {
-                            vmp[e] = fmaxf(vmp[e], vp[e]);
-                            denom = sqrtf(vmp[e]) * inv_sqrt_bc2 + p.eps;
-                        } else {
-                            denom = sqrtf(vp[e]) * inv_sqrt_bc2 + p.eps;
-                        }
-                        pp[e] -= step_size * (mp[e] / denom);
+                for (int e = 0; e < 2; ++e) {
+                    float grad = own ? (jflip ? acc[4 * (k ^ 2) + e] : acc[4 * k + e])
+                                     : (jflip ? xg[2 * (k ^ 2) + e] : xg[2 * k + e]);
+                    if constexpr (WD == WD_L2) grad += p.wd * pp[e];
+                    if constexpr (WD == WD_DECOUPLED) pp[e] = __fmul_rn(pp[e], p.wd);   // rounded alone, as p.mul_()
+                    mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
+                    vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
+                    float denom;
+                    if (p.amsgrad) {
+                        vmp[e] = fmaxf(vmp[e], vp[e]);
+                        denom = sqrtf(vmp[e]) * inv_sqrt_bc2 + p.eps;
+                    } else {
+                        denom = sqrtf(vp[e]) * inv_sqrt_bc2 + p.eps;
                     }
-                    *sp = pw;
-                    *sm = m;
-                    *sv = v;
-                    if (p.amsgrad) *svm = vm;
-                    const long long o = (row_base + 8 * h) * p.K + col_base + CH_COLS * c + 8 * jj;
-                    *reinterpret_cast<uint32_t*>(p.p_bf16 + o) = pack_bf16x2(pw.x, pw.y);
+                    pp[e] -= step_size * (mp[e] / denom);
                 }
+                *sp = pw;
+                *sm = m;
+                *sv = v;
+                if (p.amsgrad) *svm = vm;
+                *reinterpret_cast<uint32_t*>(p.p_bf16 + o_row + 8 * j) = pack_bf16x2(pw.x, pw.y);
+            }
             // the updated chunk goes back to HBM by TMA; its slot returns to the producer once the store has read it
             fence_proxy_async_smem();
             named_bar_sync(1, 256);
             if (threadIdx.x == 0) {
-                for (int a = 0; a < n_arr; ++a)
-                    tma_store_2d(&tmS.a[a], ss + a * ARR_BYTES, t.nt * BN_MAX + c * CH_COLS, srow);
+                state_chunk_tma(tmS, n_arr, ss, nullptr, t.nt * BN_MAX, srow, c);
                 tma_store_commit();
                 tma_store_wait_read<0>();
                 mbar_arrive(&st_empty[sstage]);
@@ -566,10 +593,15 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                 sstage = 0;
                 sphase ^= 1;
             }
-            // the next chunk's gradient moves to acc[0, 16): the chunk loop is not unrolled, and a run-time index into
+            // after the first two chunks the gradient of row lrow + 8 moves to the slots of row lrow: a run-time index into
             // the accumulator would put it in local memory
+            if (c == 1) {
 #pragma unroll
-            for (int i = 0; i < BN_MAX / 2 - 16; ++i) acc[i] = acc[i + 16];
+                for (int j = 0; j < BN_MAX / 8; ++j) {
+                    acc[4 * j] = acc[4 * j + 2];
+                    acc[4 * j + 1] = acc[4 * j + 3];
+                }
+            }
         }
     }
     if (threadIdx.x == 0) tma_store_wait<0>();
@@ -668,11 +700,11 @@ int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long l
     wa::StateMaps tmS;
     {
         float* arrs[4] = {p, m, v, amsgrad ? vmax : p};   // without amsgrad the vmax map is never used
-        uint64_t dims[2] = {(uint64_t)K, (uint64_t)G * N};
-        uint64_t str[1] = {(uint64_t)K * 4};
-        uint32_t box[2] = {wa::CH_COLS, BM};
+        uint64_t dims[3] = {(uint64_t)K, 16, (uint64_t)G * N / 16};
+        uint64_t str[2] = {(uint64_t)K * 4, (uint64_t)K * 64};
+        uint32_t box[3] = {wa::SUB_COLS, wa::BAND_ROWS, BM / 16};
         for (int a = 0; a < 4; ++a) {
-            int r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, arrs[a], dims, str, box);
+            int r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, arrs[a], dims, str, box);
             if (r) return r;
         }
     }
