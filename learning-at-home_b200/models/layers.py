@@ -42,6 +42,16 @@ class FeedforwardBlock(nn.Module):
         return x + self.layers(x)
 
 
+#: the parameters of a FeedforwardBlock, in ``parameters()`` order: the segment name the sm_90a code knows each by -> its
+#: state_dict key (the reference's names, layers.py:8-16)
+FFN_SEG_KEYS = {"w1": "layers.0.weight", "b1": "layers.0.bias", "g1": "layers.1.weight", "be1": "layers.1.bias",
+                "w2": "layers.3.weight", "b2": "layers.3.bias", "g2": "layers.4.weight", "be2": "layers.4.bias",
+                "w3": "layers.6.weight", "b3": "layers.6.bias"}
+FFN_SEG_NAMES = tuple(FFN_SEG_KEYS)
+#: bit s set: segment s is a bias or LayerNorm vector (the weight matrices are stepped by the fused wgrad + Adam kernel)
+FFN_SMALL_SEG_MASK = sum(1 << s for s, n in enumerate(FFN_SEG_NAMES) if not n.startswith("w"))
+
+
 class TransformerEncoderLayer(nn.Module):
     def __init__(self, d_model: int, nhead: int, dim_feedforward: int = 2048, dropout: float = 0.1):
         super().__init__()

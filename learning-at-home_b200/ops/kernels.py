@@ -576,6 +576,20 @@ def weight_decay_args(lr, weight_decay, decoupled):
     return float(weight_decay), 1.0
 
 
+def segment_views(flat, shapes, slots=1):
+    """
+    The layout ``adam_step`` / ``adam_step_ref`` work on, as views of ``flat``: consecutive segments, one per entry of
+    ``shapes`` (name -> shape, in segment order), segment s holding ``slots`` tensors of its shape: {name: [slots, *shape]}.
+    """
+    views, off = {}, 0
+    for name, shape in shapes.items():
+        n = slots * math.prod(shape)
+        views[name] = flat[off: off + n].view(slots, *shape)
+        off += n
+    assert off == flat.numel(), (off, flat.numel())
+    return views
+
+
 def adam_step(p, g, m, v, vmax, p_bf16, seg_sizes, G, *, step=None, group_rows=None, step_scalar=0, lr=1e-3,
               betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, decoupled=False, amsgrad=True, zero_mask=0, world=1,
               peer_grad_off=-1, peer_bases=None, grad_scale=1.0, G_active=0, shadow_of=None, shadow_g_off=-1, me=0,

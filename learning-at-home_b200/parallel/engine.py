@@ -25,14 +25,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..models.layers import FFN_SEG_KEYS as REF_KEYS, FFN_SEG_NAMES as SEG_NAMES, FFN_SMALL_SEG_MASK as SMALL_SEG_MASK
 from ..ops import fp8, gemm, kernels as K, native
-
-SEG_NAMES = ("w1", "b1", "g1", "be1", "w2", "b2", "g2", "be2", "w3", "b3")
-#: name of each segment inside a reference FeedforwardBlock state_dict (layers.py:8-16)
-REF_KEYS = {"w1": "layers.0.weight", "b1": "layers.0.bias", "g1": "layers.1.weight", "be1": "layers.1.bias",
-            "w2": "layers.3.weight", "b2": "layers.3.bias", "g2": "layers.4.weight", "be2": "layers.4.bias",
-            "w3": "layers.6.weight", "b3": "layers.6.bias"}
-SMALL_SEG_MASK = sum(1 << i for i, n in enumerate(SEG_NAMES) if not n.startswith("w"))
 
 
 @dataclass
@@ -374,7 +368,8 @@ class ExpertShard:
         # slots = owned experts + shadow slots (replicas of other ranks' hot experts, only on multi-GPU runs)
         self.slots = slots = E_loc + (ctx.S if ctx is not None else 0)
         shapes = cfg.seg_shapes()
-        self.seg_sizes = [int(math.prod(shapes[n])) for n in SEG_NAMES]
+        shapes = {n: shapes[n] for n in SEG_NAMES}   # in segment order
+        self.seg_sizes = [int(math.prod(shape)) for shape in shapes.values()]
         total = sum(self.seg_sizes) * slots
         f32 = dict(dtype=torch.float32, device=device)
         self.p_off = self.g_off = self.pbf16_off = -1
@@ -391,23 +386,9 @@ class ExpertShard:
         self.v = torch.zeros(total, **f32)
         self.vmax = torch.zeros(total, **f32) if cfg.amsgrad else None
         self.step = torch.zeros(E_loc, dtype=torch.int32, device=device)
-        self.views: Dict[str, torch.Tensor] = {}
-        self.grads: Dict[str, torch.Tensor] = {}
-        self.bf16: Dict[str, torch.Tensor] = {}
-        self.m_views: Dict[str, torch.Tensor] = {}
-        self.v_views: Dict[str, torch.Tensor] = {}
-        self.vmax_views: Dict[str, torch.Tensor] = {}
-        off = 0
-        for name, size in zip(SEG_NAMES, self.seg_sizes):
-            sl = slice(off, off + size * slots)
-            self.views[name] = self.p[sl].view(slots, *shapes[name])
-            self.grads[name] = self.g[sl].view(slots, *shapes[name])
-            self.bf16[name] = self.p_bf16[sl].view(slots, *shapes[name])
-            self.m_views[name] = self.m[sl].view(slots, *shapes[name])
-            self.v_views[name] = self.v[sl].view(slots, *shapes[name])
-            if self.vmax is not None:
-                self.vmax_views[name] = self.vmax[sl].view(slots, *shapes[name])
-            off += size * slots
+        self.views, self.grads, self.bf16, self.m_views, self.v_views = (
+            K.segment_views(flat, shapes, slots) for flat in (self.p, self.g, self.p_bf16, self.m, self.v))
+        self.vmax_views = K.segment_views(self.vmax, shapes, slots) if self.vmax is not None else {}
         # asynchronous-update bookkeeping (DMoEConfig.update_every_*): rows / steps pending since the last optimizer step
         self.pending_rows = torch.zeros(E_loc, dtype=torch.int32, device=device)
         self.pending_steps = torch.zeros(E_loc, dtype=torch.int32, device=device)
@@ -462,13 +443,10 @@ class ExpertShard:
         """torch.optim.Adam-compatible state_dict of local expert `le` (parameter order = module.parameters())"""
         state = {}
         for i, n in enumerate(SEG_NAMES):
-            off = self._seg_offset(n) + le * self.seg_sizes[i]
-            sl = slice(off, off + self.seg_sizes[i])
-            shape = self.views[n].shape[1:]
-            entry = dict(step=torch.tensor(float(self.step[le].item())), exp_avg=self.m[sl].view(shape).clone().cpu(),
-                         exp_avg_sq=self.v[sl].view(shape).clone().cpu())
+            entry = dict(step=torch.tensor(float(self.step[le].item())), exp_avg=self.m_views[n][le].clone().cpu(),
+                         exp_avg_sq=self.v_views[n][le].clone().cpu())
             if self.vmax is not None:
-                entry["max_exp_avg_sq"] = self.vmax[sl].view(shape).clone().cpu()
+                entry["max_exp_avg_sq"] = self.vmax_views[n][le].clone().cpu()
             state[i] = entry
         cfg = self.cfg
         group = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, weight_decay=cfg.weight_decay, amsgrad=cfg.amsgrad,
@@ -487,21 +465,12 @@ class ExpertShard:
                 entry = opt_state["state"].get(i)
                 if entry is None:
                     continue
-                off = self._seg_offset(n) + le * self.seg_sizes[i]
-                sl = slice(off, off + self.seg_sizes[i])
-                self.m[sl].copy_(entry["exp_avg"].reshape(-1))
-                self.v[sl].copy_(entry["exp_avg_sq"].reshape(-1))
+                shape = self.m_views[n].shape[1:]
+                self.m_views[n][le].copy_(entry["exp_avg"].reshape(shape))
+                self.v_views[n][le].copy_(entry["exp_avg_sq"].reshape(shape))
                 if self.vmax is not None and "max_exp_avg_sq" in entry:
-                    self.vmax[sl].copy_(entry["max_exp_avg_sq"].reshape(-1))
+                    self.vmax_views[n][le].copy_(entry["max_exp_avg_sq"].reshape(shape))
                 self.step[le] = int(entry["step"])
-
-    def _seg_offset(self, name: str) -> int:
-        off = 0
-        for n, size in zip(SEG_NAMES, self.seg_sizes):
-            if n == name:
-                return off
-            off += size * self.slots
-        raise KeyError(name)
 
 
 # =========================================================================================================

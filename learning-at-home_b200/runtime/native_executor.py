@@ -17,7 +17,7 @@ from typing import List, NamedTuple, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-from ..models.layers import FeedforwardBlock, TransformerEncoderLayer
+from ..models.layers import FFN_SEG_KEYS, FFN_SEG_NAMES, FFN_SMALL_SEG_MASK, FeedforwardBlock, TransformerEncoderLayer
 from ..ops import kernels as K, native
 
 TORCH_ENCODER_LAYER = "torch.nn.modules.transformer.TransformerEncoderLayer"
@@ -141,37 +141,100 @@ def group_hyper(group) -> dict:
                 amsgrad=bool(group.get("amsgrad", False)))
 
 
-def bind_optimizer_state(opt, params, names, groups, pv, mv, vv, vmv):
-    """load the module's parameters and the optimizer's state into the flat buffers' views and re-bind both to them;
-    returns the step count (the largest of the parameters').  ``max_exp_avg_sq`` exists for the groups with amsgrad, as
-    in torch."""
-    amsgrad = {}
-    for g, mask in zip(opt.param_groups, groups):
-        for s in range(len(params)):
-            if (mask >> s) & 1:
-                amsgrad[s] = bool(g.get("amsgrad", False))
-    steps = 0
-    for s, (name, param) in enumerate(zip(names, params)):
-        pv[name][0].copy_(param.data)
-        param.data = pv[name][0]
-        param.grad = None
-        st = opt.state.get(param, {})
-        if st:
-            mv[name][0].copy_(st["exp_avg"])
-            vv[name][0].copy_(st["exp_avg_sq"])
-            if amsgrad[s] and "max_exp_avg_sq" in st:
-                vmv[name][0].copy_(st["max_exp_avg_sq"])
-            steps = max(steps, int(float(st["step"])))
-        new = dict(step=torch.tensor(float(steps)), exp_avg=mv[name][0], exp_avg_sq=vv[name][0])
-        if amsgrad[s]:
-            new["max_exp_avg_sq"] = vmv[name][0]
-        opt.state[param] = new
-    return steps
+class FlatAdamState:
+    """
+    The parameters, gradients and Adam state of one expert as flat fp32 buffers in the layout of ``K.adam_step`` (one
+    segment per parameter, ``names`` / ``params`` in segment order) with a bf16 mirror of the parameters, and the binding
+    of the module and the torch optimizer to them: the parameters and the optimizer's state tensors are views of the
+    buffers, so ``state_dict()`` of both stays live and keeps torch's layout.
+    """
+
+    def __init__(self, opt, params, names, device):
+        self.opt, self.params, self.names = opt, params, names
+        self.groups = optimizer_groups(opt, params)
+        self.sizes = [p.numel() for p in params]
+        self.all_segs = (1 << len(params)) - 1
+        total = sum(self.sizes)
+        f32 = dict(dtype=torch.float32, device=device)
+        self.p, self.g = torch.zeros(total, **f32), torch.zeros(total, **f32)
+        self.m, self.v, self.vmax = torch.zeros(total, **f32), torch.zeros(total, **f32), torch.zeros(total, **f32)
+        self.p_bf16 = torch.zeros(total, dtype=torch.bfloat16, device=device)
+        self.step = torch.zeros(1, dtype=torch.int32, device=device)   # the step count the kernels read
+        self.one = torch.ones(1, dtype=torch.int32, device=device)
+        shapes = {name: p.shape for name, p in zip(names, params)}
+        self.pv, self.gv, self.mv, self.vv, self.vmv, self.bv = (
+            K.segment_views(flat, shapes) for flat in (self.p, self.g, self.m, self.v, self.vmax, self.p_bf16))
+        self.bind()
+
+    @torch.no_grad()
+    def bind(self):
+        """(re)load the module's parameters and the optimizer's state into the flat buffers and make them views of it; the
+        step count becomes the largest of the parameters'.  ``max_exp_avg_sq`` exists for the groups with amsgrad, as in
+        torch."""
+        amsgrad = {}
+        for g, mask in zip(self.opt.param_groups, self.groups):
+            for s in range(len(self.params)):
+                if (mask >> s) & 1:
+                    amsgrad[s] = bool(g.get("amsgrad", False))
+        steps = 0
+        for s, (name, param) in enumerate(zip(self.names, self.params)):
+            self.pv[name][0].copy_(param.data)
+            param.data = self.pv[name][0]
+            param.grad = None
+            st = self.opt.state.get(param, {})
+            if st:
+                self.mv[name][0].copy_(st["exp_avg"])
+                self.vv[name][0].copy_(st["exp_avg_sq"])
+                if amsgrad[s] and "max_exp_avg_sq" in st:
+                    self.vmv[name][0].copy_(st["max_exp_avg_sq"])
+                steps = max(steps, int(float(st["step"])))
+            new = dict(step=torch.tensor(float(steps)), exp_avg=self.mv[name][0], exp_avg_sq=self.vv[name][0])
+            if amsgrad[s]:
+                new["max_exp_avg_sq"] = self.vmv[name][0]
+            self.opt.state[param] = new
+        self.steps_host = steps
+        self.step.fill_(steps)
+        if self.p.is_cuda:
+            K.cast_bf16(self.p, self.p_bf16)
+        else:
+            self.p_bf16.copy_(self.p)
+
+    def hypers(self):
+        """[(``group_hyper`` of the group, mask of its segments)] of the optimizer's param groups"""
+        return [(group_hyper(g), mask) for g, mask in zip(self.opt.param_groups, self.groups)]
+
+    def begin_step(self):
+        """count the step on the device; before the first optimizer kernel of a backward call"""
+        K.bump_steps(self.step, self.one)
+
+    def adam_step(self, segs):
+        """step the segments of the mask ``segs`` from the gradients in ``g`` and zero those gradients: one launch per
+        param group that holds any of them"""
+        for hyper, mask in self.hypers():
+            m = mask & segs
+            if m:
+                K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step,
+                            zero_mask=segs, seg_mask=0 if m == self.all_segs else m, **hyper)
+
+    def end_step(self):
+        """count the step on the host, in the optimizer's state"""
+        self.steps_host += 1
+        # one step tensor per parameter, as torch keeps them: an eager optimizer that loads a shared one from a checkpoint
+        # increments it once per parameter
+        for param in self.params:
+            self.opt.state[param]["step"] = torch.tensor(float(self.steps_host))
 
 
-SEGS = (("w1", 0, "weight"), ("b1", 0, "bias"), ("g1", 1, "weight"), ("be1", 1, "bias"), ("w2", 3, "weight"),
-        ("b2", 3, "bias"), ("g2", 4, "weight"), ("be2", 4, "bias"), ("w3", 6, "weight"), ("b3", 6, "bias"))
-SMALL_MASK = sum(1 << i for i, (n, _, _) in enumerate(SEGS) if not n.startswith("w"))
+def _runs_natively(params, opt) -> bool:
+    """what both executors ask of the segment parameters and the optimizer: fp32 CUDA parameters, an optimizer
+    ``optimizer_groups`` accepts, and the compiled kernels"""
+    if not params[0].is_cuda or params[0].dtype != torch.float32:
+        return False
+    if optimizer_groups(opt, params) is None:
+        return False
+    return native.have_cuda_kernels()
+
+
 ALIGN = 16
 
 
@@ -193,58 +256,32 @@ class NativeFFNExecutor:
         if spec is None or not torch.cuda.is_available():
             return False
         hid = spec.hid
-        params = list(expert.parameters())
         # both LayerNorms run at 4 * hid columns
-        if (hid % 128 or 4 * hid > K.LN_MAX_WIDTH or not params or not params[0].is_cuda
-                or params[0].dtype != torch.float32):
+        if hid % 128 or 4 * hid > K.LN_MAX_WIDTH or not list(expert.parameters()):
             return False
-        if optimizer_groups(opt, NativeFFNExecutor._segment_params(expert)) is None:
-            return False
-        return native.have_cuda_kernels()
+        return _runs_natively(NativeFFNExecutor._segment_params(expert), opt)
 
     @staticmethod
     def _segment_params(expert):
-        return [getattr(expert.layers[li], attr) for _, li, attr in SEGS]
+        """the parameters in the order of FFN_SEG_NAMES (the segments of the flat buffers); the layers are reached by
+        index, which a scripted block allows too"""
+        keys = (key.split(".") for key in FFN_SEG_KEYS.values())   # "layers.3.weight" -> expert.layers[3].weight
+        return [getattr(expert.layers[int(index)], attr) for _, index, attr in keys]
 
     def __init__(self, expert, opt):
         self.expert, self.opt = expert, opt
         dev = next(expert.parameters()).device
         self.device = dev
         self.hid, self.inner = expert.layers[0].in_features, expert.layers[0].out_features
-        self.params = self._segment_params(expert)
-        self.groups = optimizer_groups(opt, self.params)
-        self.sizes = [p.numel() for p in self.params]
-        total = sum(self.sizes)
-        f32 = dict(dtype=torch.float32, device=dev)
-        self.p, self.g = torch.zeros(total, **f32), torch.zeros(total, **f32)
-        self.m, self.v, self.vmax = torch.zeros(total, **f32), torch.zeros(total, **f32), torch.zeros(total, **f32)
-        self.p_bf16 = torch.zeros(total, dtype=torch.bfloat16, device=dev)
-        self.step = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.one = torch.ones(1, dtype=torch.int32, device=dev)
+        self.state = FlatAdamState(opt, self._segment_params(expert), FFN_SEG_NAMES, dev)
+        self.p, self.m = self.state.p, self.state.m   # the flat parameter and exp_avg buffers
         self.group_off = torch.zeros(1, dtype=torch.int32, device=dev)
         self.group_rows = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.steps_host = 0
         self._cap = 0
-        self.bind()
 
-    # ------------------------------------------------------------------ parameter / optimizer-state binding
-    def _views(self, flat):
-        out, off = {}, 0
-        for (name, _, _), p, n in zip(SEGS, self.params, self.sizes):
-            out[name] = flat[off: off + n].view(1, *p.shape)
-            off += n
-        return out
-
-    @torch.no_grad()
     def bind(self):
-        """(re)load the module's parameters and the optimizer's state into the flat buffers and make them views of it"""
-        self.pv, self.gv = self._views(self.p), self._views(self.g)
-        self.mv, self.vv, self.vmv, self.bv = self._views(self.m), self._views(self.v), self._views(self.vmax), self._views(self.p_bf16)
-        steps = bind_optimizer_state(self.opt, self.params, [n for n, _, _ in SEGS], self.groups, self.pv, self.mv, self.vv,
-                                     self.vmv)
-        self.steps_host = steps
-        self.step.fill_(steps)
-        K.cast_bf16(self.p, self.p_bf16)
+        """re-bind after the module or the optimizer was loaded from a checkpoint (``FlatAdamState.bind``)"""
+        self.state.bind()
 
     def _workspace(self, rows: int):
         cap = (rows + ALIGN - 1) // ALIGN * ALIGN
@@ -266,7 +303,7 @@ class NativeFFNExecutor:
         self.xd[:rows].copy_(x)
         if padded > rows:
             self.xd[rows:padded].zero_()
-        go, gr, pv, bv = self.group_off, self.group_rows, self.pv, self.bv
+        go, gr, pv, bv = self.group_off, self.group_rows, self.state.pv, self.state.bv
         K.swapab_linear(self.xd, bv["w1"], go, gr, out=self.h1, bias=pv["b1"])
         K.ln_relu_fwd(self.h1[:padded], pv["g1"], pv["be1"], None, out=self.a1[:padded], mean=self.stats[0], rstd=self.stats[1],
                       tile_rows=ALIGN)
@@ -288,15 +325,15 @@ class NativeFFNExecutor:
         self.gyd[:rows].copy_(grad_out)
         if padded > rows:
             self.gyd[rows:padded].zero_()
-        go, gr, pv, bv, gv = self.group_off, self.group_rows, self.pv, self.bv, self.gv
-        hypers = [group_hyper(g) for g in self.opt.param_groups]
-        seg_hyper = {SEGS[s][0]: h for h, mask in zip(hypers, self.groups) for s in range(len(SEGS)) if (mask >> s) & 1}
-        K.bump_steps(self.step, self.one)
+        st = self.state
+        go, gr, pv, bv, gv = self.group_off, self.group_rows, st.pv, st.bv, st.gv
+        seg_hyper = {name: h for h, mask in st.hypers() for s, name in enumerate(st.names) if (mask >> s) & 1}
+        st.begin_step()
 
         def wgrad(name, dy, xin):   # each weight matrix with the settings of its own group
             hyper = seg_hyper[name]
-            K.wgrad_adam(dy, xin, go, gr, p=pv[name], m=self.mv[name], v=self.vv[name],
-                         vmax=self.vmv[name] if hyper["amsgrad"] else None, p_bf16=bv[name], step=self.step, **hyper)
+            K.wgrad_adam(dy, xin, go, gr, p=pv[name], m=st.mv[name], v=st.vv[name],
+                         vmax=st.vmv[name] if hyper["amsgrad"] else None, p_bf16=bv[name], step=st.step, **hyper)
 
         K.grouped_colsum(self.gyd[:padded], None, out=gv["b3"], tile_rows=ALIGN)
         K.swapab_linear(self.gyd, bv["w3"], go, gr, out=self.da, w_is_kn=True)
@@ -309,15 +346,8 @@ class NativeFFNExecutor:
                       dh=self.dh[:padded], dgamma=gv["g1"], dbeta=gv["be1"], dbias=gv["b1"], tile_rows=ALIGN)
         K.swapab_linear(self.dh, bv["w1"], go, gr, out=self.dxd, w_is_kn=True, residual=self.gyd)
         wgrad("w1", self.dh, self.xd)
-        for hyper, mask in zip(hypers, self.groups):   # the small vectors: one launch per group that holds any
-            if mask & SMALL_MASK:
-                K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step,
-                            zero_mask=SMALL_MASK, seg_mask=mask & SMALL_MASK, **hyper)
-        self.steps_host += 1
-        # one step tensor per parameter, as torch keeps them: an eager optimizer that loads a shared one from a checkpoint
-        # increments it once per parameter
-        for param in self.params:
-            self.opt.state[param]["step"] = torch.tensor(float(self.steps_host))
+        st.adam_step(FFN_SMALL_SEG_MASK)   # the small vectors
+        st.end_step()
         return self.dxd[:rows].to(x.dtype)
 
 
@@ -392,16 +422,12 @@ class NativeTransformerExecutor:
         if spec is None or not torch.cuda.is_available():
             return False
         d, heads, ff = spec.d, spec.heads, spec.ff
-        params = list(expert.parameters())
         # d = 128 stays refused: its GEMMs would run 128-wide tiles, and the dropout epilogue runs 256-wide ones only
-        if (d % heads or d // heads not in K.HEAD_DIMS or d % 128 or not 256 <= d <= K.LN_MAX_WIDTH or ff % 128
-                or not params[0].is_cuda or params[0].dtype != torch.float32):
+        if d % heads or d // heads not in K.HEAD_DIMS or d % 128 or not 256 <= d <= K.LN_MAX_WIDTH or ff % 128:
             return False
         if not all(0.0 <= p < 1.0 for p in spec.ps):
             return False   # p = 1 zeroes a whole branch: eager PyTorch handles that configuration
-        if optimizer_groups(opt, NativeTransformerExecutor._segment_params(expert)) is None:
-            return False
-        return native.have_cuda_kernels()
+        return _runs_natively(NativeTransformerExecutor._segment_params(expert), opt)
 
     @staticmethod
     def _segment_params(expert):
@@ -429,37 +455,15 @@ class NativeTransformerExecutor:
         self.d, self.heads, self.ff = spec.d, spec.heads, spec.ff
         self.takes_key_padding_mask = class_name(expert) == TORCH_ENCODER_LAYER   # this package's layer has no mask input
         self.norm_first, self.relu, self.batch_first = spec.norm_first, spec.activation == "relu", spec.batch_first
-        self.params = self._segment_params(expert)
-        self.groups = optimizer_groups(opt, self.params)
-        dev = self.params[0].device
-        self.device = dev
-        self.sizes = [p.numel() for p in self.params]
-        total = sum(self.sizes)
-        f32 = dict(dtype=torch.float32, device=dev)
-        self.p, self.g = torch.zeros(total, **f32), torch.zeros(total, **f32)
-        self.m, self.v, self.vmax = torch.zeros(total, **f32), torch.zeros(total, **f32), torch.zeros(total, **f32)
-        self.p_bf16 = torch.zeros(total, dtype=torch.bfloat16, device=dev)
-        self.step = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.one = torch.ones(1, dtype=torch.int32, device=dev)
-        self.steps_host = 0
+        params = self._segment_params(expert)
+        self.device = params[0].device
+        self.state = FlatAdamState(opt, params, self.NAMES, self.device)
+        self.p, self.m = self.state.p, self.state.m   # the flat parameter and exp_avg buffers
         self._ws = {}
-        self.bind()
 
-    def _views(self, flat):
-        out, off = {}, 0
-        for name, p, n in zip(self.NAMES, self.params, self.sizes):
-            out[name] = flat[off: off + n].view(1, *p.shape)
-            off += n
-        return out
-
-    @torch.no_grad()
     def bind(self):
-        self.pv, self.gv, self.bv = self._views(self.p), self._views(self.g), self._views(self.p_bf16)
-        mv, vv, vmv = self._views(self.m), self._views(self.v), self._views(self.vmax)
-        steps = bind_optimizer_state(self.opt, self.params, self.NAMES, self.groups, self.pv, mv, vv, vmv)
-        self.steps_host = steps
-        self.step.fill_(steps)
-        K.cast_bf16(self.p, self.p_bf16)
+        """re-bind after the module or the optimizer was loaded from a checkpoint (``FlatAdamState.bind``)"""
+        self.state.bind()
 
     def _workspace(self, T):
         """buffers for T padded token rows (T a multiple of 128)"""
@@ -519,7 +523,7 @@ class NativeTransformerExecutor:
         if T > Tr:
             ws["x"][Tr:].zero_()
             ws["att"][Tr:].zero_()   # attention writes only the real rows
-        x, bv, pv, site, stats = ws["x"], self.bv, self.pv, self._site, ws["stats"]
+        x, bv, pv, site, stats = ws["x"], self.state.bv, self.state.pv, self._site, ws["stats"]
         if self.norm_first:
             K.ln_relu_fwd(x, pv["g1"], pv["be1"], None, out=ws["xa"], mean=stats[0], rstd=stats[1], relu=False)
         gemm.grouped_linear(ws["xa"] if self.norm_first else x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
@@ -554,7 +558,8 @@ class NativeTransformerExecutor:
         drop = self._dropout()
         key_mask = self._pack(key_padding_mask)
         ws, Tr, T = self._forward(src, drop, key_mask)   # reference semantics: the client re-sends the inputs, the server recomputes the forward
-        d, bv, pv, gv, site, stats = self.d, self.bv, self.pv, self.gv, self._site, ws["stats"]
+        st = self.state
+        d, bv, pv, gv, site, stats = self.d, st.bv, st.pv, st.gv, self._site, ws["stats"]
         go = ws["group_off"]
         bf = dict(dtype=torch.bfloat16, device=self.device)
         seq = self._batch_seq(src)[1]
@@ -626,17 +631,9 @@ class NativeTransformerExecutor:
         else:
             gemm.grouped_wgrad(dqkv, ws["x"], go, 1, out=gv["w_in"])
             dx = gemm.grouped_linear(dqkv, bv["w_in"], w_is_kn=True, residual=dh)
-        K.bump_steps(self.step, self.one)
-        all_segs = (1 << len(self.sizes)) - 1
-        for g, mask in zip(self.opt.param_groups, self.groups):   # one launch per group, over its segments
-            if mask:
-                K.adam_step(self.p, self.g, self.m, self.v, self.vmax, self.p_bf16, self.sizes, 1, step=self.step,
-                            zero_mask=all_segs, seg_mask=0 if mask == all_segs else mask, **group_hyper(g))
-        self.steps_host += 1
-        # one step tensor per parameter, as torch keeps them: an eager optimizer that loads a shared one from a checkpoint
-        # increments it once per parameter
-        for param in self.params:
-            self.opt.state[param]["step"] = torch.tensor(float(self.steps_host))
+        st.begin_step()
+        st.adam_step(st.all_segs)
+        st.end_step()
         return self._from_rows(dx[:Tr], src)
 
 

@@ -129,7 +129,8 @@ def test_fused_layer_oracle_matches_baseline_and_checkpoints_are_interchangeable
     other.shard.load_expert_state_dict(3, sd)
     other.shard.load_expert_optimizer_state(3, opt_state)
     assert torch.equal(other.shard.views["w3"][3], fused.shard.views["w3"][3]) and int(other.shard.step[3]) == 7
-    off = other.shard._seg_offset("w2") + 3 * other.shard.seg_sizes[4]
+    off = other.shard.m_views["w2"][3].storage_offset()   # where expert 3's exp_avg of w2 begins in the flat buffer
+    assert off == other.shard.slots * sum(other.shard.seg_sizes[:4]) + 3 * other.shard.seg_sizes[4]
     assert torch.equal(other.shard.m[off: off + 10], fused.shard.m[off: off + 10])
     assert E.expert_uid(cfg, 6) == "expert.1.2"
 
