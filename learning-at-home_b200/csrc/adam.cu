@@ -40,11 +40,22 @@ struct AdamArgs {
     // computed in double by the caller and rounded to fp32 once, as torch's scalar multiply does.  Read only by the
     // DECOUPLED instantiation; the other one keeps the L2 form (grad += weight_decay * p)
     float decay;
+    // DEV_LR instantiations: {lr, decay} in device memory, written by the host between steps (appended: the fields above
+    // keep their offsets)
+    const float* lr_dev;
 };
 
-template <bool DECOUPLED>
+// DEV_LR: the learning rate and the decoupled factor come from a.lr_dev = {lr, decay} in device memory instead of a.lr /
+// a.decay, so a captured CUDA graph follows a schedule.  Read once per thread; the update expressions are the same, so a
+// launch whose block holds x is bit-identical to a by-value launch with x
+template <bool DECOUPLED, bool DEV_LR>
 __global__ void __launch_bounds__(256) adam_kernel(AdamArgs a) {
     if (a.poison && (*a.poison & 1)) return;
+    float dev_lr = 0.f, dev_decay = 1.f;   // the by-value instantiations read a.lr / a.decay where they are used
+    if constexpr (DEV_LR) {
+        dev_lr = a.lr_dev[0];
+        if constexpr (DECOUPLED) dev_decay = a.lr_dev[1];
+    }
     const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
     const long long span = a.num_ranges ? a.r_cum[a.num_ranges] : a.total;
     for (long long j = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; j < span; j += stride) {
@@ -66,7 +77,7 @@ __global__ void __launch_bounds__(256) adam_kernel(AdamArgs a) {
         const int step = a.step ? a.step[g] : a.step_scalar;
         const float bc1 = 1.f - powf(a.beta1, static_cast<float>(step));
         const float bc2 = 1.f - powf(a.beta2, static_cast<float>(step));
-        const float step_size = a.lr / bc1;
+        const float step_size = (DEV_LR ? dev_lr : a.lr) / bc1;
         const float inv_sqrt_bc2 = rsqrtf(bc2);
         float4 gr;
         if (a.peer_grad_off >= 0) {
@@ -99,7 +110,7 @@ __global__ void __launch_bounds__(256) adam_kernel(AdamArgs a) {
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
             float grad = gp[t];
-            if constexpr (DECOUPLED) pp[t] = __fmul_rn(pp[t], a.decay);   // rounded on its own, as torch's p.mul_()
+            if constexpr (DECOUPLED) pp[t] = __fmul_rn(pp[t], DEV_LR ? dev_decay : a.decay);   // rounded on its own, as torch's p.mul_()
             else if (a.weight_decay != 0.f) grad += a.weight_decay * pp[t];
             mp[t] = mp[t] + (1.f - a.beta1) * (grad - mp[t]);
             vp[t] = vp[t] * a.beta2 + (1.f - a.beta2) * grad * grad;
@@ -150,18 +161,16 @@ using namespace lah;
 
 extern "C" const int* lah_get_poison_word();
 
-extern "C" {
-
-// decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); weight_decay: the L2 coefficient.  At most one of the
-// two forms per launch.
-int lah_adam_step_wd(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
-                     const long long* seg_n, int G,
-                     const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
-                     float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
-                     const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
-                     long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay, cudaStream_t st) {
+// the launch behind lah_adam_step_wd and lah_adam_step_dev: decoupled selects the DECOUPLED instantiation; lr_dev != nullptr
+// the DEV_LR one, which ignores lr and decay
+static int adam_step_launch(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
+                            const long long* seg_n, int G, const int* step, const int* group_rows, int step_scalar, float lr,
+                            float beta1, float beta2, float eps, float weight_decay, int amsgrad, int zero_mask, int world,
+                            long long peer_grad_off, const unsigned long long* peer_bases, float grad_scale, int G_active,
+                            const int* shadow_of, long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay,
+                            bool decoupled, const float* lr_dev, cudaStream_t st) {
     if (num_segs < 1 || num_segs > 12) return -2;
-    if (decay != 1.f && weight_decay != 0.f) return -2;
+    if (decoupled && weight_decay != 0.f) return -2;
     AdamArgs a;
     a.num_segs = num_segs;
     long long off = 0;
@@ -183,6 +192,7 @@ int lah_adam_step_wd(float* p, float* g, float* m, float* v, float* vmax, void* 
     a.poison = lah_get_poison_word();
     a.dead_mask = dead_mask;
     a.decay = decay;
+    a.lr_dev = lr_dev;
     a.num_ranges = 0;
     a.r_cum[0] = 0;
     if (seg_mask) {   // adjacent selected segments merge into one range
@@ -204,11 +214,47 @@ int lah_adam_step_wd(float* p, float* g, float* m, float* v, float* vmax, void* 
     if (span <= 0) return 0;
     long long blocks = (span / 4 + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    if (decay != 1.f)
-        adam_kernel<true><<<(int)blocks, 256, 0, st>>>(a);
-    else
-        adam_kernel<false><<<(int)blocks, 256, 0, st>>>(a);
+    if (lr_dev) {
+        if (decoupled)
+            adam_kernel<true, true><<<(int)blocks, 256, 0, st>>>(a);
+        else
+            adam_kernel<false, true><<<(int)blocks, 256, 0, st>>>(a);
+    } else if (decoupled) {
+        adam_kernel<true, false><<<(int)blocks, 256, 0, st>>>(a);
+    } else {
+        adam_kernel<false, false><<<(int)blocks, 256, 0, st>>>(a);
+    }
     return -(int)cudaGetLastError();
+}
+
+extern "C" {
+
+// decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); weight_decay: the L2 coefficient.  At most one of the
+// two forms per launch.
+int lah_adam_step_wd(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
+                     const long long* seg_n, int G,
+                     const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
+                     float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
+                     const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
+                     long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay, cudaStream_t st) {
+    return adam_step_launch(p, g, m, v, vmax, p_bf16, num_segs, seg_n, G, step, group_rows, step_scalar, lr, beta1, beta2,
+                            eps, weight_decay, amsgrad, zero_mask, world, peer_grad_off, peer_bases, grad_scale, G_active,
+                            shadow_of, shadow_g_off, me, seg_mask, dead_mask, decay, decay != 1.f, nullptr, st);
+}
+
+// lah_adam_step_wd with the learning rate and the decoupled factor read from device memory: lr_dev = {lr, 1 - lr * wd}
+// (the factor computed on the host in double and rounded to fp32 once, only read when decoupled).  decoupled: the
+// configuration's form (AdamW with wd != 0), not inferred from the factor, which is exactly 1 at lr = 0
+int lah_adam_step_dev(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
+                      const long long* seg_n, int G,
+                      const int* step, const int* group_rows, int step_scalar, const float* lr_dev, float beta1, float beta2,
+                      float eps, float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
+                      const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
+                      long long shadow_g_off, int me, int seg_mask, int dead_mask, int decoupled, cudaStream_t st) {
+    if (!lr_dev) return -2;
+    return adam_step_launch(p, g, m, v, vmax, p_bf16, num_segs, seg_n, G, step, group_rows, step_scalar, 0.f, beta1, beta2,
+                            eps, weight_decay, amsgrad, zero_mask, world, peer_grad_off, peer_bases, grad_scale, G_active,
+                            shadow_of, shadow_g_off, me, seg_mask, dead_mask, 1.f, decoupled != 0, lr_dev, st);
 }
 
 int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,

@@ -329,6 +329,9 @@ struct Params {
     int* tile_counter;        // work-stealing tile counter (zeroed before the launch)
     const int* poison;        // optional status word: a step that timed out on a peer must not update anything
 };
+// the tensor maps follow Params in parameter space at 64-B alignment.  Params fills its 128 B exactly, so the device-resident
+// learning rate is not a field here (one more pointer would move the maps by 64 B) but the kernel's last parameter
+static_assert(sizeof(Params) == 128 && sizeof(Params) % alignof(CUtensorMap) == 0, "Params layout");
 
 // weight-decay form of one launch (a template parameter: the WD_NONE instantiation is the kernel without decay)
 constexpr int WD_NONE = 0, WD_L2 = 1, WD_DECOUPLED = 2;
@@ -354,10 +357,13 @@ __device__ __forceinline__ void state_chunk_tma(const StateMaps& tm, int n_arr, 
         }
 }
 
-template <int WD>
+// DEV_LR: the learning rate and, with WD_DECOUPLED, the factor 1 - lr * weight_decay come from lr_dev = {lr, decay} in device
+// memory instead of p.lr / p.wd, so a captured CUDA graph follows a schedule.  Read once per consumer thread; the update
+// expressions are the same, so a launch whose block holds x is bit-identical to a by-value launch with x
+template <int WD, bool DEV_LR>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX,
-                  const __grid_constant__ StateMaps tmS) {
+                  const __grid_constant__ StateMaps tmS, const float* __restrict__ lr_dev) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* st_smem = smem + ST_OFFSET;
@@ -469,6 +475,11 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
     }
 
     // =================================================================== consumers: wgrad tile (MMA) + AMSGrad epilogue
+    float lr = p.lr, wd = p.wd;
+    if constexpr (DEV_LR) {
+        lr = lr_dev[0];
+        if constexpr (WD == WD_DECOUPLED) wd = lr_dev[1];
+    }
     const int wg = warp >> 2;
     int qi = 0, stage = 0, sstage = 0;
     uint32_t phase = 0, qphase = 0, sphase = 0;
@@ -527,7 +538,7 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
 
         // ---- AMSGrad on the accumulator positions: rows r (+8), columns 8j + 2(lane%4) (+1), state from the chunk ring
         const float st = static_cast<float>(__ldg(p.step + t.g));
-        const float step_size = p.lr / (1.f - powf(p.beta1, st));
+        const float step_size = lr / (1.f - powf(p.beta1, st));
         const float inv_sqrt_bc2 = rsqrtf(1.f - powf(p.beta2, st));
         const int srow = t.g * p.N + t.mt * BM;
         const int col_base = t.nt * BN_MAX + 2 * (lane & 3);
@@ -561,8 +572,8 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                 for (int e = 0; e < 2; ++e) {
                     float grad = own ? (jflip ? acc[4 * (k ^ 2) + e] : acc[4 * k + e])
                                      : (jflip ? xg[2 * (k ^ 2) + e] : xg[2 * k + e]);
-                    if constexpr (WD == WD_L2) grad += p.wd * pp[e];
-                    if constexpr (WD == WD_DECOUPLED) pp[e] = __fmul_rn(pp[e], p.wd);   // rounded alone, as p.mul_()
+                    if constexpr (WD == WD_L2) grad += wd * pp[e];
+                    if constexpr (WD == WD_DECOUPLED) pp[e] = __fmul_rn(pp[e], wd);   // rounded alone, as p.mul_()
                     mp[e] = mp[e] + (1.f - p.beta1) * (grad - mp[e]);
                     vp[e] = vp[e] * p.beta2 + (1.f - p.beta2) * grad * grad;
                     float denom;
@@ -687,14 +698,25 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
     return -(int)cudaGetLastError();
 }
 
-// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
-// weight_decay: the L2 coefficient; decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); at most one of the two
-int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                      const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                      float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
-                      float weight_decay, float decay, int max_ctas, cudaStream_t st) {
+}  // extern "C"
+
+template <int WD, bool DEV_LR>
+static int launch_wgrad_adam(const wa::Params& a, const CUtensorMap& tmDY, const CUtensorMap& tmX, const wa::StateMaps& tmS,
+                             const float* lr_dev, int ctas, cudaStream_t st) {
+    if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<WD, DEV_LR>>(wa::SMEM_TOTAL)) return e;
+    wa::wgrad_adam_kernel<WD, DEV_LR><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS, lr_dev);
+    return -(int)cudaGetLastError();
+}
+
+// the launch behind lah_wgrad_adam_wd and lah_wgrad_adam_dev: decoupled selects WD_DECOUPLED (with factor `decay`),
+// weight_decay != 0 WD_L2; lr_dev != nullptr the DEV_LR instantiation, which ignores lr and decay
+static int wgrad_adam_launch(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                             const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                             float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
+                             float weight_decay, float decay, bool decoupled, const float* lr_dev, int max_ctas,
+                             cudaStream_t st) {
     if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8) || 1ll * G * N > INT_MAX) return -2;
-    if (decay != 1.f && weight_decay != 0.f) return -2;
+    if (decoupled && weight_decay != 0.f) return -2;
     if (amsgrad && !vmax) return -2;   // AMSGrad streams vmax through its own tensor map
     CUtensorMap tmDY, tmX;
     wa::StateMaps tmS;
@@ -725,7 +747,7 @@ int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long l
     wa::Params a;
     a.G = G; a.N = N; a.K = K; a.group_off = group_off; a.group_rows = group_rows; a.skip = skip; a.step = step;
     a.p = p; a.m = m; a.v = v; a.vmax = vmax; a.p_bf16 = (bf16*)p_bf16; a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.amsgrad = amsgrad;
-    a.wd = decay != 1.f ? decay : weight_decay;
+    a.wd = decoupled ? decay : weight_decay;
     a.tile_counter = tile_counter() ? tile_counter() + 16 : nullptr;   // own word (64 B apart from the GEMM's)
     a.poison = g_poison;
     if (!a.tile_counter) return -3;
@@ -733,17 +755,38 @@ int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long l
     if (total <= 0) return 0;
     if (cudaMemsetAsync(a.tile_counter, 0, sizeof(int), st) != cudaSuccess) return -4;
     const int ctas = persistent_grid(total, max_ctas);
-    if (decay != 1.f) {
-        if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<wa::WD_DECOUPLED>>(wa::SMEM_TOTAL)) return e;
-        wa::wgrad_adam_kernel<wa::WD_DECOUPLED><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
-    } else if (weight_decay != 0.f) {
-        if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<wa::WD_L2>>(wa::SMEM_TOTAL)) return e;
-        wa::wgrad_adam_kernel<wa::WD_L2><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
-    } else {
-        if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<wa::WD_NONE>>(wa::SMEM_TOTAL)) return e;
-        wa::wgrad_adam_kernel<wa::WD_NONE><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS);
+    if (lr_dev) {
+        if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, true>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
+        if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, true>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
+        return launch_wgrad_adam<wa::WD_NONE, true>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
     }
-    return -(int)cudaGetLastError();
+    if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+    if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+    return launch_wgrad_adam<wa::WD_NONE, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+}
+
+extern "C" {
+
+// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
+// weight_decay: the L2 coefficient; decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); at most one of the two
+int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                      const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                      float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
+                      float weight_decay, float decay, int max_ctas, cudaStream_t st) {
+    return wgrad_adam_launch(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, m, v, vmax, p_bf16,
+                             lr, beta1, beta2, eps, amsgrad, weight_decay, decay, decay != 1.f, nullptr, max_ctas, st);
+}
+
+// lah_wgrad_adam_wd with the learning rate and the decoupled factor read from device memory: lr_dev = {lr, 1 - lr * wd}
+// (the factor computed on the host in double and rounded to fp32 once, only read when decoupled).  decoupled: the
+// configuration's form (AdamW with wd != 0), not inferred from the factor, which is exactly 1 at lr = 0
+int lah_wgrad_adam_dev(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                       const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                       float* v, float* vmax, void* p_bf16, const float* lr_dev, float beta1, float beta2, float eps,
+                       int amsgrad, float weight_decay, int decoupled, int max_ctas, cudaStream_t st) {
+    if (!lr_dev) return -2;
+    return wgrad_adam_launch(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, m, v, vmax, p_bf16,
+                             0.f, beta1, beta2, eps, amsgrad, weight_decay, 1.f, decoupled != 0, lr_dev, max_ctas, st);
 }
 
 int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,

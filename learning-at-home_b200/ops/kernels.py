@@ -41,6 +41,7 @@ def _lib():
         "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, P, I, P],
         "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, I, P],
         "lah_wgrad_adam_wd": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, Fl, Fl, I, P],
+        "lah_wgrad_adam_dev": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, I, Fl, I, I, P],
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
@@ -55,6 +56,8 @@ def _lib():
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, P],
         "lah_adam_step_wd": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
                              P],
+        "lah_adam_step_dev": [P, P, P, P, P, P, I, P, I, P, P, I, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, I,
+                              P],
         "lah_bump_steps": [P, P, I, P],
         "lah_cast_bf16": [P, P, L, P],
         "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
@@ -576,6 +579,17 @@ def weight_decay_args(lr, weight_decay, decoupled):
     return float(weight_decay), 1.0
 
 
+def lr_block_values(lr, weight_decay, decoupled):
+    """the two floats of the device block that ``lr_dev`` points to: [lr, decoupled factor 1 - lr * wd] (the factor as
+    ``weight_decay_args`` forms it, 1 without decoupled decay)"""
+    return float(lr), weight_decay_args(lr, weight_decay, decoupled)[1]
+
+
+def _check_lr_dev(lr_dev):
+    assert (lr_dev.is_cuda and lr_dev.dtype == torch.float32 and lr_dev.numel() == 2 and lr_dev.is_contiguous()), \
+        "lr_dev: a contiguous float32 CUDA tensor [lr, decay] (lr_block_values)"
+
+
 def segment_views(flat, shapes, slots=1):
     """
     The layout ``adam_step`` / ``adam_step_ref`` work on, as views of ``flat``: consecutive segments, one per entry of
@@ -593,9 +607,12 @@ def segment_views(flat, shapes, slots=1):
 def adam_step(p, g, m, v, vmax, p_bf16, seg_sizes, G, *, step=None, group_rows=None, step_scalar=0, lr=1e-3,
               betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, decoupled=False, amsgrad=True, zero_mask=0, world=1,
               peer_grad_off=-1, peer_bases=None, grad_scale=1.0, G_active=0, shadow_of=None, shadow_g_off=-1, me=0,
-              seg_mask=0, dead_mask=0):
+              seg_mask=0, dead_mask=0, lr_dev=None):
     """
     One fused Adam/AMSGrad step over a flat fp32 buffer laid out as consecutive segments [G, seg_sizes[s]].
+    :param lr_dev: optional float32 CUDA tensor [2] = ``lr_block_values(lr, weight_decay, decoupled)``: the kernel reads the
+        learning rate and the decoupled factor from it when it runs (``lr`` is then not used), so a captured CUDA graph
+        follows a schedule.  Bit-identical to the by-value launch with the same values
     :param step: int32 [G] per-group step counts (already incremented) or None -> step_scalar for everything
     :param group_rows: int32 [G]; groups with 0 rows are skipped (experts that received no tokens are not stepped)
     :param weight_decay: torch's ``weight_decay``: L2 (added to the gradient), or with ``decoupled`` AdamW's p *= 1 - lr wd
@@ -610,6 +627,18 @@ def adam_step(p, g, m, v, vmax, p_bf16, seg_sizes, G, *, step=None, group_rows=N
         seg_sizes = [seg_sizes]
     segs = (c_ll * len(seg_sizes))(*[int(s) for s in seg_sizes])
     l2, decay = weight_decay_args(lr, weight_decay, decoupled)
+    if lr_dev is not None:
+        _check_lr_dev(lr_dev)
+        native.check(_lib().lah_adam_step_dev(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
+                                              ctypes.cast(segs, c_void_p), G, ptr(step), ptr(group_rows), int(step_scalar),
+                                              ptr(lr_dev), betas[0], betas[1], eps, l2, int(amsgrad), int(zero_mask), world,
+                                              peer_grad_off,
+                                              ctypes.cast(arr, c_void_p) if arr is not None else c_void_p(0), grad_scale,
+                                              int(G_active), ptr(shadow_of), int(shadow_g_off), int(me), int(seg_mask),
+                                              int(dead_mask), int(bool(decoupled and weight_decay)), stream_ptr()),
+                     "lah_adam_step_dev")
+        native.count_launch()
+        return
     native.check(_lib().lah_adam_step_wd(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
                                          ctypes.cast(segs, c_void_p), G, ptr(step),
                                          ptr(group_rows), int(step_scalar), lr, betas[0], betas[1], eps, l2,
@@ -660,12 +689,12 @@ def swapab_linear_ref(x, w, group_off, group_rows, *, bias=None, residual=None, 
 
 
 def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, skip=None, lr=1e-3, betas=(0.9, 0.999),
-               eps=1e-8, amsgrad=True, weight_decay=0.0, decoupled=False, max_ctas=0):
+               eps=1e-8, amsgrad=True, weight_decay=0.0, decoupled=False, max_ctas=0, lr_dev=None):
     """
     Fused weight gradient + per-expert AMSGrad (csrc/small_m.cu): for every group g with rows > 0,
     dW[g] = dy_g^T x_g is formed in registers and applied to p / m / v / vmax ([G, N, K] fp32) and the bf16 mirror in the same
     kernel; the gradient never reaches HBM.  ``step`` holds the per-expert step counts AFTER this update.
-    ``weight_decay`` / ``decoupled``: as in ``adam_step``.
+    ``weight_decay`` / ``decoupled`` / ``lr_dev``: as in ``adam_step``.
     """
     G, N, Kd = p.shape
     assert dy.shape[1] == N and x.shape[1] == Kd and dy.shape[0] == x.shape[0] and p.is_contiguous()
@@ -673,6 +702,15 @@ def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, ski
     if amsgrad and vmax is None:
         raise ValueError("wgrad_adam: amsgrad needs a vmax tensor (vmax=None only with amsgrad=False)")
     l2, decay = weight_decay_args(lr, weight_decay, decoupled)
+    if lr_dev is not None:
+        _check_lr_dev(lr_dev)
+        native.check(_lib().lah_wgrad_adam_dev(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd,
+                                               ptr(group_off), ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m),
+                                               ptr(v), ptr(vmax), ptr(p_bf16), ptr(lr_dev), betas[0], betas[1], eps,
+                                               int(amsgrad), l2, int(bool(decoupled and weight_decay)), int(max_ctas),
+                                               stream_ptr()), "lah_wgrad_adam_dev")
+        native.count_launch()
+        return
     native.check(_lib().lah_wgrad_adam_wd(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd,
                                           ptr(group_off), ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v),
                                           ptr(vmax), ptr(p_bf16), lr, betas[0], betas[1], eps, int(amsgrad), l2, decay,

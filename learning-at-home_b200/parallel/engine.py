@@ -219,6 +219,10 @@ class EngineContext:
         self._opt_pending = False
         self.defer_join = False   # DMoETrainer joins the optimizer stream itself, at the very end of its step
         K.set_poison_word(self.status)   # a step in which a peer timed out applies no optimizer update (the batch fails)
+        # learning rate of every expert and trainer optimizer launch, read by the kernels from device memory (K.lr_block_values:
+        # [lr, 1 - lr * wd]) so that a captured graph of the step follows cfg.lr.  Allocated once: the graph holds its address
+        self._lr_written = K.lr_block_values(cfg.lr, cfg.weight_decay, cfg.decoupled_weight_decay)
+        self.lr_dev = torch.tensor(self._lr_written, dtype=torch.float32, device=self.device)
         assert 2 * cfg.num_layers + 4 < self.EPOCH_STRIDE
         self.alive = torch.ones(self.E, dtype=torch.uint8, device=self.device)
         # device-resident expert index shared by ALL ranks ("DHT collapse", SURVEY 5.8): hb[e] = last heartbeat (ms) of expert
@@ -240,6 +244,23 @@ class EngineContext:
         self.heap.barrier()
 
     EPOCH_STRIDE = 64   # epochs a step may consume; the device-side base advances by this much per begin_step()
+
+    def adam_kwargs(self) -> Dict:
+        """``cfg.adam_kwargs()`` plus the device block ``lr_dev``: the keywords of every optimizer launch on the GPU"""
+        return dict(self.cfg.adam_kwargs(), lr_dev=self.lr_dev)
+
+    def refresh_lr(self):
+        """Write cfg.lr (and the decoupled factor it implies) into ``lr_dev`` when it differs from the last value written.
+        Call at a step boundary: the optimizer stream of the previous step has been joined, and the next step's optimizer
+        launches wait on the current stream.  Two in-place fills on the current stream, so the host does not wait.  Never
+        while a graph is being captured: a captured write would put the capture-time rate back at every replay."""
+        cfg = self.cfg
+        vals = K.lr_block_values(cfg.lr, cfg.weight_decay, cfg.decoupled_weight_decay)
+        if vals == self._lr_written or torch.cuda.is_current_stream_capturing():
+            return
+        self.lr_dev[0].fill_(vals[0])
+        self.lr_dev[1].fill_(vals[1])
+        self._lr_written = vals
 
     def close(self):
         """release the symmetric heap (peer mappings + the arena); idempotent.  All tensors carved out of the heap become
@@ -622,6 +643,7 @@ class FusedDMoE(nn.Module):
         B, k = x.shape[0], cfg.k
         P = B * k
         c.join_optimizer_stream()   # no-op inside DMoETrainer steps (joined there); protects layer-level callers
+        c.refresh_lr()              # layer-level callers: a step begins here (DMoETrainer refreshed before the step)
         epoch = c.next_epoch()
         idx, w, pos, pair_row = ws.idx[:P], ws.w[:P], ws.pos[:P], ws.pair_row[:P]
         K.gate_topk(logits, self.grid_size, k, alive=c.alive, failure_rate=cfg.failure_rate if self.training else 0.0,
@@ -742,7 +764,7 @@ class FusedDMoE(nn.Module):
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         tg, go, rows, T = ws.tile_group, ws.group_off, ws.group_rows, c.tile_rows
         gr = sh.grads
-        opt = cfg.adam_kwargs()
+        opt = c.adam_kwargs()
         main = torch.cuda.current_stream(c.device)
         side, chain_ctas = c.opt_stream, c.chain_ctas
 
@@ -794,7 +816,7 @@ class FusedDMoE(nn.Module):
             rows, zero_mask = sh.fire, (1 << len(SEG_NAMES)) - 1
         K.bump_steps(sh.step, rows)
         K.adam_step(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
-                    group_rows=rows, **cfg.adam_kwargs(), zero_mask=zero_mask, G_active=self.E_loc, world=c.world,
+                    group_rows=rows, **c.adam_kwargs(), zero_mask=zero_mask, G_active=self.E_loc, world=c.world,
                     peer_bases=c.heap.peer_bases if c.S else None, shadow_of=ws.owned_shadow if c.S else None,
                     shadow_g_off=sh.g_off, me=c.rank)
         sh.w8_dirty = True

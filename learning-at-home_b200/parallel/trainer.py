@@ -12,6 +12,7 @@ Linear, reference notebook cell 2), the symmetric-heap context, and the trainer-
 
 ``train_step(x_host, y_host)`` is the end-to-end call: pinned host tensors in, python float (loss) out.
 """
+import math
 from typing import Optional
 
 import torch
@@ -43,9 +44,9 @@ class DMoETrainer:
         :param metrics_path: append one JSON record per ``log_step()`` call to this file (structured step metrics)
         :param use_graph: capture the WHOLE training step (forward, loss, backward, expert and trainer optimizers, the peer
             flag protocol) in one CUDA graph after two eager steps and replay it afterwards.  Everything that changes from
-            step to step (flag epochs, failure-injection stream, Adam step counters) lives in device memory, so the replayed
-            graph is exact.  None = automatic: on for the small-batch (weight-streaming) regime where a step is ~130 short
-            kernels, off for the saturated regime where launch latency is hidden anyway.
+            step to step (flag epochs, failure-injection stream, Adam step counters, the learning rate) lives in device
+            memory, so the replayed graph is exact.  None = automatic: on for the small-batch (weight-streaming) regime
+            where a step is ~130 short kernels, off for the saturated regime where launch latency is hidden anyway.
         """
         from .profiler import MetricsLog
         self.cfg = cfg
@@ -99,6 +100,22 @@ class DMoETrainer:
         self.close()
         return False
 
+    # ------------------------------------------------------------------ learning rate
+    @property
+    def lr(self) -> float:
+        """the learning rate of every expert and trainer optimizer (``cfg.lr``)"""
+        return self.cfg.lr
+
+    def set_lr(self, lr: float) -> None:
+        """Set the learning rate of every expert and trainer optimizer from the next step on: eager, CPU and CUDA-graph
+        replay alike, without re-capturing (the kernels read it from device memory).  Assigning ``cfg.lr`` does the same.
+        Collective on multi-GPU runs: every rank must set the same value before the same step, or the replicated trainer
+        parameters diverge."""
+        lr = float(lr)
+        if not math.isfinite(lr) or lr < 0.0:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        self.cfg.lr = lr
+
     # ------------------------------------------------------------------ trainer-side flat parameters
     def _flatten_trainer_params(self):
         params = [p for p in self.model.parameters() if p.requires_grad]  # a frozen (emulator-style) gate stays out
@@ -146,7 +163,7 @@ class DMoETrainer:
             epoch = c.next_epoch()
             K.signal_wait(c.flags_off, K.SLOT_TRAINER, epoch, c.status, signal=True, wait=True)
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, **cfg.adam_kwargs(),
+                        step=self.step_dev, **c.adam_kwargs(),
                         world=c.world, peer_grad_off=self.flat_g_off, peer_bases=c.heap.peer_bases,
                         grad_scale=1.0 / alive, dead_mask=c.dead_mask)
             K.signal_wait(c.flags_off, K.SLOT_BARRIER, epoch, c.status, signal=True, wait=True)
@@ -159,12 +176,12 @@ class DMoETrainer:
             K.nvls_allreduce(self.flat_g_off, self._n_pad, 1.0 / c.world)
             K.signal_wait(c.flags_off, K.SLOT_BARRIER, epoch, c.status, signal=True, wait=True)
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, **cfg.adam_kwargs(), zero_mask=1)
+                        step=self.step_dev, **c.adam_kwargs(), zero_mask=1)
         elif c.world > 1:
             epoch = c.next_epoch()
             K.signal_wait(c.flags_off, K.SLOT_TRAINER, epoch, c.status, signal=True, wait=True)
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, **cfg.adam_kwargs(),
+                        step=self.step_dev, **c.adam_kwargs(),
                         world=c.world, peer_grad_off=self.flat_g_off, peer_bases=c.heap.peer_bases,
                         grad_scale=1.0 / c.world)
             # nobody may overwrite its gradient buffer before every peer has consumed it
@@ -172,7 +189,7 @@ class DMoETrainer:
             self.flat_g.zero_()
         else:
             K.adam_step(self.flat_p, self.flat_g, self.flat_m, self.flat_v, self.flat_vmax, None, [self._n_pad], 1,
-                        step=self.step_dev, **cfg.adam_kwargs(), zero_mask=1)
+                        step=self.step_dev, **c.adam_kwargs(), zero_mask=1)
 
     # ------------------------------------------------------------------ steps
     def train_step_device(self, x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
@@ -188,6 +205,7 @@ class DMoETrainer:
             self._capture(B)
         self._gx.copy_(x, non_blocking=True)
         self._gy.copy_(y, non_blocking=True)
+        self.ctx.refresh_lr()
         self._graph.replay()
         self.step_count += 1
         native.count_launch(self._graph_launches)
@@ -212,6 +230,7 @@ class DMoETrainer:
         self.model.train()
         timer = self.ctx.timer if self.cuda else None
         if self.cuda:
+            self.ctx.refresh_lr()   # skipped while this step is being captured
             self.ctx.begin_step()
             self.ctx.defer_join = True   # this step joins the optimizer stream itself (below), not at the end of backward()
         if timer is not None:
@@ -415,7 +434,7 @@ class DMoETrainer:
             torch.cuda.synchronize(self.device)
         trainer = dict(model={k: v.detach().clone().cpu() for k, v in self.model.state_dict().items()},
                        exp_avg=self.flat_m.detach().clone().cpu(), exp_avg_sq=self.flat_v.detach().clone().cpu(),
-                       max_exp_avg_sq=self.flat_vmax.detach().clone().cpu(), step=self.step_count)
+                       max_exp_avg_sq=self.flat_vmax.detach().clone().cpu(), step=self.step_count, lr=self.lr)
         # the failure-injection stream position: device-side token base on GPU runs (csrc/moe.cu Peers::step_ctr)
         token_base = int(self.ctx.step_ctr[2:4].view(torch.int64).item()) if self.cuda else 0
         state = dict(trainer=trainer, experts=experts, rng=torch.get_rng_state(), token_base=token_base)
@@ -443,6 +462,8 @@ class DMoETrainer:
                 block.shard.pending_steps.copy_(pend["steps"])
                 block.shard.g.copy_(pend["grad"])
         self.step_count = int(state["trainer"]["step"])
+        if "lr" in state["trainer"]:   # checkpoints without it keep cfg.lr
+            self.set_lr(state["trainer"]["lr"])
         if self.cuda:
             self.step_dev.fill_(self.step_count)
             self.ctx.step_ctr[2:4].view(torch.int64).fill_(int(state.get("token_base", 0)))
