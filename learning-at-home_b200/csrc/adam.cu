@@ -161,14 +161,17 @@ using namespace lah;
 
 extern "C" const int* lah_get_poison_word();
 
-// the launch behind lah_adam_step_wd and lah_adam_step_dev: decoupled selects the DECOUPLED instantiation; lr_dev != nullptr
-// the DEV_LR one, which ignores lr and decay
-static int adam_step_launch(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
-                            const long long* seg_n, int G, const int* step, const int* group_rows, int step_scalar, float lr,
-                            float beta1, float beta2, float eps, float weight_decay, int amsgrad, int zero_mask, int world,
-                            long long peer_grad_off, const unsigned long long* peer_bases, float grad_scale, int G_active,
-                            const int* shadow_of, long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay,
-                            bool decoupled, const float* lr_dev, cudaStream_t st) {
+extern "C" {
+
+// weight_decay: the L2 coefficient; decay: the decoupled weight-decay factor 1 - lr * wd, read only when `decoupled` is set,
+// which selects the DECOUPLED instantiation.  At most one of the two forms per launch.  lr_dev == NULL: lr and decay by
+// value; otherwise lr_dev = {lr, 1 - lr * wd} in device memory (the factor computed on the host in double and rounded to
+// fp32 once) and the DEV_LR instantiation, which ignores lr and decay, so a captured CUDA graph follows a schedule
+int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs, const long long* seg_n,
+                  int G, const int* step, const int* group_rows, int step_scalar, float lr, const float* lr_dev, float beta1,
+                  float beta2, float eps, float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
+                  const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
+                  long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay, int decoupled, cudaStream_t st) {
     if (num_segs < 1 || num_segs > 12) return -2;
     if (decoupled && weight_decay != 0.f) return -2;
     AdamArgs a;
@@ -225,47 +228,6 @@ static int adam_step_launch(float* p, float* g, float* m, float* v, float* vmax,
         adam_kernel<false, false><<<(int)blocks, 256, 0, st>>>(a);
     }
     return -(int)cudaGetLastError();
-}
-
-extern "C" {
-
-// decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); weight_decay: the L2 coefficient.  At most one of the
-// two forms per launch.
-int lah_adam_step_wd(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
-                     const long long* seg_n, int G,
-                     const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
-                     float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
-                     const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
-                     long long shadow_g_off, int me, int seg_mask, int dead_mask, float decay, cudaStream_t st) {
-    return adam_step_launch(p, g, m, v, vmax, p_bf16, num_segs, seg_n, G, step, group_rows, step_scalar, lr, beta1, beta2,
-                            eps, weight_decay, amsgrad, zero_mask, world, peer_grad_off, peer_bases, grad_scale, G_active,
-                            shadow_of, shadow_g_off, me, seg_mask, dead_mask, decay, decay != 1.f, nullptr, st);
-}
-
-// lah_adam_step_wd with the learning rate and the decoupled factor read from device memory: lr_dev = {lr, 1 - lr * wd}
-// (the factor computed on the host in double and rounded to fp32 once, only read when decoupled).  decoupled: the
-// configuration's form (AdamW with wd != 0), not inferred from the factor, which is exactly 1 at lr = 0
-int lah_adam_step_dev(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
-                      const long long* seg_n, int G,
-                      const int* step, const int* group_rows, int step_scalar, const float* lr_dev, float beta1, float beta2,
-                      float eps, float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
-                      const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
-                      long long shadow_g_off, int me, int seg_mask, int dead_mask, int decoupled, cudaStream_t st) {
-    if (!lr_dev) return -2;
-    return adam_step_launch(p, g, m, v, vmax, p_bf16, num_segs, seg_n, G, step, group_rows, step_scalar, 0.f, beta1, beta2,
-                            eps, weight_decay, amsgrad, zero_mask, world, peer_grad_off, peer_bases, grad_scale, G_active,
-                            shadow_of, shadow_g_off, me, seg_mask, dead_mask, 1.f, decoupled != 0, lr_dev, st);
-}
-
-int lah_adam_step(float* p, float* g, float* m, float* v, float* vmax, void* p_bf16, int num_segs,
-                  const long long* seg_n, int G,
-                  const int* step, const int* group_rows, int step_scalar, float lr, float beta1, float beta2, float eps,
-                  float weight_decay, int amsgrad, int zero_mask, int world, long long peer_grad_off,
-                  const unsigned long long* peer_bases, float grad_scale, int G_active, const int* shadow_of,
-                  long long shadow_g_off, int me, int seg_mask, int dead_mask, cudaStream_t st) {
-    return lah_adam_step_wd(p, g, m, v, vmax, p_bf16, num_segs, seg_n, G, step, group_rows, step_scalar, lr, beta1, beta2,
-                            eps, weight_decay, amsgrad, zero_mask, world, peer_grad_off, peer_bases, grad_scale, G_active,
-                            shadow_of, shadow_g_off, me, seg_mask, dead_mask, 1.f, st);
 }
 
 int lah_bump_steps(int* step, const int* group_rows, int G, cudaStream_t st) {

@@ -319,20 +319,6 @@ __global__ void __launch_bounds__(256) attention_pack_key_mask_kernel(const uint
     words[w] = bits;
 }
 
-static int attention_fwd_entry(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads,
-                               int d_model, unsigned long long seed, int drop_thr, float rescale, cudaStream_t st,
-                               const uint32_t* key_mask) {
-    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
-    const int hd = d_model / num_heads;
-    if (hd != 32 && hd != 64 && hd != 128) return -2;
-    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
-    const long long batch = tokens / seq_len;
-    if (batch == 0) return 0;
-    if (hd == 32) return v2::launch_fwd<32>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
-    if (hd == 64) return v2::launch_fwd<64>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
-    return v2::launch_fwd<128>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
-}
-
 }  // namespace attn
 }  // namespace lah
 
@@ -345,17 +331,19 @@ extern "C" {
 // lse2: [tokens, heads] fp32 or NULL.  Returns -2 for a head dim d_model / num_heads other than 32, 64 or 128 (or heads that
 // do not divide d_model), a sequence length out of range or one that does not divide tokens.
 // drop_thr < 0: no dropout; otherwise attention dropout with threshold drop_thr (dropout.cuh), seed, rescale = 1 / (1 - p)
+// key_mask: [batch, ceil(seq_len / 32)] uint32 key padding mask from lah_pack_key_mask, NULL for none.  A sequence without a
+// valid key gets out = 0 and lse2 = +inf.
 int lah_attention_fwd(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
-                      unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
-    return attention_fwd_entry(qkv, out, lse2, tokens, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, nullptr);
-}
-
-// lah_attention_fwd with a key padding mask: key_mask [batch, ceil(seq_len / 32)] uint32 from lah_pack_key_mask (NULL: no
-// mask).  A sequence without a valid key gets out = 0 and lse2 = +inf.
-int lah_attention_fwd_masked(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads,
-                             int d_model, unsigned long long seed, int drop_thr, float rescale, cudaStream_t st,
-                             const uint32_t* key_mask) {
-    return attention_fwd_entry(qkv, out, lse2, tokens, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+                      unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
+    if (hd == 32) return v2::launch_fwd<32>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    if (hd == 64) return v2::launch_fwd<64>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    return v2::launch_fwd<128>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
 }
 
 // pad: [batch, seq_len] bool (torch's src_key_padding_mask, true = ignored key) -> words [batch, ceil(seq_len / 32)] uint32

@@ -425,25 +425,6 @@ int launch_bwd(const void* qkv, const void* out, const void* dout, const float* 
     return -(int)cudaGetLastError();
 }
 
-static int attention_bwd_entry(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta,
-                               void* dqkv, void* dq_part, long long tokens, int seq_len, int num_heads, int d_model,
-                               unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
-    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
-    const int hd = d_model / num_heads;
-    if (hd != 32 && hd != 64 && hd != 128) return -2;
-    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
-    const long long batch = tokens / seq_len;
-    if (batch == 0) return 0;
-    if (hd == 32)
-        return launch_bwd<32>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                              drop_thr, rescale, st, key_mask);
-    if (hd == 64)
-        return launch_bwd<64>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                              drop_thr, rescale, st, key_mask);
-    return launch_bwd<128>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                           drop_thr, rescale, st, key_mask);
-}
-
 }  // namespace attnb
 }  // namespace lah
 
@@ -458,19 +439,24 @@ extern "C" {
 // Scratch: delta [T, H] fp32 (rowsum(dout o out), computed here), dq_part [ceil(seq_len / 128), T, D] bf16 (one partial
 // of dQ per key block, reduced into the Q third of dqkv here).  Three launches, no PyTorch ops around them.
 // drop_thr < 0: the forward ran without dropout; otherwise the same (seed, drop_thr, rescale) as lah_attention_fwd.
+// key_mask: the key padding mask of lah_attention_fwd (NULL: no mask).
 int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
                       void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
-                      int drop_thr, float rescale, cudaStream_t st) {
-    return attention_bwd_entry(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, seq_len, num_heads, d_model, seed, drop_thr,
-                               rescale, st, nullptr);
-}
-
-// lah_attention_bwd with the key padding mask of lah_attention_fwd_masked (NULL: no mask)
-int lah_attention_bwd_masked(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
-                             void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
-                             int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
-    return attention_bwd_entry(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, seq_len, num_heads, d_model, seed, drop_thr,
-                               rescale, st, key_mask);
+                      int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
+    if (hd == 32)
+        return launch_bwd<32>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
+                              drop_thr, rescale, st, key_mask);
+    if (hd == 64)
+        return launch_bwd<64>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
+                              drop_thr, rescale, st, key_mask);
+    return launch_bwd<128>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
+                           drop_thr, rescale, st, key_mask);
 }
 
 }  // extern "C"

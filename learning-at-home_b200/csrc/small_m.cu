@@ -652,7 +652,7 @@ const int* lah_get_poison_word() { return g_poison; }
 int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, int G, int M_out, int K, int a_mn,
                       void* out, long long ldo, const int* group_off, const int* group_rows, const float* bias,
                       const void* residual, long long ldr, const int* wait_flags, int wait_count, int wait_epoch,
-                      const int* epoch_base, int* status, int max_ctas, cudaStream_t st) {
+                      int* status, int max_ctas, cudaStream_t st) {
     if ((K % BK) || (M_out % BM) || (ldx % 8) || G > sab::MAX_G) return -2;
     CUtensorMap tmA, tmB[4];
     if (!a_mn) {
@@ -679,7 +679,7 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
     sab::Params p;
     p.G = G; p.M_out = M_out; p.K = K; p.group_off = group_off; p.group_rows = group_rows; p.out = (bf16*)out; p.ldo = ldo;
     p.bias = bias; p.residual = (const bf16*)residual; p.ldr = ldr; p.wait_flags = wait_flags; p.wait_count = wait_count;
-    p.wait_epoch = wait_epoch; p.epoch_base = epoch_base ? epoch_base : lah_get_epoch_base(); p.status = status;
+    p.wait_epoch = wait_epoch; p.epoch_base = lah_get_epoch_base(); p.status = status;
     p.tile_counter = tile_counter();
     if (!p.tile_counter) return -3;
     // upper bound of the tile count (the real one depends on the device-side row counts): every group has at least one
@@ -708,13 +708,17 @@ static int launch_wgrad_adam(const wa::Params& a, const CUtensorMap& tmDY, const
     return -(int)cudaGetLastError();
 }
 
-// the launch behind lah_wgrad_adam_wd and lah_wgrad_adam_dev: decoupled selects WD_DECOUPLED (with factor `decay`),
-// weight_decay != 0 WD_L2; lr_dev != nullptr the DEV_LR instantiation, which ignores lr and decay
-static int wgrad_adam_launch(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                             const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                             float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
-                             float weight_decay, float decay, bool decoupled, const float* lr_dev, int max_ctas,
-                             cudaStream_t st) {
+extern "C" {
+
+// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
+// weight_decay: the L2 coefficient (WD_L2); decay: the decoupled weight-decay factor 1 - lr * wd, read only when `decoupled`
+// is set, which selects WD_DECOUPLED.  At most one of the two forms per launch.  lr_dev == NULL: lr and decay by value;
+// otherwise lr_dev = {lr, 1 - lr * wd} in device memory (the factor computed on the host in double and rounded to fp32
+// once) and the DEV_LR instantiation, which ignores lr and decay, so a captured CUDA graph follows a schedule
+int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                   const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                   float* v, float* vmax, void* p_bf16, float lr, const float* lr_dev, float beta1, float beta2, float eps,
+                   int amsgrad, float weight_decay, float decay, int decoupled, int max_ctas, cudaStream_t st) {
     if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8) || 1ll * G * N > INT_MAX) return -2;
     if (decoupled && weight_decay != 0.f) return -2;
     if (amsgrad && !vmax) return -2;   // AMSGrad streams vmax through its own tensor map
@@ -763,38 +767,6 @@ static int wgrad_adam_launch(const void* dy, long long lddy, const void* x, long
     if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
     if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
     return launch_wgrad_adam<wa::WD_NONE, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
-}
-
-extern "C" {
-
-// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
-// weight_decay: the L2 coefficient; decay: the decoupled weight-decay factor 1 - lr * wd (1 = none); at most one of the two
-int lah_wgrad_adam_wd(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                      const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                      float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
-                      float weight_decay, float decay, int max_ctas, cudaStream_t st) {
-    return wgrad_adam_launch(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, m, v, vmax, p_bf16,
-                             lr, beta1, beta2, eps, amsgrad, weight_decay, decay, decay != 1.f, nullptr, max_ctas, st);
-}
-
-// lah_wgrad_adam_wd with the learning rate and the decoupled factor read from device memory: lr_dev = {lr, 1 - lr * wd}
-// (the factor computed on the host in double and rounded to fp32 once, only read when decoupled).  decoupled: the
-// configuration's form (AdamW with wd != 0), not inferred from the factor, which is exactly 1 at lr = 0
-int lah_wgrad_adam_dev(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                       const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                       float* v, float* vmax, void* p_bf16, const float* lr_dev, float beta1, float beta2, float eps,
-                       int amsgrad, float weight_decay, int decoupled, int max_ctas, cudaStream_t st) {
-    if (!lr_dev) return -2;
-    return wgrad_adam_launch(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, m, v, vmax, p_bf16,
-                             0.f, beta1, beta2, eps, amsgrad, weight_decay, 1.f, decoupled != 0, lr_dev, max_ctas, st);
-}
-
-int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                   const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                   float* v, float* vmax, void* p_bf16, float lr, float beta1, float beta2, float eps, int amsgrad,
-                   int max_ctas, cudaStream_t st) {
-    return lah_wgrad_adam_wd(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, m, v, vmax, p_bf16,
-                             lr, beta1, beta2, eps, amsgrad, 0.f, 1.f, max_ctas, st);
 }
 
 }  // extern "C"

@@ -38,10 +38,8 @@ def _lib():
         "lah_alive_from_heartbeats": [P, P, I, L, L, P],
         "lah_set_spin_timeout_ms": [I],
         "lah_step_begin": [I, L, P],
-        "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, P, I, P],
-        "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, I, P],
-        "lah_wgrad_adam_wd": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, Fl, I, Fl, Fl, I, P],
-        "lah_wgrad_adam_dev": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, P, Fl, Fl, Fl, I, Fl, I, I, P],
+        "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, I, P],
+        "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, P, Fl, Fl, Fl, I, Fl, Fl, I, I, P],
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
@@ -53,17 +51,12 @@ def _lib():
         "lah_signal_wait": [L, I, I, I, I, P, P],
         "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P],
         "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P],
-        "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, P],
-        "lah_adam_step_wd": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
-                             P],
-        "lah_adam_step_dev": [P, P, P, P, P, P, I, P, I, P, P, I, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, I,
-                              P],
+        "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
+                          I, P],
         "lah_bump_steps": [P, P, I, P],
         "lah_cast_bf16": [P, P, L, P],
-        "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
-        "lah_attention_bwd": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P],
-        "lah_attention_fwd_masked": [P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
-        "lah_attention_bwd_masked": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
+        "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
+        "lah_attention_bwd": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
         "lah_pack_key_mask": [P, P, L, I, P],
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
@@ -362,8 +355,8 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=5
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == tokens * num_heads
     _check_key_mask(key_mask, tokens, seq_len, qkv.device)
     seed, thr, rescale = _dropout_args(dropout)
-    native.check(_lib().lah_attention_fwd_masked(ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed,
-                                                 thr, rescale, stream_ptr(), ptr(key_mask)), "lah_attention_fwd_masked")
+    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed, thr,
+                                          rescale, stream_ptr(), ptr(key_mask)), "lah_attention_fwd")
     native.count_launch()
     return out
 
@@ -393,10 +386,10 @@ def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, 
     blocks = (seq_len + 127) // 128
     dq_part = torch.empty(blocks, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
     _check_key_mask(key_mask, tokens, seq_len, qkv.device)
-    native.check(_lib().lah_attention_bwd_masked(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
-                                                 tokens, int(seq_len), num_heads, d_model, *_dropout_args(dropout), stream_ptr(),
-                                                 ptr(key_mask)),
-                 "lah_attention_bwd_masked")
+    native.check(_lib().lah_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
+                                          tokens, int(seq_len), num_heads, d_model, *_dropout_args(dropout), stream_ptr(),
+                                          ptr(key_mask)),
+                 "lah_attention_bwd")
     native.count_launch(3)   # delta prologue, wgmma backward, dQ partial reduction
     return dqkv
 
@@ -626,26 +619,16 @@ def adam_step(p, g, m, v, vmax, p_bf16, seg_sizes, G, *, step=None, group_rows=N
     if isinstance(seg_sizes, int):
         seg_sizes = [seg_sizes]
     segs = (c_ll * len(seg_sizes))(*[int(s) for s in seg_sizes])
-    l2, decay = weight_decay_args(lr, weight_decay, decoupled)
     if lr_dev is not None:
         _check_lr_dev(lr_dev)
-        native.check(_lib().lah_adam_step_dev(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
-                                              ctypes.cast(segs, c_void_p), G, ptr(step), ptr(group_rows), int(step_scalar),
-                                              ptr(lr_dev), betas[0], betas[1], eps, l2, int(amsgrad), int(zero_mask), world,
-                                              peer_grad_off,
-                                              ctypes.cast(arr, c_void_p) if arr is not None else c_void_p(0), grad_scale,
-                                              int(G_active), ptr(shadow_of), int(shadow_g_off), int(me), int(seg_mask),
-                                              int(dead_mask), int(bool(decoupled and weight_decay)), stream_ptr()),
-                     "lah_adam_step_dev")
-        native.count_launch()
-        return
-    native.check(_lib().lah_adam_step_wd(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
-                                         ctypes.cast(segs, c_void_p), G, ptr(step),
-                                         ptr(group_rows), int(step_scalar), lr, betas[0], betas[1], eps, l2,
-                                         int(amsgrad), int(zero_mask), world, peer_grad_off,
-                                         ctypes.cast(arr, c_void_p) if arr is not None else c_void_p(0), grad_scale,
-                                         int(G_active), ptr(shadow_of), int(shadow_g_off), int(me), int(seg_mask),
-                                         int(dead_mask), decay, stream_ptr()), "lah_adam_step_wd")
+    l2, decay = weight_decay_args(lr, weight_decay, decoupled)
+    native.check(_lib().lah_adam_step(ptr(p), ptr(g), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), len(seg_sizes),
+                                      ctypes.cast(segs, c_void_p), G, ptr(step), ptr(group_rows), int(step_scalar), lr,
+                                      ptr(lr_dev), betas[0], betas[1], eps, l2, int(amsgrad), int(zero_mask), world,
+                                      peer_grad_off, ctypes.cast(arr, c_void_p) if arr is not None else c_void_p(0),
+                                      grad_scale, int(G_active), ptr(shadow_of), int(shadow_g_off), int(me), int(seg_mask),
+                                      int(dead_mask), decay, int(bool(decoupled and weight_decay)), stream_ptr()),
+                 "lah_adam_step")
     native.count_launch()
 
 
@@ -665,7 +648,7 @@ def swapab_linear(x, w, group_off, group_rows, *, out, bias=None, residual=None,
     native.check(_lib().lah_swapab_linear(ptr(x), x.stride(0), rows, ptr(w), G, M_out, K, int(w_is_kn), ptr(out),
                                           out.stride(0), ptr(group_off), ptr(group_rows), ptr(bias), ptr(residual),
                                           residual.stride(0) if residual is not None else 0, ptr(wait_flags), wait_count,
-                                          wait_epoch, c_void_p(0), ptr(wait_status), int(max_ctas), stream_ptr()),
+                                          wait_epoch, ptr(wait_status), int(max_ctas), stream_ptr()),
                  "lah_swapab_linear")
     native.count_launch()
     return out
@@ -701,20 +684,14 @@ def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, ski
     assert dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16 and p.dtype == torch.float32
     if amsgrad and vmax is None:
         raise ValueError("wgrad_adam: amsgrad needs a vmax tensor (vmax=None only with amsgrad=False)")
-    l2, decay = weight_decay_args(lr, weight_decay, decoupled)
     if lr_dev is not None:
         _check_lr_dev(lr_dev)
-        native.check(_lib().lah_wgrad_adam_dev(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd,
-                                               ptr(group_off), ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m),
-                                               ptr(v), ptr(vmax), ptr(p_bf16), ptr(lr_dev), betas[0], betas[1], eps,
-                                               int(amsgrad), l2, int(bool(decoupled and weight_decay)), int(max_ctas),
-                                               stream_ptr()), "lah_wgrad_adam_dev")
-        native.count_launch()
-        return
-    native.check(_lib().lah_wgrad_adam_wd(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd,
-                                          ptr(group_off), ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v),
-                                          ptr(vmax), ptr(p_bf16), lr, betas[0], betas[1], eps, int(amsgrad), l2, decay,
-                                          int(max_ctas), stream_ptr()), "lah_wgrad_adam_wd")
+    l2, decay = weight_decay_args(lr, weight_decay, decoupled)
+    native.check(_lib().lah_wgrad_adam(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd, ptr(group_off),
+                                       ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16),
+                                       lr, ptr(lr_dev), betas[0], betas[1], eps, int(amsgrad), l2, decay,
+                                       int(bool(decoupled and weight_decay)), int(max_ctas), stream_ptr()),
+                 "lah_wgrad_adam")
     native.count_launch()
 
 

@@ -152,18 +152,20 @@ def test_attention_bwd_hd128_is_deterministic(dropout):
 # ------------------------------------------------------------------------------------------------ GPU: refused head dims
 @pytest.mark.gpu
 @pytest.mark.parametrize("d,heads", REFUSED + [(1000, 16)])
-def test_attention_refuses_other_head_dims(d, heads):
+def test_attention_refuses_other_head_dims_masked_or_not(d, heads):
     from lah_b200.ops.native import c_void_p, stream_ptr
     S = 128
     qkv = torch.zeros(S, 3 * d, dtype=torch.bfloat16, device="cuda")
     out = torch.zeros(S, d, dtype=torch.bfloat16, device="cuda")
     lse = torch.zeros(S, heads, device="cuda")
+    mask = torch.full((1, S // 32), -1, dtype=torch.int32, device="cuda")   # every key valid
     lib = K._lib()
     P = c_void_p
-    assert lib.lah_attention_fwd(P(qkv.data_ptr()), P(out.data_ptr()), P(lse.data_ptr()), S, S, heads, d, 0, -1, 1.0,
-                                 stream_ptr()) == -2
-    assert lib.lah_attention_bwd(P(qkv.data_ptr()), P(out.data_ptr()), P(out.data_ptr()), P(lse.data_ptr()), P(0), P(0), P(0),
-                                 S, S, heads, d, 0, -1, 1.0, stream_ptr()) == -2
+    for key_mask in (P(0), P(mask.data_ptr())):
+        assert lib.lah_attention_fwd(P(qkv.data_ptr()), P(out.data_ptr()), P(lse.data_ptr()), S, S, heads, d, 0, -1, 1.0,
+                                     stream_ptr(), key_mask) == -2
+        assert lib.lah_attention_bwd(P(qkv.data_ptr()), P(out.data_ptr()), P(out.data_ptr()), P(lse.data_ptr()), P(0), P(0),
+                                     P(0), S, S, heads, d, 0, -1, 1.0, stream_ptr(), key_mask) == -2
     with pytest.raises(Exception):
         K.attention_fwd(qkv, heads, seq_len=S)
     with pytest.raises(Exception):

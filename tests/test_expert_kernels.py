@@ -300,21 +300,30 @@ def test_gemm_c_abi_refuses_misaligned_epilogue_operands():
 
 
 @host_abi_only
-def test_swapab_and_adam_c_abi_refusals():
+def test_swapab_linear_host_abi_refusals():
     lib = _lib()
     v = ctypes.c_void_p
     # 1024 groups: the prefix table of 128-token chunks holds at most MAX_G = 1023
     assert lib.lah_swapab_linear(v(0x200000), 64, 128, v(0x300000), 1024, 128, 64, 0, v(0x400000), 128, v(0x500000),
-                                 v(0x600000), v(0), v(0), 0, v(0), 0, 0, v(0), v(0), 0, v(0)) == -2
+                                 v(0x600000), v(0), v(0), 0, v(0), 0, 0, v(0), 0, v(0)) == -2
 
-    def adam(segs, seg_mask=0):
-        arr = (ctypes.c_longlong * len(segs))(*segs)
-        return lib.lah_adam_step(v(0x100000), v(0x200000), v(0x300000), v(0x400000), v(0x500000), v(0), len(segs),
-                                 ctypes.cast(arr, v), 2, v(0), v(0), 1, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1, 0, 1, -1, v(0),
-                                 1.0, 0, v(0), -1, 0, seg_mask, 0, v(0))
-    assert adam([4] * 13) == -2                          # 13 segments
-    assert adam([4, 6, 8]) == -2                         # a segment size that is not a multiple of 4
-    assert adam([]) == -2                                # no segment at all
+
+@host_abi_only
+def test_adam_step_host_abi_refusals():
+    lib = _lib()
+    v = ctypes.c_void_p
+    # every case by value (lr_dev NULL) and with a device rate block (a fake address)
+    for lr_dev in (0, 0x600000):
+        def adam(segs=(4, 8), l2=0.0, decay=1.0, decoupled=0):
+            arr = (ctypes.c_longlong * len(segs))(*segs)
+            return lib.lah_adam_step(v(0x100000), v(0x200000), v(0x300000), v(0x400000), v(0x500000), v(0), len(segs),
+                                     ctypes.cast(arr, v), 2, v(0), v(0), 1, 1e-3, v(lr_dev), 0.9, 0.999, 1e-8, l2, 1, 0, 1,
+                                     -1, v(0), 1.0, 0, v(0), -1, 0, 0, 0, decay, decoupled, v(0))
+        # the controls: these arguments pass the host checks, with either decay form
+        assert adam() != -2 and adam(l2=0.1) != -2 and adam(decay=0.99, decoupled=1) != -2, lr_dev
+        for segs in ((4,) * 13, (4, 6, 8), ()):           # 13 segments, a size not a multiple of 4, no segment at all
+            assert adam(segs) == -2 and adam(segs, l2=0.1) == -2 and adam(segs, decay=0.99, decoupled=1) == -2, segs
+        assert adam(l2=0.1, decay=0.99, decoupled=1) == -2, lr_dev     # L2 and decoupled decay at once
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU

@@ -88,21 +88,24 @@ def test_wgrad_adam_oracle_matches_linear_autograd_and_torch_adam(amsgrad):
 
 
 @host_abi_only
-def test_wgrad_adam_c_abi_refusals():
+def test_wgrad_adam_host_abi_refusals():
     lib = _lib()
     v = ctypes.c_void_p
 
-    def wa(N=256, K_=384, lddy=256, ldx=384, G=4):
-        return lib.lah_wgrad_adam(v(0x200000), lddy, v(0x300000), ldx, 1024, G, N, K_, v(0x400000), v(0x400100), v(0),
-                                  v(0x400200), v(0x500000), v(0x600000), v(0x700000), v(0x800000), v(0x900000), 1e-3,
-                                  0.9, 0.999, 1e-8, 1, 0, v(0))
-    assert wa() != -2                                   # the control: these arguments pass the host checks
-    assert wa(N=192) == -2 and wa(K_=320) == -2         # N, K not multiples of the 128 x 128 tile
-    assert wa(lddy=260) == -2 and wa(ldx=388) == -2     # row strides off the 16-byte TMA granule
-    assert wa(G=1 << 20, N=4096) == -2                  # G * N rows of the state maps overflow an int
-    assert lib.lah_wgrad_adam(v(0x200000), 256, v(0x300000), 384, 1024, 4, 256, 384, v(0x400000), v(0x400100), v(0),
-                              v(0x400200), v(0x500000), v(0x600000), v(0x700000), v(0), v(0x900000), 1e-3, 0.9, 0.999,
-                              1e-8, 1, 0, v(0)) == -2   # amsgrad without vmax
+    # every case by value (lr_dev NULL) and with a device rate block (a fake address)
+    for lr_dev in (0, 0xa00000):
+        def wa(N=256, K_=384, lddy=256, ldx=384, G=4, vmax=0x800000, l2=0.0, decay=1.0, decoupled=0):
+            return lib.lah_wgrad_adam(v(0x200000), lddy, v(0x300000), ldx, 1024, G, N, K_, v(0x400000), v(0x400100), v(0),
+                                      v(0x400200), v(0x500000), v(0x600000), v(0x700000), v(vmax), v(0x900000), 1e-3,
+                                      v(lr_dev), 0.9, 0.999, 1e-8, 1, l2, decay, decoupled, 0, v(0))
+        # the controls: these arguments pass the host checks, with either decay form
+        assert wa() != -2 and wa(l2=0.1) != -2 and wa(decay=0.99, decoupled=1) != -2, lr_dev
+        for kw in (dict(N=192), dict(K_=320),             # N, K not multiples of the 128 x 128 tile
+                   dict(lddy=260), dict(ldx=388),         # row strides off the 16-byte TMA granule
+                   dict(G=1 << 20, N=4096),               # G * N rows of the state maps overflow an int
+                   dict(vmax=0)):                         # amsgrad without vmax
+            assert wa(**kw) == -2 and wa(l2=0.1, **kw) == -2 and wa(decay=0.99, decoupled=1, **kw) == -2, (lr_dev, kw)
+        assert wa(l2=0.1, decay=0.99, decoupled=1) == -2, lr_dev        # L2 and decoupled decay at once
 
 
 @host_abi_only

@@ -7,13 +7,12 @@ The kernels are compared with their by-value launches bit for bit (``lr_dev`` ho
 compared with itself: graph == eager under a rate that changes every step, a rate change == a restart from a checkpoint
 at the new rate, lr = 0 freezes every parameter while the moments move, and a resumed run == the continued one.
 """
-import ctypes
 import math
 
 import pytest
 import torch
 
-from test_expert_kernels import _lib, adam_state, host_abi_only, poison  # noqa: F401
+from test_expert_kernels import adam_state, poison  # noqa: F401
 from test_fused_adam_fp8_kernels import WA_ADAM_ROWS, WA_ADAM_STEPS, wa_adam_setup
 
 import lah_b200  # noqa: F401
@@ -152,29 +151,6 @@ def test_checkpoint_carries_the_rate():
     assert not torch.equal(snapshot(fresh)["layer0.p"], snapshot(old)["layer0.p"])
 
 
-@host_abi_only
-def test_device_rate_entry_points_refuse_what_the_by_value_ones_refuse():
-    """no block, L2 and decoupled decay at once, and the shape refusals of the by-value entry points (fake addresses: only
-    the host checks before the launch run)"""
-    lib = _lib()
-    v = ctypes.c_void_p
-
-    def adam(segs=(4, 8), lr_dev=0x600000, l2=0.0, decoupled=0):
-        arr = (ctypes.c_longlong * len(segs))(*segs)
-        return lib.lah_adam_step_dev(v(0x100000), v(0x200000), v(0x300000), v(0x400000), v(0x500000), v(0), len(segs),
-                                     ctypes.cast(arr, v), 2, v(0), v(0), 1, v(lr_dev), 0.9, 0.999, 1e-8, l2, 1, 0, 1, -1,
-                                     v(0), 1.0, 0, v(0), -1, 0, 0, 0, decoupled, v(0))
-    assert adam(lr_dev=0) == -2 and adam(l2=0.1, decoupled=1) == -2
-    assert adam(segs=(4, 6)) == -2 and adam(segs=(4,) * 13) == -2
-
-    def wa(lr_dev=0x600000, N=256, l2=0.0, decoupled=0, vmax=0x800000):
-        return lib.lah_wgrad_adam_dev(v(0x200000), 256, v(0x300000), 384, 1024, 4, N, 384, v(0x400000), v(0x400100), v(0),
-                                      v(0x400200), v(0x500000), v(0x600000), v(0x700000), v(vmax), v(0x900000), v(lr_dev),
-                                      0.9, 0.999, 1e-8, 1, l2, decoupled, 0, v(0))
-    assert wa() != -2                                             # the control: these arguments pass the host checks
-    assert wa(lr_dev=0) == -2 and wa(l2=0.1, decoupled=1) == -2 and wa(N=192) == -2 and wa(vmax=0) == -2
-
-
 # ---------------------------------------------------------------------------------------------------------------- GPU
 WD_MODES = {"none": dict(weight_decay=0.0, decoupled=False), "l2": dict(weight_decay=0.1, decoupled=False),
             "decoupled": dict(weight_decay=0.3, decoupled=True)}
@@ -215,23 +191,24 @@ def test_adam_step_device_rate_equals_by_value(mode, amsgrad, seg_mask, lr, pois
 @pytest.mark.parametrize("amsgrad", [True, False])
 @pytest.mark.parametrize("mode", list(WD_MODES))
 def test_wgrad_adam_device_rate_equals_by_value(mode, amsgrad, max_ctas, poison):
-    """groups of 0 rows (and a skipped group) included: WA_ADAM_ROWS"""
+    """groups of 0 rows (and a skipped group) included: WA_ADAM_ROWS; lr = 0 as well (AdamW's factor is then exactly 1)"""
     assert 0 in WA_ADAM_ROWS
-    N, K_, lr = 256, 384, 2.3e-3
+    N, K_ = 256, 384
     dy, x, go, gr, skip, _, _, st, _ = wa_adam_setup(31, N, K_)
     step = torch.tensor(WA_ADAM_STEPS, dtype=torch.int32, device="cuda")
     wd = WD_MODES[mode]
-    out = []
-    for dev in (False, True):
-        t = {k: (v.clone() if v is not None else None) for k, v in st.items()}
-        kw = dict(lr_dev=lr_block(lr, **wd), lr=0.5) if dev else dict(lr=lr)
-        K.wgrad_adam(dy, x, go, gr, p=t["p"], m=t["m"], v=t["v"], vmax=t["vmax"], p_bf16=t["p_bf16"], step=step, skip=skip,
-                     amsgrad=amsgrad, max_ctas=max_ctas, **wd, **kw)
-        out.append(t)
-    torch.cuda.synchronize()
-    for n in ("p", "m", "v", "vmax", "p_bf16"):
-        assert torch.equal(out[0][n], out[1][n]), n
-    assert not torch.equal(out[1]["m"], st["m"])
+    for lr in (2.3e-3, 0.0):
+        out = []
+        for dev in (False, True):
+            t = {k: (v.clone() if v is not None else None) for k, v in st.items()}
+            kw = dict(lr_dev=lr_block(lr, **wd), lr=0.5) if dev else dict(lr=lr)
+            K.wgrad_adam(dy, x, go, gr, p=t["p"], m=t["m"], v=t["v"], vmax=t["vmax"], p_bf16=t["p_bf16"], step=step,
+                         skip=skip, amsgrad=amsgrad, max_ctas=max_ctas, **wd, **kw)
+            out.append(t)
+        torch.cuda.synchronize()
+        for n in ("p", "m", "v", "vmax", "p_bf16"):
+            assert torch.equal(out[0][n], out[1][n]), (lr, n)
+        assert not torch.equal(out[1]["m"], st["m"]), lr
 
 
 def gpu_cfg(path, **kw):

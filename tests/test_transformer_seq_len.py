@@ -131,18 +131,20 @@ def test_attention_bwd_any_seq_len(S, batch, d, heads):
 
 
 @pytest.mark.gpu
-def test_attention_rejects_bad_seq_len():
+def test_attention_rejects_bad_seq_len_masked_or_not():
     qkv = torch.zeros(300, 3 * 256, dtype=torch.bfloat16, device="cuda")
     for S in (0, 7, K.MAX_SEQ + 1):
         with pytest.raises(Exception):
             K.attention_fwd(qkv, 4, seq_len=S)
     from lah_b200.ops.native import c_void_p, stream_ptr
     lib = K._lib()
-    for tokens, S in ((300, 7), (K.MAX_SEQ + 1, K.MAX_SEQ + 1), (300, 0)):
-        assert lib.lah_attention_fwd(c_void_p(qkv.data_ptr()), c_void_p(0), c_void_p(0), tokens, S, 4, 256, 0, -1, 1.0,
-                                     stream_ptr()) == -2
-        assert lib.lah_attention_bwd(c_void_p(qkv.data_ptr()), c_void_p(0), c_void_p(0), c_void_p(0), c_void_p(0), c_void_p(0),
-                                     c_void_p(0), tokens, S, 4, 256, 0, -1, 1.0, stream_ptr()) == -2
+    mask = torch.full((1, 1), -1, dtype=torch.int32, device="cuda")   # never read: the host checks refuse first
+    for key_mask in (c_void_p(0), c_void_p(mask.data_ptr())):
+        for tokens, S in ((300, 7), (K.MAX_SEQ + 1, K.MAX_SEQ + 1), (300, 0)):
+            assert lib.lah_attention_fwd(c_void_p(qkv.data_ptr()), c_void_p(0), c_void_p(0), tokens, S, 4, 256, 0, -1, 1.0,
+                                         stream_ptr(), key_mask) == -2
+            assert lib.lah_attention_bwd(c_void_p(qkv.data_ptr()), c_void_p(0), c_void_p(0), c_void_p(0), c_void_p(0),
+                                         c_void_p(0), c_void_p(0), tokens, S, 4, 256, 0, -1, 1.0, stream_ptr(), key_mask) == -2
 
 
 @pytest.mark.gpu

@@ -11,14 +11,13 @@ training tests on random gradients.  The in-box engine's CPU path is compared wi
 GPU trainer with that CPU path.
 """
 import copy
-import ctypes
 
 import pytest
 import torch
 from torch import nn
 
-from test_expert_kernels import (BF16, SENTINEL, U, _lib, adam_ref64, adam_state, f32, host_abi_only, poison,  # noqa: F401
-                                 sentinel_like, untouched, within)
+from test_expert_kernels import (BF16, SENTINEL, U, adam_ref64, adam_state, f32, poison, sentinel_like,  # noqa: F401
+                                 untouched, within)
 from test_fused_adam_fp8_kernels import WA_ADAM_ROWS, WA_ADAM_STEPS, same_bytes, wa_adam_setup
 
 import lah_b200
@@ -182,31 +181,6 @@ def test_engine_cpu_path_weight_decay_matches_torch_per_expert(decoupled):
     assert moved
     group = fused.shard.expert_optimizer_state(0)["param_groups"][0]
     assert group["weight_decay"] == 0.5 and group["decoupled_weight_decay"] == decoupled
-
-
-@host_abi_only
-def test_weight_decay_c_abi_refusals():
-    """the new entry points refuse what the old ones refuse, and both decay forms at once"""
-    lib = _lib()
-    v = ctypes.c_void_p
-
-    def adam(segs, l2=0.0, decay=1.0):
-        arr = (ctypes.c_longlong * len(segs))(*segs)
-        return lib.lah_adam_step_wd(v(0x100000), v(0x200000), v(0x300000), v(0x400000), v(0x500000), v(0), len(segs),
-                                    ctypes.cast(arr, v), 2, v(0), v(0), 1, 1e-3, 0.9, 0.999, 1e-8, l2, 1, 0, 1, -1, v(0),
-                                    1.0, 0, v(0), -1, 0, 0, 0, decay, v(0))
-    assert adam([4] * 13) == -2 and adam([4, 6, 8]) == -2 and adam([]) == -2
-    assert adam([4] * 13, decay=0.99) == -2 and adam([4, 6, 8], l2=0.1) == -2
-    assert adam([4, 8], l2=0.1, decay=0.99) == -2                 # L2 and decoupled at once
-
-    def wa(N=256, K_=384, lddy=256, ldx=384, G=4, vmax=0x800000, l2=0.0, decay=1.0):
-        return lib.lah_wgrad_adam_wd(v(0x200000), lddy, v(0x300000), ldx, 1024, G, N, K_, v(0x400000), v(0x400100), v(0),
-                                     v(0x400200), v(0x500000), v(0x600000), v(0x700000), v(vmax), v(0x900000), 1e-3,
-                                     0.9, 0.999, 1e-8, 1, l2, decay, 0, v(0))
-    assert wa() != -2                                             # the control: these arguments pass the host checks
-    for kw in (dict(N=192), dict(K_=320), dict(lddy=260), dict(ldx=388), dict(G=1 << 20, N=4096), dict(vmax=0)):
-        assert wa(**kw) == -2 and wa(decay=0.99, **kw) == -2 and wa(l2=0.1, **kw) == -2, kw
-    assert wa(l2=0.1, decay=0.99) == -2
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU
