@@ -29,6 +29,13 @@
 // consumers walk the same list of key blocks that hold a valid key: a block without one is neither loaded nor computed.  In
 // a partially valid block the scores of masked keys are set to -inf, as in the tail.  The mask is per key, so after the
 // first block every row maximum is finite.  A sequence without a valid key processes no block: out = 0, lse2 = +inf.
+//
+// Causal attention (CAUSAL instantiations, never with MASK): query q attends to keys <= q.  Query tile i walks key blocks
+// 0 .. i only (Q_TILE = KB, so block i is the diagonal one); producer and consumers both stop after it.  In the diagonal
+// block the scores of keys > query are set to -inf before the row maximum (one uniform branch, as for the tail): that also
+// covers keys >= S, which only the diagonal block of the last tile holds.  Every row keeps its own key, so l > 0.  CTAs are
+// launched heaviest first within groups of CAUSAL_GROUP (batch, head) pairs: each group counts its query tiles down from
+// the last one, so short tiles end each group and the grid, and the group's K / V stay in L2.
 #include "sm90.cuh"
 #include "dropout.cuh"
 #include <stdlib.h>
@@ -43,6 +50,10 @@ namespace v2 {
 constexpr int KB = 128;                       // keys per block
 constexpr int NUM_THREADS2 = 256;             // two consumer warpgroups; thread 0 also drives TMA
 constexpr int NUM_BARS = 1 + 2;
+// causal launch order: heaviest query tiles first within groups of this many (batch, head) pairs, whose K / V (1 MB per pair
+// at S = 2048, HD = 128) stay in L2 while the group's tiles run; one order over all pairs would stream every pair's K / V
+// from HBM once per query tile
+constexpr int CAUSAL_GROUP = 8;
 
 // shared-memory layout of one head dim: a 128 x HD bf16 tile (Q tile, K block, V block) is HD / ATOM_COLS atoms of
 // [128 rows][ATOM_COLS columns], each loaded by one TMA box
@@ -64,8 +75,9 @@ struct Fwd {
 // DROP: attention dropout (dropout.cuh, site 0).  The kept bf16 probabilities feed O += P V; the row sum l (and so the LSE)
 // keeps summing ALL of them, and 1 / (1 - p) is folded into the final 1 / l.
 // MASK without DROP at HD <= 64 is held to 128 registers, as the unmasked kernel is: two CTAs per SM (129 would allow one)
-template <int HD, bool DROP, bool MASK>
-__global__ void __launch_bounds__(NUM_THREADS2, MASK && !DROP && HD <= 64 ? 2 : 1)
+// CAUSAL without DROP at HD <= 64 is held to 128 registers for the same reason
+template <int HD, bool DROP, bool MASK, bool CAUSAL>
+__global__ void __launch_bounds__(NUM_THREADS2, (MASK || CAUSAL) && !DROP && HD <= 64 ? 2 : 1)
 attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __restrict__ out, float* __restrict__ lse2,
                         int d_model, int num_heads, int seq_len, float scale_log2e, unsigned long long seed, uint32_t thr,
                         float rescale, const uint32_t* __restrict__ key_mask) {
@@ -79,10 +91,19 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     uint64_t* kv_full = bars + 1;   // [2]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+    static_assert(!(MASK && CAUSAL), "causal attention takes no key padding mask");
     const int num_kb = (seq_len + KB - 1) / KB;   // key blocks = query tiles per sequence
-    const int qt = blockIdx.x % num_kb;
-    const int head = (blockIdx.x / num_kb) % num_heads;
-    const int batch = (blockIdx.x / num_kb) / num_heads;
+    // CAUSAL: groups of CAUSAL_GROUP (batch, head) pairs, each group's last query tiles first; g0 = the group's first pair,
+    // gs its size
+    const int nbh = CAUSAL ? gridDim.x / num_kb : 0;
+    const int g0 = CAUSAL ? blockIdx.x / (CAUSAL_GROUP * num_kb) * CAUSAL_GROUP : 0;
+    const int gs = CAUSAL ? min(CAUSAL_GROUP, nbh - g0) : 1;
+    const int r = CAUSAL ? blockIdx.x - g0 * num_kb : 0;
+    const int qt = CAUSAL ? num_kb - 1 - r / gs : blockIdx.x % num_kb;
+    const unsigned bh = CAUSAL ? g0 + r % gs : blockIdx.x / num_kb;
+    const int head = bh % num_heads;
+    const int batch = bh / num_heads;
+    const int end_kb = CAUSAL ? qt + 1 : num_kb;   // key blocks 0 .. end_kb - 1 (CAUSAL: up to the diagonal block qt)
 
     // one 128-row tile of HD columns starting at column c0: one TMA box per atom
     auto load_tile = [&](uint8_t* dst, uint64_t* bar, int c0, int row) {
@@ -121,7 +142,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         load_tile(smem + OFF_Q2, bar_q, head * HD, qt * Q_TILE);
         if constexpr (!MASK) {
             load_kv(0, 0);
-            if (num_kb > 1) load_kv(1, 1);
+            if (end_kb > 1) load_kv(1, 1);
         }
     }
     // j: the key block being processed, n: how many blocks were processed before it (its stage and phase); without MASK
@@ -145,7 +166,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
     mbar_wait(bar_q, 0);
 #pragma unroll 1
-    for (int n = 0; j < num_kb; ++n) {
+    for (int n = 0; j < end_kb; ++n) {
         const int st = (MASK ? n : j) & 1;
         // MASK: bit 2 jj + i of kbits = key 8 jj + 2 (lane & 3) + i of block j is valid, i.e. bits 2c, 2c + 1 of every byte of
         // the block's words, c = lane & 3; j2 = the block after j1, looked up before the MMAs so that its loads overlap them
@@ -199,6 +220,18 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
                     for (int i = 0; i < 2; ++i)
                         if (!((kbits >> (2 * jj + i)) & 1u)) s[4 * jj + i] = s[4 * jj + 2 + i] = -INFINITY;
             }
+        } else if constexpr (CAUSAL) {
+            if (j == qt) {   // diagonal block: s[4 jj + 2 h + i] is key 8 jj + 2 (lane & 3) + i of row r + 8 h, masked iff
+                             // key > row, i.e. 8 (jj - h) + i > t = r - 2 (lane & 3)
+                const int t = wg * 64 + (warp & 3) * 16 + (lane >> 2) - 2 * (lane & 3);
+#pragma unroll
+                for (int jj = 0; jj < KB / 8; ++jj)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        if (8 * jj + i > t) s[4 * jj + i] = -INFINITY;
+                        if (8 * jj - 8 + i > t) s[4 * jj + 2 + i] = -INFINITY;
+                    }
+            }
         } else if (j * KB + KB > seq_len) {   // last block of a partial sequence: s[4 jj + 2 h + i] is key 8 jj + 2 (lane & 3) + i
 #pragma unroll
             for (int jj = 0; jj < KB / 8; ++jj)
@@ -249,7 +282,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
         wgmma_wait<0>();
         wgmma_fence_regs(o);
         if constexpr (!MASK) j2 = j + 2;
-        if (j2 < num_kb) {
+        if (j2 < end_kb) {
             named_bar_sync(1, NUM_THREADS2);   // both warpgroups are done with stage st
             if (tid == 0) load_kv((MASK ? n : j2) & 1, j2);
         }
@@ -275,7 +308,7 @@ attention_fwd_v2_kernel(const __grid_constant__ CUtensorMap tm_qkv, bf16* __rest
     }
 }
 
-template <int HD>
+template <int HD, bool CAUSAL>
 int launch_fwd(const void* qkv, void* out, float* lse2, long long batch, int seq_len, int num_heads, int d_model,
                unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
     using C = Fwd<HD>;
@@ -288,19 +321,41 @@ int launch_fwd(const void* qkv, void* out, float* lse2, long long batch, int seq
                           C::ATOM_COLS == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B);
         if (r) return r;
     }
-    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, false>>(C::SMEM_TOTAL2)) return e;
-    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, false>>(C::SMEM_TOTAL2)) return e;
-    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, true>>(C::SMEM_TOTAL2)) return e;
-    if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, true>>(C::SMEM_TOTAL2)) return e;
+    decltype(&attention_fwd_v2_kernel<HD, false, false, CAUSAL>) kern;
+    if constexpr (CAUSAL) {
+        if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, false, true>>(C::SMEM_TOTAL2)) return e;
+        if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, false, true>>(C::SMEM_TOTAL2)) return e;
+        kern = drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, false, true> : attention_fwd_v2_kernel<HD, true, false, true>;
+    } else {
+        if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, false, false>>(C::SMEM_TOTAL2)) return e;
+        if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, false, false>>(C::SMEM_TOTAL2)) return e;
+        if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, false, true, false>>(C::SMEM_TOTAL2)) return e;
+        if (int e = set_max_dynamic_smem<attention_fwd_v2_kernel<HD, true, true, false>>(C::SMEM_TOTAL2)) return e;
+        kern = key_mask ? (drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, true, false> : attention_fwd_v2_kernel<HD, true, true, false>)
+                        : (drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, false, false> : attention_fwd_v2_kernel<HD, true, false, false>);
+    }
     const float scale_log2e = 1.4426950408889634f / sqrtf((float)HD);
     const long long ctas = batch * num_heads * ((seq_len + Q_TILE - 1) / Q_TILE);
     if (ctas > 0x7fffffffll) return -2;
-    auto kern = key_mask ? (drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, true> : attention_fwd_v2_kernel<HD, true, true>)
-                         : (drop_thr < 0 ? attention_fwd_v2_kernel<HD, false, false> : attention_fwd_v2_kernel<HD, true, false>);
     kern<<<(unsigned)ctas, NUM_THREADS2, C::SMEM_TOTAL2, st>>>(
         tm, (bf16*)out, lse2, d_model, num_heads, seq_len, scale_log2e, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr),
         rescale, key_mask);
     return -(int)cudaGetLastError();
+}
+
+// shape checks and head-dim dispatch of both entry points
+template <bool CAUSAL>
+int attention_fwd(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
+                  unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
+    if (hd == 32) return launch_fwd<32, CAUSAL>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    if (hd == 64) return launch_fwd<64, CAUSAL>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    return launch_fwd<128, CAUSAL>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
 }
 
 }  // namespace v2
@@ -335,15 +390,14 @@ extern "C" {
 // valid key gets out = 0 and lse2 = +inf.
 int lah_attention_fwd(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
                       unsigned long long seed, int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
-    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
-    const int hd = d_model / num_heads;
-    if (hd != 32 && hd != 64 && hd != 128) return -2;
-    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
-    const long long batch = tokens / seq_len;
-    if (batch == 0) return 0;
-    if (hd == 32) return v2::launch_fwd<32>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
-    if (hd == 64) return v2::launch_fwd<64>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
-    return v2::launch_fwd<128>(qkv, out, lse2, batch, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+    return v2::attention_fwd<false>(qkv, out, lse2, tokens, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, key_mask);
+}
+
+// causal self-attention (query q attends to keys <= q): the arguments and return codes of lah_attention_fwd without a key
+// padding mask
+int lah_attention_fwd_causal(const void* qkv, void* out, float* lse2, long long tokens, int seq_len, int num_heads, int d_model,
+                             unsigned long long seed, int drop_thr, float rescale, cudaStream_t st) {
+    return v2::attention_fwd<true>(qkv, out, lse2, tokens, seq_len, num_heads, d_model, seed, drop_thr, rescale, st, nullptr);
 }
 
 // pad: [batch, seq_len] bool (torch's src_key_padding_mask, true = ignored key) -> words [batch, ceil(seq_len / 32)] uint32

@@ -42,6 +42,14 @@
 // valid key does no MMA and loads nothing; it writes exact zeros to its dK / dV rows and a zero dQ partial (slice j), so
 // attn_dq_reduce_kernel stays mask-blind.  In a partially valid block S^T of masked keys is set to -inf, as for keys >= S,
 // so P^T and dS^T are exactly 0 and so are those dK / dV rows.  A sequence without a valid key has LSE = +inf.
+//
+// Causal attention (CAUSAL instantiations, never with MASK): key block j walks only the query blocks that hold a query
+// >= 128 j, i.e. i >= 128 j / QB (at HD = 128 both 64-query halves of the diagonal, of which the first straddles it).  In
+// a query block that starts inside the key block, S^T of keys > query is set to -inf, so P^T and dS^T are exactly 0 there;
+// that also covers keys >= S for every valid query.  dQ partial j then holds only queries >= 128 j:
+// attn_dq_reduce_kernel<true> sums, for query q, the partials j <= q / 128 in the same order, and the rows of partial j
+// below 128 j are neither written nor read.  CTAs are launched heaviest first: blockIdx.x / (batch * heads) is j, and key
+// block 0 walks every query block.
 #include "sm90.cuh"
 #include "dropout.cuh"
 
@@ -75,7 +83,7 @@ struct Bwd {
     static constexpr int SMEM_TOTAL = OFF_BAR + NUM_BARS * 8 + 16 + 1024;
 };
 
-template <int HD, bool DROP, bool MASK>
+template <int HD, bool DROP, bool MASK, bool CAUSAL>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                      const float* __restrict__ lse2, const float* __restrict__ delta, bf16* __restrict__ dqkv,
@@ -97,9 +105,13 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
     const int num_kb = (seq_len + BLK - 1) / BLK;   // key blocks per sequence
     const int num_qb = (seq_len + QB - 1) / QB;     // query blocks per sequence
-    const int j = blockIdx.x % num_kb;
-    const int head = (blockIdx.x / num_kb) % num_heads;
-    const int batch = (blockIdx.x / num_kb) / num_heads;
+    static_assert(!(MASK && CAUSAL), "causal attention takes no key padding mask");
+    const int nbh = CAUSAL ? gridDim.x / num_kb : 0;   // CAUSAL: (batch, head) pairs; key block 0 comes first
+    const int j = CAUSAL ? static_cast<int>(blockIdx.x / nbh) : blockIdx.x % num_kb;
+    const unsigned bh = CAUSAL ? blockIdx.x % nbh : blockIdx.x / num_kb;
+    const int head = bh % num_heads;
+    const int batch = bh / num_heads;
+    const int i0 = CAUSAL ? j * (BLK / QB) : 0;     // first query block; CAUSAL: the first holding a query >= 128 j
     const long long seq0 = static_cast<long long>(batch) * seq_len;
     const int key_row = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // row of the block (+ 8 for h = 1)
     uint32_t kvalid = 3u;   // MASK: bit h set iff key key_row + 8 h of this block is valid
@@ -128,8 +140,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
         kvalid = static_cast<uint32_t>(mine & 1u) | static_cast<uint32_t>((mine >> 8) & 1u) << 1;
     }
 
-    auto load_q = [&](int i) {   // thread 0 only; stage i & 1 must be free
-        const int st = i & 1;
+    auto load_q = [&](int i) {   // thread 0 only; stage (i - i0) & 1 must be free
+        const int st = (i - i0) & 1;
         mbar_arrive_expect_tx(&q_full[st], 2 * C::Q_TILE);
         tma_load_3d(smem + OFF_Q + st * C::Q_TILE, &tm_qkv, &q_full[st], head * HD, i * QB, batch);
         tma_load_3d(smem + OFF_DO + st * C::Q_TILE, &tm_do, &q_full[st], head * HD, i * QB, batch);
@@ -160,8 +172,8 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
                     tma_load_3d(smem + OFF_V + off, &tm_qkv, kv_full, 2 * d_model + head * HD + a * 64, j * BLK + r * QB, batch);
                 }
         }
-        load_q(0);
-        if (num_qb > 1) load_q(1);
+        load_q(i0);
+        if (i0 + 1 < num_qb) load_q(i0 + 1);
     }
     if constexpr (QB != BLK) {
         // key rows [QB, 128) all >= S: zeros, as TMA would have filled them (garbage there could be inf / NaN in dP^T)
@@ -183,14 +195,14 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
     for (int e = 0; e < HD / 2; ++e) dv[e] = dk[e] = 0.f;
     mbar_wait(kv_full, 0);
 #pragma unroll 1
-    for (int i = 0; i < num_qb; ++i) {
-        const int st = i & 1;
+    for (int i = i0; i < num_qb; ++i) {
+        const int st = (i - i0) & 1;
         const long long tok0 = seq0 + i * QB;
         const int qr = tid & (QB - 1);   // query row of the block whose LSE (tid < QB) or Delta this thread loads
         const bool qvalid = i * QB + qr < seq_len;
         if (tid < QB) s_lse[qr] = qvalid ? __ldg(lse2 + (tok0 + qr) * num_heads + head) : INFINITY;
         else if (QB == BLK || tid < 2 * QB) s_delta[qr] = qvalid ? __ldg(delta + (tok0 + qr) * num_heads + head) : 0.f;
-        mbar_wait(&q_full[st], (i >> 1) & 1);
+        mbar_wait(&q_full[st], ((i - i0) >> 1) & 1);
         const uint32_t sq = smem_u32(smem + OFF_Q + st * C::Q_TILE), sdo = smem_u32(smem + OFF_DO + st * C::Q_TILE);
         float sacc[QB / 2], dpacc[QB / 2];
         wgmma_fence();
@@ -217,6 +229,18 @@ attention_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_co
                 if (!((kvalid >> h) & 1u))
 #pragma unroll
                     for (int jj = 0; jj < QB / 8; ++jj) sacc[4 * jj + 2 * h] = sacc[4 * jj + 2 * h + 1] = -INFINITY;
+        } else if constexpr (CAUSAL) {
+            if (i * QB < j * BLK + BLK) {   // the block meets the diagonal: sacc[4 jj + 2 h + par] is key j BLK + key_row + 8 h,
+                                           // query i QB + 8 jj + qcol + par; masked iff 8 jj + par < t + 8 h
+                const int t = j * BLK + key_row - i * QB - qcol;
+#pragma unroll
+                for (int jj = 0; jj < QB / 8; ++jj)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int par = 0; par < 2; ++par)
+                            if (8 * jj + par < t + 8 * h) sacc[4 * jj + 2 * h + par] = -INFINITY;
+            }
         } else if (j * BLK + BLK > seq_len) {   // last key block of a partial sequence: sacc[4 jj + 2 h + par] is key key_row + 8 h
 #pragma unroll
             for (int h = 0; h < 2; ++h)
@@ -362,12 +386,15 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const bf16* __restrict_
     if (lane == 0) delta[w] = acc;
 }
 
-// epilogue: dQ = sum of the per-key-block partials in key-block order (deterministic), written as bf16 into the Q third of dqkv
+// epilogue: dQ = sum of the per-key-block partials in key-block order (deterministic), written as bf16 into the Q third of dqkv.
+// CAUSAL: query q of its sequence sums partials 0 .. q / BLK only (the key blocks that hold a key <= q)
+template <bool CAUSAL>
 __global__ void __launch_bounds__(256) attn_dq_reduce_kernel(const bf16* __restrict__ dq_part, bf16* __restrict__ dqkv,
-                                                             long long tokens, int d_model, int parts) {
+                                                             long long tokens, int d_model, int parts, int seq_len) {
     const long long i8 = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;   // 8-element (16 B) index inside [T, D]
     const long long n8 = tokens * d_model / 8;
     if (i8 >= n8) return;
+    if constexpr (CAUSAL) parts = static_cast<int>((i8 * 8 / d_model) % seq_len) / BLK + 1;
     float acc[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) acc[e] = 0.f;
@@ -386,7 +413,7 @@ __global__ void __launch_bounds__(256) attn_dq_reduce_kernel(const bf16* __restr
         make_int4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]), pack_bf16x2(acc[4], acc[5]), pack_bf16x2(acc[6], acc[7]));
 }
 
-template <int HD>
+template <int HD, bool CAUSAL>
 int launch_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv, void* dq_part,
                long long tokens, long long batch, int seq_len, int num_heads, int d_model, unsigned long long seed,
                int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
@@ -406,23 +433,51 @@ int launch_bwd(const void* qkv, const void* out, const void* dout, const float* 
         int r = make_tmap(&tm_do, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dout, dims, str, box, swz);
         if (r) return r;
     }
-    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, false>>(C::SMEM_TOTAL)) return e;
-    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, false>>(C::SMEM_TOTAL)) return e;
-    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, true>>(C::SMEM_TOTAL)) return e;
-    if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, true>>(C::SMEM_TOTAL)) return e;
+    decltype(&attention_bwd_kernel<HD, false, false, CAUSAL>) kern;
+    if constexpr (CAUSAL) {
+        if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, false, true>>(C::SMEM_TOTAL)) return e;
+        if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, false, true>>(C::SMEM_TOTAL)) return e;
+        kern = drop_thr < 0 ? attention_bwd_kernel<HD, false, false, true> : attention_bwd_kernel<HD, true, false, true>;
+    } else {
+        if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, false, false>>(C::SMEM_TOTAL)) return e;
+        if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, false, false>>(C::SMEM_TOTAL)) return e;
+        if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, false, true, false>>(C::SMEM_TOTAL)) return e;
+        if (int e = set_max_dynamic_smem<attention_bwd_kernel<HD, true, true, false>>(C::SMEM_TOTAL)) return e;
+        kern = key_mask ? (drop_thr < 0 ? attention_bwd_kernel<HD, false, true, false> : attention_bwd_kernel<HD, true, true, false>)
+                        : (drop_thr < 0 ? attention_bwd_kernel<HD, false, false, false> : attention_bwd_kernel<HD, true, false, false>);
+    }
     const float scale = 1.f / sqrtf((float)HD);
     const int blocks = (seq_len + BLK - 1) / BLK;
     const long long pairs = tokens * num_heads, ctas = batch * num_heads * blocks;
     if (ctas > 0x7fffffffll) return -2;
     attn_delta_kernel<HD><<<(unsigned)((pairs * 32 + 255) / 256), 256, 0, st>>>((const bf16*)dout, (const bf16*)out, delta, pairs);
-    auto kern = key_mask ? (drop_thr < 0 ? attention_bwd_kernel<HD, false, true> : attention_bwd_kernel<HD, true, true>)
-                         : (drop_thr < 0 ? attention_bwd_kernel<HD, false, false> : attention_bwd_kernel<HD, true, false>);
     kern<<<(unsigned)ctas, NUM_THREADS, C::SMEM_TOTAL, st>>>(
         tm_qkv, tm_do, lse2, delta, (bf16*)dqkv, (bf16*)dq_part, tokens, d_model, num_heads, seq_len, scale,
         scale * 1.4426950408889634f, seed, static_cast<uint32_t>(drop_thr < 0 ? 0 : drop_thr), rescale, key_mask);
-    attn_dq_reduce_kernel<<<(unsigned)((tokens * d_model / 8 + 255) / 256), 256, 0, st>>>((const bf16*)dq_part, (bf16*)dqkv, tokens, d_model,
-                                                                                         blocks);
+    attn_dq_reduce_kernel<CAUSAL><<<(unsigned)((tokens * d_model / 8 + 255) / 256), 256, 0, st>>>(
+        (const bf16*)dq_part, (bf16*)dqkv, tokens, d_model, blocks, seq_len);
     return -(int)cudaGetLastError();
+}
+
+// shape checks and head-dim dispatch of both entry points
+template <bool CAUSAL>
+int attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
+                  void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
+                  int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
+    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
+    const int hd = d_model / num_heads;
+    if (hd != 32 && hd != 64 && hd != 128) return -2;
+    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
+    const long long batch = tokens / seq_len;
+    if (batch == 0) return 0;
+    if (hd == 32)
+        return launch_bwd<32, CAUSAL>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model,
+                                      seed, drop_thr, rescale, st, key_mask);
+    if (hd == 64)
+        return launch_bwd<64, CAUSAL>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model,
+                                      seed, drop_thr, rescale, st, key_mask);
+    return launch_bwd<128, CAUSAL>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model,
+                                   seed, drop_thr, rescale, st, key_mask);
 }
 
 }  // namespace attnb
@@ -443,20 +498,17 @@ extern "C" {
 int lah_attention_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
                       void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
                       int drop_thr, float rescale, cudaStream_t st, const uint32_t* key_mask) {
-    if (num_heads < 1 || d_model % num_heads || drop_thr > 65535) return -2;
-    const int hd = d_model / num_heads;
-    if (hd != 32 && hd != 64 && hd != 128) return -2;
-    if (seq_len < 1 || seq_len > drop::MAX_SEQ || tokens < 0 || tokens % seq_len) return -2;
-    const long long batch = tokens / seq_len;
-    if (batch == 0) return 0;
-    if (hd == 32)
-        return launch_bwd<32>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                              drop_thr, rescale, st, key_mask);
-    if (hd == 64)
-        return launch_bwd<64>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                              drop_thr, rescale, st, key_mask);
-    return launch_bwd<128>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, batch, seq_len, num_heads, d_model, seed,
-                           drop_thr, rescale, st, key_mask);
+    return attention_bwd<false>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, seq_len, num_heads, d_model, seed, drop_thr,
+                                rescale, st, key_mask);
+}
+
+// backward of lah_attention_fwd_causal: the arguments and return codes of lah_attention_bwd without a key padding mask.
+// Rows of dq_part's slice j below query 128 j are not written.
+int lah_attention_bwd_causal(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
+                             void* dq_part, long long tokens, int seq_len, int num_heads, int d_model, unsigned long long seed,
+                             int drop_thr, float rescale, cudaStream_t st) {
+    return attention_bwd<true>(qkv, out, dout, lse2, delta, dqkv, dq_part, tokens, seq_len, num_heads, d_model, seed, drop_thr,
+                               rescale, st, nullptr);
 }
 
 }  // extern "C"

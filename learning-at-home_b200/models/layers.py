@@ -14,7 +14,10 @@ Expert architectures (the L1 "ops/models" layer of SURVEY.md).
   Philox masks (DESIGN.md §9), so the reference's default ``name_to_block["transformer"]`` trains natively.  Like
   ``nn.MultiheadAttention`` it takes any sequence length; the sm_90a executor runs 1 <= S <= ``kernels.MAX_SEQ`` (65536)
   and head dims ``d_model / nhead`` in ``kernels.HEAD_DIMS`` = (32, 64, 128), so ``name_to_block["transformer"](hid_dim)``
-  (nhead 16) trains natively at hid_dim 512, 1024 and 2048.
+  (nhead 16) trains natively at hid_dim 512, 1024 and 2048.  ``causal=True`` makes it a causal (decoder-style) layer:
+  position t attends to positions <= t, through an upper-triangular -inf [S, S] ``attn_mask``, which is what
+  ``nn.TransformerEncoderLayer`` computes with ``is_causal=True`` and its square subsequent mask; the sm_90a executor
+  runs it on the causal attention kernels.  ``causal=False`` (the default) is the reference's layer.
 
 These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_90a execution of the same
 maths lives in ``lah_b200.parallel.engine`` (grouped wgmma GEMMs + fused LN/ReLU/Adam kernels).
@@ -53,8 +56,9 @@ FFN_SMALL_SEG_MASK = sum(1 << s for s, n in enumerate(FFN_SEG_NAMES) if not n.st
 
 
 class TransformerEncoderLayer(nn.Module):
-    def __init__(self, d_model: int, nhead: int, dim_feedforward: int = 2048, dropout: float = 0.1):
+    def __init__(self, d_model: int, nhead: int, dim_feedforward: int = 2048, dropout: float = 0.1, causal: bool = False):
         super().__init__()
+        self.causal = causal
         self.self_attn = nn.MultiheadAttention(d_model, nhead, dropout=dropout)
         self.linear1 = nn.Linear(d_model, dim_feedforward)
         self.dropout = nn.Dropout(dropout)
@@ -68,7 +72,12 @@ class TransformerEncoderLayer(nn.Module):
     def forward(self, src):
         # src: [batch, seq, d_model]; attention runs sequence-first on a transposed VIEW (no in-place transpose)
         x = src.transpose(0, 1)
-        attn = self.self_attn(x, x, x, need_weights=False)[0]
+        if self.causal:   # position t attends to positions <= t
+            S = x.shape[0]
+            mask = torch.triu(torch.full((S, S), float("-inf"), dtype=x.dtype, device=x.device), diagonal=1)
+            attn = self.self_attn(x, x, x, attn_mask=mask, need_weights=False)[0]
+        else:
+            attn = self.self_attn(x, x, x, need_weights=False)[0]
         x = self.norm1(x + self.dropout1(attn))
         ff = self.linear2(self.dropout(self.activation(self.linear1(x))))
         x = self.norm2(x + self.dropout2(ff))

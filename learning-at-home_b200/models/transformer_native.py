@@ -20,6 +20,7 @@ class NativeTransformerLayer(nn.Module):
         device = device or torch.device("cuda", torch.cuda.current_device())
         attn = layer.self_attn
         self.d_model, self.num_heads = attn.embed_dim, attn.num_heads
+        self.causal = bool(layer.causal)   # a causal layer runs the causal attention kernel, never the bidirectional one
         assert self.d_model % self.num_heads == 0 and self.d_model // self.num_heads in K.HEAD_DIMS, \
             f"the attention kernels run head_dim {K.HEAD_DIMS}, not {self.d_model} / {self.num_heads}"
 
@@ -66,7 +67,7 @@ class NativeTransformerLayer(nn.Module):
         elif x.dtype != torch.bfloat16 or not x.is_contiguous():
             x = x.to(torch.bfloat16).contiguous()
         gemm.grouped_linear(x, self.w_in, bias=self.b_in, out=ws["qkv"])
-        K.attention_fwd(ws["qkv"][:rows], self.num_heads, out=ws["att"][:rows], seq_len=seq)
+        K.attention_fwd(ws["qkv"][:rows], self.num_heads, out=ws["att"][:rows], seq_len=seq, causal=self.causal)
         gemm.grouped_linear(ws["att"], self.w_out, bias=self.b_out, residual=x, out=ws["h"])
         K.ln_relu_fwd(ws["h"], self.g1, self.be1, None, out=ws["x1"], mean=ws["mean"], rstd=ws["rstd"], relu=False)
         gemm.grouped_linear(ws["x1"], self.w1, bias=self.b1, out=ws["f"], act=2)

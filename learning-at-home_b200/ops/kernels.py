@@ -57,6 +57,8 @@ def _lib():
         "lah_cast_bf16": [P, P, L, P],
         "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
         "lah_attention_bwd": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
+        "lah_attention_fwd_causal": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
+        "lah_attention_bwd_causal": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P],
         "lah_pack_key_mask": [P, P, L, I, P],
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
@@ -321,13 +323,14 @@ def pack_key_mask_ref(pad):
     return torch.where(bits >= 2 ** 31, bits - 2 ** 32, bits).to(torch.int32)
 
 
-def _check_key_mask(key_mask, tokens, seq_len, device):
+def _check_key_mask(key_mask, tokens, seq_len, device, causal):
+    assert not (causal and key_mask is not None), "causal attention takes no key padding mask"
     if key_mask is not None:
         assert key_mask.dtype == torch.int32 and key_mask.is_contiguous() and key_mask.device == device
         assert key_mask.shape == (tokens // seq_len, (seq_len + 31) // 32), (tuple(key_mask.shape), tokens, seq_len)
 
 
-def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=512, key_mask=None):
+def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=512, key_mask=None, causal=False):
     """
     Self-attention over sequences of ``seq_len`` tokens (1 <= seq_len <= MAX_SEQ) on wgmma (csrc/attention.cu).
     :param qkv: [batch*seq_len, 3*d_model] bf16 = in_proj output, [q | k | v] per token; num_heads must divide d_model and
@@ -341,27 +344,32 @@ def attention_fwd(qkv, num_heads, *, out=None, lse=None, dropout=None, seq_len=5
     :param key_mask: optional key padding mask from ``pack_key_mask``: masked keys are ignored by every query of their
         sequence (queries at padded positions are still computed); key blocks of 128 without a valid key are skipped.  A
         sequence without a valid key gets out = 0.  None launches the unmasked kernel
+    :param causal: query q attends to keys <= q only (key blocks above the diagonal are neither loaded nor computed); takes
+        no ``key_mask``
     :returns: [batch*seq_len, d_model] bf16, heads concatenated (input of out_proj)
     """
     tokens, three_d = qkv.shape
     d_model = three_d // 3
-    assert qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.is_contiguous()
     assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
+    assert qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.is_contiguous()
     assert num_heads > 0 and d_model % num_heads == 0 and d_model // num_heads in HEAD_DIMS, (d_model, num_heads)
     if out is None:
         out = torch.empty(tokens, d_model, dtype=torch.bfloat16, device=qkv.device)
     assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == (tokens, d_model)
     if lse is not None:
         assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == tokens * num_heads
-    _check_key_mask(key_mask, tokens, seq_len, qkv.device)
+    _check_key_mask(key_mask, tokens, seq_len, qkv.device, causal)
     seed, thr, rescale = _dropout_args(dropout)
-    native.check(_lib().lah_attention_fwd(ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed, thr,
-                                          rescale, stream_ptr(), ptr(key_mask)), "lah_attention_fwd")
+    args = (ptr(qkv), ptr(out), ptr(lse), tokens, int(seq_len), num_heads, d_model, seed, thr, rescale, stream_ptr())
+    if causal:
+        native.check(_lib().lah_attention_fwd_causal(*args), "lah_attention_fwd_causal")
+    else:
+        native.check(_lib().lah_attention_fwd(*args, ptr(key_mask)), "lah_attention_fwd")
     native.count_launch()
     return out
 
 
-def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, dqkv=None, key_mask=None):
+def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, dqkv=None, key_mask=None, causal=False):
     """
     Backward of ``attention_fwd`` on wgmma (csrc/attention_bwd.cu): recomputes P from the saved log-sum-exp, forms dV / dK /
     dQ on tensor cores (nothing of size S x S touches HBM).  Returns dqkv [tokens, 3*d_model] bf16.  Same head dims as
@@ -372,12 +380,13 @@ def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, 
     :param dqkv: optional contiguous [tokens, 3*d_model] bf16 destination
     :param key_mask: the ``pack_key_mask`` words of the forward.  dK / dV rows of masked keys are exactly 0; a 128-key block
         without a valid key does no MMA and writes a zero dQ partial
+    :param causal: the ``causal`` of the forward: key block j walks only the query blocks that hold a query >= 128 j
     """
     tokens, three_d = qkv.shape
     d_model = three_d // 3
+    assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
     assert dout.dtype == torch.bfloat16 and dout.is_contiguous() and out.is_contiguous() and lse.dtype == torch.float32
     assert out.dtype == torch.bfloat16 and qkv.is_contiguous()
-    assert 1 <= seq_len <= MAX_SEQ and tokens % seq_len == 0, (tokens, seq_len)
     assert num_heads > 0 and d_model % num_heads == 0 and d_model // num_heads in HEAD_DIMS, (d_model, num_heads)
     delta = torch.empty(tokens, num_heads, dtype=torch.float32, device=qkv.device)      # rowsum(dout o out), filled by the prologue kernel
     if dqkv is None:
@@ -385,25 +394,30 @@ def attention_bwd(qkv, out, dout, lse, num_heads, *, dropout=None, seq_len=512, 
     assert dqkv.dtype == torch.bfloat16 and dqkv.is_contiguous() and dqkv.shape == qkv.shape
     blocks = (seq_len + 127) // 128
     dq_part = torch.empty(blocks, tokens, d_model, dtype=torch.bfloat16, device=qkv.device)  # one partial per 128-key block
-    _check_key_mask(key_mask, tokens, seq_len, qkv.device)
-    native.check(_lib().lah_attention_bwd(ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part),
-                                          tokens, int(seq_len), num_heads, d_model, *_dropout_args(dropout), stream_ptr(),
-                                          ptr(key_mask)),
-                 "lah_attention_bwd")
+    _check_key_mask(key_mask, tokens, seq_len, qkv.device, causal)
+    args = (ptr(qkv), ptr(out), ptr(dout), ptr(lse), ptr(delta), ptr(dqkv), ptr(dq_part), tokens, int(seq_len), num_heads,
+            d_model, *_dropout_args(dropout), stream_ptr())
+    if causal:
+        native.check(_lib().lah_attention_bwd_causal(*args), "lah_attention_bwd_causal")
+    else:
+        native.check(_lib().lah_attention_bwd(*args, ptr(key_mask)), "lah_attention_bwd")
     native.count_launch(3)   # delta prologue, wgmma backward, dQ partial reduction
     return dqkv
 
 
-def attention_ref(qkv, num_heads, seq_len=512, key_mask=None):
+def attention_ref(qkv, num_heads, seq_len=512, key_mask=None, causal=False):
     """fp32 oracle (fp64 for a fp64 input): softmax(q k^T / sqrt(d)) v per head.
     :param key_mask: optional bool [batch, seq_len], True = key ignored (torch's src_key_padding_mask): its scores are -inf;
-        rows without a valid key give 0 (``softmax(...).nan_to_num(0)``, which is what torch's layer computes in training mode)"""
+        rows without a valid key give 0 (``softmax(...).nan_to_num(0)``, which is what torch's layer computes in training mode)
+    :param causal: scores of keys > query are -inf"""
     tokens, three_d = qkv.shape
     d = three_d // 3
     x = qkv if qkv.dtype == torch.float64 else qkv.float()
     q, k, v = x.view(tokens // seq_len, seq_len, 3, num_heads, d // num_heads).unbind(2)
     q, k, v = (t.transpose(1, 2) for t in (q, k, v))  # [B, H, S, hd]
     s = q @ k.transpose(-1, -2) / (d // num_heads) ** 0.5
+    if causal:
+        s = s.masked_fill(torch.ones(seq_len, seq_len, dtype=torch.bool, device=s.device).triu(1), float("-inf"))
     if key_mask is None:
         att = torch.softmax(s, dim=-1) @ v
     else:

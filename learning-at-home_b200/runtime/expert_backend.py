@@ -39,7 +39,8 @@ class ExpertBackend(nn.Module):
             ``norm_first`` True or False, ``batch_first`` True or False, LayerNorm eps 1e-5 and all biases, head dim
             d_model / nhead in (32, 64, 128), d_model a multiple of 128 with 256 <= d_model <= 4096, dim_feedforward a
             multiple of 128, dropout p < 1 at every site, sequence length 1 <= S <= 65536 (wgmma attention and GEMMs,
-            in-kernel dropout, fused AMSGrad).
+            in-kernel dropout, fused AMSGrad).  This package's layer with ``causal=True`` (position t attends to
+            positions <= t) runs natively under the same conditions, on the causal attention kernels.
         ``torch.nn.TransformerEncoderLayer`` also runs natively with a key padding mask: one positional input and
         ``kwargs_schema={"src_key_padding_mask": BatchTensorProto(S, dtype=torch.bool)}`` (True = padding key, [batch, S]
         for sequence-first layers too).  The flat inputs are then (src, mask) for forward and (src, mask, grad_out) for

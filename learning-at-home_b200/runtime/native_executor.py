@@ -53,6 +53,7 @@ class EncoderLayerSpec(NamedTuple):
     activation: str          # "relu" or "gelu" (erf)
     batch_first: bool        # interface layout: [B, S, d] or [S, B, d]
     ps: Tuple[float, float, float, float]   # drop probabilities of sites 0-3: attention, dropout1, dropout, dropout2
+    causal: bool = False     # position t attends to positions <= t (this package's layer with causal=True)
 
 
 def ffn_spec(module) -> Optional[FFNSpec]:
@@ -77,16 +78,18 @@ def _activation(layer) -> Optional[str]:
 def encoder_layer_spec(module) -> Optional[EncoderLayerSpec]:
     """
     What NativeTransformerExecutor needs of an encoder layer, or None when it cannot run it.  Accepted, plain or
-    ``torch.jit.script``-ed: this package's TransformerEncoderLayer (batch-first, post-LN, GELU) and
+    ``torch.jit.script``-ed: this package's TransformerEncoderLayer (batch-first, post-LN, GELU, ``causal`` read from the
+    module) and
     torch.nn.TransformerEncoderLayer with either ``norm_first`` and ``batch_first``, ReLU or erf GELU.  Refused: any other
     activation (tanh GELU too), a LayerNorm eps other than 1e-5, missing biases or LayerNorm affine parameters, ``kdim`` /
     ``vdim`` other than d_model, ``add_bias_kv``, ``add_zero_attn``, and every other class.
     """
     name = class_name(module)
     if name == OWN_ENCODER_LAYER:
-        norm_first, activation, batch_first = False, "gelu", True
-    elif name == TORCH_ENCODER_LAYER:
+        norm_first, activation, batch_first, causal = False, "gelu", True, bool(module.causal)
+    elif name == TORCH_ENCODER_LAYER:   # is_causal is an argument of its forward, not of the layer: never causal here
         norm_first, activation, batch_first = bool(module.norm_first), _activation(module), bool(module.self_attn.batch_first)
+        causal = False
         if activation is None:
             return None
     else:
@@ -102,7 +105,7 @@ def encoder_layer_spec(module) -> Optional[EncoderLayerSpec]:
         return None
     ps = (float(attn.dropout), float(module.dropout1.p), float(module.dropout.p), float(module.dropout2.p))
     return EncoderLayerSpec(int(attn.embed_dim), int(attn.num_heads), int(module.linear1.out_features), norm_first,
-                            activation, batch_first, ps)
+                            activation, batch_first, ps, causal)
 
 def optimizer_groups(opt, params) -> Optional[List[int]]:
     """
@@ -402,6 +405,10 @@ class NativeTransformerExecutor:
     call (``K.pack_key_mask``) and given to the attention forward, its backward recompute and the attention backward; every
     other kernel is unchanged.  A sequence whose keys are all masked gets a zero attention output, as torch's layer in
     training mode; torch's eval fast path returns NaN for it.
+
+    Causal layers (this package's layer with ``causal=True``): the attention forward, its backward recompute and the
+    attention backward run the causal kernels (``causal=True`` of ``K.attention_fwd`` / ``K.attention_bwd``); every other
+    kernel is unchanged.
     """
     NAMES = ("w_in", "b_in", "w_out", "b_out", "w1", "b1", "w2", "b2", "g1", "be1", "g2", "be2")
     INPUT_DIMS = 3   # [batch, seq, d_model], or [seq, batch, d_model] for a sequence-first layer
@@ -455,6 +462,7 @@ class NativeTransformerExecutor:
         self.d, self.heads, self.ff = spec.d, spec.heads, spec.ff
         self.takes_key_padding_mask = class_name(expert) == TORCH_ENCODER_LAYER   # this package's layer has no mask input
         self.norm_first, self.relu, self.batch_first = spec.norm_first, spec.activation == "relu", spec.batch_first
+        self.causal = spec.causal
         params = self._segment_params(expert)
         self.device = params[0].device
         self.state = FlatAdamState(opt, params, self.NAMES, self.device)
@@ -528,7 +536,7 @@ class NativeTransformerExecutor:
             K.ln_relu_fwd(x, pv["g1"], pv["be1"], None, out=ws["xa"], mean=stats[0], rstd=stats[1], relu=False)
         gemm.grouped_linear(ws["xa"] if self.norm_first else x, bv["w_in"], bias=pv["b_in"], out=ws["qkv"])
         K.attention_fwd(ws["qkv"][:Tr], self.heads, out=ws["att"][:Tr], lse=ws["lse"][:Tr], dropout=site(drop, K.SITE_ATTN),
-                        seq_len=seq, key_mask=key_mask)
+                        seq_len=seq, key_mask=key_mask, causal=self.causal)
         gemm.grouped_linear(ws["att"], bv["w_out"], bias=pv["b_out"], residual=x, out=ws["h"],
                             dropout=site(drop, K.SITE_OUT_PROJ))
         if self.norm_first:   # x1 = LN2(h) feeds the feed-forward branch, h is its residual
@@ -617,10 +625,10 @@ class NativeTransformerExecutor:
             dqkv = torch.empty(T, 3 * d, **bf)
             dqkv[Tr:].zero_()
             K.attention_bwd(ws["qkv"][:Tr], ws["att"][:Tr], datt[:Tr], ws["lse"][:Tr], self.heads, dropout=site(drop, K.SITE_ATTN),
-                            seq_len=seq, dqkv=dqkv[:Tr], key_mask=key_mask)
+                            seq_len=seq, dqkv=dqkv[:Tr], key_mask=key_mask, causal=self.causal)
         else:
             dqkv = K.attention_bwd(ws["qkv"], ws["att"], datt, ws["lse"], self.heads, dropout=site(drop, K.SITE_ATTN), seq_len=seq,
-                                   key_mask=key_mask)
+                                   key_mask=key_mask, causal=self.causal)
         K.grouped_colsum(dqkv, None, out=gv["b_in"])
         if self.norm_first:   # dx = dh + LN1 backward(dxa)
             gemm.grouped_wgrad(dqkv, ws["xa"], go, 1, out=gv["w_in"])
