@@ -8,6 +8,12 @@
 //
 // One thread owns one mask granule ({r, r+8} x {b, b+1, b+8, b+9}): one Philox call, eight elements, 4-byte accesses that a
 // quad of threads turns into 32 contiguous bytes per row.  GELU is the erf form, as nn.GELU().
+//
+// The gated activation of GatedFeedforwardBlock lives here too (no dropout): over the stacked pre-activation
+// h = [g | u] ([rows, 2 inner], the output of the one GEMM over [W1; W3])
+//   forward   a  = silu(g) o u
+//   backward  dh = [da o u o s (1 + g (1 - s)) | da o silu(g)],  s = sigmoid(g)
+// in fp32 with one bf16 rounding per output, 16-byte accesses (one thread per 8 columns of a row).
 #include "sm90.cuh"
 #include "dropout.cuh"
 
@@ -74,6 +80,58 @@ __global__ void __launch_bounds__(256) dropout_mask_kernel(uint8_t* __restrict__
 }
 
 }  // namespace drop
+
+// sigmoid that saturates to exactly 0 / 1 for large |g| (exp overflows to inf, 1 / inf = 0), so that no product below
+// meets inf * 0
+__device__ __forceinline__ float sigmoid_f(float g) { return 1.f / (1.f + __expf(-g)); }
+
+__device__ __forceinline__ void unpack8(const int4& q, float (&f)[8]) {
+    const uint32_t w[4] = {(uint32_t)q.x, (uint32_t)q.y, (uint32_t)q.z, (uint32_t)q.w};
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+        const float2 v = unpack_bf16x2(w[t]);
+        f[2 * t] = v.x;
+        f[2 * t + 1] = v.y;
+    }
+}
+
+__device__ __forceinline__ int4 pack8(const float (&f)[8]) {
+    return make_int4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
+}
+
+// thread t: row t / (inner / 8), columns 8 (t % (inner / 8)) .. + 7 of g, u, a / da and dg, du
+template <bool BWD>
+__global__ void __launch_bounds__(256) swiglu_kernel(const bf16* __restrict__ h, const bf16* __restrict__ da,
+                                                     bf16* __restrict__ out, long long vecs, int inner) {
+    const long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (t >= vecs) return;
+    const int per_row = inner >> 3;
+    const long long row = t / per_row;
+    const int col = static_cast<int>(t - row * per_row) * 8;
+    const bf16* hr = h + row * 2 * inner;
+    float g[8], u[8];
+    unpack8(__ldg(reinterpret_cast<const int4*>(hr + col)), g);
+    unpack8(__ldg(reinterpret_cast<const int4*>(hr + inner + col)), u);
+    if (!BWD) {
+        float a[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) a[i] = g[i] * sigmoid_f(g[i]) * u[i];
+        *reinterpret_cast<int4*>(out + row * inner + col) = pack8(a);
+    } else {
+        float d[8], dg[8], du[8];
+        unpack8(__ldg(reinterpret_cast<const int4*>(da + row * inner + col)), d);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const float s = sigmoid_f(g[i]);
+            dg[i] = d[i] * u[i] * (s * (1.f + g[i] * (1.f - s)));
+            du[i] = d[i] * (g[i] * s);
+        }
+        bf16* o = out + row * 2 * inner;
+        *reinterpret_cast<int4*>(o + col) = pack8(dg);
+        *reinterpret_cast<int4*>(o + inner + col) = pack8(du);
+    }
+}
+
 }  // namespace lah
 
 using namespace lah;
@@ -115,6 +173,25 @@ int lah_dropout_ew(int op, const void* x, const void* f, void* out, long long ro
                                                             scale);
     else
         return -3;
+    return -(int)cudaGetLastError();
+}
+
+// SwiGLU forward: a [rows, inner] = silu(g) o u of h = [g | u] [rows, 2 inner]; contiguous bf16, inner a multiple of 128
+int lah_swiglu_fwd(const void* h, void* a, long long rows, int inner, cudaStream_t st) {
+    if (rows < 0 || inner <= 0 || inner % 128) return -2;
+    const long long vecs = rows * (inner / 8);
+    if (vecs == 0) return 0;
+    swiglu_kernel<false><<<(unsigned)((vecs + 255) / 256), 256, 0, st>>>((const bf16*)h, nullptr, (bf16*)a, vecs, inner);
+    return -(int)cudaGetLastError();
+}
+
+// SwiGLU backward: dh [rows, 2 inner] = [dg | du] from da [rows, inner] and the forward's h
+int lah_swiglu_bwd(const void* da, const void* h, void* dh, long long rows, int inner, cudaStream_t st) {
+    if (rows < 0 || inner <= 0 || inner % 128) return -2;
+    const long long vecs = rows * (inner / 8);
+    if (vecs == 0) return 0;
+    swiglu_kernel<true><<<(unsigned)((vecs + 255) / 256), 256, 0, st>>>((const bf16*)h, (const bf16*)da, (bf16*)dh, vecs,
+                                                                       inner);
     return -(int)cudaGetLastError();
 }
 

@@ -1,5 +1,5 @@
 // layernorm.cu — fused (bias already added by the GEMM epilogue) LayerNorm + ReLU forward / backward over
-// expert-grouped rows, plus grouped column sums (bias gradients).
+// expert-grouped rows, plus grouped column sums (bias gradients), and the RMSNorm forward / backward of the gated expert.
 //
 // Reference semantics: nn.LayerNorm(4h) -> nn.ReLU between the expert's Linear layers
 // (/root/reference/experiments/throughput/layers.py:9-15); per-expert affine parameters gamma/beta are stacked [G, C].
@@ -370,6 +370,226 @@ __global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS)
 }
 
 // ------------------------------------------------------------------------------------------------
+// RMSNorm, the pre-norm of GatedFeedforwardBlock (one expert: gamma is [C], no tile groups).
+//   forward   n = x * rstd * gamma,  rstd = 1 / sqrt(mean(x^2) + eps) saved per row (fp32); eps is an argument
+//   backward  dx = dres + rstd * (gamma o dn - x * mean(gamma o dn o x) * rstd^2)   (one rounding, dres optional)
+//             dgamma += column sums of dn o x * rstd, per tile into part[tile][C], added in tile order by
+//             group_tile_sum_kernel (run-to-run identical)
+// They are separate kernels, not a flag of the LayerNorm ones: those take no eps argument, and giving them one would change
+// the code of every LayerNorm instantiation.  They share the LayerNorm sizing: the chunks per lane of LnFwdCfg (rows per
+// warp: RmsFwdCfg below) and the CTA shape and rows per batch of LnBwdCfg.
+// ------------------------------------------------------------------------------------------------
+// Rows per warp: the LayerNorm rule for the widths it was not tuned at (R = 4 up to NV = 2, 2 up to NV = 6, else 1), at
+// every width; the tuned power-of-two configurations hold 2-4x the rows and spill here.  Above NV = 11 one row no longer
+// fits in 128 registers (2944 spilled), so those widths ask for one CTA per SM.
+template <int C>
+struct RmsFwdCfg {
+    static constexpr int NV = LnFwdCfg<C>::NV;
+    static constexpr int R = NV <= 2 ? 4 : (NV <= 6 ? 2 : 1);
+    static constexpr int MIN_BLOCKS = NV <= 11 ? 2 : 1;
+};
+
+template <int C, int R>
+__global__ void __launch_bounds__(256, RmsFwdCfg<C>::MIN_BLOCKS) rms_norm_fwd_kernel(
+    const bf16* __restrict__ x, bf16* __restrict__ n, float* __restrict__ rstd_out, const float* __restrict__ gamma,
+    int rows, float eps) {
+    constexpr int NV = LnFwdCfg<C>::NV;
+    constexpr bool HALF = C % 256 != 0;
+    static_assert(C % 128 == 0 && C <= LN_MAX_C, "unsupported RMSNorm width");
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int row0 = (blockIdx.x * 8 + warp) * R;
+    if (row0 >= rows) return;
+    int4 q[R][NV];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const int4* xp = reinterpret_cast<const int4*>(x + static_cast<long long>(min(row0 + r, rows - 1)) * C);
+#pragma unroll
+        for (int j = 0; j < NV; ++j) {
+            if constexpr (HALF) {
+                if (j == NV - 1 && lane >= 16) {
+                    q[r][j] = make_int4(0, 0, 0, 0);
+                    continue;
+                }
+            }
+            q[r][j] = ld_nc_v4(xp + j * 32 + lane);
+        }
+    }
+    float rstd[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        float ss = 0.f;
+#pragma unroll
+        for (int j = 0; j < NV; ++j) {
+            const uint32_t w[4] = {(uint32_t)q[r][j].x, (uint32_t)q[r][j].y, (uint32_t)q[r][j].z, (uint32_t)q[r][j].w};
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const float2 f = unpack_bf16x2(w[t]);
+                ss += f.x * f.x + f.y * f.y;
+            }
+        }
+        ss = warp_sum(ss);
+        rstd[r] = rsqrtf(ss * (1.f / C) + eps);
+        if (lane == 0 && row0 + r < rows) rstd_out[row0 + r] = rstd[r];
+    }
+#pragma unroll
+    for (int j = 0; j < NV; ++j) {
+        if constexpr (HALF) {
+            if (j == NV - 1 && lane >= 16) break;
+        }
+        const int col = (j * 32 + lane) * 8;
+        const int4 g0 = ld_nc_v4(reinterpret_cast<const int4*>(gamma + col));
+        const int4 g1 = ld_nc_v4(reinterpret_cast<const int4*>(gamma + col + 4));
+        const float gg[8] = {__int_as_float(g0.x), __int_as_float(g0.y), __int_as_float(g0.z), __int_as_float(g0.w),
+                             __int_as_float(g1.x), __int_as_float(g1.y), __int_as_float(g1.z), __int_as_float(g1.w)};
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const int row = row0 + r;
+            if (row >= rows) continue;   // warp-uniform
+            const uint32_t w[4] = {(uint32_t)q[r][j].x, (uint32_t)q[r][j].y, (uint32_t)q[r][j].z, (uint32_t)q[r][j].w};
+            float y[8];
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const float2 f = unpack_bf16x2(w[t]);
+                y[2 * t] = f.x * rstd[r] * gg[2 * t];
+                y[2 * t + 1] = f.y * rstd[r] * gg[2 * t + 1];
+            }
+            int4 o;
+            o.x = pack_bf16x2(y[0], y[1]);
+            o.y = pack_bf16x2(y[2], y[3]);
+            o.z = pack_bf16x2(y[4], y[5]);
+            o.w = pack_bf16x2(y[6], y[7]);
+            st_v4(reinterpret_cast<int4*>(n + static_cast<long long>(row) * C) + j * 32 + lane, o);
+        }
+    }
+}
+
+template <int C, bool RES>
+__global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS) rms_norm_bwd_kernel(
+    const bf16* __restrict__ dn, const bf16* __restrict__ x, const float* __restrict__ rstd_in,
+    const float* __restrict__ gamma, bf16* __restrict__ dx, float* __restrict__ part, int rows, int tile_rows,
+    const bf16* __restrict__ dres) {
+    constexpr int THREADS = LnBwdCfg<C>::THREADS;
+    constexpr int WARPS = THREADS / 32;
+    constexpr bool IDLE = THREADS * 8 != C;
+    static_assert(C % 128 == 0 && C <= LN_MAX_C, "unsupported RMSNorm width");
+    constexpr int RB = LnBwdCfg<C>::RB;
+    __shared__ float red[WARPS][RB];
+    __shared__ float tot[RB];
+    const int tile = blockIdx.x;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int col = tid * 8;
+    const bool live = !IDLE || col < C;
+    float gam[8];
+    if (!live) {
+#pragma unroll
+        for (int t = 0; t < 8; ++t) gam[t] = 0.f;
+    } else {
+        const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + col));
+        const float4 g1 = __ldg(reinterpret_cast<const float4*>(gamma + col + 4));
+        gam[0] = g0.x; gam[1] = g0.y; gam[2] = g0.z; gam[3] = g0.w; gam[4] = g1.x; gam[5] = g1.y; gam[6] = g1.z; gam[7] = g1.w;
+    }
+    float acc_dg[8];
+#pragma unroll
+    for (int t = 0; t < 8; ++t) acc_dg[t] = 0.f;
+
+    const int row0 = tile * tile_rows;
+    const int row_end = min(rows, row0 + tile_rows);
+    // software pipeline, as in ln_relu_bwd_kernel: the loads of batch i+1 are in flight while batch i is reduced / written
+    int4 nqd[RB], nqx[RB];
+    float nrs[RB];
+    auto issue_loads = [&](int rb) {
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+            const int row = rb + r;
+            const int rr = row < row_end ? row : row0;
+            const long long off = static_cast<long long>(rr) * C + col;
+            if (live) {
+                nqd[r] = ld_nc_v4(reinterpret_cast<const int4*>(dn + off));
+                nqx[r] = ld_nc_v4(reinterpret_cast<const int4*>(x + off));
+            } else {
+                nqd[r] = nqx[r] = make_int4(0, 0, 0, 0);
+            }
+            nrs[r] = __ldg(rstd_in + rr);
+        }
+    };
+    issue_loads(row0);
+    for (int rb = row0; rb < row_end; rb += RB) {
+        int4 qd[RB], qx[RB];
+        float rs[RB], sum[RB];
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+            qd[r] = nqd[r];
+            qx[r] = nqx[r];
+            rs[r] = nrs[r];
+        }
+        if (rb + RB < row_end) issue_loads(rb + RB);
+        auto unpack8 = [](const int4& q, float (&f)[8]) {
+            const uint32_t w[4] = {(uint32_t)q.x, (uint32_t)q.y, (uint32_t)q.z, (uint32_t)q.w};
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const float2 v = unpack_bf16x2(w[t]);
+                f[2 * t] = v.x;
+                f[2 * t + 1] = v.y;
+            }
+        };
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {   // sum over the row of gamma o dn o x (rows past the tile: zero)
+            float d[8], xv[8], s = 0.f;
+            unpack8(qd[r], d);
+            unpack8(qx[r], xv);
+#pragma unroll
+            for (int t = 0; t < 8; ++t) s += d[t] * gam[t] * xv[t];
+            sum[r] = rb + r < row_end ? s : 0.f;
+        }
+#pragma unroll
+        for (int r = 0; r < RB; ++r) sum[r] = warp_sum(sum[r]);
+        if (lane == 0) {
+#pragma unroll
+            for (int r = 0; r < RB; ++r) red[warp][r] = sum[r];
+        }
+        __syncthreads();
+        if (tid < RB) {
+            float s = 0.f;
+#pragma unroll
+            for (int w = 0; w < WARPS; ++w) s += red[w][tid];
+            tot[tid] = s * (1.f / C);
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+            const int row = rb + r;
+            if (row >= row_end || !live) continue;
+            float d[8], xv[8], o[8];
+            unpack8(qd[r], d);
+            unpack8(qx[r], xv);
+            const float m = tot[r] * rs[r] * rs[r];
+            if (RES) {
+                float res[8];
+                unpack8(ld_nc_v4(reinterpret_cast<const int4*>(dres + static_cast<long long>(row) * C + col)), res);
+#pragma unroll
+                for (int t = 0; t < 8; ++t) o[t] = rs[r] * (d[t] * gam[t] - xv[t] * m) + res[t];
+            } else {
+#pragma unroll
+                for (int t = 0; t < 8; ++t) o[t] = rs[r] * (d[t] * gam[t] - xv[t] * m);
+            }
+#pragma unroll
+            for (int t = 0; t < 8; ++t) acc_dg[t] += d[t] * (xv[t] * rs[r]);
+            int4 q;
+            q.x = pack_bf16x2(o[0], o[1]);
+            q.y = pack_bf16x2(o[2], o[3]);
+            q.z = pack_bf16x2(o[4], o[5]);
+            q.w = pack_bf16x2(o[6], o[7]);
+            *reinterpret_cast<int4*>(dx + static_cast<long long>(row) * C + col) = q;
+        }
+        // `tot` is rewritten only after the next batch's first __syncthreads (see ln_relu_bwd_kernel)
+    }
+    if (!live) return;
+    float* pg = part + static_cast<long long>(tile) * C + col;
+#pragma unroll
+    for (int t = 0; t < 8; ++t) pg[t] = acc_dg[t];
+}
+
+// ------------------------------------------------------------------------------------------------
 // grouped column sum: out[g, c] += sum over the rows of every 128-row tile of group g of x[row, c]
 // CTA = (tile, 256-column slab); thread owns one column pair, 4 row phases; the tile's sums go to part[tile][C] and are
 // added to out by group_tile_sum_kernel
@@ -481,6 +701,42 @@ constexpr auto ln_bwd_table(std::integer_sequence<int, I...>) {
 constexpr auto kLnFwd = ln_fwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
 constexpr auto kLnBwd = ln_bwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
 
+using RmsFwdLaunch = void (*)(const void*, void*, float*, const float*, int, float, cudaStream_t);
+using RmsBwdLaunch = void (*)(const void*, const void*, const float*, const float*, void*, float*, float*, int, int,
+                              const void*, cudaStream_t);
+
+template <int C>
+void rms_fwd_launch(const void* x, void* n, float* rstd, const float* gamma, int rows, float eps, cudaStream_t st) {
+    constexpr int RR = RmsFwdCfg<C>::R;
+    rms_norm_fwd_kernel<C, RR><<<(rows + 8 * RR - 1) / (8 * RR), 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma,
+                                                                               rows, eps);
+}
+
+template <int C>
+void rms_bwd_launch(const void* dn, const void* x, const float* rstd, const float* gamma, void* dx, float* dgamma,
+                    float* part, int rows, int tile_rows, const void* dres, cudaStream_t st) {
+    const int grid = (rows + tile_rows - 1) / tile_rows;
+    constexpr int T = LnBwdCfg<C>::THREADS;
+    if (dres)
+        rms_norm_bwd_kernel<C, true><<<grid, T, 0, st>>>((const bf16*)dn, (const bf16*)x, rstd, gamma, (bf16*)dx, part,
+                                                         rows, tile_rows, (const bf16*)dres);
+    else
+        rms_norm_bwd_kernel<C, false><<<grid, T, 0, st>>>((const bf16*)dn, (const bf16*)x, rstd, gamma, (bf16*)dx, part,
+                                                          rows, tile_rows, nullptr);
+    group_tile_sum_kernel<<<(C + 255) / 256, 256, 0, st>>>(part, grid, 1, C, nullptr, dgamma, nullptr, nullptr);
+}
+
+template <int... I>
+constexpr auto rms_fwd_table(std::integer_sequence<int, I...>) {
+    return std::array<RmsFwdLaunch, sizeof...(I)>{rms_fwd_launch<(I + 1) * 128>...};
+}
+template <int... I>
+constexpr auto rms_bwd_table(std::integer_sequence<int, I...>) {
+    return std::array<RmsBwdLaunch, sizeof...(I)>{rms_bwd_launch<(I + 1) * 128>...};
+}
+constexpr auto kRmsFwd = rms_fwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
+constexpr auto kRmsBwd = rms_bwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
+
 // widths the LayerNorm entry points run: multiples of 128 up to LN_MAX_C (the column sum has no upper limit)
 static bool ln_width_ok(int C) { return C > 0 && C % 128 == 0 && C <= LN_MAX_C; }
 
@@ -535,6 +791,25 @@ int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const floa
     if (shift_of(tile_rows) < 0 || !ln_width_ok(C)) return -2;
     kLnBwd[C / 128 - 1](da, h, mean, rstd, gamma, beta, dh, dgamma, dbeta, dbias, part, tile_group, rows, relu,
                         tile_rows, dres, st);
+    return -(int)cudaGetLastError();
+}
+
+// RMSNorm forward over [rows, C] bf16 (n: [rows, C] bf16, rstd: [rows] fp32, gamma: [C] fp32); eps > 0
+int lah_rms_norm_fwd(const void* x, void* n, float* rstd, const float* gamma, int rows, int C, float eps,
+                     cudaStream_t st) {
+    if (rows <= 0) return 0;
+    if (!ln_width_ok(C) || !(eps > 0.f)) return -2;
+    kRmsFwd[C / 128 - 1](x, n, rstd, gamma, rows, eps, st);
+    return -(int)cudaGetLastError();
+}
+
+// RMSNorm backward: dx [rows, C] bf16, dgamma [C] fp32 (+=); part: scratch of [ceil(rows / tile_rows), C] fp32;
+// dres: optional [rows, C] bf16 gradient of a residual that bypasses the norm, added to dx before its rounding; NULL = none
+int lah_rms_norm_bwd(const void* dn, const void* x, const float* rstd, const float* gamma, void* dx, float* dgamma,
+                     float* part, int rows, int C, int tile_rows, const void* dres, cudaStream_t st) {
+    if (rows <= 0) return 0;
+    if (shift_of(tile_rows) < 0 || !ln_width_ok(C)) return -2;
+    kRmsBwd[C / 128 - 1](dn, x, rstd, gamma, dx, dgamma, part, rows, tile_rows, dres, st);
     return -(int)cudaGetLastError();
 }
 

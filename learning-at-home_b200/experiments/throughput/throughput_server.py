@@ -14,7 +14,7 @@ from ...models.layers import name_to_block, SEQ_LEN
 
 
 def build_experts(args, device=None):
-    inp_shape = (args.hid_dim,) if args.block_type == "ffn" else (SEQ_LEN, args.hid_dim)
+    inp_shape = (args.hid_dim,) if args.block_type in ("ffn", "swiglu") else (SEQ_LEN, args.hid_dim)
     experts = {}
     for i in range(args.layers_per_gpu):
         expert = name_to_block[args.block_type](args.hid_dim)

@@ -1,2 +1,2 @@
-from .layers import FeedforwardBlock, TransformerEncoderLayer, name_to_block, name_to_input
+from .layers import FeedforwardBlock, GatedFeedforwardBlock, TransformerEncoderLayer, name_to_block, name_to_input
 from .emulator import EmulatedDMoE, EmulatedFaultyDMoE, get_non_expert_params

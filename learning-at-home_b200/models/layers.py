@@ -18,6 +18,8 @@ Expert architectures (the L1 "ops/models" layer of SURVEY.md).
   position t attends to positions <= t, through an upper-triangular -inf [S, S] ``attn_mask``, which is what
   ``nn.TransformerEncoderLayer`` computes with ``is_causal=True`` and its square subsequent mask; the sm_90a executor
   runs it on the causal attention kernels.  ``causal=False`` (the default) is the reference's layer.
+* ``GatedFeedforwardBlock(hid, inner_dim=0, eps=1e-6)``: x + w2(silu(w1(h)) * w3(h)), h = RMSNorm(x), no biases: the
+  SwiGLU expert MLP of today's MoE models (parameter names of a Mixtral expert), ``name_to_block["swiglu"]``.
 
 These are the plain PyTorch definitions (CPU path, oracle, checkpoint container).  The sm_90a execution of the same
 maths lives in ``lah_b200.parallel.engine`` (grouped wgmma GEMMs + fused LN/ReLU/Adam kernels).
@@ -55,6 +57,32 @@ FFN_SEG_NAMES = tuple(FFN_SEG_KEYS)
 FFN_SMALL_SEG_MASK = sum(1 << s for s, n in enumerate(FFN_SEG_NAMES) if not n.startswith("w"))
 
 
+def gated_inner_dim(hid_dim: int) -> int:
+    """the default inner width of GatedFeedforwardBlock: 8 hid / 3 rounded up to a multiple of 128 (Llama's convention;
+    2816 at hid 1024, 11008 at hid 4096), the parameter count of a 4 hid MLP"""
+    return -(-8 * hid_dim // (3 * 128)) * 128
+
+
+class GatedFeedforwardBlock(nn.Module):
+    """
+    The gated (SwiGLU) expert MLP of Mixtral, DeepSeek-MoE, Qwen-MoE and Llama, with its RMSNorm pre-norm and residual:
+    ``x + w2(silu(w1(h)) * w3(h))``, ``h = norm(x)``.  No biases.  Parameter names ``norm.weight``, ``w1.weight``,
+    ``w2.weight``, ``w3.weight`` are those of a Mixtral expert.  ``inner_dim = 0`` selects ``gated_inner_dim(hid_dim)``.
+    """
+
+    def __init__(self, hid_dim: int, inner_dim: int = 0, eps: float = 1e-6):
+        super().__init__()
+        inner = inner_dim or gated_inner_dim(hid_dim)
+        self.norm = nn.RMSNorm(hid_dim, eps=eps)
+        self.w1 = nn.Linear(hid_dim, inner, bias=False)
+        self.w2 = nn.Linear(inner, hid_dim, bias=False)
+        self.w3 = nn.Linear(hid_dim, inner, bias=False)
+
+    def forward(self, x):
+        h = self.norm(x)
+        return x + self.w2(F.silu(self.w1(h)) * self.w3(h))
+
+
 class TransformerEncoderLayer(nn.Module):
     def __init__(self, d_model: int, nhead: int, dim_feedforward: int = 2048, dropout: float = 0.1, causal: bool = False):
         super().__init__()
@@ -89,8 +117,10 @@ SEQ_LEN = 512  # input shape of the throughput experiment (reference layers.py:5
 name_to_block = {
     "ffn": lambda hid_dim: FeedforwardBlock(hid_dim),
     "transformer": lambda hid_dim: TransformerEncoderLayer(hid_dim, nhead=16),
+    "swiglu": lambda hid_dim: GatedFeedforwardBlock(hid_dim),
 }
 name_to_input = {
     "ffn": lambda batch_size, hid_dim: torch.empty((batch_size, hid_dim)),
+    "swiglu": lambda batch_size, hid_dim: torch.empty((batch_size, hid_dim)),
     "transformer": lambda batch_size, hid_dim: torch.empty((batch_size, SEQ_LEN, hid_dim)),
 }

@@ -62,6 +62,10 @@ def _lib():
         "lah_pack_key_mask": [P, P, L, I, P],
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
+        "lah_rms_norm_fwd": [P, P, P, P, I, I, Fl, P],
+        "lah_rms_norm_bwd": [P, P, P, P, P, P, P, I, I, I, P, P],
+        "lah_swiglu_fwd": [P, P, L, I, P],
+        "lah_swiglu_bwd": [P, P, P, L, I, P],
         "lah_symm_alloc": [c_ull, ctypes.POINTER(c_void_p)],
         "lah_symm_free": [P],
         "lah_symm_get_handle": [P, ctypes.c_char_p],
@@ -128,6 +132,76 @@ def ln_relu_bwd(da, h, mean, rstd, gamma, beta, tile_group, *, dh, dgamma, dbeta
                                         int(relu), int(tile_rows), ptr(dres), stream_ptr()), "lah_ln_relu_bwd")
     native.count_launch(2)
     return dh
+
+
+def _bf16_rows(t, what, shape):
+    if t.dtype != torch.bfloat16 or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{what}: expected a contiguous bf16 tensor of shape {tuple(shape)}, got {t.dtype} "
+                         f"{tuple(t.shape)}{'' if t.is_contiguous() else ' (not contiguous)'}")
+
+
+def _f32_vec(t, what, n):
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n:
+        raise ValueError(f"{what}: expected a contiguous float32 tensor of {n} elements, got {t.dtype} {tuple(t.shape)}")
+
+
+def rms_norm_fwd(x, gamma, eps, *, out, rstd):
+    """RMSNorm over the rows of x (csrc/layernorm.cu): out = bf16(x * rstd * gamma), rstd[r] = 1 / sqrt(mean(x_r^2) + eps)
+    kept in fp32.  x, out: bf16 [rows, C] with C in LN_WIDTHS; gamma: fp32 [C]; rstd: fp32 [rows]; eps > 0"""
+    if x.dim() != 2:
+        raise ValueError(f"rms_norm_fwd: x must be [rows, C], got {tuple(x.shape)}")
+    rows, C = x.shape
+    _check_ln_width(C, "rms_norm_fwd")
+    _bf16_rows(x, "rms_norm_fwd x", (rows, C))
+    _bf16_rows(out, "rms_norm_fwd out", (rows, C))
+    _f32_vec(gamma, "rms_norm_fwd gamma", C)
+    _f32_vec(rstd, "rms_norm_fwd rstd", rows)
+    if not eps > 0:
+        raise ValueError(f"rms_norm_fwd: eps must be > 0, got {eps}")
+    native.check(_lib().lah_rms_norm_fwd(ptr(x), ptr(out), ptr(rstd), ptr(gamma), rows, C, float(eps), stream_ptr()),
+                 "lah_rms_norm_fwd")
+    native.count_launch()
+    return out
+
+
+def rms_norm_bwd(dn, x, rstd, gamma, *, dx, dgamma, dres=None, tile_rows=16):
+    """backward of ``rms_norm_fwd``: dx = dres + rstd (gamma o dn - x mean(gamma o dn o x) rstd^2), rounded once;
+    dgamma (+)= the column sums of dn o x rstd, per ``tile_rows`` rows (a power of two >= 8) and then in tile order
+    (run-to-run identical).  dres: optional bf16 [rows, C] gradient of a residual that bypasses the norm"""
+    if x.dim() != 2:
+        raise ValueError(f"rms_norm_bwd: x must be [rows, C], got {tuple(x.shape)}")
+    rows, C = x.shape
+    _check_ln_width(C, "rms_norm_bwd")
+    for t, what in ((dn, "dn"), (x, "x"), (dx, "dx")) + (((dres, "dres"),) if dres is not None else ()):
+        _bf16_rows(t, f"rms_norm_bwd {what}", (rows, C))
+    _f32_vec(gamma, "rms_norm_bwd gamma", C)
+    _f32_vec(dgamma, "rms_norm_bwd dgamma", C)
+    _f32_vec(rstd, "rms_norm_bwd rstd", rows)
+    if tile_rows < 8 or tile_rows & (tile_rows - 1):
+        raise ValueError(f"rms_norm_bwd: tile_rows must be a power of two >= 8, got {tile_rows}")
+    part = torch.empty((rows + tile_rows - 1) // tile_rows, C, device=x.device, dtype=torch.float32)
+    native.check(_lib().lah_rms_norm_bwd(ptr(dn), ptr(x), ptr(rstd), ptr(gamma), ptr(dx), ptr(dgamma), ptr(part), rows, C,
+                                         int(tile_rows), ptr(dres), stream_ptr()), "lah_rms_norm_bwd")
+    native.count_launch(2)
+    return dx
+
+
+def rms_norm_fwd_ref(x, gamma, eps):
+    """oracle of ``rms_norm_fwd`` in fp32 (fp64 for a fp64 input): (n, rstd)"""
+    xf = x if x.dtype == torch.float64 else x.float()
+    rstd = torch.rsqrt(xf.pow(2).mean(-1) + eps)
+    return xf * rstd[:, None] * gamma.to(xf.dtype), rstd
+
+
+def rms_norm_bwd_ref(dn, x, gamma, eps, dres=None):
+    """oracle of ``rms_norm_bwd`` in fp32 (fp64 for a fp64 input), closed form: (dx, dgamma)"""
+    xf = x if x.dtype == torch.float64 else x.float()
+    d, g = dn.to(xf.dtype), gamma.to(xf.dtype)
+    rstd = torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)
+    dx = rstd * (g * d - xf * (g * d * xf).mean(-1, keepdim=True) * rstd * rstd)
+    if dres is not None:
+        dx = dx + dres.to(xf.dtype)
+    return dx, (d * xf * rstd).sum(0)
 
 
 def grouped_colsum(x, tile_group, *, out, tile_rows=128):
@@ -509,6 +583,56 @@ def relu_dropout_ref(f, mask, p):
 def relu_dropout_bwd_ref(dg, f, mask, p):
     """fp32 oracle of ``relu_dropout_bwd``"""
     return (f.float() > 0).float() * mask.float() * dg.float() / (1 - p)
+
+
+# ---------------------------------------------------------------------------------------------------------
+# SwiGLU of the gated expert (csrc/dropout.cu): h = [g | u] is the output of the one GEMM over [W1; W3]
+# ---------------------------------------------------------------------------------------------------------
+def _check_swiglu(h, what):
+    if h.dim() != 2 or h.shape[1] % 256:
+        raise ValueError(f"{what}: h must be [rows, 2 * inner] with inner a multiple of 128, got {tuple(h.shape)}")
+    rows, inner = h.shape[0], h.shape[1] // 2
+    _bf16_rows(h, f"{what} h", (rows, 2 * inner))
+    return rows, inner
+
+
+def swiglu_fwd(h, *, out=None):
+    """a = silu(g) o u for h = [g | u] (bf16 [rows, 2 inner], inner a multiple of 128): bf16 [rows, inner], computed in
+    fp32 and rounded once"""
+    rows, inner = _check_swiglu(h, "swiglu_fwd")
+    out = torch.empty(rows, inner, dtype=torch.bfloat16, device=h.device) if out is None else out
+    _bf16_rows(out, "swiglu_fwd out", (rows, inner))
+    native.check(_lib().lah_swiglu_fwd(ptr(h), ptr(out), rows, inner, stream_ptr()), "lah_swiglu_fwd")
+    native.count_launch()
+    return out
+
+
+def swiglu_bwd(da, h, *, out=None):
+    """dh = [da o u o s (1 + g (1 - s)) | da o silu(g)], s = sigmoid(g): bf16 [rows, 2 inner], the backward of
+    ``swiglu_fwd``"""
+    rows, inner = _check_swiglu(h, "swiglu_bwd")
+    _bf16_rows(da, "swiglu_bwd da", (rows, inner))
+    out = torch.empty_like(h) if out is None else out
+    _bf16_rows(out, "swiglu_bwd out", (rows, 2 * inner))
+    native.check(_lib().lah_swiglu_bwd(ptr(da), ptr(h), ptr(out), rows, inner, stream_ptr()), "lah_swiglu_bwd")
+    native.count_launch()
+    return out
+
+
+def swiglu_ref(h):
+    """oracle of ``swiglu_fwd`` in fp32 (fp64 for a fp64 input)"""
+    hf = h if h.dtype == torch.float64 else h.float()
+    g, u = hf.chunk(2, dim=-1)
+    return F.silu(g) * u
+
+
+def swiglu_bwd_ref(da, h):
+    """oracle of ``swiglu_bwd`` in fp32 (fp64 for a fp64 input)"""
+    hf = h if h.dtype == torch.float64 else h.float()
+    g, u = hf.chunk(2, dim=-1)
+    d = da.to(hf.dtype)
+    s = torch.sigmoid(g)
+    return torch.cat([d * u * s * (1 + g * (1 - s)), d * g * s], dim=-1)
 
 
 _PHILOX_M0, _PHILOX_M1, _PHILOX_W0, _PHILOX_W1 = 0xD2511F53, 0xCD9E8D57, 0x9E3779B9, 0xBB67AE85

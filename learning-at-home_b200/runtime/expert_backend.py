@@ -40,15 +40,19 @@ class ExpertBackend(nn.Module):
             d_model / nhead in (32, 64, 128), d_model a multiple of 128 with 256 <= d_model <= 4096, dim_feedforward a
             multiple of 128, dropout p < 1 at every site, sequence length 1 <= S <= 65536 (wgmma attention and GEMMs,
             in-kernel dropout, fused AMSGrad).  This package's layer with ``causal=True`` (position t attends to
-            positions <= t) runs natively under the same conditions, on the causal attention kernels.
+            positions <= t) runs natively under the same conditions, on the causal attention kernels;
+          * ``GatedFeedforwardBlock(hid, inner)`` (the SwiGLU expert MLP with its RMSNorm pre-norm and residual) with hid
+            a multiple of 128 in [128, 4096], inner any multiple of 128 (so up to hid 4096, inner 11008), no biases, an
+            RMSNorm with a weight, ``normalized_shape`` (hid,) and any eps > 0 (RMSNorm and SwiGLU kernels, one swap-AB GEMM
+            and one fused weight-gradient + AMSGrad launch over the adjacent [W1; W3]).
         ``torch.nn.TransformerEncoderLayer`` also runs natively with a key padding mask: one positional input and
         ``kwargs_schema={"src_key_padding_mask": BatchTensorProto(S, dtype=torch.bool)}`` (True = padding key, [batch, S]
         for sequence-first layers too).  The flat inputs are then (src, mask) for forward and (src, mask, grad_out) for
         backward, which returns (dx, zeros_like(mask)), as on the module.  A sequence whose keys are all masked gets the
         result of torch's layer in training mode (zero attention output) in eval mode too; torch's eval fast path returns
         NaN for it.
-        Anything else (another class, tanh GELU, kdim / vdim, bias=False, other widths or inputs, float masks, other
-        keyword inputs, CPU tensors) runs on the module itself"""
+        Anything else (another class, tanh GELU, kdim / vdim, bias=False in the encoder layers, biases in the gated block,
+        other widths or inputs, float masks, other keyword inputs, CPU tensors) runs on the module itself"""
         super().__init__()
         self.expert, self.opt, self.name = expert, opt, name
         self.native, self._executor, self._executor_key = native, None, None

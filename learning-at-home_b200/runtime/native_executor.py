@@ -8,6 +8,8 @@ hand-written sm_90a kernels instead of eager PyTorch, so that a ``TesseractServe
             expert's optimizer immediately, return the gradients w.r.t. the inputs — with swap-AB dgrads, the LayerNorm
             backward kernel and the FUSED weight-gradient + AMSGrad kernel (the gradient of a weight matrix never reaches HBM)
 
+NativeGatedFFNExecutor does the same for a ``GatedFeedforwardBlock`` (RMSNorm, one GEMM over [W1; W3], SwiGLU, W2) and
+NativeTransformerExecutor for encoder layers.
 The module's parameters and the torch optimizer's state tensors are re-bound as VIEWS of the executor's flat fp32 buffers:
 ``expert.state_dict()``, ``opt.state_dict()`` and ``ExpertBackend.checkpoint()`` stay live and keep the reference layout.
 """
@@ -17,12 +19,14 @@ from typing import List, NamedTuple, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-from ..models.layers import FFN_SEG_KEYS, FFN_SEG_NAMES, FFN_SMALL_SEG_MASK, FeedforwardBlock, TransformerEncoderLayer
+from ..models.layers import (FFN_SEG_KEYS, FFN_SEG_NAMES, FFN_SMALL_SEG_MASK, FeedforwardBlock, GatedFeedforwardBlock,
+                              TransformerEncoderLayer)
 from ..ops import kernels as K, native
 
 TORCH_ENCODER_LAYER = "torch.nn.modules.transformer.TransformerEncoderLayer"
 OWN_ENCODER_LAYER = "lah_b200.models.layers.TransformerEncoderLayer"
 OWN_FFN = "lah_b200.models.layers.FeedforwardBlock"
+OWN_GATED_FFN = "lah_b200.models.layers.GatedFeedforwardBlock"
 LN_EPS = 1e-5   # the LayerNorm epsilon compiled into csrc/layernorm.cu
 
 
@@ -34,7 +38,7 @@ def class_name(module) -> str:
     if type(module) is torch.jit.RecursiveScriptModule:
         name = module._c._type().qualified_name()
         return re.sub(r"___torch_mangle_\d+\.", "", name[len("__torch__."):] if name.startswith("__torch__.") else name)
-    for own in (TransformerEncoderLayer, FeedforwardBlock):
+    for own in (TransformerEncoderLayer, FeedforwardBlock, GatedFeedforwardBlock):
         if isinstance(module, own):
             return f"{own.__module__}.{own.__qualname__}"
     return f"{type(module).__module__}.{type(module).__qualname__}"
@@ -61,6 +65,29 @@ def ffn_spec(module) -> Optional[FFNSpec]:
     if class_name(module) != OWN_FFN:
         return None
     return FFNSpec(module.layers[0].in_features, module.layers[0].out_features)
+
+
+class GatedFFNSpec(NamedTuple):
+    hid: int
+    inner: int
+    eps: float
+
+
+def gated_ffn_spec(module) -> Optional[GatedFFNSpec]:
+    """what NativeGatedFFNExecutor needs of a GatedFeedforwardBlock (plain or scripted), or None when it cannot run it:
+    refused are a Linear with a bias, an RMSNorm without a weight, an eps that is None or <= 0, a ``normalized_shape``
+    other than (hid,), and every other class"""
+    if class_name(module) != OWN_GATED_FFN:
+        return None
+    norm, w1, w2, w3 = module.norm, module.w1, module.w2, module.w3
+    if any(lin.bias is not None for lin in (w1, w2, w3)) or norm.weight is None:
+        return None
+    if norm.eps is None or not float(norm.eps) > 0:
+        return None
+    hid, inner = int(w1.in_features), int(w1.out_features)
+    if tuple(norm.normalized_shape) != (hid,):
+        return None
+    return GatedFFNSpec(hid, inner, float(norm.eps))
 
 
 def _activation(layer) -> Optional[str]:
@@ -229,7 +256,7 @@ class FlatAdamState:
 
 
 def _runs_natively(params, opt) -> bool:
-    """what both executors ask of the segment parameters and the optimizer: fp32 CUDA parameters, an optimizer
+    """what every executor asks of the segment parameters and the optimizer: fp32 CUDA parameters, an optimizer
     ``optimizer_groups`` accepts, and the compiled kernels"""
     if not params[0].is_cuda or params[0].dtype != torch.float32:
         return False
@@ -350,6 +377,141 @@ class NativeFFNExecutor:
         K.swapab_linear(self.dh, bv["w1"], go, gr, out=self.dxd, w_is_kn=True, residual=self.gyd)
         wgrad("w1", self.dh, self.xd)
         st.adam_step(FFN_SMALL_SEG_MASK)   # the small vectors
+        st.end_step()
+        return self.dxd[:rows].to(x.dtype)
+
+
+class NativeGatedFFNExecutor:
+    """
+    Trainable sm_90a ``GatedFeedforwardBlock(hid, inner)`` expert (``gated_ffn_spec``) for hid a multiple of 128 in
+    [128, K.LN_MAX_WIDTH = 4096] (the RMSNorm kernels' widest row) and inner any multiple of 128, so up to the Llama-7B
+    shape hid 4096, inner 11008.  Rows are padded to a multiple of 16 with zero rows, as in NativeFFNExecutor.
+
+      forward   xd = bf16(x);  n, rstd = RMSNorm(xd);  h = [g | u] = n [W1; W3]^T (one swap-AB GEMM);  a = silu(g) o u;
+                y = a W2^T + xd (swap-AB GEMM, residual in its epilogue)
+      backward  the reference semantics (recompute the forward, one optimizer step, return dx):
+                da = gy W2 (swap-AB dgrad);  W2 <- fused wgrad + AMSGrad(gy, a)
+                dh = SwiGLU backward(da, h)
+                dn = dh [W1; W3] (one dgrad);  [W1; W3] <- fused wgrad + AMSGrad(dh, n)
+                dx = gy + RMSNorm backward(dn) (the residual gradient added before the one rounding), dgamma into the
+                gradient buffer;  Adam step of the norm segment
+
+    The flat buffers hold the segments ("g", "w1", "w3", "w2"): w1 and w3 are adjacent in p, m, v, vmax and the bf16
+    mirror, so [W1; W3] is one contiguous [2 inner, hid] matrix, which takes one GEMM forward, one dgrad and, when w1 and
+    w3 are in the same param group, one fused wgrad + AMSGrad launch (two launches, one per half of dh, when they are not).
+    Module parameters and optimizer state are views of the flat buffers (``FlatAdamState``).
+
+    Padding rows contribute exactly zero to every gradient: their gy is zero, so their rows of da, dh and dn are zero (the
+    GEMMs write the padding rows of a 16-row block from zero inputs, and SwiGLU backward of da = 0 is 0), and the RMSNorm
+    backward of a zero row with a zero dn adds nothing to dgamma.
+    """
+    NAMES = ("g", "w1", "w3", "w2")
+    INPUT_DIMS = 2   # [rows, hid]
+
+    def accepts(self, x) -> bool:
+        """True when ``x`` is an input this executor runs: [rows, hid]"""
+        return x.dim() == self.INPUT_DIMS and x.shape[1] == self.hid
+
+    @staticmethod
+    def supports(expert, opt) -> bool:
+        spec = gated_ffn_spec(expert)
+        if spec is None or not torch.cuda.is_available():
+            return False
+        if spec.hid % 128 or not 128 <= spec.hid <= K.LN_MAX_WIDTH or spec.inner <= 0 or spec.inner % 128:
+            return False
+        return _runs_natively(NativeGatedFFNExecutor._segment_params(expert), opt)
+
+    @staticmethod
+    def _segment_params(expert):
+        """the parameters in the order of NAMES (the segments of the flat buffers)"""
+        return [expert.norm.weight, expert.w1.weight, expert.w3.weight, expert.w2.weight]
+
+    def __init__(self, expert, opt):
+        self.expert, self.opt = expert, opt
+        spec = gated_ffn_spec(expert)
+        self.hid, self.inner, self.eps = spec.hid, spec.inner, spec.eps
+        params = self._segment_params(expert)
+        self.device = params[0].device
+        self.state = st = FlatAdamState(opt, params, self.NAMES, self.device)
+        self.p, self.m = st.p, st.m   # the flat parameter and exp_avg buffers
+        H, I = self.hid, self.inner
+        # [W1; W3] in every flat buffer: the two segments after the norm's
+        self.w13 = {name: flat[H: H + 2 * I * H].view(1, 2 * I, H)
+                    for name, flat in (("p", st.p), ("m", st.m), ("v", st.v), ("vmax", st.vmax), ("bf16", st.p_bf16))}
+        self.group_off = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.group_rows = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self._cap = 0
+
+    def bind(self):
+        """re-bind after the module or the optimizer was loaded from a checkpoint (``FlatAdamState.bind``)"""
+        self.state.bind()
+
+    def _workspace(self, rows: int):
+        cap = (rows + ALIGN - 1) // ALIGN * ALIGN
+        if cap > self._cap:
+            cap = max(cap, 2 * self._cap, 128)
+            bf = dict(dtype=torch.bfloat16, device=self.device)
+            H, I = self.hid, self.inner
+            self.xd, self.n, self.yo, self.gyd, self.dn, self.dxd = (torch.zeros(cap, H, **bf) for _ in range(6))
+            self.h, self.dh = torch.zeros(cap, 2 * I, **bf), torch.zeros(cap, 2 * I, **bf)
+            self.a, self.da = torch.zeros(cap, I, **bf), torch.zeros(cap, I, **bf)
+            self.rstd = torch.zeros(cap, device=self.device)
+            self._cap = cap
+        self.group_rows.fill_(rows)
+        return (rows + ALIGN - 1) // ALIGN * ALIGN
+
+    def _forward(self, x: torch.Tensor):
+        rows = x.shape[0]
+        padded = self._workspace(rows)
+        self.xd[:rows].copy_(x)
+        if padded > rows:
+            self.xd[rows:padded].zero_()
+        go, gr, pv, bv = self.group_off, self.group_rows, self.state.pv, self.state.bv
+        K.rms_norm_fwd(self.xd[:padded], pv["g"][0], self.eps, out=self.n[:padded], rstd=self.rstd[:padded])
+        K.swapab_linear(self.n, self.w13["bf16"], go, gr, out=self.h)
+        K.swiglu_fwd(self.h[:padded], out=self.a[:padded])
+        K.swapab_linear(self.a, bv["w2"], go, gr, out=self.yo, residual=self.xd)
+        return rows, padded
+
+    @torch.no_grad()
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        rows, _ = self._forward(x)
+        return self.yo[:rows].to(x.dtype)
+
+    @torch.no_grad()
+    def backward(self, x: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
+        """recompute forward, back-propagate, ONE optimizer step (reference: expert_backend.py:73-97); returns dL/dx"""
+        rows, padded = self._forward(x)
+        self.gyd[:rows].copy_(grad_out)
+        if padded > rows:
+            self.gyd[rows:padded].zero_()
+        st = self.state
+        go, gr, pv, bv, gv, I = self.group_off, self.group_rows, st.pv, st.bv, st.gv, self.inner
+        hypers = st.hypers()
+        group_of = {name: k for k, (_, mask) in enumerate(hypers) for s, name in enumerate(st.names) if (mask >> s) & 1}
+        st.begin_step()
+
+        def wgrad(dy, xin, name, p, m, v, vmax, p_bf16):   # with the settings of the group that holds segment `name`
+            hyper = hypers[group_of[name]][0]
+            K.wgrad_adam(dy, xin, go, gr, p=p, m=m, v=v, vmax=vmax if hyper["amsgrad"] else None, p_bf16=p_bf16,
+                         step=st.step, **hyper)
+
+        def seg(name):
+            return st.pv[name], st.mv[name], st.vv[name], st.vmv[name], bv[name]
+
+        K.swapab_linear(self.gyd, bv["w2"], go, gr, out=self.da, w_is_kn=True)
+        wgrad(self.gyd, self.a, "w2", *seg("w2"))
+        K.swiglu_bwd(self.da[:padded], self.h[:padded], out=self.dh[:padded])
+        K.swapab_linear(self.dh, self.w13["bf16"], go, gr, out=self.dn, w_is_kn=True)
+        if group_of["w1"] == group_of["w3"]:
+            w = self.w13
+            wgrad(self.dh, self.n, "w1", w["p"], w["m"], w["v"], w["vmax"], w["bf16"])
+        else:
+            wgrad(self.dh[:, :I], self.n, "w1", *seg("w1"))
+            wgrad(self.dh[:, I:], self.n, "w3", *seg("w3"))
+        K.rms_norm_bwd(self.dn[:padded], self.xd[:padded], self.rstd[:padded], pv["g"][0], dx=self.dxd[:padded],
+                       dgamma=gv["g"][0], dres=self.gyd[:padded], tile_rows=ALIGN)
+        st.adam_step(1 << self.NAMES.index("g"))
         st.end_step()
         return self.dxd[:rows].to(x.dtype)
 
@@ -651,6 +813,8 @@ def make_executor(expert, opt):
             return NativeTransformerExecutor(expert, opt)
         if NativeFFNExecutor.supports(expert, opt):
             return NativeFFNExecutor(expert, opt)
+        if NativeGatedFFNExecutor.supports(expert, opt):
+            return NativeGatedFFNExecutor(expert, opt)
     except Exception as e:  # noqa: an executor that cannot be built must not break the server; eager PyTorch still works
         print(f"[lah_b200] native expert executor unavailable ({type(e).__name__}: {e}); using eager PyTorch", flush=True)
     return None
