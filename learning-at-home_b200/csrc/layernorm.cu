@@ -370,7 +370,7 @@ __global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS)
 }
 
 // ------------------------------------------------------------------------------------------------
-// RMSNorm, the pre-norm of GatedFeedforwardBlock (one expert: gamma is [C], no tile groups).
+// RMSNorm, the pre-norm of GatedFeedforwardBlock (one expert: gamma is [C]; GROUPED below: one gamma per expert).
 //   forward   n = x * rstd * gamma,  rstd = 1 / sqrt(mean(x^2) + eps) saved per row (fp32); eps is an argument
 //   backward  dx = dres + rstd * (gamma o dn - x * mean(gamma o dn o x) * rstd^2)   (one rounding, dres optional)
 //             dgamma += column sums of dn o x * rstd, per tile into part[tile][C], added in tile order by
@@ -378,6 +378,11 @@ __global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS)
 // They are separate kernels, not a flag of the LayerNorm ones: those take no eps argument, and giving them one would change
 // the code of every LayerNorm instantiation.  They share the LayerNorm sizing: the chunks per lane of LnFwdCfg (rows per
 // warp: RmsFwdCfg below) and the CTA shape and rows per batch of LnBwdCfg.
+// GROUPED (the DMoE engine's gated expert): rows are grouped by expert in tiles of 2^tile_shift rows (backward: tile_rows),
+// gamma is [G, C] and tile t uses gamma[tile_group[t]]; tiles with group -1 are skipped (nothing is stored for their
+// rows).  The backward's per-tile dgamma partials go through group_tile_sum_kernel with tile_group, so dgamma[g] is summed in
+// tile order.  tile_group (and tile_shift) are the LAST parameters, read only when GROUPED, so that the single-gamma
+// instantiations keep the parameter layout, and the code, they had before the flag existed.
 // ------------------------------------------------------------------------------------------------
 // Rows per warp: the LayerNorm rule for the widths it was not tuned at (R = 4 up to NV = 2, 2 up to NV = 6, else 1), at
 // every width; the tuned power-of-two configurations hold 2-4x the rows and spill here.  Above NV = 11 one row no longer
@@ -389,16 +394,23 @@ struct RmsFwdCfg {
     static constexpr int MIN_BLOCKS = NV <= 11 ? 2 : 1;
 };
 
-template <int C, int R>
+template <int C, int R, bool GROUPED>
 __global__ void __launch_bounds__(256, RmsFwdCfg<C>::MIN_BLOCKS) rms_norm_fwd_kernel(
     const bf16* __restrict__ x, bf16* __restrict__ n, float* __restrict__ rstd_out, const float* __restrict__ gamma,
-    int rows, float eps) {
+    int rows, float eps, const int* __restrict__ tile_group, int tile_shift) {
     constexpr int NV = LnFwdCfg<C>::NV;
     constexpr bool HALF = C % 256 != 0;
     static_assert(C % 128 == 0 && C <= LN_MAX_C, "unsupported RMSNorm width");
+    // a warp's R rows lie in one tile: row0 is a multiple of R, and R (a power of two <= 4) divides every tile size (>= 8)
+    static_assert(R == 1 || R == 2 || R == 4, "rows per warp must divide the smallest tile (8 rows)");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int row0 = (blockIdx.x * 8 + warp) * R;
     if (row0 >= rows) return;
+    if constexpr (GROUPED) {
+        const int g = __ldg(tile_group + (row0 >> tile_shift));
+        if (g < 0) return;
+        gamma += static_cast<long long>(g) * C;
+    }
     int4 q[R][NV];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
@@ -463,11 +475,11 @@ __global__ void __launch_bounds__(256, RmsFwdCfg<C>::MIN_BLOCKS) rms_norm_fwd_ke
     }
 }
 
-template <int C, bool RES>
+template <int C, bool RES, bool GROUPED>
 __global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS) rms_norm_bwd_kernel(
     const bf16* __restrict__ dn, const bf16* __restrict__ x, const float* __restrict__ rstd_in,
     const float* __restrict__ gamma, bf16* __restrict__ dx, float* __restrict__ part, int rows, int tile_rows,
-    const bf16* __restrict__ dres) {
+    const bf16* __restrict__ dres, const int* __restrict__ tile_group) {
     constexpr int THREADS = LnBwdCfg<C>::THREADS;
     constexpr int WARPS = THREADS / 32;
     constexpr bool IDLE = THREADS * 8 != C;
@@ -476,6 +488,11 @@ __global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS)
     __shared__ float red[WARPS][RB];
     __shared__ float tot[RB];
     const int tile = blockIdx.x;
+    if constexpr (GROUPED) {   // an unused tile writes no partial: group_tile_sum_kernel skips it by its group -1
+        const int g = __ldg(tile_group + tile);
+        if (g < 0) return;
+        gamma += static_cast<long long>(g) * C;
+    }
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int col = tid * 8;
     const bool live = !IDLE || col < C;
@@ -701,29 +718,47 @@ constexpr auto ln_bwd_table(std::integer_sequence<int, I...>) {
 constexpr auto kLnFwd = ln_fwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
 constexpr auto kLnBwd = ln_bwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
 
-using RmsFwdLaunch = void (*)(const void*, void*, float*, const float*, int, float, cudaStream_t);
+using RmsFwdLaunch = void (*)(const void*, void*, float*, const float*, int, float, const int*, int, cudaStream_t);
 using RmsBwdLaunch = void (*)(const void*, const void*, const float*, const float*, void*, float*, float*, int, int,
-                              const void*, cudaStream_t);
+                              const void*, const int*, cudaStream_t);
 
 template <int C>
-void rms_fwd_launch(const void* x, void* n, float* rstd, const float* gamma, int rows, float eps, cudaStream_t st) {
+void rms_fwd_launch(const void* x, void* n, float* rstd, const float* gamma, int rows, float eps, const int* tile_group,
+                    int tile_shift, cudaStream_t st) {
     constexpr int RR = RmsFwdCfg<C>::R;
-    rms_norm_fwd_kernel<C, RR><<<(rows + 8 * RR - 1) / (8 * RR), 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma,
-                                                                               rows, eps);
+    const int grid = (rows + 8 * RR - 1) / (8 * RR);
+    if (tile_group)
+        rms_norm_fwd_kernel<C, RR, true><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
+                                                               tile_group, tile_shift);
+    else
+        rms_norm_fwd_kernel<C, RR, false><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
+                                                                nullptr, 0);
+}
+
+template <int C, bool GROUPED>
+void rms_bwd_kernel_launch(int grid, const void* dn, const void* x, const float* rstd, const float* gamma, void* dx,
+                           float* part, int rows, int tile_rows, const void* dres, const int* tile_group,
+                           cudaStream_t st) {
+    constexpr int T = LnBwdCfg<C>::THREADS;
+    if (dres)
+        rms_norm_bwd_kernel<C, true, GROUPED><<<grid, T, 0, st>>>((const bf16*)dn, (const bf16*)x, rstd, gamma,
+                                                                  (bf16*)dx, part, rows, tile_rows, (const bf16*)dres,
+                                                                  tile_group);
+    else
+        rms_norm_bwd_kernel<C, false, GROUPED><<<grid, T, 0, st>>>((const bf16*)dn, (const bf16*)x, rstd, gamma,
+                                                                   (bf16*)dx, part, rows, tile_rows, nullptr,
+                                                                   tile_group);
 }
 
 template <int C>
 void rms_bwd_launch(const void* dn, const void* x, const float* rstd, const float* gamma, void* dx, float* dgamma,
-                    float* part, int rows, int tile_rows, const void* dres, cudaStream_t st) {
+                    float* part, int rows, int tile_rows, const void* dres, const int* tile_group, cudaStream_t st) {
     const int grid = (rows + tile_rows - 1) / tile_rows;
-    constexpr int T = LnBwdCfg<C>::THREADS;
-    if (dres)
-        rms_norm_bwd_kernel<C, true><<<grid, T, 0, st>>>((const bf16*)dn, (const bf16*)x, rstd, gamma, (bf16*)dx, part,
-                                                         rows, tile_rows, (const bf16*)dres);
+    if (tile_group)
+        rms_bwd_kernel_launch<C, true>(grid, dn, x, rstd, gamma, dx, part, rows, tile_rows, dres, tile_group, st);
     else
-        rms_norm_bwd_kernel<C, false><<<grid, T, 0, st>>>((const bf16*)dn, (const bf16*)x, rstd, gamma, (bf16*)dx, part,
-                                                          rows, tile_rows, nullptr);
-    group_tile_sum_kernel<<<(C + 255) / 256, 256, 0, st>>>(part, grid, 1, C, nullptr, dgamma, nullptr, nullptr);
+        rms_bwd_kernel_launch<C, false>(grid, dn, x, rstd, gamma, dx, part, rows, tile_rows, dres, nullptr, st);
+    group_tile_sum_kernel<<<(C + 255) / 256, 256, 0, st>>>(part, grid, 1, C, tile_group, dgamma, nullptr, nullptr);
 }
 
 template <int... I>
@@ -794,22 +829,27 @@ int lah_ln_relu_bwd(const void* da, const void* h, const float* mean, const floa
     return -(int)cudaGetLastError();
 }
 
-// RMSNorm forward over [rows, C] bf16 (n: [rows, C] bf16, rstd: [rows] fp32, gamma: [C] fp32); eps > 0
+// RMSNorm forward over [rows, C] bf16 (n: [rows, C] bf16, rstd: [rows] fp32, gamma: [C] fp32); eps > 0.
+// tile_group: NULL (one gamma), or the expert of every tile of tile_rows rows (power of two >= 8); gamma is then [G, C]
+// and the rows of tiles with group -1 are not written
 int lah_rms_norm_fwd(const void* x, void* n, float* rstd, const float* gamma, int rows, int C, float eps,
-                     cudaStream_t st) {
+                     const int* tile_group, int tile_rows, cudaStream_t st) {
     if (rows <= 0) return 0;
-    if (!ln_width_ok(C) || !(eps > 0.f)) return -2;
-    kRmsFwd[C / 128 - 1](x, n, rstd, gamma, rows, eps, st);
+    const int tile_shift = tile_group ? shift_of(tile_rows) : 0;
+    if (!ln_width_ok(C) || !(eps > 0.f) || tile_shift < 0) return -2;
+    kRmsFwd[C / 128 - 1](x, n, rstd, gamma, rows, eps, tile_group, tile_shift, st);
     return -(int)cudaGetLastError();
 }
 
 // RMSNorm backward: dx [rows, C] bf16, dgamma [C] fp32 (+=); part: scratch of [ceil(rows / tile_rows), C] fp32;
-// dres: optional [rows, C] bf16 gradient of a residual that bypasses the norm, added to dx before its rounding; NULL = none
+// dres: optional [rows, C] bf16 gradient of a residual that bypasses the norm, added to dx before its rounding; NULL = none.
+// tile_group: NULL, or the expert of every tile (gamma and dgamma [G, C]; tiles with group -1 are skipped)
 int lah_rms_norm_bwd(const void* dn, const void* x, const float* rstd, const float* gamma, void* dx, float* dgamma,
-                     float* part, int rows, int C, int tile_rows, const void* dres, cudaStream_t st) {
+                     float* part, int rows, int C, int tile_rows, const void* dres, const int* tile_group,
+                     cudaStream_t st) {
     if (rows <= 0) return 0;
     if (shift_of(tile_rows) < 0 || !ln_width_ok(C)) return -2;
-    kRmsBwd[C / 128 - 1](dn, x, rstd, gamma, dx, dgamma, part, rows, tile_rows, dres, st);
+    kRmsBwd[C / 128 - 1](dn, x, rstd, gamma, dx, dgamma, part, rows, tile_rows, dres, tile_group, st);
     return -(int)cudaGetLastError();
 }
 

@@ -57,6 +57,67 @@ FFN_SEG_NAMES = tuple(FFN_SEG_KEYS)
 FFN_SMALL_SEG_MASK = sum(1 << s for s, n in enumerate(FFN_SEG_NAMES) if not n.startswith("w"))
 
 
+class ExpertLayout:
+    """How the DMoE engine (``parallel/engine.py``) keeps one expert kind in its flat ``[slots, *shape]`` segments.
+
+    * ``keys``: segment -> the module's state_dict keys it holds, stacked by rows (``[W1; W3]`` is one segment, so the two
+      matrices are contiguous per expert and take one GEMM, one dgrad and one fused wgrad + AMSGrad launch);
+    * ``params``: the module's parameter keys in ``parameters()`` order (the indices of its optimizer state);
+    * ``shapes(hidden, inner)``: segment -> per-expert shape, in segment order;
+    * ``small_mask``: bit s set = segment s is a vector (norm / bias), stepped by ``adam_step``, pulled from fp32 into
+      shadow slots, zeroed before a shadow gradient reduce; the matrices are stepped by the fused wgrad + AMSGrad kernel;
+    * ``buffers(hidden, inner)``: the engine's bf16 row buffers of the kind (see ``LayerWorkspace``).
+    """
+
+    def __init__(self, keys, params, shapes, buffers):
+        self.keys = dict(keys)
+        self.names = tuple(self.keys)
+        self.params = tuple(params)
+        self.shapes = shapes
+        self.buffers = buffers
+        self.small_mask = sum(1 << s for s, n in enumerate(self.names) if not n.startswith("w"))
+        # parameter key -> (segment, row block, blocks in the segment)
+        self.slices = {key: (n, i, len(ks)) for n, ks in self.keys.items() for i, key in enumerate(ks)}
+        assert sorted(self.slices) == sorted(self.params)
+
+    def module_state(self, segments):
+        """segment -> tensor of one expert  =>  the module's state_dict (in ``params`` order)"""
+        out = {}
+        for key in self.params:
+            n, i, parts = self.slices[key]
+            out[key] = segments[n].chunk(parts, 0)[i] if parts > 1 else segments[n]
+        return out
+
+    def segment_state(self, state, prefix=""):
+        """a module's state_dict  =>  segment -> tensor of one expert (row blocks joined)"""
+        return {n: torch.cat([state[prefix + k] for k in ks], 0) if len(ks) > 1 else state[prefix + ks[0]]
+                for n, ks in self.keys.items()}
+
+
+# buffers(H, I): "rows": bf16 [rows, width] activations kept per layer until the backward; "stats": fp32 [rows] per layer;
+# "scratch": bf16 [rows, width] backward temporaries shared by all layers; "per_layer": backward buffers read by the fused
+# wgrad + AMSGrad launches of the optimizer stream, per layer when that stream is used (else the scratch buffer named)
+FFN_LAYOUT = ExpertLayout(
+    keys={n: (k,) for n, k in FFN_SEG_KEYS.items()}, params=tuple(FFN_SEG_KEYS.values()),
+    shapes=lambda H, I: {"w1": (I, H), "b1": (I,), "g1": (I,), "be1": (I,), "w2": (I, I), "b2": (I,), "g2": (I,),
+                         "be2": (I,), "w3": (H, I), "b3": (H,)},
+    buffers=lambda H, I: dict(rows={"h1": I, "a1": I, "h2": I, "a2": I}, stats=("mean1", "rstd1", "mean2", "rstd2"),
+                              scratch={"da": I, "dh": I}, per_layer={"dh2": "dh", "dh1": "dh"}))
+assert FFN_LAYOUT.names == FFN_SEG_NAMES and FFN_LAYOUT.small_mask == FFN_SMALL_SEG_MASK
+
+#: GatedFeedforwardBlock in the engine: the RMSNorm weight, [W1; W3] ([2 inner, hid]: W1 rows [0, inner), W3 rows
+#: [inner, 2 inner)) and W2; the keys and parameter order are a Mixtral expert's
+GATED_LAYOUT = ExpertLayout(
+    keys={"g": ("norm.weight",), "w13": ("w1.weight", "w3.weight"), "w2": ("w2.weight",)},
+    params=("norm.weight", "w1.weight", "w2.weight", "w3.weight"),
+    shapes=lambda H, I: {"g": (H,), "w13": (2 * I, H), "w2": (H, I)},
+    buffers=lambda H, I: dict(rows={"n": H, "h": 2 * I, "a": I}, stats=("rstd",),
+                              scratch={"da": I, "dh": 2 * I, "dn": H}, per_layer={"dh13": "dh"}))
+
+#: the layout of every expert kind the engine trains, by its ``name_to_block`` key
+EXPERT_LAYOUTS = {"ffn": FFN_LAYOUT, "swiglu": GATED_LAYOUT}
+
+
 def gated_inner_dim(hid_dim: int) -> int:
     """the default inner width of GatedFeedforwardBlock: 8 hid / 3 rounded up to a multiple of 128 (Llama's convention;
     2816 at hid 1024, 11008 at hid 4096), the parameter count of a 4 hid MLP"""

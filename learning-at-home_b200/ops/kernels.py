@@ -62,8 +62,8 @@ def _lib():
         "lah_pack_key_mask": [P, P, L, I, P],
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
-        "lah_rms_norm_fwd": [P, P, P, P, I, I, Fl, P],
-        "lah_rms_norm_bwd": [P, P, P, P, P, P, P, I, I, I, P, P],
+        "lah_rms_norm_fwd": [P, P, P, P, I, I, Fl, P, I, P],
+        "lah_rms_norm_bwd": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_swiglu_fwd": [P, P, L, I, P],
         "lah_swiglu_bwd": [P, P, P, L, I, P],
         "lah_symm_alloc": [c_ull, ctypes.POINTER(c_void_p)],
@@ -145,45 +145,98 @@ def _f32_vec(t, what, n):
         raise ValueError(f"{what}: expected a contiguous float32 tensor of {n} elements, got {t.dtype} {tuple(t.shape)}")
 
 
-def rms_norm_fwd(x, gamma, eps, *, out, rstd):
+def _check_rms_groups(what, gamma, tile_group, tile_rows, rows, C):
+    """gamma of a grouped RMSNorm call: [G, C] with one row per group; tile_group: int32, one entry per tile_rows rows"""
+    if tile_rows < 8 or tile_rows & (tile_rows - 1):
+        raise ValueError(f"{what}: tile_rows must be a power of two >= 8, got {tile_rows}")
+    if tile_group is None:
+        return 1
+    tiles = (rows + tile_rows - 1) // tile_rows
+    if tile_group.dtype != torch.int32 or not tile_group.is_contiguous() or tile_group.numel() < tiles:
+        raise ValueError(f"{what}: tile_group must be a contiguous int32 tensor of >= {tiles} entries, got "
+                         f"{tile_group.dtype} {tuple(tile_group.shape)}")
+    if gamma.numel() % C or gamma.numel() == 0:
+        raise ValueError(f"{what}: grouped gamma must be [G, {C}], got {tuple(gamma.shape)}")
+    return gamma.numel() // C
+
+
+def rms_norm_fwd(x, gamma, eps, *, out, rstd, tile_group=None, tile_rows=16):
     """RMSNorm over the rows of x (csrc/layernorm.cu): out = bf16(x * rstd * gamma), rstd[r] = 1 / sqrt(mean(x_r^2) + eps)
-    kept in fp32.  x, out: bf16 [rows, C] with C in LN_WIDTHS; gamma: fp32 [C]; rstd: fp32 [rows]; eps > 0"""
+    kept in fp32.  x, out: bf16 [rows, C] with C in LN_WIDTHS; gamma: fp32 [C]; rstd: fp32 [rows]; eps > 0.
+    With ``tile_group`` (int32, the group of every ``tile_rows`` rows, -1 = unused) gamma is fp32 [G, C] and the rows of
+    tile t are normalised with gamma[tile_group[t]]; the rows of -1 tiles are left as they were"""
     if x.dim() != 2:
         raise ValueError(f"rms_norm_fwd: x must be [rows, C], got {tuple(x.shape)}")
     rows, C = x.shape
     _check_ln_width(C, "rms_norm_fwd")
     _bf16_rows(x, "rms_norm_fwd x", (rows, C))
     _bf16_rows(out, "rms_norm_fwd out", (rows, C))
-    _f32_vec(gamma, "rms_norm_fwd gamma", C)
+    G = _check_rms_groups("rms_norm_fwd", gamma, tile_group, tile_rows, rows, C)
+    _f32_vec(gamma, "rms_norm_fwd gamma", G * C)
     _f32_vec(rstd, "rms_norm_fwd rstd", rows)
     if not eps > 0:
         raise ValueError(f"rms_norm_fwd: eps must be > 0, got {eps}")
-    native.check(_lib().lah_rms_norm_fwd(ptr(x), ptr(out), ptr(rstd), ptr(gamma), rows, C, float(eps), stream_ptr()),
-                 "lah_rms_norm_fwd")
+    native.check(_lib().lah_rms_norm_fwd(ptr(x), ptr(out), ptr(rstd), ptr(gamma), rows, C, float(eps), ptr(tile_group),
+                                         int(tile_rows), stream_ptr()), "lah_rms_norm_fwd")
     native.count_launch()
     return out
 
 
-def rms_norm_bwd(dn, x, rstd, gamma, *, dx, dgamma, dres=None, tile_rows=16):
+def rms_norm_bwd(dn, x, rstd, gamma, *, dx, dgamma, dres=None, tile_rows=16, tile_group=None):
     """backward of ``rms_norm_fwd``: dx = dres + rstd (gamma o dn - x mean(gamma o dn o x) rstd^2), rounded once;
     dgamma (+)= the column sums of dn o x rstd, per ``tile_rows`` rows (a power of two >= 8) and then in tile order
-    (run-to-run identical).  dres: optional bf16 [rows, C] gradient of a residual that bypasses the norm"""
+    (run-to-run identical).  dres: optional bf16 [rows, C] gradient of a residual that bypasses the norm.
+    With ``tile_group`` gamma and dgamma are fp32 [G, C]: tile t uses gamma[g] and adds into dgamma[g], g = tile_group[t];
+    -1 tiles are skipped (their rows of dx are not written)"""
     if x.dim() != 2:
         raise ValueError(f"rms_norm_bwd: x must be [rows, C], got {tuple(x.shape)}")
     rows, C = x.shape
     _check_ln_width(C, "rms_norm_bwd")
     for t, what in ((dn, "dn"), (x, "x"), (dx, "dx")) + (((dres, "dres"),) if dres is not None else ()):
         _bf16_rows(t, f"rms_norm_bwd {what}", (rows, C))
-    _f32_vec(gamma, "rms_norm_bwd gamma", C)
-    _f32_vec(dgamma, "rms_norm_bwd dgamma", C)
+    G = _check_rms_groups("rms_norm_bwd", gamma, tile_group, tile_rows, rows, C)
+    _f32_vec(gamma, "rms_norm_bwd gamma", G * C)
+    _f32_vec(dgamma, "rms_norm_bwd dgamma", G * C)
     _f32_vec(rstd, "rms_norm_bwd rstd", rows)
-    if tile_rows < 8 or tile_rows & (tile_rows - 1):
-        raise ValueError(f"rms_norm_bwd: tile_rows must be a power of two >= 8, got {tile_rows}")
     part = torch.empty((rows + tile_rows - 1) // tile_rows, C, device=x.device, dtype=torch.float32)
     native.check(_lib().lah_rms_norm_bwd(ptr(dn), ptr(x), ptr(rstd), ptr(gamma), ptr(dx), ptr(dgamma), ptr(part), rows, C,
-                                         int(tile_rows), ptr(dres), stream_ptr()), "lah_rms_norm_bwd")
+                                         int(tile_rows), ptr(dres), ptr(tile_group), stream_ptr()), "lah_rms_norm_bwd")
     native.count_launch(2)
     return dx
+
+
+def _tile_rows_of(tile_group, tile_rows, rows):
+    """the group of every row (-1: an unused tile) from the per-tile table"""
+    return tile_group.long().repeat_interleave(tile_rows)[:rows]
+
+
+def rms_norm_grouped_fwd_ref(x, gamma, eps, tile_group, tile_rows):
+    """oracle of the grouped ``rms_norm_fwd`` in fp32 (fp64 for a fp64 input): (n, rstd); rows of -1 tiles are 0 in n"""
+    xf = x if x.dtype == torch.float64 else x.float()
+    g = _tile_rows_of(tile_group.cpu(), tile_rows, x.shape[0]).to(x.device)
+    live = (g >= 0)[:, None]
+    gam = gamma.reshape(-1, x.shape[1]).to(xf.dtype)[g.clamp(min=0)]
+    n, rstd = rms_norm_fwd_ref(xf, torch.ones(x.shape[1], dtype=xf.dtype, device=x.device), eps)
+    return torch.where(live, n * gam, torch.zeros_like(n)), rstd
+
+
+def rms_norm_grouped_bwd_ref(dn, x, gamma, eps, tile_group, tile_rows, dres=None):
+    """oracle of the grouped ``rms_norm_bwd`` in fp32 (fp64 for a fp64 input): (dx, dgamma [G, C]); rows of -1 tiles are
+    0 in dx and add nothing to dgamma"""
+    xf = x if x.dtype == torch.float64 else x.float()
+    C = x.shape[1]
+    gam = gamma.reshape(-1, C).to(xf.dtype)
+    g = _tile_rows_of(tile_group.cpu(), tile_rows, x.shape[0]).to(x.device)
+    live = g >= 0
+    d = dn.to(xf.dtype) * live[:, None]
+    gr = gam[g.clamp(min=0)]
+    rstd = torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)
+    dx = rstd * (gr * d - xf * (gr * d * xf).mean(-1, keepdim=True) * rstd * rstd)
+    if dres is not None:
+        dx = dx + dres.to(xf.dtype)
+    dx = dx * live[:, None]
+    dgamma = torch.zeros_like(gam).index_add_(0, g[live], (d * xf * rstd)[live])
+    return dx, dgamma
 
 
 def rms_norm_fwd_ref(x, gamma, eps):

@@ -4,7 +4,8 @@ gloo on CPU) + cuBLAS ``F.linear`` + ``torch.optim.Adam`` per expert.  "A path t
 baseline, not the product" (BASELINE.json) — this module exists to be measured against (``bench.py --impl baseline``)
 and as a second, independently written oracle for the fused engine (same routing, same maths, autograd everywhere).
 
-Experts are real ``FeedforwardBlock`` modules (reference architecture, /root/reference/experiments/throughput/layers.py).
+Experts are real ``FeedforwardBlock`` modules (reference architecture, /root/reference/experiments/throughput/layers.py),
+or ``GatedFeedforwardBlock`` modules with ``DMoEConfig(expert="swiglu")``.
 """
 import math
 from typing import List, Optional
@@ -14,9 +15,9 @@ import torch.distributed as dist
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..models.layers import FeedforwardBlock
+from ..models.layers import FeedforwardBlock, GatedFeedforwardBlock
 from ..ops.kernels import product_key_scores
-from .engine import DMoEConfig, REF_KEYS, SEG_NAMES
+from .engine import GATED_EPS, DMoEConfig
 
 
 class _AllToAll(torch.autograd.Function):
@@ -57,7 +58,8 @@ class BaselineDMoE(nn.Module):
         for le in range(self.E_loc):  # per-(layer, global expert) seed: identical weights for any number of ranks
             with torch.random.fork_rng(devices=[]):
                 torch.manual_seed(cfg.seed * 1000003 + layer_index * 10007 + self.first_expert + le)
-                experts.append(FeedforwardBlock(cfg.hidden))
+                experts.append(GatedFeedforwardBlock(cfg.hidden, cfg.inner, eps=GATED_EPS) if cfg.expert == "swiglu"
+                               else FeedforwardBlock(cfg.hidden))
         self.experts = nn.ModuleList(experts)
         if device is not None:
             self.to(device)
@@ -71,8 +73,7 @@ class BaselineDMoE(nn.Module):
         """copy the parameters of a fused-engine ExpertShard (same rank / same experts)"""
         with torch.no_grad():
             for le, expert in enumerate(self.experts):
-                state = {REF_KEYS[n]: shard.views[n][le] for n in SEG_NAMES}
-                expert.load_state_dict(state)
+                expert.load_state_dict(shard.layout.module_state({n: shard.views[n][le] for n in shard.layout.names}))
 
     def non_expert_parameters(self):
         return list(self.proj.parameters())

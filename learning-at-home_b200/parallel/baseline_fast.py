@@ -7,7 +7,8 @@ written the way a competent PyTorch user would write it, with NO host synchronis
   all-to-all      ``dist.all_to_all_single`` with EQUAL splits (NCCL) — shapes never depend on the routing, so there is no
                   .tolist() / .item() anywhere
   experts         stacked parameters [E_loc, ...]; three ``torch.bmm`` (cuBLAS batched GEMM, bf16 autocast of fp32 masters),
-                  ``F.layer_norm`` + per-expert affine, autograd backward
+                  ``F.layer_norm`` + per-expert affine, autograd backward; SwiGLU experts (``expert="swiglu"``):
+                  ``F.rms_norm`` * per-expert weight, one bmm over [W1 | W3], silu(g) * u, one bmm over W2
   optimizers      ONE fused ``torch.optim.Adam(amsgrad=True, fused=True)`` over the stacked expert parameters, one over the
                   trainer parameters (gradients all-reduced with NCCL)
 
@@ -25,7 +26,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.kernels import product_key_scores
-from .engine import DMoEConfig
+from .engine import GATED_EPS, DMoEConfig
 
 
 class _EqualAllToAll(torch.autograd.Function):
@@ -68,6 +69,12 @@ class FastBaselineDMoE(nn.Module):
             return (nn.Parameter(torch.empty(self.E_loc, i, o, device=device).uniform_(-bound, bound)),
                     nn.Parameter(torch.empty(self.E_loc, 1, o, device=device).uniform_(-bound, bound)))
 
+        if cfg.expert == "swiglu":
+            # GatedFeedforwardBlock: RMSNorm weight, [W1 | W3] as one [H, 2I] bmm operand (w1 columns first), W2
+            self.w13 = nn.Parameter(torch.empty(self.E_loc, H, 2 * I, device=device).uniform_(-1 / math.sqrt(H), 1 / math.sqrt(H)))
+            self.w2 = nn.Parameter(torch.empty(self.E_loc, I, H, device=device).uniform_(-1 / math.sqrt(I), 1 / math.sqrt(I)))
+            self.g = nn.Parameter(torch.ones(self.E_loc, 1, H, device=device))
+            return
         self.w1, self.b1 = lin(I, H)
         self.w2, self.b2 = lin(I, I)
         self.w3, self.b3 = lin(H, I)
@@ -75,6 +82,8 @@ class FastBaselineDMoE(nn.Module):
         self.g2, self.be2 = nn.Parameter(torch.ones(self.E_loc, 1, I, device=device)), nn.Parameter(torch.zeros(self.E_loc, 1, I, device=device))
 
     def expert_parameters(self):
+        if self.cfg.expert == "swiglu":
+            return [self.g, self.w13, self.w2]
         return [self.w1, self.b1, self.g1, self.be1, self.w2, self.b2, self.g2, self.be2, self.w3, self.b3]
 
     def gate_parameters(self):
@@ -106,17 +115,30 @@ class FastBaselineDMoE(nn.Module):
         if not x.is_cuda:
             rows = rows.float()   # CPU smoke path of this arm: fp32 maths
         with torch.autocast("cuda", dtype=torch.bfloat16, enabled=x.is_cuda):
-            h = torch.baddbmm(self.b1, rows, self.w1)
-            a = F.relu(F.layer_norm(h, (cfg.inner,)) * self.g1 + self.be1)
-            h = torch.baddbmm(self.b2, a, self.w2)
-            a = F.relu(F.layer_norm(h, (cfg.inner,)) * self.g2 + self.be2)
-            y = torch.baddbmm(self.b3, a, self.w3) + rows
+            if cfg.expert == "swiglu":
+                y = self._gated_experts(rows)
+            else:
+                y = self._ffn_experts(rows)
         y = y.to(torch.bfloat16).view(self.E_loc, self.world, C, H).transpose(0, 1).reshape(self.world, self.E_loc * C, H)
         back = _EqualAllToAll.apply(y.contiguous(), self.group).reshape(E * C, H)
         back = torch.cat([back, back.new_zeros(1, H)], 0)
         pair_out = back[slot] * (weights.reshape(-1)[order] * keep).to(back.dtype).unsqueeze(-1)
         out = torch.zeros(B, H, dtype=pair_out.dtype, device=x.device).index_add(0, tokens, pair_out)
         return out.to(x.dtype)
+
+    def _ffn_experts(self, rows):
+        cfg = self.cfg
+        h = torch.baddbmm(self.b1, rows, self.w1)
+        a = F.relu(F.layer_norm(h, (cfg.inner,)) * self.g1 + self.be1)
+        h = torch.baddbmm(self.b2, a, self.w2)
+        a = F.relu(F.layer_norm(h, (cfg.inner,)) * self.g2 + self.be2)
+        return torch.baddbmm(self.b3, a, self.w3) + rows
+
+    def _gated_experts(self, rows):
+        """rms_norm -> bmm over [W1 | W3] -> silu(g) * u -> bmm(W2) + rows"""
+        n = F.rms_norm(rows, (self.cfg.hidden,), eps=GATED_EPS) * self.g
+        hg, hu = torch.bmm(n, self.w13).chunk(2, dim=-1)
+        return torch.bmm(F.silu(hg) * hu, self.w2) + rows
 
 
 class FastBaselineTrainer:

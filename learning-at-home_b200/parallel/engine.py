@@ -26,7 +26,11 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..models.layers import FFN_SEG_KEYS as REF_KEYS, FFN_SEG_NAMES as SEG_NAMES, FFN_SMALL_SEG_MASK as SMALL_SEG_MASK
+from ..models.layers import EXPERT_LAYOUTS, gated_inner_dim
 from ..ops import fp8, gemm, kernels as K, native
+
+#: eps of the gated expert's RMSNorm (GatedFeedforwardBlock's default)
+GATED_EPS = 1e-6
 
 
 @dataclass
@@ -99,6 +103,39 @@ class DMoEConfig:
     # peer-flag wait timeout in ms (0 = ~10 s).  On expiry the waiting rank marks the step degraded (status bit) and goes on
     # with whatever arrived — the fused-path analogue of run_and_await_k's timeout_after_k_min (lib/utils/threading.py:76-125)
     peer_timeout_ms: int = 0
+    # the expert architecture, a ``name_to_block`` key: "ffn" = FeedforwardBlock (the reference's expert), "swiglu" =
+    # GatedFeedforwardBlock (RMSNorm -> [W1; W3] -> silu(g) * u -> W2, + x: the expert of Mixtral / DeepSeek-MoE / Qwen-MoE)
+    expert: str = "ffn"
+    # inner width of a "swiglu" expert; 0 = gated_inner_dim(hidden).  "ffn" is fixed at 4 * hidden (must stay 0)
+    inner_dim: int = 0
+
+    def __post_init__(self):
+        if self.expert not in EXPERT_LAYOUTS:
+            raise ValueError(f"DMoEConfig.expert must be one of {sorted(EXPERT_LAYOUTS)}, got {self.expert!r}")
+        if self.expert == "ffn" and self.inner_dim:
+            raise ValueError("DMoEConfig.inner_dim: FeedforwardBlock experts are 4 * hidden wide; inner_dim is for "
+                             "expert='swiglu' only")
+        if self.inner_dim < 0:
+            raise ValueError(f"DMoEConfig.inner_dim must be >= 0, got {self.inner_dim}")
+        if self.expert == "swiglu" and self.expert_dtype != "bf16":
+            raise ValueError("expert='swiglu' runs bf16 expert GEMMs only (its RMSNorm and SwiGLU kernels do not emit "
+                             f"MXFP8 operands); got expert_dtype={self.expert_dtype!r}")
+
+    def check_native_sizes(self):
+        """the widths the sm_90a kernels run for this expert (the CPU oracle path takes any size)"""
+        if self.expert == "swiglu" and (self.hidden % 128 or not 128 <= self.hidden <= K.LN_MAX_WIDTH or self.inner % 128):
+            raise ValueError(f"expert='swiglu' on the GPU needs hidden a multiple of 128 in [128, {K.LN_MAX_WIDTH}] and "
+                             f"an inner width that is a multiple of 128; got hidden={self.hidden}, inner={self.inner}")
+
+    @property
+    def layout(self):
+        """the segment layout of the expert kind (models/layers.py)"""
+        return EXPERT_LAYOUTS[self.expert]
+
+    def gemm_widths(self) -> Tuple[int, ...]:
+        """N of the expert's GEMMs (forward and dgrad): every one must be a multiple of 256 for 256-row groups"""
+        H, I = self.hidden, self.inner
+        return (2 * I, H, I) if self.expert == "swiglu" else (I, H)
 
     def resolved_path(self, world: int = 1) -> str:
         if self.accumulate:
@@ -107,8 +144,8 @@ class DMoEConfig:
             return self.expert_path
         rows_per_expert = self.tokens_per_rank * world * self.k / max(1, self.num_experts)
         experts_per_rank = -(-self.num_experts // max(1, world))
-        return "small" if (rows_per_expert < 512 and self.expert_dtype == "bf16" and self.inner % 128 == 0
-                           and self.hidden % 128 == 0
+        return "small" if (rows_per_expert < 512 and self.expert_dtype == "bf16"
+                           and all(n % 128 == 0 for n in self.gemm_widths())
                            and experts_per_rank <= 1023) else "big"   # swap-AB keeps a per-group prefix table in smem (MAX_G)
 
     @property
@@ -128,6 +165,9 @@ class DMoEConfig:
 
     @property
     def inner(self) -> int:
+        """the expert's inner width: 4 * hidden for "ffn", inner_dim or gated_inner_dim(hidden) for "swiglu\""""
+        if self.expert == "swiglu":
+            return self.inner_dim or gated_inner_dim(self.hidden)
         return 4 * self.hidden
 
     def adam_kwargs(self) -> Dict:
@@ -136,9 +176,7 @@ class DMoEConfig:
                     decoupled=self.decoupled_weight_decay)
 
     def seg_shapes(self) -> Dict[str, Tuple[int, ...]]:
-        H, I = self.hidden, self.inner
-        return {"w1": (I, H), "b1": (I,), "g1": (I,), "be1": (I,), "w2": (I, I), "b2": (I,), "g2": (I,), "be2": (I,),
-                "w3": (H, I), "b3": (H,)}
+        return self.layout.shapes(self.hidden, self.inner)
 
 
 def expert_uid(cfg: DMoEConfig, e: int) -> str:
@@ -159,6 +197,7 @@ class EngineContext:
     def __init__(self, cfg: DMoEConfig, group=None, device=None, heap_bytes: Optional[int] = None):
         from .symmetric import SymmetricHeap
         import torch.distributed as dist
+        cfg.check_native_sizes()
         self.cfg = cfg
         self.device = device or torch.device("cuda", torch.cuda.current_device())
         distributed = dist.is_available() and dist.is_initialized()
@@ -176,7 +215,7 @@ class EngineContext:
             self.S = 0
         else:
             # expert groups are padded to this many rows: 256 when every GEMM of the expert runs on 128 x 256 tiles
-            self.align = 256 if cfg.hidden % 256 == 0 and cfg.inner % 256 == 0 else 128
+            self.align = 256 if all(n % 256 == 0 for n in cfg.gemm_widths()) else 128
             self.tile_rows = 128
             self.S = min(int(cfg.shadow_experts), 2 * K.MAX_WORLD) if self.world > 1 else 0   # shadow slots per rank / layer
         self.G_tot = self.E_loc + self.S
@@ -239,8 +278,9 @@ class EngineContext:
         self.gyd, self.gyd_off = self.heap.alloc((self.max_rows, H), torch.bfloat16)
         self.dxd, self.dxd_off = self.heap.alloc((self.max_rows, H), torch.bfloat16)
         bf = dict(dtype=torch.bfloat16, device=self.device)
-        self.da = torch.empty(self.max_rows, cfg.inner, **bf)
-        self.dh = torch.empty(self.max_rows, cfg.inner, **bf)
+        # the expert's backward temporaries (FeedforwardBlock: da, dh; GatedFeedforwardBlock: da, dh = [dg | du], dn)
+        for name, width in cfg.layout.buffers(H, cfg.inner)["scratch"].items():
+            setattr(self, name, torch.empty(self.max_rows, width, **bf))
         self.heap.barrier()
 
     EPOCH_STRIDE = 64   # epochs a step may consume; the device-side base advances by this much per begin_step()
@@ -388,8 +428,9 @@ class ExpertShard:
         self.cfg, self.E_loc, self.first_expert = cfg, E_loc, first_expert
         # slots = owned experts + shadow slots (replicas of other ranks' hot experts, only on multi-GPU runs)
         self.slots = slots = E_loc + (ctx.S if ctx is not None else 0)
+        self.layout = cfg.layout
         shapes = cfg.seg_shapes()
-        shapes = {n: shapes[n] for n in SEG_NAMES}   # in segment order
+        shapes = {n: shapes[n] for n in self.layout.names}   # in segment order
         self.seg_sizes = [int(math.prod(shape)) for shape in shapes.values()]
         total = sum(self.seg_sizes) * slots
         f32 = dict(dtype=torch.float32, device=device)
@@ -423,21 +464,24 @@ class ExpertShard:
 
     @torch.no_grad()
     def reset_parameters(self, layer_index: int = 0):
-        """nn.Linear / nn.LayerNorm default initialisation, seeded per (layer, global expert) so that the same expert
-        gets the same weights regardless of the number of ranks"""
+        """nn.Linear / nn.LayerNorm / nn.RMSNorm default initialisation (weights and biases uniform in +-1/sqrt(fan_in),
+        norm weights 1, norm biases 0), seeded per (layer, global expert) so that the same expert gets the same weights
+        regardless of the number of ranks"""
         cfg = self.cfg
         dev = self.p.device
         for le in range(self.E_loc):
             gen = torch.Generator(device=dev)
             gen.manual_seed(cfg.seed * 1000003 + layer_index * 10007 + self.first_expert + le)
-            for w, b in (("w1", "b1"), ("w2", "b2"), ("w3", "b3")):
-                fan_in = self.views[w].shape[-1]
-                bound = 1.0 / math.sqrt(fan_in)
-                self.views[w][le].uniform_(-bound, bound, generator=gen)
-                self.views[b][le].uniform_(-bound, bound, generator=gen)
-            for gname, bname in (("g1", "be1"), ("g2", "be2")):
-                self.views[gname][le].fill_(1.0)
-                self.views[bname][le].zero_()
+            for n in self.layout.names:   # segment order: a matrix is followed by its bias (FeedforwardBlock)
+                t = self.views[n][le]
+                if n.startswith("be"):       # LayerNorm bias
+                    t.zero_()
+                elif n.startswith("g"):      # LayerNorm / RMSNorm weight
+                    t.fill_(1.0)
+                else:                        # Linear weight wX or its bias bX (fan_in from wX)
+                    fan_in = self.views["w" + n[1:]].shape[-1]
+                    bound = 1.0 / math.sqrt(fan_in)
+                    t.uniform_(-bound, bound, generator=gen)
         self.sync_bf16()
 
     def fp8_weights(self):
@@ -456,41 +500,49 @@ class ExpertShard:
             self.p_bf16.copy_(self.p)
 
     # ------------------------------------------------------------------ checkpoint layout (SURVEY.md §5.4)
+    def _expert_tensors(self, views, le: int) -> Dict[str, torch.Tensor]:
+        """one expert's rows of a per-segment view, as the module's tensors (parameters() order)"""
+        return self.layout.module_state({n: views[n][le] for n in self.layout.names})
+
     def expert_state_dict(self, le: int, prefix: str = "expert.") -> Dict[str, torch.Tensor]:
-        """state of local expert `le` with the key names of ``ExpertBackend.state_dict()`` of the reference"""
-        return {prefix + REF_KEYS[n]: self.views[n][le].detach().clone().cpu() for n in SEG_NAMES}
+        """state of local expert `le` with the key names of ``ExpertBackend.state_dict()`` of the reference (the module of
+        ``cfg.expert``: FeedforwardBlock or GatedFeedforwardBlock)"""
+        return {prefix + k: t.detach().clone().cpu() for k, t in self._expert_tensors(self.views, le).items()}
 
     def expert_optimizer_state(self, le: int) -> Dict:
         """torch.optim.Adam-compatible state_dict of local expert `le` (parameter order = module.parameters())"""
-        state = {}
-        for i, n in enumerate(SEG_NAMES):
-            entry = dict(step=torch.tensor(float(self.step[le].item())), exp_avg=self.m_views[n][le].clone().cpu(),
-                         exp_avg_sq=self.v_views[n][le].clone().cpu())
-            if self.vmax is not None:
-                entry["max_exp_avg_sq"] = self.vmax_views[n][le].clone().cpu()
-            state[i] = entry
+        step = torch.tensor(float(self.step[le].item()))
+        moments = [("exp_avg", self.m_views), ("exp_avg_sq", self.v_views)]
+        if self.vmax is not None:
+            moments.append(("max_exp_avg_sq", self.vmax_views))
+        per_key = {name: self._expert_tensors(views, le) for name, views in moments}
+        state = {i: dict(step=step.clone(), **{name: per_key[name][k].clone().cpu() for name, _ in moments})
+                 for i, k in enumerate(self.layout.params)}
         cfg = self.cfg
         group = dict(lr=cfg.lr, betas=cfg.betas, eps=cfg.eps, weight_decay=cfg.weight_decay, amsgrad=cfg.amsgrad,
-                     decoupled_weight_decay=cfg.decoupled_weight_decay, params=list(range(len(SEG_NAMES))))
+                     decoupled_weight_decay=cfg.decoupled_weight_decay, params=list(range(len(self.layout.params))))
         return dict(state=state, param_groups=[group])
 
     def load_expert_state_dict(self, le: int, state: Dict[str, torch.Tensor], prefix: str = "expert."):
         with torch.no_grad():
-            for n in SEG_NAMES:
-                self.views[n][le].copy_(state[prefix + REF_KEYS[n]])
+            for n, t in self.layout.segment_state(state, prefix).items():
+                self.views[n][le].copy_(t)
         self.sync_bf16()
 
     def load_expert_optimizer_state(self, le: int, opt_state: Dict):
         with torch.no_grad():
-            for i, n in enumerate(SEG_NAMES):
+            for i, k in enumerate(self.layout.params):
                 entry = opt_state["state"].get(i)
                 if entry is None:
                     continue
-                shape = self.m_views[n].shape[1:]
-                self.m_views[n][le].copy_(entry["exp_avg"].reshape(shape))
-                self.v_views[n][le].copy_(entry["exp_avg_sq"].reshape(shape))
-                if self.vmax is not None and "max_exp_avg_sq" in entry:
-                    self.vmax_views[n][le].copy_(entry["max_exp_avg_sq"].reshape(shape))
+                n, block, parts = self.layout.slices[k]
+                for name, views in (("exp_avg", self.m_views), ("exp_avg_sq", self.v_views),
+                                    ("max_exp_avg_sq", self.vmax_views if self.vmax is not None else None)):
+                    if views is None or name not in entry:
+                        continue
+                    dst = views[n][le]
+                    dst = dst.chunk(parts, 0)[block] if parts > 1 else dst
+                    dst.copy_(entry[name].reshape(dst.shape))
                 self.step[le] = int(entry["step"])
 
 
@@ -506,14 +558,17 @@ class LayerWorkspace:
         f32 = dict(dtype=torch.float32, device=dev)
         self.xd, self.xd_off = ctx.heap.alloc((R, H), torch.bfloat16)   # dispatched inputs (peers push)
         self.yo, self.yo_off = ctx.heap.alloc((R, H), torch.bfloat16)   # expert outputs (peers pull)
-        self.h1, self.a1 = torch.empty(R, I, **bf), torch.empty(R, I, **bf)
-        self.h2, self.a2 = torch.empty(R, I, **bf), torch.empty(R, I, **bf)
+        # the expert's activations (FeedforwardBlock: h1, a1, h2, a2 and the LayerNorm statistics; GatedFeedforwardBlock:
+        # n = RMSNorm(xd), h = [hg | hu], a = silu(hg) * hu and rstd)
+        buffers = cfg.layout.buffers(H, I)
+        for name, width in buffers["rows"].items():
+            setattr(self, name, torch.empty(R, width, **bf))
+        for name in buffers["stats"]:
+            setattr(self, name, torch.empty(R, **f32))
         self.xq = self.aq = None
         if cfg.expert_dtype == "fp8":   # MXFP8 operands of the forward GEMMs (aq is shared by a1 and a2)
             self.xq = fp8.MXFP8Tensor(R, 1, H, fp8.ACT_TILE, dev)
             self.aq = fp8.MXFP8Tensor(R, 1, I, fp8.ACT_TILE, dev)
-        self.mean1, self.rstd1 = torch.empty(R, **f32), torch.empty(R, **f32)
-        self.mean2, self.rstd2 = torch.empty(R, **f32), torch.empty(R, **f32)
         P = cfg.tokens_per_rank * cfg.k
         self.idx, self.pos, self.pair_row = torch.empty(P, **i32), torch.empty(P, **i32), torch.empty(P, **i32)
         self.w = torch.empty(P, **f32)
@@ -529,11 +584,15 @@ class LayerWorkspace:
         self.outstanding = False   # a training-mode forward whose backward has not run yet owns this workspace
         # small path with optimizer overlap: the fused wgrad+AMSGrad kernels of layer L read dY buffers while the main stream is
         # already in the backward of layer L-1, so they must be per layer (a few MB each at this batch size)
+        # (FeedforwardBlock: dh2 and dh1; GatedFeedforwardBlock: dh13 = [dg | du]; its other inputs, a and n, are activations)
         if ctx.small and ctx.opt_stream is not None:
             self.gyd, self.gyd_off = ctx.heap.alloc((R, H), torch.bfloat16)
-            self.dh2, self.dh1 = torch.zeros(R, I, **bf), torch.zeros(R, I, **bf)
+            for name, shared in buffers["per_layer"].items():
+                setattr(self, name, torch.zeros_like(getattr(ctx, shared)))
         else:
-            self.gyd, self.gyd_off, self.dh2, self.dh1 = ctx.gyd, ctx.gyd_off, ctx.dh, ctx.dh
+            self.gyd, self.gyd_off = ctx.gyd, ctx.gyd_off
+            for name, shared in buffers["per_layer"].items():
+                setattr(self, name, getattr(ctx, shared))
 
 
 # =========================================================================================================
@@ -658,7 +717,7 @@ class FusedDMoE(nn.Module):
                           shadow_tol=cfg.shadow_tol, min_shadow_rows=cfg.shadow_min_rows, route_owner=ws.route_owner,
                           step_rows=ws.step_rows, shadow_info=ws.shadow_info, owned_shadow=ws.owned_shadow)
         if c.S:  # replicas of this step's hot experts: weights from the owners' bf16 mirror, small params from fp32
-            K.pull_shadow(ws.shadow_info, c.S, c.E_loc, sh.p_off, sh.pbf16_off, sh.seg_sizes, SMALL_SEG_MASK)
+            K.pull_shadow(ws.shadow_info, c.S, c.E_loc, sh.p_off, sh.pbf16_off, sh.seg_sizes, sh.layout.small_mask)
             sh.w8_dirty = True
         K.scatter_rows(x, None, idx, pos, ws.dst_row, pair_row, ws.xd_off, c.flags_off, K.SLOT_DISPATCH, epoch, k,
                        c.E_loc, c.max_rows, ws.group_off, ws.group_rows, c.done_counter, c.status, align=c.align,
@@ -668,7 +727,9 @@ class FusedDMoE(nn.Module):
         # producer polls the peers' dispatch flags itself (no separate wait kernel)
         tg = ws.tile_group
         wait = (c.flags[K.SLOT_DISPATCH, :c.world], epoch, c.status) if c.world > 1 else None
-        if c.small:
+        if cfg.expert == "swiglu":
+            self._expert_gated_fwd(wait, epoch)
+        elif c.small:
             # weight-streaming regime: swap-AB tiles (weights on MMA-M, the group's 16..128 tokens on MMA-N), groups of 16 rows
             go, gr_, T = ws.group_off, ws.group_rows, c.tile_rows
             K.swapab_linear(ws.xd, sh.bf16["w1"], go, gr_, out=ws.h1, bias=sh.views["b1"], wait=wait)
@@ -690,6 +751,29 @@ class FusedDMoE(nn.Module):
                        signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner)
         c.timer.mark("combine")
         return y
+
+    def _expert_gated_fwd(self, wait, epoch):
+        """GatedFeedforwardBlock on the received rows: n = RMSNorm(xd) with each expert's gamma, h = [hg | hu] = n [W1; W3]^T
+        (one GEMM), a = silu(hg) * hu, yo = a W2^T + xd.  The rows of unused tiles (group -1) of n, h and a are not
+        written by the norm and GEMMs and hold stale values; no result depends on them.  The big path's GEMMs skip -1
+        tiles.  The small path's GEMMs load a group's tokens in power-of-two TMA boxes (16..128 rows) from group_off, so
+        the box of a group's last block may extend past its padded rows (into the next group or a -1 tile): the extra
+        rows are separate GEMM columns whose outputs are not stored.  The wgrads read only the groups' rows, and SwiGLU
+        maps stale rows elementwise to rows that are equally unread."""
+        c, ws, sh = self.ctx, self.ws, self.shard
+        tg, T = ws.tile_group, c.tile_rows
+        if wait is not None:  # the norm, not a GEMM, is the first consumer of the rows pushed by the peers
+            K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
+        K.rms_norm_fwd(ws.xd, sh.views["g"], GATED_EPS, out=ws.n, rstd=ws.rstd, tile_group=tg, tile_rows=T)
+        if c.small:
+            go, gr_ = ws.group_off, ws.group_rows
+            K.swapab_linear(ws.n, sh.bf16["w13"], go, gr_, out=ws.h)
+            K.swiglu_fwd(ws.h, out=ws.a)
+            K.swapab_linear(ws.a, sh.bf16["w2"], go, gr_, out=ws.yo, residual=ws.xd)
+        else:
+            gemm.grouped_linear(ws.n, sh.bf16["w13"], tile_group=tg, out=ws.h)
+            K.swiglu_fwd(ws.h, out=ws.a)
+            gemm.grouped_linear(ws.a, sh.bf16["w2"], tile_group=tg, residual=ws.xd, out=ws.yo)
 
     def _expert_ffn_fp8(self, wait, epoch):
         """forward GEMMs on block-scaled FP8 tensor cores; LayerNorm emits the next GEMM's MXFP8 operand directly (and the
@@ -719,8 +803,8 @@ class FusedDMoE(nn.Module):
         K.scatter_rows(gy, w, idx, pos, None, pair_row, ws.gyd_off, c.flags_off, K.SLOT_GRAD, epoch, k, c.E_loc,
                        c.max_rows, ws.group_off, ws.group_rows, c.done_counter, c.status, align=c.align,
                        route_owner=ws.route_owner, num_groups=c.G_tot)
-        if c.S:  # atomically accumulated (bias / LayerNorm) partial gradients of my shadow slots start from zero
-            K.zero_slots(sh.g, sh.seg_sizes, c.G_tot, c.E_loc, c.S, SMALL_SEG_MASK)
+        if c.S:  # atomically accumulated (bias / norm) partial gradients of my shadow slots start from zero
+            K.zero_slots(sh.g, sh.seg_sizes, c.G_tot, c.E_loc, c.S, sh.layout.small_mask)
         if c.world > 1:  # the first consumers of the pushed gradients are the colsum / wgrad kernels
             K.signal_wait(c.flags_off, K.SLOT_GRAD, epoch, c.status, signal=False, wait=True)
         c.timer.mark("bwd_gate+dispatch_grad")
@@ -734,17 +818,29 @@ class FusedDMoE(nn.Module):
                            epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner)
             c.timer.mark("bwd_combine")
             return dx, dlogits
-        K.grouped_colsum(c.gyd, tg, out=gr["b3"])
-        gemm.grouped_wgrad(c.gyd, ws.a2, go, G, out=gr["w3"], accumulate=cfg.accumulate)
-        gemm.grouped_linear(c.gyd, sh.bf16["w3"], tile_group=tg, w_is_kn=True, out=c.da)
-        K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=c.dh, dgamma=gr["g2"],
-                      dbeta=gr["be2"], dbias=gr["b2"])
-        gemm.grouped_wgrad(c.dh, ws.a1, go, G, out=gr["w2"], accumulate=cfg.accumulate)
-        gemm.grouped_linear(c.dh, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
-        K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=c.dh, dgamma=gr["g1"],
-                      dbeta=gr["be1"], dbias=gr["b1"])
-        gemm.grouped_wgrad(c.dh, ws.xd, go, G, out=gr["w1"], accumulate=cfg.accumulate)
-        gemm.grouped_linear(c.dh, sh.bf16["w1"], tile_group=tg, w_is_kn=True, residual=c.gyd, out=c.dxd)
+        if cfg.expert == "swiglu":
+            # padding rows: scatter_rows zeroed them in xd and gyd, so da, dh and dn are zero there, and the RMSNorm
+            # backward of a row with dn = 0 adds nothing to dgamma.  dgamma is added (+=) to the gradient buffer, which
+            # apply_expert_gradients zeroes once the expert steps (with update_every_* it accumulates until then)
+            gemm.grouped_wgrad(c.gyd, ws.a, go, G, out=gr["w2"], accumulate=cfg.accumulate)
+            gemm.grouped_linear(c.gyd, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
+            K.swiglu_bwd(c.da, ws.h, out=c.dh)
+            gemm.grouped_wgrad(c.dh, ws.n, go, G, out=gr["w13"], accumulate=cfg.accumulate)
+            gemm.grouped_linear(c.dh, sh.bf16["w13"], tile_group=tg, w_is_kn=True, out=c.dn)
+            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.views["g"], dx=c.dxd, dgamma=gr["g"], dres=c.gyd,
+                           tile_rows=c.tile_rows, tile_group=tg)
+        else:
+            K.grouped_colsum(c.gyd, tg, out=gr["b3"])
+            gemm.grouped_wgrad(c.gyd, ws.a2, go, G, out=gr["w3"], accumulate=cfg.accumulate)
+            gemm.grouped_linear(c.gyd, sh.bf16["w3"], tile_group=tg, w_is_kn=True, out=c.da)
+            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=c.dh, dgamma=gr["g2"],
+                          dbeta=gr["be2"], dbias=gr["b2"])
+            gemm.grouped_wgrad(c.dh, ws.a1, go, G, out=gr["w2"], accumulate=cfg.accumulate)
+            gemm.grouped_linear(c.dh, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
+            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=c.dh, dgamma=gr["g1"],
+                          dbeta=gr["be1"], dbias=gr["b1"])
+            gemm.grouped_wgrad(c.dh, ws.xd, go, G, out=gr["w1"], accumulate=cfg.accumulate)
+            gemm.grouped_linear(c.dh, sh.bf16["w1"], tile_group=tg, w_is_kn=True, residual=c.gyd, out=c.dxd)
         c.timer.mark("expert_ffn_bwd(wgrad+dgrad+ln)")
         # ---- expert-side optimizer step (reference: ExpertBackend.apply_gradients right after backward)
         if c.S:  # the owners read every rank's partial gradients of the shadowed experts: all ranks must be done
@@ -782,27 +878,41 @@ class FusedDMoE(nn.Module):
                 K.wgrad_adam(dy, x, go, rows, max_ctas=c.opt_ctas, **kw)
             c._opt_pending = True
 
-        gyd, dh2, dh1 = ws.gyd, ws.dh2, ws.dh1
+        gyd = ws.gyd
         K.bump_steps(sh.step, ws.step_rows)
-        K.grouped_colsum(gyd, tg, out=gr["b3"], tile_rows=T)
-        K.swapab_linear(gyd, sh.bf16["w3"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
-        wgrad("w3", gyd, ws.a2)
-        K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=dh2, dgamma=gr["g2"],
-                      dbeta=gr["be2"], dbias=gr["b2"], tile_rows=T)
-        K.swapab_linear(dh2, sh.bf16["w2"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
-        wgrad("w2", dh2, ws.a1)
-        K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=dh1, dgamma=gr["g1"],
-                      dbeta=gr["be1"], dbias=gr["b1"], tile_rows=T)
-        K.swapab_linear(dh1, sh.bf16["w1"], go, rows, out=c.dxd, w_is_kn=True, residual=gyd, max_ctas=chain_ctas)
-        wgrad("w1", dh1, ws.xd)
-        # biases / LayerNorm affine: the ordinary fused AMSGrad restricted to the small segments
+        if cfg.expert == "swiglu":
+            # the fused launches read gyd, a, dh13 and n: per-layer buffers whenever the optimizer stream is used.  Padding
+            # rows: xd and gyd are zero there, so da, dh13 and dn are too, and add nothing to dgamma (see _backward_cuda)
+            dh13 = ws.dh13
+            K.swapab_linear(gyd, sh.bf16["w2"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
+            wgrad("w2", gyd, ws.a)
+            K.swiglu_bwd(c.da, ws.h, out=dh13)
+            K.swapab_linear(dh13, sh.bf16["w13"], go, rows, out=c.dn, w_is_kn=True, max_ctas=chain_ctas)
+            wgrad("w13", dh13, ws.n)
+            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.views["g"], dx=c.dxd, dgamma=gr["g"], dres=gyd, tile_rows=T,
+                           tile_group=tg)
+        else:
+            dh2, dh1 = ws.dh2, ws.dh1
+            K.grouped_colsum(gyd, tg, out=gr["b3"], tile_rows=T)
+            K.swapab_linear(gyd, sh.bf16["w3"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
+            wgrad("w3", gyd, ws.a2)
+            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=dh2, dgamma=gr["g2"],
+                          dbeta=gr["be2"], dbias=gr["b2"], tile_rows=T)
+            K.swapab_linear(dh2, sh.bf16["w2"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
+            wgrad("w2", dh2, ws.a1)
+            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=dh1, dgamma=gr["g1"],
+                          dbeta=gr["be1"], dbias=gr["b1"], tile_rows=T)
+            K.swapab_linear(dh1, sh.bf16["w1"], go, rows, out=c.dxd, w_is_kn=True, residual=gyd, max_ctas=chain_ctas)
+            wgrad("w1", dh1, ws.xd)
+        # biases / norm weights: the ordinary fused AMSGrad restricted to the small segments
+        small = sh.layout.small_mask
         K.adam_step(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
-                    group_rows=ws.step_rows, zero_mask=SMALL_SEG_MASK, G_active=self.E_loc, seg_mask=SMALL_SEG_MASK, **opt)
+                    group_rows=ws.step_rows, zero_mask=small, G_active=self.E_loc, seg_mask=small, **opt)
         sh.w8_dirty = True
 
     def apply_expert_gradients(self):
         sh, cfg, ws, c = self.shard, self.cfg, self.ws, self.ctx
-        rows, zero_mask = ws.step_rows, SMALL_SEG_MASK
+        rows, zero_mask = ws.step_rows, sh.layout.small_mask
         if cfg.accumulate:
             # asynchronous expert updates (dmoe_emulator.py:70-77): gradients accumulate in sh.g (wgrad accumulate=True) until
             # the expert has seen >= update_every_inputs rows or >= update_every_steps steps since its first pending row
@@ -813,7 +923,7 @@ class FusedDMoE(nn.Module):
             sh.fire.copy_(due.to(torch.int32))
             sh.pending_rows.mul_(1 - sh.fire)
             sh.pending_steps.mul_(1 - sh.fire)
-            rows, zero_mask = sh.fire, (1 << len(SEG_NAMES)) - 1
+            rows, zero_mask = sh.fire, (1 << len(sh.layout.names)) - 1
         K.bump_steps(sh.step, rows)
         K.adam_step(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
                     group_rows=rows, **c.adam_kwargs(), zero_mask=zero_mask, G_active=self.E_loc, world=c.world,
@@ -832,10 +942,10 @@ class FusedDMoE(nn.Module):
             # (Slicing one big leaf instead makes autograd materialise a full-size zero tensor per slice.)
             leaves = self._ref_leaves.get(e_local)
             if leaves is None:
-                leaves = {n: self.shard.views[n][e_local].detach().requires_grad_(True) for n in SEG_NAMES}
+                leaves = {n: self.shard.views[n][e_local].detach().requires_grad_(True) for n in self.shard.layout.names}
                 self._ref_leaves[e_local] = leaves
             return leaves
-        return {n: self.shard.views[n][e_local].to(dtype) for n in SEG_NAMES}
+        return {n: self.shard.views[n][e_local].to(dtype) for n in self.shard.layout.names}
 
     def apply_expert_gradients_ref(self):
         """CPU-mode counterpart of apply_expert_gradients (same per-expert AMSGrad rule, PyTorch ops)"""
@@ -862,7 +972,7 @@ class FusedDMoE(nn.Module):
                 keep = (~due).to(sh.pending_rows.dtype)
                 sh.pending_rows.mul_(keep)
                 sh.pending_steps.mul_(keep)
-                rows, zero_mask = due.to(rows.dtype), (1 << len(SEG_NAMES)) - 1
+                rows, zero_mask = due.to(rows.dtype), (1 << len(sh.layout.names)) - 1
             sh.step += (rows > 0).to(sh.step.dtype)
             K.adam_step_ref(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.seg_sizes, self.E_loc, step=sh.step,
                             group_rows=rows, **cfg.adam_kwargs(), zero_mask=zero_mask)
@@ -898,14 +1008,23 @@ class FusedDMoE(nn.Module):
             if emulate_bf16:
                 p = {n: (rnd(v) if n.startswith("w") else v) for n, v in p.items()}
             tok, slot = torch.nonzero(idx == e, as_tuple=True)
-            xe = rnd(xf[tok])
-            h1 = rnd(F.linear(xe, p["w1"], p["b1"]))
-            a1 = rnd(F.relu(F.layer_norm(h1, (cfg.inner,), p["g1"], p["be1"])))
-            h2 = rnd(F.linear(a1, p["w2"], p["b2"]))
-            a2 = rnd(F.relu(F.layer_norm(h2, (cfg.inner,), p["g2"], p["be2"])))
-            ye = rnd(F.linear(a2, p["w3"], p["b3"]) + xe)
+            ye = self._expert_ref(p, rnd(xf[tok]), rnd)
             out = out.index_put((tok,), ye * weights[tok, slot].unsqueeze(-1), accumulate=True)
         return out.to(x.dtype)
+
+    def _expert_ref(self, p, xe, rnd):
+        """one expert on its rows in fp32; ``rnd`` rounds where the GPU path stores bf16"""
+        cfg = self.cfg
+        if cfg.expert == "swiglu":   # GatedFeedforwardBlock: x + w2(silu(w1 n) * w3 n), n = RMSNorm(x)
+            n = rnd(F.rms_norm(xe, (cfg.hidden,), p["g"], GATED_EPS))
+            hg, hu = rnd(F.linear(n, p["w13"])).chunk(2, dim=-1)
+            a = rnd(F.silu(hg) * hu)
+            return rnd(F.linear(a, p["w2"]) + xe)
+        h1 = rnd(F.linear(xe, p["w1"], p["b1"]))
+        a1 = rnd(F.relu(F.layer_norm(h1, (cfg.inner,), p["g1"], p["be1"])))
+        h2 = rnd(F.linear(a1, p["w2"], p["b2"]))
+        a2 = rnd(F.relu(F.layer_norm(h2, (cfg.inner,), p["g2"], p["be2"])))
+        return rnd(F.linear(a2, p["w3"], p["b3"]) + xe)
 
 
 # =========================================================================================================

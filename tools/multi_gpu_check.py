@@ -25,9 +25,11 @@ def main():
     B = 256
     force_shadow = "--force-shadow" in sys.argv  # shadow as many experts as there are slots (exercises the replica path)
     small = "--small" in sys.argv   # weight-streaming expert path (swap-AB GEMMs + fused wgrad/AMSGrad; no shadowing)
+    swiglu = "--swiglu" in sys.argv   # GatedFeedforwardBlock experts (compares [W1; W3] and the RMSNorm weight)
+    mat, vec = ("w13", "g") if swiglu else ("w1", "b2")
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=B, capacity_factor=float(max(4, world)),
                        shadow_experts=4, shadow_tol=0.0 if force_shadow else 1.1, shadow_min_rows=1 if force_shadow else 64,
-                       expert_path="small" if small else "big")
+                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn")
     ctx = E.EngineContext(cfg)
     torch.manual_seed(0)  # identical gate on every rank (DMoETrainer does the same)
     layer = E.FusedDMoE(cfg, ctx).cuda()
@@ -53,10 +55,10 @@ def main():
     dist.all_gather(dxs, x.grad.contiguous())
     gw = layer.proj.weight.grad.clone()
     dist.all_reduce(gw)
-    w1 = layer.shard.views["w1"][:layer.E_loc].clone()
+    w1 = layer.shard.views[mat][:layer.E_loc].clone()
     w1s = [torch.empty_like(w1) for _ in range(world)]
     dist.all_gather(w1s, w1)
-    b2 = layer.shard.views["b2"][:layer.E_loc].clone()
+    b2 = layer.shard.views[vec][:layer.E_loc].clone()
     b2s = [torch.empty_like(b2) for _ in range(world)]
     dist.all_gather(b2s, b2)
     steps = [torch.empty_like(layer.shard.step) for _ in range(world)]
@@ -74,12 +76,12 @@ def main():
         yr.backward(g_all.cuda().float())
         ref.apply_expert_gradients_ref()
         errs = dict(y=rel(torch.cat(ys), yr), dx=rel(torch.cat(dxs), xr.grad), dproj=rel(gw, ref.proj.weight.grad),
-                    w1_mean_abs=(torch.cat(w1s) - ref.shard.views["w1"]).abs().mean().item(),
-                    b2_max_abs=(torch.cat(b2s) - ref.shard.views["b2"]).abs().max().item(),
+                    w1_mean_abs=(torch.cat(w1s) - ref.shard.views[mat]).abs().mean().item(),
+                    b2_max_abs=(torch.cat(b2s) - ref.shard.views[vec]).abs().max().item(),
                     steps=bool((torch.cat(steps).cpu() == ref.shard.step.cpu()).all()))
         ok = errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2 and errs["w1_mean_abs"] < 1e-4 and errs["b2_max_abs"] < 2.5e-3 and errs["steps"]
         ok = ok and (shadowed > 0 or not force_shadow) and plan_ok
-        print("multi_gpu_check", dict(path="small" if small else "big", force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
+        print("multi_gpu_check", dict(path="small" if small else "big", expert=cfg.expert, force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
                                       plan=plan, kernel=got), errs, flush=True)
         print("MULTI_GPU_OK" if ok else "MULTI_GPU_FAILED", flush=True)
     dist.barrier()
