@@ -923,6 +923,212 @@ __global__ void __launch_bounds__(256) zero_slots_kernel(float* g, SegLayout L, 
         base[v] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
+// ------------------------------------------------------------------------------------------------
+// router losses of the product-key gate (load balancing and z-loss, DESIGN.md §6a).  With A the live experts, N = |A|:
+//   p_{b,e} = softmax_{e in A}(s_{b,e}),  z_b = logsumexp_{e in A}(s_{b,e}),  f_e = c_e / sum c  (box-wide routed pairs),
+//   F_b = sum_{e in A} f_e p_{b,e},  L_aux = (N/B) sum_b F_b,  L_z = (1/B) sum_b z_b^2
+// A token without a finite score has z_b = F_b = 0 and no gradient.  Every sum runs in a fixed order (no float atomics).
+// ------------------------------------------------------------------------------------------------
+constexpr int RL_WARPS = 4;   // tokens per CTA of the router-loss kernels (one warp each)
+
+// f_e = c_e / sum_e c_e with c_e = sum over the `rows` rank rows of the count table; f[E] = N (live experts).  One CTA of
+// 1024 threads: the sums are integers, so their order does not matter.  B == 0 writes zero losses (no token kernel runs)
+__global__ void __launch_bounds__(1024) router_f_kernel(const int* __restrict__ cnt, int rows, int E,
+                                                        const unsigned char* __restrict__ alive, float* __restrict__ f,
+                                                        int B, float* __restrict__ loss) {
+    __shared__ long long s_total;
+    __shared__ int s_live;
+    if (threadIdx.x == 0) {
+        s_total = 0;
+        s_live = 0;
+    }
+    __syncthreads();
+    long long tot = 0;
+    int live = 0;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+        for (int r = 0; r < rows; ++r) tot += cnt[static_cast<long long>(r) * E + e];
+        live += (!alive || alive[e]) ? 1 : 0;
+    }
+    atomicAdd(reinterpret_cast<unsigned long long*>(&s_total), static_cast<unsigned long long>(tot));
+    atomicAdd(&s_live, live);
+    __syncthreads();
+    const float inv = s_total > 0 ? 1.f / static_cast<float>(s_total) : 0.f;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+        long long c = 0;
+        for (int r = 0; r < rows; ++r) c += cnt[static_cast<long long>(r) * E + e];
+        f[e] = static_cast<float>(c) * inv;
+    }
+    if (threadIdx.x == 0) {
+        f[E] = static_cast<float>(s_live);
+        if (B <= 0) loss[0] = loss[1] = 0.f;
+    }
+}
+
+// product-key score of expert c, summed last grid dimension first (the order of gate_topk_kernel)
+__device__ __forceinline__ float pk_score(const float* lg, const GridSpec& gs, int c) {
+    int rem = c;
+    float s = 0.f;
+#pragma unroll
+    for (int d = MAX_GRID_DIMS - 1; d >= 0; --d) {
+        if (d < gs.ndim) {
+            const int i = rem % gs.size[d];
+            rem /= gs.size[d];
+            s += lg[gs.offset[d] + i];
+        }
+    }
+    return s;
+}
+
+// largest score of a live expert (-inf: none is finite), over the lanes of the warp
+__device__ __forceinline__ float router_max_score(const float* lg, const GridSpec& gs, const unsigned char* alive, int lane) {
+    float mx = -INFINITY;
+    for (int c = lane; c < gs.num_experts; c += 32)
+        if (!alive || alive[c]) mx = fmaxf(mx, pk_score(lg, gs, c));
+    return warp_max(mx);
+}
+
+// one warp per token: z_b and F_b into z / Fb, the CTA's sums of F_b and z_b^2 into partials[2 * blockIdx.x]; the last CTA
+// to finish adds the partials in CTA order: loss = ((N/B) sum F_b, (1/B) sum z_b^2)
+__global__ void __launch_bounds__(RL_WARPS * 32) router_loss_fwd_kernel(const float* __restrict__ logits, int B, GridSpec gs,
+                                                                        const unsigned char* __restrict__ alive,
+                                                                        const float* __restrict__ f, float* __restrict__ z,
+                                                                        float* __restrict__ Fb, float* __restrict__ partials,
+                                                                        int* __restrict__ ticket, float* __restrict__ loss) {
+    extern __shared__ float s_lg[];   // [RL_WARPS][gs.total]
+    __shared__ float s_warp[RL_WARPS][2];
+    __shared__ bool s_last;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.x * RL_WARPS + warp;
+    float Fv = 0.f, zv = 0.f;
+    if (b < B) {
+        float* lg = s_lg + warp * gs.total;
+        for (int i = lane; i < gs.total; i += 32) lg[i] = logits[static_cast<long long>(b) * gs.total + i];
+        __syncwarp();
+        const float mx = router_max_score(lg, gs, alive, lane);
+        float se = 0.f, sf = 0.f;
+        if (mx > -INFINITY) {
+            for (int c = lane; c < gs.num_experts; c += 32) {
+                if (alive && !alive[c]) continue;
+                const float p = __expf(pk_score(lg, gs, c) - mx);
+                se += p;
+                sf += f[c] * p;
+            }
+        }
+        se = warp_sum(se);
+        sf = warp_sum(sf);
+        if (mx > -INFINITY && se > 0.f) {
+            zv = mx + __logf(se);
+            Fv = sf / se;
+        }
+        if (lane == 0) {
+            z[b] = zv;
+            Fb[b] = Fv;
+        }
+    }
+    if (lane == 0) {
+        s_warp[warp][0] = Fv;
+        s_warp[warp][1] = zv * zv;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float a = 0.f, q = 0.f;
+#pragma unroll
+        for (int w = 0; w < RL_WARPS; ++w) {
+            a += s_warp[w][0];
+            q += s_warp[w][1];
+        }
+        partials[2 * blockIdx.x] = a;
+        partials[2 * blockIdx.x + 1] = q;
+        __threadfence();
+        s_last = atomicAdd(ticket, 1) == static_cast<int>(gridDim.x) - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    // the last CTA: thread t sums the partials t, t + 128, ... in order, then a fixed tree over the threads
+    float a = 0.f, q = 0.f;
+    for (int i = threadIdx.x; i < static_cast<int>(gridDim.x); i += blockDim.x) {
+        a += __ldcg(partials + 2 * i);
+        q += __ldcg(partials + 2 * i + 1);
+    }
+    a = warp_sum(a);
+    q = warp_sum(q);
+    if (lane == 0) {
+        s_warp[warp][0] = a;
+        s_warp[warp][1] = q;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float ta = 0.f, tq = 0.f;
+#pragma unroll
+        for (int w = 0; w < RL_WARPS; ++w) {
+            ta += s_warp[w][0];
+            tq += s_warp[w][1];
+        }
+        loss[0] = f[gs.num_experts] * ta / static_cast<float>(B);
+        loss[1] = tq / static_cast<float>(B);
+        *ticket = 0;
+    }
+}
+
+// shared memory of one warp of router_loss_bwd_kernel: the token's grid logits, then (grids of 2+ dims) the expert
+// gradients at skewed positions e + e / 32, so that lanes summing grid dimension 0 (experts i * stride + inner) do not all
+// hit one bank
+__host__ __device__ __forceinline__ int router_bwd_warp_floats(const GridSpec& gs) {
+    return gs.total + (gs.ndim > 1 ? gs.num_experts + gs.num_experts / 32 + 1 : 0);
+}
+
+// one warp per token: dlogits[b] += d/dl of (aux_coef * L_aux + z_coef * L_z) with f constant.  The expert gradient is
+// g_e = p_e (aux_coef N (f_e - F_b) + 2 z_coef z_b) / B.  On a 1-d grid it is the logit's gradient itself and is added
+// directly; otherwise it is staged in shared memory and each grid logit (d, i) is summed by one lane over the experts
+// whose d-th coordinate is i, in increasing expert order
+__global__ void __launch_bounds__(RL_WARPS * 32) router_loss_bwd_kernel(const float* __restrict__ logits, int B, GridSpec gs,
+                                                                        const unsigned char* __restrict__ alive,
+                                                                        const float* __restrict__ f,
+                                                                        const float* __restrict__ z,
+                                                                        const float* __restrict__ Fb, float aux_coef,
+                                                                        float z_coef, float* __restrict__ dlogits) {
+    extern __shared__ float s_buf[];   // [RL_WARPS][router_bwd_warp_floats(gs)]
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.x * RL_WARPS + warp;
+    if (b >= B) return;
+    float* lg = s_buf + warp * router_bwd_warp_floats(gs);
+    float* g = lg + gs.total;
+    float* dl = dlogits + static_cast<long long>(b) * gs.total;
+    for (int i = lane; i < gs.total; i += 32) lg[i] = logits[static_cast<long long>(b) * gs.total + i];
+    __syncwarp();
+    // z_b >= every live score; a token without a finite score has z_b = 0 and p = exp(-inf) = 0: no gradient
+    const float zb = z[b];
+    const float invB = 1.f / static_cast<float>(B);
+    const float base_aux = aux_coef * f[gs.num_experts];
+    const float c0 = 2.f * z_coef * zb - base_aux * Fb[b];
+    for (int c = lane; c < gs.num_experts; c += 32) {
+        float v = 0.f;
+        if (!alive || alive[c]) v = __expf(pk_score(lg, gs, c) - zb) * (base_aux * f[c] + c0) * invB;
+        if (gs.ndim == 1)
+            dl[c] += v;
+        else
+            g[c + (c >> 5)] = v;
+    }
+    if (gs.ndim == 1) return;
+    __syncwarp();
+    for (int o = lane; o < gs.total; o += 32) {
+        int d = 0;
+        while (d + 1 < gs.ndim && o >= gs.offset[d + 1]) ++d;
+        const int i = o - gs.offset[d];
+        int stride = 1;   // expert id = row-major index over the grid: the last dimension varies fastest
+        for (int dd = gs.ndim - 1; dd > d; --dd) stride *= gs.size[dd];
+        const int block = stride * gs.size[d];
+        float acc = 0.f;
+        for (int outer = 0; outer < gs.num_experts; outer += block)
+            for (int inner = 0; inner < stride; ++inner) {
+                const int e = outer + i * stride + inner;
+                acc += g[e + (e >> 5)];
+            }
+        dl[o] += acc;
+    }
+}
+
 static Peers g_peers = {};
 static bool g_peers_set = false;
 
@@ -1113,6 +1319,53 @@ int lah_gate_bwd(long long yo_off, const void* grad, const int* idx, const int* 
     else if (H == 512) gate_bwd_kernel<2><<<grid, 256, 0, st>>>(g_peers, a, gs);
     else if (H == 1024) gate_bwd_kernel<4><<<grid, 256, 0, st>>>(g_peers, a, gs);
     else return -2;
+    return -(int)cudaGetLastError();
+}
+
+// grid of the router-loss kernels: 1..MAX_GRID_DIMS positive sizes, at most LAYOUT_MAX_E grid logits and experts
+static int router_grid_spec(GridSpec* gs, const int* grid, int ndim) {
+    if (!grid || ndim < 1 || ndim > MAX_GRID_DIMS) return -2;
+    long long total = 0, experts = 1;
+    for (int d = 0; d < ndim; ++d) {
+        if (grid[d] < 1) return -2;
+        total += grid[d];
+        experts *= grid[d];
+        if (total > LAYOUT_MAX_E || experts > LAYOUT_MAX_E) return -2;
+    }
+    return make_grid_spec(gs, grid, ndim);
+}
+
+// forward of the router losses: f (E + 1 floats: f_e, then N) from the count table [count_rows][E], z_b and F_b of every
+// token ([B] each), loss = (L_aux, L_z).  partials: 2 * ceil(B / 4) floats; ticket: one int that is 0 between calls
+int lah_router_loss_fwd(const float* logits, int B, const int* grid, int ndim, const unsigned char* alive, const int* counts,
+                        int count_rows, float* f, float* z, float* Fb, float* loss, float* partials, int* ticket,
+                        cudaStream_t st) {
+    GridSpec gs;
+    if (router_grid_spec(&gs, grid, ndim)) return -2;
+    if (B < 0 || count_rows < 1 || count_rows > MAX_WORLD) return -3;
+    if (!counts || !f || !loss || (B > 0 && (!logits || !z || !Fb || !partials || !ticket))) return -4;
+    if (int e = set_max_dynamic_smem<router_loss_fwd_kernel>(RL_WARPS * sizeof(float) * LAYOUT_MAX_E)) return e;
+    router_f_kernel<<<1, 1024, 0, st>>>(counts, count_rows, gs.num_experts, alive, f, B, loss);
+    if (B > 0)
+        router_loss_fwd_kernel<<<(B + RL_WARPS - 1) / RL_WARPS, RL_WARPS * 32, RL_WARPS * gs.total * sizeof(float), st>>>(
+            logits, B, gs, alive, f, z, Fb, partials, ticket, loss);
+    return -(int)cudaGetLastError();
+}
+
+// backward of the router losses: dlogits [B, sum(grid)] += the gradient of aux_coef * L_aux + z_coef * L_z
+int lah_router_loss_bwd(const float* logits, int B, const int* grid, int ndim, const unsigned char* alive, const float* f,
+                        const float* z, const float* Fb, float aux_coef, float z_coef, float* dlogits, cudaStream_t st) {
+    GridSpec gs;
+    if (router_grid_spec(&gs, grid, ndim)) return -2;
+    if (B < 0) return -3;
+    if (B > 0 && (!logits || !f || !z || !Fb || !dlogits)) return -4;
+    if (int e = set_max_dynamic_smem<router_loss_bwd_kernel>(RL_WARPS * sizeof(float) *
+                                                              (2 * LAYOUT_MAX_E + LAYOUT_MAX_E / 32 + 1)))
+        return e;
+    if (B == 0) return 0;
+    router_loss_bwd_kernel<<<(B + RL_WARPS - 1) / RL_WARPS, RL_WARPS * 32,
+                             RL_WARPS * router_bwd_warp_floats(gs) * sizeof(float), st>>>(logits, B, gs, alive, f, z, Fb,
+                                                                                         aux_coef, z_coef, dlogits);
     return -(int)cudaGetLastError();
 }
 

@@ -51,6 +51,8 @@ def _lib():
         "lah_signal_wait": [L, I, I, I, I, P, P],
         "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P],
         "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P],
+        "lah_router_loss_fwd": [P, I, P, I, P, P, I, P, P, P, P, P, P, P],
+        "lah_router_loss_bwd": [P, I, P, I, P, P, P, P, Fl, Fl, P, P],
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
                           I, P],
         "lah_bump_steps": [P, P, I, P],
@@ -404,6 +406,87 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
                                      stream_ptr()),
                  "lah_gate_bwd")
     native.count_launch()
+    return dlogits
+
+
+# ---------------------------------------------------------------------------------------------------------
+# router losses of the product-key gate (load balancing + z-loss; csrc/moe.cu router_*_kernel)
+# ---------------------------------------------------------------------------------------------------------
+MAX_GRID_DIMS = 4        # csrc/moe.cu MAX_GRID_DIMS
+LAYOUT_MAX_E = 4096      # csrc/moe.cu LAYOUT_MAX_E: most experts (and grid logits) of a gate
+ROUTER_WARPS = 4         # tokens per CTA of the router-loss kernels
+
+
+def check_router_grid(grid_size):
+    """the grids the router-loss kernels take: 1..MAX_GRID_DIMS positive sizes, at most LAYOUT_MAX_E experts and logits"""
+    grid = tuple(int(g) for g in grid_size)
+    if not 1 <= len(grid) <= MAX_GRID_DIMS or min(grid) < 1 or sum(grid) > LAYOUT_MAX_E or math.prod(grid) > LAYOUT_MAX_E:
+        raise ValueError(f"router losses: grid_size must have 1..{MAX_GRID_DIMS} positive sizes with at most "
+                         f"{LAYOUT_MAX_E} experts, got {grid_size}")
+    return grid
+
+
+def _router_args(what, logits, grid_size, alive):
+    grid = check_router_grid(grid_size)
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.shape[1] != sum(grid) or not logits.is_contiguous():
+        raise ValueError(f"{what}: logits must be a contiguous float32 [B, {sum(grid)}] tensor, got {logits.dtype} "
+                         f"{tuple(logits.shape)}")
+    E = math.prod(grid)
+    if alive is not None and (alive.dtype != torch.uint8 or alive.numel() != E or not alive.is_contiguous()):
+        raise ValueError(f"{what}: alive must be a contiguous uint8 tensor of {E} entries, got {alive.dtype} "
+                         f"{tuple(alive.shape)}")
+    return grid, logits.shape[0], E
+
+
+def router_loss_fwd(logits, grid_size, counts, *, alive=None, f, z, Fb, loss, partials=None, ticket=None):
+    """Router losses of one training forward (two launches).  ``counts``: int32 [R, E] count table (one row per rank,
+    R <= MAX_WORLD), summed over its rows.  Writes f (float32 [E + 1]: f_e = c_e / sum c, then N = live experts), z and
+    Fb (float32, >= B entries: logsumexp z_b and F_b = sum_e f_e p_{b,e}) and loss (float32 [2]: unweighted L_aux, L_z).
+    ``partials`` (float32, >= 2 * ceil(B / ROUTER_WARPS)) and ``ticket`` (int32 [1], zero between calls) are scratch,
+    allocated when None."""
+    grid, B, E = _router_args("router_loss_fwd", logits, grid_size, alive)
+    if counts.dtype != torch.int32 or counts.dim() != 2 or counts.shape[1] != E or not counts.is_contiguous() \
+            or not 1 <= counts.shape[0] <= MAX_WORLD:
+        raise ValueError(f"router_loss_fwd: counts must be a contiguous int32 [R <= {MAX_WORLD}, {E}] tensor, got "
+                         f"{counts.dtype} {tuple(counts.shape)}")
+    nblk = (B + ROUTER_WARPS - 1) // ROUTER_WARPS
+    if partials is None:
+        partials = torch.empty(max(1, 2 * nblk), dtype=torch.float32, device=logits.device)
+    if ticket is None:
+        ticket = torch.zeros(1, dtype=torch.int32, device=logits.device)
+    _f32_vec(f, "router_loss_fwd: f", E + 1)
+    _f32_vec(loss, "router_loss_fwd: loss", 2)
+    for t, name, n in ((z, "z", B), (Fb, "Fb", B), (partials, "partials", 2 * nblk)):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() < n:
+            raise ValueError(f"router_loss_fwd: {name} must be a contiguous float32 tensor of >= {n} entries, got "
+                             f"{t.dtype} {tuple(t.shape)}")
+    if ticket.dtype != torch.int32 or ticket.numel() < 1:
+        raise ValueError("router_loss_fwd: ticket must be an int32 tensor")
+    native.check(_lib().lah_router_loss_fwd(ptr(logits), B, ctypes.cast(_grid_array(grid), c_void_p), len(grid),
+                                            ptr(alive), ptr(counts), counts.shape[0], ptr(f), ptr(z), ptr(Fb), ptr(loss),
+                                            ptr(partials), ptr(ticket), stream_ptr()), "lah_router_loss_fwd")
+    native.count_launch(2 if B > 0 else 1)
+    return loss
+
+
+def router_loss_bwd(logits, grid_size, *, alive=None, f, z, Fb, aux_coef, z_coef, dlogits):
+    """dlogits += the gradient of aux_coef * L_aux + z_coef * L_z w.r.t. the grid logits (f constant), from the f, z and
+    Fb the forward wrote for the same logits (one launch)"""
+    grid, B, E = _router_args("router_loss_bwd", logits, grid_size, alive)
+    _f32_vec(f, "router_loss_bwd: f", E + 1)
+    for t, name in ((z, "z"), (Fb, "Fb")):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() < B:
+            raise ValueError(f"router_loss_bwd: {name} must be a contiguous float32 tensor of >= {B} entries")
+    if dlogits.dtype != torch.float32 or tuple(dlogits.shape) != tuple(logits.shape) or not dlogits.is_contiguous():
+        raise ValueError(f"router_loss_bwd: dlogits must be a contiguous float32 {tuple(logits.shape)} tensor, got "
+                         f"{dlogits.dtype} {tuple(dlogits.shape)}")
+    if not (math.isfinite(aux_coef) and math.isfinite(z_coef)):
+        raise ValueError("router_loss_bwd: the coefficients must be finite")
+    native.check(_lib().lah_router_loss_bwd(ptr(logits), B, ctypes.cast(_grid_array(grid), c_void_p), len(grid),
+                                            ptr(alive), ptr(f), ptr(z), ptr(Fb), float(aux_coef), float(z_coef),
+                                            ptr(dlogits), stream_ptr()), "lah_router_loss_bwd")
+    if B > 0:
+        native.count_launch()
     return dlogits
 
 
@@ -929,6 +1012,29 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None):
     w = torch.softmax(top_v.masked_fill(~valid, float("-inf")), dim=-1)
     w = torch.where(valid, w, torch.zeros_like(w)).nan_to_num(0.0)
     return torch.where(valid, top_i, torch.full_like(top_i, -1)), w
+
+
+def router_loss_ref(logits, grid_size, counts, alive=None):
+    """Oracle of the router-loss kernels: (L_aux, L_z) as 0-d tensors in the dtype of ``logits`` (float64 works),
+    differentiable in the logits with f detached.  ``counts``: [E] routed pairs per expert, or [R, E] (summed over R).
+    L_aux = N * sum_e f_e * mean_b p_{b,e} over the N live experts, L_z = mean_b z_b^2; a token without a finite live
+    score contributes 0 to both, and N = 0 gives zeros."""
+    scores = product_key_scores(logits, grid_size)
+    B, E = scores.shape
+    live = torch.ones(E, dtype=torch.bool, device=scores.device) if alive is None else alive.bool().reshape(-1).to(scores.device)
+    c = counts.reshape(-1, E).sum(0).to(scores.dtype).to(scores.device)
+    f = (c / c.sum() if float(c.sum()) > 0 else torch.zeros_like(c)).detach()
+    N = int(live.sum())
+    masked = scores.masked_fill(~live.view(1, -1), float("-inf"))
+    ok = torch.isfinite(masked).any(-1, keepdim=True)   # tokens with at least one finite live score
+    masked = torch.where(ok, masked, torch.zeros_like(masked))
+    if N == 0 or B == 0:
+        zero = scores.sum() * 0
+        return zero, zero
+    z = torch.logsumexp(masked, -1, keepdim=True)
+    p = torch.where(live.view(1, -1) & ok, torch.exp(masked - z), torch.zeros_like(masked))
+    z = torch.where(ok, z, torch.zeros_like(z)).squeeze(-1)
+    return N * (p * f).sum() / B, (z * z).sum() / B
 
 
 _SPLITMIX_GAMMA = 0x9E3779B97F4A7C15

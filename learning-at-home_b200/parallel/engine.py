@@ -108,6 +108,14 @@ class DMoEConfig:
     expert: str = "ffn"
     # inner width of a "swiglu" expert; 0 = gated_inner_dim(hidden).  "ffn" is fixed at 4 * hidden (must stay 0)
     inner_dim: int = 0
+    # router losses of the product-key gate (DESIGN.md §6a): every training forward adds the gradient of
+    # router_aux_loss_coef * L_aux + router_z_loss_coef * L_z to the gate's logits in its backward, so the objective is the
+    # task loss plus the sum over layers of those terms.  L_aux = N * sum_e f_e * mean_b p_{b,e} is the load-balancing loss
+    # of Switch / GShard (f_e: share of the box-wide routed pairs that went to expert e, p: softmax over the N live experts),
+    # L_z = mean_b logsumexp_e(s_{b,e})^2 the router z-loss of ST-MoE.  A layer reads them at construction: they are fixed
+    # for the life of a layer or trainer.  0 and 0 (the default) launch nothing
+    router_aux_loss_coef: float = 0.0
+    router_z_loss_coef: float = 0.0
 
     def __post_init__(self):
         if self.expert not in EXPERT_LAYOUTS:
@@ -120,6 +128,18 @@ class DMoEConfig:
         if self.expert == "swiglu" and self.expert_dtype != "bf16":
             raise ValueError("expert='swiglu' runs bf16 expert GEMMs only (its RMSNorm and SwiGLU kernels do not emit "
                              f"MXFP8 operands); got expert_dtype={self.expert_dtype!r}")
+        for name in ("router_aux_loss_coef", "router_z_loss_coef"):
+            v = float(getattr(self, name))
+            if not math.isfinite(v) or v < 0.0:
+                raise ValueError(f"DMoEConfig.{name} must be a finite value >= 0, got {v}")
+            if v > 0.0 and self.gate_mode == "emulator":
+                raise ValueError(f"DMoEConfig.{name}: the emulator gate is frozen (not trained), so a router loss would "
+                                 "train nothing; use gate_mode='product_key'")
+
+    @property
+    def router_losses(self) -> bool:
+        """a router loss is trained (a coefficient is nonzero)"""
+        return self.router_aux_loss_coef > 0.0 or self.router_z_loss_coef > 0.0
 
     def check_native_sizes(self):
         """the widths the sm_90a kernels run for this expert (the CPU oracle path takes any size)"""
@@ -177,6 +197,13 @@ class DMoEConfig:
 
     def seg_shapes(self) -> Dict[str, Tuple[int, ...]]:
         return self.layout.shapes(self.hidden, self.inner)
+
+
+def refuse_router_losses(cfg: DMoEConfig, arm: str):
+    """the baseline arms train no router loss: refuse nonzero coefficients instead of silently dropping them"""
+    if cfg.router_losses:
+        raise ValueError(f"{arm} does not train router losses; set router_aux_loss_coef and router_z_loss_coef to 0 "
+                         "(FusedDMoE / DMoETrainer train them)")
 
 
 def expert_uid(cfg: DMoEConfig, e: int) -> str:
@@ -277,6 +304,10 @@ class EngineContext:
         # transient backward buffers shared by all layers
         self.gyd, self.gyd_off = self.heap.alloc((self.max_rows, H), torch.bfloat16)
         self.dxd, self.dxd_off = self.heap.alloc((self.max_rows, H), torch.bfloat16)
+        if cfg.router_losses:   # scratch of the router-loss forward, shared by all layers: per-CTA sums and a CTA ticket
+            blocks = -(-cfg.tokens_per_rank // K.ROUTER_WARPS)
+            self.router_partials = torch.zeros(2 * blocks, dtype=torch.float32, device=self.device)
+            self.router_ticket = torch.zeros(1, dtype=torch.int32, device=self.device)
         bf = dict(dtype=torch.bfloat16, device=self.device)
         # the expert's backward temporaries (FeedforwardBlock: da, dh; GatedFeedforwardBlock: da, dh = [dg | du], dn)
         for name, width in cfg.layout.buffers(H, cfg.inner)["scratch"].items():
@@ -581,6 +612,14 @@ class LayerWorkspace:
         self.owned_shadow = torch.full((ctx.E_loc * 2,), -1, **i32)
         self.tile_group = torch.full((ctx.max_tiles,), -1, **i32)
         self.total_rows = torch.zeros(1, **i32)
+        self.router_loss = None
+        if cfg.router_losses:
+            # router losses: f (box-wide routing shares, snapshotted from the count table the next layer overwrites, then
+            # N), z_b and F_b of every token for the backward, and the layer's unweighted (L_aux, L_z)
+            self.router_f = torch.zeros(ctx.E + 1, **f32)
+            self.router_z = torch.zeros(cfg.tokens_per_rank, **f32)
+            self.router_F = torch.zeros(cfg.tokens_per_rank, **f32)
+            self.router_loss = torch.zeros(2, **f32)
         self.outstanding = False   # a training-mode forward whose backward has not run yet owns this workspace
         # small path with optimizer overlap: the fused wgrad+AMSGrad kernels of layer L read dY buffers while the main stream is
         # already in the backward of layer L-1, so they must be per layer (a few MB each at this batch size)
@@ -610,13 +649,17 @@ class _FusedDMoEFunction(torch.autograd.Function):
                                "backward, or call layer.release_workspace() to drop the pending forward)")
         ctx.tracked = bool(x.requires_grad or logits.requires_grad)
         ws.outstanding = ctx.tracked
+        ctx.router = layer.training and layer.router_on
+        if ctx.router:
+            ctx.save_for_backward(logits)
         return layer._forward_cuda(x, logits)
 
     @staticmethod
     def backward(ctx, grad_out):
         if not ctx.layer.ws.outstanding:
             raise RuntimeError("FusedDMoE: backward() without a pending forward (the workspace was released or reused)")
-        dx, dlogits = ctx.layer._backward_cuda(grad_out.contiguous(), ctx.B)
+        logits = ctx.saved_tensors[0] if ctx.router else None
+        dx, dlogits = ctx.layer._backward_cuda(grad_out.contiguous(), ctx.B, logits)
         ctx.layer.ws.outstanding = False
         ec = ctx.layer.ctx
         if ec._opt_pending and not ec.defer_join:
@@ -624,6 +667,20 @@ class _FusedDMoEFunction(torch.autograd.Function):
             # expert optimizers on the second stream, so reading the parameters right after backward() is safe
             torch.autograd.Variable._execution_engine.queue_callback(ec.join_optimizer_stream)
         return dx, dlogits, None
+
+
+class _AddRouterLoss(torch.autograd.Function):
+    """identity on the layer output whose backward also sends gradient 1 into the router-loss term: the term joins the
+    objective without the caller adding it to the loss (the CPU counterpart of the router-loss kernels)"""
+
+    @staticmethod
+    def forward(ctx, out, aux):
+        ctx.aux_dtype = aux.dtype
+        return out.view_as(out)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        return grad_out, torch.ones((), dtype=ctx.aux_dtype, device=grad_out.device)
 
 
 class FusedDMoE(nn.Module):
@@ -636,6 +693,10 @@ class FusedDMoE(nn.Module):
 
     def __init__(self, cfg: DMoEConfig, ctx: Optional[EngineContext] = None, layer_index: int = 0, device=None):
         super().__init__()
+        if ctx is not None and cfg.router_losses and not ctx.cfg.router_losses:
+            # the router-loss buffers (per layer and the shared scratch) are allocated from the context's configuration
+            raise ValueError("FusedDMoE: router losses need an EngineContext built from a DMoEConfig with a nonzero "
+                             "router_aux_loss_coef or router_z_loss_coef (the context allocates their buffers)")
         self.cfg, self.ctx, self.layer_index = cfg, ctx, layer_index
         self.grid_size = tuple(cfg.grid_size)
         if cfg.gate_mode == "emulator":
@@ -657,6 +718,16 @@ class FusedDMoE(nn.Module):
         self.ref_emulate_bf16 = False   # oracle path: round activations / weights to bf16 where the GPU path stores bf16
         self._ref_rows = None
         self._ref_leaves = {}   # CPU mode: local expert -> {segment: leaf view} of the experts used since the last update
+        # router losses (cfg.router_*_coef, read here once): the unweighted (L_aux, L_z) of the last training forward, this
+        # rank's term, on the layer's device (kernels write it on the GPU path, so it stays valid after graph replay)
+        self.router_aux_coef = float(cfg.router_aux_loss_coef)
+        self.router_z_coef = float(cfg.router_z_loss_coef)
+        self.router_on = self.router_aux_coef > 0.0 or self.router_z_coef > 0.0
+        self.router_grad_scale = 1.0   # DMoETrainer: 1 / trainer_microbatches, like each micro-batch's cross-entropy
+        if self.ws is not None:   # written by the kernels at a fixed address (a captured graph holds it)
+            self.router_loss = self.ws.router_loss if self.router_on else None
+        else:                     # a buffer, so that .to() / .cuda() move it with the layer (not saved in state_dict)
+            self.register_buffer("router_loss", torch.zeros(2, device=dev) if self.router_on else None, persistent=False)
 
     # ------------------------------------------------------------------ public forward
     def forward(self, x):
@@ -716,6 +787,11 @@ class FusedDMoE(nn.Module):
                           tile_group=ws.tile_group, total_rows=ws.total_rows, status=c.status, shadow_slots=c.S,
                           shadow_tol=cfg.shadow_tol, min_shadow_rows=cfg.shadow_min_rows, route_owner=ws.route_owner,
                           step_rows=ws.step_rows, shadow_info=ws.shadow_info, owned_shadow=ws.owned_shadow)
+        if self.training and self.router_on:
+            # before combine_rows: no peer can reach the next layer's count exchange (which rewrites cnt_all) until this
+            # rank's combine has signalled
+            K.router_loss_fwd(logits, self.grid_size, c.cnt_all[:c.world], alive=c.alive, f=ws.router_f, z=ws.router_z,
+                              Fb=ws.router_F, loss=ws.router_loss, partials=c.router_partials, ticket=c.router_ticket)
         if c.S:  # replicas of this step's hot experts: weights from the owners' bf16 mirror, small params from fp32
             K.pull_shadow(ws.shadow_info, c.S, c.E_loc, sh.p_off, sh.pbf16_off, sh.seg_sizes, sh.layout.small_mask)
             sh.w8_dirty = True
@@ -791,7 +867,8 @@ class FusedDMoE(nn.Module):
         K.ln_relu_fwd(ws.h2, sh.views["g2"], sh.views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, quant=ws.aq)
         fp8.grouped_linear_fp8(ws.aq, w8["w3"], tile_group=tg, bias=sh.views["b3"], residual=ws.xd, out=ws.yo)
 
-    def _backward_cuda(self, gy, B):
+    def _backward_cuda(self, gy, B, logits=None):
+        """:param logits: the gate logits of the forward when it computed router losses (their gradient is added here)"""
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         k = cfg.k
         P = B * k
@@ -800,6 +877,10 @@ class FusedDMoE(nn.Module):
         gy = gy.to(torch.bfloat16)
         dlogits = torch.empty(B, sum(self.grid_size), dtype=torch.float32, device=gy.device)
         K.gate_bwd(ws.yo_off, gy, idx, pair_row, w, dlogits, k, c.E_loc, self.grid_size, route_owner=ws.route_owner)
+        if logits is not None:
+            K.router_loss_bwd(logits, self.grid_size, alive=c.alive, f=ws.router_f, z=ws.router_z, Fb=ws.router_F,
+                              aux_coef=self.router_aux_coef * self.router_grad_scale,
+                              z_coef=self.router_z_coef * self.router_grad_scale, dlogits=dlogits)
         K.scatter_rows(gy, w, idx, pos, None, pair_row, ws.gyd_off, c.flags_off, K.SLOT_GRAD, epoch, k, c.E_loc,
                        c.max_rows, ws.group_off, ws.group_rows, c.done_counter, c.status, align=c.align,
                        route_owner=ws.route_owner, num_groups=c.G_tot)
@@ -1010,6 +1091,15 @@ class FusedDMoE(nn.Module):
             tok, slot = torch.nonzero(idx == e, as_tuple=True)
             ye = self._expert_ref(p, rnd(xf[tok]), rnd)
             out = out.index_put((tok,), ye * weights[tok, slot].unsqueeze(-1), accumulate=True)
+        if self.training and self.router_on:
+            alive = self.ctx.alive if self.ctx is not None else getattr(self, "alive_ref", None)
+            counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
+            l_aux, l_z = K.router_loss_ref(logits, self.grid_size, counts, alive=alive)
+            with torch.no_grad():
+                self.router_loss.copy_(torch.stack([l_aux, l_z]).detach())
+            if torch.is_grad_enabled() and logits.requires_grad:
+                aux = self.router_grad_scale * (self.router_aux_coef * l_aux + self.router_z_coef * l_z)
+                out = _AddRouterLoss.apply(out, aux)
         return out.to(x.dtype)
 
     def _expert_ref(self, p, xe, rnd):

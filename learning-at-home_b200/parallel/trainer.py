@@ -64,6 +64,8 @@ class DMoETrainer:
             self.ctx, self.device, self.world, self.rank = None, torch.device("cpu"), 1, 0
         torch.manual_seed(cfg.seed)  # identical trainer parameters on every rank
         self.model = DMoEClassifier(cfg, self.ctx, device=self.device).to(self.device)
+        for block in self.model.blocks:   # every micro-batch's router gradient is scaled like its cross-entropy
+            block.router_grad_scale = 1.0 / max(1, int(cfg.trainer_microbatches))
         self._flatten_trainer_params()
         self.step_count = 0
         # automatic: whenever a step is short enough to be launch-bound (always on the small path; on the big path up to a few
@@ -298,9 +300,13 @@ class DMoETrainer:
             layers = []
             for block in self.model.blocks:
                 rows = block.ws.step_rows.float()
-                layers.append(dict(active_experts=int((rows > 0).sum()), max_rows=int(rows.max()),
-                                   mean_rows=float(rows.mean()), padded_rows=int(block.ws.total_rows.item()),
-                                   shadowed_experts=int((block.ws.shadow_info.view(-1, 4)[:, 0] >= 0).sum())))
+                layer = dict(active_experts=int((rows > 0).sum()), max_rows=int(rows.max()),
+                             mean_rows=float(rows.mean()), padded_rows=int(block.ws.total_rows.item()),
+                             shadowed_experts=int((block.ws.shadow_info.view(-1, 4)[:, 0] >= 0).sum()))
+                if block.router_loss is not None:   # this rank's unweighted router losses of the layer's last forward
+                    aux, z = block.router_loss.tolist()
+                    layer.update(router_aux_loss=aux, router_z_loss=z)
+                layers.append(layer)
             rec["layers"] = layers
             if self.last_stage_ms:
                 rec["stage_ms"] = dict(self.last_stage_ms)

@@ -9,8 +9,10 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.distributed as dist
+import torch.nn.functional as F
 
 import lah_b200  # noqa
+from lah_b200.ops import kernels as K
 from lah_b200.parallel import engine as E
 
 
@@ -26,10 +28,12 @@ def main():
     force_shadow = "--force-shadow" in sys.argv  # shadow as many experts as there are slots (exercises the replica path)
     small = "--small" in sys.argv   # weight-streaming expert path (swap-AB GEMMs + fused wgrad/AMSGrad; no shadowing)
     swiglu = "--swiglu" in sys.argv   # GatedFeedforwardBlock experts (compares [W1; W3] and the RMSNorm weight)
+    # router losses of the product-key gate: f from the box-wide count table, P from each rank's own tokens
+    router = dict(router_aux_loss_coef=0.01, router_z_loss_coef=0.001) if "--router-loss" in sys.argv else {}
     mat, vec = ("w13", "g") if swiglu else ("w1", "b2")
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=B, capacity_factor=float(max(4, world)),
                        shadow_experts=4, shadow_tol=0.0 if force_shadow else 1.1, shadow_min_rows=1 if force_shadow else 64,
-                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn")
+                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router)
     ctx = E.EngineContext(cfg)
     torch.manual_seed(0)  # identical gate on every rank (DMoETrainer does the same)
     layer = E.FusedDMoE(cfg, ctx).cuda()
@@ -55,6 +59,10 @@ def main():
     dist.all_gather(dxs, x.grad.contiguous())
     gw = layer.proj.weight.grad.clone()
     dist.all_reduce(gw)
+    if router:   # the mean over ranks of the per-rank losses is the box-wide value
+        rl = layer.router_loss.clone()
+        dist.all_reduce(rl)
+        rl /= world
     w1 = layer.shard.views[mat][:layer.E_loc].clone()
     w1s = [torch.empty_like(w1) for _ in range(world)]
     dist.all_gather(w1s, w1)
@@ -63,11 +71,23 @@ def main():
     dist.all_gather(b2s, b2)
     steps = [torch.empty_like(layer.shard.step) for _ in range(world)]
     dist.all_gather(steps, layer.shard.step)
+    if router:
+        # the router gradient alone: a second step with a zero output gradient, where gate_bwd adds exactly 0 to the gate
+        # logits.  Summed over ranks, it is the gradient of the whole-batch losses times the world size
+        layer.proj.weight.grad = None
+        layer(x.detach()).backward(torch.zeros(B, 512, dtype=torch.bfloat16, device="cuda"))
+        torch.cuda.synchronize()
+        ctx.check_status()
+        g_router = layer.proj.weight.grad.clone()
+        dist.all_reduce(g_router)
+        counts_box = ctx.cnt_all[:world].clone()   # the box-wide count table of that step, the same on every rank
     ok = True
     if rank == 0:
         # single-GPU reference in the same process: a fresh world-1 context is impossible inside an initialised group,
         # so use the PyTorch oracle of the layer (all experts local) on the whole batch
-        ref_cfg = cfg
+        # the gate gradients are SUMMED over ranks here (a trainer averages them): the router part of that sum is the
+        # gradient of the whole-batch losses times the world size
+        ref_cfg = E.DMoEConfig(**{**cfg.__dict__, **{k: v * world for k, v in router.items()}}) if router else cfg
         ref = E.FusedDMoE(ref_cfg, None, device=torch.device("cuda")).cuda()
         ref.proj.load_state_dict(layer.proj.state_dict())
         ref.train()
@@ -79,9 +99,18 @@ def main():
                     w1_mean_abs=(torch.cat(w1s) - ref.shard.views[mat]).abs().mean().item(),
                     b2_max_abs=(torch.cat(b2s) - ref.shard.views[vec]).abs().max().item(),
                     steps=bool((torch.cat(steps).cpu() == ref.shard.step.cpu()).all()))
+        if router:
+            errs["router_loss"] = rel(rl, ref.router_loss)
+            xa = x_all.cuda()
+            l64 = F.linear(xa.float(), layer.proj.weight, layer.proj.bias).detach().double().requires_grad_(True)
+            aux, zl = K.router_loss_ref(l64, cfg.grid_size, counts_box)
+            (g,) = torch.autograd.grad(world * (cfg.router_aux_loss_coef * aux + cfg.router_z_loss_coef * zl), l64)
+            ref_router = g.t() @ xa.double()
+            errs["router_grad_max_err"] = ((g_router.double() - ref_router).abs().max() / ref_router.abs().max()).item()
         ok = errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2 and errs["w1_mean_abs"] < 1e-4 and errs["b2_max_abs"] < 2.5e-3 and errs["steps"]
-        ok = ok and (shadowed > 0 or not force_shadow) and plan_ok
-        print("multi_gpu_check", dict(path="small" if small else "big", expert=cfg.expert, force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
+        ok = ok and (shadowed > 0 or not force_shadow) and plan_ok and errs.get("router_loss", 0.0) < 1e-4
+        ok = ok and errs.get("router_grad_max_err", 0.0) < 1e-4
+        print("multi_gpu_check", dict(path="small" if small else "big", expert=cfg.expert, router_loss=bool(router), force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
                                       plan=plan, kernel=got), errs, flush=True)
         print("MULTI_GPU_OK" if ok else "MULTI_GPU_FAILED", flush=True)
     dist.barrier()
