@@ -155,6 +155,45 @@ __global__ void cast_bf16_kernel(const float* __restrict__ src, bf16* __restrict
     }
 }
 
+// split master weight (split_decode, sm90.cuh): hi, lo and the tie bits in the sign of v from p
+__global__ void split_encode_kernel(const float* __restrict__ p, bf16* __restrict__ hi, uint16_t* __restrict__ lo,
+                                    float* __restrict__ v, long long n) {
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
+    for (long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; i < n; i += stride) {
+        const float4 w = *reinterpret_cast<const float4*>(p + i);
+        float4 s = *reinterpret_cast<const float4*>(v + i);
+        uint2 h, l;
+        h.x = pack_bf16x2(w.x, w.y);
+        h.y = pack_bf16x2(w.z, w.w);
+        l.x = (__float_as_uint(w.x) & 0xffffu) | (__float_as_uint(w.y) << 16);
+        l.y = (__float_as_uint(w.z) & 0xffffu) | (__float_as_uint(w.w) << 16);
+        s.x = with_tie_bit(without_tie_bit(s.x), split_tie_up(w.x));
+        s.y = with_tie_bit(without_tie_bit(s.y), split_tie_up(w.y));
+        s.z = with_tie_bit(without_tie_bit(s.z), split_tie_up(w.z));
+        s.w = with_tie_bit(without_tie_bit(s.w), split_tie_up(w.w));
+        *reinterpret_cast<uint2*>(hi + i) = h;
+        *reinterpret_cast<uint2*>(lo + i) = l;
+        *reinterpret_cast<float4*>(v + i) = s;
+    }
+}
+
+// p from hi, lo and the tie bits
+__global__ void split_decode_kernel(const bf16* __restrict__ hi, const uint16_t* __restrict__ lo,
+                                    const float* __restrict__ v, float* __restrict__ p, long long n) {
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
+    for (long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; i < n; i += stride) {
+        const uint2 h = *reinterpret_cast<const uint2*>(hi + i);
+        const uint2 l = *reinterpret_cast<const uint2*>(lo + i);
+        const float4 s = *reinterpret_cast<const float4*>(v + i);
+        float4 w;
+        w.x = split_decode(h.x & 0xffffu, l.x & 0xffffu, __float_as_uint(s.x) >> 31);
+        w.y = split_decode(h.x >> 16, l.x >> 16, __float_as_uint(s.y) >> 31);
+        w.z = split_decode(h.y & 0xffffu, l.y & 0xffffu, __float_as_uint(s.z) >> 31);
+        w.w = split_decode(h.y >> 16, l.y >> 16, __float_as_uint(s.w) >> 31);
+        *reinterpret_cast<float4*>(p + i) = w;
+    }
+}
+
 }  // namespace lah
 
 using namespace lah;
@@ -241,6 +280,19 @@ int lah_cast_bf16(const float* src, void* dst, long long n, cudaStream_t st) {
     long long blocks = (n / 4 + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
     cast_bf16_kernel<<<(int)blocks, 256, 0, st>>>(src, (bf16*)dst, n);
+    return -(int)cudaGetLastError();
+}
+
+// split master weight of n values: encode == 1 writes hi, lo and v's tie bits from p; encode == 0 writes p from them
+int lah_split_master(float* p, void* hi, void* lo, float* v, long long n, int encode, cudaStream_t st) {
+    if (n % 4) return -2;
+    if (n <= 0) return 0;
+    long long blocks = (n / 4 + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    if (encode)
+        split_encode_kernel<<<(int)blocks, 256, 0, st>>>(p, (bf16*)hi, (uint16_t*)lo, v, n);
+    else
+        split_decode_kernel<<<(int)blocks, 256, 0, st>>>((const bf16*)hi, (const uint16_t*)lo, v, p, n);
     return -(int)cudaGetLastError();
 }
 

@@ -343,6 +343,20 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
     __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
     return __bfloat1622float2(v);
 }
+// Split master weight: an fp32 weight with bits b is kept as hi = RNE_bf16(b) (the GEMM operand, exactly the mirror of
+// pack_bf16x2) and lo = b & 0xffff.  hi - (b >> 16) is 1 when the cast rounded up, which lo tells except at a tie
+// (lo == 0x8000): there `tie_up` (b >> 16 odd) is kept in the sign bit of the weight's exp_avg_sq, which is >= +0 and
+// read and written in the same pass.  Exact for every finite weight.
+__device__ __forceinline__ float split_decode(uint32_t hi, uint32_t lo, bool tie_up) {
+    const uint32_t up = (lo > 0x8000u || (lo == 0x8000u && tie_up)) ? 1u : 0u;
+    return __uint_as_float(((hi - up) << 16) | lo);
+}
+__device__ __forceinline__ uint32_t split_tie_up(float p) {   // 1 << 31 when p's cast to bf16 is a tie rounded up
+    const uint32_t b = __float_as_uint(p);
+    return ((b & 0xffffu) == 0x8000u && (b & 0x10000u)) ? 0x80000000u : 0u;
+}
+__device__ __forceinline__ float with_tie_bit(float v, uint32_t tie) { return __uint_as_float(__float_as_uint(v) | tie); }
+__device__ __forceinline__ float without_tie_bit(float v) { return __uint_as_float(__float_as_uint(v) & 0x7fffffffu); }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -18,7 +18,9 @@
 //                      (loaded while the MMAs run), every thread updates them in shared memory at the positions of its
 //                      accumulator registers and writes the bf16 mirror, and the chunk goes back to HBM by TMA store.
 //                      The weight gradient never exists in HBM: 34 B / parameter
-//                      instead of 46 (wgrad write 4 + Adam 38 + re-read 4).
+//                      instead of 46 (wgrad write 4 + Adam 38 + re-read 4).  The SPLIT instantiation keeps the master
+//                      weight as its bf16 mirror plus a 16-bit low half (split_decode, sm90.cuh): both planes stream
+//                      through the ring like the rest of the state, and nothing is stored from registers: 32 B / parameter.
 //                      Reference semantics: one torch.optim.Adam(amsgrad=True) step per expert right after its backward
 //                      (/root/reference/lib/runtime/expert_backend.py:90-97).
 #include "sm90.cuh"
@@ -340,30 +342,51 @@ struct Tile {
     int g, mt, nt;
 };
 
-// state tensor maps: p, m, v, vmax viewed as [G * N / 16][16][K] fp32 (vmax only read when amsgrad)
+// state tensor maps: p, m, v, vmax viewed as [G * N / 16][16][K] fp32 (vmax only read when amsgrad).  SPLIT: the hi and lo
+// planes of the master weight as [G * N / 16][16][K] 16-bit, then m, v, vmax
+template <bool SPLIT>
 struct StateMaps {
-    CUtensorMap a[4];
+    CUtensorMap a[SPLIT ? 5 : 4];
 };
+// SPLIT: a chunk's 16 KB of p hold the two planes, 8 KB each as two [8 bands][4 rows][64 x 16 bit] boxes (128-B swizzle);
+// m, v and vmax keep their places
+constexpr int PLANE_COLS = 64;
+constexpr int PLANE_BYTES = ARR_BYTES / 2;
+static_assert(PLANE_BYTES == (BN_MAX / PLANE_COLS) * SUB_BYTES, "a plane box has the rows and bytes of an fp32 box");
 
-// TMA load (bar != nullptr) or store of chunk c of the tile whose rows start at srow and columns at col0, arrays [0, n_arr)
-__device__ __forceinline__ void state_chunk_tma(const StateMaps& tm, int n_arr, uint8_t* ss, uint64_t* bar, int col0, int srow,
-                                                int c) {
-    for (int a = 0; a < n_arr; ++a)
+// TMA load (bar != nullptr) or store of chunk c of the tile whose rows start at srow and columns at col0, 16-KB arrays
+// [0, n_arr) (array 0: p, or the two planes)
+template <bool SPLIT>
+__device__ __forceinline__ void state_chunk_tma(const StateMaps<SPLIT>& tm, int n_arr, uint8_t* ss, uint64_t* bar, int col0,
+                                                int srow, int c) {
+    if constexpr (SPLIT) {
+        for (int a = 0; a < 2; ++a)
+#pragma unroll
+            for (int q = 0; q < BN_MAX / PLANE_COLS; ++q) {
+                uint8_t* s = ss + a * PLANE_BYTES + q * SUB_BYTES;
+                if (bar) tma_load_3d(s, &tm.a[a], bar, col0 + q * PLANE_COLS, BAND_ROWS * c, srow / 16);
+                else tma_store_3d(&tm.a[a], s, col0 + q * PLANE_COLS, BAND_ROWS * c, srow / 16);
+            }
+    }
+    for (int a = SPLIT ? 1 : 0; a < n_arr; ++a)
 #pragma unroll
         for (int q = 0; q < BN_MAX / SUB_COLS; ++q) {
             uint8_t* s = ss + a * ARR_BYTES + q * SUB_BYTES;
-            if (bar) tma_load_3d(s, &tm.a[a], bar, col0 + q * SUB_COLS, BAND_ROWS * c, srow / 16);
-            else tma_store_3d(&tm.a[a], s, col0 + q * SUB_COLS, BAND_ROWS * c, srow / 16);
+            const CUtensorMap* m = &tm.a[SPLIT ? a + 1 : a];
+            if (bar) tma_load_3d(s, m, bar, col0 + q * SUB_COLS, BAND_ROWS * c, srow / 16);
+            else tma_store_3d(m, s, col0 + q * SUB_COLS, BAND_ROWS * c, srow / 16);
         }
 }
 
 // DEV_LR: the learning rate and, with WD_DECOUPLED, the factor 1 - lr * weight_decay come from lr_dev = {lr, decay} in device
 // memory instead of p.lr / p.wd, so a captured CUDA graph follows a schedule.  Read once per consumer thread; the update
-// expressions are the same, so a launch whose block holds x is bit-identical to a by-value launch with x
-template <int WD, bool DEV_LR>
+// expressions are the same, so a launch whose block holds x is bit-identical to a by-value launch with x.
+// SPLIT: the master weight is decoded from its planes in shared memory, updated by the same expressions and encoded back
+// (p.p and p.p_bf16 are unused), so p, m, v, vmax and the mirror get the bits of the fp32 instantiation
+template <int WD, bool DEV_LR, bool SPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX,
-                  const __grid_constant__ StateMaps tmS, const float* __restrict__ lr_dev) {
+                  const __grid_constant__ StateMaps<SPLIT> tmS, const float* __restrict__ lr_dev) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* st_smem = smem + ST_OFFSET;
@@ -383,7 +406,7 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
     if (warp == 8 && lane == 0) {
         tma_prefetch_desc(&tmDY);
         tma_prefetch_desc(&tmX);
-        for (int a = 0; a < n_arr; ++a) tma_prefetch_desc(&tmS.a[a]);
+        for (int a = 0; a < n_arr + (SPLIT ? 1 : 0); ++a) tma_prefetch_desc(&tmS.a[a]);
         for (int i = 0; i < OP_STAGES; ++i) {
             mbar_init(&op_full[i], 1);
             mbar_init(&op_empty[i], 8);
@@ -565,7 +588,20 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                 float2* sm = reinterpret_cast<float2*>(ss + ARR_BYTES + so);
                 float2* sv = reinterpret_cast<float2*>(ss + 2 * ARR_BYTES + so);
                 float2* svm = reinterpret_cast<float2*>(ss + 3 * ARR_BYTES + so);
-                float2 pw = *sp, m = *sm, v = *sv;
+                // SPLIT: columns 8j + 2 (lane % 4) + {0, 1} of a plane are one 32-bit word of 16-B unit j % 8 of box j / 8
+                const int po = (j >> 3) * SUB_BYTES + R * 128 + (((j & 7) ^ (R & 7)) << 4) + 4 * (lane & 3);
+                uint32_t* shi = reinterpret_cast<uint32_t*>(ss + po);
+                uint32_t* slo = reinterpret_cast<uint32_t*>(ss + PLANE_BYTES + po);
+                float2 pw, m = *sm, v = *sv;
+                if constexpr (SPLIT) {
+                    const uint32_t hw = *shi, lw = *slo;
+                    pw.x = split_decode(hw & 0xffffu, lw & 0xffffu, __float_as_uint(v.x) >> 31);
+                    pw.y = split_decode(hw >> 16, lw >> 16, __float_as_uint(v.y) >> 31);
+                    v.x = without_tie_bit(v.x);
+                    v.y = without_tie_bit(v.y);
+                } else {
+                    pw = *sp;
+                }
                 float2 vm = p.amsgrad ? *svm : make_float2(0.f, 0.f);
                 float* pp = &pw.x; float* mp = &m.x; float* vp = &v.x; float* vmp = &vm.x;
 #pragma unroll
@@ -585,11 +621,18 @@ wgrad_adam_kernel(const Params p, const __grid_constant__ CUtensorMap tmDY, cons
                     }
                     pp[e] -= step_size * (mp[e] / denom);
                 }
-                *sp = pw;
+                if constexpr (SPLIT) {
+                    *shi = pack_bf16x2(pw.x, pw.y);
+                    *slo = (__float_as_uint(pw.x) & 0xffffu) | (__float_as_uint(pw.y) << 16);
+                    v.x = with_tie_bit(v.x, split_tie_up(pw.x));
+                    v.y = with_tie_bit(v.y, split_tie_up(pw.y));
+                } else {
+                    *sp = pw;
+                }
                 *sm = m;
                 *sv = v;
                 if (p.amsgrad) *svm = vm;
-                *reinterpret_cast<uint32_t*>(p.p_bf16 + o_row + 8 * j) = pack_bf16x2(pw.x, pw.y);
+                if constexpr (!SPLIT) *reinterpret_cast<uint32_t*>(p.p_bf16 + o_row + 8 * j) = pack_bf16x2(pw.x, pw.y);
             }
             // the updated chunk goes back to HBM by TMA; its slot returns to the producer once the store has read it
             fence_proxy_async_smem();
@@ -700,37 +743,42 @@ int lah_swapab_linear(const void* x, long long ldx, int x_rows, const void* W, i
 
 }  // extern "C"
 
-template <int WD, bool DEV_LR>
-static int launch_wgrad_adam(const wa::Params& a, const CUtensorMap& tmDY, const CUtensorMap& tmX, const wa::StateMaps& tmS,
-                             const float* lr_dev, int ctas, cudaStream_t st) {
-    if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<WD, DEV_LR>>(wa::SMEM_TOTAL)) return e;
-    wa::wgrad_adam_kernel<WD, DEV_LR><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS, lr_dev);
+template <int WD, bool DEV_LR, bool SPLIT>
+static int launch_wgrad_adam(const wa::Params& a, const CUtensorMap& tmDY, const CUtensorMap& tmX,
+                             const wa::StateMaps<SPLIT>& tmS, const float* lr_dev, int ctas, cudaStream_t st) {
+    if (int e = set_max_dynamic_smem<wa::wgrad_adam_kernel<WD, DEV_LR, SPLIT>>(wa::SMEM_TOTAL)) return e;
+    wa::wgrad_adam_kernel<WD, DEV_LR, SPLIT><<<ctas, NUM_THREADS, wa::SMEM_TOTAL, st>>>(a, tmDY, tmX, tmS, lr_dev);
     return -(int)cudaGetLastError();
 }
 
-extern "C" {
-
-// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
-// weight_decay: the L2 coefficient (WD_L2); decay: the decoupled weight-decay factor 1 - lr * wd, read only when `decoupled`
-// is set, which selects WD_DECOUPLED.  At most one of the two forms per launch.  lr_dev == NULL: lr and decay by value;
-// otherwise lr_dev = {lr, 1 - lr * wd} in device memory (the factor computed on the host in double and rounded to fp32
-// once) and the DEV_LR instantiation, which ignores lr and decay, so a captured CUDA graph follows a schedule
-int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
-                   const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
-                   float* v, float* vmax, void* p_bf16, float lr, const float* lr_dev, float beta1, float beta2, float eps,
-                   int amsgrad, float weight_decay, float decay, int decoupled, int max_ctas, cudaStream_t st) {
+// the two entry points below; SPLIT: p is the hi plane (p_bf16 is unused), lo the low-half plane
+template <bool SPLIT>
+static int wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                      const int* group_off, const int* group_rows, const int* skip, const int* step, void* p, void* lo,
+                      float* m, float* v, float* vmax, void* p_bf16, float lr, const float* lr_dev, float beta1, float beta2,
+                      float eps, int amsgrad, float weight_decay, float decay, int decoupled, int max_ctas, cudaStream_t st) {
     if ((N % BM) || (K % BN_MAX) || (lddy % 8) || (ldx % 8) || 1ll * G * N > INT_MAX) return -2;
     if (decoupled && weight_decay != 0.f) return -2;
     if (amsgrad && !vmax) return -2;   // AMSGrad streams vmax through its own tensor map
     CUtensorMap tmDY, tmX;
-    wa::StateMaps tmS;
+    wa::StateMaps<SPLIT> tmS;
     {
-        float* arrs[4] = {p, m, v, amsgrad ? vmax : p};   // without amsgrad the vmax map is never used
+        void* arrs[5] = {p, m, v, amsgrad ? vmax : (float*)m, nullptr};   // without amsgrad the vmax map is never used
+        if (SPLIT) {
+            arrs[1] = lo; arrs[2] = m; arrs[3] = v; arrs[4] = amsgrad ? vmax : m;
+        }
         uint64_t dims[3] = {(uint64_t)K, 16, (uint64_t)G * N / 16};
         uint64_t str[2] = {(uint64_t)K * 4, (uint64_t)K * 64};
         uint32_t box[3] = {wa::SUB_COLS, wa::BAND_ROWS, BM / 16};
-        for (int a = 0; a < 4; ++a) {
-            int r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, arrs[a], dims, str, box);
+        for (int a = 0; a < (SPLIT ? 5 : 4); ++a) {
+            int r;
+            if (SPLIT && a < 2) {
+                uint64_t pstr[2] = {(uint64_t)K * 2, (uint64_t)K * 32};
+                uint32_t pbox[3] = {wa::PLANE_COLS, wa::BAND_ROWS, BM / 16};
+                r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, arrs[a], dims, pstr, pbox);
+            } else {
+                r = make_tmap(&tmS.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, arrs[a], dims, str, box);
+            }
             if (r) return r;
         }
     }
@@ -750,7 +798,7 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
     }
     wa::Params a;
     a.G = G; a.N = N; a.K = K; a.group_off = group_off; a.group_rows = group_rows; a.skip = skip; a.step = step;
-    a.p = p; a.m = m; a.v = v; a.vmax = vmax; a.p_bf16 = (bf16*)p_bf16; a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.amsgrad = amsgrad;
+    a.p = SPLIT ? nullptr : (float*)p; a.m = m; a.v = v; a.vmax = vmax; a.p_bf16 = (bf16*)p_bf16; a.lr = lr; a.beta1 = beta1; a.beta2 = beta2; a.eps = eps; a.amsgrad = amsgrad;
     a.wd = decoupled ? decay : weight_decay;
     a.tile_counter = tile_counter() ? tile_counter() + 16 : nullptr;   // own word (64 B apart from the GEMM's)
     a.poison = g_poison;
@@ -760,13 +808,40 @@ int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx,
     if (cudaMemsetAsync(a.tile_counter, 0, sizeof(int), st) != cudaSuccess) return -4;
     const int ctas = persistent_grid(total, max_ctas);
     if (lr_dev) {
-        if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, true>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
-        if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, true>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
-        return launch_wgrad_adam<wa::WD_NONE, true>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
+        if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, true, SPLIT>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
+        if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, true, SPLIT>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
+        return launch_wgrad_adam<wa::WD_NONE, true, SPLIT>(a, tmDY, tmX, tmS, lr_dev, ctas, st);
     }
-    if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
-    if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
-    return launch_wgrad_adam<wa::WD_NONE, false>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+    if (decoupled) return launch_wgrad_adam<wa::WD_DECOUPLED, false, SPLIT>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+    if (weight_decay != 0.f) return launch_wgrad_adam<wa::WD_L2, false, SPLIT>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+    return launch_wgrad_adam<wa::WD_NONE, false, SPLIT>(a, tmDY, tmX, tmS, nullptr, ctas, st);
+}
+
+extern "C" {
+
+// W[g] -= AMSGrad(dW[g] = dy_g^T x_g) for every group with rows > 0; p / m / v / vmax are [G, N, K] fp32, p_bf16 the mirror.
+// weight_decay: the L2 coefficient (WD_L2); decay: the decoupled weight-decay factor 1 - lr * wd, read only when `decoupled`
+// is set, which selects WD_DECOUPLED.  At most one of the two forms per launch.  lr_dev == NULL: lr and decay by value;
+// otherwise lr_dev = {lr, 1 - lr * wd} in device memory (the factor computed on the host in double and rounded to fp32
+// once) and the DEV_LR instantiation, which ignores lr and decay, so a captured CUDA graph follows a schedule
+int lah_wgrad_adam(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                   const int* group_off, const int* group_rows, const int* skip, const int* step, float* p, float* m,
+                   float* v, float* vmax, void* p_bf16, float lr, const float* lr_dev, float beta1, float beta2, float eps,
+                   int amsgrad, float weight_decay, float decay, int decoupled, int max_ctas, cudaStream_t st) {
+    return wgrad_adam<false>(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, p, nullptr, m, v,
+                             vmax, p_bf16, lr, lr_dev, beta1, beta2, eps, amsgrad, weight_decay, decay, decoupled, max_ctas,
+                             st);
+}
+
+// the same step on a split master weight: hi ([G, N, K] bf16, the GEMM operand) and lo ([G, N, K] 16 bit) instead of p and
+// its mirror, the tie bits in the sign of v (split_decode, sm90.cuh).  p, m, v, vmax and hi come out as lah_wgrad_adam's
+int lah_wgrad_adam_split(const void* dy, long long lddy, const void* x, long long ldx, int total_rows, int G, int N, int K,
+                         const int* group_off, const int* group_rows, const int* skip, const int* step, void* hi, void* lo,
+                         float* m, float* v, float* vmax, float lr, const float* lr_dev, float beta1, float beta2, float eps,
+                         int amsgrad, float weight_decay, float decay, int decoupled, int max_ctas, cudaStream_t st) {
+    if (!hi || !lo) return -2;
+    return wgrad_adam<true>(dy, lddy, x, ldx, total_rows, G, N, K, group_off, group_rows, skip, step, hi, lo, m, v, vmax,
+                            nullptr, lr, lr_dev, beta1, beta2, eps, amsgrad, weight_decay, decay, decoupled, max_ctas, st);
 }
 
 }  // extern "C"

@@ -40,6 +40,7 @@ def _lib():
         "lah_step_begin": [I, L, P],
         "lah_swapab_linear": [P, L, I, P, I, I, I, I, P, L, P, P, P, P, L, P, I, I, P, I, P],
         "lah_wgrad_adam": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, P, Fl, Fl, Fl, I, Fl, Fl, I, I, P],
+        "lah_wgrad_adam_split": [P, L, P, L, I, I, I, I, P, P, P, P, P, P, P, P, P, Fl, P, Fl, Fl, Fl, I, Fl, Fl, I, I, P],
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
@@ -57,6 +58,7 @@ def _lib():
                           I, P],
         "lah_bump_steps": [P, P, I, P],
         "lah_cast_bf16": [P, P, L, P],
+        "lah_split_master": [P, P, P, P, L, I, P],
         "lah_attention_fwd": [P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
         "lah_attention_bwd": [P, P, P, P, P, P, P, L, I, I, I, c_ull, I, Fl, P, P],
         "lah_attention_fwd_causal": [P, P, P, L, I, I, I, c_ull, I, Fl, P],
@@ -946,26 +948,38 @@ def swapab_linear_ref(x, w, group_off, group_rows, *, bias=None, residual=None, 
 
 
 def wgrad_adam(dy, x, group_off, group_rows, *, p, m, v, vmax, p_bf16, step, skip=None, lr=1e-3, betas=(0.9, 0.999),
-               eps=1e-8, amsgrad=True, weight_decay=0.0, decoupled=False, max_ctas=0, lr_dev=None):
+               eps=1e-8, amsgrad=True, weight_decay=0.0, decoupled=False, max_ctas=0, lr_dev=None, p_lo=None):
     """
     Fused weight gradient + per-expert AMSGrad (csrc/small_m.cu): for every group g with rows > 0,
     dW[g] = dy_g^T x_g is formed in registers and applied to p / m / v / vmax ([G, N, K] fp32) and the bf16 mirror in the same
     kernel; the gradient never reaches HBM.  ``step`` holds the per-expert step counts AFTER this update.
     ``weight_decay`` / ``decoupled`` / ``lr_dev``: as in ``adam_step``.
+    ``p_lo``: a split master weight (``split_encode``): p=None, the weight is ``p_bf16`` plus its low half ``p_lo`` ([G, N, K]
+    int16) with the tie bits in the sign of ``v``; the step computes the same bits as on fp32 p.
     """
-    G, N, Kd = p.shape
-    assert dy.shape[1] == N and x.shape[1] == Kd and dy.shape[0] == x.shape[0] and p.is_contiguous()
-    assert dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16 and p.dtype == torch.float32
+    G, N, Kd = (p if p_lo is None else p_lo).shape
+    assert dy.shape[1] == N and x.shape[1] == Kd and dy.shape[0] == x.shape[0]
+    assert dy.dtype == torch.bfloat16 and x.dtype == torch.bfloat16
+    if p_lo is None:
+        assert p.is_contiguous() and p.dtype == torch.float32
+    else:
+        assert p is None and p_lo.dtype == torch.int16 and p_bf16.dtype == torch.bfloat16
+        assert p_lo.is_contiguous() and p_bf16.is_contiguous() and p_bf16.shape[1:] == p_lo.shape[1:]
     if amsgrad and vmax is None:
         raise ValueError("wgrad_adam: amsgrad needs a vmax tensor (vmax=None only with amsgrad=False)")
     if lr_dev is not None:
         _check_lr_dev(lr_dev)
     l2, decay = weight_decay_args(lr, weight_decay, decoupled)
-    native.check(_lib().lah_wgrad_adam(ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd, ptr(group_off),
-                                       ptr(group_rows), ptr(skip), ptr(step), ptr(p), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16),
-                                       lr, ptr(lr_dev), betas[0], betas[1], eps, int(amsgrad), l2, decay,
-                                       int(bool(decoupled and weight_decay)), int(max_ctas), stream_ptr()),
-                 "lah_wgrad_adam")
+    common = (ptr(dy), dy.stride(0), ptr(x), x.stride(0), dy.shape[0], G, N, Kd, ptr(group_off), ptr(group_rows),
+              ptr(skip), ptr(step))
+    tail = (lr, ptr(lr_dev), betas[0], betas[1], eps, int(amsgrad), l2, decay, int(bool(decoupled and weight_decay)),
+            int(max_ctas), stream_ptr())
+    if p_lo is None:
+        native.check(_lib().lah_wgrad_adam(*common, ptr(p), ptr(m), ptr(v), ptr(vmax), ptr(p_bf16), *tail),
+                     "lah_wgrad_adam")
+    else:
+        native.check(_lib().lah_wgrad_adam_split(*common, ptr(p_bf16), ptr(p_lo), ptr(m), ptr(v), ptr(vmax), *tail),
+                     "lah_wgrad_adam_split")
     native.count_launch()
 
 
@@ -977,6 +991,30 @@ def bump_steps(step, group_rows):
 def cast_bf16(src, dst):
     assert src.dtype == torch.float32 and dst.dtype == torch.bfloat16 and src.numel() == dst.numel()
     native.check(_lib().lah_cast_bf16(ptr(src), ptr(dst), src.numel(), stream_ptr()), "lah_cast_bf16")
+    native.count_launch()
+
+
+def _check_split(p, hi, lo, v):
+    n = p.numel()
+    assert p.dtype == torch.float32 and hi.dtype == torch.bfloat16 and lo.dtype == torch.int16 and v.dtype == torch.float32
+    assert hi.numel() == n and lo.numel() == n and v.numel() == n
+    assert all(t.is_contiguous() and t.is_cuda for t in (p, hi, lo, v))
+
+
+def split_encode(p, hi, lo, v):
+    """Split master weight: hi = bf16(p) (round to nearest even, the GEMM operand), lo = the low 16 bits of p, and the bit
+    that tells a tie rounded up (low half 0x8000, p's upper half odd) in the sign of v (exp_avg_sq, >= 0).  csrc/sm90.cuh,
+    split_decode, has the exact rule; ``split_decode`` inverts it for every finite p."""
+    _check_split(p, hi, lo, v)
+    native.check(_lib().lah_split_master(ptr(p), ptr(hi), ptr(lo), ptr(v), p.numel(), 1, stream_ptr()), "lah_split_master")
+    native.count_launch()
+
+
+def split_decode(hi, lo, v, out):
+    """the fp32 master weight of a split one (``split_encode``), into ``out``"""
+    _check_split(out, hi, lo, v)
+    native.check(_lib().lah_split_master(ptr(out), ptr(hi), ptr(lo), ptr(v), out.numel(), 0, stream_ptr()),
+                 "lah_split_master")
     native.count_launch()
 
 

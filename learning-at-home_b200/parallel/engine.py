@@ -453,7 +453,14 @@ class EngineContext:
 # =========================================================================================================
 class ExpertShard:
     """Stacked parameters / gradients / Adam state of the E_loc local experts of one layer (flat fp32 buffers, segments
-    [E_loc, size] per tensor kind) plus the bf16 mirror consumed by the GEMMs."""
+    [E_loc, size] per tensor kind) plus the bf16 mirror consumed by the GEMMs.
+
+    On the small expert path (``split``) the weight matrices are kept split: the mirror plus their low 16 bits in ``lo``,
+    with the tie bit of the rounding in the sign of exp_avg_sq (``K.split_encode``).  The fused wgrad + AMSGrad kernel
+    then streams 32 B per parameter instead of 34, and computes the same bits.  ``p``, ``views``, ``v`` and ``v_views``
+    hide the format: they return the fp32 values, decoded on access; after writing ``p`` / ``views``, ``sync_bf16()``
+    encodes them.  The kernels work on ``p_raw``, ``raw_views``, ``v_raw`` and ``v_raw_views``, whose matrix segments
+    hold stale weights and tie bits in a split shard."""
 
     def __init__(self, cfg: DMoEConfig, E_loc: int, first_expert: int, device, layer_index: int = 0, ctx=None):
         self.cfg, self.E_loc, self.first_expert = cfg, E_loc, first_expert
@@ -467,21 +474,29 @@ class ExpertShard:
         f32 = dict(dtype=torch.float32, device=device)
         self.p_off = self.g_off = self.pbf16_off = -1
         if ctx is not None and ctx.S > 0:   # peer-visible: replicas are pulled from p / p_bf16, partial grads read from g
-            self.p, self.p_off = ctx.heap.alloc((total,), torch.float32)
+            self.p_raw, self.p_off = ctx.heap.alloc((total,), torch.float32)
             self.g, self.g_off = ctx.heap.alloc((total,), torch.float32)
             self.p_bf16, self.pbf16_off = ctx.heap.alloc((total,), torch.bfloat16)
-            self.p.zero_(), self.g.zero_(), self.p_bf16.zero_()
+            self.p_raw.zero_(), self.g.zero_(), self.p_bf16.zero_()
         else:
-            self.p = torch.zeros(total, **f32)
+            self.p_raw = torch.zeros(total, **f32)
             self.g = torch.zeros(total, **f32)
             self.p_bf16 = torch.zeros(total, dtype=torch.bfloat16, device=device)
         self.m = torch.zeros(total, **f32)
-        self.v = torch.zeros(total, **f32)
+        self.v_raw = torch.zeros(total, **f32)
         self.vmax = torch.zeros(total, **f32) if cfg.amsgrad else None
         self.step = torch.zeros(E_loc, dtype=torch.int32, device=device)
-        self.views, self.grads, self.bf16, self.m_views, self.v_views = (
-            K.segment_views(flat, shapes, slots) for flat in (self.p, self.g, self.p_bf16, self.m, self.v))
+        self._shapes = shapes
+        self.raw_views, self.grads, self.bf16, self.m_views, self.v_raw_views = (
+            K.segment_views(flat, shapes, slots) for flat in (self.p_raw, self.g, self.p_bf16, self.m, self.v_raw))
         self.vmax_views = K.segment_views(self.vmax, shapes, slots) if self.vmax is not None else {}
+        # the small path updates the weight matrices only in the fused wgrad + AMSGrad kernel, which takes them split
+        self.split = ctx is not None and ctx.small
+        self.matrices = [n for s, n in enumerate(self.layout.names) if not (self.layout.small_mask >> s) & 1]
+        self.lo_views = {}
+        if self.split:
+            self.lo_views = {n: torch.zeros(self.raw_views[n].shape, dtype=torch.int16, device=device)
+                             for n in self.matrices}
         # asynchronous-update bookkeeping (DMoEConfig.update_every_*): rows / steps pending since the last optimizer step
         self.pending_rows = torch.zeros(E_loc, dtype=torch.int32, device=device)
         self.pending_steps = torch.zeros(E_loc, dtype=torch.int32, device=device)
@@ -499,18 +514,19 @@ class ExpertShard:
         norm weights 1, norm biases 0), seeded per (layer, global expert) so that the same expert gets the same weights
         regardless of the number of ranks"""
         cfg = self.cfg
-        dev = self.p.device
+        dev = self.p_raw.device
+        views = self.raw_views   # every weight of the owned experts is written, then encoded by sync_bf16()
         for le in range(self.E_loc):
             gen = torch.Generator(device=dev)
             gen.manual_seed(cfg.seed * 1000003 + layer_index * 10007 + self.first_expert + le)
             for n in self.layout.names:   # segment order: a matrix is followed by its bias (FeedforwardBlock)
-                t = self.views[n][le]
+                t = views[n][le]
                 if n.startswith("be"):       # LayerNorm bias
                     t.zero_()
                 elif n.startswith("g"):      # LayerNorm / RMSNorm weight
                     t.fill_(1.0)
                 else:                        # Linear weight wX or its bias bX (fan_in from wX)
-                    fan_in = self.views["w" + n[1:]].shape[-1]
+                    fan_in = views["w" + n[1:]].shape[-1]
                     bound = 1.0 / math.sqrt(fan_in)
                     t.uniform_(-bound, bound, generator=gen)
         self.sync_bf16()
@@ -524,11 +540,35 @@ class ExpertShard:
         return self.w8
 
     def sync_bf16(self):
+        """the mirror (and in a split shard lo and the tie bits) from the fp32 weights in ``p_raw``"""
         self.w8_dirty = True
-        if self.p.is_cuda:
-            K.cast_bf16(self.p, self.p_bf16)
+        if self.p_raw.is_cuda:
+            K.cast_bf16(self.p_raw, self.p_bf16)
         else:
-            self.p_bf16.copy_(self.p)
+            self.p_bf16.copy_(self.p_raw)
+        for n in (self.matrices if self.split else ()):
+            K.split_encode(self.raw_views[n], self.bf16[n], self.lo_views[n], self.v_raw_views[n])
+
+    @property
+    def p(self) -> torch.Tensor:
+        """the flat fp32 weights; a split shard decodes its matrices into ``p_raw`` first"""
+        for n in (self.matrices if self.split else ()):
+            K.split_decode(self.bf16[n], self.lo_views[n], self.v_raw_views[n], out=self.raw_views[n])
+        return self.p_raw
+
+    @property
+    def views(self) -> Dict[str, torch.Tensor]:
+        self.p
+        return self.raw_views
+
+    @property
+    def v(self) -> torch.Tensor:
+        """the flat exp_avg_sq; in a split shard a copy without the tie bits"""
+        return self.v_raw.abs() if self.split else self.v_raw
+
+    @property
+    def v_views(self) -> Dict[str, torch.Tensor]:
+        return K.segment_views(self.v, self._shapes, self.slots) if self.split else self.v_raw_views
 
     # ------------------------------------------------------------------ checkpoint layout (SURVEY.md §5.4)
     def _expert_tensors(self, views, le: int) -> Dict[str, torch.Tensor]:
@@ -556,18 +596,20 @@ class ExpertShard:
 
     def load_expert_state_dict(self, le: int, state: Dict[str, torch.Tensor], prefix: str = "expert."):
         with torch.no_grad():
+            views = self.views   # decoded once: a split shard's next decode would overwrite what is written here
             for n, t in self.layout.segment_state(state, prefix).items():
-                self.views[n][le].copy_(t)
+                views[n][le].copy_(t)
         self.sync_bf16()
 
     def load_expert_optimizer_state(self, le: int, opt_state: Dict):
         with torch.no_grad():
+            self.p   # a split shard decodes its weights while v still holds their tie bits, and encodes them again below
             for i, k in enumerate(self.layout.params):
                 entry = opt_state["state"].get(i)
                 if entry is None:
                     continue
                 n, block, parts = self.layout.slices[k]
-                for name, views in (("exp_avg", self.m_views), ("exp_avg_sq", self.v_views),
+                for name, views in (("exp_avg", self.m_views), ("exp_avg_sq", self.v_raw_views),
                                     ("max_exp_avg_sq", self.vmax_views if self.vmax is not None else None)):
                     if views is None or name not in entry:
                         continue
@@ -575,6 +617,8 @@ class ExpertShard:
                     dst = dst.chunk(parts, 0)[block] if parts > 1 else dst
                     dst.copy_(entry[name].reshape(dst.shape))
                 self.step[le] = int(entry["step"])
+            if self.split:
+                self.sync_bf16()
 
 
 # =========================================================================================================
@@ -808,19 +852,19 @@ class FusedDMoE(nn.Module):
         elif c.small:
             # weight-streaming regime: swap-AB tiles (weights on MMA-M, the group's 16..128 tokens on MMA-N), groups of 16 rows
             go, gr_, T = ws.group_off, ws.group_rows, c.tile_rows
-            K.swapab_linear(ws.xd, sh.bf16["w1"], go, gr_, out=ws.h1, bias=sh.views["b1"], wait=wait)
-            K.ln_relu_fwd(ws.h1, sh.views["g1"], sh.views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1, tile_rows=T)
-            K.swapab_linear(ws.a1, sh.bf16["w2"], go, gr_, out=ws.h2, bias=sh.views["b2"])
-            K.ln_relu_fwd(ws.h2, sh.views["g2"], sh.views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, tile_rows=T)
-            K.swapab_linear(ws.a2, sh.bf16["w3"], go, gr_, out=ws.yo, bias=sh.views["b3"], residual=ws.xd)
+            K.swapab_linear(ws.xd, sh.bf16["w1"], go, gr_, out=ws.h1, bias=sh.raw_views["b1"], wait=wait)
+            K.ln_relu_fwd(ws.h1, sh.raw_views["g1"], sh.raw_views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1, tile_rows=T)
+            K.swapab_linear(ws.a1, sh.bf16["w2"], go, gr_, out=ws.h2, bias=sh.raw_views["b2"])
+            K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, tile_rows=T)
+            K.swapab_linear(ws.a2, sh.bf16["w3"], go, gr_, out=ws.yo, bias=sh.raw_views["b3"], residual=ws.xd)
         elif cfg.expert_dtype == "fp8":
             self._expert_ffn_fp8(wait, epoch)
         else:
-            gemm.grouped_linear(ws.xd, sh.bf16["w1"], tile_group=tg, bias=sh.views["b1"], out=ws.h1, wait=wait)
-            K.ln_relu_fwd(ws.h1, sh.views["g1"], sh.views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1)
-            gemm.grouped_linear(ws.a1, sh.bf16["w2"], tile_group=tg, bias=sh.views["b2"], out=ws.h2)
-            K.ln_relu_fwd(ws.h2, sh.views["g2"], sh.views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2)
-            gemm.grouped_linear(ws.a2, sh.bf16["w3"], tile_group=tg, bias=sh.views["b3"], residual=ws.xd, out=ws.yo)
+            gemm.grouped_linear(ws.xd, sh.bf16["w1"], tile_group=tg, bias=sh.raw_views["b1"], out=ws.h1, wait=wait)
+            K.ln_relu_fwd(ws.h1, sh.raw_views["g1"], sh.raw_views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1)
+            gemm.grouped_linear(ws.a1, sh.bf16["w2"], tile_group=tg, bias=sh.raw_views["b2"], out=ws.h2)
+            K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2)
+            gemm.grouped_linear(ws.a2, sh.bf16["w3"], tile_group=tg, bias=sh.raw_views["b3"], residual=ws.xd, out=ws.yo)
         c.timer.mark("expert_ffn_fwd")
         y = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=x.device)
         K.combine_rows(ws.yo_off, idx, pair_row, w, y, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_OUTPUT, epoch=epoch,
@@ -840,7 +884,7 @@ class FusedDMoE(nn.Module):
         tg, T = ws.tile_group, c.tile_rows
         if wait is not None:  # the norm, not a GEMM, is the first consumer of the rows pushed by the peers
             K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
-        K.rms_norm_fwd(ws.xd, sh.views["g"], GATED_EPS, out=ws.n, rstd=ws.rstd, tile_group=tg, tile_rows=T)
+        K.rms_norm_fwd(ws.xd, sh.raw_views["g"], GATED_EPS, out=ws.n, rstd=ws.rstd, tile_group=tg, tile_rows=T)
         if c.small:
             go, gr_ = ws.group_off, ws.group_rows
             K.swapab_linear(ws.n, sh.bf16["w13"], go, gr_, out=ws.h)
@@ -861,11 +905,11 @@ class FusedDMoE(nn.Module):
             K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
         w8 = sh.fp8_weights()
         fp8.quantize(ws.xd, tile_group=tg, out=ws.xq)
-        fp8.grouped_linear_fp8(ws.xq, w8["w1"], tile_group=tg, bias=sh.views["b1"], out=ws.h1)
-        K.ln_relu_fwd(ws.h1, sh.views["g1"], sh.views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1, quant=ws.aq)
-        fp8.grouped_linear_fp8(ws.aq, w8["w2"], tile_group=tg, bias=sh.views["b2"], out=ws.h2)
-        K.ln_relu_fwd(ws.h2, sh.views["g2"], sh.views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, quant=ws.aq)
-        fp8.grouped_linear_fp8(ws.aq, w8["w3"], tile_group=tg, bias=sh.views["b3"], residual=ws.xd, out=ws.yo)
+        fp8.grouped_linear_fp8(ws.xq, w8["w1"], tile_group=tg, bias=sh.raw_views["b1"], out=ws.h1)
+        K.ln_relu_fwd(ws.h1, sh.raw_views["g1"], sh.raw_views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1, quant=ws.aq)
+        fp8.grouped_linear_fp8(ws.aq, w8["w2"], tile_group=tg, bias=sh.raw_views["b2"], out=ws.h2)
+        K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, quant=ws.aq)
+        fp8.grouped_linear_fp8(ws.aq, w8["w3"], tile_group=tg, bias=sh.raw_views["b3"], residual=ws.xd, out=ws.yo)
 
     def _backward_cuda(self, gy, B, logits=None):
         """:param logits: the gate logits of the forward when it computed router losses (their gradient is added here)"""
@@ -908,17 +952,17 @@ class FusedDMoE(nn.Module):
             K.swiglu_bwd(c.da, ws.h, out=c.dh)
             gemm.grouped_wgrad(c.dh, ws.n, go, G, out=gr["w13"], accumulate=cfg.accumulate)
             gemm.grouped_linear(c.dh, sh.bf16["w13"], tile_group=tg, w_is_kn=True, out=c.dn)
-            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.views["g"], dx=c.dxd, dgamma=gr["g"], dres=c.gyd,
+            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.raw_views["g"], dx=c.dxd, dgamma=gr["g"], dres=c.gyd,
                            tile_rows=c.tile_rows, tile_group=tg)
         else:
             K.grouped_colsum(c.gyd, tg, out=gr["b3"])
             gemm.grouped_wgrad(c.gyd, ws.a2, go, G, out=gr["w3"], accumulate=cfg.accumulate)
             gemm.grouped_linear(c.gyd, sh.bf16["w3"], tile_group=tg, w_is_kn=True, out=c.da)
-            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=c.dh, dgamma=gr["g2"],
+            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.raw_views["g2"], sh.raw_views["be2"], tg, dh=c.dh, dgamma=gr["g2"],
                           dbeta=gr["be2"], dbias=gr["b2"])
             gemm.grouped_wgrad(c.dh, ws.a1, go, G, out=gr["w2"], accumulate=cfg.accumulate)
             gemm.grouped_linear(c.dh, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
-            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=c.dh, dgamma=gr["g1"],
+            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.raw_views["g1"], sh.raw_views["be1"], tg, dh=c.dh, dgamma=gr["g1"],
                           dbeta=gr["be1"], dbias=gr["b1"])
             gemm.grouped_wgrad(c.dh, ws.xd, go, G, out=gr["w1"], accumulate=cfg.accumulate)
             gemm.grouped_linear(c.dh, sh.bf16["w1"], tile_group=tg, w_is_kn=True, residual=c.gyd, out=c.dxd)
@@ -949,8 +993,11 @@ class FusedDMoE(nn.Module):
             """dW never reaches HBM: register accumulator -> AMSGrad epilogue -> p / m / v / vmax updated in place.  With the overlap
             enabled the kernel goes to the optimizer stream, ordered after everything the main stream has launched so far (in
             particular the dgrad that still reads the OLD weights); its inputs live in per-layer buffers."""
-            kw = dict(p=sh.views[name][:self.E_loc], m=sh.m_views[name][:self.E_loc], v=sh.v_views[name][:self.E_loc],
-                      vmax=sh.vmax_views[name][:self.E_loc] if cfg.amsgrad else None, p_bf16=sh.bf16[name], step=sh.step, **opt)
+            E = self.E_loc
+            kw = dict(p=None, p_lo=sh.lo_views[name][:E], p_bf16=sh.bf16[name][:E]) if sh.split else \
+                dict(p=sh.raw_views[name][:E], p_bf16=sh.bf16[name])
+            kw.update(m=sh.m_views[name][:E], v=sh.v_raw_views[name][:E],
+                      vmax=sh.vmax_views[name][:E] if cfg.amsgrad else None, step=sh.step, **opt)
             if side is None:
                 K.wgrad_adam(dy, x, go, rows, **kw)
                 return
@@ -970,24 +1017,24 @@ class FusedDMoE(nn.Module):
             K.swiglu_bwd(c.da, ws.h, out=dh13)
             K.swapab_linear(dh13, sh.bf16["w13"], go, rows, out=c.dn, w_is_kn=True, max_ctas=chain_ctas)
             wgrad("w13", dh13, ws.n)
-            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.views["g"], dx=c.dxd, dgamma=gr["g"], dres=gyd, tile_rows=T,
+            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.raw_views["g"], dx=c.dxd, dgamma=gr["g"], dres=gyd, tile_rows=T,
                            tile_group=tg)
         else:
             dh2, dh1 = ws.dh2, ws.dh1
             K.grouped_colsum(gyd, tg, out=gr["b3"], tile_rows=T)
             K.swapab_linear(gyd, sh.bf16["w3"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
             wgrad("w3", gyd, ws.a2)
-            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.views["g2"], sh.views["be2"], tg, dh=dh2, dgamma=gr["g2"],
+            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.raw_views["g2"], sh.raw_views["be2"], tg, dh=dh2, dgamma=gr["g2"],
                           dbeta=gr["be2"], dbias=gr["b2"], tile_rows=T)
             K.swapab_linear(dh2, sh.bf16["w2"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
             wgrad("w2", dh2, ws.a1)
-            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.views["g1"], sh.views["be1"], tg, dh=dh1, dgamma=gr["g1"],
+            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.raw_views["g1"], sh.raw_views["be1"], tg, dh=dh1, dgamma=gr["g1"],
                           dbeta=gr["be1"], dbias=gr["b1"], tile_rows=T)
             K.swapab_linear(dh1, sh.bf16["w1"], go, rows, out=c.dxd, w_is_kn=True, residual=gyd, max_ctas=chain_ctas)
             wgrad("w1", dh1, ws.xd)
         # biases / norm weights: the ordinary fused AMSGrad restricted to the small segments
         small = sh.layout.small_mask
-        K.adam_step(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
+        K.adam_step(sh.p_raw, sh.g, sh.m, sh.v_raw, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
                     group_rows=ws.step_rows, zero_mask=small, G_active=self.E_loc, seg_mask=small, **opt)
         sh.w8_dirty = True
 
@@ -1006,7 +1053,7 @@ class FusedDMoE(nn.Module):
             sh.pending_steps.mul_(1 - sh.fire)
             rows, zero_mask = sh.fire, (1 << len(sh.layout.names)) - 1
         K.bump_steps(sh.step, rows)
-        K.adam_step(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
+        K.adam_step(sh.p_raw, sh.g, sh.m, sh.v_raw, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
                     group_rows=rows, **c.adam_kwargs(), zero_mask=zero_mask, G_active=self.E_loc, world=c.world,
                     peer_bases=c.heap.peer_bases if c.S else None, shadow_of=ws.owned_shadow if c.S else None,
                     shadow_g_off=sh.g_off, me=c.rank)
@@ -1055,7 +1102,7 @@ class FusedDMoE(nn.Module):
                 sh.pending_steps.mul_(keep)
                 rows, zero_mask = due.to(rows.dtype), (1 << len(sh.layout.names)) - 1
             sh.step += (rows > 0).to(sh.step.dtype)
-            K.adam_step_ref(sh.p, sh.g, sh.m, sh.v, sh.vmax, sh.seg_sizes, self.E_loc, step=sh.step,
+            K.adam_step_ref(sh.p_raw, sh.g, sh.m, sh.v_raw, sh.vmax, sh.seg_sizes, self.E_loc, step=sh.step,
                             group_rows=rows, **cfg.adam_kwargs(), zero_mask=zero_mask)
         sh.sync_bf16()
         self._ref_rows = None

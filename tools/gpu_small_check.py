@@ -175,6 +175,16 @@ def perf():
                     flush=flush)
         record("perf_wgrad_adam_w2" + tag, ok=True, ms=ms, ctas=ctas or "all", state_GB=nbytes / 1e9,
                TBps=nbytes / ms / 1e9, frac_of_hbm=nbytes / ms / 1e6 / HBM, frac_of_copy=nbytes / ms / 1e6 / copy_gbs)
+    # the same step on a split master weight (the small path's format): pb and its low half, 32 B / param
+    lo = torch.empty(G, I, I, device="cuda", dtype=torch.int16)
+    K.split_encode(p.view(-1), pb.view(-1), lo.view(-1), v.view(-1))
+    nbytes = p.numel() * 32
+    for tag, ctas in [("", 0), ("_opt_share", 132 * 17 // 28)]:
+        ms = timeit(lambda: K.wgrad_adam(dy, a, off, rows, p=None, p_lo=lo, m=m, v=v, vmax=vmax, p_bf16=pb, step=step,
+                                         max_ctas=ctas), flush=flush)
+        record("perf_wgrad_adam_split_w2" + tag, ok=True, ms=ms, ctas=ctas or "all", state_GB=nbytes / 1e9,
+               TBps=nbytes / ms / 1e9, frac_of_hbm=nbytes / ms / 1e6 / HBM, frac_of_copy=nbytes / ms / 1e6 / copy_gbs)
+    v.abs_()   # the tie bits out again: p is stale from here on, the unfused pair below only needs the shapes
     # the unfused pair it replaces: fp32 gradient written by a wgrad GEMM + the stand-alone AMSGrad kernel (38 B / param)
     g = torch.randn_like(p)
     rows_all = torch.full((G,), 16, dtype=torch.int32, device="cuda")

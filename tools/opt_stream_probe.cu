@@ -2,7 +2,8 @@
 // a persistent, warp-specialised kernel that walks 128 x 128 tiles of four fp32 [G*N, K] arrays (p, m, v, vmax), brings
 // each tile in as four 64 KB chunks through a 3-stage TMA ring, optionally reads p back from shared memory at the
 // accumulator positions of the fused kernel and writes the bf16 mirror, and stores every chunk back by TMA.  The chunk
-// geometry is a run-time argument, so one process can compare the ways of cutting a tile into chunks.
+// geometry is a run-time argument, so one process can compare the ways of cutting a tile into chunks.  GEO_SPLIT streams the
+// master weight as two 16-bit planes (its bf16 GEMM operand and its low half) instead of fp32 p + a bf16 mirror.
 //
 // Built and driven by tools/opt_stream_probe.py.
 #include "sm90.cuh"
@@ -27,14 +28,29 @@ constexpr int NUM_THREADS = 288;
 //   GEO_BANDS       rows 4c .. 4c + 3 of each of the tile's eight 16-row bands, all 128 columns: a 3-D map (K, 16, G*N/16)
 //                   and four [8 bands][4 rows][32 fp32] boxes per array, 512-B row runs
 //   GEO_BANDS_FLAT  the same rows as one unswizzled [8][4][128 fp32] box per array
-enum { GEO_COLS = 0, GEO_ROWS = 1, GEO_BANDS = 2, GEO_BANDS_FLAT = 3 };
+//   GEO_SPLIT       the rows of GEO_BANDS for five arrays: the hi and lo 16-bit planes of the master weight, two
+//                   [8 bands][4 rows][64 x 16 bit] boxes each (256-B row runs, 8 KB per plane), then m, v, vmax as in
+//                   GEO_BANDS; 64 KB per chunk as before, everything moved by TMA
+enum { GEO_COLS = 0, GEO_ROWS = 1, GEO_BANDS = 2, GEO_BANDS_FLAT = 3, GEO_SPLIT = 4 };
 
 struct Maps {
-    CUtensorMap a[4];
+    CUtensorMap a[5];
 };
 
 __device__ __forceinline__ void chunk_tma(int geo, bool store, const Maps& tm, uint8_t* ss, uint64_t* bar, int col0, int srow,
                                           int c) {
+    if (geo == GEO_SPLIT) {
+        for (int a = 0; a < 5; ++a) {
+            const int plane = a < 2;
+            uint8_t* s = ss + (plane ? a * 8192 : (a - 1) * ARR_BYTES);
+            for (int q = 0; q < (plane ? 2 : 4); ++q) {
+                const int x = col0 + (plane ? 64 : 32) * q;
+                if (store) tma_store_3d(&tm.a[a], s + q * 4096, x, 4 * c, srow / 16);
+                else tma_load_3d(s + q * 4096, &tm.a[a], bar, x, 4 * c, srow / 16);
+            }
+        }
+        return;
+    }
     for (int a = 0; a < 4; ++a) {
         uint8_t* s = ss + a * ARR_BYTES;
         const CUtensorMap* m = &tm.a[a];
@@ -109,7 +125,7 @@ probe_kernel(int geo, int mirror_on, int GN, int K, bf16* mirror, int* tile_coun
     volatile int* q_tile = reinterpret_cast<volatile int*>(q_empty + QD);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (warp == 8 && lane == 0) {
-        for (int a = 0; a < 4; ++a) tma_prefetch_desc(&tm.a[a]);
+        for (int a = 0; a < (geo == GEO_SPLIT ? 5 : 4); ++a) tma_prefetch_desc(&tm.a[a]);
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&st_full[i], 1);
             mbar_init(&st_empty[i], 1);
@@ -194,14 +210,23 @@ int* counter() {
 
 }  // namespace
 
+// GEO_SPLIT: mirror is the hi plane, lo the low-half plane, p unused; mirror_on must be 0 (the planes go back by TMA)
 extern "C" int probe_stream(int geo, int mirror_on, int GN, int K, float* p, float* m, float* v, float* vmax, void* mirror,
-                            int ctas, cudaStream_t st) {
-    if (geo < 0 || geo > GEO_BANDS_FLAT || GN % BM || K % BN) return -2;
+                            void* lo, int ctas, cudaStream_t st) {
+    if (geo < 0 || geo > GEO_SPLIT || GN % BM || K % BN || (geo == GEO_SPLIT && mirror_on)) return -2;
     Maps tm;
-    float* arrs[4] = {p, m, v, vmax};
-    for (int a = 0; a < 4; ++a) {
+    void* arrs[5] = {p, m, v, vmax, nullptr};
+    if (geo == GEO_SPLIT) {
+        arrs[0] = mirror; arrs[1] = lo; arrs[2] = m; arrs[3] = v; arrs[4] = vmax;
+    }
+    for (int a = 0; a < (geo == GEO_SPLIT ? 5 : 4); ++a) {
         int r;
-        if (geo == GEO_COLS || geo == GEO_ROWS) {
+        if (geo == GEO_SPLIT && a < 2) {
+            const uint64_t dims[3] = {(uint64_t)K, 16, (uint64_t)GN / 16};
+            const uint64_t str[2] = {(uint64_t)K * 2, (uint64_t)K * 32};
+            const uint32_t box[3] = {64, 4, 8};
+            r = make_tmap(&tm.a[a], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, arrs[a], dims, str, box);
+        } else if (geo == GEO_COLS || geo == GEO_ROWS) {
             const uint64_t dims[2] = {(uint64_t)K, (uint64_t)GN};
             const uint64_t str[1] = {(uint64_t)K * 4};
             const uint32_t box[2] = {32, geo == GEO_COLS ? 128u : 32u};
@@ -209,9 +234,9 @@ extern "C" int probe_stream(int geo, int mirror_on, int GN, int K, float* p, flo
         } else {
             const uint64_t dims[3] = {(uint64_t)K, 16, (uint64_t)GN / 16};
             const uint64_t str[2] = {(uint64_t)K * 4, (uint64_t)K * 64};
-            const uint32_t box[3] = {geo == GEO_BANDS ? 32u : 128u, 4, 8};
+            const uint32_t box[3] = {geo == GEO_BANDS_FLAT ? 128u : 32u, 4, 8};
             r = make_tmap(&tm.a[a], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, arrs[a], dims, str, box,
-                          geo == GEO_BANDS ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE);
+                          geo == GEO_BANDS_FLAT ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B);
         }
         if (r) return r;
     }

@@ -4,8 +4,10 @@ The state stream alone — no MMA, no AMSGrad math — at the shapes of the benc
 vmax) read and written back, 58 experts of FeedforwardBlock(512): w1 [2048, 512], w2 [2048, 2048], w3 [512, 2048].  One
 "step" is the three launches.  Every chunk geometry of the probe kernel runs at 80 CTAs (the optimizer stream's share of a
 132-SM H100 in the training step) and on all SMs, TMA only and with the bf16 mirror written by the consumer warps, next to a
-device-to-device copy of the same byte count.  Configurations alternate inside every timing window; the report is the
-median over windows.
+device-to-device copy of the same byte count.  "split_planes" streams the master weight as its bf16 GEMM operand plus a
+16-bit low half (hi, lo, m, v, vmax: 32 B per parameter, all by TMA) instead of fp32 p + the mirror (34 B); every
+configuration's rate counts the bytes it really moves, and the step times compare directly.  Configurations alternate
+inside every timing window; the report is the median over windows.
 
 Run on the GPU: python tools/opt_stream_probe.py [--windows N] [--steps N]; writes check_out/opt_stream_probe.json"""
 import argparse
@@ -22,9 +24,11 @@ import torch
 
 from tools import output_path
 
-GEOS = {"cols_128x32": 0, "rows_32x128": 1, "bands_3d_swz": 2, "bands_3d_flat": 3}
+GEOS = {"cols_128x32": 0, "rows_32x128": 1, "bands_3d_swz": 2, "bands_3d_flat": 3, "split_planes": 4}
+SPLIT = GEOS["split_planes"]
 SHAPES = [(2048, 512), (2048, 2048), (512, 2048)]
 STATE_BYTES_PER_PARAM = 4 * 4 * 2 + 2   # p, m, v, vmax read and written + the bf16 mirror
+SPLIT_BYTES_PER_PARAM = (2 + 2 + 4 * 3) * 2   # hi, lo, m, v, vmax read and written
 
 
 def build(tmp):
@@ -33,7 +37,7 @@ def build(tmp):
     src = os.path.join(ROOT, "tools", "opt_stream_probe.cu")
     subprocess.run([_nvcc(), *NVCC_FLAGS, "-shared", "-I", str(CSRC), src, "-o", so], check=True)
     lib = ctypes.CDLL(so)
-    lib.probe_stream.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p] * 5 + [ctypes.c_int, ctypes.c_void_p]
+    lib.probe_stream.argtypes = [ctypes.c_int] * 4 + [ctypes.c_void_p] * 6 + [ctypes.c_int, ctypes.c_void_p]
     lib.probe_stream.restype = ctypes.c_int
     return lib
 
@@ -50,13 +54,14 @@ def card():
 
 def make_state(G, N, K):
     arrs = [torch.empty(G * N, K, device="cuda").uniform_(0.5, 1.5) for _ in range(4)]
-    return arrs, torch.zeros(G * N, K, device="cuda", dtype=torch.bfloat16)
+    mir = torch.zeros(G * N, K, device="cuda", dtype=torch.bfloat16)
+    return arrs, mir, torch.randint(-2 ** 15, 2 ** 15, (G * N, K), device="cuda", dtype=torch.int16)
 
 
 def launch(lib, geo, mirror_on, st, ctas):
-    (p, m, v, vm), mir = st
+    (p, m, v, vm), mir, lo = st
     r = lib.probe_stream(geo, mirror_on, p.shape[0], p.shape[1], p.data_ptr(), m.data_ptr(), v.data_ptr(), vm.data_ptr(),
-                         mir.data_ptr(), ctas, torch.cuda.current_stream().cuda_stream)
+                         mir.data_ptr(), lo.data_ptr(), ctas, torch.cuda.current_stream().cuda_stream)
     if r:
         raise RuntimeError(f"probe_stream returned {r}")
 
@@ -66,6 +71,13 @@ def check_geometries(lib):
     out = {}
     for name, geo in GEOS.items():
         st = make_state(3, 256, 384)
+        if geo == SPLIT:   # no mirror: every plane and array comes back as it was
+            st[1].copy_(st[0][0])
+            ref = [a.clone() for a in (*st[0][1:], st[1], st[2])]
+            launch(lib, geo, 0, st, 0)
+            torch.cuda.synchronize()
+            out[name] = {"state_unchanged": all(torch.equal(a, b) for a, b in zip((*st[0][1:], st[1], st[2]), ref))}
+            continue
         ref = [a.clone() for a in st[0]]
         launch(lib, geo, 1, st, 0)
         torch.cuda.synchronize()
@@ -96,13 +108,17 @@ def main():
         src = torch.empty(nbytes // 2, dtype=torch.uint8, device="cuda")
         dst = torch.empty_like(src)
         configs = {"copy": lambda: dst.copy_(src)}
+        moved = {"copy": nbytes}
         for gname, geo in GEOS.items():
-            for mirror_on in (0, 1):
+            for mirror_on in ((0,) if geo == SPLIT else (0, 1)):
                 for ctas in (80, sms):
                     def step(geo=geo, mirror_on=mirror_on, ctas=ctas):
                         for st in states:
                             launch(lib, geo, mirror_on, st, ctas)
-                    configs[f"{gname}{'_mirror' if mirror_on else ''}_{ctas}ctas"] = step
+                    key = f"{gname}{'_mirror' if mirror_on else ''}_{ctas}ctas"
+                    configs[key] = step
+                    per_param = SPLIT_BYTES_PER_PARAM if geo == SPLIT else 4 * 4 * 2 + 2 * mirror_on
+                    moved[key] = params * per_param
         for fn in configs.values():
             fn()
         torch.cuda.synchronize()
@@ -121,8 +137,8 @@ def main():
         for k, ts in times.items():
             ts.sort()
             ms = ts[len(ts) // 2]
-            report["results"][k] = {"ms": ms, "TBps": nbytes / ms / 1e9, "spread_ms": [ts[0], ts[-1]]}
-            print(f"{k:32s} {ms:8.3f} ms  {nbytes / ms / 1e9:6.3f} TB/s  (windows {ts[0]:.3f} .. {ts[-1]:.3f})", flush=True)
+            report["results"][k] = {"ms": ms, "bytes": moved[k], "TBps": moved[k] / ms / 1e9, "spread_ms": [ts[0], ts[-1]]}
+            print(f"{k:32s} {ms:8.3f} ms  {moved[k] / ms / 1e9:6.3f} TB/s  (windows {ts[0]:.3f} .. {ts[-1]:.3f})", flush=True)
     with open(output_path("opt_stream_probe.json"), "w") as f:
         json.dump(report, f, indent=1)
     ok = all(all(v.values()) for v in checks.values())
