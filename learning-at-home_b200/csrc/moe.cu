@@ -17,6 +17,8 @@
 // Memory ordering protocol (SURVEY.md §5.2): data is written with plain stores, then `__threadfence_system()` +
 // `st.release.sys` of a monotonically increasing epoch into the consumer's flag word; consumers poll with
 // `ld.acquire.sys`.  Flags never need resetting.  Every poll loop has a clock64() timeout that raises status[0].
+#include <cfloat>
+
 #include "sm90.cuh"
 
 namespace lah {
@@ -113,14 +115,18 @@ __device__ __forceinline__ void account_wait(const Peers& peers, unsigned long l
 }
 
 // ------------------------------------------------------------------------------------------------
-// gate: one warp per token
+// gate: one warp per token.  BIAS (auxiliary-loss-free balancing, DESIGN.md §6b): the top-k is taken over the keys
+// s_{b,e} + bias[e], while the softmax weights use the unbiased s_{b,e} of the selected experts; each candidate carries
+// both values through the per-lane lists and the warp merge.  The bias is read with __ldg: a warp reads 32 consecutive
+// entries per candidate round, which stay in L1 for every token of the SM
 // ------------------------------------------------------------------------------------------------
+template <bool BIAS>
 __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict__ logits, int B, GridSpec gs, int k,
                                                         const unsigned char* __restrict__ alive, float failure_rate,
                                                         unsigned long long seed, long long token_offset,
                                                         int* __restrict__ idx_out, float* __restrict__ w_out,
                                                         int* __restrict__ pos_out, int* __restrict__ counts,
-                                                        const int* __restrict__ step_ctr) {
+                                                        const int* __restrict__ step_ctr, const float* __restrict__ bias) {
     if (step_ctr) token_offset += *reinterpret_cast<const long long*>(step_ctr + 2);
     extern __shared__ float s_logits[];  // [8 warps][gs.total]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -131,11 +137,13 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
     __syncwarp();
 
     // per-lane sorted top-k over the candidates this lane owns (c = lane, lane+32, ...)
-    float best_v[MAX_K];
+    float best_v[MAX_K];   // selection keys (biased when BIAS)
+    float best_u[MAX_K];   // BIAS: the unbiased scores of the same candidates
     int best_i[MAX_K];
 #pragma unroll
     for (int j = 0; j < MAX_K; ++j) {
         best_v[j] = -INFINITY;
+        best_u[j] = -INFINITY;
         best_i[j] = -1;
     }
     for (int c = lane; c < gs.num_experts; c += 32) {
@@ -155,9 +163,11 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
                 s += lg[gs.offset[d] + i];
             }
         }
+        float key = s;
+        if constexpr (BIAS) key = __fadd_rn(s, __ldg(bias + c));
         // insertion (ties keep the smaller expert id first because candidates arrive in increasing order)
-        if (s > best_v[MAX_K - 1] || best_i[MAX_K - 1] < 0) {
-            float v = s;
+        if (key > best_v[MAX_K - 1] || best_i[MAX_K - 1] < 0) {
+            float v = key, u = s;
             int id = c;
             bool shifting = false;  // once inserted, everything below shifts down by one
 #pragma unroll
@@ -171,12 +181,17 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
                     best_i[j] = id;
                     v = tv;
                     id = ti;
+                    if constexpr (BIAS) {
+                        const float tu = best_u[j];
+                        best_u[j] = u;
+                        u = tu;
+                    }
                 }
             }
         }
     }
     // merge: k rounds of warp arg-max over the heads of the per-lane lists
-    float sel_v[MAX_K];
+    float sel_v[MAX_K];   // the unbiased scores of the selected experts (the softmax inputs)
     int sel_i[MAX_K];
     int head = 0;
 #pragma unroll
@@ -184,27 +199,31 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
         sel_v[j] = -INFINITY;
         sel_i[j] = -1;
         if (j < k) {
-            float v = -INFINITY;
+            float v = -INFINITY, u = -INFINITY;
             int id = -1;
 #pragma unroll
             for (int t = 0; t < MAX_K; ++t)
                 if (t == head) {
                     v = best_v[t];
                     id = best_i[t];
+                    if constexpr (BIAS) u = best_u[t];
                 }
-            float bv = v;
+            float bv = v, bu = u;
             int bi = id;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
                 const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
                 const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                float ou = 0.f;
+                if constexpr (BIAS) ou = __shfl_xor_sync(0xffffffffu, bu, o);
                 const bool better = (oi >= 0) && (bi < 0 || ov > bv || (ov == bv && oi < bi));
                 if (better) {
                     bv = ov;
                     bi = oi;
+                    if constexpr (BIAS) bu = ou;
                 }
             }
-            sel_v[j] = bv;
+            sel_v[j] = BIAS ? bu : bv;
             sel_i[j] = bi;
             if (bi >= 0 && bi == id) ++head;  // the winning lane pops its head
         }
@@ -964,6 +983,41 @@ __global__ void __launch_bounds__(1024) router_f_kernel(const int* __restrict__ 
     }
 }
 
+// auxiliary-loss-free balancing (DESIGN.md §6b): with c_e = sum over the `rows` rank rows of the count table, T = sum_e c_e
+// and N the live experts, every live expert moves its bias by rate toward balance: + if N c_e < T, - if N c_e > T.  Dead
+// experts and T = 0 change nothing.  One CTA of 1024 threads; the comparisons are exact in 64-bit integers, and each
+// bias gets one float add, so every rank (same table) and every run computes the same bits
+__global__ void __launch_bounds__(1024) expert_bias_update_kernel(const int* __restrict__ cnt, int rows, int E,
+                                                                  const unsigned char* __restrict__ alive, float rate,
+                                                                  float* __restrict__ bias) {
+    __shared__ long long s_total;
+    __shared__ int s_live;
+    if (threadIdx.x == 0) {
+        s_total = 0;
+        s_live = 0;
+    }
+    __syncthreads();
+    long long tot = 0;
+    int live = 0;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+        for (int r = 0; r < rows; ++r) tot += cnt[static_cast<long long>(r) * E + e];
+        live += (!alive || alive[e]) ? 1 : 0;
+    }
+    atomicAdd(reinterpret_cast<unsigned long long*>(&s_total), static_cast<unsigned long long>(tot));
+    atomicAdd(&s_live, live);
+    __syncthreads();
+    const long long T = s_total, N = s_live;
+    if (T == 0) return;
+    for (int e = threadIdx.x; e < E; e += blockDim.x) {
+        if (alive && !alive[e]) continue;
+        long long c = 0;
+        for (int r = 0; r < rows; ++r) c += cnt[static_cast<long long>(r) * E + e];
+        const long long nc = N * c;
+        if (nc < T) bias[e] = __fadd_rn(bias[e], rate);
+        else if (nc > T) bias[e] = __fsub_rn(bias[e], rate);
+    }
+}
+
 // product-key score of expert c, summed last grid dimension first (the order of gate_topk_kernel)
 __device__ __forceinline__ float pk_score(const float* lg, const GridSpec& gs, int c) {
     int rem = c;
@@ -1224,20 +1278,27 @@ static int make_grid_spec(GridSpec* gs, const int* grid, int ndim) {
     return 0;
 }
 
+// bias: float [prod(grid)] added to the scores for the selection only (DESIGN.md §6b); nullptr selects without one
 int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, const unsigned char* alive,
                   float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w, int* pos,
-                  int* counts, cudaStream_t st) {
+                  int* counts, const float* bias, cudaStream_t st) {
     GridSpec gs;
     if (make_grid_spec(&gs, grid, ndim)) return -2;
     if (k < 1 || k > MAX_K) return -3;
     // each of the 8 warps stages its token's grid logits in shared memory: 4096 of them (a dense gate over as many experts
     // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in
     if (gs.total > LAYOUT_MAX_E) return -2;
-    if (int e = set_max_dynamic_smem<gate_topk_kernel>(8 * sizeof(float) * LAYOUT_MAX_E)) return e;
+    if (bias && gs.num_experts > LAYOUT_MAX_E) return -2;
+    if (int e = bias ? set_max_dynamic_smem<gate_topk_kernel<true>>(8 * sizeof(float) * LAYOUT_MAX_E)
+                     : set_max_dynamic_smem<gate_topk_kernel<false>>(8 * sizeof(float) * LAYOUT_MAX_E))
+        return e;
     if (B <= 0) return 0;
-    gate_topk_kernel<<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(logits, B, gs, k, alive, failure_rate, seed,
-                                                                           token_offset, idx, w, pos, counts,
-                                                                           g_peers.step_ctr);
+    if (bias)
+        gate_topk_kernel<true><<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(
+            logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, bias);
+    else
+        gate_topk_kernel<false><<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(
+            logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, nullptr);
     rank_slots_kernel<<<gs.num_experts, 1024, 0, st>>>(idx, B * k, pos, counts);
     return -(int)cudaGetLastError();
 }
@@ -1366,6 +1427,17 @@ int lah_router_loss_bwd(const float* logits, int B, const int* grid, int ndim, c
     router_loss_bwd_kernel<<<(B + RL_WARPS - 1) / RL_WARPS, RL_WARPS * 32,
                              RL_WARPS * router_bwd_warp_floats(gs) * sizeof(float), st>>>(logits, B, gs, alive, f, z, Fb,
                                                                                          aux_coef, z_coef, dlogits);
+    return -(int)cudaGetLastError();
+}
+
+// auxiliary-loss-free balancing: bias [E] moves by rate toward balance from the count table [count_rows][E] (one launch)
+int lah_expert_bias_update(const int* counts, int count_rows, int E, const unsigned char* alive, float rate, float* bias,
+                           cudaStream_t st) {
+    if (E < 1 || E > LAYOUT_MAX_E) return -2;
+    if (count_rows < 1 || count_rows > MAX_WORLD) return -3;
+    if (!counts || !bias) return -4;
+    if (!(rate >= 0.f && rate <= FLT_MAX)) return -5;   // finite and >= 0 (NaN fails both)
+    expert_bias_update_kernel<<<1, 1024, 0, st>>>(counts, count_rows, E, alive, rate, bias);
     return -(int)cudaGetLastError();
 }
 

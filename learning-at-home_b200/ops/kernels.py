@@ -44,7 +44,8 @@ def _lib():
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
-        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P],
+        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, P],
+        "lah_expert_bias_update": [P, I, I, P, Fl, P, P],
         "lah_layout_exchange": [L, L, I, I, I, I, I, I, I, P, P, P, P, P, P, P, I, Fl, I, P, P, P, P, P],
         "lah_scatter_rows": [P, P, P, P, P, P, L, L, I, I, I, I, I, I, I, I, P, P, P, P, P, I, P],
         "lah_pull_shadow": [P, I, I, L, L, I, P, I, P],
@@ -331,13 +332,47 @@ def set_spin_timeout_ms(ms):
     native.check(_lib().lah_set_spin_timeout_ms(int(ms)), "lah_set_spin_timeout_ms")
 
 
-def gate_topk(logits, grid_size, k, *, alive=None, failure_rate=0.0, seed=0, token_offset=0, idx, w, pos, counts):
+def _check_expert_bias(what, bias, E, device):
+    if bias.dtype != torch.float32 or bias.dim() != 1 or bias.numel() != E or not bias.is_contiguous() \
+            or bias.device != device:
+        raise ValueError(f"{what}: bias must be a contiguous float32 [{E}] tensor on {device}, got {bias.dtype} "
+                         f"{tuple(bias.shape)} on {bias.device}")
+
+
+def gate_topk(logits, grid_size, k, *, alive=None, failure_rate=0.0, seed=0, token_offset=0, idx, w, pos, counts,
+              bias=None):
+    """top-k routing of the grid logits (two launches).  ``bias``: float32 [prod(grid)] added to the scores for the
+    selection only; the weights stay the softmax over the unbiased scores of the selected experts (DESIGN.md §6b)"""
     B = logits.shape[0]
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.shape[1] == sum(grid_size)
+    if bias is not None:
+        _check_expert_bias("gate_topk", bias, math.prod(grid_size), logits.device)
     native.check(_lib().lah_gate_topk(ptr(logits), B, ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), k,
                                       ptr(alive), float(failure_rate), int(seed) & (2 ** 64 - 1), int(token_offset),
-                                      ptr(idx), ptr(w), ptr(pos), ptr(counts), stream_ptr()), "lah_gate_topk")
+                                      ptr(idx), ptr(w), ptr(pos), ptr(counts), ptr(bias), stream_ptr()), "lah_gate_topk")
     native.count_launch(2)
+
+
+def expert_bias_update(counts, *, alive=None, bias, rate):
+    """Auxiliary-loss-free balancing step (one launch): every live expert's ``bias`` moves by ``rate`` toward balance,
+    + when N c_e < T, - when N c_e > T (c_e: routed pairs of the int32 [R, E] count table summed over R, T = sum_e c_e,
+    N = live experts).  Dead experts and T = 0 change nothing (DESIGN.md §6b)."""
+    if counts.dtype != torch.int32 or counts.dim() != 2 or not counts.is_contiguous() \
+            or not 1 <= counts.shape[0] <= MAX_WORLD or not 1 <= counts.shape[1] <= LAYOUT_MAX_E:
+        raise ValueError(f"expert_bias_update: counts must be a contiguous int32 [R <= {MAX_WORLD}, E <= {LAYOUT_MAX_E}] "
+                         f"tensor, got {counts.dtype} {tuple(counts.shape)}")
+    E = counts.shape[1]
+    _check_expert_bias("expert_bias_update", bias, E, counts.device)
+    if alive is not None and (alive.dtype != torch.uint8 or alive.numel() != E or not alive.is_contiguous()):
+        raise ValueError(f"expert_bias_update: alive must be a contiguous uint8 tensor of {E} entries, got {alive.dtype} "
+                         f"{tuple(alive.shape)}")
+    rate = float(rate)
+    if not math.isfinite(rate) or rate < 0.0:
+        raise ValueError(f"expert_bias_update: rate must be a finite value >= 0, got {rate}")
+    native.check(_lib().lah_expert_bias_update(ptr(counts), counts.shape[0], E, ptr(alive), rate, ptr(bias),
+                                               stream_ptr()), "lah_expert_bias_update")
+    native.count_launch()
+    return bias
 
 
 def layout_exchange(cnt_all_off, flags_off, slot, epoch, E, E_loc, max_rows, *, align=128, tile_rows=None, counts, dst_row, group_off, group_rows,
@@ -1030,11 +1065,13 @@ def product_key_scores(logits, grid_size):
     return scores
 
 
-def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None):
+def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None):
     """returns idx [B,k] (-1 for missing), weights [B,k] (softmax over alive selected).  Equal scores select the smaller
     expert id first, like gate_topk_kernel (torch.topk leaves the order of ties unspecified, so it sorts stably instead).
     The scores are summed first grid dimension first and the kernel last dimension first: on 3-d and 4-d grids they can
-    differ in the last bit unless the logits are exact in any order (e.g. small multiples of a power of two)."""
+    differ in the last bit unless the logits are exact in any order (e.g. small multiples of a power of two).
+    ``bias`` ([E]): the selection ranks the float32 keys score + bias[e]; the weights stay the softmax over the unbiased
+    scores of the selected experts."""
     scores = product_key_scores(logits.float(), grid_size)
     dead = torch.zeros_like(scores, dtype=torch.bool)
     if alive is not None:
@@ -1044,8 +1081,14 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None):
     scores = scores.masked_fill(dead, float("-inf"))
     if scores.shape[-1] < k:
         scores = F.pad(scores, (0, k - scores.shape[-1]), value=float("-inf"))
-    top_v, top_i = torch.sort(scores, dim=-1, descending=True, stable=True)
-    top_v, top_i = top_v[..., :k], top_i[..., :k]
+    if bias is None:
+        top_v, top_i = torch.sort(scores, dim=-1, descending=True, stable=True)
+        top_v, top_i = top_v[..., :k], top_i[..., :k]
+    else:
+        b = bias.to(device=scores.device, dtype=torch.float32).reshape(1, -1)
+        keys = scores + F.pad(b, (0, scores.shape[-1] - b.shape[-1]))
+        top_i = torch.sort(keys, dim=-1, descending=True, stable=True)[1][..., :k]
+        top_v = torch.gather(scores, -1, top_i)
     valid = torch.isfinite(top_v)
     w = torch.softmax(top_v.masked_fill(~valid, float("-inf")), dim=-1)
     w = torch.where(valid, w, torch.zeros_like(w)).nan_to_num(0.0)
@@ -1073,6 +1116,22 @@ def router_loss_ref(logits, grid_size, counts, alive=None):
     p = torch.where(live.view(1, -1) & ok, torch.exp(masked - z), torch.zeros_like(masked))
     z = torch.where(ok, z, torch.zeros_like(z)).squeeze(-1)
     return N * (p * f).sum() / B, (z * z).sum() / B
+
+
+def expert_bias_update_ref(counts, bias, rate, alive=None):
+    """Oracle of expert_bias_update: the updated float32 bias (a new tensor).  ``counts``: [E] or [R, E] routed pairs
+    (summed over R).  The comparisons N c_e <> T are exact integers; a moving bias gets one float32 add of +-rate."""
+    bias = bias.to(torch.float32)
+    E = bias.numel()
+    c = counts.reshape(-1, E).to(torch.int64).sum(0).cpu()
+    live = torch.ones(E, dtype=torch.bool) if alive is None else alive.bool().reshape(-1).cpu()
+    T, N = int(c.sum()), int(live.sum())
+    step = torch.sign(T - N * c) * live   # +1: below the mean load, -1: above, 0: balanced or dead
+    if T == 0:
+        step.zero_()
+    rate32 = torch.tensor(rate, dtype=torch.float32)
+    out = torch.where(step != 0, bias.cpu() + step.to(torch.float32) * rate32, bias.cpu())
+    return out.to(bias.device)
 
 
 _SPLITMIX_GAMMA = 0x9E3779B97F4A7C15

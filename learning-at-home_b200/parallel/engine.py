@@ -116,6 +116,12 @@ class DMoEConfig:
     # for the life of a layer or trainer.  0 and 0 (the default) launch nothing
     router_aux_loss_coef: float = 0.0
     router_z_loss_coef: float = 0.0
+    # auxiliary-loss-free balancing (DESIGN.md §6b, DeepSeek-V3): each layer keeps a bias per expert that is added to the
+    # scores for the top-k selection only (the weights stay the softmax over the unbiased scores).  After the count
+    # exchange of every training forward, each live expert's bias moves by this rate toward balance: + when it received
+    # fewer than the mean box-wide routed pairs, - when more.  No loss and no gradient, so it also balances the frozen
+    # emulator gate.  Read at construction; 0 (the default) allocates and launches nothing
+    expert_bias_update_rate: float = 0.0
 
     def __post_init__(self):
         if self.expert not in EXPERT_LAYOUTS:
@@ -135,6 +141,9 @@ class DMoEConfig:
             if v > 0.0 and self.gate_mode == "emulator":
                 raise ValueError(f"DMoEConfig.{name}: the emulator gate is frozen (not trained), so a router loss would "
                                  "train nothing; use gate_mode='product_key'")
+        v = float(self.expert_bias_update_rate)
+        if not math.isfinite(v) or v < 0.0:
+            raise ValueError(f"DMoEConfig.expert_bias_update_rate must be a finite value >= 0, got {v}")
 
     @property
     def router_losses(self) -> bool:
@@ -204,6 +213,13 @@ def refuse_router_losses(cfg: DMoEConfig, arm: str):
     if cfg.router_losses:
         raise ValueError(f"{arm} does not train router losses; set router_aux_loss_coef and router_z_loss_coef to 0 "
                          "(FusedDMoE / DMoETrainer train them)")
+
+
+def refuse_expert_bias(cfg: DMoEConfig, arm: str):
+    """the baseline arms route without expert biases: refuse a nonzero update rate instead of silently dropping it"""
+    if cfg.expert_bias_update_rate > 0.0:
+        raise ValueError(f"{arm} does not balance with expert biases; set expert_bias_update_rate to 0 "
+                         "(FusedDMoE / DMoETrainer apply them)")
 
 
 def expert_uid(cfg: DMoEConfig, e: int) -> str:
@@ -772,6 +788,12 @@ class FusedDMoE(nn.Module):
             self.router_loss = self.ws.router_loss if self.router_on else None
         else:                     # a buffer, so that .to() / .cuda() move it with the layer (not saved in state_dict)
             self.register_buffer("router_loss", torch.zeros(2, device=dev) if self.router_on else None, persistent=False)
+        # auxiliary-loss-free balancing (cfg.expert_bias_update_rate, read here once): router state like proj, the same on
+        # every rank; a persistent buffer, so it is saved with the trainer-side parameters, and kept at one device address
+        # (a captured graph reads it)
+        self.expert_bias_rate = float(cfg.expert_bias_update_rate)
+        self.register_buffer("expert_bias", torch.zeros(cfg.num_experts, dtype=torch.float32, device=dev)
+                             if self.expert_bias_rate > 0.0 else None)
 
     # ------------------------------------------------------------------ public forward
     def forward(self, x):
@@ -822,7 +844,7 @@ class FusedDMoE(nn.Module):
         idx, w, pos, pair_row = ws.idx[:P], ws.w[:P], ws.pos[:P], ws.pair_row[:P]
         K.gate_topk(logits, self.grid_size, k, alive=c.alive, failure_rate=cfg.failure_rate if self.training else 0.0,
                     seed=cfg.seed * 7919 + self.layer_index, token_offset=c.token_counter, idx=idx, w=w, pos=pos,
-                    counts=c.counts)
+                    counts=c.counts, bias=self.expert_bias)
         c.token_counter += B
         c.timer.mark("gate_topk")
         K.layout_exchange(c.cnt_all_off, c.flags_off, K.SLOT_COUNTS, epoch, c.E, c.E_loc, c.max_rows, align=c.align,
@@ -836,6 +858,8 @@ class FusedDMoE(nn.Module):
             # rank's combine has signalled
             K.router_loss_fwd(logits, self.grid_size, c.cnt_all[:c.world], alive=c.alive, f=ws.router_f, z=ws.router_z,
                               Fb=ws.router_F, loss=ws.router_loss, partials=c.router_partials, ticket=c.router_ticket)
+        if self.training and self.expert_bias is not None:   # same cnt_all lifetime as the router losses above
+            K.expert_bias_update(c.cnt_all[:c.world], alive=c.alive, bias=self.expert_bias, rate=self.expert_bias_rate)
         if c.S:  # replicas of this step's hot experts: weights from the owners' bf16 mirror, small params from fp32
             K.pull_shadow(ws.shadow_info, c.S, c.E_loc, sh.p_off, sh.pbf16_off, sh.seg_sizes, sh.layout.small_mask)
             sh.w8_dirty = True
@@ -1115,9 +1139,13 @@ class FusedDMoE(nn.Module):
         fail_mask = self.ref_fail_mask
         if fail_mask is None and self.failure_rate_ref() > 0:
             fail_mask = torch.rand(x.shape[0], cfg.num_experts, device=x.device) < cfg.failure_rate
-        idx, w_sel = K.gate_topk_ref(logits.detach(), self.grid_size, cfg.k,
-                                     alive=self.ctx.alive if self.ctx is not None else getattr(self, "alive_ref", None),
-                                     fail_mask=fail_mask)
+        alive = self.ctx.alive if self.ctx is not None else getattr(self, "alive_ref", None)
+        idx, w_sel = K.gate_topk_ref(logits.detach(), self.grid_size, cfg.k, alive=alive, fail_mask=fail_mask,
+                                     bias=self.expert_bias)
+        if self.training and self.expert_bias is not None:
+            with torch.no_grad():
+                counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
+                self.expert_bias.copy_(K.expert_bias_update_ref(counts, self.expert_bias, self.expert_bias_rate, alive))
         # differentiable weights: softmax over the selected logits
         scores = K.product_key_scores(logits, self.grid_size)
         safe_idx = idx.clamp(min=0)
@@ -1139,7 +1167,6 @@ class FusedDMoE(nn.Module):
             ye = self._expert_ref(p, rnd(xf[tok]), rnd)
             out = out.index_put((tok,), ye * weights[tok, slot].unsqueeze(-1), accumulate=True)
         if self.training and self.router_on:
-            alive = self.ctx.alive if self.ctx is not None else getattr(self, "alive_ref", None)
             counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
             l_aux, l_z = K.router_loss_ref(logits, self.grid_size, counts, alive=alive)
             with torch.no_grad():

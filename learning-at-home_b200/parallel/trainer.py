@@ -306,6 +306,8 @@ class DMoETrainer:
                 if block.router_loss is not None:   # this rank's unweighted router losses of the layer's last forward
                     aux, z = block.router_loss.tolist()
                     layer.update(router_aux_loss=aux, router_z_loss=z)
+                if block.expert_bias is not None:
+                    layer["expert_bias_absmax"] = float(block.expert_bias.abs().max())
                 layers.append(layer)
             rec["layers"] = layers
             if self.last_stage_ms:
@@ -455,9 +457,19 @@ class DMoETrainer:
 
     def load_state_dict(self, state):
         from .engine import expert_uid
+        own = self.model.state_dict()
+        saved = state["trainer"]["model"]
+        biases = [k for k in own if k.endswith(".expert_bias")]
+        if any(k.endswith(".expert_bias") and k not in own for k in saved):
+            # dropping the saved biases would silently change which experts the gates select
+            raise ValueError("checkpoint holds expert routing biases, but this trainer has expert_bias_update_rate=0; "
+                             "build it with expert_bias_update_rate > 0 to resume them")
         with torch.no_grad():
-            for k, v in state["trainer"]["model"].items():
-                self.model.state_dict()[k].copy_(v)
+            for k in biases:   # a checkpoint without biases starts them at zero (in place: a captured graph reads them)
+                if k not in saved:
+                    own[k].zero_()
+            for k, v in saved.items():
+                own[k].copy_(v)
             self.flat_m.copy_(state["trainer"]["exp_avg"])
             self.flat_v.copy_(state["trainer"]["exp_avg_sq"])
             self.flat_vmax.copy_(state["trainer"]["max_exp_avg_sq"])

@@ -30,10 +30,12 @@ def main():
     swiglu = "--swiglu" in sys.argv   # GatedFeedforwardBlock experts (compares [W1; W3] and the RMSNorm weight)
     # router losses of the product-key gate: f from the box-wide count table, P from each rank's own tokens
     router = dict(router_aux_loss_coef=0.01, router_z_loss_coef=0.001) if "--router-loss" in sys.argv else {}
+    # auxiliary-loss-free balancing: every rank moves its copy of the expert biases from the same box-wide count table
+    bias = dict(expert_bias_update_rate=0.01) if "--expert-bias" in sys.argv else {}
     mat, vec = ("w13", "g") if swiglu else ("w1", "b2")
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=B, capacity_factor=float(max(4, world)),
                        shadow_experts=4, shadow_tol=0.0 if force_shadow else 1.1, shadow_min_rows=1 if force_shadow else 64,
-                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router)
+                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router, **bias)
     ctx = E.EngineContext(cfg)
     torch.manual_seed(0)  # identical gate on every rank (DMoETrainer does the same)
     layer = E.FusedDMoE(cfg, ctx).cuda()
@@ -81,6 +83,22 @@ def main():
         g_router = layer.proj.weight.grad.clone()
         dist.all_reduce(g_router)
         counts_box = ctx.cnt_all[:world].clone()   # the box-wide count table of that step, the same on every rank
+    bias_ok = True
+    if bias:
+        # after several more steps on per-rank batches, each step's update must equal the oracle over that step's gathered
+        # count table, and every rank must hold the same bits
+        gen_r = torch.Generator().manual_seed(100 + rank)
+        for _ in range(4):
+            before = layer.expert_bias.clone()
+            xs = torch.randn(B, 512, generator=gen_r).to(torch.bfloat16).cuda()
+            layer(xs).backward(torch.randn(B, 512, generator=gen_r).to(torch.bfloat16).cuda())
+            torch.cuda.synchronize()
+            ctx.check_status()
+            want = K.expert_bias_update_ref(ctx.cnt_all[:world], before, cfg.expert_bias_update_rate)
+            bias_ok = bias_ok and torch.equal(layer.expert_bias, want) and not torch.equal(layer.expert_bias, before)
+        biases = [torch.empty_like(layer.expert_bias) for _ in range(world)]
+        dist.all_gather(biases, layer.expert_bias)
+        bias_ok = bias_ok and all(torch.equal(b, biases[0]) for b in biases)
     ok = True
     if rank == 0:
         # single-GPU reference in the same process: a fresh world-1 context is impossible inside an initialised group,
@@ -109,7 +127,9 @@ def main():
             errs["router_grad_max_err"] = ((g_router.double() - ref_router).abs().max() / ref_router.abs().max()).item()
         ok = errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2 and errs["w1_mean_abs"] < 1e-4 and errs["b2_max_abs"] < 2.5e-3 and errs["steps"]
         ok = ok and (shadowed > 0 or not force_shadow) and plan_ok and errs.get("router_loss", 0.0) < 1e-4
-        ok = ok and errs.get("router_grad_max_err", 0.0) < 1e-4
+        ok = ok and errs.get("router_grad_max_err", 0.0) < 1e-4 and bias_ok
+        if bias:
+            errs["expert_bias_bit_identical_and_equal_to_oracle"] = bias_ok
         print("multi_gpu_check", dict(path="small" if small else "big", expert=cfg.expert, router_loss=bool(router), force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
                                       plan=plan, kernel=got), errs, flush=True)
         print("MULTI_GPU_OK" if ok else "MULTI_GPU_FAILED", flush=True)
