@@ -734,6 +734,8 @@ __global__ void step_begin_kernel(int* step_ctr, int epoch_delta, long long toke
 
 // ------------------------------------------------------------------------------------------------
 // combine: warp per token; out[b] = sum_j w[b,j] * src_owner(j)[row(b,j)]     (w == nullptr -> plain sum)
+//   ADD: out[b] = addend[b] + sum_j ...: the bf16 [B, H] addend (the shared expert's output or input gradient) starts the
+//   fp32 accumulator, so the sum is rounded to bf16 once
 // ------------------------------------------------------------------------------------------------
 struct CombineArgs {
     long long src_off;        // symmetric [max_rows, H] bf16 on the owners
@@ -749,8 +751,8 @@ struct CombineArgs {
     const int* route_owner;   // [E] rank that holds MY rows of expert e (nullptr: e / E_loc)
 };
 
-template <int VEC_PER_LANE>
-__global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineArgs a) {
+template <int VEC_PER_LANE, bool ADD>
+__global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineArgs a, const bf16* __restrict__ addend) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (a.do_signal || a.do_wait) a.epoch = epoch_of(peers, a.epoch);
     if (a.do_signal && blockIdx.x == 0 && threadIdx.x < 32) {
@@ -769,8 +771,23 @@ __global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineA
     const int b = blockIdx.x * 8 + warp;
     if (b >= a.B) return;
     float acc[VEC_PER_LANE * 8];
+    if constexpr (ADD) {
+        const int4* ap = reinterpret_cast<const int4*>(addend + static_cast<long long>(b) * a.H);
 #pragma unroll
-    for (int i = 0; i < VEC_PER_LANE * 8; ++i) acc[i] = 0.f;
+        for (int v = 0; v < VEC_PER_LANE; ++v) {
+            const int4 q = __ldg(ap + v * 32 + lane);
+            const uint32_t u[4] = {(uint32_t)q.x, (uint32_t)q.y, (uint32_t)q.z, (uint32_t)q.w};
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+                const float2 f = unpack_bf16x2(u[t]);
+                acc[v * 8 + 2 * t] = f.x;
+                acc[v * 8 + 2 * t + 1] = f.y;
+            }
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < VEC_PER_LANE * 8; ++i) acc[i] = 0.f;
+    }
     for (int j = 0; j < a.k; ++j) {
         const long long p = static_cast<long long>(b) * a.k + j;
         const int e = a.idx[p];
@@ -1347,9 +1364,10 @@ int lah_signal_wait(long long flags_off, int slot, int epoch, int do_signal, int
     return -(int)cudaGetLastError();
 }
 
+// addend: optional bf16 [B, H] added to every output row before its one rounding (nullptr: the plain kernel)
 int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, const float* w, void* out, int B, int k,
                      int H, int E_loc, long long flags_off, int slot, int epoch, int do_signal, int do_wait, int* status,
-                     const int* route_owner, cudaStream_t st) {
+                     const int* route_owner, const void* addend, cudaStream_t st) {
     if (!g_peers_set) return -10;
     if (B <= 0) return 0;
     CombineArgs a;
@@ -1357,10 +1375,16 @@ int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, con
     a.E_loc = E_loc; a.flags_off = flags_off; a.slot = slot; a.epoch = epoch; a.do_signal = do_signal; a.do_wait = do_wait;
     a.status = status; a.route_owner = route_owner;
     const int grid = (B + 7) / 8;
-    if (H == 256) combine_rows_kernel<1><<<grid, 256, 0, st>>>(g_peers, a);
-    else if (H == 512) combine_rows_kernel<2><<<grid, 256, 0, st>>>(g_peers, a);
-    else if (H == 1024) combine_rows_kernel<4><<<grid, 256, 0, st>>>(g_peers, a);
+    const bf16* add = (const bf16*)addend;
+    if (add && (reinterpret_cast<uintptr_t>(add) % 16)) return -3;   // read as 16-byte vectors
+#define LAH_COMBINE(V)                                                                   \
+    if (add) combine_rows_kernel<V, true><<<grid, 256, 0, st>>>(g_peers, a, add);        \
+    else combine_rows_kernel<V, false><<<grid, 256, 0, st>>>(g_peers, a, nullptr);
+    if (H == 256) { LAH_COMBINE(1) }
+    else if (H == 512) { LAH_COMBINE(2) }
+    else if (H == 1024) { LAH_COMBINE(4) }
     else return -2;
+#undef LAH_COMBINE
     return -(int)cudaGetLastError();
 }
 

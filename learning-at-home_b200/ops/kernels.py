@@ -51,7 +51,7 @@ def _lib():
         "lah_pull_shadow": [P, I, I, L, L, I, P, I, P],
         "lah_zero_slots": [P, I, P, I, I, I, I, P],
         "lah_signal_wait": [L, I, I, I, I, P, P],
-        "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P],
+        "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P, P],
         "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P],
         "lah_router_loss_fwd": [P, I, P, I, P, P, I, P, P, P, P, P, P, P],
         "lah_router_loss_bwd": [P, I, P, I, P, P, P, P, Fl, Fl, P, P],
@@ -423,16 +423,35 @@ def signal_wait(flags_off, slot, epoch, status, *, signal=True, wait=True):
 
 
 def combine_rows(src_off, idx, pair_row, w, out, k, E_loc, *, flags_off=0, slot=0, epoch=0, signal=False, wait=False,
-                 status=None, route_owner=None):
+                 status=None, route_owner=None, addend=None):
     """weighted P2P gather; with signal/wait the kernel itself publishes 'my expert outputs are ready' to every peer
-    and waits for all peers' flags before pulling their rows (no separate flag kernels)"""
+    and waits for all peers' flags before pulling their rows (no separate flag kernels).
+    :param addend: optional bf16 [B, H] (contiguous, 16-byte aligned) that starts every row's fp32 accumulator:
+        out = bf16(addend + sum_j w_j src_j), rounded once.  None launches the plain kernel"""
     B, H = out.shape
+    if addend is not None:
+        _bf16_rows(addend, "combine_rows addend", (B, H))
+        if addend.data_ptr() % 16:
+            raise ValueError("combine_rows: the addend must be 16-byte aligned")
     native.check(_lib().lah_combine_rows(src_off, ptr(idx), ptr(pair_row), ptr(w), ptr(out), B, k, H, E_loc, flags_off,
                                          slot, epoch, int(signal), int(wait), ptr(status), ptr(route_owner),
-                                         stream_ptr()),
+                                         ptr(addend), stream_ptr()),
                  "lah_combine_rows")
     native.count_launch()
     return out
+
+
+def combine_rows_ref(src, idx, pair_row, w=None, addend=None):
+    """exact oracle of ``combine_rows`` on one rank's rows: the float64 sum addend[b] + sum_j w[b, j] src[pair_row[b, j]]
+    over the pairs with an expert and a row, rounded to bf16 once.  ``src``: [R, H]; idx, pair_row, w: [B, k]"""
+    present = ((idx >= 0) & (pair_row >= 0)).double()
+    if w is not None:
+        present = present * w.double()
+    terms = src.double()[pair_row.clamp(min=0).long()] * present.unsqueeze(-1)
+    total = terms.sum(1)
+    if addend is not None:
+        total = total + addend.double()
+    return total.to(torch.bfloat16)
 
 
 def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route_owner=None):

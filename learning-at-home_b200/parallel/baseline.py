@@ -5,7 +5,8 @@ baseline, not the product" (BASELINE.json) — this module exists to be measured
 and as a second, independently written oracle for the fused engine (same routing, same maths, autograd everywhere).
 
 Experts are real ``FeedforwardBlock`` modules (reference architecture, /root/reference/experiments/throughput/layers.py),
-or ``GatedFeedforwardBlock`` modules with ``DMoEConfig(expert="swiglu")``.
+or ``GatedFeedforwardBlock`` modules with ``DMoEConfig(expert="swiglu")``; ``DMoEConfig(shared_inner_dim=...)`` adds a real
+``GatedFeedforwardBlock`` shared expert whose ``module(x) - x`` every token receives.
 """
 import math
 from typing import List, Optional
@@ -63,6 +64,9 @@ class BaselineDMoE(nn.Module):
                 experts.append(GatedFeedforwardBlock(cfg.hidden, cfg.inner, eps=GATED_EPS) if cfg.expert == "swiglu"
                                else FeedforwardBlock(cfg.hidden))
         self.experts = nn.ModuleList(experts)
+        # the shared expert: a trainer-side module (replicated, averaged over ranks by BaselineTrainer), like proj
+        self.shared_expert = (GatedFeedforwardBlock(cfg.hidden, cfg.shared_inner_dim, eps=GATED_EPS)
+                              if cfg.shared_inner_dim else None)
         if device is not None:
             self.to(device)
         self.expert_optimizers = [torch.optim.Adam(e.parameters(), lr=cfg.lr, betas=cfg.betas, eps=cfg.eps,
@@ -78,7 +82,8 @@ class BaselineDMoE(nn.Module):
                 expert.load_state_dict(shard.layout.module_state({n: shard.views[n][le] for n in shard.layout.names}))
 
     def non_expert_parameters(self):
-        return list(self.proj.parameters())
+        shared = list(self.shared_expert.parameters()) if self.shared_expert is not None else []
+        return list(self.proj.parameters()) + shared
 
     def forward(self, x):
         cfg, k = self.cfg, self.cfg.k
@@ -127,6 +132,9 @@ class BaselineDMoE(nn.Module):
         w_pairs = weights.reshape(-1)[order].to(returned.dtype)
         out = torch.zeros(B, cfg.hidden, dtype=returned.dtype, device=x.device)
         out = out.index_add(0, tokens, returned * w_pairs.unsqueeze(-1))
+        if self.shared_expert is not None:
+            xs = x.to(self.dtype)
+            out = out + (self.shared_expert(xs) - xs)
         self._rows = torch.tensor(sizes)
         return out.to(x.dtype)
 

@@ -26,11 +26,16 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..models.layers import FFN_SEG_KEYS as REF_KEYS, FFN_SEG_NAMES as SEG_NAMES, FFN_SMALL_SEG_MASK as SMALL_SEG_MASK
-from ..models.layers import EXPERT_LAYOUTS, gated_inner_dim
+from ..models.layers import EXPERT_LAYOUTS, GATED_LAYOUT, GatedFeedforwardBlock, gated_inner_dim
 from ..ops import fp8, gemm, kernels as K, native
 
 #: eps of the gated expert's RMSNorm (GatedFeedforwardBlock's default)
 GATED_EPS = 1e-6
+#: the shared expert's GEMMs stream its weights through swap-AB tiles below this many rows per call, and run on 128-row
+#: wgmma tiles from there on (the routed experts' "auto" switch)
+SHARED_SWAPAB_ROWS = 512
+#: rows of the shared expert's buffers are padded to this (the 128-row tiles; swap-AB and wgrad read whole pads)
+SHARED_PAD = 128
 
 
 @dataclass
@@ -122,6 +127,11 @@ class DMoEConfig:
     # fewer than the mean box-wide routed pairs, - when more.  No loss and no gradient, so it also balances the frozen
     # emulator gate.  Read at construction; 0 (the default) allocates and launches nothing
     expert_bias_update_rate: float = 0.0
+    # shared-expert isolation (DESIGN.md §9c, DeepSeek-MoE / Qwen-MoE): every token also passes through one always-active
+    # GatedFeedforwardBlock of this inner width, added to the combine of the routed experts with weight 1 and without a
+    # second residual.  Its parameters are trainer-side (replicated on every rank, averaged over ranks, stepped once per
+    # step, like proj).  expert="swiglu" only; 0 (the default) allocates and launches nothing
+    shared_inner_dim: int = 0
 
     def __post_init__(self):
         if self.expert not in EXPERT_LAYOUTS:
@@ -144,6 +154,11 @@ class DMoEConfig:
         v = float(self.expert_bias_update_rate)
         if not math.isfinite(v) or v < 0.0:
             raise ValueError(f"DMoEConfig.expert_bias_update_rate must be a finite value >= 0, got {v}")
+        if self.shared_inner_dim < 0:
+            raise ValueError(f"DMoEConfig.shared_inner_dim must be >= 0, got {self.shared_inner_dim}")
+        if self.shared_inner_dim and self.expert != "swiglu":
+            raise ValueError("DMoEConfig.shared_inner_dim: the shared expert is a GatedFeedforwardBlock and needs "
+                             f"expert='swiglu', got expert={self.expert!r}")
 
     @property
     def router_losses(self) -> bool:
@@ -155,6 +170,9 @@ class DMoEConfig:
         if self.expert == "swiglu" and (self.hidden % 128 or not 128 <= self.hidden <= K.LN_MAX_WIDTH or self.inner % 128):
             raise ValueError(f"expert='swiglu' on the GPU needs hidden a multiple of 128 in [128, {K.LN_MAX_WIDTH}] and "
                              f"an inner width that is a multiple of 128; got hidden={self.hidden}, inner={self.inner}")
+        if self.shared_inner_dim % 128:
+            raise ValueError("the shared expert on the GPU needs shared_inner_dim a multiple of 128; got "
+                             f"{self.shared_inner_dim}")
 
     @property
     def layout(self):
@@ -222,6 +240,13 @@ def refuse_expert_bias(cfg: DMoEConfig, arm: str):
                          "(FusedDMoE / DMoETrainer apply them)")
 
 
+def refuse_shared_expert(cfg: DMoEConfig, arm: str):
+    """an arm without a shared expert: refuse shared_inner_dim > 0 instead of silently dropping it"""
+    if cfg.shared_inner_dim > 0:
+        raise ValueError(f"{arm} has no shared expert; set shared_inner_dim to 0 (FusedDMoE / DMoETrainer / "
+                         "BaselineDMoE train it)")
+
+
 def expert_uid(cfg: DMoEConfig, e: int) -> str:
     """global expert index -> 'prefix.i0.i1...' (row-major over the grid; reference uid schema README.md:106)"""
     parts = []
@@ -271,6 +296,8 @@ class EngineContext:
         if self.S:  # parameters, bf16 mirror and gradients of the shards are peer-visible (replica pull / gradient reduce)
             rec = sum(int(math.prod(shape)) for shape in cfg.seg_shapes().values())
             need += cfg.num_layers * (self.G_tot * rec * 10 + (1 << 20))
+        if cfg.shared_inner_dim:   # DMoETrainer's flat gradient in the heap also holds the shared experts' gradients
+            need += cfg.num_layers * (H + 3 * H * cfg.shared_inner_dim + 256) * 4
         self.heap = SymmetricHeap(heap_bytes or need, group=group, device=self.device)
         self.flags, self.flags_off = self.heap.alloc((K.NUM_SLOTS, K.MAX_WORLD), torch.int32)
         self.cnt_all, self.cnt_all_off = self.heap.alloc((K.MAX_WORLD, self.E), torch.int32)
@@ -328,6 +355,18 @@ class EngineContext:
         # the expert's backward temporaries (FeedforwardBlock: da, dh; GatedFeedforwardBlock: da, dh = [dg | du], dn)
         for name, width in cfg.layout.buffers(H, cfg.inner)["scratch"].items():
             setattr(self, name, torch.empty(self.max_rows, width, **bf))
+        if cfg.shared_inner_dim:
+            # the shared expert's backward temporaries (shared by all layers; zero, so that padding rows start at zero) and
+            # its one-group tables: row t of shared_go is the group_off [0, 128 (t + 1)] of a batch padded to 128 (t + 1)
+            # rows, its column 1 the group_rows; shared_tg is the tile_group of the 128-row GEMMs (every tile in group 0)
+            Is, R = cfg.shared_inner_dim, -(-cfg.tokens_per_rank // SHARED_PAD) * SHARED_PAD
+            self.shared_da = torch.zeros(R, Is, **bf)
+            self.shared_dh = torch.zeros(R, 2 * Is, **bf)
+            self.shared_dn = torch.zeros(R, H, **bf)
+            self.shared_dx = torch.zeros(R, H, **bf)
+            tiles = torch.arange(1, R // SHARED_PAD + 1, dtype=torch.int32) * SHARED_PAD
+            self.shared_go = torch.stack([torch.zeros_like(tiles), tiles], 1).to(self.device)
+            self.shared_tg = torch.zeros(R // SHARED_PAD, dtype=torch.int32, device=self.device)
         self.heap.barrier()
 
     EPOCH_STRIDE = 64   # epochs a step may consume; the device-side base advances by this much per begin_step()
@@ -680,6 +719,17 @@ class LayerWorkspace:
             self.router_z = torch.zeros(cfg.tokens_per_rank, **f32)
             self.router_F = torch.zeros(cfg.tokens_per_rank, **f32)
             self.router_loss = torch.zeros(2, **f32)
+        if cfg.shared_inner_dim:
+            # the shared expert's activations on this rank's rows, padded to SHARED_PAD rows (zero, so that the padding rows
+            # start at zero), its output ys (the forward combine's addend), the padded copy of the output gradient and the
+            # bf16 GEMM operands cast from the fp32 parameters at every forward
+            Is, Rs = cfg.shared_inner_dim, -(-cfg.tokens_per_rank // SHARED_PAD) * SHARED_PAD
+            self.shared_n, self.shared_h = torch.zeros(Rs, H, **bf), torch.zeros(Rs, 2 * Is, **bf)
+            self.shared_a, self.shared_y = torch.zeros(Rs, Is, **bf), torch.zeros(Rs, H, **bf)
+            self.shared_gy = torch.zeros(Rs, H, **bf)
+            self.shared_rstd = torch.zeros(Rs, **f32)
+            self.shared_w13 = torch.zeros(1, 2 * Is, H, **bf)
+            self.shared_w2 = torch.zeros(1, H, Is, **bf)
         self.outstanding = False   # a training-mode forward whose backward has not run yet owns this workspace
         # small path with optimizer overlap: the fused wgrad+AMSGrad kernels of layer L read dY buffers while the main stream is
         # already in the backward of layer L-1, so they must be per layer (a few MB each at this batch size)
@@ -710,16 +760,19 @@ class _FusedDMoEFunction(torch.autograd.Function):
         ctx.tracked = bool(x.requires_grad or logits.requires_grad)
         ws.outstanding = ctx.tracked
         ctx.router = layer.training and layer.router_on
-        if ctx.router:
-            ctx.save_for_backward(logits)
+        ctx.shared = layer.shared_inner > 0   # the shared expert's norm backward reads the layer input
+        if ctx.router or ctx.shared:
+            ctx.save_for_backward(*([logits] if ctx.router else []), *([x] if ctx.shared else []))
         return layer._forward_cuda(x, logits)
 
     @staticmethod
     def backward(ctx, grad_out):
         if not ctx.layer.ws.outstanding:
             raise RuntimeError("FusedDMoE: backward() without a pending forward (the workspace was released or reused)")
-        logits = ctx.saved_tensors[0] if ctx.router else None
-        dx, dlogits = ctx.layer._backward_cuda(grad_out.contiguous(), ctx.B, logits)
+        saved = ctx.saved_tensors
+        logits = saved[0] if ctx.router else None
+        x = saved[-1] if ctx.shared else None
+        dx, dlogits = ctx.layer._backward_cuda(grad_out.contiguous(), ctx.B, logits, x)
         ctx.layer.ws.outstanding = False
         ec = ctx.layer.ctx
         if ec._opt_pending and not ec.defer_join:
@@ -748,7 +801,9 @@ class FusedDMoE(nn.Module):
     Decentralized-MoE layer over the experts of the whole box.  Trainer-side parameters: ``proj`` (product-key gating,
     identical to ``GatingFunction.proj``: Linear(in_features, sum(grid_size))).  Expert parameters live in
     ``self.shard`` and are updated by the layer itself during backward (they are NOT nn.Parameters, mirroring
-    ``get_non_expert_params`` of the reference emulator).
+    ``get_non_expert_params`` of the reference emulator).  With ``cfg.shared_inner_dim`` the layer also owns a shared
+    expert (DESIGN.md §9c): the trainer-side parameters ``shared_g`` [H], ``shared_w13`` [2 I_s, H] and ``shared_w2``
+    [H, I_s] of one GatedFeedforwardBlock, whose ``module(x) - x`` is added to every token's combined output.
     """
 
     def __init__(self, cfg: DMoEConfig, ctx: Optional[EngineContext] = None, layer_index: int = 0, device=None):
@@ -794,6 +849,40 @@ class FusedDMoE(nn.Module):
         self.expert_bias_rate = float(cfg.expert_bias_update_rate)
         self.register_buffer("expert_bias", torch.zeros(cfg.num_experts, dtype=torch.float32, device=dev)
                              if self.expert_bias_rate > 0.0 else None)
+        # shared expert (cfg.shared_inner_dim, read here once): initialised like GatedFeedforwardBlock(hidden, I_s), drawn
+        # from the global RNG like proj (DMoETrainer seeds it, so every rank starts identical), kept as the segments of
+        # GATED_LAYOUT so that [W1; W3] is one GEMM operand and one contiguous gradient
+        self.shared_inner = int(cfg.shared_inner_dim)
+        if self.shared_inner:
+            block = GatedFeedforwardBlock(cfg.hidden, self.shared_inner, eps=GATED_EPS)
+            seg = GATED_LAYOUT.segment_state({k: v.detach() for k, v in block.state_dict().items()})
+            self.shared_g = nn.Parameter(seg["g"].clone())
+            self.shared_w13 = nn.Parameter(seg["w13"].clone())
+            self.shared_w2 = nn.Parameter(seg["w2"].clone())
+
+    # ------------------------------------------------------------------ shared expert (DESIGN.md §9c)
+    def shared_expert_parameters(self) -> List[nn.Parameter]:
+        """the shared expert's parameters in segment order (g, w13, w2); [] without a shared expert"""
+        return [self.shared_g, self.shared_w13, self.shared_w2] if self.shared_inner else []
+
+    def _shared_segments(self) -> Dict[str, torch.Tensor]:
+        if not self.shared_inner:
+            raise ValueError("this FusedDMoE has no shared expert (DMoEConfig.shared_inner_dim = 0)")
+        return dict(zip(GATED_LAYOUT.names, self.shared_expert_parameters()))
+
+    def shared_expert_state_dict(self, prefix: str = "") -> Dict[str, torch.Tensor]:
+        """the shared expert as a ``GatedFeedforwardBlock(hidden, shared_inner_dim)`` state_dict (``norm.weight``,
+        ``w1.weight``, ``w2.weight``, ``w3.weight``): that module's ``module(x) - x`` is the layer's shared term"""
+        return {prefix + k: t.detach().clone().cpu() for k, t in GATED_LAYOUT.module_state(self._shared_segments()).items()}
+
+    def load_shared_expert_state_dict(self, state: Dict[str, torch.Tensor], prefix: str = ""):
+        """load a ``GatedFeedforwardBlock`` state_dict into the shared expert (in place: a captured graph reads it)"""
+        segs = self._shared_segments()
+        with torch.no_grad():
+            for n, t in GATED_LAYOUT.segment_state(state, prefix).items():
+                if tuple(t.shape) != tuple(segs[n].shape):
+                    raise ValueError(f"shared expert: {n} has shape {tuple(t.shape)}, this layer {tuple(segs[n].shape)}")
+                segs[n].copy_(t)
 
     # ------------------------------------------------------------------ public forward
     def forward(self, x):
@@ -867,6 +956,10 @@ class FusedDMoE(nn.Module):
                        c.E_loc, c.max_rows, ws.group_off, ws.group_rows, c.done_counter, c.status, align=c.align,
                        route_owner=ws.route_owner, num_groups=c.G_tot)
         c.timer.mark("dispatch(layout+pull+scatter)")
+        # the shared expert needs only this rank's rows: at world > 1 it runs while the peers' rows are in flight
+        ys = self._shared_expert_fwd(x) if self.shared_inner else None
+        if ys is not None:
+            c.timer.mark("shared_expert_fwd")
         # ---- expert FFN on the rows this rank received (grouped by expert).  Receive-side fusion: the first GEMM's TMA
         # producer polls the peers' dispatch flags itself (no separate wait kernel)
         tg = ws.tile_group
@@ -892,9 +985,73 @@ class FusedDMoE(nn.Module):
         c.timer.mark("expert_ffn_fwd")
         y = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=x.device)
         K.combine_rows(ws.yo_off, idx, pair_row, w, y, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_OUTPUT, epoch=epoch,
-                       signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner)
+                       signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner, addend=ys)
         c.timer.mark("combine")
         return y
+
+    def _shared_tables(self, B):
+        """(rows padded to SHARED_PAD, group_off, group_rows, tile_group) of the shared expert's one-group GEMMs on B rows"""
+        c = self.ctx
+        Bp = -(-B // SHARED_PAD) * SHARED_PAD
+        go = c.shared_go[Bp // SHARED_PAD - 1]
+        return Bp, go, go[1:], c.shared_tg
+
+    def _shared_expert_fwd(self, x):
+        """the shared expert on this rank's B rows: n = RMSNorm(x), h = n [W1; W3]^T, a = silu(hg) * hu, ys = a W2^T (no
+        residual), into rows padded to SHARED_PAD.  The padding rows of n are zeroed here (an earlier, larger batch may have
+        written them), so those of h, a and ys are zero as well and add nothing to the weight gradients.  The bf16
+        operands are cast from the fp32 parameters at every forward, so any optimizer that steps them is seen.  Returns
+        ys[:B], the combine's addend."""
+        ws = self.ws
+        B = x.shape[0]
+        Bp, go, gr, tg = self._shared_tables(B)
+        K.cast_bf16(self.shared_w13.detach(), ws.shared_w13)
+        K.cast_bf16(self.shared_w2.detach(), ws.shared_w2)
+        n, h, a, ys = ws.shared_n[:Bp], ws.shared_h[:Bp], ws.shared_a[:Bp], ws.shared_y[:Bp]
+        K.rms_norm_fwd(x, self.shared_g.detach(), GATED_EPS, out=n[:B], rstd=ws.shared_rstd[:B])
+        if Bp > B:
+            n[B:].zero_()
+        if B < SHARED_SWAPAB_ROWS:   # weight streaming: one group of Bp tokens on MMA-N
+            K.swapab_linear(n, ws.shared_w13, go, gr, out=h)
+            K.swiglu_fwd(h, out=a)
+            K.swapab_linear(a, ws.shared_w2, go, gr, out=ys)
+        else:
+            gemm.grouped_linear(n, ws.shared_w13, tile_group=tg, out=h)
+            K.swiglu_fwd(h, out=a)
+            gemm.grouped_linear(a, ws.shared_w2, tile_group=tg, out=ys)
+        return ys[:B]
+
+    def _shared_expert_bwd(self, gy, x):
+        """backward of ``_shared_expert_fwd`` on the main stream: the dgrads, SwiGLU and RMSNorm backward give dxs (the
+        backward combine's addend), dgamma is added into ``shared_g.grad`` and the weight gradients into
+        ``shared_w13.grad`` / ``shared_w2.grad`` (the flat trainer gradient under DMoETrainer, so micro-batches add up).
+        The copy of gy is zero-padded, so the padding rows add nothing.  Returns dxs [B, H]."""
+        c, ws = self.ctx, self.ws
+        B = gy.shape[0]
+        Bp, go, gr, tg = self._shared_tables(B)
+        for p in self.shared_expert_parameters():   # layer-level callers: zero gradients on first use
+            if p.grad is None:
+                p.grad = torch.zeros_like(p)
+        gys = ws.shared_gy[:Bp]
+        gys[:B].copy_(gy)
+        if Bp > B:
+            gys[B:].zero_()
+        da, dh, dn, dxs = c.shared_da[:Bp], c.shared_dh[:Bp], c.shared_dn[:Bp], c.shared_dx[:B]
+        h, n, a = ws.shared_h[:Bp], ws.shared_n[:Bp], ws.shared_a[:Bp]
+        lim = c.chain_ctas   # the previous layer's fused wgrad + AMSGrad may still stream on the optimizer stream
+        if B < SHARED_SWAPAB_ROWS:
+            K.swapab_linear(gys, ws.shared_w2, go, gr, out=da, w_is_kn=True, max_ctas=lim)
+            K.swiglu_bwd(da, h, out=dh)
+            K.swapab_linear(dh, ws.shared_w13, go, gr, out=dn, w_is_kn=True, max_ctas=lim)
+        else:
+            gemm.grouped_linear(gys, ws.shared_w2, tile_group=tg, w_is_kn=True, out=da, max_ctas=lim)
+            K.swiglu_bwd(da, h, out=dh)
+            gemm.grouped_linear(dh, ws.shared_w13, tile_group=tg, w_is_kn=True, out=dn, max_ctas=lim)
+        K.rms_norm_bwd(dn[:B], x, ws.shared_rstd[:B], self.shared_g.detach(), dx=dxs, dgamma=self.shared_g.grad)
+        Is, H = self.shared_inner, self.cfg.hidden
+        gemm.grouped_wgrad(dh, n, go, 1, out=self.shared_w13.grad.view(1, 2 * Is, H), accumulate=True, max_ctas=lim)
+        gemm.grouped_wgrad(gys, a, go, 1, out=self.shared_w2.grad.view(1, H, Is), accumulate=True, max_ctas=lim)
+        return dxs
 
     def _expert_gated_fwd(self, wait, epoch):
         """GatedFeedforwardBlock on the received rows: n = RMSNorm(xd) with each expert's gamma, h = [hg | hu] = n [W1; W3]^T
@@ -935,8 +1092,9 @@ class FusedDMoE(nn.Module):
         K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, quant=ws.aq)
         fp8.grouped_linear_fp8(ws.aq, w8["w3"], tile_group=tg, bias=sh.raw_views["b3"], residual=ws.xd, out=ws.yo)
 
-    def _backward_cuda(self, gy, B, logits=None):
-        """:param logits: the gate logits of the forward when it computed router losses (their gradient is added here)"""
+    def _backward_cuda(self, gy, B, logits=None, x=None):
+        """:param logits: the gate logits of the forward when it computed router losses (their gradient is added here)
+        :param x: the layer input of the forward, when the layer has a shared expert"""
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         k = cfg.k
         P = B * k
@@ -954,6 +1112,8 @@ class FusedDMoE(nn.Module):
                        route_owner=ws.route_owner, num_groups=c.G_tot)
         if c.S:  # atomically accumulated (bias / norm) partial gradients of my shadow slots start from zero
             K.zero_slots(sh.g, sh.seg_sizes, c.G_tot, c.E_loc, c.S, sh.layout.small_mask)
+        # the shared expert's backward needs only this rank's gradient: at world > 1 it runs while the peers' are in flight
+        dxs = self._shared_expert_bwd(gy, x) if self.shared_inner else None
         if c.world > 1:  # the first consumers of the pushed gradients are the colsum / wgrad kernels
             K.signal_wait(c.flags_off, K.SLOT_GRAD, epoch, c.status, signal=False, wait=True)
         c.timer.mark("bwd_gate+dispatch_grad")
@@ -964,7 +1124,8 @@ class FusedDMoE(nn.Module):
             c.timer.mark("expert_ffn_bwd(dgrad+ln+fused wgrad/AMSGrad)")
             dx = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=gy.device)
             K.combine_rows(c.dxd_off, idx, pair_row, None, dx, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_DINPUT,
-                           epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner)
+                           epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner,
+                           addend=dxs)
             c.timer.mark("bwd_combine")
             return dx, dlogits
         if cfg.expert == "swiglu":
@@ -998,7 +1159,8 @@ class FusedDMoE(nn.Module):
         c.timer.mark("expert_adam")
         dx = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=gy.device)
         K.combine_rows(c.dxd_off, idx, pair_row, None, dx, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_DINPUT,
-                       epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner)
+                       epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner,
+                       addend=dxs)
         c.timer.mark("bwd_combine")
         return dx, dlogits
 
@@ -1166,6 +1328,11 @@ class FusedDMoE(nn.Module):
             tok, slot = torch.nonzero(idx == e, as_tuple=True)
             ye = self._expert_ref(p, rnd(xf[tok]), rnd)
             out = out.index_put((tok,), ye * weights[tok, slot].unsqueeze(-1), accumulate=True)
+        if self.shared_inner:   # the shared expert: weight 1, no residual; autograd reaches its parameters
+            p = self._shared_segments()
+            if emulate_bf16:
+                p = {n: (rnd(v) if n.startswith("w") else v) for n, v in p.items()}
+            out = out + rnd(self._gated_branch(p, rnd(xf), rnd))
         if self.training and self.router_on:
             counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
             l_aux, l_z = K.router_loss_ref(logits, self.grid_size, counts, alive=alive)
@@ -1176,14 +1343,19 @@ class FusedDMoE(nn.Module):
                 out = _AddRouterLoss.apply(out, aux)
         return out.to(x.dtype)
 
+    def _gated_branch(self, p, xe, rnd):
+        """w2(silu(w1 n) * w3 n), n = RMSNorm(x), of GatedFeedforwardBlock segments ``p`` in fp32, without the residual
+        and without rounding the result"""
+        n = rnd(F.rms_norm(xe, (self.cfg.hidden,), p["g"], GATED_EPS))
+        hg, hu = rnd(F.linear(n, p["w13"])).chunk(2, dim=-1)
+        a = rnd(F.silu(hg) * hu)
+        return F.linear(a, p["w2"])
+
     def _expert_ref(self, p, xe, rnd):
         """one expert on its rows in fp32; ``rnd`` rounds where the GPU path stores bf16"""
         cfg = self.cfg
         if cfg.expert == "swiglu":   # GatedFeedforwardBlock: x + w2(silu(w1 n) * w3 n), n = RMSNorm(x)
-            n = rnd(F.rms_norm(xe, (cfg.hidden,), p["g"], GATED_EPS))
-            hg, hu = rnd(F.linear(n, p["w13"])).chunk(2, dim=-1)
-            a = rnd(F.silu(hg) * hu)
-            return rnd(F.linear(a, p["w2"]) + xe)
+            return rnd(self._gated_branch(p, xe, rnd) + xe)
         h1 = rnd(F.linear(xe, p["w1"], p["b1"]))
         a1 = rnd(F.relu(F.layer_norm(h1, (cfg.inner,), p["g1"], p["be1"])))
         h2 = rnd(F.linear(a1, p["w2"], p["b2"]))

@@ -119,10 +119,21 @@ class DMoETrainer:
         self.cfg.lr = lr
 
     # ------------------------------------------------------------------ trainer-side flat parameters
+    #: the shared experts' tensors start at a multiple of this many floats of the flat buffers: their GEMM operands are
+    #: cast and their gradients accumulated by vector accesses
+    SHARED_ALIGN = 64
+
     def _flatten_trainer_params(self):
         params = [p for p in self.model.parameters() if p.requires_grad]  # a frozen (emulator-style) gate stays out
+        aligned = {id(p) for block in self.model.blocks for p in block.shared_expert_parameters()}
+        offsets, off = [], 0
+        for p in params:   # without a shared expert no tensor is aligned: the layout of earlier checkpoints
+            if id(p) in aligned:
+                off = -(-off // self.SHARED_ALIGN) * self.SHARED_ALIGN
+            offsets.append(off)
+            off += p.numel()
         n = sum(p.numel() for p in params)
-        n_pad = (n + 3) // 4 * 4
+        n_pad = (off + 3) // 4 * 4
         dev = self.device
         self.flat_p = torch.zeros(n_pad, device=dev)
         if self.cuda:
@@ -132,13 +143,11 @@ class DMoETrainer:
             self.flat_g, self.flat_g_off = torch.zeros(n_pad), -1
         self.flat_m, self.flat_v = torch.zeros(n_pad, device=dev), torch.zeros(n_pad, device=dev)
         self.flat_vmax = torch.zeros(n_pad, device=dev)
-        off = 0
-        for p in params:
+        for p, off in zip(params, offsets):
             sl = slice(off, off + p.numel())
             self.flat_p[sl].copy_(p.detach().reshape(-1))
             p.data = self.flat_p[sl].view_as(p)
             p.grad = self.flat_g[sl].view_as(p)
-            off += p.numel()
         self.num_trainer_params = n
         self._n_pad = n_pad
         d = int(self.cfg.trainer_staleness)
@@ -459,6 +468,15 @@ class DMoETrainer:
         from .engine import expert_uid
         own = self.model.state_dict()
         saved = state["trainer"]["model"]
+        shared = lambda sd: {k: tuple(v.shape) for k, v in sd.items() if k.rsplit(".", 1)[-1].startswith("shared_")}
+        own_shared, saved_shared = shared(own), shared(saved)
+        if bool(own_shared) != bool(saved_shared):
+            raise ValueError(f"checkpoint {'has' if saved_shared else 'has no'} shared expert, this trainer "
+                             f"{'has' if own_shared else 'has none'} (DMoEConfig.shared_inner_dim = "
+                             f"{self.cfg.shared_inner_dim}); build the trainer with the checkpoint's shared_inner_dim")
+        if own_shared != saved_shared:
+            raise ValueError(f"checkpoint's shared expert has other widths than this trainer's (shared_inner_dim = "
+                             f"{self.cfg.shared_inner_dim}): {saved_shared} against {own_shared}")
         biases = [k for k in own if k.endswith(".expert_bias")]
         if any(k.endswith(".expert_bias") and k not in own for k in saved):
             # dropping the saved biases would silently change which experts the gates select

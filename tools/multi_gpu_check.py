@@ -32,10 +32,14 @@ def main():
     router = dict(router_aux_loss_coef=0.01, router_z_loss_coef=0.001) if "--router-loss" in sys.argv else {}
     # auxiliary-loss-free balancing: every rank moves its copy of the expert biases from the same box-wide count table
     bias = dict(expert_bias_update_rate=0.01) if "--expert-bias" in sys.argv else {}
+    # a shared expert (trainer-side, replicated): its gradients summed over ranks against the whole-batch oracle, then
+    # N trainer steps after which its parameters must hold the same bits on every rank
+    shared = dict(shared_inner_dim=512) if "--shared-expert" in sys.argv else {}
+    swiglu = swiglu or bool(shared)
     mat, vec = ("w13", "g") if swiglu else ("w1", "b2")
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=B, capacity_factor=float(max(4, world)),
                        shadow_experts=4, shadow_tol=0.0 if force_shadow else 1.1, shadow_min_rows=1 if force_shadow else 64,
-                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router, **bias)
+                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router, **bias, **shared)
     ctx = E.EngineContext(cfg)
     torch.manual_seed(0)  # identical gate on every rank (DMoETrainer does the same)
     layer = E.FusedDMoE(cfg, ctx).cuda()
@@ -61,6 +65,9 @@ def main():
     dist.all_gather(dxs, x.grad.contiguous())
     gw = layer.proj.weight.grad.clone()
     dist.all_reduce(gw)
+    shared_grads = [p.grad.clone() for p in layer.shared_expert_parameters()]
+    for g in shared_grads:
+        dist.all_reduce(g)
     if router:   # the mean over ranks of the per-rank losses is the box-wide value
         rl = layer.router_loss.clone()
         dist.all_reduce(rl)
@@ -99,6 +106,23 @@ def main():
         biases = [torch.empty_like(layer.expert_bias) for _ in range(world)]
         dist.all_gather(biases, layer.expert_bias)
         bias_ok = bias_ok and all(torch.equal(b, biases[0]) for b in biases)
+    shared_ok = True
+    if shared:
+        from lah_b200.parallel.trainer import DMoETrainer
+        tcfg = E.DMoEConfig(hidden=512, grid_size=(16,), k=4, num_layers=2, tokens_per_rank=B, gate_mode="emulator",
+                            expert="swiglu", expert_path="small" if small else "big", **shared)
+        ctx.close()
+        trainer = DMoETrainer(tcfg)
+        gen_t = torch.Generator().manual_seed(200 + rank)
+        for _ in range(5):
+            trainer.train_step(torch.randn(B, tcfg.in_features, generator=gen_t).pin_memory(),
+                               torch.randint(0, 10, (B,), generator=gen_t).pin_memory())
+        trainer.ctx.check_status()
+        flat = trainer.flat_p.clone()
+        flats = [torch.empty_like(flat) for _ in range(world)]
+        dist.all_gather(flats, flat)
+        shared_ok = all(torch.equal(f, flats[0]) for f in flats)
+        trainer.close()
     ok = True
     if rank == 0:
         # single-GPU reference in the same process: a fresh world-1 context is impossible inside an initialised group,
@@ -108,6 +132,8 @@ def main():
         ref_cfg = E.DMoEConfig(**{**cfg.__dict__, **{k: v * world for k, v in router.items()}}) if router else cfg
         ref = E.FusedDMoE(ref_cfg, None, device=torch.device("cuda")).cuda()
         ref.proj.load_state_dict(layer.proj.state_dict())
+        if shared:
+            ref.load_shared_expert_state_dict(layer.shared_expert_state_dict())
         ref.train()
         xr = x_all.cuda().float().requires_grad_(True)
         yr = ref(xr)
@@ -117,6 +143,9 @@ def main():
                     w1_mean_abs=(torch.cat(w1s) - ref.shard.views[mat]).abs().mean().item(),
                     b2_max_abs=(torch.cat(b2s) - ref.shard.views[vec]).abs().max().item(),
                     steps=bool((torch.cat(steps).cpu() == ref.shard.step.cpu()).all()))
+        if shared:
+            errs["shared_grad"] = max(rel(a, b.grad) for a, b in zip(shared_grads, ref.shared_expert_parameters()))
+            errs["shared_params_bit_identical_after_5_steps"] = shared_ok
         if router:
             errs["router_loss"] = rel(rl, ref.router_loss)
             xa = x_all.cuda()
@@ -128,6 +157,7 @@ def main():
         ok = errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2 and errs["w1_mean_abs"] < 1e-4 and errs["b2_max_abs"] < 2.5e-3 and errs["steps"]
         ok = ok and (shadowed > 0 or not force_shadow) and plan_ok and errs.get("router_loss", 0.0) < 1e-4
         ok = ok and errs.get("router_grad_max_err", 0.0) < 1e-4 and bias_ok
+        ok = ok and errs.get("shared_grad", 0.0) < 8e-2 and shared_ok
         if bias:
             errs["expert_bias_bit_identical_and_equal_to_oracle"] = bias_ok
         print("multi_gpu_check", dict(path="small" if small else "big", expert=cfg.expert, router_loss=bool(router), force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
