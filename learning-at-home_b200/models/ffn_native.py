@@ -7,7 +7,8 @@ then emits the next GEMM's FP8 operand directly and no bf16 activation is writte
 import torch
 import torch.nn as nn
 
-from ..ops import fp8, gemm, kernels as K
+from ..ops import fp8
+from ..ops.expert_blocks import RowPlan, ffn_forward, ffn_forward_fp8
 from .layers import FeedforwardBlock
 
 
@@ -22,13 +23,13 @@ class NativeFFNLayer(nn.Module):
         def f(t):
             return t.detach().to(device=device, dtype=torch.float32).unsqueeze(0).contiguous()
 
-        self.b = [f(m.bias) for m in (lin1, lin2, lin3)]
-        self.ln = [(f(m.weight), f(m.bias)) for m in (ln1, ln2)]
-        ws = [m.weight.detach().to(device=device) for m in (lin1, lin2, lin3)]
+        self.p = dict(b1=f(lin1.bias), b2=f(lin2.bias), b3=f(lin3.bias), g1=f(ln1.weight), be1=f(ln1.bias),
+                      g2=f(ln2.weight), be2=f(ln2.bias))
+        ws = {n: m.weight.detach().to(device=device) for n, m in (("w1", lin1), ("w2", lin2), ("w3", lin3))}
         if dtype == "fp8":
-            self.w = [fp8.quantize(w.float().contiguous(), tile_rows=fp8.WEIGHT_TILE, groups=1) for w in ws]
+            self.w = {n: fp8.quantize(w.float().contiguous(), tile_rows=fp8.WEIGHT_TILE, groups=1) for n, w in ws.items()}
         else:
-            self.w = [w.to(torch.bfloat16).unsqueeze(0).contiguous() for w in ws]
+            self.w = {n: w.to(torch.bfloat16).unsqueeze(0).contiguous() for n, w in ws.items()}
         self._ws = {}
 
     def _workspace(self, rows, device):
@@ -53,19 +54,10 @@ class NativeFFNLayer(nn.Module):
         ws = self._workspace(rows, x.device)
         if out is None:
             out = torch.empty_like(x)
-        (g1, be1), (g2, be2) = self.ln
-        if self.dtype == "fp8":
-            fp8.quantize(x, out=ws["xq"])
-            fp8.grouped_linear_fp8(ws["xq"], self.w[0], bias=self.b[0], out=ws["h"])
-            K.ln_relu_fwd(ws["h"], g1, be1, None, out=None, mean=None, rstd=None, quant=ws["aq"])
-            fp8.grouped_linear_fp8(ws["aq"], self.w[1], bias=self.b[1], out=ws["h"])
-            K.ln_relu_fwd(ws["h"], g2, be2, None, out=None, mean=None, rstd=None, quant=ws["aq"])
-            fp8.grouped_linear_fp8(ws["aq"], self.w[2], bias=self.b[2], residual=x, out=out)
+        plan = RowPlan()   # 128-row tiles of one group
+        if self.dtype == "fp8":   # no bf16 activation or LayerNorm statistics: nothing reads them
+            ffn_forward_fp8(plan, self.w, self.p, x, ws["xq"], ws["aq"], (ws["h"], None, ws["h"], None), (None,) * 4, out)
         else:
-            mean = rstd = ws.setdefault("stat", torch.empty(rows, device=x.device))
-            gemm.grouped_linear(x, self.w[0], bias=self.b[0], out=ws["h"])
-            K.ln_relu_fwd(ws["h"], g1, be1, None, out=ws["a"], mean=mean, rstd=rstd)
-            gemm.grouped_linear(ws["a"], self.w[1], bias=self.b[1], out=ws["h"])
-            K.ln_relu_fwd(ws["h"], g2, be2, None, out=ws["a"], mean=mean, rstd=rstd)
-            gemm.grouped_linear(ws["a"], self.w[2], bias=self.b[2], residual=x, out=out)
+            stat = ws.setdefault("stat", torch.empty(rows, device=x.device))
+            ffn_forward(plan, self.w, self.p, x, (ws["h"], ws["a"], ws["h"], ws["a"]), (stat,) * 4, out)
         return out

@@ -28,6 +28,8 @@ import torch.nn.functional as F
 from ..models.layers import FFN_SEG_KEYS as REF_KEYS, FFN_SEG_NAMES as SEG_NAMES, FFN_SMALL_SEG_MASK as SMALL_SEG_MASK
 from ..models.layers import EXPERT_LAYOUTS, GATED_LAYOUT, GatedFeedforwardBlock, gated_inner_dim
 from ..ops import fp8, gemm, kernels as K, native
+from ..ops.expert_blocks import (RowPlan, ffn_backward, ffn_forward, ffn_forward_fp8, swiglu_mlp_backward,
+                                 swiglu_mlp_forward)
 
 #: eps of the gated expert's RMSNorm (GatedFeedforwardBlock's default)
 GATED_EPS = 1e-6
@@ -962,26 +964,28 @@ class FusedDMoE(nn.Module):
             c.timer.mark("shared_expert_fwd")
         # ---- expert FFN on the rows this rank received (grouped by expert).  Receive-side fusion: the first GEMM's TMA
         # producer polls the peers' dispatch flags itself (no separate wait kernel)
-        tg = ws.tile_group
         wait = (c.flags[K.SLOT_DISPATCH, :c.world], epoch, c.status) if c.world > 1 else None
+        plan = self._expert_plan()
         if cfg.expert == "swiglu":
-            self._expert_gated_fwd(wait, epoch)
-        elif c.small:
-            # weight-streaming regime: swap-AB tiles (weights on MMA-M, the group's 16..128 tokens on MMA-N), groups of 16 rows
-            go, gr_, T = ws.group_off, ws.group_rows, c.tile_rows
-            K.swapab_linear(ws.xd, sh.bf16["w1"], go, gr_, out=ws.h1, bias=sh.raw_views["b1"], wait=wait)
-            K.ln_relu_fwd(ws.h1, sh.raw_views["g1"], sh.raw_views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1, tile_rows=T)
-            K.swapab_linear(ws.a1, sh.bf16["w2"], go, gr_, out=ws.h2, bias=sh.raw_views["b2"])
-            K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, tile_rows=T)
-            K.swapab_linear(ws.a2, sh.bf16["w3"], go, gr_, out=ws.yo, bias=sh.raw_views["b3"], residual=ws.xd)
-        elif cfg.expert_dtype == "fp8":
-            self._expert_ffn_fp8(wait, epoch)
+            # the rows of unused tiles (group -1) of n, h and a hold stale values that no result reads: the big path's
+            # GEMMs skip -1 tiles; the small path's power-of-two TMA boxes may reach past a group's padded rows, but those
+            # GEMM columns are not stored, the wgrads read only the groups' rows and SwiGLU maps rows elementwise
+            if wait is not None:  # the norm, not a GEMM, is the first consumer of the rows pushed by the peers
+                K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
+            K.rms_norm_fwd(ws.xd, sh.raw_views["g"], GATED_EPS, out=ws.n, rstd=ws.rstd, tile_group=plan.tile_group,
+                           tile_rows=plan.tile_rows)
+            swiglu_mlp_forward(plan, sh.bf16["w13"], sh.bf16["w2"], ws.n, ws.h, ws.a, ws.yo, residual=ws.xd)
+        elif c.small or cfg.expert_dtype != "fp8":
+            ffn_forward(plan, sh.bf16, sh.raw_views, ws.xd, (ws.h1, ws.a1, ws.h2, ws.a2),
+                        (ws.mean1, ws.rstd1, ws.mean2, ws.rstd2), ws.yo, wait=wait)
         else:
-            gemm.grouped_linear(ws.xd, sh.bf16["w1"], tile_group=tg, bias=sh.raw_views["b1"], out=ws.h1, wait=wait)
-            K.ln_relu_fwd(ws.h1, sh.raw_views["g1"], sh.raw_views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1)
-            gemm.grouped_linear(ws.a1, sh.bf16["w2"], tile_group=tg, bias=sh.raw_views["b2"], out=ws.h2)
-            K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2)
-            gemm.grouped_linear(ws.a2, sh.bf16["w3"], tile_group=tg, bias=sh.raw_views["b3"], residual=ws.xd, out=ws.yo)
+            # forward GEMMs on block-scaled FP8 tensor cores; LayerNorm emits the next GEMM's MXFP8 operand directly (and
+            # the bf16 copy the bf16 wgrad needs)
+            assert c.align == 256, "the FP8 path needs 256-row expert groups (hidden and 4*hidden multiples of 256)"
+            if wait is not None:  # the quantiser is the first consumer of the rows pushed by the peers
+                K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
+            ffn_forward_fp8(plan, sh.fp8_weights(), sh.raw_views, ws.xd, ws.xq, ws.aq, (ws.h1, ws.a1, ws.h2, ws.a2),
+                            (ws.mean1, ws.rstd1, ws.mean2, ws.rstd2), ws.yo)
         c.timer.mark("expert_ffn_fwd")
         y = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=x.device)
         K.combine_rows(ws.yo_off, idx, pair_row, w, y, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_OUTPUT, epoch=epoch,
@@ -989,12 +993,20 @@ class FusedDMoE(nn.Module):
         c.timer.mark("combine")
         return y
 
-    def _shared_tables(self, B):
-        """(rows padded to SHARED_PAD, group_off, group_rows, tile_group) of the shared expert's one-group GEMMs on B rows"""
+    def _expert_plan(self):
+        """swap-AB groups of 16 rows on the small path (backward GEMMs on ``chain_ctas``), 128-row tiles on the big one"""
+        c, ws = self.ctx, self.ws
+        if c.small:
+            return RowPlan(ws.group_off, ws.group_rows, ws.tile_group, c.tile_rows, max_ctas=c.chain_ctas)
+        return RowPlan(ws.group_off, None, ws.tile_group, c.tile_rows)
+
+    def _shared_plan(self, B):
+        """(B padded to SHARED_PAD, the shared expert's RowPlan): swap-AB below SHARED_SWAPAB_ROWS, 128-row tiles from
+        there; the backward GEMMs keep to ``chain_ctas`` (the last fused wgrad + AMSGrad may still run beside them)"""
         c = self.ctx
         Bp = -(-B // SHARED_PAD) * SHARED_PAD
         go = c.shared_go[Bp // SHARED_PAD - 1]
-        return Bp, go, go[1:], c.shared_tg
+        return Bp, RowPlan(go, go[1:] if B < SHARED_SWAPAB_ROWS else None, c.shared_tg, max_ctas=c.chain_ctas)
 
     def _shared_expert_fwd(self, x):
         """the shared expert on this rank's B rows: n = RMSNorm(x), h = n [W1; W3]^T, a = silu(hg) * hu, ys = a W2^T (no
@@ -1004,21 +1016,14 @@ class FusedDMoE(nn.Module):
         ys[:B], the combine's addend."""
         ws = self.ws
         B = x.shape[0]
-        Bp, go, gr, tg = self._shared_tables(B)
+        Bp, plan = self._shared_plan(B)
         K.cast_bf16(self.shared_w13.detach(), ws.shared_w13)
         K.cast_bf16(self.shared_w2.detach(), ws.shared_w2)
         n, h, a, ys = ws.shared_n[:Bp], ws.shared_h[:Bp], ws.shared_a[:Bp], ws.shared_y[:Bp]
         K.rms_norm_fwd(x, self.shared_g.detach(), GATED_EPS, out=n[:B], rstd=ws.shared_rstd[:B])
         if Bp > B:
             n[B:].zero_()
-        if B < SHARED_SWAPAB_ROWS:   # weight streaming: one group of Bp tokens on MMA-N
-            K.swapab_linear(n, ws.shared_w13, go, gr, out=h)
-            K.swiglu_fwd(h, out=a)
-            K.swapab_linear(a, ws.shared_w2, go, gr, out=ys)
-        else:
-            gemm.grouped_linear(n, ws.shared_w13, tile_group=tg, out=h)
-            K.swiglu_fwd(h, out=a)
-            gemm.grouped_linear(a, ws.shared_w2, tile_group=tg, out=ys)
+        swiglu_mlp_forward(plan, ws.shared_w13, ws.shared_w2, n, h, a, ys)
         return ys[:B]
 
     def _shared_expert_bwd(self, gy, x):
@@ -1028,7 +1033,7 @@ class FusedDMoE(nn.Module):
         The copy of gy is zero-padded, so the padding rows add nothing.  Returns dxs [B, H]."""
         c, ws = self.ctx, self.ws
         B = gy.shape[0]
-        Bp, go, gr, tg = self._shared_tables(B)
+        Bp, plan = self._shared_plan(B)
         for p in self.shared_expert_parameters():   # layer-level callers: zero gradients on first use
             if p.grad is None:
                 p.grad = torch.zeros_like(p)
@@ -1038,59 +1043,15 @@ class FusedDMoE(nn.Module):
             gys[B:].zero_()
         da, dh, dn, dxs = c.shared_da[:Bp], c.shared_dh[:Bp], c.shared_dn[:Bp], c.shared_dx[:B]
         h, n, a = ws.shared_h[:Bp], ws.shared_n[:Bp], ws.shared_a[:Bp]
-        lim = c.chain_ctas   # the previous layer's fused wgrad + AMSGrad may still stream on the optimizer stream
-        if B < SHARED_SWAPAB_ROWS:
-            K.swapab_linear(gys, ws.shared_w2, go, gr, out=da, w_is_kn=True, max_ctas=lim)
-            K.swiglu_bwd(da, h, out=dh)
-            K.swapab_linear(dh, ws.shared_w13, go, gr, out=dn, w_is_kn=True, max_ctas=lim)
-        else:
-            gemm.grouped_linear(gys, ws.shared_w2, tile_group=tg, w_is_kn=True, out=da, max_ctas=lim)
-            K.swiglu_bwd(da, h, out=dh)
-            gemm.grouped_linear(dh, ws.shared_w13, tile_group=tg, w_is_kn=True, out=dn, max_ctas=lim)
-        K.rms_norm_bwd(dn[:B], x, ws.shared_rstd[:B], self.shared_g.detach(), dx=dxs, dgamma=self.shared_g.grad)
         Is, H = self.shared_inner, self.cfg.hidden
-        gemm.grouped_wgrad(dh, n, go, 1, out=self.shared_w13.grad.view(1, 2 * Is, H), accumulate=True, max_ctas=lim)
-        gemm.grouped_wgrad(gys, a, go, 1, out=self.shared_w2.grad.view(1, H, Is), accumulate=True, max_ctas=lim)
+        grads = {"w13": self.shared_w13.grad.view(1, 2 * Is, H), "w2": self.shared_w2.grad.view(1, H, Is)}
+
+        def wgrad(name, dy, xin):
+            gemm.grouped_wgrad(dy, xin, plan.group_off, 1, out=grads[name], accumulate=True, max_ctas=plan.max_ctas)
+
+        swiglu_mlp_backward(plan, ws.shared_w13, ws.shared_w2, n, h, a, gys, da, dh, dn, wgrad)
+        K.rms_norm_bwd(dn[:B], x, ws.shared_rstd[:B], self.shared_g.detach(), dx=dxs, dgamma=self.shared_g.grad)
         return dxs
-
-    def _expert_gated_fwd(self, wait, epoch):
-        """GatedFeedforwardBlock on the received rows: n = RMSNorm(xd) with each expert's gamma, h = [hg | hu] = n [W1; W3]^T
-        (one GEMM), a = silu(hg) * hu, yo = a W2^T + xd.  The rows of unused tiles (group -1) of n, h and a are not
-        written by the norm and GEMMs and hold stale values; no result depends on them.  The big path's GEMMs skip -1
-        tiles.  The small path's GEMMs load a group's tokens in power-of-two TMA boxes (16..128 rows) from group_off, so
-        the box of a group's last block may extend past its padded rows (into the next group or a -1 tile): the extra
-        rows are separate GEMM columns whose outputs are not stored.  The wgrads read only the groups' rows, and SwiGLU
-        maps stale rows elementwise to rows that are equally unread."""
-        c, ws, sh = self.ctx, self.ws, self.shard
-        tg, T = ws.tile_group, c.tile_rows
-        if wait is not None:  # the norm, not a GEMM, is the first consumer of the rows pushed by the peers
-            K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
-        K.rms_norm_fwd(ws.xd, sh.raw_views["g"], GATED_EPS, out=ws.n, rstd=ws.rstd, tile_group=tg, tile_rows=T)
-        if c.small:
-            go, gr_ = ws.group_off, ws.group_rows
-            K.swapab_linear(ws.n, sh.bf16["w13"], go, gr_, out=ws.h)
-            K.swiglu_fwd(ws.h, out=ws.a)
-            K.swapab_linear(ws.a, sh.bf16["w2"], go, gr_, out=ws.yo, residual=ws.xd)
-        else:
-            gemm.grouped_linear(ws.n, sh.bf16["w13"], tile_group=tg, out=ws.h)
-            K.swiglu_fwd(ws.h, out=ws.a)
-            gemm.grouped_linear(ws.a, sh.bf16["w2"], tile_group=tg, residual=ws.xd, out=ws.yo)
-
-    def _expert_ffn_fp8(self, wait, epoch):
-        """forward GEMMs on block-scaled FP8 tensor cores; LayerNorm emits the next GEMM's MXFP8 operand directly (and the
-        bf16 copy the bf16 wgrad needs)"""
-        c, ws, sh = self.ctx, self.ws, self.shard
-        assert c.align == 256, "the FP8 path needs 256-row expert groups (hidden and 4*hidden multiples of 256)"
-        tg = ws.tile_group
-        if wait is not None:  # the quantiser is the first consumer of the rows pushed by the peers
-            K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
-        w8 = sh.fp8_weights()
-        fp8.quantize(ws.xd, tile_group=tg, out=ws.xq)
-        fp8.grouped_linear_fp8(ws.xq, w8["w1"], tile_group=tg, bias=sh.raw_views["b1"], out=ws.h1)
-        K.ln_relu_fwd(ws.h1, sh.raw_views["g1"], sh.raw_views["be1"], tg, out=ws.a1, mean=ws.mean1, rstd=ws.rstd1, quant=ws.aq)
-        fp8.grouped_linear_fp8(ws.aq, w8["w2"], tile_group=tg, bias=sh.raw_views["b2"], out=ws.h2)
-        K.ln_relu_fwd(ws.h2, sh.raw_views["g2"], sh.raw_views["be2"], tg, out=ws.a2, mean=ws.mean2, rstd=ws.rstd2, quant=ws.aq)
-        fp8.grouped_linear_fp8(ws.aq, w8["w3"], tile_group=tg, bias=sh.raw_views["b3"], residual=ws.xd, out=ws.yo)
 
     def _backward_cuda(self, gy, B, logits=None, x=None):
         """:param logits: the gate logits of the forward when it computed router losses (their gradient is added here)
@@ -1117,112 +1078,63 @@ class FusedDMoE(nn.Module):
         if c.world > 1:  # the first consumers of the pushed gradients are the colsum / wgrad kernels
             K.signal_wait(c.flags_off, K.SLOT_GRAD, epoch, c.status, signal=False, wait=True)
         c.timer.mark("bwd_gate+dispatch_grad")
-        tg, go, G = ws.tile_group, ws.group_off, c.G_tot
-        gr = sh.grads
+        plan, go, gr = self._expert_plan(), ws.group_off, sh.grads
         if c.small:
-            self._backward_small(epoch)
-            c.timer.mark("expert_ffn_bwd(dgrad+ln+fused wgrad/AMSGrad)")
-            dx = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=gy.device)
-            K.combine_rows(c.dxd_off, idx, pair_row, None, dx, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_DINPUT,
-                           epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner,
-                           addend=dxs)
-            c.timer.mark("bwd_combine")
-            return dx, dlogits
+            # dW never reaches HBM: register accumulator -> AMSGrad epilogue -> p / m / v / vmax updated in place.  With
+            # the overlap enabled the kernel goes to the optimizer stream, ordered after everything the main stream has
+            # launched so far (in particular the dgrad that still reads the OLD weights); its inputs live in per-layer
+            # buffers.  The optimizer step follows the whole backward in the reference (lib/runtime/expert_backend.py:85-90)
+            opt, E = c.adam_kwargs(), self.E_loc
+            main, side = torch.cuda.current_stream(c.device), c.opt_stream
+
+            def wgrad(name, dy, xin):
+                kw = dict(p=None, p_lo=sh.lo_views[name][:E], p_bf16=sh.bf16[name][:E]) if sh.split else \
+                    dict(p=sh.raw_views[name][:E], p_bf16=sh.bf16[name])
+                kw.update(m=sh.m_views[name][:E], v=sh.v_raw_views[name][:E],
+                          vmax=sh.vmax_views[name][:E] if cfg.amsgrad else None, step=sh.step, **opt)
+                if side is None:
+                    K.wgrad_adam(dy, xin, go, ws.group_rows, **kw)
+                    return
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    K.wgrad_adam(dy, xin, go, ws.group_rows, max_ctas=c.opt_ctas, **kw)
+                c._opt_pending = True
+
+            K.bump_steps(sh.step, ws.step_rows)
+        else:
+            def wgrad(name, dy, xin):
+                gemm.grouped_wgrad(dy, xin, go, c.G_tot, out=gr[name], accumulate=cfg.accumulate)
+
         if cfg.expert == "swiglu":
             # padding rows: scatter_rows zeroed them in xd and gyd, so da, dh and dn are zero there, and the RMSNorm
             # backward of a row with dn = 0 adds nothing to dgamma.  dgamma is added (+=) to the gradient buffer, which
-            # apply_expert_gradients zeroes once the expert steps (with update_every_* it accumulates until then)
-            gemm.grouped_wgrad(c.gyd, ws.a, go, G, out=gr["w2"], accumulate=cfg.accumulate)
-            gemm.grouped_linear(c.gyd, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
-            K.swiglu_bwd(c.da, ws.h, out=c.dh)
-            gemm.grouped_wgrad(c.dh, ws.n, go, G, out=gr["w13"], accumulate=cfg.accumulate)
-            gemm.grouped_linear(c.dh, sh.bf16["w13"], tile_group=tg, w_is_kn=True, out=c.dn)
-            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.raw_views["g"], dx=c.dxd, dgamma=gr["g"], dres=c.gyd,
-                           tile_rows=c.tile_rows, tile_group=tg)
+            # the expert's optimizer step zeroes (with update_every_* it accumulates until then)
+            swiglu_mlp_backward(plan, sh.bf16["w13"], sh.bf16["w2"], ws.n, ws.h, ws.a, ws.gyd, c.da, ws.dh13, c.dn, wgrad)
+            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.raw_views["g"], dx=c.dxd, dgamma=gr["g"], dres=ws.gyd,
+                           tile_rows=plan.tile_rows, tile_group=plan.tile_group)
         else:
-            K.grouped_colsum(c.gyd, tg, out=gr["b3"])
-            gemm.grouped_wgrad(c.gyd, ws.a2, go, G, out=gr["w3"], accumulate=cfg.accumulate)
-            gemm.grouped_linear(c.gyd, sh.bf16["w3"], tile_group=tg, w_is_kn=True, out=c.da)
-            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.raw_views["g2"], sh.raw_views["be2"], tg, dh=c.dh, dgamma=gr["g2"],
-                          dbeta=gr["be2"], dbias=gr["b2"])
-            gemm.grouped_wgrad(c.dh, ws.a1, go, G, out=gr["w2"], accumulate=cfg.accumulate)
-            gemm.grouped_linear(c.dh, sh.bf16["w2"], tile_group=tg, w_is_kn=True, out=c.da)
-            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.raw_views["g1"], sh.raw_views["be1"], tg, dh=c.dh, dgamma=gr["g1"],
-                          dbeta=gr["be1"], dbias=gr["b1"])
-            gemm.grouped_wgrad(c.dh, ws.xd, go, G, out=gr["w1"], accumulate=cfg.accumulate)
-            gemm.grouped_linear(c.dh, sh.bf16["w1"], tile_group=tg, w_is_kn=True, residual=c.gyd, out=c.dxd)
-        c.timer.mark("expert_ffn_bwd(wgrad+dgrad+ln)")
-        # ---- expert-side optimizer step (reference: ExpertBackend.apply_gradients right after backward)
-        if c.S:  # the owners read every rank's partial gradients of the shadowed experts: all ranks must be done
-            K.signal_wait(c.flags_off, K.SLOT_SHADOW, epoch, c.status, signal=True, wait=True)
-        self.apply_expert_gradients()
-        c.timer.mark("expert_adam")
+            ffn_backward(plan, sh.bf16, sh.raw_views, gr, ws.xd, (ws.h1, ws.a1, ws.h2, ws.a2),
+                         (ws.mean1, ws.rstd1, ws.mean2, ws.rstd2), ws.gyd, c.da, ws.dh2, ws.dh1, c.dxd, wgrad)
+        if c.small:
+            # biases / norm weights: the ordinary fused AMSGrad restricted to the small segments
+            small = sh.layout.small_mask
+            K.adam_step(sh.p_raw, sh.g, sh.m, sh.v_raw, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
+                        group_rows=ws.step_rows, zero_mask=small, G_active=self.E_loc, seg_mask=small, **opt)
+            sh.w8_dirty = True
+            c.timer.mark("expert_ffn_bwd(dgrad+ln+fused wgrad/AMSGrad)")
+        else:
+            c.timer.mark("expert_ffn_bwd(wgrad+dgrad+ln)")
+            # ---- expert-side optimizer step (reference: ExpertBackend.apply_gradients right after backward)
+            if c.S:  # the owners read every rank's partial gradients of the shadowed experts: all ranks must be done
+                K.signal_wait(c.flags_off, K.SLOT_SHADOW, epoch, c.status, signal=True, wait=True)
+            self.apply_expert_gradients()
+            c.timer.mark("expert_adam")
         dx = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=gy.device)
         K.combine_rows(c.dxd_off, idx, pair_row, None, dx, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_DINPUT,
                        epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner,
                        addend=dxs)
         c.timer.mark("bwd_combine")
         return dx, dlogits
-
-    def _backward_small(self, epoch):
-        """expert backward of the weight-streaming regime.  Order matters: the dgrad of a Linear reads the OLD weights, so
-        it runs before the fused wgrad+AMSGrad kernel of the same matrix updates them in place (reference: the optimizer
-        step follows the whole backward, lib/runtime/expert_backend.py:85-90)."""
-        c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
-        tg, go, rows, T = ws.tile_group, ws.group_off, ws.group_rows, c.tile_rows
-        gr = sh.grads
-        opt = c.adam_kwargs()
-        main = torch.cuda.current_stream(c.device)
-        side, chain_ctas = c.opt_stream, c.chain_ctas
-
-        def wgrad(name, dy, x):
-            """dW never reaches HBM: register accumulator -> AMSGrad epilogue -> p / m / v / vmax updated in place.  With the overlap
-            enabled the kernel goes to the optimizer stream, ordered after everything the main stream has launched so far (in
-            particular the dgrad that still reads the OLD weights); its inputs live in per-layer buffers."""
-            E = self.E_loc
-            kw = dict(p=None, p_lo=sh.lo_views[name][:E], p_bf16=sh.bf16[name][:E]) if sh.split else \
-                dict(p=sh.raw_views[name][:E], p_bf16=sh.bf16[name])
-            kw.update(m=sh.m_views[name][:E], v=sh.v_raw_views[name][:E],
-                      vmax=sh.vmax_views[name][:E] if cfg.amsgrad else None, step=sh.step, **opt)
-            if side is None:
-                K.wgrad_adam(dy, x, go, rows, **kw)
-                return
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                K.wgrad_adam(dy, x, go, rows, max_ctas=c.opt_ctas, **kw)
-            c._opt_pending = True
-
-        gyd = ws.gyd
-        K.bump_steps(sh.step, ws.step_rows)
-        if cfg.expert == "swiglu":
-            # the fused launches read gyd, a, dh13 and n: per-layer buffers whenever the optimizer stream is used.  Padding
-            # rows: xd and gyd are zero there, so da, dh13 and dn are too, and add nothing to dgamma (see _backward_cuda)
-            dh13 = ws.dh13
-            K.swapab_linear(gyd, sh.bf16["w2"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
-            wgrad("w2", gyd, ws.a)
-            K.swiglu_bwd(c.da, ws.h, out=dh13)
-            K.swapab_linear(dh13, sh.bf16["w13"], go, rows, out=c.dn, w_is_kn=True, max_ctas=chain_ctas)
-            wgrad("w13", dh13, ws.n)
-            K.rms_norm_bwd(c.dn, ws.xd, ws.rstd, sh.raw_views["g"], dx=c.dxd, dgamma=gr["g"], dres=gyd, tile_rows=T,
-                           tile_group=tg)
-        else:
-            dh2, dh1 = ws.dh2, ws.dh1
-            K.grouped_colsum(gyd, tg, out=gr["b3"], tile_rows=T)
-            K.swapab_linear(gyd, sh.bf16["w3"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
-            wgrad("w3", gyd, ws.a2)
-            K.ln_relu_bwd(c.da, ws.h2, ws.mean2, ws.rstd2, sh.raw_views["g2"], sh.raw_views["be2"], tg, dh=dh2, dgamma=gr["g2"],
-                          dbeta=gr["be2"], dbias=gr["b2"], tile_rows=T)
-            K.swapab_linear(dh2, sh.bf16["w2"], go, rows, out=c.da, w_is_kn=True, max_ctas=chain_ctas)
-            wgrad("w2", dh2, ws.a1)
-            K.ln_relu_bwd(c.da, ws.h1, ws.mean1, ws.rstd1, sh.raw_views["g1"], sh.raw_views["be1"], tg, dh=dh1, dgamma=gr["g1"],
-                          dbeta=gr["be1"], dbias=gr["b1"], tile_rows=T)
-            K.swapab_linear(dh1, sh.bf16["w1"], go, rows, out=c.dxd, w_is_kn=True, residual=gyd, max_ctas=chain_ctas)
-            wgrad("w1", dh1, ws.xd)
-        # biases / norm weights: the ordinary fused AMSGrad restricted to the small segments
-        small = sh.layout.small_mask
-        K.adam_step(sh.p_raw, sh.g, sh.m, sh.v_raw, sh.vmax, sh.p_bf16, sh.seg_sizes, sh.slots, step=sh.step,
-                    group_rows=ws.step_rows, zero_mask=small, G_active=self.E_loc, seg_mask=small, **opt)
-        sh.w8_dirty = True
 
     def apply_expert_gradients(self):
         sh, cfg, ws, c = self.shard, self.cfg, self.ws, self.ctx

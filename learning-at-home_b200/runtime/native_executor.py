@@ -22,6 +22,7 @@ import torch.nn.functional as F
 from ..models.layers import (FFN_SEG_KEYS, FFN_SEG_NAMES, FFN_SMALL_SEG_MASK, FeedforwardBlock, GatedFeedforwardBlock,
                               TransformerEncoderLayer)
 from ..ops import kernels as K, native
+from ..ops.expert_blocks import RowPlan, ffn_backward, ffn_forward, swiglu_mlp_backward, swiglu_mlp_forward
 
 TORCH_ENCODER_LAYER = "torch.nn.modules.transformer.TransformerEncoderLayer"
 OWN_ENCODER_LAYER = "lah_b200.models.layers.TransformerEncoderLayer"
@@ -333,15 +334,9 @@ class NativeFFNExecutor:
         self.xd[:rows].copy_(x)
         if padded > rows:
             self.xd[rows:padded].zero_()
-        go, gr, pv, bv = self.group_off, self.group_rows, self.state.pv, self.state.bv
-        K.swapab_linear(self.xd, bv["w1"], go, gr, out=self.h1, bias=pv["b1"])
-        K.ln_relu_fwd(self.h1[:padded], pv["g1"], pv["be1"], None, out=self.a1[:padded], mean=self.stats[0], rstd=self.stats[1],
-                      tile_rows=ALIGN)
-        K.swapab_linear(self.a1, bv["w2"], go, gr, out=self.h2, bias=pv["b2"])
-        K.ln_relu_fwd(self.h2[:padded], pv["g2"], pv["be2"], None, out=self.a2[:padded], mean=self.stats[2], rstd=self.stats[3],
-                      tile_rows=ALIGN)
-        K.swapab_linear(self.a2, bv["w3"], go, gr, out=self.yo, bias=pv["b3"], residual=self.xd)
-        return rows, padded
+        plan = RowPlan(self.group_off, self.group_rows, tile_rows=ALIGN, rows=padded)
+        ffn_forward(plan, self.state.bv, self.state.pv, self.xd, (self.h1, self.a1, self.h2, self.a2), self.stats, self.yo)
+        return rows, plan
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -351,31 +346,22 @@ class NativeFFNExecutor:
     @torch.no_grad()
     def backward(self, x: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
         """recompute forward, back-propagate, ONE optimizer step (reference: expert_backend.py:73-97); returns dL/dx"""
-        rows, padded = self._forward(x)
+        rows, plan = self._forward(x)
+        padded = plan.rows
         self.gyd[:rows].copy_(grad_out)
         if padded > rows:
             self.gyd[rows:padded].zero_()
         st = self.state
-        go, gr, pv, bv, gv = self.group_off, self.group_rows, st.pv, st.bv, st.gv
         seg_hyper = {name: h for h, mask in st.hypers() for s, name in enumerate(st.names) if (mask >> s) & 1}
         st.begin_step()
 
         def wgrad(name, dy, xin):   # each weight matrix with the settings of its own group
             hyper = seg_hyper[name]
-            K.wgrad_adam(dy, xin, go, gr, p=pv[name], m=st.mv[name], v=st.vv[name],
-                         vmax=st.vmv[name] if hyper["amsgrad"] else None, p_bf16=bv[name], step=st.step, **hyper)
+            K.wgrad_adam(dy, xin, self.group_off, self.group_rows, p=st.pv[name], m=st.mv[name], v=st.vv[name],
+                         vmax=st.vmv[name] if hyper["amsgrad"] else None, p_bf16=st.bv[name], step=st.step, **hyper)
 
-        K.grouped_colsum(self.gyd[:padded], None, out=gv["b3"], tile_rows=ALIGN)
-        K.swapab_linear(self.gyd, bv["w3"], go, gr, out=self.da, w_is_kn=True)
-        wgrad("w3", self.gyd, self.a2)
-        K.ln_relu_bwd(self.da[:padded], self.h2[:padded], self.stats[2], self.stats[3], pv["g2"], pv["be2"], None,
-                      dh=self.dh[:padded], dgamma=gv["g2"], dbeta=gv["be2"], dbias=gv["b2"], tile_rows=ALIGN)
-        K.swapab_linear(self.dh, bv["w2"], go, gr, out=self.da, w_is_kn=True)
-        wgrad("w2", self.dh, self.a1)
-        K.ln_relu_bwd(self.da[:padded], self.h1[:padded], self.stats[0], self.stats[1], pv["g1"], pv["be1"], None,
-                      dh=self.dh[:padded], dgamma=gv["g1"], dbeta=gv["be1"], dbias=gv["b1"], tile_rows=ALIGN)
-        K.swapab_linear(self.dh, bv["w1"], go, gr, out=self.dxd, w_is_kn=True, residual=self.gyd)
-        wgrad("w1", self.dh, self.xd)
+        ffn_backward(plan, st.bv, st.pv, st.gv, self.xd, (self.h1, self.a1, self.h2, self.a2), self.stats, self.gyd,
+                     self.da, self.dh, self.dh, self.dxd, wgrad)
         st.adam_step(FFN_SMALL_SEG_MASK)   # the small vectors
         st.end_step()
         return self.dxd[:rows].to(x.dtype)
@@ -466,12 +452,10 @@ class NativeGatedFFNExecutor:
         self.xd[:rows].copy_(x)
         if padded > rows:
             self.xd[rows:padded].zero_()
-        go, gr, pv, bv = self.group_off, self.group_rows, self.state.pv, self.state.bv
-        K.rms_norm_fwd(self.xd[:padded], pv["g"][0], self.eps, out=self.n[:padded], rstd=self.rstd[:padded])
-        K.swapab_linear(self.n, self.w13["bf16"], go, gr, out=self.h)
-        K.swiglu_fwd(self.h[:padded], out=self.a[:padded])
-        K.swapab_linear(self.a, bv["w2"], go, gr, out=self.yo, residual=self.xd)
-        return rows, padded
+        K.rms_norm_fwd(self.xd[:padded], self.state.pv["g"][0], self.eps, out=self.n[:padded], rstd=self.rstd[:padded])
+        plan = RowPlan(self.group_off, self.group_rows, rows=padded)
+        swiglu_mlp_forward(plan, self.w13["bf16"], self.state.bv["w2"], self.n, self.h, self.a, self.yo, residual=self.xd)
+        return rows, plan
 
     @torch.no_grad()
     def forward(self, x: torch.Tensor) -> torch.Tensor:
@@ -481,34 +465,30 @@ class NativeGatedFFNExecutor:
     @torch.no_grad()
     def backward(self, x: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
         """recompute forward, back-propagate, ONE optimizer step (reference: expert_backend.py:73-97); returns dL/dx"""
-        rows, padded = self._forward(x)
+        rows, plan = self._forward(x)
+        padded = plan.rows
         self.gyd[:rows].copy_(grad_out)
         if padded > rows:
             self.gyd[rows:padded].zero_()
         st = self.state
-        go, gr, pv, bv, gv, I = self.group_off, self.group_rows, st.pv, st.bv, st.gv, self.inner
+        pv, gv, I = st.pv, st.gv, self.inner
         hypers = st.hypers()
         group_of = {name: k for k, (_, mask) in enumerate(hypers) for s, name in enumerate(st.names) if (mask >> s) & 1}
         st.begin_step()
 
-        def wgrad(dy, xin, name, p, m, v, vmax, p_bf16):   # with the settings of the group that holds segment `name`
-            hyper = hypers[group_of[name]][0]
-            K.wgrad_adam(dy, xin, go, gr, p=p, m=m, v=v, vmax=vmax if hyper["amsgrad"] else None, p_bf16=p_bf16,
-                         step=st.step, **hyper)
+        def wgrad(name, dy, xin):   # each segment with the settings of its group: [W1; W3] in one launch if they share one
+            if name == "w13" and group_of["w1"] != group_of["w3"]:
+                wgrad("w1", dy[:, :I], xin)
+                wgrad("w3", dy[:, I:], xin)
+                return
+            w = self.w13 if name == "w13" else dict(p=st.pv[name], m=st.mv[name], v=st.vv[name], vmax=st.vmv[name],
+                                                    bf16=st.bv[name])
+            hyper = hypers[group_of["w1" if name == "w13" else name]][0]
+            K.wgrad_adam(dy, xin, self.group_off, self.group_rows, p=w["p"], m=w["m"], v=w["v"],
+                         vmax=w["vmax"] if hyper["amsgrad"] else None, p_bf16=w["bf16"], step=st.step, **hyper)
 
-        def seg(name):
-            return st.pv[name], st.mv[name], st.vv[name], st.vmv[name], bv[name]
-
-        K.swapab_linear(self.gyd, bv["w2"], go, gr, out=self.da, w_is_kn=True)
-        wgrad(self.gyd, self.a, "w2", *seg("w2"))
-        K.swiglu_bwd(self.da[:padded], self.h[:padded], out=self.dh[:padded])
-        K.swapab_linear(self.dh, self.w13["bf16"], go, gr, out=self.dn, w_is_kn=True)
-        if group_of["w1"] == group_of["w3"]:
-            w = self.w13
-            wgrad(self.dh, self.n, "w1", w["p"], w["m"], w["v"], w["vmax"], w["bf16"])
-        else:
-            wgrad(self.dh[:, :I], self.n, "w1", *seg("w1"))
-            wgrad(self.dh[:, I:], self.n, "w3", *seg("w3"))
+        swiglu_mlp_backward(plan, self.w13["bf16"], st.bv["w2"], self.n, self.h, self.a, self.gyd, self.da, self.dh,
+                            self.dn, wgrad)
         K.rms_norm_bwd(self.dn[:padded], self.xd[:padded], self.rstd[:padded], pv["g"][0], dx=self.dxd[:padded],
                        dgamma=gv["g"][0], dres=self.gyd[:padded], tile_rows=ALIGN)
         st.adam_step(1 << self.NAMES.index("g"))

@@ -109,7 +109,8 @@ def gemm_rates():
     torch.cuda.synchronize()
     ctx.check_status()
     ws, sh = layer.ws, layer.shard
-    Bp, go, _, tg = layer._shared_tables(B)
+    Bp, plan = layer._shared_plan(B)
+    go, tg = plan.group_off, plan.tile_group
     rows = int(ws.total_rows.item())
     G = ctx.G_tot
     w13g, w2g = torch.zeros(1, 2 * I, H, device="cuda"), torch.zeros(1, H, I, device="cuda")
