@@ -114,19 +114,27 @@ __device__ __forceinline__ void account_wait(const Peers& peers, unsigned long l
     if (peers.wait_ns && (threadIdx.x & 31) == 0) atomicAdd(peers.wait_ns, static_cast<unsigned long long>(dt));
 }
 
+// the affinity sigma(s) of the sigmoid router (DeepSeek-V3, DESIGN.md §6c), in fp32; every kernel that needs it calls this
+// one function.  A score below about -87 gives 0 (the reciprocal of an exp beyond 2^126): such a pair has no affinity
+__device__ __forceinline__ float sigmoid_affinity(float s) { return __fdividef(1.f, 1.f + __expf(-s)); }
+
 // ------------------------------------------------------------------------------------------------
 // gate: one warp per token.  BIAS (auxiliary-loss-free balancing, DESIGN.md §6b): the top-k is taken over the keys
-// s_{b,e} + bias[e], while the softmax weights use the unbiased s_{b,e} of the selected experts; each candidate carries
-// both values through the per-lane lists and the warp merge.  The bias is read with __ldg: a warp reads 32 consecutive
-// entries per candidate round, which stay in L1 for every token of the SM
+// s_{b,e} + bias[e], while the weights use the unbiased values of the selected experts; each candidate carries both
+// values through the per-lane lists and the warp merge.  The bias is read with __ldg: a warp reads 32 consecutive
+// entries per candidate round, which stay in L1 for every token of the SM.
+// SIGMOID (DESIGN.md §6c): the weights are scale * sigma_j / sum of sigma over the valid selected pairs, and sigma_j goes to
+// sig_out.  Without a bias the selection ranks s itself (sigma is monotone), so sigma is computed for the k selected
+// only; with one the key is sigma(s) + bias[e], and the carried value is sigma(s)
 // ------------------------------------------------------------------------------------------------
-template <bool BIAS>
+template <bool BIAS, bool SIGMOID>
 __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict__ logits, int B, GridSpec gs, int k,
                                                         const unsigned char* __restrict__ alive, float failure_rate,
                                                         unsigned long long seed, long long token_offset,
                                                         int* __restrict__ idx_out, float* __restrict__ w_out,
                                                         int* __restrict__ pos_out, int* __restrict__ counts,
-                                                        const int* __restrict__ step_ctr, const float* __restrict__ bias) {
+                                                        const int* __restrict__ step_ctr, const float* __restrict__ bias,
+                                                        float scale, float* __restrict__ sig_out) {
     if (step_ctr) token_offset += *reinterpret_cast<const long long*>(step_ctr + 2);
     extern __shared__ float s_logits[];  // [8 warps][gs.total]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -138,7 +146,7 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
 
     // per-lane sorted top-k over the candidates this lane owns (c = lane, lane+32, ...)
     float best_v[MAX_K];   // selection keys (biased when BIAS)
-    float best_u[MAX_K];   // BIAS: the unbiased scores of the same candidates
+    float best_u[MAX_K];   // BIAS: the unbiased values of the same candidates (s, or sigma(s) when SIGMOID)
     int best_i[MAX_K];
 #pragma unroll
     for (int j = 0; j < MAX_K; ++j) {
@@ -163,11 +171,12 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
                 s += lg[gs.offset[d] + i];
             }
         }
-        float key = s;
-        if constexpr (BIAS) key = __fadd_rn(s, __ldg(bias + c));
+        float key = s, aff = s;
+        if constexpr (BIAS && SIGMOID) aff = sigmoid_affinity(s);
+        if constexpr (BIAS) key = __fadd_rn(aff, __ldg(bias + c));
         // insertion (ties keep the smaller expert id first because candidates arrive in increasing order)
         if (key > best_v[MAX_K - 1] || best_i[MAX_K - 1] < 0) {
-            float v = key, u = s;
+            float v = key, u = aff;
             int id = c;
             bool shifting = false;  // once inserted, everything below shifts down by one
 #pragma unroll
@@ -191,7 +200,7 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
         }
     }
     // merge: k rounds of warp arg-max over the heads of the per-lane lists
-    float sel_v[MAX_K];   // the unbiased scores of the selected experts (the softmax inputs)
+    float sel_v[MAX_K];   // the unbiased values of the selected experts (s; sigma(s) when BIAS and SIGMOID)
     int sel_i[MAX_K];
     int head = 0;
 #pragma unroll
@@ -227,6 +236,34 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
             sel_i[j] = bi;
             if (bi >= 0 && bi == id) ++head;  // the winning lane pops its head
         }
+    }
+    if constexpr (SIGMOID) {
+        // normalised affinities of the selected (alive) experts, summed in selection order
+        float sg[MAX_K];
+        float S = 0.f;
+#pragma unroll
+        for (int j = 0; j < MAX_K; ++j) {
+            sg[j] = 0.f;
+            if (sel_i[j] >= 0) sg[j] = BIAS ? sel_v[j] : sigmoid_affinity(sel_v[j]);
+            S += sg[j];
+        }
+        const float norm = S > 0.f ? __fdividef(scale, S) : 0.f;   // every sigma underflowed: zero weights
+        if (lane < k) {
+            int id = -1;
+            float v = 0.f;
+#pragma unroll
+            for (int j = 0; j < MAX_K; ++j)
+                if (j == lane) {
+                    id = sel_i[j];
+                    v = sg[j];
+                }
+            const long long o = static_cast<long long>(b) * k + lane;
+            idx_out[o] = id;
+            w_out[o] = v * norm;
+            sig_out[o] = v;
+            if (id < 0) pos_out[o] = 0;
+        }
+        return;
     }
     // softmax over the selected (alive) experts
     float mx = -INFINITY;
@@ -823,7 +860,9 @@ __global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineA
 // ------------------------------------------------------------------------------------------------
 // backward of combine (gate side): dw[b,j] = <g[b], y_j>;  dlogit_j = w_j (dw_j - sum_i w_i dw_i)
 // scattered into the gradient of the grid logits [B, gs.total].  A selected pair that scatter_rows dropped (pair_row -1)
-// has y_j = 0, so dw_j = 0, but its weight still took softmax mass from the others: its logit gets -w_j sum_i w_i dw_i
+// has y_j = 0, so dw_j = 0, but its weight still took softmax mass from the others: its logit gets -w_j sum_i w_i dw_i.
+// SIGMOID (DESIGN.md §6c, w_j = scale sigma_j / S): dlogit_j = sigma_j (1 - sigma_j) (scale dw_j - sum_i w_i dw_i) / S, with
+// sigma_j from the gate's sig array and S summed over the valid selected pairs (dropped ones included); S = 0: no gradient
 // ------------------------------------------------------------------------------------------------
 struct GateBwdArgs {
     long long yo_off;         // symmetric expert outputs [max_rows, H]
@@ -836,8 +875,11 @@ struct GateBwdArgs {
     const int* route_owner;   // [E] or nullptr
 };
 
-template <int VEC_PER_LANE>
-__global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs a, GridSpec gs) {
+// SIGMOID: sig = sigma of every selected pair [B * k] (written by gate_topk), scale = the routed scaling factor.  They follow
+// gs rather than extend GateBwdArgs, which would move gs in the parameter bank of the softmax instantiations
+template <int VEC_PER_LANE, bool SIGMOID>
+__global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs a, GridSpec gs,
+                                                       const float* __restrict__ sig, float scale) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * 8 + warp;
     if (b >= a.B) return;
@@ -854,13 +896,14 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
             g[v * 8 + 2 * t + 1] = f.y;
         }
     }
-    float dw[MAX_K], wj[MAX_K];
+    float dw[MAX_K], wj[MAX_K], sj[MAX_K];
     int ej[MAX_K];
     float dot_sum = 0.f;
 #pragma unroll
     for (int j = 0; j < MAX_K; ++j) {
         dw[j] = 0.f;
         wj[j] = 0.f;
+        if constexpr (SIGMOID) sj[j] = 0.f;
         ej[j] = -1;
         if (j < a.k) {
             const long long p = static_cast<long long>(b) * a.k + j;
@@ -869,6 +912,7 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
             if (e >= 0) {   // a pair dropped by scatter_rows (row -1) added nothing to y but keeps its softmax weight
                 wj[j] = a.w[p];
                 ej[j] = e;
+                if constexpr (SIGMOID) sj[j] = sig[p];
             }
             if (e >= 0 && row >= 0) {
                 const int4* sp = reinterpret_cast<const int4*>(peers.base[a.route_owner ? a.route_owner[e] : e / a.E_loc] + a.yo_off) +
@@ -894,10 +938,19 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
     for (int i = lane; i < gs.total; i += 32) dl[i] = 0.f;
     __syncwarp();
     if (lane == 0) {
+        float inv_s = 0.f;   // SIGMOID: 1 / S
+        if constexpr (SIGMOID) {
+            float S = 0.f;
+#pragma unroll
+            for (int j = 0; j < MAX_K; ++j) S += sj[j];
+            inv_s = S > 0.f ? __fdividef(1.f, S) : 0.f;
+        }
 #pragma unroll
         for (int j = 0; j < MAX_K; ++j) {
             if (ej[j] < 0) continue;
-            const float d = wj[j] * (dw[j] - dot_sum);
+            float d;
+            if constexpr (SIGMOID) d = sj[j] * (1.f - sj[j]) * (scale * dw[j] - dot_sum) * inv_s;
+            else d = wj[j] * (dw[j] - dot_sum);
             int rem = ej[j];
             for (int dd = gs.ndim - 1; dd >= 0; --dd) {
                 const int i = rem % gs.size[dd];
@@ -1059,7 +1112,10 @@ __device__ __forceinline__ float router_max_score(const float* lg, const GridSpe
 }
 
 // one warp per token: z_b and F_b into z / Fb, the CTA's sums of F_b and z_b^2 into partials[2 * blockIdx.x]; the last CTA
-// to finish adds the partials in CTA order: loss = ((N/B) sum F_b, (1/B) sum z_b^2)
+// to finish adds the partials in CTA order: loss = ((N/B) sum F_b, (1/B) sum z_b^2).
+// SIGMOID (DESIGN.md §6c): p_{b,e} = sigma_{b,e} / S'_b with S'_b the sum of sigma over the live experts, one pass; z[b] holds
+// S'_b for the backward and L_z is 0 (this router has no log-partition)
+template <bool SIGMOID>
 __global__ void __launch_bounds__(RL_WARPS * 32) router_loss_fwd_kernel(const float* __restrict__ logits, int B, GridSpec gs,
                                                                         const unsigned char* __restrict__ alive,
                                                                         const float* __restrict__ f, float* __restrict__ z,
@@ -1075,25 +1131,42 @@ __global__ void __launch_bounds__(RL_WARPS * 32) router_loss_fwd_kernel(const fl
         float* lg = s_lg + warp * gs.total;
         for (int i = lane; i < gs.total; i += 32) lg[i] = logits[static_cast<long long>(b) * gs.total + i];
         __syncwarp();
-        const float mx = router_max_score(lg, gs, alive, lane);
-        float se = 0.f, sf = 0.f;
-        if (mx > -INFINITY) {
+        if constexpr (SIGMOID) {
+            float se = 0.f, sf = 0.f;
             for (int c = lane; c < gs.num_experts; c += 32) {
                 if (alive && !alive[c]) continue;
-                const float p = __expf(pk_score(lg, gs, c) - mx);
+                const float p = sigmoid_affinity(pk_score(lg, gs, c));
                 se += p;
                 sf += f[c] * p;
             }
-        }
-        se = warp_sum(se);
-        sf = warp_sum(sf);
-        if (mx > -INFINITY && se > 0.f) {
-            zv = mx + __logf(se);
-            Fv = sf / se;
-        }
-        if (lane == 0) {
-            z[b] = zv;
-            Fb[b] = Fv;
+            se = warp_sum(se);
+            sf = warp_sum(sf);
+            if (se > 0.f) Fv = sf / se;
+            if (lane == 0) {
+                z[b] = se;
+                Fb[b] = Fv;
+            }
+        } else {
+            const float mx = router_max_score(lg, gs, alive, lane);
+            float se = 0.f, sf = 0.f;
+            if (mx > -INFINITY) {
+                for (int c = lane; c < gs.num_experts; c += 32) {
+                    if (alive && !alive[c]) continue;
+                    const float p = __expf(pk_score(lg, gs, c) - mx);
+                    se += p;
+                    sf += f[c] * p;
+                }
+            }
+            se = warp_sum(se);
+            sf = warp_sum(sf);
+            if (mx > -INFINITY && se > 0.f) {
+                zv = mx + __logf(se);
+                Fv = sf / se;
+            }
+            if (lane == 0) {
+                z[b] = zv;
+                Fb[b] = Fv;
+            }
         }
     }
     if (lane == 0) {
@@ -1152,7 +1225,10 @@ __host__ __device__ __forceinline__ int router_bwd_warp_floats(const GridSpec& g
 // one warp per token: dlogits[b] += d/dl of (aux_coef * L_aux + z_coef * L_z) with f constant.  The expert gradient is
 // g_e = p_e (aux_coef N (f_e - F_b) + 2 z_coef z_b) / B.  On a 1-d grid it is the logit's gradient itself and is added
 // directly; otherwise it is staged in shared memory and each grid logit (d, i) is summed by one lane over the experts
-// whose d-th coordinate is i, in increasing expert order
+// whose d-th coordinate is i, in increasing expert order.
+// SIGMOID: g_e = sigma_e (1 - sigma_e) aux_coef N (f_e - F_b) / (B S'_b) with S'_b from z[b] (S'_b = 0: no gradient); z_coef
+// is not read
+template <bool SIGMOID>
 __global__ void __launch_bounds__(RL_WARPS * 32) router_loss_bwd_kernel(const float* __restrict__ logits, int B, GridSpec gs,
                                                                         const unsigned char* __restrict__ alive,
                                                                         const float* __restrict__ f,
@@ -1172,10 +1248,18 @@ __global__ void __launch_bounds__(RL_WARPS * 32) router_loss_bwd_kernel(const fl
     const float zb = z[b];
     const float invB = 1.f / static_cast<float>(B);
     const float base_aux = aux_coef * f[gs.num_experts];
-    const float c0 = 2.f * z_coef * zb - base_aux * Fb[b];
+    const float c0 = SIGMOID ? -base_aux * Fb[b] : 2.f * z_coef * zb - base_aux * Fb[b];
+    const float inv_s = SIGMOID && zb > 0.f ? invB / zb : 0.f;   // SIGMOID: 1 / (B S'_b)
     for (int c = lane; c < gs.num_experts; c += 32) {
         float v = 0.f;
-        if (!alive || alive[c]) v = __expf(pk_score(lg, gs, c) - zb) * (base_aux * f[c] + c0) * invB;
+        if constexpr (SIGMOID) {
+            if (!alive || alive[c]) {
+                const float sg = sigmoid_affinity(pk_score(lg, gs, c));
+                v = sg * (1.f - sg) * (base_aux * f[c] + c0) * inv_s;
+            }
+        } else if (!alive || alive[c]) {
+            v = __expf(pk_score(lg, gs, c) - zb) * (base_aux * f[c] + c0) * invB;
+        }
         if (gs.ndim == 1)
             dl[c] += v;
         else
@@ -1202,6 +1286,34 @@ __global__ void __launch_bounds__(RL_WARPS * 32) router_loss_bwd_kernel(const fl
 
 static Peers g_peers = {};
 static bool g_peers_set = false;
+
+// the launches of the gate and router-loss instantiations (lah_gate_topk / lah_router_loss_bwd pick one)
+template <bool BIAS, bool SIGMOID>
+static int launch_gate_topk(const float* logits, int B, const GridSpec& gs, int k, const unsigned char* alive,
+                            float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w,
+                            int* pos, int* counts, const float* bias, float scale, float* sig, cudaStream_t st) {
+    // each of the 8 warps stages its token's grid logits in shared memory: 4096 of them (a dense gate over as many experts
+    // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in
+    if (int e = set_max_dynamic_smem<gate_topk_kernel<BIAS, SIGMOID>>(8 * sizeof(float) * LAYOUT_MAX_E)) return e;
+    if (B <= 0) return 0;
+    gate_topk_kernel<BIAS, SIGMOID><<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(
+        logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, bias, scale, sig);
+    return 0;
+}
+
+template <bool SIGMOID>
+static int launch_router_loss_bwd(const float* logits, int B, const GridSpec& gs, const unsigned char* alive,
+                                  const float* f, const float* z, const float* Fb, float aux_coef, float z_coef,
+                                  float* dlogits, cudaStream_t st) {
+    if (int e = set_max_dynamic_smem<router_loss_bwd_kernel<SIGMOID>>(RL_WARPS * sizeof(float) *
+                                                                       (2 * LAYOUT_MAX_E + LAYOUT_MAX_E / 32 + 1)))
+        return e;
+    if (B == 0) return 0;
+    router_loss_bwd_kernel<SIGMOID><<<(B + RL_WARPS - 1) / RL_WARPS, RL_WARPS * 32,
+                                      RL_WARPS * router_bwd_warp_floats(gs) * sizeof(float), st>>>(
+        logits, B, gs, alive, f, z, Fb, aux_coef, z_coef, dlogits);
+    return 0;
+}
 
 }  // namespace lah
 
@@ -1295,27 +1407,33 @@ static int make_grid_spec(GridSpec* gs, const int* grid, int ndim) {
     return 0;
 }
 
-// bias: float [prod(grid)] added to the scores for the selection only (DESIGN.md §6b); nullptr selects without one
+// bias: float [prod(grid)] added to the selection key only (DESIGN.md §6b); nullptr selects without one.
+// score_mode 0: softmax weights (scale must be 1, sig unused); 1: sigmoid weights scale * sigma_j / S with sigma_j of every
+// selected pair into sig [B * k] (DESIGN.md §6c)
 int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, const unsigned char* alive,
                   float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w, int* pos,
-                  int* counts, const float* bias, cudaStream_t st) {
+                  int* counts, const float* bias, int score_mode, float scale, float* sig, cudaStream_t st) {
     GridSpec gs;
     if (make_grid_spec(&gs, grid, ndim)) return -2;
     if (k < 1 || k > MAX_K) return -3;
-    // each of the 8 warps stages its token's grid logits in shared memory: 4096 of them (a dense gate over as many experts
-    // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in
     if (gs.total > LAYOUT_MAX_E) return -2;
     if (bias && gs.num_experts > LAYOUT_MAX_E) return -2;
-    if (int e = bias ? set_max_dynamic_smem<gate_topk_kernel<true>>(8 * sizeof(float) * LAYOUT_MAX_E)
-                     : set_max_dynamic_smem<gate_topk_kernel<false>>(8 * sizeof(float) * LAYOUT_MAX_E))
-        return e;
-    if (B <= 0) return 0;
-    if (bias)
-        gate_topk_kernel<true><<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(
-            logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, bias);
+    if (score_mode == 0 && scale != 1.f) return -5;
+    if (score_mode == 1 && (!(scale > 0.f && scale <= FLT_MAX) || !sig)) return -5;
+    int e;
+    if (score_mode == 0)
+        e = bias ? launch_gate_topk<true, false>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
+                                                 counts, bias, 1.f, nullptr, st)
+                 : launch_gate_topk<false, false>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
+                                                  counts, nullptr, 1.f, nullptr, st);
+    else if (score_mode == 1)
+        e = bias ? launch_gate_topk<true, true>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
+                                                counts, bias, scale, sig, st)
+                 : launch_gate_topk<false, true>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
+                                                 counts, nullptr, scale, sig, st);
     else
-        gate_topk_kernel<false><<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(
-            logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, nullptr);
+        return -4;
+    if (e || B <= 0) return e;
     rank_slots_kernel<<<gs.num_experts, 1024, 0, st>>>(idx, B * k, pos, counts);
     return -(int)cudaGetLastError();
 }
@@ -1388,22 +1506,28 @@ int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, con
     return -(int)cudaGetLastError();
 }
 
+// sig: nullptr for the softmax gate; the sigma array of the sigmoid gate (DESIGN.md §6c), whose weights carry scale
 int lah_gate_bwd(long long yo_off, const void* grad, const int* idx, const int* pair_row, const float* w,
                  float* dlogits, int B, int k, int H, int E_loc, const int* grid_sizes, int ndim, const int* route_owner,
-                 cudaStream_t st) {
+                 const float* sig, float scale, cudaStream_t st) {
     if (!g_peers_set) return -10;
     if (B <= 0) return 0;
     GridSpec gs;
     if (make_grid_spec(&gs, grid_sizes, ndim)) return -2;
     if (k > MAX_K) return -3;
+    if (sig ? !(scale > 0.f && scale <= FLT_MAX) : scale != 1.f) return -5;
     GateBwdArgs a;
     a.yo_off = yo_off; a.grad = (const bf16*)grad; a.idx = idx; a.pair_row = pair_row; a.w = w; a.dlogits = dlogits;
     a.B = B; a.k = k; a.H = H; a.E_loc = E_loc; a.route_owner = route_owner;
     const int grid = (B + 7) / 8;
-    if (H == 256) gate_bwd_kernel<1><<<grid, 256, 0, st>>>(g_peers, a, gs);
-    else if (H == 512) gate_bwd_kernel<2><<<grid, 256, 0, st>>>(g_peers, a, gs);
-    else if (H == 1024) gate_bwd_kernel<4><<<grid, 256, 0, st>>>(g_peers, a, gs);
+#define LAH_GATE_BWD(V)                                                                \
+    if (sig) gate_bwd_kernel<V, true><<<grid, 256, 0, st>>>(g_peers, a, gs, sig, scale);  \
+    else gate_bwd_kernel<V, false><<<grid, 256, 0, st>>>(g_peers, a, gs, nullptr, 1.f);
+    if (H == 256) { LAH_GATE_BWD(1) }
+    else if (H == 512) { LAH_GATE_BWD(2) }
+    else if (H == 1024) { LAH_GATE_BWD(4) }
     else return -2;
+#undef LAH_GATE_BWD
     return -(int)cudaGetLastError();
 }
 
@@ -1421,37 +1545,45 @@ static int router_grid_spec(GridSpec* gs, const int* grid, int ndim) {
 }
 
 // forward of the router losses: f (E + 1 floats: f_e, then N) from the count table [count_rows][E], z_b and F_b of every
-// token ([B] each), loss = (L_aux, L_z).  partials: 2 * ceil(B / 4) floats; ticket: one int that is 0 between calls
+// token ([B] each), loss = (L_aux, L_z).  partials: 2 * ceil(B / 4) floats; ticket: one int that is 0 between calls.
+// score_mode 1: the sigmoid router (DESIGN.md §6c): z_b holds S'_b and L_z is 0
 int lah_router_loss_fwd(const float* logits, int B, const int* grid, int ndim, const unsigned char* alive, const int* counts,
                         int count_rows, float* f, float* z, float* Fb, float* loss, float* partials, int* ticket,
-                        cudaStream_t st) {
+                        int score_mode, cudaStream_t st) {
     GridSpec gs;
     if (router_grid_spec(&gs, grid, ndim)) return -2;
     if (B < 0 || count_rows < 1 || count_rows > MAX_WORLD) return -3;
     if (!counts || !f || !loss || (B > 0 && (!logits || !z || !Fb || !partials || !ticket))) return -4;
-    if (int e = set_max_dynamic_smem<router_loss_fwd_kernel>(RL_WARPS * sizeof(float) * LAYOUT_MAX_E)) return e;
+    if (score_mode != 0 && score_mode != 1) return -5;
+    if (int e = score_mode ? set_max_dynamic_smem<router_loss_fwd_kernel<true>>(RL_WARPS * sizeof(float) * LAYOUT_MAX_E)
+                           : set_max_dynamic_smem<router_loss_fwd_kernel<false>>(RL_WARPS * sizeof(float) * LAYOUT_MAX_E))
+        return e;
     router_f_kernel<<<1, 1024, 0, st>>>(counts, count_rows, gs.num_experts, alive, f, B, loss);
-    if (B > 0)
-        router_loss_fwd_kernel<<<(B + RL_WARPS - 1) / RL_WARPS, RL_WARPS * 32, RL_WARPS * gs.total * sizeof(float), st>>>(
-            logits, B, gs, alive, f, z, Fb, partials, ticket, loss);
+    const int blocks = (B + RL_WARPS - 1) / RL_WARPS;
+    const size_t smem = RL_WARPS * gs.total * sizeof(float);
+    if (B > 0 && score_mode)
+        router_loss_fwd_kernel<true><<<blocks, RL_WARPS * 32, smem, st>>>(logits, B, gs, alive, f, z, Fb, partials, ticket,
+                                                                          loss);
+    else if (B > 0)
+        router_loss_fwd_kernel<false><<<blocks, RL_WARPS * 32, smem, st>>>(logits, B, gs, alive, f, z, Fb, partials, ticket,
+                                                                           loss);
     return -(int)cudaGetLastError();
 }
 
-// backward of the router losses: dlogits [B, sum(grid)] += the gradient of aux_coef * L_aux + z_coef * L_z
+// backward of the router losses: dlogits [B, sum(grid)] += the gradient of aux_coef * L_aux + z_coef * L_z.
+// score_mode 1: the sigmoid router, z from its forward; z_coef must be 0
 int lah_router_loss_bwd(const float* logits, int B, const int* grid, int ndim, const unsigned char* alive, const float* f,
-                        const float* z, const float* Fb, float aux_coef, float z_coef, float* dlogits, cudaStream_t st) {
+                        const float* z, const float* Fb, float aux_coef, float z_coef, float* dlogits, int score_mode,
+                        cudaStream_t st) {
     GridSpec gs;
     if (router_grid_spec(&gs, grid, ndim)) return -2;
     if (B < 0) return -3;
     if (B > 0 && (!logits || !f || !z || !Fb || !dlogits)) return -4;
-    if (int e = set_max_dynamic_smem<router_loss_bwd_kernel>(RL_WARPS * sizeof(float) *
-                                                              (2 * LAYOUT_MAX_E + LAYOUT_MAX_E / 32 + 1)))
+    if (score_mode != 0 && (score_mode != 1 || z_coef != 0.f)) return -5;
+    if (int e = score_mode ? launch_router_loss_bwd<true>(logits, B, gs, alive, f, z, Fb, aux_coef, z_coef, dlogits, st)
+                           : launch_router_loss_bwd<false>(logits, B, gs, alive, f, z, Fb, aux_coef, z_coef, dlogits, st))
         return e;
-    if (B == 0) return 0;
-    router_loss_bwd_kernel<<<(B + RL_WARPS - 1) / RL_WARPS, RL_WARPS * 32,
-                             RL_WARPS * router_bwd_warp_floats(gs) * sizeof(float), st>>>(logits, B, gs, alive, f, z, Fb,
-                                                                                         aux_coef, z_coef, dlogits);
-    return -(int)cudaGetLastError();
+    return B == 0 ? 0 : -(int)cudaGetLastError();
 }
 
 // auxiliary-loss-free balancing: bias [E] moves by rate toward balance from the count table [count_rows][E] (one launch)

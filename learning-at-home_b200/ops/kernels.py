@@ -44,7 +44,7 @@ def _lib():
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
-        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, P],
+        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, I, Fl, P, P],
         "lah_expert_bias_update": [P, I, I, P, Fl, P, P],
         "lah_layout_exchange": [L, L, I, I, I, I, I, I, I, P, P, P, P, P, P, P, I, Fl, I, P, P, P, P, P],
         "lah_scatter_rows": [P, P, P, P, P, P, L, L, I, I, I, I, I, I, I, I, P, P, P, P, P, I, P],
@@ -52,9 +52,9 @@ def _lib():
         "lah_zero_slots": [P, I, P, I, I, I, I, P],
         "lah_signal_wait": [L, I, I, I, I, P, P],
         "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P, P],
-        "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P],
-        "lah_router_loss_fwd": [P, I, P, I, P, P, I, P, P, P, P, P, P, P],
-        "lah_router_loss_bwd": [P, I, P, I, P, P, P, P, Fl, Fl, P, P],
+        "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P, Fl, P],
+        "lah_router_loss_fwd": [P, I, P, I, P, P, I, P, P, P, P, P, P, I, P],
+        "lah_router_loss_bwd": [P, I, P, I, P, P, P, P, Fl, Fl, P, I, P],
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
                           I, P],
         "lah_bump_steps": [P, P, I, P],
@@ -339,17 +339,42 @@ def _check_expert_bias(what, bias, E, device):
                          f"{tuple(bias.shape)} on {bias.device}")
 
 
+ROUTER_SCORES = ("softmax", "sigmoid")   # the weight functions of the gate (DESIGN.md §6c), in csrc score_mode order
+
+
+def _score_mode(what, score, scale, sig, n, device):
+    """csrc score_mode of ``score``; checks ``scale`` and the sigma array ``sig`` (float32, >= n entries) before any launch"""
+    if score not in ROUTER_SCORES:
+        raise ValueError(f"{what}: score must be one of {ROUTER_SCORES}, got {score!r}")
+    scale = float(scale)
+    if score == "softmax":
+        if scale != 1.0 or sig is not None:
+            raise ValueError(f"{what}: the softmax gate takes neither a scale ({scale}) nor a sig array")
+        return 0
+    if not math.isfinite(scale) or scale <= 0.0:
+        raise ValueError(f"{what}: scale must be a finite value > 0, got {scale}")
+    if sig is None or sig.dtype != torch.float32 or not sig.is_contiguous() or sig.numel() < n or sig.device != device:
+        got = "None" if sig is None else f"{sig.dtype} {tuple(sig.shape)} on {sig.device}"
+        raise ValueError(f"{what}: the sigmoid gate needs sig, a contiguous float32 tensor of >= {n} entries on "
+                         f"{device}, got {got}")
+    return 1
+
+
 def gate_topk(logits, grid_size, k, *, alive=None, failure_rate=0.0, seed=0, token_offset=0, idx, w, pos, counts,
-              bias=None):
-    """top-k routing of the grid logits (two launches).  ``bias``: float32 [prod(grid)] added to the scores for the
-    selection only; the weights stay the softmax over the unbiased scores of the selected experts (DESIGN.md §6b)"""
+              bias=None, score="softmax", scale=1.0, sig=None):
+    """top-k routing of the grid logits (two launches).  ``bias``: float32 [prod(grid)] added to the selection key only
+    (DESIGN.md §6b).  ``score="softmax"``: the weights are the softmax over the unbiased scores of the selected experts.
+    ``score="sigmoid"`` (DeepSeek-V3, DESIGN.md §6c): the weights are scale * sigma_j / sum of sigma over the valid selected
+    pairs, the bias is added to sigma(s), and sigma_j of every pair goes to ``sig`` (float32 [B * k], 0 for a missing pair)"""
     B = logits.shape[0]
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.shape[1] == sum(grid_size)
     if bias is not None:
         _check_expert_bias("gate_topk", bias, math.prod(grid_size), logits.device)
+    mode = _score_mode("gate_topk", score, scale, sig, B * k, logits.device)
     native.check(_lib().lah_gate_topk(ptr(logits), B, ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), k,
                                       ptr(alive), float(failure_rate), int(seed) & (2 ** 64 - 1), int(token_offset),
-                                      ptr(idx), ptr(w), ptr(pos), ptr(counts), ptr(bias), stream_ptr()), "lah_gate_topk")
+                                      ptr(idx), ptr(w), ptr(pos), ptr(counts), ptr(bias), mode, float(scale), ptr(sig),
+                                      stream_ptr()), "lah_gate_topk")
     native.count_launch(2)
 
 
@@ -454,12 +479,16 @@ def combine_rows_ref(src, idx, pair_row, w=None, addend=None):
     return total.to(torch.bfloat16)
 
 
-def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route_owner=None):
+def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route_owner=None, *, score="softmax",
+             scale=1.0, sig=None):
+    """gradient of the grid logits from the combine's (one launch).  ``score="sigmoid"``: the gate's ``sig`` array and
+    ``scale`` of the same forward (DESIGN.md §6c)"""
     B, H = grad.shape
     assert grad.is_contiguous() and grad.dtype == torch.bfloat16 and dlogits.dtype == torch.float32
+    _score_mode("gate_bwd", score, scale, sig, B * k, grad.device)
     native.check(_lib().lah_gate_bwd(yo_off, ptr(grad), ptr(idx), ptr(pair_row), ptr(w), ptr(dlogits), B, k, H, E_loc,
                                      ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), ptr(route_owner),
-                                     stream_ptr()),
+                                     ptr(sig), float(scale), stream_ptr()),
                  "lah_gate_bwd")
     native.count_launch()
     return dlogits
@@ -494,13 +523,22 @@ def _router_args(what, logits, grid_size, alive):
     return grid, logits.shape[0], E
 
 
-def router_loss_fwd(logits, grid_size, counts, *, alive=None, f, z, Fb, loss, partials=None, ticket=None):
+def _router_score_mode(what, score):
+    if score not in ROUTER_SCORES:
+        raise ValueError(f"{what}: score must be one of {ROUTER_SCORES}, got {score!r}")
+    return ROUTER_SCORES.index(score)
+
+
+def router_loss_fwd(logits, grid_size, counts, *, alive=None, f, z, Fb, loss, partials=None, ticket=None,
+                    score="softmax"):
     """Router losses of one training forward (two launches).  ``counts``: int32 [R, E] count table (one row per rank,
     R <= MAX_WORLD), summed over its rows.  Writes f (float32 [E + 1]: f_e = c_e / sum c, then N = live experts), z and
     Fb (float32, >= B entries: logsumexp z_b and F_b = sum_e f_e p_{b,e}) and loss (float32 [2]: unweighted L_aux, L_z).
     ``partials`` (float32, >= 2 * ceil(B / ROUTER_WARPS)) and ``ticket`` (int32 [1], zero between calls) are scratch,
-    allocated when None."""
+    allocated when None.  ``score="sigmoid"`` (DESIGN.md §6c): p_{b,e} = sigma_{b,e} / S'_b over the live experts, z
+    holds S'_b and L_z is 0."""
     grid, B, E = _router_args("router_loss_fwd", logits, grid_size, alive)
+    mode = _router_score_mode("router_loss_fwd", score)
     if counts.dtype != torch.int32 or counts.dim() != 2 or counts.shape[1] != E or not counts.is_contiguous() \
             or not 1 <= counts.shape[0] <= MAX_WORLD:
         raise ValueError(f"router_loss_fwd: counts must be a contiguous int32 [R <= {MAX_WORLD}, {E}] tensor, got "
@@ -520,15 +558,18 @@ def router_loss_fwd(logits, grid_size, counts, *, alive=None, f, z, Fb, loss, pa
         raise ValueError("router_loss_fwd: ticket must be an int32 tensor")
     native.check(_lib().lah_router_loss_fwd(ptr(logits), B, ctypes.cast(_grid_array(grid), c_void_p), len(grid),
                                             ptr(alive), ptr(counts), counts.shape[0], ptr(f), ptr(z), ptr(Fb), ptr(loss),
-                                            ptr(partials), ptr(ticket), stream_ptr()), "lah_router_loss_fwd")
+                                            ptr(partials), ptr(ticket), mode, stream_ptr()), "lah_router_loss_fwd")
     native.count_launch(2 if B > 0 else 1)
     return loss
 
 
-def router_loss_bwd(logits, grid_size, *, alive=None, f, z, Fb, aux_coef, z_coef, dlogits):
+def router_loss_bwd(logits, grid_size, *, alive=None, f, z, Fb, aux_coef, z_coef, dlogits, score="softmax"):
     """dlogits += the gradient of aux_coef * L_aux + z_coef * L_z w.r.t. the grid logits (f constant), from the f, z and
-    Fb the forward wrote for the same logits (one launch)"""
+    Fb the forward wrote for the same logits and score (one launch).  The sigmoid router has no z-loss: z_coef must be 0"""
     grid, B, E = _router_args("router_loss_bwd", logits, grid_size, alive)
+    mode = _router_score_mode("router_loss_bwd", score)
+    if mode and z_coef != 0.0:
+        raise ValueError(f"router_loss_bwd: the sigmoid router has no z-loss; z_coef must be 0, got {z_coef}")
     _f32_vec(f, "router_loss_bwd: f", E + 1)
     for t, name in ((z, "z"), (Fb, "Fb")):
         if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() < B:
@@ -540,7 +581,7 @@ def router_loss_bwd(logits, grid_size, *, alive=None, f, z, Fb, aux_coef, z_coef
         raise ValueError("router_loss_bwd: the coefficients must be finite")
     native.check(_lib().lah_router_loss_bwd(ptr(logits), B, ctypes.cast(_grid_array(grid), c_void_p), len(grid),
                                             ptr(alive), ptr(f), ptr(z), ptr(Fb), float(aux_coef), float(z_coef),
-                                            ptr(dlogits), stream_ptr()), "lah_router_loss_bwd")
+                                            ptr(dlogits), mode, stream_ptr()), "lah_router_loss_bwd")
     if B > 0:
         native.count_launch()
     return dlogits
@@ -1084,13 +1125,26 @@ def product_key_scores(logits, grid_size):
     return scores
 
 
-def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None):
+def sigmoid_weights_ref(sel, valid, scale=1.0):
+    """weights of the sigmoid router (DESIGN.md §6c) from the selected scores ``sel`` [B, k] and their validity:
+    scale * sigma_j / S_b with S_b the sum of sigma over the valid pairs; a token with S_b = 0 gets zeros.  Differentiable
+    (no NaN reaches the gradient of an S_b = 0 token)."""
+    sg = torch.where(valid, torch.sigmoid(sel), torch.zeros_like(sel))
+    S = sg.sum(-1, keepdim=True)
+    return torch.where(S > 0, scale * sg / torch.where(S > 0, S, torch.ones_like(S)), torch.zeros_like(sg))
+
+
+def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, score="softmax", scale=1.0):
     """returns idx [B,k] (-1 for missing), weights [B,k] (softmax over alive selected).  Equal scores select the smaller
     expert id first, like gate_topk_kernel (torch.topk leaves the order of ties unspecified, so it sorts stably instead).
     The scores are summed first grid dimension first and the kernel last dimension first: on 3-d and 4-d grids they can
     differ in the last bit unless the logits are exact in any order (e.g. small multiples of a power of two).
     ``bias`` ([E]): the selection ranks the float32 keys score + bias[e]; the weights stay the softmax over the unbiased
-    scores of the selected experts."""
+    scores of the selected experts.
+    ``score="sigmoid"`` (DESIGN.md §6c): the weights are ``sigmoid_weights_ref`` of the selected scores, and a bias is
+    added to sigmoid(score) in float32; without one the selection is the softmax router's."""
+    if score not in ROUTER_SCORES:
+        raise ValueError(f"gate_topk_ref: score must be one of {ROUTER_SCORES}, got {score!r}")
     scores = product_key_scores(logits.float(), grid_size)
     dead = torch.zeros_like(scores, dtype=torch.bool)
     if alive is not None:
@@ -1105,20 +1159,27 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None):
         top_v, top_i = top_v[..., :k], top_i[..., :k]
     else:
         b = bias.to(device=scores.device, dtype=torch.float32).reshape(1, -1)
-        keys = scores + F.pad(b, (0, scores.shape[-1] - b.shape[-1]))
+        base = scores if score == "softmax" else torch.sigmoid(scores).masked_fill(~torch.isfinite(scores), float("-inf"))
+        keys = base + F.pad(b, (0, scores.shape[-1] - b.shape[-1]))
         top_i = torch.sort(keys, dim=-1, descending=True, stable=True)[1][..., :k]
         top_v = torch.gather(scores, -1, top_i)
     valid = torch.isfinite(top_v)
+    if score == "sigmoid":
+        w = sigmoid_weights_ref(top_v.masked_fill(~valid, 0.0), valid, scale)
+        return torch.where(valid, top_i, torch.full_like(top_i, -1)), w
     w = torch.softmax(top_v.masked_fill(~valid, float("-inf")), dim=-1)
     w = torch.where(valid, w, torch.zeros_like(w)).nan_to_num(0.0)
     return torch.where(valid, top_i, torch.full_like(top_i, -1)), w
 
 
-def router_loss_ref(logits, grid_size, counts, alive=None):
+def router_loss_ref(logits, grid_size, counts, alive=None, score="softmax"):
     """Oracle of the router-loss kernels: (L_aux, L_z) as 0-d tensors in the dtype of ``logits`` (float64 works),
     differentiable in the logits with f detached.  ``counts``: [E] routed pairs per expert, or [R, E] (summed over R).
     L_aux = N * sum_e f_e * mean_b p_{b,e} over the N live experts, L_z = mean_b z_b^2; a token without a finite live
-    score contributes 0 to both, and N = 0 gives zeros."""
+    score contributes 0 to both, and N = 0 gives zeros.  ``score="sigmoid"`` (DESIGN.md §6c): p_{b,e} = sigma_{b,e} / S'_b
+    with S'_b the sum of sigma over the live experts (a token with S'_b = 0 contributes 0), and L_z = 0."""
+    if score not in ROUTER_SCORES:
+        raise ValueError(f"router_loss_ref: score must be one of {ROUTER_SCORES}, got {score!r}")
     scores = product_key_scores(logits, grid_size)
     B, E = scores.shape
     live = torch.ones(E, dtype=torch.bool, device=scores.device) if alive is None else alive.bool().reshape(-1).to(scores.device)
@@ -1131,6 +1192,11 @@ def router_loss_ref(logits, grid_size, counts, alive=None):
     if N == 0 or B == 0:
         zero = scores.sum() * 0
         return zero, zero
+    if score == "sigmoid":
+        sg = torch.where(live.view(1, -1), torch.sigmoid(scores), torch.zeros_like(scores))
+        S = sg.sum(-1, keepdim=True)
+        p = sg / torch.where(S > 0, S, torch.ones_like(S))
+        return N * (p * f).sum() / B, torch.zeros((), dtype=scores.dtype, device=scores.device)
     z = torch.logsumexp(masked, -1, keepdim=True)
     p = torch.where(live.view(1, -1) & ok, torch.exp(masked - z), torch.zeros_like(masked))
     z = torch.where(ok, z, torch.zeros_like(z)).squeeze(-1)

@@ -129,6 +129,12 @@ class DMoEConfig:
     # fewer than the mean box-wide routed pairs, - when more.  No loss and no gradient, so it also balances the frozen
     # emulator gate.  Read at construction; 0 (the default) allocates and launches nothing
     expert_bias_update_rate: float = 0.0
+    # the gate's weight function (DESIGN.md §6c): "softmax" over the selected scores, or "sigmoid" (DeepSeek-V3): affinities
+    # sigma(s), the selected ones normalised to sum to routed_scaling_factor.  With "sigmoid" an expert bias is added to
+    # sigma(s) for the selection, and the load-balancing loss uses p = sigma / sum of sigma; there is no z-loss.  Both are
+    # read at construction; a factor other than 1 needs "sigmoid"
+    router_score: str = "softmax"
+    routed_scaling_factor: float = 1.0
     # shared-expert isolation (DESIGN.md §9c, DeepSeek-MoE / Qwen-MoE): every token also passes through one always-active
     # GatedFeedforwardBlock of this inner width, added to the combine of the routed experts with weight 1 and without a
     # second residual.  Its parameters are trainer-side (replicated on every rank, averaged over ranks, stepped once per
@@ -156,6 +162,17 @@ class DMoEConfig:
         v = float(self.expert_bias_update_rate)
         if not math.isfinite(v) or v < 0.0:
             raise ValueError(f"DMoEConfig.expert_bias_update_rate must be a finite value >= 0, got {v}")
+        if self.router_score not in K.ROUTER_SCORES:
+            raise ValueError(f"DMoEConfig.router_score must be one of {K.ROUTER_SCORES}, got {self.router_score!r}")
+        v = float(self.routed_scaling_factor)
+        if not math.isfinite(v) or v <= 0.0:
+            raise ValueError(f"DMoEConfig.routed_scaling_factor must be a finite value > 0, got {v}")
+        if v != 1.0 and self.router_score != "sigmoid":
+            raise ValueError("DMoEConfig.routed_scaling_factor scales the normalised sigmoid weights; with "
+                             f"router_score={self.router_score!r} it must be 1, got {v}")
+        if self.router_score == "sigmoid" and self.router_z_loss_coef > 0.0:
+            raise ValueError("DMoEConfig.router_z_loss_coef: the z-loss penalises the softmax log-partition, which "
+                             "router_score='sigmoid' does not have; set it to 0")
         if self.shared_inner_dim < 0:
             raise ValueError(f"DMoEConfig.shared_inner_dim must be >= 0, got {self.shared_inner_dim}")
         if self.shared_inner_dim and self.expert != "swiglu":
@@ -240,6 +257,14 @@ def refuse_expert_bias(cfg: DMoEConfig, arm: str):
     if cfg.expert_bias_update_rate > 0.0:
         raise ValueError(f"{arm} does not balance with expert biases; set expert_bias_update_rate to 0 "
                          "(FusedDMoE / DMoETrainer apply them)")
+
+
+def refuse_router_score(cfg: DMoEConfig, arm: str):
+    """the baseline arms weight the selected experts with a softmax: refuse the sigmoid router instead of silently
+    routing with a softmax"""
+    if cfg.router_score != "softmax":
+        raise ValueError(f"{arm} weights the selected experts with a softmax; set router_score='softmax' "
+                         "(FusedDMoE / DMoETrainer route with sigmoid affinities)")
 
 
 def refuse_shared_expert(cfg: DMoEConfig, arm: str):
@@ -713,6 +738,8 @@ class LayerWorkspace:
         self.owned_shadow = torch.full((ctx.E_loc * 2,), -1, **i32)
         self.tile_group = torch.full((ctx.max_tiles,), -1, **i32)
         self.total_rows = torch.zeros(1, **i32)
+        # the sigmoid router (DESIGN.md §6c): sigma of every selected pair, written by gate_topk and read by gate_bwd
+        self.sig = torch.zeros(P, **f32) if cfg.router_score == "sigmoid" else None
         self.router_loss = None
         if cfg.router_losses:
             # router losses: f (box-wide routing shares, snapshotted from the count table the next layer overwrites, then
@@ -814,6 +841,10 @@ class FusedDMoE(nn.Module):
             # the router-loss buffers (per layer and the shared scratch) are allocated from the context's configuration
             raise ValueError("FusedDMoE: router losses need an EngineContext built from a DMoEConfig with a nonzero "
                              "router_aux_loss_coef or router_z_loss_coef (the context allocates their buffers)")
+        if ctx is not None and cfg.router_score != ctx.cfg.router_score:
+            # the workspace (the sigma array of the sigmoid gate) is allocated from the context's configuration
+            raise ValueError(f"FusedDMoE: router_score={cfg.router_score!r} needs an EngineContext built with the same "
+                             f"router_score, got {ctx.cfg.router_score!r}")
         self.cfg, self.ctx, self.layer_index = cfg, ctx, layer_index
         self.grid_size = tuple(cfg.grid_size)
         if cfg.gate_mode == "emulator":
@@ -851,6 +882,9 @@ class FusedDMoE(nn.Module):
         self.expert_bias_rate = float(cfg.expert_bias_update_rate)
         self.register_buffer("expert_bias", torch.zeros(cfg.num_experts, dtype=torch.float32, device=dev)
                              if self.expert_bias_rate > 0.0 else None)
+        # the gate's weight function (cfg.router_score / routed_scaling_factor, read here once; DESIGN.md §6c)
+        self.router_score = cfg.router_score
+        self.routed_scale = float(cfg.routed_scaling_factor)
         # shared expert (cfg.shared_inner_dim, read here once): initialised like GatedFeedforwardBlock(hidden, I_s), drawn
         # from the global RNG like proj (DMoETrainer seeds it, so every rank starts identical), kept as the segments of
         # GATED_LAYOUT so that [W1; W3] is one GEMM operand and one contiguous gradient
@@ -935,7 +969,7 @@ class FusedDMoE(nn.Module):
         idx, w, pos, pair_row = ws.idx[:P], ws.w[:P], ws.pos[:P], ws.pair_row[:P]
         K.gate_topk(logits, self.grid_size, k, alive=c.alive, failure_rate=cfg.failure_rate if self.training else 0.0,
                     seed=cfg.seed * 7919 + self.layer_index, token_offset=c.token_counter, idx=idx, w=w, pos=pos,
-                    counts=c.counts, bias=self.expert_bias)
+                    counts=c.counts, bias=self.expert_bias, **self._score_args(P))
         c.token_counter += B
         c.timer.mark("gate_topk")
         K.layout_exchange(c.cnt_all_off, c.flags_off, K.SLOT_COUNTS, epoch, c.E, c.E_loc, c.max_rows, align=c.align,
@@ -948,7 +982,8 @@ class FusedDMoE(nn.Module):
             # before combine_rows: no peer can reach the next layer's count exchange (which rewrites cnt_all) until this
             # rank's combine has signalled
             K.router_loss_fwd(logits, self.grid_size, c.cnt_all[:c.world], alive=c.alive, f=ws.router_f, z=ws.router_z,
-                              Fb=ws.router_F, loss=ws.router_loss, partials=c.router_partials, ticket=c.router_ticket)
+                              Fb=ws.router_F, loss=ws.router_loss, partials=c.router_partials, ticket=c.router_ticket,
+                              score=self.router_score)
         if self.training and self.expert_bias is not None:   # same cnt_all lifetime as the router losses above
             K.expert_bias_update(c.cnt_all[:c.world], alive=c.alive, bias=self.expert_bias, rate=self.expert_bias_rate)
         if c.S:  # replicas of this step's hot experts: weights from the owners' bf16 mirror, small params from fp32
@@ -992,6 +1027,12 @@ class FusedDMoE(nn.Module):
                        signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner, addend=ys)
         c.timer.mark("combine")
         return y
+
+    def _score_args(self, P):
+        """the weight-function keywords of K.gate_topk / K.gate_bwd for P routed pairs (none for the softmax gate)"""
+        if self.router_score == "softmax":
+            return {}
+        return dict(score=self.router_score, scale=self.routed_scale, sig=self.ws.sig[:P])
 
     def _expert_plan(self):
         """swap-AB groups of 16 rows on the small path (backward GEMMs on ``chain_ctas``), 128-row tiles on the big one"""
@@ -1063,11 +1104,13 @@ class FusedDMoE(nn.Module):
         idx, w, pos, pair_row = ws.idx[:P], ws.w[:P], ws.pos[:P], ws.pair_row[:P]
         gy = gy.to(torch.bfloat16)
         dlogits = torch.empty(B, sum(self.grid_size), dtype=torch.float32, device=gy.device)
-        K.gate_bwd(ws.yo_off, gy, idx, pair_row, w, dlogits, k, c.E_loc, self.grid_size, route_owner=ws.route_owner)
+        K.gate_bwd(ws.yo_off, gy, idx, pair_row, w, dlogits, k, c.E_loc, self.grid_size, route_owner=ws.route_owner,
+                   **self._score_args(P))
         if logits is not None:
             K.router_loss_bwd(logits, self.grid_size, alive=c.alive, f=ws.router_f, z=ws.router_z, Fb=ws.router_F,
                               aux_coef=self.router_aux_coef * self.router_grad_scale,
-                              z_coef=self.router_z_coef * self.router_grad_scale, dlogits=dlogits)
+                              z_coef=self.router_z_coef * self.router_grad_scale, dlogits=dlogits,
+                              score=self.router_score)
         K.scatter_rows(gy, w, idx, pos, None, pair_row, ws.gyd_off, c.flags_off, K.SLOT_GRAD, epoch, k, c.E_loc,
                        c.max_rows, ws.group_off, ws.group_rows, c.done_counter, c.status, align=c.align,
                        route_owner=ws.route_owner, num_groups=c.G_tot)
@@ -1215,17 +1258,20 @@ class FusedDMoE(nn.Module):
             fail_mask = torch.rand(x.shape[0], cfg.num_experts, device=x.device) < cfg.failure_rate
         alive = self.ctx.alive if self.ctx is not None else getattr(self, "alive_ref", None)
         idx, w_sel = K.gate_topk_ref(logits.detach(), self.grid_size, cfg.k, alive=alive, fail_mask=fail_mask,
-                                     bias=self.expert_bias)
+                                     bias=self.expert_bias, score=self.router_score, scale=self.routed_scale)
         if self.training and self.expert_bias is not None:
             with torch.no_grad():
                 counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
                 self.expert_bias.copy_(K.expert_bias_update_ref(counts, self.expert_bias, self.expert_bias_rate, alive))
-        # differentiable weights: softmax over the selected logits
+        # differentiable weights: softmax over the selected logits, or their normalised sigmoid affinities
         scores = K.product_key_scores(logits, self.grid_size)
         safe_idx = idx.clamp(min=0)
-        sel = torch.gather(scores, 1, safe_idx).masked_fill(idx < 0, float("-inf"))
-        weights = torch.softmax(sel, dim=-1)
-        weights = torch.where(idx >= 0, weights, torch.zeros_like(weights))
+        if self.router_score == "sigmoid":
+            weights = K.sigmoid_weights_ref(torch.gather(scores, 1, safe_idx), idx >= 0, self.routed_scale)
+        else:
+            sel = torch.gather(scores, 1, safe_idx).masked_fill(idx < 0, float("-inf"))
+            weights = torch.softmax(sel, dim=-1)
+            weights = torch.where(idx >= 0, weights, torch.zeros_like(weights))
         xf = x.float()
         out = torch.zeros(x.shape[0], cfg.hidden, dtype=torch.float32, device=x.device)
         rnd = (lambda t: t.to(torch.bfloat16).float()) if emulate_bf16 else (lambda t: t)
@@ -1247,7 +1293,7 @@ class FusedDMoE(nn.Module):
             out = out + rnd(self._gated_branch(p, rnd(xf), rnd))
         if self.training and self.router_on:
             counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
-            l_aux, l_z = K.router_loss_ref(logits, self.grid_size, counts, alive=alive)
+            l_aux, l_z = K.router_loss_ref(logits, self.grid_size, counts, alive=alive, score=self.router_score)
             with torch.no_grad():
                 self.router_loss.copy_(torch.stack([l_aux, l_z]).detach())
             if torch.is_grad_enabled() and logits.requires_grad:

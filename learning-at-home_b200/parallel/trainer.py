@@ -459,6 +459,8 @@ class DMoETrainer:
         # every expert's pending row / step counters and its partially accumulated gradient (per rank, like `experts`)
         if self._stale_ring is not None:
             trainer["stale_ring"] = self._stale_ring.detach().clone().cpu()
+        if self.cfg.router_score != "softmax":   # only then: default checkpoints keep their keys
+            trainer["router_score"] = self.cfg.router_score
         if self.cfg.accumulate:
             state["pending"] = [dict(rows=b.shard.pending_rows.clone().cpu(), steps=b.shard.pending_steps.clone().cpu(),
                                      grad=b.shard.g.detach().clone().cpu()) for b in self.model.blocks]
@@ -477,6 +479,11 @@ class DMoETrainer:
         if own_shared != saved_shared:
             raise ValueError(f"checkpoint's shared expert has other widths than this trainer's (shared_inner_dim = "
                              f"{self.cfg.shared_inner_dim}): {saved_shared} against {own_shared}")
+        saved_score = state["trainer"].get("router_score", "softmax")
+        if saved_score != self.cfg.router_score:
+            # the gate (and any expert biases) were trained against the other weight function
+            raise ValueError(f"checkpoint was trained with router_score={saved_score!r}, this trainer has "
+                             f"router_score={self.cfg.router_score!r}; build it with the checkpoint's router_score")
         biases = [k for k in own if k.endswith(".expert_bias")]
         if any(k.endswith(".expert_bias") and k not in own for k in saved):
             # dropping the saved biases would silently change which experts the gates select
