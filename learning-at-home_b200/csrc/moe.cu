@@ -126,23 +126,193 @@ __device__ __forceinline__ float sigmoid_affinity(float s) { return __fdividef(1
 // SIGMOID (DESIGN.md §6c): the weights are scale * sigma_j / sum of sigma over the valid selected pairs, and sigma_j goes to
 // sig_out.  Without a bias the selection ranks s itself (sigma is monotone), so sigma is computed for the k selected
 // only; with one the key is sigma(s) + bias[e], and the carried value is sigma(s)
+// GROUPED (group-limited routing, DeepSeek-V2/V3, DESIGN.md §6d): the E experts form n_group groups of E / n_group
+// consecutive flat ids; a group pass scores every group (softmax: its largest key; sigmoid: the sum of its two largest,
+// sigma(s) without a bias), topk_group rounds of warp arg-max pick the best groups into a 64-bit mask, and the selection
+// loop skips the candidates outside it
 // ------------------------------------------------------------------------------------------------
+constexpr int MAX_GROUPS = 64;
+constexpr int GROUP_WORDS = 2 * MAX_GROUPS;   // per-warp shared words of the grouped gate: group scores and flags
+
+// the group key of candidate c of token `tok` (false when c is dead or failure-injected): s + bias, sigma(s) + bias, or s
 template <bool BIAS, bool SIGMOID>
-__global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict__ logits, int B, GridSpec gs, int k,
+__device__ __forceinline__ bool group_candidate_key(const float* lg, const GridSpec& gs, int c,
+                                                    const unsigned char* __restrict__ alive, float failure_rate,
+                                                    unsigned long long seed, long long tok,
+                                                    const float* __restrict__ bias, float& key) {
+    if (alive && !alive[c]) return false;
+    if (failure_rate > 0.f) {
+        const unsigned long long h = seed ^ (static_cast<unsigned long long>(tok) * 0x100000001B3ull +
+                                             static_cast<unsigned long long>(c));
+        if (hash_uniform(h) < failure_rate) return false;
+    }
+    int rem = c;
+    float s = 0.f;
+#pragma unroll
+    for (int d = MAX_GRID_DIMS - 1; d >= 0; --d) {
+        if (d < gs.ndim) {
+            const int i = rem % gs.size[d];
+            rem /= gs.size[d];
+            s += lg[gs.offset[d] + i];
+        }
+    }
+    key = s;
+    if constexpr (BIAS) key = __fadd_rn(SIGMOID ? sigmoid_affinity(s) : s, __ldg(bias + c));
+    return true;
+}
+
+// a lane's running best key (and, for the sigmoid router, second best) of one group and its candidate count (capped at 2)
+struct GroupTop2 {
+    float v1, v2;
+    int n;
+};
+
+template <bool SIGMOID>
+__device__ __forceinline__ void group_push(GroupTop2& t, float key) {
+    if constexpr (SIGMOID) {
+        if (key > t.v1) {
+            t.v2 = t.v1;
+            t.v1 = key;
+        } else if (key > t.v2) {
+            t.v2 = key;
+        }
+        t.n = min(t.n + 1, 2);
+    } else {
+        t.v1 = fmaxf(t.v1, key);
+        t.n = 1;
+    }
+}
+
+// merge with the lane `o` away (xor butterfly): max / min only, so the result is the same in every lane order
+template <bool SIGMOID>
+__device__ __forceinline__ void group_merge(GroupTop2& t, int o) {
+    const float o1 = __shfl_xor_sync(0xffffffffu, t.v1, o);
+    const int on = __shfl_xor_sync(0xffffffffu, t.n, o);
+    if constexpr (SIGMOID) {
+        const float o2 = __shfl_xor_sync(0xffffffffu, t.v2, o);
+        t.v2 = fmaxf(fminf(t.v1, o1), fmaxf(t.v2, o2));
+        t.n = min(t.n + on, 2);
+    } else {
+        t.n |= on;
+    }
+    t.v1 = fmaxf(t.v1, o1);
+}
+
+// the group score: the largest key (softmax), or the sum of the two largest (sigmoid; one candidate scores its key).
+// The unbiased sigmoid router tracks s and scores sigma(s): sigma is monotone, so the two largest s give the two largest sigma
+template <bool BIAS, bool SIGMOID>
+__device__ __forceinline__ float group_score(const GroupTop2& t) {
+    if constexpr (!SIGMOID) return t.v1;
+    const float a = BIAS ? t.v1 : sigmoid_affinity(t.v1);
+    if (t.n < 2) return a;
+    return a + (BIAS ? t.v2 : sigmoid_affinity(t.v2));
+}
+
+// group pass of one warp (one token): writes the score and the has-a-candidate flag of every group to gscore / gvalid
+template <bool BIAS, bool SIGMOID>
+__device__ __forceinline__ void group_scores(const float* lg, const GridSpec& gs, int n_group,
+                                             const unsigned char* __restrict__ alive, float failure_rate,
+                                             unsigned long long seed, long long tok, const float* __restrict__ bias,
+                                             float* gscore, int* gvalid, int lane) {
+    const int E = gs.num_experts, gsz = E / n_group;
+    if (32 % gsz == 0) {
+        // groups of 1, 2, 4, 8, 16 or 32 experts: one candidate per lane and round, the groups are aligned lane segments
+        for (int c0 = 0; c0 < E; c0 += 32) {
+            const int c = c0 + lane;
+            GroupTop2 t{-INFINITY, -INFINITY, 0};
+            float key;
+            if (c < E && group_candidate_key<BIAS, SIGMOID>(lg, gs, c, alive, failure_rate, seed, tok, bias, key))
+                group_push<SIGMOID>(t, key);
+            for (int o = gsz >> 1; o > 0; o >>= 1) group_merge<SIGMOID>(t, o);
+            if (c < E && (lane & (gsz - 1)) == 0) {
+                gscore[c / gsz] = group_score<BIAS, SIGMOID>(t);
+                gvalid[c / gsz] = t.n > 0;
+            }
+        }
+    } else {
+        // any other size (a multiple of 32 is the fast case): the warp scans one group, then one butterfly per group
+        for (int g = 0; g < n_group; ++g) {
+            GroupTop2 t{-INFINITY, -INFINITY, 0};
+            for (int c = g * gsz + lane; c < (g + 1) * gsz; c += 32) {
+                float key;
+                if (group_candidate_key<BIAS, SIGMOID>(lg, gs, c, alive, failure_rate, seed, tok, bias, key))
+                    group_push<SIGMOID>(t, key);
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) group_merge<SIGMOID>(t, o);
+            if (lane == 0) {
+                gscore[g] = group_score<BIAS, SIGMOID>(t);
+                gvalid[g] = t.n > 0;
+            }
+        }
+    }
+    __syncwarp();
+}
+
+// topk_group rounds of warp arg-max over the scores of the groups that have a candidate (ties: the smaller group id);
+// then gvalid[g] says whether group g was selected
+__device__ __forceinline__ void select_groups(const float* gscore, int* gvalid, int n_group, int topk_group, int lane) {
+    // lane l holds groups l and l + 32
+    const float a = lane < n_group ? gscore[lane] : -INFINITY;
+    const float c = lane + 32 < n_group ? gscore[lane + 32] : -INFINITY;
+    bool av = lane < n_group && gvalid[lane], cv = lane + 32 < n_group && gvalid[lane + 32];
+    bool as = false, cs = false;
+    for (int r = 0; r < topk_group; ++r) {
+        float bv = -INFINITY;
+        int bi = -1;
+        if (av && (!cv || a >= c)) {
+            bv = a;
+            bi = lane;
+        } else if (cv) {
+            bv = c;
+            bi = lane + 32;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if ((oi >= 0) && (bi < 0 || ov > bv || (ov == bv && oi < bi))) {
+                bv = ov;
+                bi = oi;
+            }
+        }
+        if (bi < 0) break;   // fewer groups with a candidate than topk_group (the same in every lane)
+        if (bi == lane) av = false, as = true;
+        if (bi == lane + 32) cv = false, cs = true;
+    }
+    if (lane < n_group) gvalid[lane] = as;
+    if (lane + 32 < n_group) gvalid[lane + 32] = cs;
+    __syncwarp();
+}
+
+template <bool BIAS, bool SIGMOID, bool GROUPED>
+__global__ void __launch_bounds__(256, GROUPED ? 1 : 0) gate_topk_kernel(const float* __restrict__ logits, int B, GridSpec gs, int k,
                                                         const unsigned char* __restrict__ alive, float failure_rate,
                                                         unsigned long long seed, long long token_offset,
                                                         int* __restrict__ idx_out, float* __restrict__ w_out,
                                                         int* __restrict__ pos_out, int* __restrict__ counts,
                                                         const int* __restrict__ step_ctr, const float* __restrict__ bias,
-                                                        float scale, float* __restrict__ sig_out) {
+                                                        float scale, float* __restrict__ sig_out, int n_group,
+                                                        int topk_group) {
     if (step_ctr) token_offset += *reinterpret_cast<const long long*>(step_ctr + 2);
-    extern __shared__ float s_logits[];  // [8 warps][gs.total]
+    extern __shared__ float s_logits[];  // [8 warps][gs.total]; GROUPED: then [8 warps][GROUP_WORDS]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * 8 + warp;
     if (b >= B) return;
     float* lg = s_logits + warp * gs.total;
     for (int i = lane; i < gs.total; i += 32) lg[i] = logits[static_cast<long long>(b) * gs.total + i];
     __syncwarp();
+    const int* gsel = nullptr;   // GROUPED: gsel[g] != 0 for the selected groups
+    unsigned gdiv = 0;           // GROUPED: c / (E / n_group) = __umulhi(2 c, gdiv), exact for c, E <= 4096
+    if constexpr (GROUPED) {
+        float* gscore = s_logits + 8 * gs.total + warp * GROUP_WORDS;
+        int* gvalid = reinterpret_cast<int*>(gscore + MAX_GROUPS);
+        group_scores<BIAS, SIGMOID>(lg, gs, n_group, alive, failure_rate, seed, token_offset + b, bias, gscore, gvalid,
+                                    lane);
+        select_groups(gscore, gvalid, n_group, topk_group, lane);
+        gsel = gvalid;
+        gdiv = 0x7fffffffu / static_cast<unsigned>(gs.num_experts / n_group) + 1u;   // ceil(2^31 / size): 2^31 for size 1
+    }
 
     // per-lane sorted top-k over the candidates this lane owns (c = lane, lane+32, ...)
     float best_v[MAX_K];   // selection keys (biased when BIAS)
@@ -155,6 +325,8 @@ __global__ void __launch_bounds__(256) gate_topk_kernel(const float* __restrict_
         best_i[j] = -1;
     }
     for (int c = lane; c < gs.num_experts; c += 32) {
+        if constexpr (GROUPED)
+            if (!gsel[__umulhi(static_cast<unsigned>(c) << 1, gdiv)]) continue;
         if (alive && !alive[c]) continue;
         if (failure_rate > 0.f) {
             const unsigned long long key = seed ^ (static_cast<unsigned long long>(token_offset + b) * 0x100000001B3ull +
@@ -1288,16 +1460,22 @@ static Peers g_peers = {};
 static bool g_peers_set = false;
 
 // the launches of the gate and router-loss instantiations (lah_gate_topk / lah_router_loss_bwd pick one)
-template <bool BIAS, bool SIGMOID>
+template <bool BIAS, bool SIGMOID, bool GROUPED>
 static int launch_gate_topk(const float* logits, int B, const GridSpec& gs, int k, const unsigned char* alive,
                             float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w,
-                            int* pos, int* counts, const float* bias, float scale, float* sig, cudaStream_t st) {
+                            int* pos, int* counts, const float* bias, float scale, float* sig, int n_group,
+                            int topk_group, cudaStream_t st) {
     // each of the 8 warps stages its token's grid logits in shared memory: 4096 of them (a dense gate over as many experts
-    // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in
-    if (int e = set_max_dynamic_smem<gate_topk_kernel<BIAS, SIGMOID>>(8 * sizeof(float) * LAYOUT_MAX_E)) return e;
+    // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in.  GROUPED adds 512 B per
+    // warp of group scores and flags
+    const int group_floats = GROUPED ? GROUP_WORDS : 0;
+    if (int e = set_max_dynamic_smem<gate_topk_kernel<BIAS, SIGMOID, GROUPED>>(8 * sizeof(float) *
+                                                                               (LAYOUT_MAX_E + group_floats)))
+        return e;
     if (B <= 0) return 0;
-    gate_topk_kernel<BIAS, SIGMOID><<<(B + 7) / 8, 256, 8 * gs.total * sizeof(float), st>>>(
-        logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, bias, scale, sig);
+    gate_topk_kernel<BIAS, SIGMOID, GROUPED><<<(B + 7) / 8, 256, 8 * (gs.total + group_floats) * sizeof(float), st>>>(
+        logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, bias, scale, sig,
+        n_group, topk_group);
     return 0;
 }
 
@@ -1409,10 +1587,13 @@ static int make_grid_spec(GridSpec* gs, const int* grid, int ndim) {
 
 // bias: float [prod(grid)] added to the selection key only (DESIGN.md §6b); nullptr selects without one.
 // score_mode 0: softmax weights (scale must be 1, sig unused); 1: sigmoid weights scale * sigma_j / S with sigma_j of every
-// selected pair into sig [B * k] (DESIGN.md §6c)
+// selected pair into sig [B * k] (DESIGN.md §6c).
+// n_group / topk_group (DESIGN.md §6d): each token picks its experts from the topk_group best of n_group groups of
+// consecutive expert ids; 1 / 1 (or topk_group = n_group) launches the ungrouped gate
 int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, const unsigned char* alive,
                   float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w, int* pos,
-                  int* counts, const float* bias, int score_mode, float scale, float* sig, cudaStream_t st) {
+                  int* counts, const float* bias, int score_mode, float scale, float* sig, int n_group, int topk_group,
+                  cudaStream_t st) {
     GridSpec gs;
     if (make_grid_spec(&gs, grid, ndim)) return -2;
     if (k < 1 || k > MAX_K) return -3;
@@ -1420,19 +1601,24 @@ int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, 
     if (bias && gs.num_experts > LAYOUT_MAX_E) return -2;
     if (score_mode == 0 && scale != 1.f) return -5;
     if (score_mode == 1 && (!(scale > 0.f && scale <= FLT_MAX) || !sig)) return -5;
+    if (n_group < 1 || n_group > MAX_GROUPS || gs.num_experts % n_group) return -6;
+    if (n_group > 1 && gs.num_experts > LAYOUT_MAX_E) return -6;
+    if (topk_group < 1 || topk_group > n_group) return -6;
+    const bool grouped = topk_group < n_group;
     int e;
+#define LAH_GATE_TOPK(BIAS, SIGMOID, GROUPED)                                                                          \
+    launch_gate_topk<BIAS, SIGMOID, GROUPED>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,  \
+                                             counts, BIAS ? bias : nullptr, SIGMOID ? scale : 1.f,                    \
+                                             SIGMOID ? sig : nullptr, n_group, topk_group, st)
     if (score_mode == 0)
-        e = bias ? launch_gate_topk<true, false>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
-                                                 counts, bias, 1.f, nullptr, st)
-                 : launch_gate_topk<false, false>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
-                                                  counts, nullptr, 1.f, nullptr, st);
+        e = grouped ? (bias ? LAH_GATE_TOPK(true, false, true) : LAH_GATE_TOPK(false, false, true))
+                    : (bias ? LAH_GATE_TOPK(true, false, false) : LAH_GATE_TOPK(false, false, false));
     else if (score_mode == 1)
-        e = bias ? launch_gate_topk<true, true>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
-                                                counts, bias, scale, sig, st)
-                 : launch_gate_topk<false, true>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,
-                                                 counts, nullptr, scale, sig, st);
+        e = grouped ? (bias ? LAH_GATE_TOPK(true, true, true) : LAH_GATE_TOPK(false, true, true))
+                    : (bias ? LAH_GATE_TOPK(true, true, false) : LAH_GATE_TOPK(false, true, false));
     else
         return -4;
+#undef LAH_GATE_TOPK
     if (e || B <= 0) return e;
     rank_slots_kernel<<<gs.num_experts, 1024, 0, st>>>(idx, B * k, pos, counts);
     return -(int)cudaGetLastError();

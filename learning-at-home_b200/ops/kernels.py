@@ -44,7 +44,7 @@ def _lib():
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
-        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, I, Fl, P, P],
+        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, I, Fl, P, I, I, P],
         "lah_expert_bias_update": [P, I, I, P, Fl, P, P],
         "lah_layout_exchange": [L, L, I, I, I, I, I, I, I, P, P, P, P, P, P, P, I, Fl, I, P, P, P, P, P],
         "lah_scatter_rows": [P, P, P, P, P, P, L, L, I, I, I, I, I, I, I, I, P, P, P, P, P, I, P],
@@ -360,21 +360,44 @@ def _score_mode(what, score, scale, sig, n, device):
     return 1
 
 
+MAX_EXPERT_GROUPS = 64   # csrc MAX_GROUPS: the group mask of group-limited routing is one 64-bit word
+
+
+def check_expert_groups(what, E, n_group, topk_group, k=None):
+    """group-limited routing (DESIGN.md §6d): n_group must be an int in [1, 64] dividing E (and E <= LAYOUT_MAX_E when
+    n_group > 1), topk_group an int in [1, n_group]; with ``k``, k <= topk_group * E / n_group (else k pairs never fill)"""
+    for name, v in (("n_group", n_group), ("topk_group", topk_group)):
+        if not isinstance(v, int) or isinstance(v, bool):
+            raise ValueError(f"{what}: {name} must be an int, got {v!r}")
+    if not 1 <= n_group <= MAX_EXPERT_GROUPS or E % n_group:
+        raise ValueError(f"{what}: n_group must be in [1, {MAX_EXPERT_GROUPS}] and divide the {E} experts, got {n_group}")
+    if n_group > 1 and E > LAYOUT_MAX_E:
+        raise ValueError(f"{what}: group-limited routing scores at most {LAYOUT_MAX_E} experts, got {E}")
+    if not 1 <= topk_group <= n_group:
+        raise ValueError(f"{what}: topk_group must be in [1, n_group = {n_group}], got {topk_group}")
+    if k is not None and k > topk_group * (E // n_group):
+        raise ValueError(f"{what}: k = {k} experts cannot come from topk_group = {topk_group} groups of "
+                         f"{E // n_group} experts")
+
+
 def gate_topk(logits, grid_size, k, *, alive=None, failure_rate=0.0, seed=0, token_offset=0, idx, w, pos, counts,
-              bias=None, score="softmax", scale=1.0, sig=None):
+              bias=None, score="softmax", scale=1.0, sig=None, n_group=1, topk_group=1):
     """top-k routing of the grid logits (two launches).  ``bias``: float32 [prod(grid)] added to the selection key only
     (DESIGN.md §6b).  ``score="softmax"``: the weights are the softmax over the unbiased scores of the selected experts.
     ``score="sigmoid"`` (DeepSeek-V3, DESIGN.md §6c): the weights are scale * sigma_j / sum of sigma over the valid selected
-    pairs, the bias is added to sigma(s), and sigma_j of every pair goes to ``sig`` (float32 [B * k], 0 for a missing pair)"""
+    pairs, the bias is added to sigma(s), and sigma_j of every pair goes to ``sig`` (float32 [B * k], 0 for a missing pair).
+    ``n_group`` / ``topk_group`` (DeepSeek-V2/V3 group-limited routing, DESIGN.md §6d): the experts form n_group groups of
+    consecutive ids and each token picks its k experts from its topk_group best groups only"""
     B = logits.shape[0]
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.shape[1] == sum(grid_size)
     if bias is not None:
         _check_expert_bias("gate_topk", bias, math.prod(grid_size), logits.device)
     mode = _score_mode("gate_topk", score, scale, sig, B * k, logits.device)
+    check_expert_groups("gate_topk", math.prod(grid_size), n_group, topk_group)
     native.check(_lib().lah_gate_topk(ptr(logits), B, ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), k,
                                       ptr(alive), float(failure_rate), int(seed) & (2 ** 64 - 1), int(token_offset),
                                       ptr(idx), ptr(w), ptr(pos), ptr(counts), ptr(bias), mode, float(scale), ptr(sig),
-                                      stream_ptr()), "lah_gate_topk")
+                                      n_group, topk_group, stream_ptr()), "lah_gate_topk")
     native.count_launch(2)
 
 
@@ -1134,7 +1157,37 @@ def sigmoid_weights_ref(sel, valid, scale=1.0):
     return torch.where(S > 0, scale * sg / torch.where(S > 0, S, torch.ones_like(S)), torch.zeros_like(sg))
 
 
-def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, score="softmax", scale=1.0):
+def expert_group_scores_ref(scores, bias, n_group, score="softmax"):
+    """(score [B, G], has [B, G]) of group-limited routing (DESIGN.md §6d).  ``scores``: the float32 product-key scores
+    with -inf for the experts that are not candidates (dead or failure-injected).  A candidate's group key is the key the
+    selection ranks (s, s + b or sigma(s) + b), sigma(s) for the unbiased sigmoid router.  A group scores its largest key
+    (softmax) or the sum of its two largest (sigmoid; one candidate scores its key); ``has``: the group has a candidate."""
+    B, E = scores.shape
+    gsz = E // n_group
+    cand = torch.isfinite(scores)
+    base = torch.sigmoid(scores) if score == "sigmoid" else scores
+    key = base if bias is None else base + bias.to(device=scores.device, dtype=torch.float32).reshape(1, -1)
+    key = key.masked_fill(~cand, float("-inf")).view(B, n_group, gsz)
+    top = torch.sort(key, dim=-1, descending=True)[0]
+    gscore = top[..., 0]
+    if score == "sigmoid" and gsz > 1:
+        gscore = torch.where(torch.isfinite(top[..., 1]), top[..., 0] + top[..., 1], top[..., 0])
+    return gscore, cand.view(B, n_group, gsz).any(-1)
+
+
+def expert_group_mask_ref(scores, bias, n_group, topk_group, score="softmax"):
+    """[B, E] bool: the experts of each token's topk_group best groups (``expert_group_scores_ref``).  The groups are
+    sorted by score stably, descending, so equal scores go to the smaller id; a group without candidates is never taken."""
+    gscore, has = expert_group_scores_ref(scores, bias, n_group, score)
+    order = torch.sort(gscore.masked_fill(~has, float("-inf")), dim=-1, descending=True, stable=True)[1]
+    chosen = torch.zeros_like(has)
+    chosen.scatter_(1, order[:, :topk_group], True)
+    chosen &= has
+    return chosen.repeat_interleave(scores.shape[1] // n_group, dim=1)
+
+
+def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, score="softmax", scale=1.0, n_group=1,
+                  topk_group=1):
     """returns idx [B,k] (-1 for missing), weights [B,k] (softmax over alive selected).  Equal scores select the smaller
     expert id first, like gate_topk_kernel (torch.topk leaves the order of ties unspecified, so it sorts stably instead).
     The scores are summed first grid dimension first and the kernel last dimension first: on 3-d and 4-d grids they can
@@ -1142,16 +1195,21 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, s
     ``bias`` ([E]): the selection ranks the float32 keys score + bias[e]; the weights stay the softmax over the unbiased
     scores of the selected experts.
     ``score="sigmoid"`` (DESIGN.md §6c): the weights are ``sigmoid_weights_ref`` of the selected scores, and a bias is
-    added to sigmoid(score) in float32; without one the selection is the softmax router's."""
+    added to sigmoid(score) in float32; without one the selection is the softmax router's.
+    ``n_group`` / ``topk_group`` (DESIGN.md §6d): the candidates are narrowed to each token's topk_group best groups
+    (``expert_group_mask_ref``) before the selection; 1 / 1 and topk_group = n_group leave them as they are."""
     if score not in ROUTER_SCORES:
         raise ValueError(f"gate_topk_ref: score must be one of {ROUTER_SCORES}, got {score!r}")
     scores = product_key_scores(logits.float(), grid_size)
+    check_expert_groups("gate_topk_ref", scores.shape[-1], n_group, topk_group)
     dead = torch.zeros_like(scores, dtype=torch.bool)
     if alive is not None:
         dead |= ~alive.bool().view(1, -1)
     if fail_mask is not None:
         dead |= fail_mask
     scores = scores.masked_fill(dead, float("-inf"))
+    if topk_group < n_group:
+        scores = scores.masked_fill(~expert_group_mask_ref(scores, bias, n_group, topk_group, score), float("-inf"))
     if scores.shape[-1] < k:
         scores = F.pad(scores, (0, k - scores.shape[-1]), value=float("-inf"))
     if bias is None:

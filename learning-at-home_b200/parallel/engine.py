@@ -135,6 +135,12 @@ class DMoEConfig:
     # read at construction; a factor other than 1 needs "sigmoid"
     router_score: str = "softmax"
     routed_scaling_factor: float = 1.0
+    # group-limited routing (DESIGN.md §6d, DeepSeek-V2/V3 n_group / topk_group): the experts form n_group groups of
+    # consecutive flat ids, each group is scored per token (softmax: its best key; sigmoid: the sum of its two best), and a
+    # token picks its k experts from its topk_group best groups only.  With n_group = world (or a multiple), every group
+    # lives on one rank, so a token's pairs reach at most topk_group ranks.  Read at construction; 1 / 1 changes nothing
+    n_group: int = 1
+    topk_group: int = 1
     # shared-expert isolation (DESIGN.md §9c, DeepSeek-MoE / Qwen-MoE): every token also passes through one always-active
     # GatedFeedforwardBlock of this inner width, added to the combine of the routed experts with weight 1 and without a
     # second residual.  Its parameters are trainer-side (replicated on every rank, averaged over ranks, stepped once per
@@ -175,6 +181,7 @@ class DMoEConfig:
                              "router_score='sigmoid' does not have; set it to 0")
         if self.shared_inner_dim < 0:
             raise ValueError(f"DMoEConfig.shared_inner_dim must be >= 0, got {self.shared_inner_dim}")
+        K.check_expert_groups("DMoEConfig", self.num_experts, self.n_group, self.topk_group, self.k)
         if self.shared_inner_dim and self.expert != "swiglu":
             raise ValueError("DMoEConfig.shared_inner_dim: the shared expert is a GatedFeedforwardBlock and needs "
                              f"expert='swiglu', got expert={self.expert!r}")
@@ -265,6 +272,24 @@ def refuse_router_score(cfg: DMoEConfig, arm: str):
     if cfg.router_score != "softmax":
         raise ValueError(f"{arm} weights the selected experts with a softmax; set router_score='softmax' "
                          "(FusedDMoE / DMoETrainer route with sigmoid affinities)")
+
+
+def refuse_group_limited_routing(cfg: DMoEConfig, arm: str):
+    """the baseline arms route each token over all experts: refuse n_group > 1 instead of silently ignoring the limit"""
+    if cfg.n_group > 1:
+        raise ValueError(f"{arm} routes each token over all experts; set n_group=1 (FusedDMoE / DMoETrainer limit the "
+                         "routing to the topk_group best expert groups)")
+
+
+def max_groups_per_token(idx, k: int, num_experts: int, n_group: int) -> int:
+    """the most expert groups (of num_experts / n_group consecutive ids) any token's routed pairs reach; ``idx``: the
+    [B * k] or [B, k] expert ids of a gate, -1 for a missing pair.  0 for an empty batch"""
+    idx = idx.reshape(-1, k).long()
+    if idx.numel() == 0:
+        return 0
+    g = torch.where(idx >= 0, idx // (num_experts // n_group), torch.full_like(idx, n_group))
+    hit = torch.zeros(idx.shape[0], n_group + 1, dtype=torch.bool, device=idx.device).scatter_(1, g, True)
+    return int(hit[:, :n_group].sum(1).max())
 
 
 def refuse_shared_expert(cfg: DMoEConfig, arm: str):
@@ -885,6 +910,9 @@ class FusedDMoE(nn.Module):
         # the gate's weight function (cfg.router_score / routed_scaling_factor, read here once; DESIGN.md §6c)
         self.router_score = cfg.router_score
         self.routed_scale = float(cfg.routed_scaling_factor)
+        # group-limited routing (cfg.n_group / topk_group, read here once; DESIGN.md §6d)
+        self.n_group, self.topk_group = int(cfg.n_group), int(cfg.topk_group)
+        self._last_pairs = 0   # GPU path: routed pairs (B * k) of the last forward, whose ws.idx log_step reads
         # shared expert (cfg.shared_inner_dim, read here once): initialised like GatedFeedforwardBlock(hidden, I_s), drawn
         # from the global RNG like proj (DMoETrainer seeds it, so every rank starts identical), kept as the segments of
         # GATED_LAYOUT so that [W1; W3] is one GEMM operand and one contiguous gradient
@@ -969,7 +997,9 @@ class FusedDMoE(nn.Module):
         idx, w, pos, pair_row = ws.idx[:P], ws.w[:P], ws.pos[:P], ws.pair_row[:P]
         K.gate_topk(logits, self.grid_size, k, alive=c.alive, failure_rate=cfg.failure_rate if self.training else 0.0,
                     seed=cfg.seed * 7919 + self.layer_index, token_offset=c.token_counter, idx=idx, w=w, pos=pos,
-                    counts=c.counts, bias=self.expert_bias, **self._score_args(P))
+                    counts=c.counts, bias=self.expert_bias, n_group=self.n_group, topk_group=self.topk_group,
+                    **self._score_args(P))
+        self._last_pairs = P
         c.token_counter += B
         c.timer.mark("gate_topk")
         K.layout_exchange(c.cnt_all_off, c.flags_off, K.SLOT_COUNTS, epoch, c.E, c.E_loc, c.max_rows, align=c.align,
@@ -1258,7 +1288,8 @@ class FusedDMoE(nn.Module):
             fail_mask = torch.rand(x.shape[0], cfg.num_experts, device=x.device) < cfg.failure_rate
         alive = self.ctx.alive if self.ctx is not None else getattr(self, "alive_ref", None)
         idx, w_sel = K.gate_topk_ref(logits.detach(), self.grid_size, cfg.k, alive=alive, fail_mask=fail_mask,
-                                     bias=self.expert_bias, score=self.router_score, scale=self.routed_scale)
+                                     bias=self.expert_bias, score=self.router_score, scale=self.routed_scale,
+                                     n_group=self.n_group, topk_group=self.topk_group)
         if self.training and self.expert_bias is not None:
             with torch.no_grad():
                 counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)

@@ -20,7 +20,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops import kernels as K, native
-from .engine import DMoEConfig, EngineContext, DMoEClassifier
+from .engine import DMoEConfig, EngineContext, DMoEClassifier, max_groups_per_token
 
 
 class PendingLoss:
@@ -317,6 +317,9 @@ class DMoETrainer:
                     layer.update(router_aux_loss=aux, router_z_loss=z)
                 if block.expert_bias is not None:
                     layer["expert_bias_absmax"] = float(block.expert_bias.abs().max())
+                if block.n_group > 1:   # the user's check of the limit (at n_group = world: the most ranks a token reached)
+                    layer["max_groups_per_token"] = max_groups_per_token(
+                        block.ws.idx[:block._last_pairs], self.cfg.k, self.cfg.num_experts, block.n_group)
                 layers.append(layer)
             rec["layers"] = layers
             if self.last_stage_ms:

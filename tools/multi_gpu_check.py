@@ -35,11 +35,15 @@ def main():
     # a shared expert (trainer-side, replicated): its gradients summed over ranks against the whole-batch oracle, then
     # N trainer steps after which its parameters must hold the same bits on every rank
     shared = dict(shared_inner_dim=512) if "--shared-expert" in sys.argv else {}
+    # group-limited routing with one group per rank (DESIGN.md §6d): every token's pairs must reach exactly one rank, and
+    # the whole-batch oracle routes with the same limit
+    group = dict(n_group=world, topk_group=1) if "--group-limited" in sys.argv else {}
     swiglu = swiglu or bool(shared)
     mat, vec = ("w13", "g") if swiglu else ("w1", "b2")
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=B, capacity_factor=float(max(4, world)),
                        shadow_experts=4, shadow_tol=0.0 if force_shadow else 1.1, shadow_min_rows=1 if force_shadow else 64,
-                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router, **bias, **shared)
+                       expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router, **bias, **shared,
+                       **group)
     ctx = E.EngineContext(cfg)
     torch.manual_seed(0)  # identical gate on every rank (DMoETrainer does the same)
     layer = E.FusedDMoE(cfg, ctx).cuda()
@@ -51,6 +55,8 @@ def main():
     y.backward(g_all[rank * B: (rank + 1) * B].cuda())
     torch.cuda.synchronize()
     ctx.check_status()
+    # E_loc = E / world consecutive experts per rank, so with n_group = world a group is a rank
+    ranks_per_token = E.max_groups_per_token(layer.ws.idx[:B * cfg.k], cfg.k, cfg.num_experts, world)
     shadowed = int((layer.ws.shadow_info.view(-1, 4)[:, 0] >= 0).sum())
     # the kernel's hot-expert selection must equal the host model (parallel/balance.py) on the exchanged count table
     from lah_b200.parallel.balance import shadow_plan
@@ -123,6 +129,9 @@ def main():
         dist.all_gather(flats, flat)
         shared_ok = all(torch.equal(f, flats[0]) for f in flats)
         trainer.close()
+    rpt = torch.tensor([ranks_per_token], device="cuda")
+    dist.all_reduce(rpt, op=dist.ReduceOp.MAX)
+    group_ok = not group or int(rpt) == 1
     ok = True
     if rank == 0:
         # single-GPU reference in the same process: a fresh world-1 context is impossible inside an initialised group,
@@ -157,7 +166,9 @@ def main():
         ok = errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2 and errs["w1_mean_abs"] < 1e-4 and errs["b2_max_abs"] < 2.5e-3 and errs["steps"]
         ok = ok and (shadowed > 0 or not force_shadow) and plan_ok and errs.get("router_loss", 0.0) < 1e-4
         ok = ok and errs.get("router_grad_max_err", 0.0) < 1e-4 and bias_ok
-        ok = ok and errs.get("shared_grad", 0.0) < 8e-2 and shared_ok
+        ok = ok and errs.get("shared_grad", 0.0) < 8e-2 and shared_ok and group_ok
+        if group:
+            errs["max_ranks_per_token"] = int(rpt)
         if bias:
             errs["expert_bias_bit_identical_and_equal_to_oracle"] = bias_ok
         print("multi_gpu_check", dict(path="small" if small else "big", expert=cfg.expert, router_loss=bool(router), force_shadow=force_shadow, shadowed_experts=shadowed, plan_matches_host_model=plan_ok,
