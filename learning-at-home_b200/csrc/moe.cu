@@ -118,6 +118,68 @@ __device__ __forceinline__ void account_wait(const Peers& peers, unsigned long l
 // one function.  A score below about -87 gives 0 (the reciprocal of an exp beyond 2^126): such a pair has no affinity
 __device__ __forceinline__ float sigmoid_affinity(float s) { return __fdividef(1.f, 1.f + __expf(-s)); }
 
+// product-key score of expert c, summed last grid dimension first (the order of gate_topk_kernel)
+__device__ __forceinline__ float pk_score(const float* lg, const GridSpec& gs, int c) {
+    int rem = c;
+    float s = 0.f;
+#pragma unroll
+    for (int d = MAX_GRID_DIMS - 1; d >= 0; --d) {
+        if (d < gs.ndim) {
+            const int i = rem % gs.size[d];
+            rem /= gs.size[d];
+            s += lg[gs.offset[d] + i];
+        }
+    }
+    return s;
+}
+
+// running log-partition of the unnormalised softmax gate (DESIGN.md §6e): (m, l) = (largest score, sum of exp(s - m)).
+// A score of -inf adds nothing; (m, l) = (-inf, 0) is the empty sum
+__device__ __forceinline__ void lse_fold(float& m, float& l, float s) {
+    if (s > m) {
+        l = l * __expf(m - s) + 1.f;
+        m = s;
+    } else if (s > -INFINITY) {
+        l += __expf(s - m);
+    }
+}
+
+// merge with the lane `o` away (xor butterfly): both lanes form the same two products and one commutative add, so every
+// lane ends with the same bits
+__device__ __forceinline__ void lse_merge(float& m, float& l, int o) {
+    const float om = __shfl_xor_sync(0xffffffffu, m, o);
+    const float ol = __shfl_xor_sync(0xffffffffu, l, o);
+    const float M = fmaxf(m, om);
+    if (M > -INFINITY) l = l * __expf(m - M) + ol * __expf(om - M);
+    m = M;
+}
+
+// shared memory of one warp of router_loss_bwd_kernel (and of the dense pass of gate_bwd_kernel): the token's grid logits,
+// then (grids of 2+ dims) the expert gradients at skewed positions e + e / 32, so that lanes summing grid dimension 0
+// (experts i * stride + inner) do not all hit one bank
+__host__ __device__ __forceinline__ int router_bwd_warp_floats(const GridSpec& gs) {
+    return gs.total + (gs.ndim > 1 ? gs.num_experts + gs.num_experts / 32 + 1 : 0);
+}
+
+// grid logit o of a grid of 2+ dims: the sum of the staged expert terms g[e + e / 32] over the experts whose coordinate in
+// o's dimension is o's index, in increasing expert order (router_loss_bwd_kernel keeps its own copy of this loop, inlined
+// the way its SASS was measured)
+__device__ __forceinline__ float sum_expert_terms(const float* g, const GridSpec& gs, int o) {
+    int d = 0;
+    while (d + 1 < gs.ndim && o >= gs.offset[d + 1]) ++d;
+    const int i = o - gs.offset[d];
+    int stride = 1;   // expert id = row-major index over the grid: the last dimension varies fastest
+    for (int dd = gs.ndim - 1; dd > d; --dd) stride *= gs.size[dd];
+    const int block = stride * gs.size[d];
+    float acc = 0.f;
+    for (int outer = 0; outer < gs.num_experts; outer += block)
+        for (int inner = 0; inner < stride; ++inner) {
+            const int e = outer + i * stride + inner;
+            acc += g[e + (e >> 5)];
+        }
+    return acc;
+}
+
 // ------------------------------------------------------------------------------------------------
 // gate: one warp per token.  BIAS (auxiliary-loss-free balancing, DESIGN.md §6b): the top-k is taken over the keys
 // s_{b,e} + bias[e], while the weights use the unbiased values of the selected experts; each candidate carries both
@@ -130,6 +192,10 @@ __device__ __forceinline__ float sigmoid_affinity(float s) { return __fdividef(1
 // consecutive flat ids; a group pass scores every group (softmax: its largest key; sigmoid: the sum of its two largest,
 // sigma(s) without a bias), topk_group rounds of warp arg-max pick the best groups into a 64-bit mask, and the selection
 // loop skips the candidates outside it
+// !NORM (norm_topk_prob=False, DESIGN.md §6e): the weights are not renormalised over the selection.  Softmax: each lane
+// folds every live expert's score into a running (max, sum of exp) before the group and failure checks (those experts
+// stay in the partition), the warp merges the pairs with a fixed butterfly, z_b goes to lse_out and the weights are
+// scale * exp(s_j - z_b).  Sigmoid: the weights are scale * sigma_j
 // ------------------------------------------------------------------------------------------------
 constexpr int MAX_GROUPS = 64;
 constexpr int GROUP_WORDS = 2 * MAX_GROUPS;   // per-warp shared words of the grouped gate: group scores and flags
@@ -285,7 +351,7 @@ __device__ __forceinline__ void select_groups(const float* gscore, int* gvalid, 
     __syncwarp();
 }
 
-template <bool BIAS, bool SIGMOID, bool GROUPED>
+template <bool BIAS, bool SIGMOID, bool GROUPED, bool NORM>
 __global__ void __launch_bounds__(256, GROUPED ? 1 : 0) gate_topk_kernel(const float* __restrict__ logits, int B, GridSpec gs, int k,
                                                         const unsigned char* __restrict__ alive, float failure_rate,
                                                         unsigned long long seed, long long token_offset,
@@ -293,7 +359,8 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0) gate_topk_kernel(const f
                                                         int* __restrict__ pos_out, int* __restrict__ counts,
                                                         const int* __restrict__ step_ctr, const float* __restrict__ bias,
                                                         float scale, float* __restrict__ sig_out, int n_group,
-                                                        int topk_group) {
+                                                        int topk_group, float* __restrict__ lse_out) {
+    constexpr bool LSE = !NORM && !SIGMOID;   // the softmax over every live expert: its log-partition per token
     if (step_ctr) token_offset += *reinterpret_cast<const long long*>(step_ctr + 2);
     extern __shared__ float s_logits[];  // [8 warps][gs.total]; GROUPED: then [8 warps][GROUP_WORDS]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -324,23 +391,32 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0) gate_topk_kernel(const f
         best_u[j] = -INFINITY;
         best_i[j] = -1;
     }
+    float run_m = -INFINITY, run_l = 0.f;   // LSE: this lane's running (max, sum of exp) over its live experts
     for (int c = lane; c < gs.num_experts; c += 32) {
+        float s = 0.f;
+        if constexpr (LSE) {
+            // every live expert joins the partition; failures and unchosen groups are only excluded from the selection
+            if (alive && !alive[c]) continue;
+            s = pk_score(lg, gs, c);
+            lse_fold(run_m, run_l, s);
+        }
         if constexpr (GROUPED)
             if (!gsel[__umulhi(static_cast<unsigned>(c) << 1, gdiv)]) continue;
-        if (alive && !alive[c]) continue;
+        if (!LSE && alive && !alive[c]) continue;
         if (failure_rate > 0.f) {
             const unsigned long long key = seed ^ (static_cast<unsigned long long>(token_offset + b) * 0x100000001B3ull +
                                                    static_cast<unsigned long long>(c));
             if (hash_uniform(key) < failure_rate) continue;
         }
-        int rem = c;
-        float s = 0.f;
+        if constexpr (!LSE) {
+            int rem = c;
 #pragma unroll
-        for (int d = MAX_GRID_DIMS - 1; d >= 0; --d) {
-            if (d < gs.ndim) {
-                const int i = rem % gs.size[d];
-                rem /= gs.size[d];
-                s += lg[gs.offset[d] + i];
+            for (int d = MAX_GRID_DIMS - 1; d >= 0; --d) {
+                if (d < gs.ndim) {
+                    const int i = rem % gs.size[d];
+                    rem /= gs.size[d];
+                    s += lg[gs.offset[d] + i];
+                }
             }
         }
         float key = s, aff = s;
@@ -419,7 +495,8 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0) gate_topk_kernel(const f
             if (sel_i[j] >= 0) sg[j] = BIAS ? sel_v[j] : sigmoid_affinity(sel_v[j]);
             S += sg[j];
         }
-        const float norm = S > 0.f ? __fdividef(scale, S) : 0.f;   // every sigma underflowed: zero weights
+        // every sigma underflowed: zero weights.  !NORM: scale * sigma_j, not normalised
+        const float norm = !NORM ? scale : S > 0.f ? __fdividef(scale, S) : 0.f;
         if (lane < k) {
             int id = -1;
             float v = 0.f;
@@ -433,6 +510,28 @@ __global__ void __launch_bounds__(256, GROUPED ? 1 : 0) gate_topk_kernel(const f
             idx_out[o] = id;
             w_out[o] = v * norm;
             sig_out[o] = v;
+            if (id < 0) pos_out[o] = 0;
+        }
+        return;
+    }
+    if constexpr (LSE) {
+        // scale * p_j with p the softmax over every live expert: z_b = m + log(l) of the merged pair, 0 without a live score
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) lse_merge(run_m, run_l, o);
+        const float z = run_m > -INFINITY ? run_m + __logf(run_l) : 0.f;
+        if (lane == 0) lse_out[b] = z;
+        if (lane < k) {
+            int id = -1;
+            float v = 0.f;
+#pragma unroll
+            for (int j = 0; j < MAX_K; ++j)
+                if (j == lane) {
+                    id = sel_i[j];
+                    v = sel_v[j];
+                }
+            const long long o = static_cast<long long>(b) * k + lane;
+            idx_out[o] = id;
+            w_out[o] = id >= 0 ? scale * __expf(v - z) : 0.f;
             if (id < 0) pos_out[o] = 0;
         }
         return;
@@ -1048,10 +1147,19 @@ struct GateBwdArgs {
 };
 
 // SIGMOID: sig = sigma of every selected pair [B * k] (written by gate_topk), scale = the routed scaling factor.  They follow
-// gs rather than extend GateBwdArgs, which would move gs in the parameter bank of the softmax instantiations
-template <int VEC_PER_LANE, bool SIGMOID>
+// gs rather than extend GateBwdArgs, which would move gs in the parameter bank of the softmax instantiations.
+// !NORM (DESIGN.md §6e).  Sigmoid (w_j = scale sigma_j): dlogit_j = scale sigma_j (1 - sigma_j) dw_j.  Softmax (w_j = scale
+// p_j, p over every live expert): the selected pairs get w_j dw_j, and every live expert e gets the dense term
+// -p_e sum_i w_i dw_i with p_e = exp(s_e - lse[b]) from the token's grid logits (`logits`, staged in shared memory with
+// the expert terms, like router_loss_bwd_kernel).  On a 1-d grid a lane adds its experts' terms directly; otherwise grid
+// logit (d, i) is summed by one lane over the experts whose d-th coordinate is i, in increasing expert order.  A token with
+// sum_i w_i dw_i = 0 skips the dense pass
+template <int VEC_PER_LANE, bool SIGMOID, bool NORM>
 __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs a, GridSpec gs,
-                                                       const float* __restrict__ sig, float scale) {
+                                                       const float* __restrict__ sig, float scale,
+                                                       const float* __restrict__ logits, const float* __restrict__ lse,
+                                                       const unsigned char* __restrict__ alive) {
+    constexpr bool DENSE = !NORM && !SIGMOID;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * 8 + warp;
     if (b >= a.B) return;
@@ -1111,7 +1219,7 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
     __syncwarp();
     if (lane == 0) {
         float inv_s = 0.f;   // SIGMOID: 1 / S
-        if constexpr (SIGMOID) {
+        if constexpr (SIGMOID && NORM) {
             float S = 0.f;
 #pragma unroll
             for (int j = 0; j < MAX_K; ++j) S += sj[j];
@@ -1121,8 +1229,10 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
         for (int j = 0; j < MAX_K; ++j) {
             if (ej[j] < 0) continue;
             float d;
-            if constexpr (SIGMOID) d = sj[j] * (1.f - sj[j]) * (scale * dw[j] - dot_sum) * inv_s;
-            else d = wj[j] * (dw[j] - dot_sum);
+            if constexpr (SIGMOID && NORM) d = sj[j] * (1.f - sj[j]) * (scale * dw[j] - dot_sum) * inv_s;
+            else if constexpr (SIGMOID) d = scale * sj[j] * (1.f - sj[j]) * dw[j];
+            else if constexpr (NORM) d = wj[j] * (dw[j] - dot_sum);
+            else d = wj[j] * dw[j];
             int rem = ej[j];
             for (int dd = gs.ndim - 1; dd >= 0; --dd) {
                 const int i = rem % gs.size[dd];
@@ -1130,6 +1240,26 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
                 dl[gs.offset[dd] + i] += d;
             }
         }
+    }
+    if constexpr (DENSE) {
+        if (dot_sum == 0.f) return;   // the same value in every lane (warp_sum)
+        __syncwarp();
+        const float zb = lse[b];
+        const float* lgb = logits + static_cast<long long>(b) * gs.total;
+        if (gs.ndim == 1) {
+            for (int c = lane; c < gs.num_experts; c += 32)
+                if (!alive || alive[c]) dl[c] -= dot_sum * __expf(__ldg(lgb + c) - zb);
+            return;
+        }
+        extern __shared__ float s_gate_bwd[];   // [8 warps][router_bwd_warp_floats(gs)]
+        float* lg = s_gate_bwd + warp * router_bwd_warp_floats(gs);
+        float* g = lg + gs.total;
+        for (int i = lane; i < gs.total; i += 32) lg[i] = __ldg(lgb + i);
+        __syncwarp();
+        for (int c = lane; c < gs.num_experts; c += 32)
+            g[c + (c >> 5)] = !alive || alive[c] ? -dot_sum * __expf(pk_score(lg, gs, c) - zb) : 0.f;
+        __syncwarp();
+        for (int o = lane; o < gs.total; o += 32) dl[o] += sum_expert_terms(g, gs, o);
     }
 }
 
@@ -1260,21 +1390,6 @@ __global__ void __launch_bounds__(1024) expert_bias_update_kernel(const int* __r
     }
 }
 
-// product-key score of expert c, summed last grid dimension first (the order of gate_topk_kernel)
-__device__ __forceinline__ float pk_score(const float* lg, const GridSpec& gs, int c) {
-    int rem = c;
-    float s = 0.f;
-#pragma unroll
-    for (int d = MAX_GRID_DIMS - 1; d >= 0; --d) {
-        if (d < gs.ndim) {
-            const int i = rem % gs.size[d];
-            rem /= gs.size[d];
-            s += lg[gs.offset[d] + i];
-        }
-    }
-    return s;
-}
-
 // largest score of a live expert (-inf: none is finite), over the lanes of the warp
 __device__ __forceinline__ float router_max_score(const float* lg, const GridSpec& gs, const unsigned char* alive, int lane) {
     float mx = -INFINITY;
@@ -1387,13 +1502,6 @@ __global__ void __launch_bounds__(RL_WARPS * 32) router_loss_fwd_kernel(const fl
     }
 }
 
-// shared memory of one warp of router_loss_bwd_kernel: the token's grid logits, then (grids of 2+ dims) the expert
-// gradients at skewed positions e + e / 32, so that lanes summing grid dimension 0 (experts i * stride + inner) do not all
-// hit one bank
-__host__ __device__ __forceinline__ int router_bwd_warp_floats(const GridSpec& gs) {
-    return gs.total + (gs.ndim > 1 ? gs.num_experts + gs.num_experts / 32 + 1 : 0);
-}
-
 // one warp per token: dlogits[b] += d/dl of (aux_coef * L_aux + z_coef * L_z) with f constant.  The expert gradient is
 // g_e = p_e (aux_coef N (f_e - F_b) + 2 z_coef z_b) / B.  On a 1-d grid it is the logit's gradient itself and is added
 // directly; otherwise it is staged in shared memory and each grid logit (d, i) is summed by one lane over the experts
@@ -1460,22 +1568,41 @@ static Peers g_peers = {};
 static bool g_peers_set = false;
 
 // the launches of the gate and router-loss instantiations (lah_gate_topk / lah_router_loss_bwd pick one)
-template <bool BIAS, bool SIGMOID, bool GROUPED>
+template <bool BIAS, bool SIGMOID, bool GROUPED, bool NORM>
 static int launch_gate_topk(const float* logits, int B, const GridSpec& gs, int k, const unsigned char* alive,
                             float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w,
                             int* pos, int* counts, const float* bias, float scale, float* sig, int n_group,
-                            int topk_group, cudaStream_t st) {
+                            int topk_group, float* lse, cudaStream_t st) {
     // each of the 8 warps stages its token's grid logits in shared memory: 4096 of them (a dense gate over as many experts
     // as layout_exchange accepts) take 128 KB, above the 48 KB a launch gets without opting in.  GROUPED adds 512 B per
     // warp of group scores and flags
     const int group_floats = GROUPED ? GROUP_WORDS : 0;
-    if (int e = set_max_dynamic_smem<gate_topk_kernel<BIAS, SIGMOID, GROUPED>>(8 * sizeof(float) *
-                                                                               (LAYOUT_MAX_E + group_floats)))
+    if (int e = set_max_dynamic_smem<gate_topk_kernel<BIAS, SIGMOID, GROUPED, NORM>>(8 * sizeof(float) *
+                                                                                     (LAYOUT_MAX_E + group_floats)))
         return e;
     if (B <= 0) return 0;
-    gate_topk_kernel<BIAS, SIGMOID, GROUPED><<<(B + 7) / 8, 256, 8 * (gs.total + group_floats) * sizeof(float), st>>>(
+    gate_topk_kernel<BIAS, SIGMOID, GROUPED, NORM><<<(B + 7) / 8, 256, 8 * (gs.total + group_floats) * sizeof(float),
+                                                     st>>>(
         logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos, counts, g_peers.step_ctr, bias, scale, sig,
-        n_group, topk_group);
+        n_group, topk_group, lse);
+    return 0;
+}
+
+// the dense pass of gate_bwd_kernel (softmax, !NORM) stages router_bwd_warp_floats(gs) floats per warp on grids of 2+
+// dims; the most it takes: LAYOUT_MAX_E experts on 2 dims (LAYOUT_MAX_E / 2 + 2 grid logits)
+constexpr int GATE_BWD_DENSE_MAX_FLOATS = LAYOUT_MAX_E / 2 + 2 + LAYOUT_MAX_E + LAYOUT_MAX_E / 32 + 1;
+
+template <int V, bool SIGMOID, bool NORM>
+static int launch_gate_bwd(const GateBwdArgs& a, const GridSpec& gs, const float* sig, float scale, const float* logits,
+                           const float* lse, const unsigned char* alive, cudaStream_t st) {
+    int smem = 0;
+    if constexpr (!SIGMOID && !NORM) {
+        if (int e = set_max_dynamic_smem<gate_bwd_kernel<V, SIGMOID, NORM>>(8 * sizeof(float) *
+                                                                             GATE_BWD_DENSE_MAX_FLOATS))
+            return e;
+        if (gs.ndim > 1) smem = 8 * router_bwd_warp_floats(gs) * sizeof(float);
+    }
+    gate_bwd_kernel<V, SIGMOID, NORM><<<(a.B + 7) / 8, 256, smem, st>>>(g_peers, a, gs, sig, scale, logits, lse, alive);
     return 0;
 }
 
@@ -1586,38 +1713,47 @@ static int make_grid_spec(GridSpec* gs, const int* grid, int ndim) {
 }
 
 // bias: float [prod(grid)] added to the selection key only (DESIGN.md §6b); nullptr selects without one.
-// score_mode 0: softmax weights (scale must be 1, sig unused); 1: sigmoid weights scale * sigma_j / S with sigma_j of every
-// selected pair into sig [B * k] (DESIGN.md §6c).
+// score_mode 0: softmax weights (scale must be 1 when norm = 1, sig unused); 1: sigmoid weights scale * sigma_j / S with
+// sigma_j of every selected pair into sig [B * k] (DESIGN.md §6c).
 // n_group / topk_group (DESIGN.md §6d): each token picks its experts from the topk_group best of n_group groups of
-// consecutive expert ids; 1 / 1 (or topk_group = n_group) launches the ungrouped gate
+// consecutive expert ids; 1 / 1 (or topk_group = n_group) launches the ungrouped gate.
+// norm (DESIGN.md §6e): 1 renormalises the weights over the selection; 0 gives scale * p_j, with p the softmax over every
+// live expert and its log-partition z_b into lse [B] (score_mode 0; lse must be nullptr otherwise), or scale * sigma_j
 int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, const unsigned char* alive,
                   float failure_rate, unsigned long long seed, long long token_offset, int* idx, float* w, int* pos,
                   int* counts, const float* bias, int score_mode, float scale, float* sig, int n_group, int topk_group,
-                  cudaStream_t st) {
+                  int norm, float* lse, cudaStream_t st) {
     GridSpec gs;
     if (make_grid_spec(&gs, grid, ndim)) return -2;
     if (k < 1 || k > MAX_K) return -3;
     if (gs.total > LAYOUT_MAX_E) return -2;
     if (bias && gs.num_experts > LAYOUT_MAX_E) return -2;
-    if (score_mode == 0 && scale != 1.f) return -5;
-    if (score_mode == 1 && (!(scale > 0.f && scale <= FLT_MAX) || !sig)) return -5;
+    if (norm != 0 && norm != 1) return -5;
+    if (score_mode == 0 && norm && scale != 1.f) return -5;
+    if (score_mode == 0 && !norm && (!(scale > 0.f && scale <= FLT_MAX) || (!lse && B > 0))) return -5;
+    if (lse && (norm || score_mode != 0)) return -5;
+    if (score_mode == 1 && (!(scale > 0.f && scale <= FLT_MAX) || (!sig && B > 0))) return -5;   // B = 0: nullptr
     if (n_group < 1 || n_group > MAX_GROUPS || gs.num_experts % n_group) return -6;
     if (n_group > 1 && gs.num_experts > LAYOUT_MAX_E) return -6;
     if (topk_group < 1 || topk_group > n_group) return -6;
     const bool grouped = topk_group < n_group;
     int e;
-#define LAH_GATE_TOPK(BIAS, SIGMOID, GROUPED)                                                                          \
-    launch_gate_topk<BIAS, SIGMOID, GROUPED>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w, pos,  \
-                                             counts, BIAS ? bias : nullptr, SIGMOID ? scale : 1.f,                    \
-                                             SIGMOID ? sig : nullptr, n_group, topk_group, st)
+#define LAH_GATE_TOPK(BIAS, SIGMOID, GROUPED, NORM)                                                                    \
+    launch_gate_topk<BIAS, SIGMOID, GROUPED, NORM>(logits, B, gs, k, alive, failure_rate, seed, token_offset, idx, w,  \
+                                                   pos, counts, BIAS ? bias : nullptr,                                 \
+                                                   SIGMOID || !NORM ? scale : 1.f, SIGMOID ? sig : nullptr, n_group,   \
+                                                   topk_group, NORM ? nullptr : lse, st)
+#define LAH_GATE_TOPK_N(BIAS, SIGMOID, GROUPED) \
+    (norm ? LAH_GATE_TOPK(BIAS, SIGMOID, GROUPED, true) : LAH_GATE_TOPK(BIAS, SIGMOID, GROUPED, false))
     if (score_mode == 0)
-        e = grouped ? (bias ? LAH_GATE_TOPK(true, false, true) : LAH_GATE_TOPK(false, false, true))
-                    : (bias ? LAH_GATE_TOPK(true, false, false) : LAH_GATE_TOPK(false, false, false));
+        e = grouped ? (bias ? LAH_GATE_TOPK_N(true, false, true) : LAH_GATE_TOPK_N(false, false, true))
+                    : (bias ? LAH_GATE_TOPK_N(true, false, false) : LAH_GATE_TOPK_N(false, false, false));
     else if (score_mode == 1)
-        e = grouped ? (bias ? LAH_GATE_TOPK(true, true, true) : LAH_GATE_TOPK(false, true, true))
-                    : (bias ? LAH_GATE_TOPK(true, true, false) : LAH_GATE_TOPK(false, true, false));
+        e = grouped ? (bias ? LAH_GATE_TOPK_N(true, true, true) : LAH_GATE_TOPK_N(false, true, true))
+                    : (bias ? LAH_GATE_TOPK_N(true, true, false) : LAH_GATE_TOPK_N(false, true, false));
     else
         return -4;
+#undef LAH_GATE_TOPK_N
 #undef LAH_GATE_TOPK
     if (e || B <= 0) return e;
     rank_slots_kernel<<<gs.num_experts, 1024, 0, st>>>(idx, B * k, pos, counts);
@@ -1692,28 +1828,38 @@ int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, con
     return -(int)cudaGetLastError();
 }
 
-// sig: nullptr for the softmax gate; the sigma array of the sigmoid gate (DESIGN.md §6c), whose weights carry scale
+// sig: nullptr for the softmax gate; the sigma array of the sigmoid gate (DESIGN.md §6c), whose weights carry scale.
+// norm (DESIGN.md §6e): 0 for the gate_topk call with norm = 0.  The softmax gate then also needs its grid logits [B,
+// prod(grid) <= LAYOUT_MAX_E], its lse [B] and the alive table (nullptr: every expert is live); the other gates take none
 int lah_gate_bwd(long long yo_off, const void* grad, const int* idx, const int* pair_row, const float* w,
                  float* dlogits, int B, int k, int H, int E_loc, const int* grid_sizes, int ndim, const int* route_owner,
-                 const float* sig, float scale, cudaStream_t st) {
+                 const float* sig, float scale, int norm, const float* lse, const float* logits,
+                 const unsigned char* alive, cudaStream_t st) {
     if (!g_peers_set) return -10;
+    const bool dense = !sig && norm == 0;
+    if (norm != 0 && norm != 1) return -5;
+    if (dense ? B > 0 && (!lse || !logits) : lse || logits || alive) return -5;   // B = 0: empty arrays are nullptr
     if (B <= 0) return 0;
     GridSpec gs;
     if (make_grid_spec(&gs, grid_sizes, ndim)) return -2;
     if (k > MAX_K) return -3;
-    if (sig ? !(scale > 0.f && scale <= FLT_MAX) : scale != 1.f) return -5;
+    if (sig || dense ? !(scale > 0.f && scale <= FLT_MAX) : scale != 1.f) return -5;
+    if (dense && (gs.num_experts > LAYOUT_MAX_E || router_bwd_warp_floats(gs) > GATE_BWD_DENSE_MAX_FLOATS)) return -2;
     GateBwdArgs a;
     a.yo_off = yo_off; a.grad = (const bf16*)grad; a.idx = idx; a.pair_row = pair_row; a.w = w; a.dlogits = dlogits;
     a.B = B; a.k = k; a.H = H; a.E_loc = E_loc; a.route_owner = route_owner;
-    const int grid = (B + 7) / 8;
-#define LAH_GATE_BWD(V)                                                                \
-    if (sig) gate_bwd_kernel<V, true><<<grid, 256, 0, st>>>(g_peers, a, gs, sig, scale);  \
-    else gate_bwd_kernel<V, false><<<grid, 256, 0, st>>>(g_peers, a, gs, nullptr, 1.f);
+    int e;
+#define LAH_GATE_BWD(V)                                                                                     \
+    e = sig ? (norm ? launch_gate_bwd<V, true, true>(a, gs, sig, scale, nullptr, nullptr, nullptr, st)      \
+                    : launch_gate_bwd<V, true, false>(a, gs, sig, scale, nullptr, nullptr, nullptr, st))    \
+            : (norm ? launch_gate_bwd<V, false, true>(a, gs, nullptr, 1.f, nullptr, nullptr, nullptr, st)   \
+                    : launch_gate_bwd<V, false, false>(a, gs, nullptr, scale, logits, lse, alive, st));
     if (H == 256) { LAH_GATE_BWD(1) }
     else if (H == 512) { LAH_GATE_BWD(2) }
     else if (H == 1024) { LAH_GATE_BWD(4) }
     else return -2;
 #undef LAH_GATE_BWD
+    if (e) return e;
     return -(int)cudaGetLastError();
 }
 

@@ -44,7 +44,7 @@ def _lib():
         "lah_ln_relu_fwd_q": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_set_peers": [P, I, I],
         "lah_set_wait_counter": [P],
-        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, I, Fl, P, I, I, P],
+        "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, I, Fl, P, I, I, I, P, P],
         "lah_expert_bias_update": [P, I, I, P, Fl, P, P],
         "lah_layout_exchange": [L, L, I, I, I, I, I, I, I, P, P, P, P, P, P, P, I, Fl, I, P, P, P, P, P],
         "lah_scatter_rows": [P, P, P, P, P, P, L, L, I, I, I, I, I, I, I, I, P, P, P, P, P, I, P],
@@ -52,7 +52,7 @@ def _lib():
         "lah_zero_slots": [P, I, P, I, I, I, I, P],
         "lah_signal_wait": [L, I, I, I, I, P, P],
         "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P, P],
-        "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P, Fl, P],
+        "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P, Fl, I, P, P, P, P],
         "lah_router_loss_fwd": [P, I, P, I, P, P, I, P, P, P, P, P, P, I, P],
         "lah_router_loss_bwd": [P, I, P, I, P, P, P, P, Fl, Fl, P, I, P],
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
@@ -342,16 +342,23 @@ def _check_expert_bias(what, bias, E, device):
 ROUTER_SCORES = ("softmax", "sigmoid")   # the weight functions of the gate (DESIGN.md §6c), in csrc score_mode order
 
 
-def _score_mode(what, score, scale, sig, n, device):
-    """csrc score_mode of ``score``; checks ``scale`` and the sigma array ``sig`` (float32, >= n entries) before any launch"""
+def _score_mode(what, score, scale, sig, n, device, norm=True):
+    """csrc score_mode of ``score``; checks ``scale`` and the sigma array ``sig`` (float32, >= n entries) before any launch.
+    The softmax gate takes a scale other than 1 only with ``norm=False`` (DESIGN.md §6e)"""
     if score not in ROUTER_SCORES:
         raise ValueError(f"{what}: score must be one of {ROUTER_SCORES}, got {score!r}")
+    if not isinstance(norm, bool):
+        raise ValueError(f"{what}: norm must be a bool, got {norm!r}")
     scale = float(scale)
     if score == "softmax":
-        if scale != 1.0 or sig is not None:
-            raise ValueError(f"{what}: the softmax gate takes neither a scale ({scale}) nor a sig array")
-        return 0
+        if sig is not None:
+            raise ValueError(f"{what}: the softmax gate takes no sig array")
+        if norm and scale != 1.0:
+            raise ValueError(f"{what}: the normalised softmax gate takes no scale ({scale}); use norm=False")
     if not math.isfinite(scale) or scale <= 0.0:
+        raise ValueError(f"{what}: scale must be a finite value > 0, got {scale}")
+    if score == "softmax":
+        return 0
         raise ValueError(f"{what}: scale must be a finite value > 0, got {scale}")
     if sig is None or sig.dtype != torch.float32 or not sig.is_contiguous() or sig.numel() < n or sig.device != device:
         got = "None" if sig is None else f"{sig.dtype} {tuple(sig.shape)} on {sig.device}"
@@ -380,24 +387,40 @@ def check_expert_groups(what, E, n_group, topk_group, k=None):
                          f"{E // n_group} experts")
 
 
+def _check_lse(what, lse, n, device, needed):
+    """the float32 log-partition array of the unnormalised softmax gate: >= n entries when ``needed``, else None"""
+    if not needed:
+        if lse is not None:
+            raise ValueError(f"{what}: lse belongs to the unnormalised softmax gate (score='softmax', norm=False)")
+        return
+    if lse is None or lse.dtype != torch.float32 or not lse.is_contiguous() or lse.numel() < n or lse.device != device:
+        got = "None" if lse is None else f"{lse.dtype} {tuple(lse.shape)} on {lse.device}"
+        raise ValueError(f"{what}: the unnormalised softmax gate needs lse, a contiguous float32 tensor of >= {n} "
+                         f"entries on {device}, got {got}")
+
+
 def gate_topk(logits, grid_size, k, *, alive=None, failure_rate=0.0, seed=0, token_offset=0, idx, w, pos, counts,
-              bias=None, score="softmax", scale=1.0, sig=None, n_group=1, topk_group=1):
+              bias=None, score="softmax", scale=1.0, sig=None, n_group=1, topk_group=1, norm=True, lse=None):
     """top-k routing of the grid logits (two launches).  ``bias``: float32 [prod(grid)] added to the selection key only
     (DESIGN.md §6b).  ``score="softmax"``: the weights are the softmax over the unbiased scores of the selected experts.
     ``score="sigmoid"`` (DeepSeek-V3, DESIGN.md §6c): the weights are scale * sigma_j / sum of sigma over the valid selected
     pairs, the bias is added to sigma(s), and sigma_j of every pair goes to ``sig`` (float32 [B * k], 0 for a missing pair).
     ``n_group`` / ``topk_group`` (DeepSeek-V2/V3 group-limited routing, DESIGN.md §6d): the experts form n_group groups of
-    consecutive ids and each token picks its k experts from its topk_group best groups only"""
+    consecutive ids and each token picks its k experts from its topk_group best groups only.
+    ``norm=False`` (norm_topk_prob=False, DESIGN.md §6e): the weights are not renormalised over the selection.  Softmax:
+    scale * p_j with p the softmax over every live expert (failed and unchosen-group experts included), whose
+    log-partition z_b goes to ``lse`` (float32 [B]); sigmoid: scale * sigma_j"""
     B = logits.shape[0]
     assert logits.dtype == torch.float32 and logits.is_contiguous() and logits.shape[1] == sum(grid_size)
     if bias is not None:
         _check_expert_bias("gate_topk", bias, math.prod(grid_size), logits.device)
-    mode = _score_mode("gate_topk", score, scale, sig, B * k, logits.device)
+    mode = _score_mode("gate_topk", score, scale, sig, B * k, logits.device, norm)
+    _check_lse("gate_topk", lse, B, logits.device, score == "softmax" and not norm)
     check_expert_groups("gate_topk", math.prod(grid_size), n_group, topk_group)
     native.check(_lib().lah_gate_topk(ptr(logits), B, ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), k,
                                       ptr(alive), float(failure_rate), int(seed) & (2 ** 64 - 1), int(token_offset),
                                       ptr(idx), ptr(w), ptr(pos), ptr(counts), ptr(bias), mode, float(scale), ptr(sig),
-                                      n_group, topk_group, stream_ptr()), "lah_gate_topk")
+                                      n_group, topk_group, int(norm), ptr(lse), stream_ptr()), "lah_gate_topk")
     native.count_launch(2)
 
 
@@ -503,15 +526,37 @@ def combine_rows_ref(src, idx, pair_row, w=None, addend=None):
 
 
 def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route_owner=None, *, score="softmax",
-             scale=1.0, sig=None):
+             scale=1.0, sig=None, norm=True, lse=None, alive=None, logits=None):
     """gradient of the grid logits from the combine's (one launch).  ``score="sigmoid"``: the gate's ``sig`` array and
-    ``scale`` of the same forward (DESIGN.md §6c)"""
+    ``scale`` of the same forward (DESIGN.md §6c).  ``norm=False`` (DESIGN.md §6e): the gate ran with norm=False; the
+    softmax gate then also needs the forward's grid ``logits`` (float32 [B, sum(grid)]), its ``lse`` and the ``alive``
+    table it routed with, and adds the dense term -p_e sum_j w_j dw_j of every live expert"""
     B, H = grad.shape
     assert grad.is_contiguous() and grad.dtype == torch.bfloat16 and dlogits.dtype == torch.float32
-    _score_mode("gate_bwd", score, scale, sig, B * k, grad.device)
+    _score_mode("gate_bwd", score, scale, sig, B * k, grad.device, norm)
+    dense = score == "softmax" and not norm
+    _check_lse("gate_bwd", lse, B, grad.device, dense)
+    E = math.prod(grid_size)
+    if not dense:
+        if logits is not None or alive is not None:
+            raise ValueError("gate_bwd: logits and alive belong to the unnormalised softmax gate (norm=False)")
+    else:
+        if logits is None or logits.dtype != torch.float32 or not logits.is_contiguous() or logits.device != grad.device \
+                or tuple(logits.shape) != (B, sum(grid_size)):
+            got = "None" if logits is None else f"{logits.dtype} {tuple(logits.shape)} on {logits.device}"
+            raise ValueError(f"gate_bwd: the unnormalised softmax gate needs logits, a contiguous float32 "
+                             f"[{B}, {sum(grid_size)}] tensor on {grad.device}, got {got}")
+        if alive is not None and (alive.dtype != torch.uint8 or alive.numel() != E or not alive.is_contiguous()
+                                  or alive.device != grad.device):
+            raise ValueError(f"gate_bwd: alive must be a contiguous uint8 tensor of {E} entries on {grad.device}")
+        if E > LAYOUT_MAX_E or (len(grid_size) > 1 and sum(grid_size) + E + E // 32 + 1 > GATE_BWD_DENSE_MAX_FLOATS):
+            raise ValueError(f"gate_bwd: the unnormalised softmax gate takes at most {LAYOUT_MAX_E} experts (and "
+                             f"{GATE_BWD_DENSE_MAX_FLOATS - LAYOUT_MAX_E - LAYOUT_MAX_E // 32 - 1} grid logits on a "
+                             f"grid of 2+ dims), got grid {tuple(grid_size)}")
     native.check(_lib().lah_gate_bwd(yo_off, ptr(grad), ptr(idx), ptr(pair_row), ptr(w), ptr(dlogits), B, k, H, E_loc,
                                      ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), ptr(route_owner),
-                                     ptr(sig), float(scale), stream_ptr()),
+                                     ptr(sig), float(scale), int(norm), ptr(lse), ptr(logits), ptr(alive),
+                                     stream_ptr()),
                  "lah_gate_bwd")
     native.count_launch()
     return dlogits
@@ -522,6 +567,8 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
 # ---------------------------------------------------------------------------------------------------------
 MAX_GRID_DIMS = 4        # csrc/moe.cu MAX_GRID_DIMS
 LAYOUT_MAX_E = 4096      # csrc/moe.cu LAYOUT_MAX_E: most experts (and grid logits) of a gate
+# csrc GATE_BWD_DENSE_MAX_FLOATS: the shared memory per token of the dense pass of the unnormalised softmax gate_bwd
+GATE_BWD_DENSE_MAX_FLOATS = LAYOUT_MAX_E // 2 + 2 + LAYOUT_MAX_E + LAYOUT_MAX_E // 32 + 1
 ROUTER_WARPS = 4         # tokens per CTA of the router-loss kernels
 
 
@@ -1157,6 +1204,28 @@ def sigmoid_weights_ref(sel, valid, scale=1.0):
     return torch.where(S > 0, scale * sg / torch.where(S > 0, S, torch.ones_like(S)), torch.zeros_like(sg))
 
 
+def softmax_lse_ref(scores, alive=None):
+    """[B] log-partition z_b of the softmax over the live experts (DESIGN.md §6a / §6e): logsumexp of ``scores`` [B, E]
+    over the experts with ``alive`` (uint8 [E], None: all); 0 for a token without a finite live score.  Differentiable"""
+    live = torch.ones(scores.shape[-1], dtype=torch.bool, device=scores.device) if alive is None \
+        else alive.bool().reshape(-1).to(scores.device)
+    masked = scores.masked_fill(~live.view(1, -1), float("-inf"))
+    ok = torch.isfinite(masked).any(-1, keepdim=True)
+    z = torch.logsumexp(torch.where(ok, masked, torch.zeros_like(masked)), -1, keepdim=True)
+    return torch.where(ok, z, torch.zeros_like(z)).squeeze(-1)
+
+
+def softmax_weights_ref(scores, idx, alive=None, scale=1.0):
+    """weights of the unnormalised softmax router (norm_topk_prob=False, DESIGN.md §6e): scale * p_{b, idx} with p the
+    softmax of ``scores`` [B, E] over the live experts (``softmax_lse_ref``), 0 for a missing pair (idx -1).  The
+    selection does not enter the partition: failed experts and experts outside the chosen groups stay in it.
+    Differentiable in ``scores``"""
+    z = softmax_lse_ref(scores, alive)
+    sel = torch.gather(scores, 1, idx.clamp(min=0))
+    valid = idx >= 0
+    return torch.where(valid, scale * torch.exp(sel.masked_fill(~valid, 0.0) - z.unsqueeze(-1)), torch.zeros_like(sel))
+
+
 def expert_group_scores_ref(scores, bias, n_group, score="softmax"):
     """(score [B, G], has [B, G]) of group-limited routing (DESIGN.md §6d).  ``scores``: the float32 product-key scores
     with -inf for the experts that are not candidates (dead or failure-injected).  A candidate's group key is the key the
@@ -1187,7 +1256,7 @@ def expert_group_mask_ref(scores, bias, n_group, topk_group, score="softmax"):
 
 
 def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, score="softmax", scale=1.0, n_group=1,
-                  topk_group=1):
+                  topk_group=1, norm=True):
     """returns idx [B,k] (-1 for missing), weights [B,k] (softmax over alive selected).  Equal scores select the smaller
     expert id first, like gate_topk_kernel (torch.topk leaves the order of ties unspecified, so it sorts stably instead).
     The scores are summed first grid dimension first and the kernel last dimension first: on 3-d and 4-d grids they can
@@ -1197,10 +1266,13 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, s
     ``score="sigmoid"`` (DESIGN.md §6c): the weights are ``sigmoid_weights_ref`` of the selected scores, and a bias is
     added to sigmoid(score) in float32; without one the selection is the softmax router's.
     ``n_group`` / ``topk_group`` (DESIGN.md §6d): the candidates are narrowed to each token's topk_group best groups
-    (``expert_group_mask_ref``) before the selection; 1 / 1 and topk_group = n_group leave them as they are."""
+    (``expert_group_mask_ref``) before the selection; 1 / 1 and topk_group = n_group leave them as they are.
+    ``norm=False`` (DESIGN.md §6e): the same selection, weighted by ``softmax_weights_ref`` (softmax) or scale * sigma_j
+    (sigmoid), without renormalisation."""
     if score not in ROUTER_SCORES:
         raise ValueError(f"gate_topk_ref: score must be one of {ROUTER_SCORES}, got {score!r}")
     scores = product_key_scores(logits.float(), grid_size)
+    raw = scores
     check_expert_groups("gate_topk_ref", scores.shape[-1], n_group, topk_group)
     dead = torch.zeros_like(scores, dtype=torch.bool)
     if alive is not None:
@@ -1222,6 +1294,11 @@ def gate_topk_ref(logits, grid_size, k, alive=None, fail_mask=None, bias=None, s
         top_i = torch.sort(keys, dim=-1, descending=True, stable=True)[1][..., :k]
         top_v = torch.gather(scores, -1, top_i)
     valid = torch.isfinite(top_v)
+    top_i = torch.where(valid, top_i, torch.full_like(top_i, -1))
+    if not norm and score == "softmax":
+        return top_i, softmax_weights_ref(raw, top_i, alive, scale)   # valid ids < E: padding never enters
+    if not norm:
+        return top_i, torch.where(valid, scale * torch.sigmoid(top_v.masked_fill(~valid, 0.0)), torch.zeros_like(top_v))
     if score == "sigmoid":
         w = sigmoid_weights_ref(top_v.masked_fill(~valid, 0.0), valid, scale)
         return torch.where(valid, top_i, torch.full_like(top_i, -1)), w

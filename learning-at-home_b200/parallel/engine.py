@@ -141,6 +141,11 @@ class DMoEConfig:
     # lives on one rank, so a token's pairs reach at most topk_group ranks.  Read at construction; 1 / 1 changes nothing
     n_group: int = 1
     topk_group: int = 1
+    # renormalise the selected weights (DESIGN.md §6e, HF norm_topk_prob).  False weights each selected expert by its
+    # unnormalised router probability, times routed_scaling_factor: "softmax" uses p = the softmax over every live expert
+    # (Switch, GShard, DeepSeek-V2, Qwen-MoE; at k = 1 the router then trains through the task loss), "sigmoid" uses
+    # sigma(s) (DeepSeek-V3 with norm_topk_prob=False).  Read at construction; True changes nothing
+    norm_topk_prob: bool = True
     # shared-expert isolation (DESIGN.md §9c, DeepSeek-MoE / Qwen-MoE): every token also passes through one always-active
     # GatedFeedforwardBlock of this inner width, added to the combine of the routed experts with weight 1 and without a
     # second residual.  Its parameters are trainer-side (replicated on every rank, averaged over ranks, stepped once per
@@ -173,9 +178,11 @@ class DMoEConfig:
         v = float(self.routed_scaling_factor)
         if not math.isfinite(v) or v <= 0.0:
             raise ValueError(f"DMoEConfig.routed_scaling_factor must be a finite value > 0, got {v}")
-        if v != 1.0 and self.router_score != "sigmoid":
+        if not isinstance(self.norm_topk_prob, bool):
+            raise ValueError(f"DMoEConfig.norm_topk_prob must be a bool, got {self.norm_topk_prob!r}")
+        if v != 1.0 and self.router_score != "sigmoid" and self.norm_topk_prob:
             raise ValueError("DMoEConfig.routed_scaling_factor scales the normalised sigmoid weights; with "
-                             f"router_score={self.router_score!r} it must be 1, got {v}")
+                             f"router_score={self.router_score!r} it must be 1, got {v} (or set norm_topk_prob=False)")
         if self.router_score == "sigmoid" and self.router_z_loss_coef > 0.0:
             raise ValueError("DMoEConfig.router_z_loss_coef: the z-loss penalises the softmax log-partition, which "
                              "router_score='sigmoid' does not have; set it to 0")
@@ -272,6 +279,15 @@ def refuse_router_score(cfg: DMoEConfig, arm: str):
     if cfg.router_score != "softmax":
         raise ValueError(f"{arm} weights the selected experts with a softmax; set router_score='softmax' "
                          "(FusedDMoE / DMoETrainer route with sigmoid affinities)")
+    if not cfg.norm_topk_prob:
+        raise ValueError(f"{arm} renormalises the weights over the selected experts; set norm_topk_prob=True "
+                         "(FusedDMoE / DMoETrainer weight them by their unnormalised router probabilities)")
+
+
+def dense_gate_backward(cfg: DMoEConfig) -> bool:
+    """the unnormalised softmax router (DESIGN.md §6e): every live expert's probability depends on every score, so the
+    gate backward reads the logits and the log-partition of the forward"""
+    return cfg.router_score == "softmax" and not cfg.norm_topk_prob
 
 
 def refuse_group_limited_routing(cfg: DMoEConfig, arm: str):
@@ -765,6 +781,9 @@ class LayerWorkspace:
         self.total_rows = torch.zeros(1, **i32)
         # the sigmoid router (DESIGN.md §6c): sigma of every selected pair, written by gate_topk and read by gate_bwd
         self.sig = torch.zeros(P, **f32) if cfg.router_score == "sigmoid" else None
+        # the unnormalised softmax router (DESIGN.md §6e): each token's log-partition z_b, written by gate_topk and read by
+        # gate_bwd
+        self.lse = torch.zeros(cfg.tokens_per_rank, **f32) if dense_gate_backward(cfg) else None
         self.router_loss = None
         if cfg.router_losses:
             # router losses: f (box-wide routing shares, snapshotted from the count table the next layer overwrites, then
@@ -814,9 +833,10 @@ class _FusedDMoEFunction(torch.autograd.Function):
         ctx.tracked = bool(x.requires_grad or logits.requires_grad)
         ws.outstanding = ctx.tracked
         ctx.router = layer.training and layer.router_on
+        ctx.dense = layer.dense_gate   # the gate backward of the unnormalised softmax reads the logits too
         ctx.shared = layer.shared_inner > 0   # the shared expert's norm backward reads the layer input
-        if ctx.router or ctx.shared:
-            ctx.save_for_backward(*([logits] if ctx.router else []), *([x] if ctx.shared else []))
+        if ctx.router or ctx.dense or ctx.shared:
+            ctx.save_for_backward(*([logits] if ctx.router or ctx.dense else []), *([x] if ctx.shared else []))
         return layer._forward_cuda(x, logits)
 
     @staticmethod
@@ -824,9 +844,9 @@ class _FusedDMoEFunction(torch.autograd.Function):
         if not ctx.layer.ws.outstanding:
             raise RuntimeError("FusedDMoE: backward() without a pending forward (the workspace was released or reused)")
         saved = ctx.saved_tensors
-        logits = saved[0] if ctx.router else None
+        logits = saved[0] if ctx.router or ctx.dense else None
         x = saved[-1] if ctx.shared else None
-        dx, dlogits = ctx.layer._backward_cuda(grad_out.contiguous(), ctx.B, logits, x)
+        dx, dlogits = ctx.layer._backward_cuda(grad_out.contiguous(), ctx.B, logits, x, router=ctx.router)
         ctx.layer.ws.outstanding = False
         ec = ctx.layer.ctx
         if ec._opt_pending and not ec.defer_join:
@@ -870,6 +890,10 @@ class FusedDMoE(nn.Module):
             # the workspace (the sigma array of the sigmoid gate) is allocated from the context's configuration
             raise ValueError(f"FusedDMoE: router_score={cfg.router_score!r} needs an EngineContext built with the same "
                              f"router_score, got {ctx.cfg.router_score!r}")
+        if ctx is not None and cfg.norm_topk_prob != ctx.cfg.norm_topk_prob:
+            # the workspace (the log-partition array of the unnormalised softmax gate) follows the context's configuration
+            raise ValueError(f"FusedDMoE: norm_topk_prob={cfg.norm_topk_prob!r} needs an EngineContext built with the "
+                             f"same norm_topk_prob, got {ctx.cfg.norm_topk_prob!r}")
         self.cfg, self.ctx, self.layer_index = cfg, ctx, layer_index
         self.grid_size = tuple(cfg.grid_size)
         if cfg.gate_mode == "emulator":
@@ -910,6 +934,9 @@ class FusedDMoE(nn.Module):
         # the gate's weight function (cfg.router_score / routed_scaling_factor, read here once; DESIGN.md §6c)
         self.router_score = cfg.router_score
         self.routed_scale = float(cfg.routed_scaling_factor)
+        # unnormalised weights (cfg.norm_topk_prob, read here once; DESIGN.md §6e)
+        self.norm_topk_prob = bool(cfg.norm_topk_prob)
+        self.dense_gate = dense_gate_backward(cfg)
         # group-limited routing (cfg.n_group / topk_group, read here once; DESIGN.md §6d)
         self.n_group, self.topk_group = int(cfg.n_group), int(cfg.topk_group)
         self._last_pairs = 0   # GPU path: routed pairs (B * k) of the last forward, whose ws.idx log_step reads
@@ -998,7 +1025,7 @@ class FusedDMoE(nn.Module):
         K.gate_topk(logits, self.grid_size, k, alive=c.alive, failure_rate=cfg.failure_rate if self.training else 0.0,
                     seed=cfg.seed * 7919 + self.layer_index, token_offset=c.token_counter, idx=idx, w=w, pos=pos,
                     counts=c.counts, bias=self.expert_bias, n_group=self.n_group, topk_group=self.topk_group,
-                    **self._score_args(P))
+                    **self._score_args(P, B))
         self._last_pairs = P
         c.token_counter += B
         c.timer.mark("gate_topk")
@@ -1058,11 +1085,16 @@ class FusedDMoE(nn.Module):
         c.timer.mark("combine")
         return y
 
-    def _score_args(self, P):
-        """the weight-function keywords of K.gate_topk / K.gate_bwd for P routed pairs (none for the softmax gate)"""
-        if self.router_score == "softmax":
-            return {}
-        return dict(score=self.router_score, scale=self.routed_scale, sig=self.ws.sig[:P])
+    def _score_args(self, P, B):
+        """the weight-function keywords of K.gate_topk / K.gate_bwd for P routed pairs of B tokens (none for the default
+        softmax gate)"""
+        args = {} if self.router_score == "softmax" else dict(score=self.router_score, scale=self.routed_scale,
+                                                               sig=self.ws.sig[:P])
+        if not self.norm_topk_prob:
+            args.update(norm=False, scale=self.routed_scale)
+            if self.dense_gate:
+                args["lse"] = self.ws.lse[:B]
+        return args
 
     def _expert_plan(self):
         """swap-AB groups of 16 rows on the small path (backward GEMMs on ``chain_ctas``), 128-row tiles on the big one"""
@@ -1124,9 +1156,11 @@ class FusedDMoE(nn.Module):
         K.rms_norm_bwd(dn[:B], x, ws.shared_rstd[:B], self.shared_g.detach(), dx=dxs, dgamma=self.shared_g.grad)
         return dxs
 
-    def _backward_cuda(self, gy, B, logits=None, x=None):
-        """:param logits: the gate logits of the forward when it computed router losses (their gradient is added here)
-        :param x: the layer input of the forward, when the layer has a shared expert"""
+    def _backward_cuda(self, gy, B, logits=None, x=None, router=False):
+        """:param logits: the gate logits of the forward when it computed router losses or the layer has the dense gate
+        backward of the unnormalised softmax router
+        :param x: the layer input of the forward, when the layer has a shared expert
+        :param router: the forward computed router losses (their gradient is added here)"""
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         k = cfg.k
         P = B * k
@@ -1134,9 +1168,10 @@ class FusedDMoE(nn.Module):
         idx, w, pos, pair_row = ws.idx[:P], ws.w[:P], ws.pos[:P], ws.pair_row[:P]
         gy = gy.to(torch.bfloat16)
         dlogits = torch.empty(B, sum(self.grid_size), dtype=torch.float32, device=gy.device)
+        dense = dict(alive=c.alive, logits=logits) if self.dense_gate else {}
         K.gate_bwd(ws.yo_off, gy, idx, pair_row, w, dlogits, k, c.E_loc, self.grid_size, route_owner=ws.route_owner,
-                   **self._score_args(P))
-        if logits is not None:
+                   **self._score_args(P, B), **dense)
+        if router:
             K.router_loss_bwd(logits, self.grid_size, alive=c.alive, f=ws.router_f, z=ws.router_z, Fb=ws.router_F,
                               aux_coef=self.router_aux_coef * self.router_grad_scale,
                               z_coef=self.router_z_coef * self.router_grad_scale, dlogits=dlogits,
@@ -1294,10 +1329,16 @@ class FusedDMoE(nn.Module):
             with torch.no_grad():
                 counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
                 self.expert_bias.copy_(K.expert_bias_update_ref(counts, self.expert_bias, self.expert_bias_rate, alive))
-        # differentiable weights: softmax over the selected logits, or their normalised sigmoid affinities
+        # differentiable weights: softmax over the selected logits, or their normalised sigmoid affinities; without
+        # renormalisation the softmax over every live expert, or the sigmoid affinities, times the scale (DESIGN.md §6e)
         scores = K.product_key_scores(logits, self.grid_size)
         safe_idx = idx.clamp(min=0)
-        if self.router_score == "sigmoid":
+        if not self.norm_topk_prob and self.router_score == "softmax":
+            weights = K.softmax_weights_ref(scores, idx, alive, self.routed_scale)
+        elif not self.norm_topk_prob:
+            sg = torch.sigmoid(torch.gather(scores, 1, safe_idx))
+            weights = torch.where(idx >= 0, self.routed_scale * sg, torch.zeros_like(sg))
+        elif self.router_score == "sigmoid":
             weights = K.sigmoid_weights_ref(torch.gather(scores, 1, safe_idx), idx >= 0, self.routed_scale)
         else:
             sel = torch.gather(scores, 1, safe_idx).masked_fill(idx < 0, float("-inf"))

@@ -320,6 +320,9 @@ class DMoETrainer:
                 if block.n_group > 1:   # the user's check of the limit (at n_group = world: the most ranks a token reached)
                     layer["max_groups_per_token"] = max_groups_per_token(
                         block.ws.idx[:block._last_pairs], self.cfg.k, self.cfg.num_experts, block.n_group)
+                if not block.norm_topk_prob and block._last_pairs:   # the router mass the top k carries (DESIGN.md §6e)
+                    layer["routed_weight_mean"] = float(
+                        block.ws.w[:block._last_pairs].view(-1, self.cfg.k).sum(1).mean())
                 layers.append(layer)
             rec["layers"] = layers
             if self.last_stage_ms:
