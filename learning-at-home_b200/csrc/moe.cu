@@ -627,6 +627,21 @@ struct LayoutArgs {
 
 constexpr int LAYOUT_MAX_E = 4096;
 
+// expert capacity (DESIGN.md §6f): C = max(1, ceil(f * P / E)) in float64, P the routed pairs of the count table.  Rank r
+// keeps the first kept(r, e) = clamp(C - sum_{s<r} cnt(s, e), 0, cnt(r, e)) of its pairs of expert e (rank-major, then
+// token order).  !CAP: every pair is kept
+template <bool CAP>
+__device__ __forceinline__ int kept_rows(const int* cnt_all, int E, int r, int e, int cap) {
+    const int c = cnt_all[static_cast<long long>(r) * E + e];
+    if constexpr (!CAP) {
+        return c;
+    } else {
+        int before = 0;
+        for (int s = 0; s < r; ++s) before += cnt_all[static_cast<long long>(s) * E + e];
+        return max(0, min(cap - before, c));
+    }
+}
+
 // Load balancing.  Expert popularity is heavily skewed once training starts (a handful of experts receive most rows),
 // so a static expert -> GPU placement leaves most GPUs idle behind the owner of a hot expert.  After the count exchange
 // every rank knows the full [rank][expert] histogram and runs the SAME greedy selection: while the most loaded rank
@@ -634,7 +649,12 @@ constexpr int LAYOUT_MAX_E = 4096;
 // every rank processes its own rows with a replica of the expert's weights (pulled from the owner over NVLink, see
 // pull_shadow_kernel) in one of its S_max shadow groups, and the owner's optimizer sums the partial weight gradients of
 // all ranks (adam.cu).  Shadowing an expert spreads its rows exactly like the tokens are spread (data parallel).
-__global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, LayoutArgs a) {
+// CAP (expert capacity, DESIGN.md §6f): every table below is derived from the kept counts, computed on the fly from the
+// count table (which the router losses and the bias update read unchanged); keep[e] = kept(me, e) tells scatter_rows which
+// pairs to send, cap_stats = (C, box-wide dropped pairs)
+template <bool CAP>
+__global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, LayoutArgs a, double cap_factor, int* keep,
+                                                               int* cap_stats) {
     __shared__ int warp_tot[32];
     __shared__ int owner_base_s[MAX_WORLD + 1];
     __shared__ int s_tot[LAYOUT_MAX_E];
@@ -682,15 +702,37 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
     if (tid < MAX_WORLD * 2) s_shadow[tid] = -1;
     __syncthreads();
     const int* cnt_all = reinterpret_cast<const int*>(peers.base[me] + a.cnt_all_off);
+    int cap = 0;
+    long long routed = 0;
+    if constexpr (CAP) {   // P = every routed pair of the box (the rows [0, world) of the count table are contiguous)
+        int part = 0;
+        for (int i = tid; i < world * a.E; i += blockDim.x) part += cnt_all[i];
+        part = __reduce_add_sync(0xffffffffu, part);
+        if (lane == 0) warp_tot[warp] = part;
+        __syncthreads();
+        for (int w = 0; w < 32; ++w) routed += warp_tot[w];
+        const double c = ceil(cap_factor * static_cast<double>(routed) / static_cast<double>(a.E));
+        cap = c >= 2147483647.0 ? 2147483647 : max(1, static_cast<int>(c));
+        __syncthreads();   // warp_tot is the scan's scratch below
+    }
     // 3. totals per expert and the initial load of every rank (= rows of the experts it owns)
     for (int e = tid; e < a.E; e += blockDim.x) {
         int tot = 0;
         for (int s = 0; s < world; ++s) tot += cnt_all[static_cast<long long>(s) * a.E + e];
+        if constexpr (CAP) tot = min(tot, cap);
         s_tot[e] = tot;
         s_slot[e] = -1;
         if (tot) atomicAdd(reinterpret_cast<unsigned long long*>(&s_load[e / a.E_loc]), static_cast<unsigned long long>(tot));
     }
     __syncthreads();
+    if constexpr (CAP) {
+        if (tid == 0) {   // the kept pairs are the loads before any shadowing
+            long long kept = 0;
+            for (int r = 0; r < world; ++r) kept += s_load[r];
+            cap_stats[0] = cap;
+            cap_stats[1] = static_cast<int>(routed - kept);
+        }
+    }
     // 4. greedy shadow selection (identical on every rank: same inputs, deterministic tie-breaks)
     int num_shadow = 0;
     for (int it = 0; it < a.S_max && world > 1; ++it) {
@@ -747,7 +789,7 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
                 s_slot[i] = static_cast<short>(it);
                 s_shadow[it] = i;
                 s_load[rmax] -= v;
-                for (int r = 0; r < world; ++r) s_load[r] += cnt_all[static_cast<long long>(r) * a.E + i];
+                for (int r = 0; r < world; ++r) s_load[r] += kept_rows<CAP>(cnt_all, a.E, r, i, cap);
             }
         }
         __syncthreads();
@@ -764,10 +806,12 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
         int rows = 0, before = 0;
         if (e < a.E) {
             if (s_slot[e] >= 0) {
-                rows = cnt_all[static_cast<long long>(e / a.E_loc) * a.E + e];
+                rows = CAP ? kept_rows<true>(cnt_all, a.E, e / a.E_loc, e, cap)
+                           : cnt_all[static_cast<long long>(e / a.E_loc) * a.E + e];
             } else {
                 rows = s_tot[e];
                 for (int s = 0; s < me; ++s) before += cnt_all[static_cast<long long>(s) * a.E + e];
+                if constexpr (CAP) before = min(before, cap);
             }
         }
         const int padded = (rows + a.align - 1) / a.align * a.align;
@@ -807,14 +851,14 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
         int cur = owner_base_s[me + 1] - owner_base_s[me];
         for (int s = 0; s < a.S_max; ++s) {
             const int e = s_shadow[s];
-            const int rows = (e >= 0 && e / a.E_loc != me) ? cnt_all[static_cast<long long>(me) * a.E + e] : 0;
+            const int rows = (e >= 0 && e / a.E_loc != me) ? kept_rows<CAP>(cnt_all, a.E, me, e, cap) : 0;
             const int padded = (rows + a.align - 1) / a.align * a.align;
             a.group_off[G_own + s] = cur;
             a.group_rows[G_own + s] = rows;
             for (int t = cur / a.tile_rows; t < (cur + padded) / a.tile_rows && t < a.max_tiles; ++t) a.tile_group[t] = G_own + s;
             int mask = 0;
             if (e >= 0)
-                for (int r = 0; r < world; ++r) mask |= (cnt_all[static_cast<long long>(r) * a.E + e] > 0) << r;
+                for (int r = 0; r < world; ++r) mask |= (kept_rows<CAP>(cnt_all, a.E, r, e, cap) > 0) << r;
             a.shadow_info[4 * s + 0] = e;
             a.shadow_info[4 * s + 1] = e >= 0 ? e / a.E_loc : -1;
             a.shadow_info[4 * s + 2] = rows;
@@ -829,7 +873,7 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
         for (int s = 0; s < a.S_max; ++s) {
             const int e = s_shadow[s];
             if (e >= 0 && e / a.E_loc != tid)
-                total += (cnt_all[static_cast<long long>(tid) * a.E + e] + a.align - 1) / a.align * a.align;
+                total += (kept_rows<CAP>(cnt_all, a.E, tid, e, cap) + a.align - 1) / a.align * a.align;
         }
         if (total > a.max_rows) atomicOr(a.status, STATUS_OVERFLOW);
     }
@@ -850,7 +894,7 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
             if (a.owned_shadow) {
                 int mask = 0;
                 if (slot >= 0)
-                    for (int r = 0; r < world; ++r) mask |= (cnt_all[static_cast<long long>(r) * a.E + e] > 0) << r;
+                    for (int r = 0; r < world; ++r) mask |= (kept_rows<CAP>(cnt_all, a.E, r, e, cap) > 0) << r;
                 a.owned_shadow[2 * le] = slot;
                 a.owned_shadow[2 * le + 1] = mask;
             }
@@ -868,6 +912,7 @@ __global__ void __launch_bounds__(1024) layout_exchange_kernel(Peers peers, Layo
         }
         a.dst_row[e] = dst;
         if (a.route_owner) a.route_owner[e] = route;
+        if constexpr (CAP) keep[e] = kept_rows<true>(cnt_all, a.E, me, e, cap);
     }
 }
 
@@ -896,15 +941,19 @@ struct ScatterArgs {
     int* status;
 };
 
-template <int VEC_PER_LANE>
-__global__ void __launch_bounds__(256) scatter_rows_kernel(Peers peers, ScatterArgs a) {
+// CAP (forward dispatch with an expert capacity, DESIGN.md §6f): a pair at or past keep[e] (layout_exchange) is dropped:
+// pair_row -1, nothing sent, no overflow
+template <int VEC_PER_LANE, bool CAP>
+__global__ void __launch_bounds__(256) scatter_rows_kernel(Peers peers, ScatterArgs a, const int* __restrict__ keep) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (static_cast<int>(blockIdx.x) < a.pair_blocks) {
         const int p = blockIdx.x * 8 + warp;
         if (p < a.num_pairs) {
             const int e = a.idx[p];
             int row = -1;
-            if (e >= 0) {
+            bool kept = e >= 0;
+            if constexpr (CAP) kept = kept && a.pos[p] < keep[e];
+            if (kept) {
                 row = (a.pair_row && !a.dst_row) ? a.pair_row[p] : a.dst_row[e] + a.pos[p];
                 if (row >= a.max_rows) {
                     if (lane == 0) atomicOr(a.status, STATUS_OVERFLOW);
@@ -1059,8 +1108,12 @@ struct CombineArgs {
     const int* route_owner;   // [E] rank that holds MY rows of expert e (nullptr: e / E_loc)
 };
 
-template <int VEC_PER_LANE, bool ADD>
-__global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineArgs a, const bf16* __restrict__ addend) {
+// PASS (expert capacity, DESIGN.md §6f): a routed pair that scatter_rows dropped (idx >= 0, pair_row -1) sees its expert
+// as the identity and adds pass_w[p] * self[b] in its place (forward: self = x, backward: self = the output gradient;
+// pass_w = the gate weights in both)
+template <int VEC_PER_LANE, bool ADD, bool PASS>
+__global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineArgs a, const bf16* __restrict__ addend,
+                                                           const bf16* __restrict__ self, const float* __restrict__ pass_w) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (a.do_signal || a.do_wait) a.epoch = epoch_of(peers, a.epoch);
     if (a.do_signal && blockIdx.x == 0 && threadIdx.x < 32) {
@@ -1100,10 +1153,16 @@ __global__ void __launch_bounds__(256) combine_rows_kernel(Peers peers, CombineA
         const long long p = static_cast<long long>(b) * a.k + j;
         const int e = a.idx[p];
         const int row = a.pair_row[p];
-        if (e < 0 || row < 0) continue;
-        const float w = a.w ? a.w[p] : 1.f;
-        const int4* sp = reinterpret_cast<const int4*>(peers.base[a.route_owner ? a.route_owner[e] : e / a.E_loc] + a.src_off) +
-                         static_cast<long long>(row) * (a.H / 8);
+        if constexpr (PASS) {
+            if (e < 0) continue;
+        } else {
+            if (e < 0 || row < 0) continue;
+        }
+        const float w = PASS && row < 0 ? pass_w[p] : (a.w ? a.w[p] : 1.f);
+        const int4* sp = PASS && row < 0
+                             ? reinterpret_cast<const int4*>(self + static_cast<long long>(b) * a.H)
+                             : reinterpret_cast<const int4*>(peers.base[a.route_owner ? a.route_owner[e] : e / a.E_loc] +
+                                                             a.src_off) + static_cast<long long>(row) * (a.H / 8);
 #pragma unroll
         for (int v = 0; v < VEC_PER_LANE; ++v) {
             const int4 q = ld_v4(sp + v * 32 + lane);
@@ -1154,11 +1213,14 @@ struct GateBwdArgs {
 // the expert terms, like router_loss_bwd_kernel).  On a 1-d grid a lane adds its experts' terms directly; otherwise grid
 // logit (d, i) is summed by one lane over the experts whose d-th coordinate is i, in increasing expert order.  A token with
 // sum_i w_i dw_i = 0 skips the dense pass
-template <int VEC_PER_LANE, bool SIGMOID, bool NORM>
+// PASS (expert capacity, DESIGN.md §6f): a pair that scatter_rows dropped saw its expert as the identity (y_j = x_b), so
+// dw_j = <g_b, x_b> with x the layer input [B, H]; every formula above then holds as it is
+template <int VEC_PER_LANE, bool SIGMOID, bool NORM, bool PASS>
 __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs a, GridSpec gs,
                                                        const float* __restrict__ sig, float scale,
                                                        const float* __restrict__ logits, const float* __restrict__ lse,
-                                                       const unsigned char* __restrict__ alive) {
+                                                       const unsigned char* __restrict__ alive,
+                                                       const bf16* __restrict__ x_self) {
     constexpr bool DENSE = !NORM && !SIGMOID;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * 8 + warp;
@@ -1194,9 +1256,11 @@ __global__ void __launch_bounds__(256) gate_bwd_kernel(Peers peers, GateBwdArgs 
                 ej[j] = e;
                 if constexpr (SIGMOID) sj[j] = sig[p];
             }
-            if (e >= 0 && row >= 0) {
-                const int4* sp = reinterpret_cast<const int4*>(peers.base[a.route_owner ? a.route_owner[e] : e / a.E_loc] + a.yo_off) +
-                                 static_cast<long long>(row) * (a.H / 8);
+            if (e >= 0 && (PASS || row >= 0)) {
+                const int4* sp = PASS && row < 0
+                                     ? reinterpret_cast<const int4*>(x_self + static_cast<long long>(b) * a.H)
+                                     : reinterpret_cast<const int4*>(peers.base[a.route_owner ? a.route_owner[e] : e / a.E_loc] + a.yo_off) +
+                                           static_cast<long long>(row) * (a.H / 8);
                 float d = 0.f;
 #pragma unroll
                 for (int v = 0; v < VEC_PER_LANE; ++v) {
@@ -1592,17 +1656,18 @@ static int launch_gate_topk(const float* logits, int B, const GridSpec& gs, int 
 // dims; the most it takes: LAYOUT_MAX_E experts on 2 dims (LAYOUT_MAX_E / 2 + 2 grid logits)
 constexpr int GATE_BWD_DENSE_MAX_FLOATS = LAYOUT_MAX_E / 2 + 2 + LAYOUT_MAX_E + LAYOUT_MAX_E / 32 + 1;
 
-template <int V, bool SIGMOID, bool NORM>
+template <int V, bool SIGMOID, bool NORM, bool PASS>
 static int launch_gate_bwd(const GateBwdArgs& a, const GridSpec& gs, const float* sig, float scale, const float* logits,
-                           const float* lse, const unsigned char* alive, cudaStream_t st) {
+                           const float* lse, const unsigned char* alive, const bf16* x_self, cudaStream_t st) {
     int smem = 0;
     if constexpr (!SIGMOID && !NORM) {
-        if (int e = set_max_dynamic_smem<gate_bwd_kernel<V, SIGMOID, NORM>>(8 * sizeof(float) *
-                                                                             GATE_BWD_DENSE_MAX_FLOATS))
+        if (int e = set_max_dynamic_smem<gate_bwd_kernel<V, SIGMOID, NORM, PASS>>(8 * sizeof(float) *
+                                                                                   GATE_BWD_DENSE_MAX_FLOATS))
             return e;
         if (gs.ndim > 1) smem = 8 * router_bwd_warp_floats(gs) * sizeof(float);
     }
-    gate_bwd_kernel<V, SIGMOID, NORM><<<(a.B + 7) / 8, 256, smem, st>>>(g_peers, a, gs, sig, scale, logits, lse, alive);
+    gate_bwd_kernel<V, SIGMOID, NORM, PASS><<<(a.B + 7) / 8, 256, smem, st>>>(g_peers, a, gs, sig, scale, logits, lse,
+                                                                              alive, x_self);
     return 0;
 }
 
@@ -1763,9 +1828,12 @@ int lah_gate_topk(const float* logits, int B, const int* grid, int ndim, int k, 
 int lah_layout_exchange(long long cnt_all_off, long long flags_off, int slot, int epoch, int E, int E_loc, int max_rows,
                         int align, int tile_rows, int* counts, int* dst_row, int* group_off, int* group_rows, int* tile_group, int* total_rows,
                         int* status, int S_max, float shadow_tol, int min_shadow_rows, int* route_owner, int* step_rows,
-                        int* shadow_info, int* owned_shadow, cudaStream_t st) {
+                        int* shadow_info, int* owned_shadow, double cap_factor, int* keep, int* cap_stats,
+                        cudaStream_t st) {
     if (!g_peers_set) return -10;
     if (E > LAYOUT_MAX_E || S_max < 0 || S_max > 2 * MAX_WORLD) return -2;
+    // cap_factor 0: dropless.  > 0 (finite): the expert capacity of DESIGN.md §6f, with keep [E] and cap_stats [2]
+    if (!(cap_factor >= 0.0 && cap_factor <= DBL_MAX) || (cap_factor > 0.0) != (keep && cap_stats)) return -5;
     LayoutArgs a;
     a.cnt_all_off = cnt_all_off; a.flags_off = flags_off; a.slot = slot; a.epoch = epoch; a.E = E; a.E_loc = E_loc;
     if (tile_rows <= 0 || align % tile_rows) return -2;
@@ -1773,14 +1841,16 @@ int lah_layout_exchange(long long cnt_all_off, long long flags_off, int slot, in
     a.group_rows = group_rows; a.tile_group = tile_group; a.total_rows = total_rows; a.status = status;
     a.S_max = S_max; a.shadow_tol = shadow_tol; a.min_shadow_rows = min_shadow_rows; a.route_owner = route_owner;
     a.step_rows = step_rows; a.shadow_info = shadow_info; a.owned_shadow = owned_shadow;
-    layout_exchange_kernel<<<1, 1024, 0, st>>>(g_peers, a);
+    if (cap_factor > 0.0) layout_exchange_kernel<true><<<1, 1024, 0, st>>>(g_peers, a, cap_factor, keep, cap_stats);
+    else layout_exchange_kernel<false><<<1, 1024, 0, st>>>(g_peers, a, 0.0, nullptr, nullptr);
     return -(int)cudaGetLastError();
 }
 
 int lah_scatter_rows(const void* src, const float* scale, const int* idx, const int* pos, const int* dst_row,
                      int* pair_row, long long dst_off, long long flags_off, int slot, int epoch, int num_pairs, int k,
                      int H, int E_loc, int max_rows, int align, const int* group_off, const int* group_rows,
-                     int* done_counter, int* status, const int* route_owner, int num_groups, cudaStream_t st) {
+                     int* done_counter, int* status, const int* route_owner, int num_groups, const int* keep,
+                     cudaStream_t st) {
     if (!g_peers_set) return -10;
     ScatterArgs a;
     a.src = (const bf16*)src; a.scale = scale; a.idx = idx; a.pos = pos; a.dst_row = dst_row; a.pair_row = pair_row;
@@ -1788,12 +1858,17 @@ int lah_scatter_rows(const void* src, const float* scale, const int* idx, const 
     a.H = H; a.E_loc = E_loc; a.max_rows = max_rows; a.group_off = group_off; a.group_rows = group_rows;
     a.pair_blocks = (num_pairs + 7) / 8; a.align = align; a.done_counter = done_counter; a.status = status;
     a.route_owner = route_owner; a.num_groups = num_groups > 0 ? num_groups : E_loc;
+    if (keep && (!dst_row || !pair_row)) return -3;   // the capacity drops pairs in the forward dispatch only
     const int pad_blocks = a.num_groups < 64 ? a.num_groups : 64;
     const int grid = a.pair_blocks + pad_blocks;
-    if (H == 256) scatter_rows_kernel<1><<<grid, 256, 0, st>>>(g_peers, a);
-    else if (H == 512) scatter_rows_kernel<2><<<grid, 256, 0, st>>>(g_peers, a);
-    else if (H == 1024) scatter_rows_kernel<4><<<grid, 256, 0, st>>>(g_peers, a);
+#define LAH_SCATTER(V)                                                             \
+    if (keep) scatter_rows_kernel<V, true><<<grid, 256, 0, st>>>(g_peers, a, keep); \
+    else scatter_rows_kernel<V, false><<<grid, 256, 0, st>>>(g_peers, a, nullptr);
+    if (H == 256) { LAH_SCATTER(1) }
+    else if (H == 512) { LAH_SCATTER(2) }
+    else if (H == 1024) { LAH_SCATTER(4) }
     else return -2;
+#undef LAH_SCATTER
     return -(int)cudaGetLastError();
 }
 
@@ -1807,8 +1882,10 @@ int lah_signal_wait(long long flags_off, int slot, int epoch, int do_signal, int
 // addend: optional bf16 [B, H] added to every output row before its one rounding (nullptr: the plain kernel)
 int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, const float* w, void* out, int B, int k,
                      int H, int E_loc, long long flags_off, int slot, int epoch, int do_signal, int do_wait, int* status,
-                     const int* route_owner, const void* addend, cudaStream_t st) {
+                     const int* route_owner, const void* addend, const void* pass_self, const float* pass_w,
+                     cudaStream_t st) {
     if (!g_peers_set) return -10;
+    if (!pass_self != !pass_w) return -5;
     if (B <= 0) return 0;
     CombineArgs a;
     a.src_off = src_off; a.idx = idx; a.pair_row = pair_row; a.w = w; a.out = (bf16*)out; a.B = B; a.k = k; a.H = H;
@@ -1816,10 +1893,14 @@ int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, con
     a.status = status; a.route_owner = route_owner;
     const int grid = (B + 7) / 8;
     const bf16* add = (const bf16*)addend;
+    const bf16* self = (const bf16*)pass_self;
     if (add && (reinterpret_cast<uintptr_t>(add) % 16)) return -3;   // read as 16-byte vectors
-#define LAH_COMBINE(V)                                                                   \
-    if (add) combine_rows_kernel<V, true><<<grid, 256, 0, st>>>(g_peers, a, add);        \
-    else combine_rows_kernel<V, false><<<grid, 256, 0, st>>>(g_peers, a, nullptr);
+    if (self && (reinterpret_cast<uintptr_t>(self) % 16)) return -3;
+#define LAH_COMBINE(V)                                                                                         \
+    if (self && add) combine_rows_kernel<V, true, true><<<grid, 256, 0, st>>>(g_peers, a, add, self, pass_w);  \
+    else if (self) combine_rows_kernel<V, false, true><<<grid, 256, 0, st>>>(g_peers, a, nullptr, self, pass_w); \
+    else if (add) combine_rows_kernel<V, true, false><<<grid, 256, 0, st>>>(g_peers, a, add, nullptr, nullptr); \
+    else combine_rows_kernel<V, false, false><<<grid, 256, 0, st>>>(g_peers, a, nullptr, nullptr, nullptr);
     if (H == 256) { LAH_COMBINE(1) }
     else if (H == 512) { LAH_COMBINE(2) }
     else if (H == 1024) { LAH_COMBINE(4) }
@@ -1834,9 +1915,11 @@ int lah_combine_rows(long long src_off, const int* idx, const int* pair_row, con
 int lah_gate_bwd(long long yo_off, const void* grad, const int* idx, const int* pair_row, const float* w,
                  float* dlogits, int B, int k, int H, int E_loc, const int* grid_sizes, int ndim, const int* route_owner,
                  const float* sig, float scale, int norm, const float* lse, const float* logits,
-                 const unsigned char* alive, cudaStream_t st) {
+                 const unsigned char* alive, const void* pass_x, cudaStream_t st) {
     if (!g_peers_set) return -10;
     const bool dense = !sig && norm == 0;
+    const bf16* px = (const bf16*)pass_x;
+    if (px && (reinterpret_cast<uintptr_t>(px) % 16)) return -3;   // read as 16-byte vectors
     if (norm != 0 && norm != 1) return -5;
     if (dense ? B > 0 && (!lse || !logits) : lse || logits || alive) return -5;   // B = 0: empty arrays are nullptr
     if (B <= 0) return 0;
@@ -1849,16 +1932,20 @@ int lah_gate_bwd(long long yo_off, const void* grad, const int* idx, const int* 
     a.yo_off = yo_off; a.grad = (const bf16*)grad; a.idx = idx; a.pair_row = pair_row; a.w = w; a.dlogits = dlogits;
     a.B = B; a.k = k; a.H = H; a.E_loc = E_loc; a.route_owner = route_owner;
     int e;
-#define LAH_GATE_BWD(V)                                                                                     \
-    e = sig ? (norm ? launch_gate_bwd<V, true, true>(a, gs, sig, scale, nullptr, nullptr, nullptr, st)      \
-                    : launch_gate_bwd<V, true, false>(a, gs, sig, scale, nullptr, nullptr, nullptr, st))    \
-            : (norm ? launch_gate_bwd<V, false, true>(a, gs, nullptr, 1.f, nullptr, nullptr, nullptr, st)   \
-                    : launch_gate_bwd<V, false, false>(a, gs, nullptr, scale, logits, lse, alive, st));
+#define LAH_GATE_BWD_P(V, PASS, X)                                                                                 \
+    e = sig ? (norm ? launch_gate_bwd<V, true, true, PASS>(a, gs, sig, scale, nullptr, nullptr, nullptr, X, st)     \
+                    : launch_gate_bwd<V, true, false, PASS>(a, gs, sig, scale, nullptr, nullptr, nullptr, X, st))   \
+            : (norm ? launch_gate_bwd<V, false, true, PASS>(a, gs, nullptr, 1.f, nullptr, nullptr, nullptr, X, st)  \
+                    : launch_gate_bwd<V, false, false, PASS>(a, gs, nullptr, scale, logits, lse, alive, X, st));
+#define LAH_GATE_BWD(V)                          \
+    if (px) { LAH_GATE_BWD_P(V, true, px) }      \
+    else { LAH_GATE_BWD_P(V, false, nullptr) }
     if (H == 256) { LAH_GATE_BWD(1) }
     else if (H == 512) { LAH_GATE_BWD(2) }
     else if (H == 1024) { LAH_GATE_BWD(4) }
     else return -2;
 #undef LAH_GATE_BWD
+#undef LAH_GATE_BWD_P
     if (e) return e;
     return -(int)cudaGetLastError();
 }

@@ -46,13 +46,14 @@ def _lib():
         "lah_set_wait_counter": [P],
         "lah_gate_topk": [P, I, P, I, I, P, Fl, c_ull, L, P, P, P, P, P, I, Fl, P, I, I, I, P, P],
         "lah_expert_bias_update": [P, I, I, P, Fl, P, P],
-        "lah_layout_exchange": [L, L, I, I, I, I, I, I, I, P, P, P, P, P, P, P, I, Fl, I, P, P, P, P, P],
-        "lah_scatter_rows": [P, P, P, P, P, P, L, L, I, I, I, I, I, I, I, I, P, P, P, P, P, I, P],
+        "lah_layout_exchange": [L, L, I, I, I, I, I, I, I, P, P, P, P, P, P, P, I, Fl, I, P, P, P, P, ctypes.c_double, P,
+                                P, P],
+        "lah_scatter_rows": [P, P, P, P, P, P, L, L, I, I, I, I, I, I, I, I, P, P, P, P, P, I, P, P],
         "lah_pull_shadow": [P, I, I, L, L, I, P, I, P],
         "lah_zero_slots": [P, I, P, I, I, I, I, P],
         "lah_signal_wait": [L, I, I, I, I, P, P],
-        "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P, P],
-        "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P, Fl, I, P, P, P, P],
+        "lah_combine_rows": [L, P, P, P, P, I, I, I, I, L, I, I, I, I, P, P, P, P, P, P],
+        "lah_gate_bwd": [L, P, P, P, P, P, I, I, I, I, P, I, P, P, Fl, I, P, P, P, P, P],
         "lah_router_loss_fwd": [P, I, P, I, P, P, I, P, P, P, P, P, P, I, P],
         "lah_router_loss_bwd": [P, I, P, I, P, P, P, P, Fl, Fl, P, I, P],
         "lah_adam_step": [P, P, P, P, P, P, I, P, I, P, P, I, Fl, P, Fl, Fl, Fl, Fl, I, I, I, L, P, Fl, I, P, L, I, I, I, Fl,
@@ -448,15 +449,71 @@ def expert_bias_update(counts, *, alive=None, bias, rate):
 
 def layout_exchange(cnt_all_off, flags_off, slot, epoch, E, E_loc, max_rows, *, align=128, tile_rows=None, counts, dst_row, group_off, group_rows,
                     tile_group, total_rows, status, shadow_slots=0, shadow_tol=1.1, min_shadow_rows=512, route_owner=None,
-                    step_rows=None, shadow_info=None, owned_shadow=None):
-    """count exchange + global layout; with ``shadow_slots`` > 0 also the hot-expert shadow selection (csrc/moe.cu)"""
+                    step_rows=None, shadow_info=None, owned_shadow=None, capacity_factor=0.0, keep=None,
+                    capacity_stats=None):
+    """count exchange + global layout; with ``shadow_slots`` > 0 also the hot-expert shadow selection (csrc/moe.cu).
+    ``capacity_factor`` > 0 (DESIGN.md §6f): every table follows the kept counts of ``expert_capacity_ref``; ``keep``
+    (int32 [E]) receives this rank's kept pairs per expert, ``capacity_stats`` (int32 [2]) C and the box-wide dropped
+    pairs.  0 (dropless) takes neither"""
+    f = check_capacity_factor("layout_exchange", capacity_factor)
+    if (f > 0.0) != (keep is not None and capacity_stats is not None):
+        raise ValueError("layout_exchange: keep and capacity_stats go with capacity_factor > 0, and only with it")
+    if f > 0.0:
+        for name, t, n in (("keep", keep, E), ("capacity_stats", capacity_stats, 2)):
+            if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() < n or not t.is_cuda:
+                raise ValueError(f"layout_exchange: {name} must be a contiguous CUDA int32 tensor of >= {n} entries")
     native.check(_lib().lah_layout_exchange(cnt_all_off, flags_off, slot, epoch, E, E_loc, max_rows, align,
                                             int(tile_rows or min(align, 128)), ptr(counts),
                                             ptr(dst_row), ptr(group_off), ptr(group_rows), ptr(tile_group),
                                             ptr(total_rows), ptr(status), int(shadow_slots), float(shadow_tol),
                                             int(min_shadow_rows), ptr(route_owner), ptr(step_rows), ptr(shadow_info),
-                                            ptr(owned_shadow), stream_ptr()), "lah_layout_exchange")
+                                            ptr(owned_shadow), f, ptr(keep), ptr(capacity_stats), stream_ptr()),
+                 "lah_layout_exchange")
     native.count_launch()
+
+
+CAPACITY_MAX = 2 ** 31 - 1   # C saturates here (csrc/moe.cu layout_exchange_kernel): no count table holds more pairs
+
+
+def check_capacity_factor(what, f):
+    """the expert capacity factor as a float: finite and >= 0 (0 = dropless)"""
+    f = float(f)
+    if not math.isfinite(f) or f < 0.0:
+        raise ValueError(f"{what}: the expert capacity factor must be a finite value >= 0, got {f}")
+    return f
+
+
+def expert_capacity(factor, routed_pairs, num_experts):
+    """C = max(1, ceil((factor * P) / E)) in float64, in this order (DESIGN.md §6f), saturated at CAPACITY_MAX"""
+    c = math.ceil((float(factor) * float(routed_pairs)) / float(num_experts))
+    return max(1, min(c, CAPACITY_MAX))
+
+
+def expert_capacity_ref(cnt, factor):
+    """the expert capacity of a count table ``cnt`` [world, E] (rank r's routed pairs per expert; rows of excluded ranks
+    zero): dict(capacity=C, kept=[world, E] with kept(r, e) = clamp(C - sum_{s<r} cnt(s, e), 0, cnt(r, e)),
+    dropped=P - sum(kept)).  Rank r keeps its pairs of expert e with pos < kept(r, e)"""
+    cnt = torch.as_tensor(cnt).long().cpu()
+    P = int(cnt.sum())
+    C = expert_capacity(factor, P, cnt.shape[1])
+    before = torch.cumsum(cnt, 0) - cnt
+    kept = torch.minimum(torch.clamp(C - before, min=0), cnt)
+    return dict(capacity=C, kept=kept, dropped=P - int(kept.sum()))
+
+
+def capacity_keep_ref(idx, factor, num_experts):
+    """world-1 form of ``expert_capacity_ref`` on one batch's expert ids ``idx`` [B, k] (-1: no pair): (kept mask [B, k],
+    C, dropped).  A pair is kept when fewer than C earlier pairs (token-major order) chose its expert"""
+    flat = idx.reshape(-1).long()
+    valid = flat >= 0
+    key = torch.where(valid, flat, torch.full_like(flat, num_experts))
+    order = torch.sort(key, stable=True).indices
+    srt = key[order]
+    pos = torch.empty_like(flat)
+    pos[order] = torch.arange(flat.numel(), device=flat.device) - torch.searchsorted(srt, srt)
+    C = expert_capacity(factor, int(valid.sum()), num_experts)
+    kept = valid & (pos < C)
+    return kept.view(idx.shape), C, int(valid.sum() - kept.sum())
 
 
 def pull_shadow(shadow_info, shadow_slots, E_loc, p_off, pbf16_off, seg_sizes, small_mask):
@@ -475,14 +532,18 @@ def zero_slots(g, seg_sizes, slots, first_slot, num_slots, seg_mask):
 
 
 def scatter_rows(src, scale, idx, pos, dst_row, pair_row, dst_off, flags_off, slot, epoch, k, E_loc, max_rows,
-                 group_off, group_rows, done_counter, status, align=128, route_owner=None, num_groups=0):
+                 group_off, group_rows, done_counter, status, align=128, route_owner=None, num_groups=0, keep=None):
+    """P2P dispatch of one row per routed pair.  ``keep`` (forward only: with ``dst_row`` and ``pair_row``): the kept
+    pairs per expert of ``layout_exchange(capacity_factor > 0)``; a pair with pos >= keep[e] is dropped (pair_row -1)"""
     num_pairs = idx.numel()
     H = src.shape[1]
     assert src.is_contiguous() and src.dtype == torch.bfloat16
+    if keep is not None and (dst_row is None or pair_row is None):
+        raise ValueError("scatter_rows: keep drops pairs in the forward dispatch (dst_row and pair_row given) only")
     native.check(_lib().lah_scatter_rows(ptr(src), ptr(scale), ptr(idx), ptr(pos), ptr(dst_row), ptr(pair_row), dst_off,
                                          flags_off, slot, epoch, num_pairs, k, H, E_loc, max_rows, align, ptr(group_off),
                                          ptr(group_rows), ptr(done_counter), ptr(status), ptr(route_owner),
-                                         int(num_groups), stream_ptr()),
+                                         int(num_groups), ptr(keep), stream_ptr()),
                  "lah_scatter_rows")
     native.count_launch()
 
@@ -494,27 +555,37 @@ def signal_wait(flags_off, slot, epoch, status, *, signal=True, wait=True):
 
 
 def combine_rows(src_off, idx, pair_row, w, out, k, E_loc, *, flags_off=0, slot=0, epoch=0, signal=False, wait=False,
-                 status=None, route_owner=None, addend=None):
+                 status=None, route_owner=None, addend=None, pass_self=None, pass_w=None):
     """weighted P2P gather; with signal/wait the kernel itself publishes 'my expert outputs are ready' to every peer
     and waits for all peers' flags before pulling their rows (no separate flag kernels).
     :param addend: optional bf16 [B, H] (contiguous, 16-byte aligned) that starts every row's fp32 accumulator:
-        out = bf16(addend + sum_j w_j src_j), rounded once.  None launches the plain kernel"""
+        out = bf16(addend + sum_j w_j src_j), rounded once.  None launches the plain kernel
+    :param pass_self, pass_w: expert capacity (DESIGN.md §6f): a routed pair without a row (dropped) adds
+        pass_w[p] * pass_self[b] instead, with pass_self bf16 [B, H] like the addend and pass_w float32 [B * k]"""
     B, H = out.shape
     if addend is not None:
         _bf16_rows(addend, "combine_rows addend", (B, H))
         if addend.data_ptr() % 16:
             raise ValueError("combine_rows: the addend must be 16-byte aligned")
+    if (pass_self is None) != (pass_w is None):
+        raise ValueError("combine_rows: pass_self and pass_w go together")
+    if pass_self is not None:
+        _bf16_rows(pass_self, "combine_rows pass_self", (B, H))
+        _f32_vec(pass_w, "combine_rows pass_w", B * k)
+        if pass_self.data_ptr() % 16:
+            raise ValueError("combine_rows: pass_self must be 16-byte aligned")
     native.check(_lib().lah_combine_rows(src_off, ptr(idx), ptr(pair_row), ptr(w), ptr(out), B, k, H, E_loc, flags_off,
                                          slot, epoch, int(signal), int(wait), ptr(status), ptr(route_owner),
-                                         ptr(addend), stream_ptr()),
+                                         ptr(addend), ptr(pass_self), ptr(pass_w), stream_ptr()),
                  "lah_combine_rows")
     native.count_launch()
     return out
 
 
-def combine_rows_ref(src, idx, pair_row, w=None, addend=None):
+def combine_rows_ref(src, idx, pair_row, w=None, addend=None, pass_self=None, pass_w=None):
     """exact oracle of ``combine_rows`` on one rank's rows: the float64 sum addend[b] + sum_j w[b, j] src[pair_row[b, j]]
-    over the pairs with an expert and a row, rounded to bf16 once.  ``src``: [R, H]; idx, pair_row, w: [B, k]"""
+    over the pairs with an expert and a row, rounded to bf16 once.  ``src``: [R, H]; idx, pair_row, w: [B, k].  With
+    ``pass_self`` [B, H] and ``pass_w`` [B, k], every pair with an expert and no row adds pass_w[b, j] pass_self[b]"""
     present = ((idx >= 0) & (pair_row >= 0)).double()
     if w is not None:
         present = present * w.double()
@@ -522,17 +593,25 @@ def combine_rows_ref(src, idx, pair_row, w=None, addend=None):
     total = terms.sum(1)
     if addend is not None:
         total = total + addend.double()
+    if pass_self is not None:
+        dropped = ((idx >= 0) & (pair_row < 0)).double() * pass_w.double()
+        total = total + dropped.sum(1, keepdim=True) * pass_self.double()
     return total.to(torch.bfloat16)
 
 
 def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route_owner=None, *, score="softmax",
-             scale=1.0, sig=None, norm=True, lse=None, alive=None, logits=None):
+             scale=1.0, sig=None, norm=True, lse=None, alive=None, logits=None, pass_x=None):
     """gradient of the grid logits from the combine's (one launch).  ``score="sigmoid"``: the gate's ``sig`` array and
     ``scale`` of the same forward (DESIGN.md §6c).  ``norm=False`` (DESIGN.md §6e): the gate ran with norm=False; the
     softmax gate then also needs the forward's grid ``logits`` (float32 [B, sum(grid)]), its ``lse`` and the ``alive``
-    table it routed with, and adds the dense term -p_e sum_j w_j dw_j of every live expert"""
+    table it routed with, and adds the dense term -p_e sum_j w_j dw_j of every live expert.  ``pass_x`` (expert
+    capacity, DESIGN.md §6f): the layer input, bf16 [B, H]; a routed pair without a row then has dw_j = <g_b, x_b>"""
     B, H = grad.shape
     assert grad.is_contiguous() and grad.dtype == torch.bfloat16 and dlogits.dtype == torch.float32
+    if pass_x is not None:
+        _bf16_rows(pass_x, "gate_bwd pass_x", (B, H))
+        if pass_x.data_ptr() % 16:
+            raise ValueError("gate_bwd: pass_x must be 16-byte aligned")
     _score_mode("gate_bwd", score, scale, sig, B * k, grad.device, norm)
     dense = score == "softmax" and not norm
     _check_lse("gate_bwd", lse, B, grad.device, dense)
@@ -556,7 +635,7 @@ def gate_bwd(yo_off, grad, idx, pair_row, w, dlogits, k, E_loc, grid_size, route
     native.check(_lib().lah_gate_bwd(yo_off, ptr(grad), ptr(idx), ptr(pair_row), ptr(w), ptr(dlogits), B, k, H, E_loc,
                                      ctypes.cast(_grid_array(grid_size), c_void_p), len(grid_size), ptr(route_owner),
                                      ptr(sig), float(scale), int(norm), ptr(lse), ptr(logits), ptr(alive),
-                                     stream_ptr()),
+                                     ptr(pass_x), stream_ptr()),
                  "lah_gate_bwd")
     native.count_launch()
     return dlogits

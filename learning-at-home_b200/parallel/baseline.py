@@ -18,8 +18,8 @@ import torch.nn.functional as F
 
 from ..models.layers import FeedforwardBlock, GatedFeedforwardBlock
 from ..ops.kernels import product_key_scores
-from .engine import (GATED_EPS, DMoEConfig, refuse_expert_bias, refuse_group_limited_routing, refuse_router_losses,
-                     refuse_router_score)
+from .engine import (GATED_EPS, DMoEConfig, refuse_expert_bias, refuse_expert_capacity, refuse_group_limited_routing,
+                     refuse_router_losses, refuse_router_score)
 
 
 class _AllToAll(torch.autograd.Function):
@@ -52,6 +52,7 @@ class BaselineDMoE(nn.Module):
         refuse_expert_bias(cfg, "BaselineDMoE")
         refuse_router_score(cfg, "BaselineDMoE")
         refuse_group_limited_routing(cfg, "BaselineDMoE")
+        refuse_expert_capacity(cfg, "BaselineDMoE")
         self.cfg, self.group, self.dtype = cfg, group, dtype
         distributed = dist.is_available() and dist.is_initialized()
         self.world = dist.get_world_size(group) if distributed else 1
@@ -181,6 +182,7 @@ class BaselineTrainer:
         refuse_expert_bias(cfg, "BaselineTrainer")
         refuse_router_score(cfg, "BaselineTrainer")
         refuse_group_limited_routing(cfg, "BaselineTrainer")
+        refuse_expert_capacity(cfg, "BaselineTrainer")
         self.cfg, self.group = cfg, group
         self.device = device or (torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available()
                                  else torch.device("cpu"))

@@ -26,8 +26,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.kernels import product_key_scores
-from .engine import (GATED_EPS, DMoEConfig, refuse_expert_bias, refuse_group_limited_routing, refuse_router_losses,
-                     refuse_router_score, refuse_shared_expert)
+from .engine import (GATED_EPS, DMoEConfig, refuse_expert_bias, refuse_expert_capacity, refuse_group_limited_routing,
+                     refuse_router_losses, refuse_router_score, refuse_shared_expert)
 
 
 class _EqualAllToAll(torch.autograd.Function):
@@ -56,6 +56,7 @@ class FastBaselineDMoE(nn.Module):
         refuse_expert_bias(cfg, "FastBaselineDMoE")
         refuse_router_score(cfg, "FastBaselineDMoE")
         refuse_group_limited_routing(cfg, "FastBaselineDMoE")
+        refuse_expert_capacity(cfg, "FastBaselineDMoE")
         refuse_shared_expert(cfg, "FastBaselineDMoE")
         self.cfg, self.group, self.capacity = cfg, group, capacity
         distributed = dist.is_available() and dist.is_initialized()
@@ -153,6 +154,7 @@ class FastBaselineTrainer:
         refuse_expert_bias(cfg, "FastBaselineTrainer")
         refuse_router_score(cfg, "FastBaselineTrainer")
         refuse_group_limited_routing(cfg, "FastBaselineTrainer")
+        refuse_expert_capacity(cfg, "FastBaselineTrainer")
         refuse_shared_expert(cfg, "FastBaselineTrainer")
         self.cfg, self.group = cfg, group
         self.device = device or torch.device("cuda", torch.cuda.current_device())

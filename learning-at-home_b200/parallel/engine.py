@@ -49,7 +49,9 @@ class DMoEConfig:
     in_features: int = 784
     num_classes: int = 10
     tokens_per_rank: int = 1024          # maximum batch (rows) a rank feeds per step
-    capacity_factor: float = 2.0         # receive-buffer rows = capacity_factor * tokens_per_rank * k (+ padding)
+    # receive-buffer rows = capacity_factor * tokens_per_rank * k (+ padding) in dropless mode (expert_capacity_factor = 0);
+    # not used when expert_capacity_factor > 0, which bounds the buffer itself
+    capacity_factor: float = 2.0
     failure_rate: float = 0.0            # Bernoulli per (token, expert) failure injection (faulty_dmoe_emulator.py:49-51)
     lr: float = 1e-3
     betas: Tuple[float, float] = (0.9, 0.999)
@@ -151,6 +153,13 @@ class DMoEConfig:
     # second residual.  Its parameters are trainer-side (replicated on every rank, averaged over ranks, stepped once per
     # step, like proj).  expert="swiglu" only; 0 (the default) allocates and launches nothing
     shared_inner_dim: int = 0
+    # expert capacity (DESIGN.md §6f, Switch / GShard): each forward, expert e takes at most C = max(1, ceil(f * P / E))
+    # of the P box-wide routed pairs, rank 0's first, then rank 1's, ..., each rank's in token order.  A dropped pair sees
+    # its expert as the identity (adds w_j * x_b; the weights are not renormalised), so a token whose pairs all drop rides
+    # the residual.  The router losses and the bias update see the routed counts, the layout and the optimizer the kept
+    # ones.  Bounds the receive buffer (no overflow) and the rows of a hot expert's owner.  Read at construction; 0 (the
+    # default) is dropless and changes nothing
+    expert_capacity_factor: float = 0.0
 
     def __post_init__(self):
         if self.expert not in EXPERT_LAYOUTS:
@@ -189,6 +198,7 @@ class DMoEConfig:
         if self.shared_inner_dim < 0:
             raise ValueError(f"DMoEConfig.shared_inner_dim must be >= 0, got {self.shared_inner_dim}")
         K.check_expert_groups("DMoEConfig", self.num_experts, self.n_group, self.topk_group, self.k)
+        K.check_capacity_factor("DMoEConfig.expert_capacity_factor", self.expert_capacity_factor)
         if self.shared_inner_dim and self.expert != "swiglu":
             raise ValueError("DMoEConfig.shared_inner_dim: the shared expert is a GatedFeedforwardBlock and needs "
                              f"expert='swiglu', got expert={self.expert!r}")
@@ -315,6 +325,24 @@ def refuse_shared_expert(cfg: DMoEConfig, arm: str):
                          "BaselineDMoE train it)")
 
 
+def refuse_expert_capacity(cfg: DMoEConfig, arm: str):
+    """the baseline arms process every routed pair: refuse an expert capacity instead of silently ignoring it"""
+    if cfg.expert_capacity_factor > 0.0:
+        raise ValueError(f"{arm} processes every routed pair; set expert_capacity_factor to 0 (FusedDMoE / DMoETrainer "
+                         "cap the rows of each expert)")
+
+
+def capacity_buffer_rows(cfg: DMoEConfig, world: int, E_loc: int, shadow_slots: int, align: int) -> int:
+    """receive-buffer rows that no routing can exceed with an expert capacity (DESIGN.md §6f): the largest C that
+    tokens_per_rank, world and k allow, for each owned group and shadow slot, never more than one row per token and
+    expert, each group padded to align"""
+    T = cfg.tokens_per_rank
+    C = K.expert_capacity(cfg.expert_capacity_factor, world * T * cfg.k, cfg.num_experts)
+    pad = lambda r: -(-r // align) * align   # noqa: E731
+    owned = min(E_loc * pad(min(C, world * T)), pad(min(E_loc * min(C, world * T), world * T * cfg.k)) + E_loc * align)
+    return owned + shadow_slots * pad(min(C, T))
+
+
 def expert_uid(cfg: DMoEConfig, e: int) -> str:
     """global expert index -> 'prefix.i0.i1...' (row-major over the grid; reference uid schema README.md:106)"""
     parts = []
@@ -355,7 +383,10 @@ class EngineContext:
             self.tile_rows = 128
             self.S = min(int(cfg.shadow_experts), 2 * K.MAX_WORLD) if self.world > 1 else 0   # shadow slots per rank / layer
         self.G_tot = self.E_loc + self.S
-        self.max_rows = ((cap + self.align - 1) // self.align + self.G_tot) * self.align
+        if cfg.expert_capacity_factor > 0.0:
+            self.max_rows = capacity_buffer_rows(cfg, self.world, self.E_loc, self.S, self.align)
+        else:
+            self.max_rows = ((cap + self.align - 1) // self.align + self.G_tot) * self.align
         self.max_rows = (self.max_rows + 127) // 128 * 128
         self.max_tiles = self.max_rows // self.tile_rows
         H = cfg.hidden
@@ -779,6 +810,12 @@ class LayerWorkspace:
         self.owned_shadow = torch.full((ctx.E_loc * 2,), -1, **i32)
         self.tile_group = torch.full((ctx.max_tiles,), -1, **i32)
         self.total_rows = torch.zeros(1, **i32)
+        # expert capacity (DESIGN.md §6f): this rank's kept pairs per expert and (C, box-wide dropped pairs), written by
+        # layout_exchange
+        self.keep = self.capacity_stats = None
+        if cfg.expert_capacity_factor > 0.0:
+            self.keep = torch.zeros(ctx.E, **i32)
+            self.capacity_stats = torch.zeros(2, **i32)
         # the sigmoid router (DESIGN.md §6c): sigma of every selected pair, written by gate_topk and read by gate_bwd
         self.sig = torch.zeros(P, **f32) if cfg.router_score == "sigmoid" else None
         # the unnormalised softmax router (DESIGN.md §6e): each token's log-partition z_b, written by gate_topk and read by
@@ -834,7 +871,8 @@ class _FusedDMoEFunction(torch.autograd.Function):
         ws.outstanding = ctx.tracked
         ctx.router = layer.training and layer.router_on
         ctx.dense = layer.dense_gate   # the gate backward of the unnormalised softmax reads the logits too
-        ctx.shared = layer.shared_inner > 0   # the shared expert's norm backward reads the layer input
+        # the shared expert's norm backward and the dropped pairs of an expert capacity (gate_bwd) read the layer input
+        ctx.shared = layer.shared_inner > 0 or layer.capacity_factor > 0.0
         if ctx.router or ctx.dense or ctx.shared:
             ctx.save_for_backward(*([logits] if ctx.router or ctx.dense else []), *([x] if ctx.shared else []))
         return layer._forward_cuda(x, logits)
@@ -890,6 +928,10 @@ class FusedDMoE(nn.Module):
             # the workspace (the sigma array of the sigmoid gate) is allocated from the context's configuration
             raise ValueError(f"FusedDMoE: router_score={cfg.router_score!r} needs an EngineContext built with the same "
                              f"router_score, got {ctx.cfg.router_score!r}")
+        if ctx is not None and (cfg.expert_capacity_factor > 0.0) != (ctx.cfg.expert_capacity_factor > 0.0):
+            # the receive buffer and the workspace's keep table follow the context's configuration
+            raise ValueError(f"FusedDMoE: expert_capacity_factor={cfg.expert_capacity_factor} needs an EngineContext "
+                             f"built with an expert capacity as well, got {ctx.cfg.expert_capacity_factor}")
         if ctx is not None and cfg.norm_topk_prob != ctx.cfg.norm_topk_prob:
             # the workspace (the log-partition array of the unnormalised softmax gate) follows the context's configuration
             raise ValueError(f"FusedDMoE: norm_topk_prob={cfg.norm_topk_prob!r} needs an EngineContext built with the "
@@ -939,6 +981,9 @@ class FusedDMoE(nn.Module):
         self.dense_gate = dense_gate_backward(cfg)
         # group-limited routing (cfg.n_group / topk_group, read here once; DESIGN.md §6d)
         self.n_group, self.topk_group = int(cfg.n_group), int(cfg.topk_group)
+        # expert capacity (cfg.expert_capacity_factor, read here once; DESIGN.md §6f)
+        self.capacity_factor = float(cfg.expert_capacity_factor)
+        self._ref_capacity = None   # CPU path: (C, dropped pairs) of the last forward
         self._last_pairs = 0   # GPU path: routed pairs (B * k) of the last forward, whose ws.idx log_step reads
         # shared expert (cfg.shared_inner_dim, read here once): initialised like GatedFeedforwardBlock(hidden, I_s), drawn
         # from the global RNG like proj (DMoETrainer seeds it, so every rank starts identical), kept as the segments of
@@ -1034,7 +1079,8 @@ class FusedDMoE(nn.Module):
                           dst_row=ws.dst_row, group_off=ws.group_off, group_rows=ws.group_rows,
                           tile_group=ws.tile_group, total_rows=ws.total_rows, status=c.status, shadow_slots=c.S,
                           shadow_tol=cfg.shadow_tol, min_shadow_rows=cfg.shadow_min_rows, route_owner=ws.route_owner,
-                          step_rows=ws.step_rows, shadow_info=ws.shadow_info, owned_shadow=ws.owned_shadow)
+                          step_rows=ws.step_rows, shadow_info=ws.shadow_info, owned_shadow=ws.owned_shadow,
+                          capacity_factor=self.capacity_factor, keep=ws.keep, capacity_stats=ws.capacity_stats)
         if self.training and self.router_on:
             # before combine_rows: no peer can reach the next layer's count exchange (which rewrites cnt_all) until this
             # rank's combine has signalled
@@ -1048,7 +1094,7 @@ class FusedDMoE(nn.Module):
             sh.w8_dirty = True
         K.scatter_rows(x, None, idx, pos, ws.dst_row, pair_row, ws.xd_off, c.flags_off, K.SLOT_DISPATCH, epoch, k,
                        c.E_loc, c.max_rows, ws.group_off, ws.group_rows, c.done_counter, c.status, align=c.align,
-                       route_owner=ws.route_owner, num_groups=c.G_tot)
+                       route_owner=ws.route_owner, num_groups=c.G_tot, keep=ws.keep)
         c.timer.mark("dispatch(layout+pull+scatter)")
         # the shared expert needs only this rank's rows: at world > 1 it runs while the peers' rows are in flight
         ys = self._shared_expert_fwd(x) if self.shared_inner else None
@@ -1080,8 +1126,11 @@ class FusedDMoE(nn.Module):
                             (ws.mean1, ws.rstd1, ws.mean2, ws.rstd2), ws.yo)
         c.timer.mark("expert_ffn_fwd")
         y = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=x.device)
+        # expert capacity: a dropped pair adds w_j * x_b (its expert as the identity)
+        passing = dict(pass_self=x, pass_w=w) if self.capacity_factor > 0.0 else {}
         K.combine_rows(ws.yo_off, idx, pair_row, w, y, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_OUTPUT, epoch=epoch,
-                       signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner, addend=ys)
+                       signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner, addend=ys,
+                       **passing)
         c.timer.mark("combine")
         return y
 
@@ -1159,7 +1208,7 @@ class FusedDMoE(nn.Module):
     def _backward_cuda(self, gy, B, logits=None, x=None, router=False):
         """:param logits: the gate logits of the forward when it computed router losses or the layer has the dense gate
         backward of the unnormalised softmax router
-        :param x: the layer input of the forward, when the layer has a shared expert
+        :param x: the layer input of the forward, when the layer has a shared expert or an expert capacity
         :param router: the forward computed router losses (their gradient is added here)"""
         c, ws, sh, cfg = self.ctx, self.ws, self.shard, self.cfg
         k = cfg.k
@@ -1169,8 +1218,9 @@ class FusedDMoE(nn.Module):
         gy = gy.to(torch.bfloat16)
         dlogits = torch.empty(B, sum(self.grid_size), dtype=torch.float32, device=gy.device)
         dense = dict(alive=c.alive, logits=logits) if self.dense_gate else {}
+        capped = self.capacity_factor > 0.0   # a dropped pair: dw_j = <g_b, x_b>, and w_j * g_b joins dx
         K.gate_bwd(ws.yo_off, gy, idx, pair_row, w, dlogits, k, c.E_loc, self.grid_size, route_owner=ws.route_owner,
-                   **self._score_args(P, B), **dense)
+                   pass_x=x if capped else None, **self._score_args(P, B), **dense)
         if router:
             K.router_loss_bwd(logits, self.grid_size, alive=c.alive, f=ws.router_f, z=ws.router_z, Fb=ws.router_F,
                               aux_coef=self.router_aux_coef * self.router_grad_scale,
@@ -1240,7 +1290,7 @@ class FusedDMoE(nn.Module):
         dx = torch.empty(B, cfg.hidden, dtype=torch.bfloat16, device=gy.device)
         K.combine_rows(c.dxd_off, idx, pair_row, None, dx, k, c.E_loc, flags_off=c.flags_off, slot=K.SLOT_DINPUT,
                        epoch=epoch, signal=c.world > 1, wait=c.world > 1, status=c.status, route_owner=ws.route_owner,
-                       addend=dxs)
+                       addend=dxs, **(dict(pass_self=gy, pass_w=w) if capped else {}))
         c.timer.mark("bwd_combine")
         return dx, dlogits
 
@@ -1347,6 +1397,15 @@ class FusedDMoE(nn.Module):
         xf = x.float()
         out = torch.zeros(x.shape[0], cfg.hidden, dtype=torch.float32, device=x.device)
         rnd = (lambda t: t.to(torch.bfloat16).float()) if emulate_bf16 else (lambda t: t)
+        routed = idx   # the router losses see every routed pair
+        if self.capacity_factor > 0.0:
+            # expert capacity (DESIGN.md §6f): the pairs past C of their expert, in token order, see the expert as the
+            # identity; the experts and their optimizer steps see the kept pairs only
+            kept, C, dropped = K.capacity_keep_ref(idx, self.capacity_factor, cfg.num_experts)
+            self._ref_capacity = (C, dropped)
+            drop_w = torch.where(kept | (idx < 0), torch.zeros_like(weights), weights)
+            out = out + drop_w.sum(1, keepdim=True) * rnd(xf)
+            idx = torch.where(kept, idx, torch.full_like(idx, -1))
         if self.training:
             rows = torch.bincount(idx[idx >= 0].flatten() - self.first_expert, minlength=self.E_loc)
             self._ref_rows = rows if self._ref_rows is None else self._ref_rows + rows
@@ -1364,7 +1423,7 @@ class FusedDMoE(nn.Module):
                 p = {n: (rnd(v) if n.startswith("w") else v) for n, v in p.items()}
             out = out + rnd(self._gated_branch(p, rnd(xf), rnd))
         if self.training and self.router_on:
-            counts = torch.bincount(idx[idx >= 0].flatten(), minlength=cfg.num_experts)
+            counts = torch.bincount(routed[routed >= 0].flatten(), minlength=cfg.num_experts)
             l_aux, l_z = K.router_loss_ref(logits, self.grid_size, counts, alive=alive, score=self.router_score)
             with torch.no_grad():
                 self.router_loss.copy_(torch.stack([l_aux, l_z]).detach())

@@ -323,6 +323,9 @@ class DMoETrainer:
                 if not block.norm_topk_prob and block._last_pairs:   # the router mass the top k carries (DESIGN.md §6e)
                     layer["routed_weight_mean"] = float(
                         block.ws.w[:block._last_pairs].view(-1, self.cfg.k).sum(1).mean())
+                if block.ws.capacity_stats is not None:   # the layer's last forward, box-wide (DESIGN.md §6f)
+                    cap, dropped = block.ws.capacity_stats.tolist()
+                    layer.update(expert_capacity=cap, dropped_pairs=dropped)
                 layers.append(layer)
             rec["layers"] = layers
             if self.last_stage_ms:

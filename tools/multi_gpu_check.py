@@ -38,15 +38,21 @@ def main():
     # group-limited routing with one group per rank (DESIGN.md §6d): every token's pairs must reach exactly one rank, and
     # the whole-batch oracle routes with the same limit
     group = dict(n_group=world, topk_group=1) if "--group-limited" in sys.argv else {}
+    # expert capacity (DESIGN.md §6f) under collapsed routing: the gate sends every token to the first rank's experts, C =
+    # P / E drops most pairs, and the whole-batch oracle drops the same ones under rank-major priority
+    capacity = dict(expert_capacity_factor=1.0) if "--expert-capacity" in sys.argv else {}
     swiglu = swiglu or bool(shared)
     mat, vec = ("w13", "g") if swiglu else ("w1", "b2")
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=B, capacity_factor=float(max(4, world)),
                        shadow_experts=4, shadow_tol=0.0 if force_shadow else 1.1, shadow_min_rows=1 if force_shadow else 64,
                        expert_path="small" if small else "big", expert="swiglu" if swiglu else "ffn", **router, **bias, **shared,
-                       **group)
+                       **group, **capacity)
     ctx = E.EngineContext(cfg)
     torch.manual_seed(0)  # identical gate on every rank (DMoETrainer does the same)
     layer = E.FusedDMoE(cfg, ctx).cuda()
+    if capacity:   # the first grid coordinate picks the rank: coordinate 0 gets every token
+        with torch.no_grad():
+            layer.proj.bias[0] += 50.0
     gen = torch.Generator().manual_seed(0)
     x_all = torch.randn(world * B, 512, generator=gen).to(torch.bfloat16)
     g_all = torch.randn(world * B, 512, generator=gen).to(torch.bfloat16)
@@ -63,7 +69,7 @@ def main():
     counts = ctx.cnt_all[:world].cpu().tolist()
     plan, _ = shadow_plan(counts, ctx.E_loc, ctx.S, tol=cfg.shadow_tol, min_rows=cfg.shadow_min_rows)
     got = [int(e) for e in layer.ws.shadow_info.view(-1, 4)[:, 0].cpu().tolist() if e >= 0]
-    plan_ok = plan == got or small
+    plan_ok = plan == got or small or bool(capacity)   # the host model plans from the routed counts, not the kept ones
     # gather what the distributed run produced
     ys = [torch.empty_like(y) for _ in range(world)]
     dxs = [torch.empty_like(x.grad) for _ in range(world)]
@@ -132,6 +138,12 @@ def main():
     rpt = torch.tensor([ranks_per_token], device="cuda")
     dist.all_reduce(rpt, op=dist.ReduceOp.MAX)
     group_ok = not group or int(rpt) == 1
+    capacity_ok = True
+    if capacity:   # the same (C, dropped pairs) on every rank, some pairs dropped, and the status word clean
+        stats = layer.ws.capacity_stats.clone()
+        every = [torch.empty_like(stats) for _ in range(world)]
+        dist.all_gather(every, stats)
+        capacity_ok = all(torch.equal(s, stats) for s in every) and int(stats[1]) > 0 and int(ctx.status[0]) == 0
     ok = True
     if rank == 0:
         # single-GPU reference in the same process: a fresh world-1 context is impossible inside an initialised group,
@@ -166,7 +178,11 @@ def main():
         ok = errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2 and errs["w1_mean_abs"] < 1e-4 and errs["b2_max_abs"] < 2.5e-3 and errs["steps"]
         ok = ok and (shadowed > 0 or not force_shadow) and plan_ok and errs.get("router_loss", 0.0) < 1e-4
         ok = ok and errs.get("router_grad_max_err", 0.0) < 1e-4 and bias_ok
-        ok = ok and errs.get("shared_grad", 0.0) < 8e-2 and shared_ok and group_ok
+        ok = ok and errs.get("shared_grad", 0.0) < 8e-2 and shared_ok and group_ok and capacity_ok
+        if capacity:
+            errs["capacity"] = dict(kernel=layer.ws.capacity_stats.tolist(), oracle=list(ref._ref_capacity),
+                                    same_on_every_rank_and_clean=capacity_ok)
+            ok = ok and layer.ws.capacity_stats.tolist() == list(ref._ref_capacity)
         if group:
             errs["max_ranks_per_token"] = int(rpt)
         if bias:
