@@ -14,6 +14,9 @@
 //   forward   a  = silu(g) o u
 //   backward  dh = [da o u o s (1 + g (1 - s)) | da o silu(g)],  s = sigmoid(g)
 // in fp32 with one bf16 rounding per output, 16-byte accesses (one thread per 8 columns of a row).
+// swiglu_quant_kernel is the forward of the FP8 expert: it ALSO writes a as the MXFP8 operand of the W2 GEMM (E4M3 payload
+// and scales in the activation layout, from the fp32 product before its bf16 rounding), and the bf16 a only when asked.
+#include "mxfp8.cuh"
 #include "sm90.cuh"
 #include "dropout.cuh"
 
@@ -132,6 +135,32 @@ __global__ void __launch_bounds__(256) swiglu_kernel(const bf16* __restrict__ h,
     }
 }
 
+// the forward above plus the MXFP8 copy of a (aq, sf; a may be nullptr).  The 4 threads of a 32-column block are adjacent
+// lanes of one row (inner / 8 is a multiple of 4), so a quad is wholly live or wholly skipped and shuffles within itself.
+// Rows of tiles whose group is -1 (tile_group128: one entry per 128 rows) and rows >= *total_rows are skipped.
+__global__ void __launch_bounds__(256) swiglu_quant_kernel(const bf16* __restrict__ h, bf16* __restrict__ a,
+                                                           uint8_t* __restrict__ aq, uint8_t* __restrict__ sf,
+                                                           long long vecs, int inner,
+                                                           const int* __restrict__ tile_group128,
+                                                           const int* __restrict__ total_rows) {
+    const long long t = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (t >= vecs) return;
+    const int per_row = inner >> 3;
+    const long long row = t / per_row;
+    if (total_rows && row >= __ldg(total_rows)) return;
+    if (tile_group128 && __ldg(tile_group128 + (row >> 7)) < 0) return;
+    const int v = static_cast<int>(t - row * per_row), col = v * 8;
+    const bf16* hr = h + row * 2 * inner;
+    float g[8], u[8], y[8];
+    unpack8(__ldg(reinterpret_cast<const int4*>(hr + col)), g);
+    unpack8(__ldg(reinterpret_cast<const int4*>(hr + inner + col)), u);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) y[i] = g[i] * sigmoid_f(g[i]) * u[i];
+    if (a) *reinterpret_cast<int4*>(a + row * inner + col) = pack8(y);
+    const int lane = threadIdx.x & 31;
+    quant_quad8(y, 0xFu << (lane & ~3), lane, aq + row * inner + col, sf + act_sf_byte(row, inner, v >> 2));
+}
+
 }  // namespace lah
 
 using namespace lah;
@@ -182,6 +211,23 @@ int lah_swiglu_fwd(const void* h, void* a, long long rows, int inner, cudaStream
     const long long vecs = rows * (inner / 8);
     if (vecs == 0) return 0;
     swiglu_kernel<false><<<(unsigned)((vecs + 255) / 256), 256, 0, st>>>((const bf16*)h, nullptr, (bf16*)a, vecs, inner);
+    return -(int)cudaGetLastError();
+}
+
+// the same + a as an MXFP8 GEMM operand (aq: e4m3 [rows, inner]; sf: activation scale layout, tile_rows = 128); a may be
+// NULL.  tile_group128 (optional): the group of every 128 rows, -1 = skipped; total_rows (optional, device): rows past it
+// are skipped.  inner a multiple of 128; h and a 16-byte aligned, aq 8-byte aligned (the vector widths of the kernel)
+int lah_swiglu_fwd_q(const void* h, void* a, void* aq, void* sf, long long rows, int inner, const int* tile_group128,
+                     const int* total_rows, cudaStream_t st) {
+    if (rows < 0 || inner <= 0 || inner % 128 || !aq || !sf) return -2;
+    if ((reinterpret_cast<uintptr_t>(h) % 16) || (reinterpret_cast<uintptr_t>(a) % 16) ||
+        (reinterpret_cast<uintptr_t>(aq) % 8))
+        return -2;
+    const long long vecs = rows * (inner / 8);
+    if (vecs == 0) return 0;
+    swiglu_quant_kernel<<<(unsigned)((vecs + 255) / 256), 256, 0, st>>>((const bf16*)h, (bf16*)a, (uint8_t*)aq,
+                                                                       (uint8_t*)sf, vecs, inner, tile_group128,
+                                                                       total_rows);
     return -(int)cudaGetLastError();
 }
 

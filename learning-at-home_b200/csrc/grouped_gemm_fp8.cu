@@ -11,6 +11,7 @@
 //     straight from the quantiser's layout (sf_word) through the read-only cache.
 //
 // Used for the expert FFN forward GEMMs (BASELINE.json config "fp8 expert GEMM"); dgrad / wgrad stay in bf16.
+#include "mxfp8.cuh"
 #include "sm90.cuh"
 #include <cuda_fp8.h>
 
@@ -226,15 +227,6 @@ __host__ __device__ inline long long sf_chunks(long long rows, int tile_rows, in
     return tiles * num_kb * ((tile_rows + 127) / 128);
 }
 
-__device__ __forceinline__ uint32_t e8m0_from_amax(float amax) {
-    // smallest power of two s with amax / s <= 448 (the E4M3 maximum): no element saturates
-    const float s = amax * (1.f / 448.f);
-    uint32_t bits = __float_as_uint(s);
-    uint32_t e = (bits >> 23) & 0xFFu;
-    if (bits & 0x7FFFFFu) e += 1;
-    return min(max(e, 1u), 253u);
-}
-
 // one thread per (row, 32-element block): 64 B (bf16) or 128 B (fp32) in, 32 B + one scale byte out
 template <typename T>
 __global__ void __launch_bounds__(256) quant_mxfp8_kernel(const T* __restrict__ in, long long ld_in,
@@ -277,7 +269,7 @@ __global__ void __launch_bounds__(256) quant_mxfp8_kernel(const T* __restrict__ 
     float amax = 0.f;
 #pragma unroll
     for (int j = 0; j < 32; ++j) amax = fmaxf(amax, fabsf(v[j]));
-    const uint32_t e = e8m0_from_amax(amax);
+    const uint32_t e = e8m0_from_amax(amax);   // csrc/mxfp8.cuh
     const float inv = __uint_as_float((254u - e) << 23);
     uint32_t packed[8];
 #pragma unroll

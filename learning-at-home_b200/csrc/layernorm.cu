@@ -5,6 +5,7 @@
 // (/root/reference/experiments/throughput/layers.py:9-15); per-expert affine parameters gamma/beta are stacked [G, C].
 //
 // Rows are grouped by expert in 128-row tiles; tile_group[t] gives the expert (or -1: tile unused, skipped).
+#include "mxfp8.cuh"
 #include "sm90.cuh"
 #include <cuda_fp8.h>
 #include <stdlib.h>
@@ -383,6 +384,10 @@ __global__ void __launch_bounds__(LnBwdCfg<C>::THREADS, LnBwdCfg<C>::MIN_BLOCKS)
 // rows).  The backward's per-tile dgamma partials go through group_tile_sum_kernel with tile_group, so dgamma[g] is summed in
 // tile order.  tile_group (and tile_shift) are the LAST parameters, read only when GROUPED, so that the single-gamma
 // instantiations keep the parameter layout, and the code, they had before the flag existed.
+// QUANT (the FP8 expert forward): the forward ALSO emits the MXFP8 operand of the next GEMM, as ln_relu_fwd_kernel does
+// (E4M3 payload nq and scales sf in the activation layout, from the fp32 value before its bf16 rounding; 4 lanes share a
+// 32-column block); the bf16 n is then optional (nullptr: serving, which has no weight gradient to feed).  Widths: the
+// multiples of 256 (no half chunk).  nq and sf come after tile_shift, for the same reason as tile_group.
 // ------------------------------------------------------------------------------------------------
 // Rows per warp: the LayerNorm rule for the widths it was not tuned at (R = 4 up to NV = 2, 2 up to NV = 6, else 1), at
 // every width; the tuned power-of-two configurations hold 2-4x the rows and spill here.  Above NV = 11 one row no longer
@@ -394,13 +399,14 @@ struct RmsFwdCfg {
     static constexpr int MIN_BLOCKS = NV <= 11 ? 2 : 1;
 };
 
-template <int C, int R, bool GROUPED>
+template <int C, int R, bool GROUPED, bool QUANT>
 __global__ void __launch_bounds__(256, RmsFwdCfg<C>::MIN_BLOCKS) rms_norm_fwd_kernel(
     const bf16* __restrict__ x, bf16* __restrict__ n, float* __restrict__ rstd_out, const float* __restrict__ gamma,
-    int rows, float eps, const int* __restrict__ tile_group, int tile_shift) {
+    int rows, float eps, const int* __restrict__ tile_group, int tile_shift, uint8_t* __restrict__ nq,
+    uint8_t* __restrict__ sf) {
     constexpr int NV = LnFwdCfg<C>::NV;
     constexpr bool HALF = C % 256 != 0;
-    static_assert(C % 128 == 0 && C <= LN_MAX_C, "unsupported RMSNorm width");
+    static_assert(C % 128 == 0 && C <= LN_MAX_C && !(QUANT && HALF), "unsupported RMSNorm width");
     // a warp's R rows lie in one tile: row0 is a multiple of R, and R (a power of two <= 4) divides every tile size (>= 8)
     static_assert(R == 1 || R == 2 || R == 4, "rows per warp must divide the smallest tile (8 rows)");
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -465,12 +471,17 @@ __global__ void __launch_bounds__(256, RmsFwdCfg<C>::MIN_BLOCKS) rms_norm_fwd_ke
                 y[2 * t] = f.x * rstd[r] * gg[2 * t];
                 y[2 * t + 1] = f.y * rstd[r] * gg[2 * t + 1];
             }
-            int4 o;
-            o.x = pack_bf16x2(y[0], y[1]);
-            o.y = pack_bf16x2(y[2], y[3]);
-            o.z = pack_bf16x2(y[4], y[5]);
-            o.w = pack_bf16x2(y[6], y[7]);
-            st_v4(reinterpret_cast<int4*>(n + static_cast<long long>(row) * C) + j * 32 + lane, o);
+            if (!QUANT || n) {
+                int4 o;
+                o.x = pack_bf16x2(y[0], y[1]);
+                o.y = pack_bf16x2(y[2], y[3]);
+                o.z = pack_bf16x2(y[4], y[5]);
+                o.w = pack_bf16x2(y[6], y[7]);
+                st_v4(reinterpret_cast<int4*>(n + static_cast<long long>(row) * C) + j * 32 + lane, o);
+            }
+            if constexpr (QUANT)
+                quant_quad8(y, 0xffffffffu, lane, nq + static_cast<long long>(row) * C + (j * 32 + lane) * 8,
+                            sf + act_sf_byte(row, C, j * 8 + (lane >> 2)));
         }
     }
 }
@@ -728,11 +739,27 @@ void rms_fwd_launch(const void* x, void* n, float* rstd, const float* gamma, int
     constexpr int RR = RmsFwdCfg<C>::R;
     const int grid = (rows + 8 * RR - 1) / (8 * RR);
     if (tile_group)
-        rms_norm_fwd_kernel<C, RR, true><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
-                                                               tile_group, tile_shift);
+        rms_norm_fwd_kernel<C, RR, true, false><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
+                                                                      tile_group, tile_shift, nullptr, nullptr);
     else
-        rms_norm_fwd_kernel<C, RR, false><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
-                                                                nullptr, 0);
+        rms_norm_fwd_kernel<C, RR, false, false><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
+                                                                       nullptr, 0, nullptr, nullptr);
+}
+
+using RmsFwdQLaunch = void (*)(const void*, void*, float*, const float*, int, float, const int*, int, void*, void*,
+                               cudaStream_t);
+
+template <int C>
+void rms_fwd_q_launch(const void* x, void* n, float* rstd, const float* gamma, int rows, float eps,
+                      const int* tile_group, int tile_shift, void* nq, void* sf, cudaStream_t st) {
+    constexpr int RR = RmsFwdCfg<C>::R;
+    const int grid = (rows + 8 * RR - 1) / (8 * RR);
+    if (tile_group)
+        rms_norm_fwd_kernel<C, RR, true, true><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
+                                                                     tile_group, tile_shift, (uint8_t*)nq, (uint8_t*)sf);
+    else
+        rms_norm_fwd_kernel<C, RR, false, true><<<grid, 256, 0, st>>>((const bf16*)x, (bf16*)n, rstd, gamma, rows, eps,
+                                                                      nullptr, 0, (uint8_t*)nq, (uint8_t*)sf);
 }
 
 template <int C, bool GROUPED>
@@ -770,6 +797,11 @@ constexpr auto rms_bwd_table(std::integer_sequence<int, I...>) {
     return std::array<RmsBwdLaunch, sizeof...(I)>{rms_bwd_launch<(I + 1) * 128>...};
 }
 constexpr auto kRmsFwd = rms_fwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
+template <int... I>
+constexpr auto rms_fwd_q_table(std::integer_sequence<int, I...>) {
+    return std::array<RmsFwdQLaunch, sizeof...(I)>{rms_fwd_q_launch<(I + 1) * 256>...};
+}
+constexpr auto kRmsFwdQ = rms_fwd_q_table(std::make_integer_sequence<int, LN_MAX_C / 256>{});
 constexpr auto kRmsBwd = rms_bwd_table(std::make_integer_sequence<int, LN_MAX_C / 128>{});
 
 // widths the LayerNorm entry points run: multiples of 128 up to LN_MAX_C (the column sum has no upper limit)
@@ -838,6 +870,20 @@ int lah_rms_norm_fwd(const void* x, void* n, float* rstd, const float* gamma, in
     const int tile_shift = tile_group ? shift_of(tile_rows) : 0;
     if (!ln_width_ok(C) || !(eps > 0.f) || tile_shift < 0) return -2;
     kRmsFwd[C / 128 - 1](x, n, rstd, gamma, rows, eps, tile_group, tile_shift, st);
+    return -(int)cudaGetLastError();
+}
+
+// same + the MXFP8 copy of n (nq: e4m3 [rows, C]; sf: activation scale layout, tile_rows = 128); n may be NULL.
+// C a multiple of 256 up to LN_MAX_C; x and n 16-byte aligned, nq 8-byte aligned (the vector widths of the kernel)
+int lah_rms_norm_fwd_q(const void* x, void* n, float* rstd, const float* gamma, int rows, int C, float eps,
+                       const int* tile_group, int tile_rows, void* nq, void* sf, cudaStream_t st) {
+    const int tile_shift = tile_group ? shift_of(tile_rows) : 0;
+    if (!ln_width_ok(C) || C % 256 || !(eps > 0.f) || tile_shift < 0 || !nq || !sf) return -2;
+    if ((reinterpret_cast<uintptr_t>(x) % 16) || (reinterpret_cast<uintptr_t>(n) % 16) ||
+        (reinterpret_cast<uintptr_t>(nq) % 8))
+        return -2;
+    if (rows <= 0) return 0;
+    kRmsFwdQ[C / 256 - 1](x, n, rstd, gamma, rows, eps, tile_group, tile_shift, nq, sf, st);
     return -(int)cudaGetLastError();
 }
 

@@ -41,14 +41,14 @@ def chain_schedule(tick: int, rank: int, world: int, num_layers: int):
 
 def make_parser():
     p = ArgumentParser()
-    p.add_argument("--block-type", choices=["ffn", "transformer"], default="transformer")
+    p.add_argument("--block-type", choices=["ffn", "swiglu", "transformer"], default="transformer")
     p.add_argument("--hid-dim", type=int, default=1024)
     p.add_argument("--layers-per-gpu", type=int, default=56)
     p.add_argument("-j", "--jobs", type=int, default=64, help="concurrent trainers")
     p.add_argument("--batch-size", type=int, default=None, help="samples per trainer batch (default: 4 sequences / 2048 rows)")
     p.add_argument("--passes", type=int, default=3, help="timed passes of all trainers' batches through the whole chain")
     p.add_argument("--warmup", type=int, default=1)
-    p.add_argument("--dtype", choices=["bf16", "fp8"], default="bf16", help="fp8: MXFP8 GEMMs (ffn blocks only)")
+    p.add_argument("--dtype", choices=["bf16", "fp8"], default="bf16", help="fp8: MXFP8 GEMMs (ffn and swiglu blocks)")
     return p
 
 
@@ -72,6 +72,9 @@ def run(args):
     if transformer:
         from ...models.transformer_native import NativeTransformerLayer as Native
         kw = {}
+    elif args.block_type == "swiglu":
+        from ...models.ffn_native import NativeGatedFFNLayer as Native
+        kw = dict(dtype=args.dtype)
     else:
         from ...models.ffn_native import NativeFFNLayer as Native
         kw = dict(dtype=args.dtype)

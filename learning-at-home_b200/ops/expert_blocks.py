@@ -1,8 +1,9 @@
 """
 The expert programs as sm_90a kernel chains, written once for the routed and shared experts of ``FusedDMoE``, the
-``ExpertBackend`` executors and ``NativeFFNLayer``: ``FeedforwardBlock`` (``ffn_forward``, ``ffn_forward_fp8``,
-``ffn_backward``) and the MLP of ``GatedFeedforwardBlock`` after its RMSNorm, which stays with each caller
-(``swiglu_mlp_forward`` / ``_backward``).  A ``RowPlan`` says how one call's kernels see their rows.
+``ExpertBackend`` executors, ``NativeFFNLayer`` and ``NativeGatedFFNLayer``: ``FeedforwardBlock`` (``ffn_forward``,
+``ffn_forward_fp8``, ``ffn_backward``) and the MLP of ``GatedFeedforwardBlock`` after its RMSNorm, which stays with each
+caller (``swiglu_mlp_forward``, ``swiglu_mlp_forward_fp8``, ``swiglu_mlp_backward``).  A ``RowPlan`` says how one call's
+kernels see their rows.
 
 Weight gradients go to the caller's ``wgrad(name, dy, x)``.  The backward functions call it for a matrix only after the
 dgrad that reads that matrix, so the callback may update the weights in place (fused wgrad + AMSGrad).
@@ -98,6 +99,15 @@ def swiglu_mlp_forward(plan: RowPlan, w13, w2, n, h, a, y, residual=None):
     plan.linear(n, w13, out=h)
     K.swiglu_fwd(plan.span(h), out=plan.span(a))
     plan.linear(a, w2, out=y, residual=residual)
+
+
+def swiglu_mlp_forward_fp8(plan: RowPlan, w13q, w2q, nq, h, a, aq, y, residual=None):
+    """``swiglu_mlp_forward`` on block-scaled FP8 tensor cores, from the MXFP8 copy ``nq`` of n (the caller's RMSNorm
+    writes it): h = nq [W1; W3]^T in bf16, then the SwiGLU writes the W2 operand ``aq`` (and the bf16 a unless it is
+    None), y = aq W2^T (+ residual).  Rows of -1 tiles of ``plan.tile_group`` are skipped throughout"""
+    fp8.grouped_linear_fp8(nq, w13q, tile_group=plan.tile_group, out=h)
+    K.swiglu_fwd(plan.span(h), out=plan.span(a), quant=aq, tile_group=plan.tile_group)
+    fp8.grouped_linear_fp8(aq, w2q, tile_group=plan.tile_group, residual=residual, out=y)
 
 
 def swiglu_mlp_backward(plan: RowPlan, w13, w2, n, h, a, gy, da, dh, dn, wgrad):

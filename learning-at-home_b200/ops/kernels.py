@@ -69,8 +69,10 @@ def _lib():
         "lah_dropout_mask": [P, I, I, I, I, I, c_ull, I, P],
         "lah_dropout_ew": [I, P, P, P, L, I, c_ull, I, I, Fl, P],
         "lah_rms_norm_fwd": [P, P, P, P, I, I, Fl, P, I, P],
+        "lah_rms_norm_fwd_q": [P, P, P, P, I, I, Fl, P, I, P, P, P],
         "lah_rms_norm_bwd": [P, P, P, P, P, P, P, I, I, I, P, P, P],
         "lah_swiglu_fwd": [P, P, L, I, P],
+        "lah_swiglu_fwd_q": [P, P, P, P, L, I, P, P, P],
         "lah_swiglu_bwd": [P, P, P, L, I, P],
         "lah_symm_alloc": [c_ull, ctypes.POINTER(c_void_p)],
         "lah_symm_free": [P],
@@ -166,24 +168,44 @@ def _check_rms_groups(what, gamma, tile_group, tile_rows, rows, C):
     return gamma.numel() // C
 
 
-def rms_norm_fwd(x, gamma, eps, *, out, rstd, tile_group=None, tile_rows=16):
+def _check_quant_out(what, quant, rows, K_):
+    """``quant``: an activation-layout ops.fp8.MXFP8Tensor (one group, 128-row scale tiles) of width K_ and >= rows rows"""
+    if quant.K != K_ or quant.groups != 1 or quant.rows_per_group < rows or quant.tile_rows != 128:
+        raise ValueError(f"{what}: quant must be an activation MXFP8Tensor of width {K_} with >= {rows} rows, got "
+                         f"K={quant.K}, groups={quant.groups}, rows={quant.rows_per_group}, tile_rows={quant.tile_rows}")
+    if not quant.q.is_contiguous() or quant.q.data_ptr() % 8:
+        raise ValueError(f"{what}: the payload of quant must be contiguous and 8-byte aligned")
+
+
+def rms_norm_fwd(x, gamma, eps, *, out, rstd, tile_group=None, tile_rows=16, quant=None):
     """RMSNorm over the rows of x (csrc/layernorm.cu): out = bf16(x * rstd * gamma), rstd[r] = 1 / sqrt(mean(x_r^2) + eps)
     kept in fp32.  x, out: bf16 [rows, C] with C in LN_WIDTHS; gamma: fp32 [C]; rstd: fp32 [rows]; eps > 0.
     With ``tile_group`` (int32, the group of every ``tile_rows`` rows, -1 = unused) gamma is fp32 [G, C] and the rows of
-    tile t are normalised with gamma[tile_group[t]]; the rows of -1 tiles are left as they were"""
+    tile t are normalised with gamma[tile_group[t]]; the rows of -1 tiles are left as they were.
+    :param quant: optional ops.fp8.MXFP8Tensor (activation layout) that additionally receives the output as an MXFP8 GEMM
+        operand, quantised from the fp32 value before its bf16 rounding; ``out`` may then be None.  C a multiple of 256"""
     if x.dim() != 2:
         raise ValueError(f"rms_norm_fwd: x must be [rows, C], got {tuple(x.shape)}")
     rows, C = x.shape
     _check_ln_width(C, "rms_norm_fwd")
     _bf16_rows(x, "rms_norm_fwd x", (rows, C))
-    _bf16_rows(out, "rms_norm_fwd out", (rows, C))
+    if out is not None or quant is None:
+        _bf16_rows(out, "rms_norm_fwd out", (rows, C))
     G = _check_rms_groups("rms_norm_fwd", gamma, tile_group, tile_rows, rows, C)
     _f32_vec(gamma, "rms_norm_fwd gamma", G * C)
     _f32_vec(rstd, "rms_norm_fwd rstd", rows)
     if not eps > 0:
         raise ValueError(f"rms_norm_fwd: eps must be > 0, got {eps}")
-    native.check(_lib().lah_rms_norm_fwd(ptr(x), ptr(out), ptr(rstd), ptr(gamma), rows, C, float(eps), ptr(tile_group),
-                                         int(tile_rows), stream_ptr()), "lah_rms_norm_fwd")
+    if quant is None:
+        native.check(_lib().lah_rms_norm_fwd(ptr(x), ptr(out), ptr(rstd), ptr(gamma), rows, C, float(eps),
+                                             ptr(tile_group), int(tile_rows), stream_ptr()), "lah_rms_norm_fwd")
+    else:
+        if C % 256:
+            raise ValueError(f"rms_norm_fwd: the MXFP8 output needs a width that is a multiple of 256, got {C}")
+        _check_quant_out("rms_norm_fwd", quant, rows, C)
+        native.check(_lib().lah_rms_norm_fwd_q(ptr(x), ptr(out), ptr(rstd), ptr(gamma), rows, C, float(eps),
+                                               ptr(tile_group), int(tile_rows), ptr(quant.q), ptr(quant.sf),
+                                               stream_ptr()), "lah_rms_norm_fwd_q")
     native.count_launch()
     return out
 
@@ -978,13 +1000,31 @@ def _check_swiglu(h, what):
     return rows, inner
 
 
-def swiglu_fwd(h, *, out=None):
+def swiglu_fwd(h, *, out=None, quant=None, tile_group=None, total_rows=None):
     """a = silu(g) o u for h = [g | u] (bf16 [rows, 2 inner], inner a multiple of 128): bf16 [rows, inner], computed in
-    fp32 and rounded once"""
+    fp32 and rounded once.
+    :param quant: optional ops.fp8.MXFP8Tensor (activation layout) that additionally receives a as an MXFP8 GEMM operand,
+        quantised from the fp32 product before its bf16 rounding; ``out`` is then written only when given.  With it,
+        ``tile_group`` (int32, one entry per 128 rows, -1 = skipped) and ``total_rows`` (int32 [1] on the device: rows
+        past it are skipped) limit the rows processed"""
     rows, inner = _check_swiglu(h, "swiglu_fwd")
-    out = torch.empty(rows, inner, dtype=torch.bfloat16, device=h.device) if out is None else out
-    _bf16_rows(out, "swiglu_fwd out", (rows, inner))
-    native.check(_lib().lah_swiglu_fwd(ptr(h), ptr(out), rows, inner, stream_ptr()), "lah_swiglu_fwd")
+    if quant is None:
+        if tile_group is not None or total_rows is not None:
+            raise ValueError("swiglu_fwd: tile_group and total_rows apply to the MXFP8 output (quant) only")
+        out = torch.empty(rows, inner, dtype=torch.bfloat16, device=h.device) if out is None else out
+        _bf16_rows(out, "swiglu_fwd out", (rows, inner))
+        native.check(_lib().lah_swiglu_fwd(ptr(h), ptr(out), rows, inner, stream_ptr()), "lah_swiglu_fwd")
+    else:
+        if out is not None:
+            _bf16_rows(out, "swiglu_fwd out", (rows, inner))
+        _check_quant_out("swiglu_fwd", quant, rows, inner)
+        if tile_group is not None and (tile_group.dtype != torch.int32 or not tile_group.is_contiguous()
+                                       or tile_group.numel() < -(-rows // 128)):
+            raise ValueError(f"swiglu_fwd: tile_group must be a contiguous int32 tensor of >= {-(-rows // 128)} entries")
+        if total_rows is not None and (total_rows.dtype != torch.int32 or total_rows.numel() < 1):
+            raise ValueError("swiglu_fwd: total_rows must be an int32 device tensor of one element")
+        native.check(_lib().lah_swiglu_fwd_q(ptr(h), ptr(out), ptr(quant.q), ptr(quant.sf), rows, inner, ptr(tile_group),
+                                             ptr(total_rows), stream_ptr()), "lah_swiglu_fwd_q")
     native.count_launch()
     return out
 

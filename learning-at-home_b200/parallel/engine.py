@@ -29,7 +29,7 @@ from ..models.layers import FFN_SEG_KEYS as REF_KEYS, FFN_SEG_NAMES as SEG_NAMES
 from ..models.layers import EXPERT_LAYOUTS, GATED_LAYOUT, GatedFeedforwardBlock, gated_inner_dim
 from ..ops import fp8, gemm, kernels as K, native
 from ..ops.expert_blocks import (RowPlan, ffn_backward, ffn_forward, ffn_forward_fp8, swiglu_mlp_backward,
-                                 swiglu_mlp_forward)
+                                 swiglu_mlp_forward, swiglu_mlp_forward_fp8)
 
 #: eps of the gated expert's RMSNorm (GatedFeedforwardBlock's default)
 GATED_EPS = 1e-6
@@ -76,8 +76,9 @@ class DMoEConfig:
     shadow_experts: int = 8
     shadow_tol: float = 1.1
     shadow_min_rows: int = 1024
-    # "bf16" or "fp8": with "fp8" the three forward GEMMs of every expert run on block-scaled FP8 tensor cores (MXFP8:
-    # E4M3 + UE8M0 scale per 1x32 block, csrc/grouped_gemm_fp8.cu); dgrad / wgrad / optimizer are unchanged (bf16 / fp32)
+    # "bf16" or "fp8": with "fp8" the forward GEMMs of every expert (FeedforwardBlock: three; GatedFeedforwardBlock:
+    # [W1; W3] and W2) run on block-scaled FP8 tensor cores on the big expert path (MXFP8: E4M3 + UE8M0 scale per 1x32
+    # block, csrc/grouped_gemm_fp8.cu); dgrad / wgrad / optimizer are unchanged (bf16 / fp32)
     expert_dtype: str = "bf16"
     # which expert kernels run (csrc/):
     #   "big":   rows grouped per expert and padded to 256 rows, 128x256 wgmma tiles (grouped_gemm.cu) — compute-bound regime
@@ -169,9 +170,10 @@ class DMoEConfig:
                              "expert='swiglu' only")
         if self.inner_dim < 0:
             raise ValueError(f"DMoEConfig.inner_dim must be >= 0, got {self.inner_dim}")
-        if self.expert == "swiglu" and self.expert_dtype != "bf16":
-            raise ValueError("expert='swiglu' runs bf16 expert GEMMs only (its RMSNorm and SwiGLU kernels do not emit "
-                             f"MXFP8 operands); got expert_dtype={self.expert_dtype!r}")
+        if self.expert == "swiglu" and self.expert_dtype == "fp8" and (self.hidden % 256 or self.inner % 256):
+            # the FP8 forward runs on expert groups padded to 256 rows, which needs every GEMM width a multiple of 256
+            raise ValueError("expert='swiglu' with expert_dtype='fp8' needs hidden and the inner width to be multiples of "
+                             f"256; got hidden={self.hidden}, inner={self.inner}")
         for name in ("router_aux_loss_coef", "router_z_loss_coef"):
             v = float(getattr(self, name))
             if not math.isfinite(v) or v < 0.0:
@@ -655,11 +657,11 @@ class ExpertShard:
         self.pending_rows = torch.zeros(E_loc, dtype=torch.int32, device=device)
         self.pending_steps = torch.zeros(E_loc, dtype=torch.int32, device=device)
         self.fire = torch.zeros(E_loc, dtype=torch.int32, device=device)
-        self.w8 = None        # MXFP8 copies of w1/w2/w3 (expert_dtype == "fp8"), refreshed lazily from the bf16 mirror
+        self.w8 = None        # MXFP8 copies of the matrices (expert_dtype == "fp8"), refreshed lazily from the bf16 mirror
         self.w8_dirty = True
         if cfg.expert_dtype == "fp8" and ctx is not None:
             self.w8 = {n: fp8.MXFP8Tensor(shapes[n][0], slots, shapes[n][1], fp8.WEIGHT_TILE, device)
-                       for n in ("w1", "w2", "w3")}
+                       for n in self.matrices}
         self.reset_parameters(layer_index)
 
     @torch.no_grad()
@@ -795,7 +797,9 @@ class LayerWorkspace:
         for name in buffers["stats"]:
             setattr(self, name, torch.empty(R, **f32))
         self.xq = self.aq = None
-        if cfg.expert_dtype == "fp8":   # MXFP8 operands of the forward GEMMs (aq is shared by a1 and a2)
+        # MXFP8 operands of the forward GEMMs: FeedforwardBlock: xq = x, aq = a1 then a2; GatedFeedforwardBlock: xq = n,
+        # aq = a
+        if cfg.expert_dtype == "fp8":
             self.xq = fp8.MXFP8Tensor(R, 1, H, fp8.ACT_TILE, dev)
             self.aq = fp8.MXFP8Tensor(R, 1, I, fp8.ACT_TILE, dev)
         P = cfg.tokens_per_rank * cfg.k
@@ -1110,9 +1114,17 @@ class FusedDMoE(nn.Module):
             # GEMM columns are not stored, the wgrads read only the groups' rows and SwiGLU maps rows elementwise
             if wait is not None:  # the norm, not a GEMM, is the first consumer of the rows pushed by the peers
                 K.signal_wait(c.flags_off, K.SLOT_DISPATCH, epoch, c.status, signal=False, wait=True)
+            fp8_fwd = not c.small and cfg.expert_dtype == "fp8"
+            # FP8: the norm and the SwiGLU also write the next GEMM's MXFP8 operand (xq holds n, aq holds a); the bf16 n
+            # and a stay, for the weight gradients
             K.rms_norm_fwd(ws.xd, sh.raw_views["g"], GATED_EPS, out=ws.n, rstd=ws.rstd, tile_group=plan.tile_group,
-                           tile_rows=plan.tile_rows)
-            swiglu_mlp_forward(plan, sh.bf16["w13"], sh.bf16["w2"], ws.n, ws.h, ws.a, ws.yo, residual=ws.xd)
+                           tile_rows=plan.tile_rows, quant=ws.xq if fp8_fwd else None)
+            if fp8_fwd:
+                assert c.align == 256, "the FP8 path needs 256-row expert groups (hidden and inner multiples of 256)"
+                w8 = sh.fp8_weights()
+                swiglu_mlp_forward_fp8(plan, w8["w13"], w8["w2"], ws.xq, ws.h, ws.a, ws.aq, ws.yo, residual=ws.xd)
+            else:
+                swiglu_mlp_forward(plan, sh.bf16["w13"], sh.bf16["w2"], ws.n, ws.h, ws.a, ws.yo, residual=ws.xd)
         elif c.small or cfg.expert_dtype != "fp8":
             ffn_forward(plan, sh.bf16, sh.raw_views, ws.xd, (ws.h1, ws.a1, ws.h2, ws.a2),
                         (ws.mean1, ws.rstd1, ws.mean2, ws.rstd2), ws.yo, wait=wait)
