@@ -5,7 +5,6 @@ CPU: the configuration and its refusals, the oracles K.gate_topk_ref(bias=...) a
 schedule of the CPU layer and trainer, checkpoints, and the balance a small trainer reaches with either gate.
 GPU: the biased gate_topk and expert_bias_update kernels against the oracles, one layer on both expert paths, both expert
 kinds and both gates against the CPU oracle, and the trainer under its CUDA graph with its launch budget."""
-import ctypes
 import math
 
 import pytest
@@ -15,34 +14,21 @@ import lah_b200  # noqa
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import collapse, cpu_cfg, layer_against_the_oracle, load, run_gate, slots
+from routing_support import one_thread, step_counters  # noqa: F401 (fixtures)
 
 RATE = dict(expert_bias_update_rate=0.01)
-
-
-@pytest.fixture
-def one_thread():
-    """the CPU trainer tests run many tiny ops: one intra-op thread is faster"""
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
-
-
-def _cpu_cfg(**kw):
-    base = dict(hidden=64, grid_size=(4, 4), k=4, num_layers=1, in_features=16, tokens_per_rank=64, seed=5)
-    base.update(kw)
-    return E.DMoEConfig(**base)
 
 
 # ======================================================================================================== CPU: config
 def test_default_rate_is_zero_and_allocates_nothing():
     assert E.DMoEConfig().expert_bias_update_rate == 0.0
-    plain = E.FusedDMoE(_cpu_cfg())
-    zero = E.FusedDMoE(_cpu_cfg(expert_bias_update_rate=0.0))
+    plain = E.FusedDMoE(cpu_cfg())
+    zero = E.FusedDMoE(cpu_cfg(expert_bias_update_rate=0.0))
     assert plain.expert_bias is None and zero.expert_bias is None
     assert "expert_bias" not in dict(zero.named_buffers())
     assert list(plain.state_dict()) == list(zero.state_dict())
-    biased = E.FusedDMoE(_cpu_cfg(**RATE))
+    biased = E.FusedDMoE(cpu_cfg(**RATE))
     assert set(biased.state_dict()) == set(plain.state_dict()) | {"expert_bias"}
     assert biased.expert_bias.dtype == torch.float32 and torch.equal(biased.expert_bias, torch.zeros(16))
 
@@ -56,7 +42,7 @@ def test_config_refuses_bad_rates(rate):
 @pytest.mark.parametrize("expert", ["ffn", "swiglu"])
 @pytest.mark.parametrize("gate", ["product_key", "emulator"])
 def test_every_gate_and_expert_kind_accepts_a_rate(gate, expert):
-    cfg = _cpu_cfg(grid_size=(16,), gate_mode=gate, expert=expert, **RATE)
+    cfg = cpu_cfg(grid_size=(16,), gate_mode=gate, expert=expert, **RATE)
     for path in ("small", "big"):
         E.DMoEConfig(**{**cfg.__dict__, "expert_path": path})
     assert E.FusedDMoE(cfg).expert_bias.shape == (16,)
@@ -182,7 +168,7 @@ def _count_updates(monkeypatch):
 @pytest.mark.parametrize("m", [1, 2])
 def test_one_update_per_training_forward_and_micro_batch(monkeypatch, one_thread, m):
     calls = _count_updates(monkeypatch)
-    t = DMoETrainer(_cpu_cfg(num_layers=2, trainer_microbatches=m, **RATE))
+    t = DMoETrainer(cpu_cfg(num_layers=2, trainer_microbatches=m, **RATE))
     x, y = torch.randn(64, 16), torch.randint(0, 10, (64,))
     t.train_step(x, y)
     assert len(calls) == 2 * m
@@ -196,7 +182,7 @@ def test_one_update_per_training_forward_and_micro_batch(monkeypatch, one_thread
 
 
 def test_layer_update_uses_the_routed_pairs_of_the_forward():
-    layer = E.FusedDMoE(_cpu_cfg(**RATE)).train()
+    layer = E.FusedDMoE(cpu_cfg(**RATE)).train()
     with torch.no_grad():
         layer.expert_bias.copy_(torch.arange(16).float() / 8 - 1)
     before = layer.expert_bias.clone()
@@ -214,7 +200,7 @@ def test_layer_update_uses_the_routed_pairs_of_the_forward():
 
 
 def test_resumed_run_equals_the_continued_run(one_thread):
-    cfg = _cpu_cfg(num_layers=2, **RATE)
+    cfg = cpu_cfg(num_layers=2, **RATE)
     gen = torch.Generator().manual_seed(4)
     xs = [torch.randn(64, 16, generator=gen) for _ in range(6)]
     ys = [torch.randint(0, 10, (64,), generator=gen) for _ in range(6)]
@@ -237,38 +223,17 @@ def test_resumed_run_equals_the_continued_run(one_thread):
 
 def test_checkpoint_rules(one_thread):
     x, y = torch.randn(64, 16), torch.randint(0, 10, (64,))
-    biased = DMoETrainer(_cpu_cfg(**RATE))
+    biased = DMoETrainer(cpu_cfg(**RATE))
     biased.train_step(x, y)
     with pytest.raises(ValueError, match="expert_bias_update_rate"):
-        DMoETrainer(_cpu_cfg()).load_state_dict(biased.state_dict())
+        DMoETrainer(cpu_cfg()).load_state_dict(biased.state_dict())
     # a checkpoint without biases loads into a biased trainer with zero biases
-    plain = DMoETrainer(_cpu_cfg())
+    plain = DMoETrainer(cpu_cfg())
     plain.train_step(x, y)
     assert float(biased.model.blocks[0].expert_bias.abs().max()) > 0
     biased.load_state_dict(plain.state_dict())
     assert torch.equal(biased.model.blocks[0].expert_bias, torch.zeros(16))
     assert torch.equal(biased.flat_p, plain.flat_p)
-
-
-def _load(trainer, x):
-    """max / mean rows per expert of every layer on batch x (eval-mode routing, with the layers' biases)"""
-    out, h = [], trainer.model.stem(x)
-    with torch.no_grad():
-        for block in trainer.model.blocks:
-            idx, _ = K.gate_topk_ref(block.gate_logits(h, block.proj), block.grid_size, block.cfg.k, bias=block.expert_bias)
-            rows = torch.bincount(idx[idx >= 0].flatten(), minlength=block.cfg.num_experts).float()
-            out.append(float(rows.max() / rows.mean()))
-            h = block(h)
-    return out
-
-
-def _collapse(block, gate):
-    with torch.no_grad():
-        if gate == "product_key":   # the gate's bias favours experts 0 and 1
-            block.proj.bias[:2] += 2.0
-        else:                       # frozen keys whose first two columns win most rows
-            block.gating_pre_normalize.bias.fill_(0.5)
-            block.expert_keys[:, :2] += 0.5
 
 
 @pytest.mark.parametrize("gate", ["product_key", "emulator"])
@@ -281,13 +246,13 @@ def test_expert_bias_spreads_a_collapsed_router(one_thread, gate):
     x = protos[y] + 0.5 * torch.randn(128, 16, generator=gen)
     results = {}
     for rate in (0.0, 0.05):
-        cfg = _cpu_cfg(grid_size=(8,), k=2, num_layers=1, tokens_per_rank=128, lr=3e-3, gate_mode=gate,
-                       expert_bias_update_rate=rate)
+        cfg = cpu_cfg(grid_size=(8,), k=2, num_layers=1, tokens_per_rank=128, lr=3e-3, gate_mode=gate,
+                      expert_bias_update_rate=rate)
         t = DMoETrainer(cfg)
-        _collapse(t.model.blocks[0], gate)
-        before = _load(t, x)
+        collapse(t.model.blocks[0], gate)
+        before = load(t, x)
         losses = [t.train_step(x, y) for _ in range(120)]
-        results[rate] = (before, _load(t, x), losses)
+        results[rate] = (before, load(t, x), losses)
     (b0, a0, l0), (b1, a1, l1) = results[0.0], results[0.05]
     assert b0 == b1 and b0[0] > 3.0
     assert a1[0] < 0.6 * a0[0] and a1[0] < 1.5, (a0, a1)
@@ -295,91 +260,29 @@ def test_expert_bias_spreads_a_collapsed_router(one_thread, gate):
 
 
 # ======================================================================================================== GPU
-@pytest.fixture(scope="module")
-def step_counters():
-    """the gate adds the device token base (step counters [2:4]) to its failure-injection stream: install zeroed
-    counters for this module's direct kernel calls, and put back whatever was installed before"""
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    prev = lib.lah_get_epoch_base()
-    ctr = torch.zeros(4, dtype=torch.int32, device="cuda")
-    yield ctr
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev))
-
-
-def _run_gate(logits, grid, k, *, alive, rate, bias):
-    B = logits.shape[0]
-    idx = torch.full((B * k,), 12345, dtype=torch.int32, device="cuda")
-    pos, w = torch.full_like(idx, 12345), torch.full((B * k,), 7.0, device="cuda")
-    counts = torch.zeros(math.prod(grid), dtype=torch.int32, device="cuda")
-    K.gate_topk(logits, grid, k, alive=alive, failure_rate=rate, seed=99, token_offset=0, idx=idx, w=w, pos=pos,
-                counts=counts, bias=bias)
-    torch.cuda.synchronize()
-    return idx.view(B, k), w.view(B, k), pos.view(B, k), counts
-
-
-def _u64(c):
-    """a uint64 constant as the int64 with the same bits"""
-    return c - (1 << 64) if c >= 1 << 63 else c
-
-
-def _shr(x, n):
-    """logical right shift of int64 tensors holding uint64 bits"""
-    return (x >> n) & ((1 << (64 - n)) - 1)
-
-
-def _fail_mask(B, E_, rate, seed=99):
-    """K.gate_fail_mask_ref (token base 0) on the device: int64 tensors wrap modulo 2**64 like the kernel's uint64"""
-    tok = torch.arange(B, dtype=torch.int64, device="cuda") * 0x100000001B3
-    x = _u64(seed) ^ (tok[:, None] + torch.arange(E_, dtype=torch.int64, device="cuda")[None, :])
-    x = x + _u64(0x9E3779B97F4A7C15)
-    x = (x ^ _shr(x, 30)) * _u64(0xBF58476D1CE4E5B9)
-    x = (x ^ _shr(x, 27)) * _u64(0x94D049BB133111EB)
-    x = x ^ _shr(x, 31)
-    return _shr(x, 40).double() / 2.0 ** 24 < float(torch.tensor(rate, dtype=torch.float32))
-
-
-def _slots(idx):
-    """pos oracle: the number of earlier pairs (token-major) routed to the same expert; 0 for missing pairs"""
-    flat = idx.reshape(-1).long()
-    order = torch.argsort(flat, stable=True)
-    srt = flat[order]
-    first = torch.searchsorted(srt, srt, side="left")
-    pos = torch.empty_like(flat)
-    pos[order] = torch.arange(flat.numel(), device=flat.device) - first
-    return torch.where(flat >= 0, pos, torch.zeros_like(pos)).view_as(idx)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("B", [1, 7, 256, 65536])
 @pytest.mark.parametrize("grid", [(64,), (8, 8), (32, 32), (64, 64), (4096,), (4, 4, 4, 4)])
 def test_biased_gate_topk_against_the_oracle(step_counters, grid, B):
     """dyadic logits and biases: the keys are exact in any summation order, so idx, pos and counts must be equal"""
-    K.set_step_counters(step_counters)
-    step_counters.zero_()
     E_ = math.prod(grid)
     gen = torch.Generator(device="cuda").manual_seed(B * 7 + E_)
     logits = torch.randint(-12, 13, (B, sum(grid)), generator=gen, device="cuda").float() / 4
     bias = torch.randint(-8, 9, (E_,), generator=gen, device="cuda").float() / 8
     alive = (torch.rand(E_, generator=gen, device="cuda") > 0.2).to(torch.uint8)
     rate = 0.1
-    fail = _fail_mask(B, E_, rate)
-    n = min(B, 7)
-    assert torch.equal(fail[:n].cpu(), K.gate_fail_mask_ref(n, E_, rate, 99, 0))
+    fail = K.gate_fail_mask_ref(B, E_, rate, 99, 0).cuda()
     for k in range(1, 9):
-        idx, w, pos, counts = _run_gate(logits, grid, k, alive=alive, rate=rate, bias=bias)
+        idx, w, pos, counts, _, _ = run_gate(logits, grid, k, alive=alive, rate=rate, bias=bias)
         ridx, rw = K.gate_topk_ref(logits, grid, k, alive=alive, fail_mask=fail, bias=bias)
         assert torch.equal(idx.long(), ridx), (k, int((idx.long() != ridx).any(1).sum()))
-        assert torch.equal(pos.long(), _slots(ridx))
+        assert torch.equal(pos.long(), slots(ridx))
         assert torch.equal(counts.long(), torch.bincount(ridx[ridx >= 0], minlength=E_))
         assert float((w.double() - rw.double()).abs().max()) < 1e-6
         # bias=None is the zero bias, bit for bit
-        plain = _run_gate(logits, grid, k, alive=alive, rate=rate, bias=None)
-        zero = _run_gate(logits, grid, k, alive=alive, rate=rate, bias=torch.zeros_like(bias))
-        assert all(torch.equal(a, b) for a, b in zip(plain, zero))
+        plain = run_gate(logits, grid, k, alive=alive, rate=rate, bias=None)
+        zero = run_gate(logits, grid, k, alive=alive, rate=rate, bias=torch.zeros_like(bias))
+        assert all(torch.equal(a, b) for a, b in zip(plain[:4], zero[:4]))
 
 
 @pytest.mark.gpu
@@ -425,11 +328,6 @@ def test_expert_bias_update_is_bit_equal_to_the_oracle(E_):
                 assert torch.equal(got.cpu(), bias)
 
 
-def _rel(a, b):
-    a, b = a.detach().float(), b.detach().float()
-    return float((a - b).norm() / b.norm().clamp_min(1e-12))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("gate", ["emulator", "product_key"])
 @pytest.mark.parametrize("expert", ["ffn", "swiglu"])
@@ -439,39 +337,16 @@ def test_layer_against_the_cpu_oracle(path, expert, gate):
     grid = (16,) if gate == "emulator" else (4, 4)
     cfg = E.DMoEConfig(hidden=512, grid_size=grid, k=4, num_layers=1, tokens_per_rank=512, expert=expert,
                        expert_path=path, gate_mode=gate, expert_bias_update_rate=0.01)
-    ctx = E.EngineContext(cfg)
-    try:
-        layer = E.FusedDMoE(cfg, ctx).cuda().train()
-        assert ctx.small == (path == "small")
-        oracle = E.FusedDMoE(cfg, device=torch.device("cuda")).cuda().train()
-        oracle.ref_emulate_bf16 = True
-        bias0 = (torch.randint(-8, 9, (16,)).float() / 8).cuda()
-        with torch.no_grad():
-            layer.expert_bias.copy_(bias0)
-            oracle.load_state_dict(layer.state_dict())
-            oracle.shard.p.copy_(layer.shard.p[:oracle.shard.p.numel()])
-        B = 512
-        x = torch.randn(B, 512, device="cuda").to(torch.bfloat16)
-        gy = torch.randn(B, 512, device="cuda").to(torch.bfloat16)
-        logits = layer.gate_logits(x, layer.proj).detach()
-        lg = logits.clone().requires_grad_(True)
-        y = E._FusedDMoEFunction.apply(x, lg, layer)
-        y.backward(gy)
-        torch.cuda.synchronize()
-        ctx.check_status()
-        lr_ = logits.clone().requires_grad_(True)
-        yr = oracle._forward_ref(x.float(), lr_, emulate_bf16=True)
-        yr.backward(gy.float())
-        ridx, _ = K.gate_topk_ref(logits, grid, cfg.k, alive=ctx.alive, bias=bias0)
-        assert not torch.equal(ridx, K.gate_topk_ref(logits, grid, cfg.k, alive=ctx.alive)[0])   # the bias mattered
-        assert torch.equal(layer.ws.idx[:B * cfg.k].view(B, cfg.k).long(), ridx)
-        assert torch.equal(ctx.cnt_all[0, :16].long(), torch.bincount(ridx.flatten(), minlength=16))
-        assert torch.equal(layer.expert_bias, oracle.expert_bias)
-        assert torch.equal(layer.expert_bias, K.expert_bias_update_ref(ctx.cnt_all[:1, :16], bias0, 0.01))
-        assert not torch.equal(layer.expert_bias, bias0)
-        assert _rel(y, yr) < 2e-2 and _rel(lg.grad, lr_.grad) < 5e-2
-    finally:
-        ctx.close()
+
+    def check(r):
+        assert r.ctx.small == (path == "small")
+        unbiased = K.gate_topk_ref(r.logits, grid, cfg.k, alive=r.ctx.alive)[0]
+        assert not torch.equal(r.ridx, unbiased)   # the bias mattered
+        assert torch.equal(r.layer.expert_bias, r.oracle.expert_bias)
+        assert torch.equal(r.layer.expert_bias, K.expert_bias_update_ref(r.ctx.cnt_all[:1, :16], r.bias0, 0.01))
+        assert not torch.equal(r.layer.expert_bias, r.bias0)
+
+    layer_against_the_oracle(cfg, bias_step=1 / 8, check=check)
 
 
 def _trainer_cfg(path, gate, **kw):

@@ -8,13 +8,11 @@ GPU: layout_exchange, scatter_rows, combine_rows and gate_bwd against their orac
 under collapsed routing, bit-identity with f = 0 when nothing drops, graph replay, launch counts, and (two GPUs) the
 sharded layer against the whole-batch oracle.
 """
-import ctypes
 import math
 import os
 import subprocess
 import sys
 import zlib
-from types import SimpleNamespace
 
 import pytest
 import torch
@@ -23,28 +21,11 @@ import lah_b200  # noqa: F401
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import F64, cpu_cfg, layer_against_the_oracle, rel
+from routing_support import one_thread, rt, world1  # noqa: F401 (fixtures)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BF16 = torch.bfloat16
-
-
-@pytest.fixture
-def one_thread():
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
-
-
-def _cpu_cfg(**kw):
-    base = dict(hidden=64, grid_size=(4, 4), k=4, num_layers=1, in_features=16, tokens_per_rank=64, seed=5)
-    base.update(kw)
-    return E.DMoEConfig(**base)
-
-
-def _rel(a, b):
-    a, b = a.detach().double(), b.detach().double()
-    return float((a - b).norm() / b.norm().clamp_min(1e-30))
 
 
 # ======================================================================================================== CPU: config
@@ -104,7 +85,7 @@ def _run_ref(layer, x, logits, gy):
 @pytest.mark.parametrize("expert", ["ffn", "swiglu"])
 def test_a_factor_that_drops_nothing_is_identical_to_dropless(expert):
     torch.manual_seed(0)
-    cfgs = [_cpu_cfg(expert=expert, expert_capacity_factor=f) for f in (0.0, 64.0)]
+    cfgs = [cpu_cfg(expert=expert, expert_capacity_factor=f) for f in (0.0, 64.0)]
     layers = [E.FusedDMoE(c).train() for c in cfgs]
     layers[1].load_state_dict(layers[0].state_dict())
     layers[1].shard.p.copy_(layers[0].shard.p)
@@ -120,7 +101,7 @@ def test_a_factor_that_drops_nothing_is_identical_to_dropless(expert):
 def test_top1_capacity_one_returns_later_tokens_unchanged():
     """k = 1, C = 1, softmax router: the first token of each expert goes through it, every later one returns exactly x"""
     torch.manual_seed(1)
-    layer = E.FusedDMoE(_cpu_cfg(grid_size=(8,), k=1, expert_capacity_factor=1e-9)).eval()
+    layer = E.FusedDMoE(cpu_cfg(grid_size=(8,), k=1, expert_capacity_factor=1e-9)).eval()
     x = torch.randn(40, 64)
     with torch.no_grad():
         y = layer(x)
@@ -168,8 +149,8 @@ def _identity_formula(layer, x, logits, kept, idx, score, norm, scale):
 def test_cpu_layer_gradients_with_drops_equal_the_identity_formula(score, norm):
     torch.manual_seed(2)
     scale = 1.0 if score == "softmax" and norm else 2.5
-    cfg = _cpu_cfg(k=2, tokens_per_rank=32, router_score=score, norm_topk_prob=norm, routed_scaling_factor=scale,
-                   expert_capacity_factor=0.75)
+    cfg = cpu_cfg(k=2, tokens_per_rank=32, router_score=score, norm_topk_prob=norm, routed_scaling_factor=scale,
+                  expert_capacity_factor=0.75)
     layer = E.FusedDMoE(cfg).eval()   # eval: the leaves of the expert parameters are not created
     x = torch.randn(24, 64)
     with torch.no_grad():
@@ -189,9 +170,9 @@ def test_cpu_layer_gradients_with_drops_equal_the_identity_formula(score, norm):
     assert (C2, dropped2) == (C, dropped)
     ref = _identity_formula(layer, xd, lg, kept, idx, score, norm, scale)
     (ref * gy.double()).sum().backward()
-    assert _rel(out, ref) < 1e-5
-    assert _rel(xr.grad, xd.grad) < 1e-5 and _rel(proj_w.grad, pw.grad) < 1e-5, (_rel(xr.grad, xd.grad),
-                                                                                   _rel(proj_w.grad, pw.grad))
+    assert rel(out, ref, *F64) < 1e-5
+    errs = rel(xr.grad, xd.grad, *F64), rel(proj_w.grad, pw.grad, *F64)
+    assert errs[0] < 1e-5 and errs[1] < 1e-5, errs
 
 
 def test_router_losses_see_the_routed_counts():
@@ -199,7 +180,7 @@ def test_router_losses_see_the_routed_counts():
     losses = []
     for f in (0.0, 0.25):
         torch.manual_seed(3)
-        layer = E.FusedDMoE(_cpu_cfg(router_aux_loss_coef=0.01, router_z_loss_coef=1e-3, expert_capacity_factor=f)).train()
+        layer = E.FusedDMoE(cpu_cfg(router_aux_loss_coef=0.01, router_z_loss_coef=1e-3, expert_capacity_factor=f)).train()
         with torch.no_grad():
             layer.proj.bias[:4] += torch.tensor([3.0, 0.0, 0.0, 0.0])
         layer(torch.randn(64, 64, generator=torch.Generator().manual_seed(0)))
@@ -212,7 +193,7 @@ def test_router_losses_see_the_routed_counts():
 def test_experts_step_on_kept_rows_only():
     """C = 1 on a gate that sends everything to one grid row: only the experts with a kept row are stepped, once"""
     torch.manual_seed(4)
-    layer = E.FusedDMoE(_cpu_cfg(k=1, expert_capacity_factor=1e-9)).train()
+    layer = E.FusedDMoE(cpu_cfg(k=1, expert_capacity_factor=1e-9)).train()
     x = torch.randn(32, 64)
     (layer(x) * torch.randn(32, 64)).sum().backward()
     idx, _ = K.gate_topk_ref(layer.gate_logits(x, layer.proj).detach(), layer.grid_size, 1)
@@ -229,13 +210,13 @@ def test_cpu_trainer_learns_and_resumes(one_thread):
     gen = torch.Generator().manual_seed(6)
     xs = [torch.randn(64, 16, generator=gen) for _ in range(12)]
     ys = [(x[:, 0] > 0).long() for x in xs]
-    cfg = _cpu_cfg(num_layers=2, expert_capacity_factor=1.0, lr=3e-3)
+    cfg = cpu_cfg(num_layers=2, expert_capacity_factor=1.0, lr=3e-3)
     torch.manual_seed(0)
     a = DMoETrainer(cfg)
     losses = [a.train_step(x, y) for x, y in zip(xs[:8], ys[:8])]
     assert losses[-1] < losses[0], losses
     state = a.state_dict()
-    plain = DMoETrainer(_cpu_cfg(num_layers=2))   # checkpoints load across the setting
+    plain = DMoETrainer(cpu_cfg(num_layers=2))   # checkpoints load across the setting
     plain.load_state_dict(state)
     b = DMoETrainer(cfg)
     b.load_state_dict(plain.state_dict())
@@ -245,45 +226,6 @@ def test_cpu_trainer_learns_and_resumes(one_thread):
 
 
 # ======================================================================================================== GPU: kernels
-@pytest.fixture(scope="module")
-def world1():
-    """a world-1 symmetric heap made directly (no EngineContext): flags, the count table and one receive region"""
-    from lah_b200.ops import native
-    from lah_b200.parallel.symmetric import SymmetricHeap
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    lib.lah_get_poison_word.restype = ctypes.c_void_p
-    prev_ctr, prev_poison = lib.lah_get_epoch_base(), lib.lah_get_poison_word()
-    heap = SymmetricHeap(80 << 20)
-    flags, flags_off = heap.alloc((K.NUM_SLOTS, K.MAX_WORLD), torch.int32)
-    cnt_all, cnt_all_off = heap.alloc((K.MAX_WORLD, K.LAYOUT_MAX_E), torch.int32)
-    region, region_off = heap.alloc((64 << 20,), torch.uint8)
-    i32 = dict(dtype=torch.int32, device="cuda")
-    w = SimpleNamespace(heap=heap, native=native, flags=flags, flags_off=flags_off, cnt_all=cnt_all,
-                        cnt_all_off=cnt_all_off, region=region, region_off=region_off, step_ctr=torch.zeros(4, **i32),
-                        status=torch.zeros(4, **i32), done_counter=torch.zeros(1, **i32))
-    yield w
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev_ctr))
-    lib.lah_set_poison_word(ctypes.c_void_p(prev_poison))
-    heap.close()
-
-
-@pytest.fixture
-def rt(world1):
-    w = world1
-    K.set_peers(w.heap.peer_bases, 0)
-    K.set_multicast(0)
-    K.set_step_counters(w.step_ctr)
-    K.set_poison_word(w.status)
-    w.status.zero_()
-    w.step_ctr.zero_()
-    w.done_counter.zero_()
-    return w
-
-
 def _counts(kind, gen):
     if kind == "sparse":
         return (torch.randint(0, 40, (64,), generator=gen) * (torch.rand(64, generator=gen) > 0.5)).to(torch.int32)
@@ -509,54 +451,29 @@ def test_pass_through_gate_bwd_matches_float64(rt, grid, H, k, score, norm):
 
 
 # ======================================================================================================== GPU: layer
-def _collapse(layer, cfg):
+def _collapse(layer):
     """bias the gate so that most tokens pick experts of the first grid row (the first rank's at world > 1)"""
-    with torch.no_grad():
-        if cfg.gate_mode == "emulator":
-            layer.expert_keys[:, : cfg.num_experts // 4] += 0.5 * layer.expert_keys.abs().mean()
-        else:
-            layer.proj.bias[0] += 3.0
+    cfg = layer.cfg
+    if cfg.gate_mode == "emulator":
+        layer.expert_keys[:, : cfg.num_experts // 4] += 0.5 * layer.expert_keys.abs().mean()
+    else:
+        layer.proj.bias[0] += 3.0
 
 
-def _layer_against_the_oracle(cfg, B=512):
-    ctx = E.EngineContext(cfg)
-    try:
-        layer = E.FusedDMoE(cfg, ctx).cuda().train()
-        _collapse(layer, cfg)
-        oracle = E.FusedDMoE(cfg, device=torch.device("cuda")).cuda().train()
-        oracle.ref_emulate_bf16 = True
-        with torch.no_grad():
-            oracle.load_state_dict(layer.state_dict())
-            oracle.shard.p.copy_(layer.shard.p[:oracle.shard.p.numel()])
-        x = torch.randn(B, cfg.hidden, device="cuda").to(BF16)
-        gy = torch.randn(B, cfg.hidden, device="cuda").to(BF16)
-        logits = layer.gate_logits(x, layer.proj).detach()
-        xf, lg = x.clone().requires_grad_(True), logits.clone().requires_grad_(True)
-        y = E._FusedDMoEFunction.apply(xf, lg, layer)
-        got_idx = layer.ws.idx[:B * cfg.k].view(B, cfg.k).long().clone()
-        y.backward(gy)
-        torch.cuda.synchronize()
-        ctx.check_status()
-        xr, lr_ = x.float().requires_grad_(True), logits.clone().requires_grad_(True)
-        yr = oracle._forward_ref(xr, lr_, emulate_bf16=True)
-        yr.backward(gy.float())
-        oracle.apply_expert_gradients_ref()
-        C, dropped = layer.ws.capacity_stats.tolist()
-        assert (C, dropped) == oracle._ref_capacity and dropped > 0, ((C, dropped), oracle._ref_capacity)
-        assert torch.equal(got_idx, K.gate_topk_ref(logits, cfg.grid_size, cfg.k, alive=ctx.alive,
-                                                    score=cfg.router_score, scale=cfg.routed_scaling_factor)[0])
-        kept, _, _ = K.capacity_keep_ref(got_idx, cfg.expert_capacity_factor, cfg.num_experts)
-        pr = layer.ws.pair_row[:B * cfg.k].view(B, cfg.k).cpu()
-        assert torch.equal(pr[~kept.cpu() & (got_idx.cpu() >= 0)], torch.full_like(pr[~kept.cpu() & (got_idx.cpu() >= 0)], -1))
-        assert bool((pr[kept.cpu()] >= 0).all())
-        errs = dict(y=_rel(y, yr), dx=_rel(xf.grad, xr.grad), dlogits=_rel(lg.grad, lr_.grad))
-        assert torch.equal(layer.shard.step.cpu(), oracle.shard.step.cpu())
-        p, pr_ = layer.shard.p[:oracle.shard.p.numel()], oracle.shard.p
-        errs["params_mean_abs"] = float((p - pr_).abs().mean())
-        assert errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dlogits"] < 5e-2 and errs["params_mean_abs"] < 1e-4, errs
-        return errs
-    finally:
-        ctx.close()
+def _check(r):
+    """the capacity and the dropped pairs of the oracle, pass-through rows for the dropped pairs, and the experts the
+    oracle's update steps and moves"""
+    cfg, B = r.layer.cfg, r.idx.shape[0]
+    r.oracle.apply_expert_gradients_ref()
+    C, dropped = r.layer.ws.capacity_stats.tolist()
+    assert (C, dropped) == r.oracle._ref_capacity and dropped > 0, ((C, dropped), r.oracle._ref_capacity)
+    kept, _, _ = K.capacity_keep_ref(r.idx, cfg.expert_capacity_factor, cfg.num_experts)
+    pr = r.layer.ws.pair_row[:B * cfg.k].view(B, cfg.k).cpu()
+    assert torch.equal(pr[~kept.cpu() & (r.idx.cpu() >= 0)], torch.full_like(pr[~kept.cpu() & (r.idx.cpu() >= 0)], -1))
+    assert bool((pr[kept.cpu()] >= 0).all())
+    assert torch.equal(r.layer.shard.step.cpu(), r.oracle.shard.step.cpu())
+    params_mean_abs = float((r.layer.shard.p[:r.oracle.shard.p.numel()] - r.oracle.shard.p).abs().mean())
+    assert params_mean_abs < 1e-4, params_mean_abs
 
 
 @pytest.mark.gpu
@@ -568,7 +485,7 @@ def test_collapsed_layer_matches_the_cpu_oracle(path, expert, score):
     extra = dict(routed_scaling_factor=2.5) if score == "sigmoid" else {}
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=512, expert=expert,
                        expert_path=path, router_score=score, expert_capacity_factor=1.0, **extra)
-    _layer_against_the_oracle(cfg)
+    layer_against_the_oracle(cfg, prepare=_collapse, dx=True, precision=F64, check=_check)
 
 
 @pytest.mark.gpu
@@ -577,7 +494,7 @@ def test_collapsed_layer_with_a_shared_expert_matches_the_cpu_oracle(path):
     torch.manual_seed(4)
     cfg = E.DMoEConfig(hidden=512, grid_size=(4, 4), k=4, num_layers=1, tokens_per_rank=512, expert="swiglu",
                        shared_inner_dim=256, expert_path=path, expert_capacity_factor=1.25, norm_topk_prob=False)
-    _layer_against_the_oracle(cfg)
+    layer_against_the_oracle(cfg, prepare=_collapse, dx=True, precision=F64, check=_check)
 
 
 def _trainer_cfg(path, **kw):

@@ -17,32 +17,19 @@ import lah_b200  # noqa
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, baseline_fast, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import collapse, cpu_cfg, layer_against_the_oracle, run_gate, slots
+from routing_support import one_thread, step_counters  # noqa: F401 (fixtures)
 
 SIG = dict(router_score="sigmoid")
 CPU = torch.device("cpu")   # the CPU trainer tests run on the CPU path on a GPU machine too
-
-
-@pytest.fixture
-def one_thread():
-    """the CPU trainer tests run many tiny ops: one intra-op thread is faster"""
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
-
-
-def _cpu_cfg(**kw):
-    base = dict(hidden=64, grid_size=(4, 4), k=4, num_layers=1, in_features=16, tokens_per_rank=64, seed=5)
-    base.update(kw)
-    return E.DMoEConfig(**base)
 
 
 # ======================================================================================================== CPU: config
 def test_defaults_and_state_dict_keys():
     cfg = E.DMoEConfig()
     assert cfg.n_group == 1 and cfg.topk_group == 1
-    plain = E.FusedDMoE(_cpu_cfg())
-    grouped = E.FusedDMoE(_cpu_cfg(n_group=4, topk_group=2))
+    plain = E.FusedDMoE(cpu_cfg())
+    grouped = E.FusedDMoE(cpu_cfg(n_group=4, topk_group=2))
     assert (plain.n_group, plain.topk_group) == (1, 1) and (grouped.n_group, grouped.topk_group) == (4, 2)
     assert list(plain.state_dict()) == list(grouped.state_dict())
 
@@ -58,13 +45,13 @@ def test_defaults_and_state_dict_keys():
 ])
 def test_config_refusals(kw, match):
     with pytest.raises(ValueError, match=match):
-        _cpu_cfg(**kw)
+        cpu_cfg(**kw)
 
 
 def test_config_accepts_the_feasible_corners():
-    _cpu_cfg(n_group=16, topk_group=4, k=4)         # G = E, k = M
-    _cpu_cfg(n_group=8, topk_group=2, k=4)          # k = M * E / G
-    _cpu_cfg(grid_size=(64, 64), n_group=64, topk_group=8, k=8)
+    cpu_cfg(n_group=16, topk_group=4, k=4)         # G = E, k = M
+    cpu_cfg(n_group=8, topk_group=2, k=4)          # k = M * E / G
+    cpu_cfg(grid_size=(64, 64), n_group=64, topk_group=8, k=8)
     with pytest.raises(ValueError, match="at most 4096"):
         K.check_expert_groups("x", 8192, 2, 1)
 
@@ -74,7 +61,7 @@ def test_config_accepts_the_feasible_corners():
                                  baseline_fast.FastBaselineTrainer])
 def test_baseline_arms_refuse_group_limited_routing(arm):
     with pytest.raises(ValueError, match="n_group=1"):
-        arm(_cpu_cfg(n_group=4, topk_group=2))
+        arm(cpu_cfg(n_group=4, topk_group=2))
 
 
 # ======================================================================================================== CPU: oracle
@@ -206,7 +193,7 @@ def test_layer_gate_gradient_equals_float64_autograd_with_the_groups_fixed():
     torch.manual_seed(0)
     for score in ("softmax", "sigmoid"):
         kw = dict(routed_scaling_factor=2.5, **SIG) if score == "sigmoid" else {}
-        layer = E.FusedDMoE(_cpu_cfg(grid_size=(16,), n_group=4, topk_group=2, **kw)).train()
+        layer = E.FusedDMoE(cpu_cfg(grid_size=(16,), n_group=4, topk_group=2, **kw)).train()
         x = torch.randn(32, 64)
         logits = layer.gate_logits(x, layer.proj).detach().requires_grad_(True)
         out = layer._forward_ref(x, logits)
@@ -266,11 +253,10 @@ def test_v3_shaped_cpu_trainer_spreads_a_collapsed_gate_within_its_groups(one_th
     x = protos[y] + 0.5 * torch.randn(128, 16, generator=gen)
     results = {}
     for rate in (0.0, 0.01):
-        cfg = _cpu_cfg(grid_size=(16,), k=2, tokens_per_rank=128, lr=3e-3, expert_bias_update_rate=rate,
-                       routed_scaling_factor=2.0, n_group=4, topk_group=2, **SIG)
+        cfg = cpu_cfg(grid_size=(16,), k=2, tokens_per_rank=128, lr=3e-3, expert_bias_update_rate=rate,
+                      routed_scaling_factor=2.0, n_group=4, topk_group=2, **SIG)
         t = DMoETrainer(cfg, device=CPU)
-        with torch.no_grad():
-            t.model.blocks[0].proj.bias[:2] += 2.0
+        collapse(t.model.blocks[0], "product_key")
         before = _load(t, x)
         losses = []
         for _ in range(120):
@@ -288,7 +274,7 @@ def test_checkpoints_load_across_groupings(one_thread):
     xs = [torch.randn(64, 16, generator=gen) for _ in range(6)]
     ys = [torch.randint(0, 10, (64,), generator=gen) for _ in range(6)]
     base = dict(num_layers=2, expert_bias_update_rate=1e-3, routed_scaling_factor=2.5, **SIG)
-    grouped, plain = _cpu_cfg(n_group=4, topk_group=2, **base), _cpu_cfg(**base)
+    grouped, plain = cpu_cfg(n_group=4, topk_group=2, **base), cpu_cfg(**base)
     for src_cfg, dst_cfg in ((grouped, plain), (plain, grouped)):
         a = DMoETrainer(src_cfg, device=CPU)
         for x, y in zip(xs[:3], ys[:3]):
@@ -308,45 +294,6 @@ def test_checkpoints_load_across_groupings(one_thread):
 
 
 # ======================================================================================================== GPU
-@pytest.fixture(scope="module")
-def step_counters():
-    """the gate adds the device token base (step counters [2:4]) to its failure-injection stream: install zeroed
-    counters for this module's direct kernel calls, and put back whatever was installed before"""
-    import ctypes
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    prev = lib.lah_get_epoch_base()
-    ctr = torch.zeros(4, dtype=torch.int32, device="cuda")
-    K.set_step_counters(ctr)
-    yield ctr
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev))
-
-
-def _run_gate(logits, grid, k, *, alive, rate, bias, score="softmax", scale=1.0, G=1, M=1):
-    B = logits.shape[0]
-    idx = torch.full((B * k,), 12345, dtype=torch.int32, device="cuda")
-    pos, w = torch.full_like(idx, 12345), torch.full((B * k,), 7.0, device="cuda")
-    sig = torch.full((B * k,), 7.0, device="cuda") if score == "sigmoid" else None
-    counts = torch.zeros(math.prod(grid), dtype=torch.int32, device="cuda")
-    K.gate_topk(logits, grid, k, alive=alive, failure_rate=rate, seed=99, token_offset=0, idx=idx, w=w, pos=pos,
-                counts=counts, bias=bias, score=score, scale=scale, sig=sig, n_group=G, topk_group=M)
-    torch.cuda.synchronize()
-    return idx.view(B, k), w.view(B, k), pos.view(B, k), counts, None if sig is None else sig.view(B, k)
-
-
-def _slots(idx):
-    flat = idx.reshape(-1).long()
-    order = torch.argsort(flat, stable=True)
-    srt = flat[order]
-    first = torch.searchsorted(srt, srt, side="left")
-    pos = torch.empty_like(flat)
-    pos[order] = torch.arange(flat.numel(), device=flat.device) - first
-    return torch.where(flat >= 0, pos, torch.zeros_like(pos)).view_as(idx)
-
-
 def _gaps_clear(v, n, tol):
     """rows of v (sorted descending, -inf = missing) whose n leading entries are pairwise separated by more than tol"""
     v = v[:, :n]
@@ -381,7 +328,6 @@ GROUPINGS = {   # (n_group, topk_group) per grid: G = E, group sizes that are no
 @pytest.mark.parametrize("B", [1, 7, 256, 65536])
 @pytest.mark.parametrize("grid", list(GROUPINGS))
 def test_grouped_gate_topk_against_the_oracle(step_counters, grid, B):
-    step_counters.zero_()
     E_ = math.prod(grid)
     gen = torch.Generator(device="cuda").manual_seed(B * 3 + E_)
     # softmax arms: dyadic logits and biases, every key and group score is exact in any order
@@ -401,24 +347,25 @@ def test_grouped_gate_topk_against_the_oracle(step_counters, grid, B):
         dead = ~alive.bool().view(1, -1) | fail
         for k in range(1, min(8, M * gsz) + 1):
             for b in (None, dbias):
-                idx, w, pos, counts, _ = _run_gate(dyadic, grid, k, alive=alive, rate=rate, bias=b, G=G, M=M)
+                idx, w, pos, counts, _, _ = run_gate(dyadic, grid, k, alive=alive, rate=rate, bias=b, n_group=G,
+                                                     topk_group=M)
                 ridx, rw = K.gate_topk_ref(dyadic, grid, k, alive=alive, fail_mask=fail, bias=b, n_group=G,
                                            topk_group=M)
                 assert torch.equal(idx.long(), ridx), (G, M, k, b is None, int((idx.long() != ridx).any(1).sum()))
-                assert torch.equal(pos.long(), _slots(ridx))
+                assert torch.equal(pos.long(), slots(ridx))
                 assert torch.equal(counts.long(), torch.bincount(ridx[ridx >= 0], minlength=E_))
                 assert float((w - rw).abs().max()) < 2e-6, (G, M, k)
             c = 2.5 if k % 2 else 1.0
             for b in (None, cbias):
-                idx, w, pos, counts, sig = _run_gate(logits, grid, k, alive=alive, rate=rate, bias=b, score="sigmoid",
-                                                     scale=c, G=G, M=M)
+                idx, w, pos, counts, _, _ = run_gate(logits, grid, k, alive=alive, rate=rate, bias=b, score="sigmoid",
+                                                     scale=c, n_group=G, topk_group=M)
                 ridx, rw = K.gate_topk_ref(logits, grid, k, alive=alive, fail_mask=fail, bias=b, score="sigmoid",
                                            scale=c, n_group=G, topk_group=M)
                 clear = _clear_tokens(K.product_key_scores(logits, grid), dead, b, G, M, k, "sigmoid")
                 unclear += int((~clear).sum())
                 total += B
                 assert torch.equal(idx.long()[clear], ridx[clear]), (G, M, k, b is None)
-                assert torch.equal(pos.long(), _slots(idx.long()))
+                assert torch.equal(pos.long(), slots(idx.long()))
                 assert torch.equal(counts.long(), torch.bincount(idx.long()[idx >= 0], minlength=E_))
                 same = (idx.long() == ridx).all(1, keepdim=True)
                 assert float(torch.where(same, w.double() - rw.double(), 0.0).abs().max()) < 2e-6 * c, (G, M, k)
@@ -429,7 +376,6 @@ def test_grouped_gate_topk_against_the_oracle(step_counters, grid, B):
 @pytest.mark.gpu
 @pytest.mark.parametrize("grid", [(64,), (8, 8), (2, 3, 4), (64, 64)])
 def test_identities_give_the_bits_of_the_ungrouped_gate(step_counters, grid):
-    step_counters.zero_()
     E_ = math.prod(grid)
     gen = torch.Generator(device="cuda").manual_seed(E_)
     logits = torch.randn(999, sum(grid), generator=gen, device="cuda")
@@ -438,11 +384,11 @@ def test_identities_give_the_bits_of_the_ungrouped_gate(step_counters, grid):
     for score, scale in (("softmax", 1.0), ("sigmoid", 2.5)):
         for b in (None, bias):
             for k in (1, 5, 8):
-                ref = _run_gate(logits, grid, k, alive=alive, rate=0.1, bias=b, score=score, scale=scale)
+                ref = run_gate(logits, grid, k, alive=alive, rate=0.1, bias=b, score=score, scale=scale)
                 for G, M in ((1, 1), (2, 2), (E_ // 4 if E_ // 4 <= 64 else 64, None)):
                     M = G if M is None else M
-                    got = _run_gate(logits, grid, k, alive=alive, rate=0.1, bias=b, score=score, scale=scale, G=G,
-                                    M=M)
+                    got = run_gate(logits, grid, k, alive=alive, rate=0.1, bias=b, score=score, scale=scale,
+                                   n_group=G, topk_group=M)
                     assert all(torch.equal(x, y) for x, y in zip(got, ref) if x is not None), (score, G, M, k)
 
 
@@ -465,49 +411,14 @@ def test_wrappers_refuse_bad_groupings_before_launching(step_counters):
     assert native.launches() == before
 
 
-def _rel(a, b):
-    a, b = a.detach().float(), b.detach().float()
-    return float((a - b).norm() / b.norm().clamp_min(1e-12))
-
-
-def _layer_against_the_oracle(cfg, exact):
-    grid = cfg.grid_size
-    ctx = E.EngineContext(cfg)
-    try:
-        layer = E.FusedDMoE(cfg, ctx).cuda().train()
-        oracle = E.FusedDMoE(cfg, device=torch.device("cuda")).cuda().train()
-        oracle.ref_emulate_bf16 = True
-        E_ = math.prod(grid)
-        bias0 = (torch.randint(-8, 9, (E_,)).float() / 16).cuda()
-        with torch.no_grad():
-            layer.expert_bias.copy_(bias0)
-            oracle.load_state_dict(layer.state_dict())
-            oracle.shard.p.copy_(layer.shard.p[:oracle.shard.p.numel()])
-        B = 512
-        x = torch.randn(B, cfg.hidden, device="cuda").to(torch.bfloat16)
-        gy = torch.randn(B, cfg.hidden, device="cuda").to(torch.bfloat16)
-        logits = layer.gate_logits(x, layer.proj).detach()
-        lg = logits.clone().requires_grad_(True)
-        y = E._FusedDMoEFunction.apply(x, lg, layer)
-        y.backward(gy)
-        torch.cuda.synchronize()
-        ctx.check_status()
-        lr_ = logits.clone().requires_grad_(True)
-        yr = oracle._forward_ref(x.float(), lr_, emulate_bf16=True)
-        yr.backward(gy.float())
-        ridx, rw = K.gate_topk_ref(logits, grid, cfg.k, alive=ctx.alive, bias=bias0, score=cfg.router_score,
-                                   scale=cfg.routed_scaling_factor, n_group=cfg.n_group, topk_group=cfg.topk_group)
-        got = layer.ws.idx[:B * cfg.k].view(B, cfg.k).long()
-        same = (got == ridx).all(1)
-        assert int((~same).sum()) <= (0 if exact else 2), int((~same).sum())
-        assert E.max_groups_per_token(got, cfg.k, E_, cfg.n_group) <= cfg.topk_group
-        assert float((layer.ws.w[:B * cfg.k].view(B, cfg.k) - rw)[same].abs().max()) < 2e-6 * cfg.routed_scaling_factor
-        assert torch.equal(ctx.cnt_all[0, :E_].long(), torch.bincount(got.flatten(), minlength=E_))
-        if bool(same.all()):
-            assert torch.equal(layer.expert_bias, oracle.expert_bias)
-        assert _rel(y, yr) < 2e-2 and _rel(lg.grad, lr_.grad) < 5e-2, (_rel(y, yr), _rel(lg.grad, lr_.grad))
-    finally:
-        ctx.close()
+def _check(r):
+    """no token beyond its topk_group groups, the weights of the tokens routed alike and, when every token is, the
+    oracle's bias update"""
+    cfg = r.layer.cfg
+    assert E.max_groups_per_token(r.idx, cfg.k, cfg.num_experts, cfg.n_group) <= cfg.topk_group
+    assert float((r.w - r.rw)[r.same].abs().max()) < 2e-6 * cfg.routed_scaling_factor
+    if bool(r.same.all()):
+        assert torch.equal(r.layer.expert_bias, r.oracle.expert_bias)
 
 
 @pytest.mark.gpu
@@ -520,7 +431,7 @@ def test_layer_against_the_cpu_oracle(path, expert, gate):
     grid = (16,) if gate == "emulator" else (4, 4)
     cfg = E.DMoEConfig(hidden=512, grid_size=grid, k=4, num_layers=1, tokens_per_rank=512, expert=expert,
                        expert_path=path, gate_mode=gate, expert_bias_update_rate=0.01, n_group=4, topk_group=2)
-    _layer_against_the_oracle(cfg, exact=True)
+    layer_against_the_oracle(cfg, max_mismatch=0, check=_check)
 
 
 @pytest.mark.gpu
@@ -531,7 +442,7 @@ def test_deepseek_v3_shaped_layer_against_the_cpu_oracle(path):
     cfg = E.DMoEConfig(hidden=512, grid_size=(8, 8), k=8, num_layers=1, tokens_per_rank=512, expert="swiglu",
                        inner_dim=256, shared_inner_dim=512, expert_path=path, expert_bias_update_rate=1e-3,
                        router_aux_loss_coef=1e-2, routed_scaling_factor=2.5, n_group=8, topk_group=4, **SIG)
-    _layer_against_the_oracle(cfg, exact=False)
+    layer_against_the_oracle(cfg, max_mismatch=2, check=_check)
 
 
 def _trainer_cfg(path, **kw):

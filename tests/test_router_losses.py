@@ -14,6 +14,8 @@ import lah_b200  # noqa
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import collapse, cpu_cfg, load, rel
+from routing_support import one_thread  # noqa: F401 (fixture)
 
 GRIDS = [(64,), (8, 8), (4, 4, 4), (2, 2, 2, 2)]
 COEF = dict(router_aux_loss_coef=0.01, router_z_loss_coef=0.001)
@@ -149,28 +151,12 @@ def test_closed_form_gradient_equals_autograd(grid, dead, one_thread):
     torch.testing.assert_close(closed, auto, rtol=1e-10, atol=1e-13)
 
 
-@pytest.fixture
-def one_thread():
-    """the CPU trainer tests run many tiny ops: one intra-op thread is faster, and does not compete with the threads
-    other tests of the session may have left behind"""
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
-
-
-def _cpu_cfg(**kw):
-    base = dict(hidden=64, grid_size=(4, 4), k=4, num_layers=1, in_features=16, tokens_per_rank=64, seed=5)
-    base.update(kw)
-    return E.DMoEConfig(**base)
-
-
 @pytest.mark.parametrize("expert", ["ffn", "swiglu"])
 def test_cpu_layer_adds_the_router_gradient(expert):
     torch.manual_seed(0)
-    plain = E.FusedDMoE(_cpu_cfg(expert=expert)).train()
+    plain = E.FusedDMoE(cpu_cfg(expert=expert)).train()
     torch.manual_seed(0)
-    cfg = _cpu_cfg(expert=expert, router_aux_loss_coef=0.05, router_z_loss_coef=0.01)
+    cfg = cpu_cfg(expert=expert, router_aux_loss_coef=0.05, router_z_loss_coef=0.01)
     routed = E.FusedDMoE(cfg).train()
     x = torch.randn(32, 64)
     gy = torch.randn(32, 64)
@@ -191,22 +177,22 @@ def F_linear(x, proj):
 
 
 def test_cpu_router_loss_is_a_buffer_that_is_not_saved():
-    layer = E.FusedDMoE(_cpu_cfg(**COEF))
+    layer = E.FusedDMoE(cpu_cfg(**COEF))
     assert dict(layer.named_buffers())["router_loss"] is layer.router_loss
     assert "router_loss" not in layer.state_dict()
     assert layer.double().router_loss.dtype == torch.float64   # follows the layer's .to()
-    assert "router_loss" not in dict(E.FusedDMoE(_cpu_cfg()).named_buffers())
+    assert "router_loss" not in dict(E.FusedDMoE(cpu_cfg()).named_buffers())
 
 
 def test_cpu_layer_eval_mode_computes_nothing():
-    layer = E.FusedDMoE(_cpu_cfg(**COEF)).eval()
+    layer = E.FusedDMoE(cpu_cfg(**COEF)).eval()
     layer(torch.randn(8, 64))
     assert torch.equal(layer.router_loss, torch.zeros(2))
 
 
 def test_zero_coefficients_change_nothing():
     grads = []
-    for cfg in (_cpu_cfg(), _cpu_cfg(router_aux_loss_coef=0.0, router_z_loss_coef=0.0)):
+    for cfg in (cpu_cfg(), cpu_cfg(router_aux_loss_coef=0.0, router_z_loss_coef=0.0)):
         torch.manual_seed(0)
         layer = E.FusedDMoE(cfg).train()
         torch.manual_seed(1)
@@ -232,28 +218,16 @@ def test_microbatch_router_gradient_is_the_mean_of_the_micro_batches(one_thread)
     torch.manual_seed(2)
     x, y = torch.randn(64, 16), torch.randint(0, 10, (64,))
     kw = dict(num_layers=2, lr=0.0)
-    assert all(b.router_grad_scale == 0.5 for b in DMoETrainer(_cpu_cfg(trainer_microbatches=2, **COEF, **kw)).model.blocks)
+    assert all(b.router_grad_scale == 0.5 for b in DMoETrainer(cpu_cfg(trainer_microbatches=2, **COEF, **kw)).model.blocks)
 
     def router_part(m, xs, ys):   # the part of the gradient the router losses add (same routing: same parameters)
-        return (_first_trainer_grad(_cpu_cfg(trainer_microbatches=m, **COEF, **kw), xs, ys)
-                - _first_trainer_grad(_cpu_cfg(trainer_microbatches=m, **kw), xs, ys))
+        return (_first_trainer_grad(cpu_cfg(trainer_microbatches=m, **COEF, **kw), xs, ys)
+                - _first_trainer_grad(cpu_cfg(trainer_microbatches=m, **kw), xs, ys))
 
     two = router_part(2, x, y)
     halves = [router_part(1, x[:32], y[:32]), router_part(1, x[32:], y[32:])]
     assert float(two.abs().max()) > 1e-5
     torch.testing.assert_close(two, 0.5 * (halves[0] + halves[1]), rtol=1e-4, atol=1e-7)
-
-
-def _load(trainer, x):
-    """max / mean rows per expert of every layer on batch x (eval-mode routing)"""
-    out, h = [], trainer.model.stem(x)
-    with torch.no_grad():
-        for block in trainer.model.blocks:
-            idx, _ = K.gate_topk_ref(block.gate_logits(h, block.proj), block.grid_size, block.cfg.k)
-            rows = torch.bincount(idx[idx >= 0].flatten(), minlength=block.cfg.num_experts).float()
-            out.append(float(rows.max() / rows.mean()))
-            h = block(h)
-    return out
 
 
 def test_load_balancing_loss_spreads_a_collapsed_router(one_thread):
@@ -265,13 +239,12 @@ def test_load_balancing_loss_spreads_a_collapsed_router(one_thread):
     x = protos[y] + 0.5 * torch.randn(128, 16, generator=gen)
     results = {}
     for alpha in (0.0, 0.1):
-        cfg = _cpu_cfg(grid_size=(8,), k=2, num_layers=1, tokens_per_rank=128, lr=3e-3, router_aux_loss_coef=alpha)
+        cfg = cpu_cfg(grid_size=(8,), k=2, num_layers=1, tokens_per_rank=128, lr=3e-3, router_aux_loss_coef=alpha)
         t = DMoETrainer(cfg)
-        with torch.no_grad():
-            t.model.blocks[0].proj.bias[:2] += 2.0
-        before = _load(t, x)
+        collapse(t.model.blocks[0], "product_key")
+        before = load(t, x)
         losses = [t.train_step(x, y) for _ in range(120)]
-        results[alpha] = (before, _load(t, x), losses)
+        results[alpha] = (before, load(t, x), losses)
     (b0, a0, l0), (b1, a1, l1) = results[0.0], results[0.1]
     assert b0 == b1 and b0[0] > 3.0            # same start: two of eight experts take (nearly) every row
     assert a1[0] < a0[0] and a1[0] < 2.0, (a0, a1)
@@ -370,11 +343,6 @@ def test_wrappers_refuse_bad_arguments_before_launching():
     assert native.launches() == before
 
 
-def _rel(a, b):
-    a, b = a.detach().float(), b.detach().float()
-    return float((a - b).norm() / b.norm().clamp_min(1e-12))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("expert", ["ffn", "swiglu"])
 @pytest.mark.parametrize("path", ["small", "big"])
@@ -408,8 +376,8 @@ def test_layer_against_the_bf16_oracle(path, expert):
         yr = oracle._forward_ref(x.float(), lr_, emulate_bf16=True)
         yr.backward(gy.float())
         oracle_proj = torch.autograd.grad(F_linear(x, oracle.proj), oracle.proj.weight, lr_.grad)[0]
-        assert _rel(layer.router_loss, oracle.router_loss) < 1e-4, (layer.router_loss, oracle.router_loss)
-        assert _rel(y, yr) < 2e-2 and _rel(lg.grad, lr_.grad) < 5e-2 and _rel(proj_grad, oracle_proj) < 5e-2
+        assert rel(layer.router_loss, oracle.router_loss) < 1e-4, (layer.router_loss, oracle.router_loss)
+        assert rel(y, yr) < 2e-2 and rel(lg.grad, lr_.grad) < 5e-2 and rel(proj_grad, oracle_proj) < 5e-2
         # the router part alone, against autograd of the oracle's losses on the same routing
         counts = ctx.cnt_all[:1].view(-1)
         aux, zl = K.router_loss_ref(lg.detach().double().requires_grad_(True), cfg.grid_size, counts)

@@ -6,9 +6,7 @@ an oracle: the benchmark's default emulator gate (bf16 logits, so ties are commo
 
 The CPU tests check the host references themselves.
 """
-import ctypes
 import zlib
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -17,26 +15,12 @@ import torch.nn.functional as F
 
 import lah_b200  # noqa: F401
 from lah_b200.ops import kernels as K
+from routing_support import F64, rel, slots
+from routing_support import rt, world1  # noqa: F401 (fixtures)
 
 GAMMA = 0x9E3779B97F4A7C15
 LAYOUT_MAX_E = 4096
 BF16 = torch.bfloat16
-
-
-def rank_in_expert(idx):
-    """pos oracle: for every (token, choice) pair in token-major order, the number of earlier pairs routed to the same
-    expert; 0 for pairs without an expert"""
-    flat = idx.flatten().cpu().numpy().astype(np.int64)
-    order = np.argsort(flat, kind="stable")
-    srt = flat[order]
-    pos = np.empty_like(flat)
-    pos[order] = np.arange(len(flat)) - np.searchsorted(srt, srt, side="left")
-    pos[flat < 0] = 0
-    return torch.from_numpy(pos)
-
-
-def rel(got, ref):
-    return ((got.double() - ref.double()).norm() / (ref.double().norm() + 1e-30)).item()
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU
@@ -80,46 +64,6 @@ def test_gate_topk_ref_breaks_ties_toward_the_smaller_expert_id():
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU
-@pytest.fixture(scope="module")
-def world1():
-    """a world-1 symmetric heap made directly (no EngineContext), with its own step counters, status / poison word, flag
-    words, count-exchange table and one receive region that the tests view as [rows, H] bf16 buffers"""
-    from lah_b200.ops import native
-    from lah_b200.parallel.symmetric import SymmetricHeap
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    lib.lah_get_poison_word.restype = ctypes.c_void_p
-    prev_ctr, prev_poison = lib.lah_get_epoch_base(), lib.lah_get_poison_word()
-    heap = SymmetricHeap(80 << 20)
-    flags, flags_off = heap.alloc((K.NUM_SLOTS, K.MAX_WORLD), torch.int32)
-    cnt_all, cnt_all_off = heap.alloc((K.MAX_WORLD, LAYOUT_MAX_E), torch.int32)
-    region, region_off = heap.alloc((64 << 20,), torch.uint8)
-    i32 = dict(dtype=torch.int32, device="cuda")
-    w = SimpleNamespace(heap=heap, native=native, flags=flags, flags_off=flags_off, cnt_all=cnt_all, cnt_all_off=cnt_all_off,
-                        region=region, region_off=region_off, step_ctr=torch.zeros(4, **i32), status=torch.zeros(4, **i32),
-                        done_counter=torch.zeros(1, **i32))
-    yield w
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev_ctr))
-    lib.lah_set_poison_word(ctypes.c_void_p(prev_poison))
-    heap.close()
-
-
-@pytest.fixture
-def rt(world1):
-    """world1 with its peer table and process-global counters (re)installed: an EngineContext made by another test
-    installs its own and clears them on close"""
-    w = world1
-    K.set_peers(w.heap.peer_bases, 0)
-    K.set_multicast(0)
-    K.set_step_counters(w.step_ctr)
-    K.set_poison_word(w.status)
-    w.status.zero_()
-    w.step_ctr.zero_()
-    w.done_counter.zero_()
-    return w
-
-
 def rows_view(w, rows, H):
     """[rows, H] bf16 at the start of the receive region, and its byte offset in the heap"""
     return w.region[: rows * H * 2].view(BF16).view(rows, H), w.region_off
@@ -178,7 +122,7 @@ def check_gate_against_ref(logits, grid, k, alive, fail_mask, out, counts0):
     valid = ridx >= 0
     exp_counts = counts0.long() + torch.bincount(ridx[valid], minlength=E)
     assert torch.equal(counts, exp_counts)
-    assert torch.equal(pos.cpu(), rank_in_expert(ridx).view_as(pos))
+    assert torch.equal(pos.cpu(), slots(ridx).cpu())
     scores = K.product_key_scores(logits, grid).double()
     sel = torch.gather(scores, 1, ridx.clamp(min=0)).masked_fill(~valid, float("-inf"))
     w_ref = torch.where(valid, torch.softmax(sel, dim=-1), torch.zeros_like(sel)).nan_to_num(0.0)
@@ -358,7 +302,7 @@ def test_scatter_rows(rt, H, align, mode, case):
     gen = torch.Generator().manual_seed(H + align + len(mode) + len(case))
     B, k, E = 301, 4, 16
     idx = routed_pairs(B, k, E, gen)
-    pos = rank_in_expert(idx)
+    pos = slots(idx).flatten()
     counts = torch.bincount(idx[idx >= 0], minlength=E).to(torch.int32)
     total = int(((counts.long() + align - 1) // align * align).sum())
     max_rows = total - 2 * align if case == "overflow" else total + 2 * align
@@ -496,7 +440,7 @@ def test_gate_bwd(rt, record_property, grid, H, k):
     if k == 1:
         assert bool((dl == 0).all())
     else:
-        err = rel(dl.cpu(), lg.grad)
+        err = rel(dl.cpu(), lg.grad, *F64)
         record_property("rel_l2_err", err)
         assert err < 1e-4, err
 
@@ -543,7 +487,7 @@ def test_bench_default_layer_matches_oracle_on_tied_bf16_logits(record_property)
         torch.cuda.synchronize()
         ctx.check_status()
         assert torch.equal(idx, ridx), int((idx != ridx).any(1).sum())
-        errs = dict(y=rel(y, yr), dx=rel(xf.grad, xr.grad), dlogits=rel(lf.grad, lr_.grad))
+        errs = dict(y=rel(y, yr, *F64), dx=rel(xf.grad, xr.grad, *F64), dlogits=rel(lf.grad, lr_.grad, *F64))
         record_property("errors", errs)
         assert errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dlogits"] < 5e-2, errs
     finally:
@@ -597,7 +541,8 @@ def test_failure_injected_layer_matches_oracle(record_property, rate):
         ctx.check_status()
         assert torch.equal(idx, ridx), int((idx != ridx).any(1).sum())
         assert int((ridx < 0).sum()) > 0 or rate < 0.5
-        errs = dict(y=rel(y, yr), dx=rel(xf.grad, xr.grad), dproj=rel(layer.proj.weight.grad, dproj_ref))
+        errs = dict(y=rel(y, yr, *F64), dx=rel(xf.grad, xr.grad, *F64),
+                    dproj=rel(layer.proj.weight.grad, dproj_ref, *F64))
         record_property("errors", errs)
         assert errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2, errs
     finally:

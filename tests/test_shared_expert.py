@@ -18,6 +18,8 @@ from lah_b200.models.layers import gated_inner_dim
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import rel
+from routing_support import one_thread, rt, world1  # noqa: F401 (fixtures)
 
 BF16 = torch.bfloat16
 #: the bench operating point: 64 experts, top-4, 256 samples per step, 4 layers, emulator gate
@@ -25,14 +27,6 @@ BENCH = dict(grid_size=(64,), k=4, num_layers=4, tokens_per_rank=256, gate_mode=
 #: kernels the shared expert adds per layer and micro-batch: forward 2 casts + RMSNorm + GEMM + SwiGLU + GEMM; backward
 #: GEMM + SwiGLU + GEMM + RMSNorm (2 launches) + 2 wgrads.  The combines take the addend in their existing launch
 SHARED_LAUNCHES = 6 + 7
-
-
-@pytest.fixture
-def one_thread():
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
 
 
 def _cfg(**kw):
@@ -205,28 +199,6 @@ def test_checkpoint_mismatches_raise(one_thread):
 
 
 # ======================================================================================================== GPU
-@pytest.fixture(scope="module")
-def heap():
-    """a world-1 symmetric heap made directly, whose rank is its only peer, and a region of it for the rows"""
-    from lah_b200.parallel.symmetric import SymmetricHeap
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    h = SymmetricHeap(128 << 20)
-    region, off = h.alloc((96 << 20,), torch.uint8)
-    yield h, region, off
-    torch.cuda.synchronize()
-    h.close()
-
-
-@pytest.fixture
-def world1(heap):
-    """the heap's peer table (re)installed: an EngineContext made by another test installs its own"""
-    h, region, off = heap
-    K.set_peers(h.peer_bases, 0)
-    K.set_multicast(0)
-    return region, off
-
-
 def _combine_case(B, k, H, R, gen, dyadic):
     idx = torch.randint(0, 16, (B, k), generator=gen)
     idx[torch.rand(B, k, generator=gen) < 0.1] = -1
@@ -246,8 +218,8 @@ def _combine_case(B, k, H, R, gen, dyadic):
 @pytest.mark.gpu
 @pytest.mark.parametrize("B", [256, 4000])
 @pytest.mark.parametrize("H", [256, 512, 1024])
-def test_combine_rows_with_an_addend_against_the_exact_oracle(world1, H, B):
-    region, off = world1
+def test_combine_rows_with_an_addend_against_the_exact_oracle(rt, H, B):
+    region, off = rt.region, rt.region_off
     k = 4
     R = B * k + 64
     gen = torch.Generator().manual_seed(H + B)
@@ -283,9 +255,9 @@ def test_combine_rows_with_an_addend_against_the_exact_oracle(world1, H, B):
 
 
 @pytest.mark.gpu
-def test_combine_rows_refuses_a_bad_addend(world1):
+def test_combine_rows_refuses_a_bad_addend(rt):
     from lah_b200.ops import native
-    _, off = world1
+    off = rt.region_off
     i = torch.zeros(8, dtype=torch.int32, device="cuda")
     out = torch.zeros(2, 256, dtype=BF16, device="cuda")
     before = native.launches()
@@ -295,11 +267,6 @@ def test_combine_rows_refuses_a_bad_addend(world1):
         with pytest.raises(ValueError):
             K.combine_rows(off, i, i, None, out, 4, 16, addend=bad)
     assert native.launches() == before
-
-
-def _rel(a, b):
-    a, b = a.detach().float(), b.detach().float()
-    return float((a - b).norm() / b.norm().clamp_min(1e-12))
 
 
 @pytest.mark.gpu
@@ -349,9 +316,9 @@ def test_layer_against_the_bf16_oracle(path, B, failure_rate):
         if failure_rate:   # the failures changed the routing
             assert not torch.equal(ridx, K.gate_topk_ref(oracle.gate_logits(xr, oracle.proj).detach(), cfg.grid_size,
                                                          cfg.k)[0])
-        errs = dict(y=_rel(y, yr), dx=_rel(x.grad, xr.grad), dproj=_rel(layer.proj.weight.grad, oracle.proj.weight.grad))
-        werr = {n: _rel(a.grad, b.grad) for n, a, b in zip(E.GATED_LAYOUT.names, shared,
-                                                            oracle.shared_expert_parameters())}
+        errs = dict(y=rel(y, yr), dx=rel(x.grad, xr.grad), dproj=rel(layer.proj.weight.grad, oracle.proj.weight.grad))
+        werr = {n: rel(a.grad, b.grad) for n, a, b in zip(E.GATED_LAYOUT.names, shared,
+                                                          oracle.shared_expert_parameters())}
         assert errs["y"] < 2e-2 and errs["dx"] < 3e-2 and errs["dproj"] < 5e-2, errs
         assert max(werr.values()) < 8e-2, werr
     finally:

@@ -6,9 +6,7 @@ CPU: the configuration and its refusals, the oracles K.gate_topk_ref(score=...) 
 their written formulas in float64, a CPU trainer that balances a collapsed gate with sigmoid keys, and checkpoints.
 GPU: the gate, gate_bwd and router-loss kernels against the oracles, one layer on both paths, both expert kinds and both
 gates against the CPU oracle (and one DeepSeek-V3-shaped layer), and the trainer under its CUDA graph."""
-import ctypes
 import math
-from types import SimpleNamespace
 
 import pytest
 import torch
@@ -17,35 +15,22 @@ import lah_b200  # noqa
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import collapse, cpu_cfg, layer_against_the_oracle, load, run_gate, slots
+from routing_support import one_thread, rt, step_counters, world1  # noqa: F401 (fixtures)
 
 SIG = dict(router_score="sigmoid")
-
-
-@pytest.fixture
-def one_thread():
-    """the CPU trainer tests run many tiny ops: one intra-op thread is faster"""
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
-
-
-def _cpu_cfg(**kw):
-    base = dict(hidden=64, grid_size=(4, 4), k=4, num_layers=1, in_features=16, tokens_per_rank=64, seed=5)
-    base.update(kw)
-    return E.DMoEConfig(**base)
 
 
 # ======================================================================================================== CPU: config
 def test_defaults_and_state_dict_keys():
     cfg = E.DMoEConfig()
     assert cfg.router_score == "softmax" and cfg.routed_scaling_factor == 1.0
-    plain = E.FusedDMoE(_cpu_cfg())
+    plain = E.FusedDMoE(cpu_cfg())
     assert plain.router_score == "softmax" and plain.routed_scale == 1.0
-    sig = E.FusedDMoE(_cpu_cfg(routed_scaling_factor=2.5, **SIG))
+    sig = E.FusedDMoE(cpu_cfg(routed_scaling_factor=2.5, **SIG))
     assert sig.router_score == "sigmoid" and sig.routed_scale == 2.5
     # the weight function adds no state: every layer keeps the keys of a default layer
-    assert list(plain.state_dict()) == list(E.FusedDMoE(_cpu_cfg(router_score="softmax")).state_dict())
+    assert list(plain.state_dict()) == list(E.FusedDMoE(cpu_cfg(router_score="softmax")).state_dict())
     assert list(plain.state_dict()) == list(sig.state_dict())
 
 
@@ -71,8 +56,8 @@ def test_every_gate_and_expert_kind_accepts_the_sigmoid_router(gate, expert):
     extra = dict(router_aux_loss_coef=0.01) if gate == "product_key" else {}
     if expert == "swiglu":
         extra["shared_inner_dim"] = 128
-    cfg = _cpu_cfg(grid_size=(16,), gate_mode=gate, expert=expert, expert_bias_update_rate=1e-3, failure_rate=0.1,
-                   trainer_microbatches=2, routed_scaling_factor=2.5, **SIG, **extra)
+    cfg = cpu_cfg(grid_size=(16,), gate_mode=gate, expert=expert, expert_bias_update_rate=1e-3, failure_rate=0.1,
+                  trainer_microbatches=2, routed_scaling_factor=2.5, **SIG, **extra)
     for path in ("small", "big"):
         E.DMoEConfig(**{**cfg.__dict__, "expert_path": path})
     E.DMoEConfig(**{**cfg.__dict__, "update_every_steps": 2})
@@ -230,7 +215,7 @@ def test_sigmoid_router_loss_of_underflowed_tokens_is_zero():
 # ======================================================================================================== CPU: trainer
 def test_cpu_layer_differentiates_through_the_sigmoid_weights():
     torch.manual_seed(0)
-    layer = E.FusedDMoE(_cpu_cfg(routed_scaling_factor=2.5, router_aux_loss_coef=0.01, **SIG)).train()
+    layer = E.FusedDMoE(cpu_cfg(routed_scaling_factor=2.5, router_aux_loss_coef=0.01, **SIG)).train()
     x = torch.randn(32, 64)
     logits = layer.gate_logits(x, layer.proj).detach().requires_grad_(True)
     out = layer._forward_ref(x, logits)
@@ -239,28 +224,6 @@ def test_cpu_layer_differentiates_through_the_sigmoid_weights():
     assert torch.isfinite(logits.grad).all() and float(logits.grad.abs().max()) > 0
     aux, zl = layer.router_loss.tolist()
     assert aux > 0 and zl == 0.0
-
-
-def _load(trainer, x):
-    """max / mean rows per expert of every layer on batch x (eval-mode routing, with the layers' biases)"""
-    out, h = [], trainer.model.stem(x)
-    with torch.no_grad():
-        for block in trainer.model.blocks:
-            idx, _ = K.gate_topk_ref(block.gate_logits(h, block.proj), block.grid_size, block.cfg.k,
-                                     bias=block.expert_bias, score=block.router_score)
-            rows = torch.bincount(idx[idx >= 0].flatten(), minlength=block.cfg.num_experts).float()
-            out.append(float(rows.max() / rows.mean()))
-            h = block(h)
-    return out
-
-
-def _collapse(block, gate):
-    with torch.no_grad():
-        if gate == "product_key":   # the gate's bias favours experts 0 and 1
-            block.proj.bias[:2] += 2.0
-        else:                       # frozen keys whose first two columns win most rows
-            block.gating_pre_normalize.bias.fill_(0.5)
-            block.expert_keys[:, :2] += 0.5
 
 
 @pytest.mark.parametrize("gate", ["product_key", "emulator"])
@@ -273,13 +236,13 @@ def test_sigmoid_keys_with_expert_biases_spread_a_collapsed_router(one_thread, g
     x = protos[y] + 0.5 * torch.randn(128, 16, generator=gen)
     results = {}
     for rate in (0.0, 0.01):
-        cfg = _cpu_cfg(grid_size=(8,), k=2, num_layers=1, tokens_per_rank=128, lr=3e-3, gate_mode=gate,
-                       expert_bias_update_rate=rate, routed_scaling_factor=2.0, **SIG)
+        cfg = cpu_cfg(grid_size=(8,), k=2, num_layers=1, tokens_per_rank=128, lr=3e-3, gate_mode=gate,
+                      expert_bias_update_rate=rate, routed_scaling_factor=2.0, **SIG)
         t = DMoETrainer(cfg)
-        _collapse(t.model.blocks[0], gate)
-        before = _load(t, x)
+        collapse(t.model.blocks[0], gate)
+        before = load(t, x)
         losses = [t.train_step(x, y) for _ in range(120)]
-        results[rate] = (before, _load(t, x), losses)
+        results[rate] = (before, load(t, x), losses)
     (b0, a0, l0), (b1, a1, l1) = results[0.0], results[0.01]
     assert b0 == b1 and b0[0] > 3.0
     assert a1[0] < 0.6 * a0[0] and a1[0] < 1.5, (a0, a1)
@@ -287,8 +250,8 @@ def test_sigmoid_keys_with_expert_biases_spread_a_collapsed_router(one_thread, g
 
 
 def test_sigmoid_checkpoint_round_trip(one_thread):
-    cfg = _cpu_cfg(num_layers=2, expert_bias_update_rate=1e-3, routed_scaling_factor=2.5, router_aux_loss_coef=0.01,
-                   **SIG)
+    cfg = cpu_cfg(num_layers=2, expert_bias_update_rate=1e-3, routed_scaling_factor=2.5, router_aux_loss_coef=0.01,
+                  **SIG)
     gen = torch.Generator().manual_seed(4)
     xs = [torch.randn(64, 16, generator=gen) for _ in range(6)]
     ys = [torch.randint(0, 10, (64,), generator=gen) for _ in range(6)]
@@ -309,7 +272,7 @@ def test_sigmoid_checkpoint_round_trip(one_thread):
 
 def test_checkpoints_of_the_other_router_score_are_refused(one_thread):
     x, y = torch.randn(64, 16), torch.randint(0, 10, (64,))
-    soft, sig = DMoETrainer(_cpu_cfg()), DMoETrainer(_cpu_cfg(**SIG))
+    soft, sig = DMoETrainer(cpu_cfg()), DMoETrainer(cpu_cfg(**SIG))
     soft.train_step(x, y)
     sig.train_step(x, y)
     plain = soft.state_dict()
@@ -319,67 +282,11 @@ def test_checkpoints_of_the_other_router_score_are_refused(one_thread):
     with pytest.raises(ValueError, match="router_score"):
         soft.load_state_dict(sig.state_dict())
     # the same score loads, with or without the key
-    DMoETrainer(_cpu_cfg()).load_state_dict(plain)
-    DMoETrainer(_cpu_cfg(**SIG)).load_state_dict(sig.state_dict())
+    DMoETrainer(cpu_cfg()).load_state_dict(plain)
+    DMoETrainer(cpu_cfg(**SIG)).load_state_dict(sig.state_dict())
 
 
 # ======================================================================================================== GPU
-@pytest.fixture(scope="module")
-def step_counters():
-    """the gate adds the device token base (step counters [2:4]) to its failure-injection stream: install zeroed
-    counters for this module's direct kernel calls, and put back whatever was installed before"""
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    prev = lib.lah_get_epoch_base()
-    ctr = torch.zeros(4, dtype=torch.int32, device="cuda")
-    yield ctr
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev))
-
-
-def _run_gate(logits, grid, k, *, alive, rate, bias, score="softmax", scale=1.0):
-    B = logits.shape[0]
-    idx = torch.full((B * k,), 12345, dtype=torch.int32, device="cuda")
-    pos, w = torch.full_like(idx, 12345), torch.full((B * k,), 7.0, device="cuda")
-    sig = torch.full((B * k,), 7.0, device="cuda") if score == "sigmoid" else None
-    counts = torch.zeros(math.prod(grid), dtype=torch.int32, device="cuda")
-    K.gate_topk(logits, grid, k, alive=alive, failure_rate=rate, seed=99, token_offset=0, idx=idx, w=w, pos=pos,
-                counts=counts, bias=bias, score=score, scale=scale, sig=sig)
-    torch.cuda.synchronize()
-    return idx.view(B, k), w.view(B, k), pos.view(B, k), counts, None if sig is None else sig.view(B, k)
-
-
-def _u64(c):
-    return c - (1 << 64) if c >= 1 << 63 else c
-
-
-def _shr(x, n):
-    return (x >> n) & ((1 << (64 - n)) - 1)
-
-
-def _fail_mask(B, E_, rate, seed=99):
-    """K.gate_fail_mask_ref (token base 0) on the device: int64 tensors wrap modulo 2**64 like the kernel's uint64"""
-    tok = torch.arange(B, dtype=torch.int64, device="cuda") * 0x100000001B3
-    x = _u64(seed) ^ (tok[:, None] + torch.arange(E_, dtype=torch.int64, device="cuda")[None, :])
-    x = x + _u64(0x9E3779B97F4A7C15)
-    x = (x ^ _shr(x, 30)) * _u64(0xBF58476D1CE4E5B9)
-    x = (x ^ _shr(x, 27)) * _u64(0x94D049BB133111EB)
-    x = x ^ _shr(x, 31)
-    return _shr(x, 40).double() / 2.0 ** 24 < float(torch.tensor(rate, dtype=torch.float32))
-
-
-def _slots(idx):
-    flat = idx.reshape(-1).long()
-    order = torch.argsort(flat, stable=True)
-    srt = flat[order]
-    first = torch.searchsorted(srt, srt, side="left")
-    pos = torch.empty_like(flat)
-    pos[order] = torch.arange(flat.numel(), device=flat.device) - first
-    return torch.where(flat >= 0, pos, torch.zeros_like(pos)).view_as(idx)
-
-
 def _clear_tokens(scores, bias, dead, k):
     """tokens whose oracle keys sigma(s) + b among the k + 1 best are pairwise separated by more than 1e-6, or exactly
     tied with equal score and bias (then both sides order them by expert id)"""
@@ -397,8 +304,6 @@ def _clear_tokens(scores, bias, dead, k):
 @pytest.mark.parametrize("B", [1, 7, 256, 65536])
 @pytest.mark.parametrize("grid", [(64,), (8, 8), (64, 64), (256,), (4096,), (4, 4, 4, 4)])
 def test_sigmoid_gate_topk_against_the_oracle(step_counters, grid, B):
-    K.set_step_counters(step_counters)
-    step_counters.zero_()
     E_ = math.prod(grid)
     gen = torch.Generator(device="cuda").manual_seed(B * 5 + E_)
     if len(grid) <= 2:   # continuous scores: s = l0 (+ l1) is the same float in any order
@@ -409,30 +314,32 @@ def test_sigmoid_gate_topk_against_the_oracle(step_counters, grid, B):
     bias = torch.randint(-8, 9, (E_,), generator=gen, device="cuda").float() / 16
     alive = (torch.rand(E_, generator=gen, device="cuda") > 0.2).to(torch.uint8)
     rate = 0.1
-    fail = _fail_mask(B, E_, rate)
+    fail = K.gate_fail_mask_ref(B, E_, rate, 99, 0).cuda()
     dead = ~alive.bool().view(1, -1) | fail
     unclear = total = 0
     for k in range(1, 9):
         c = 2.5 if k % 2 else 1.0
         # unbiased: the softmax router's selection, exactly
-        idx, w, pos, counts, sig = _run_gate(logits, grid, k, alive=alive, rate=rate, bias=None, score="sigmoid", scale=c)
+        idx, w, pos, counts, sig, _ = run_gate(logits, grid, k, alive=alive, rate=rate, bias=None, score="sigmoid",
+                                               scale=c)
         ridx, rw = K.gate_topk_ref(logits, grid, k, alive=alive, fail_mask=fail, score="sigmoid", scale=c)
         assert torch.equal(idx.long(), ridx), (k, int((idx.long() != ridx).any(1).sum()))
-        assert torch.equal(pos.long(), _slots(ridx))
+        assert torch.equal(pos.long(), slots(ridx))
         assert torch.equal(counts.long(), torch.bincount(ridx[ridx >= 0], minlength=E_))
         assert float((w.double() - rw.double()).abs().max()) < 2e-6 * c, k
         rsig = torch.sigmoid(torch.gather(K.product_key_scores(logits, grid), 1, ridx.clamp(min=0))) * (ridx >= 0)
         assert float((sig - rsig).abs().max()) < 1e-6
-        assert torch.equal(idx, _run_gate(logits, grid, k, alive=alive, rate=rate, bias=None)[0])
+        assert torch.equal(idx, run_gate(logits, grid, k, alive=alive, rate=rate, bias=None)[0])
         # biased: sigma(s) + b; ids equal wherever the oracle's keys are not near-tied
-        idx, w, pos, counts, sig = _run_gate(dyadic, grid, k, alive=alive, rate=rate, bias=bias, score="sigmoid", scale=c)
+        idx, w, pos, counts, sig, _ = run_gate(dyadic, grid, k, alive=alive, rate=rate, bias=bias, score="sigmoid",
+                                               scale=c)
         ridx, rw = K.gate_topk_ref(dyadic, grid, k, alive=alive, fail_mask=fail, bias=bias, score="sigmoid", scale=c)
         clear = _clear_tokens(K.product_key_scores(dyadic, grid), bias, dead, k)
         unclear += int((~clear).sum())
         total += B
         assert torch.equal(idx.long()[clear], ridx[clear]), (k, int((idx.long() != ridx)[clear].any(1).sum()))
         assert torch.equal(counts.long(), torch.bincount(idx.long()[idx >= 0], minlength=E_))
-        assert torch.equal(pos.long(), _slots(idx.long()))
+        assert torch.equal(pos.long(), slots(idx.long()))
         same = (idx.long() == ridx).all(1, keepdim=True)
         assert float(torch.where(same, w.double() - rw.double(), 0.0).abs().max()) < 2e-6 * c, k
     assert unclear <= 1e-3 * total, (unclear, total)
@@ -462,33 +369,11 @@ def test_sigmoid_wrappers_refuse_bad_arguments_before_launching():
     assert native.launches() == before
 
 
-@pytest.fixture(scope="module")
-def world1():
-    """a world-1 symmetric heap made directly (no EngineContext) with one receive region, for gate_bwd"""
-    from lah_b200.parallel.symmetric import SymmetricHeap
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    prev_ctr = lib.lah_get_epoch_base()
-    heap = SymmetricHeap(64 << 20)
-    region, region_off = heap.alloc((48 << 20,), torch.uint8)
-    w = SimpleNamespace(heap=heap, region=region, region_off=region_off,
-                        step_ctr=torch.zeros(4, dtype=torch.int32, device="cuda"))
-    yield w
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev_ctr))
-    heap.close()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("c", [1.0, 2.5])
 @pytest.mark.parametrize("k", [1, 4, 8])
 @pytest.mark.parametrize("grid,H", [((64,), 256), ((4, 4), 512), ((2, 32), 1024), ((3, 5, 7), 512), ((256,), 1024)])
-def test_sigmoid_gate_bwd_against_the_float64_formula(world1, grid, H, k, c):
-    K.set_peers(world1.heap.peer_bases, 0)
-    K.set_multicast(0)
-    K.set_step_counters(world1.step_ctr)
+def test_sigmoid_gate_bwd_against_the_float64_formula(rt, grid, H, k, c):
     gen = torch.Generator().manual_seed(k * H + len(grid))
     B = 257
     logits = torch.randn(B, sum(grid), generator=gen, dtype=torch.float64) * 2
@@ -503,7 +388,7 @@ def test_sigmoid_gate_bwd_against_the_float64_formula(world1, grid, H, k, c):
     pair_row = torch.randperm(R, generator=gen)[: B * k].view(B, k)
     pair_row[torch.rand(B, k, generator=gen) < 0.05] = -1   # pairs that scatter_rows dropped
     pair_row = torch.where(valid, pair_row, torch.full_like(pair_row, -1))
-    yo = world1.region[: R * H * 2].view(torch.bfloat16).view(R, H)
+    yo = rt.region[: R * H * 2].view(torch.bfloat16).view(R, H)
     yo.copy_(torch.randn(R, H, generator=gen).to(torch.bfloat16))
     g = torch.randn(B, H, generator=gen).to(torch.bfloat16)
     y = yo.cpu().double()[pair_row.clamp(min=0)] * (pair_row >= 0).double().unsqueeze(-1)
@@ -511,7 +396,7 @@ def test_sigmoid_gate_bwd_against_the_float64_formula(world1, grid, H, k, c):
     ds = _gate_bwd_formula(sig.double(), w.double(), dw, valid, c)
     ref = _scatter_to_logits(ds, idx, grid)
     dl = torch.full((B, sum(grid)), 5.0, device="cuda")
-    K.gate_bwd(world1.region_off, g.cuda(), idx.flatten().to(torch.int32).cuda(),
+    K.gate_bwd(rt.region_off, g.cuda(), idx.flatten().to(torch.int32).cuda(),
                pair_row.flatten().to(torch.int32).cuda(), w.flatten().cuda(), dl, k, math.prod(grid), grid,
                score="sigmoid", scale=c, sig=sig.flatten().cuda())
     torch.cuda.synchronize()
@@ -542,8 +427,6 @@ def _router_kernels(logits, grid, counts, alive, alpha):
 @pytest.mark.parametrize("B", [1, 7, 256, 65536])
 @pytest.mark.parametrize("grid", [(64,), (8, 8), (32, 32), (64, 64), (4, 4, 4, 4)])
 def test_sigmoid_router_loss_kernels_against_float64_autograd(step_counters, grid, B):
-    K.set_step_counters(step_counters)
-    step_counters.zero_()
     dev = torch.device("cuda")
     E_ = math.prod(grid)
     gen = torch.Generator().manual_seed(B + E_)
@@ -569,53 +452,17 @@ def test_sigmoid_router_loss_kernels_against_float64_autograd(step_counters, gri
         del lg, aux, zl, ref
 
 
-def _rel(a, b):
-    a, b = a.detach().float(), b.detach().float()
-    return float((a - b).norm() / b.norm().clamp_min(1e-12))
-
-
-def _layer_against_the_oracle(cfg, grid):
-    ctx = E.EngineContext(cfg)
-    try:
-        layer = E.FusedDMoE(cfg, ctx).cuda().train()
-        oracle = E.FusedDMoE(cfg, device=torch.device("cuda")).cuda().train()
-        oracle.ref_emulate_bf16 = True
-        E_ = math.prod(grid)
-        bias0 = (torch.randint(-8, 9, (E_,)).float() / 16).cuda()
-        with torch.no_grad():
-            layer.expert_bias.copy_(bias0)
-            oracle.load_state_dict(layer.state_dict())
-            oracle.shard.p.copy_(layer.shard.p[:oracle.shard.p.numel()])
-        B = 512
-        x = torch.randn(B, cfg.hidden, device="cuda").to(torch.bfloat16)
-        gy = torch.randn(B, cfg.hidden, device="cuda").to(torch.bfloat16)
-        logits = layer.gate_logits(x, layer.proj).detach()
-        lg = logits.clone().requires_grad_(True)
-        y = E._FusedDMoEFunction.apply(x, lg, layer)
-        y.backward(gy)
-        torch.cuda.synchronize()
-        ctx.check_status()
-        lr_ = logits.clone().requires_grad_(True)
-        yr = oracle._forward_ref(x.float(), lr_, emulate_bf16=True)
-        yr.backward(gy.float())
-        ridx, rw = K.gate_topk_ref(logits, grid, cfg.k, alive=ctx.alive, bias=bias0, score="sigmoid",
-                                   scale=cfg.routed_scaling_factor)
-        got = layer.ws.idx[:B * cfg.k].view(B, cfg.k).long()
-        same = (got == ridx).all(1)
-        assert int((~same).sum()) <= 2, int((~same).sum())   # near-ties of sigma(s) + b may go either way
-        assert float((layer.ws.w[:B * cfg.k].view(B, cfg.k) - rw)[same].abs().max()) < 2e-6 * cfg.routed_scaling_factor
-        counts = torch.bincount(got.flatten(), minlength=E_)
-        assert torch.equal(ctx.cnt_all[0, :E_].long(), counts)
-        assert torch.equal(layer.expert_bias, K.expert_bias_update_ref(ctx.cnt_all[:1, :E_], bias0,
-                                                                       cfg.expert_bias_update_rate))
-        if bool(same.all()):
-            assert torch.equal(layer.expert_bias, oracle.expert_bias)
-        if layer.router_loss is not None:
-            torch.testing.assert_close(layer.router_loss, oracle.router_loss, rtol=1e-3, atol=1e-6)
-            assert float(layer.router_loss[1]) == 0.0
-        assert _rel(y, yr) < 2e-2 and _rel(lg.grad, lr_.grad) < 5e-2, (_rel(y, yr), _rel(lg.grad, lr_.grad))
-    finally:
-        ctx.close()
+def _check(r):
+    """the weights of the tokens routed alike, the bias update of the routed counts, and the sigmoid router's losses"""
+    cfg, E_ = r.layer.cfg, r.layer.cfg.num_experts
+    assert float((r.w - r.rw)[r.same].abs().max()) < 2e-6 * cfg.routed_scaling_factor
+    assert torch.equal(r.layer.expert_bias, K.expert_bias_update_ref(r.ctx.cnt_all[:1, :E_], r.bias0,
+                                                                     cfg.expert_bias_update_rate))
+    if bool(r.same.all()):
+        assert torch.equal(r.layer.expert_bias, r.oracle.expert_bias)
+    if r.layer.router_loss is not None:
+        torch.testing.assert_close(r.layer.router_loss, r.oracle.router_loss, rtol=1e-3, atol=1e-6)
+        assert float(r.layer.router_loss[1]) == 0.0
 
 
 @pytest.mark.gpu
@@ -627,7 +474,7 @@ def test_layer_against_the_cpu_oracle(path, expert, gate):
     grid = (16,) if gate == "emulator" else (4, 4)
     cfg = E.DMoEConfig(hidden=512, grid_size=grid, k=4, num_layers=1, tokens_per_rank=512, expert=expert,
                        expert_path=path, gate_mode=gate, expert_bias_update_rate=0.01, routed_scaling_factor=2.5, **SIG)
-    _layer_against_the_oracle(cfg, grid)
+    layer_against_the_oracle(cfg, max_mismatch=2, check=_check)   # near-ties of sigma(s) + b may go either way
 
 
 @pytest.mark.gpu
@@ -640,7 +487,7 @@ def test_deepseek_v3_shaped_layer_against_the_cpu_oracle(path):
     cfg = E.DMoEConfig(hidden=512, grid_size=grid, k=8, num_layers=1, tokens_per_rank=512, expert="swiglu",
                        inner_dim=256, shared_inner_dim=512, expert_path=path, expert_bias_update_rate=1e-3,
                        router_aux_loss_coef=1e-2, routed_scaling_factor=2.5, **SIG)
-    _layer_against_the_oracle(cfg, grid)
+    layer_against_the_oracle(cfg, max_mismatch=2, check=_check)
 
 
 @pytest.mark.gpu

@@ -7,9 +7,7 @@ implementation, the identities, the gate gradient against float64 autograd, a Sw
 trains only without renormalisation, and checkpoints across the setting.
 GPU: the gate kernel against the normalised kernel and the oracle, gate_bwd against the float64 formula, the wrappers'
 refusals, the layer against the CPU oracle, and the trainer under its CUDA graph."""
-import ctypes
 import math
-from types import SimpleNamespace
 
 import pytest
 import torch
@@ -18,32 +16,19 @@ import lah_b200  # noqa
 from lah_b200.ops import kernels as K
 from lah_b200.parallel import baseline, engine as E
 from lah_b200.parallel.trainer import DMoETrainer
+from routing_support import cpu_cfg, layer_against_the_oracle, run_gate
+from routing_support import one_thread, rt, step_counters, world1  # noqa: F401 (fixtures)
 
 UN = dict(norm_topk_prob=False)
-
-
-@pytest.fixture
-def one_thread():
-    """the CPU trainer tests run many tiny ops: one intra-op thread is faster"""
-    n = torch.get_num_threads()
-    torch.set_num_threads(1)
-    yield
-    torch.set_num_threads(n)
-
-
-def _cpu_cfg(**kw):
-    base = dict(hidden=64, grid_size=(4, 4), k=4, num_layers=1, in_features=16, tokens_per_rank=64, seed=5)
-    base.update(kw)
-    return E.DMoEConfig(**base)
 
 
 # ======================================================================================================== CPU: config
 def test_defaults_and_state_dict_keys():
     assert E.DMoEConfig().norm_topk_prob is True
-    plain, un = E.FusedDMoE(_cpu_cfg()), E.FusedDMoE(_cpu_cfg(routed_scaling_factor=2.5, **UN))
+    plain, un = E.FusedDMoE(cpu_cfg()), E.FusedDMoE(cpu_cfg(routed_scaling_factor=2.5, **UN))
     assert plain.norm_topk_prob and not plain.dense_gate
     assert not un.norm_topk_prob and un.dense_gate and un.routed_scale == 2.5
-    assert not E.FusedDMoE(_cpu_cfg(router_score="sigmoid", **UN)).dense_gate
+    assert not E.FusedDMoE(cpu_cfg(router_score="sigmoid", **UN)).dense_gate
     assert list(plain.state_dict()) == list(un.state_dict())
 
 
@@ -68,9 +53,9 @@ def test_every_setting_accepts_unnormalised_weights(gate, expert, score):
         extra["router_z_loss_coef"] = 1e-3
     if expert == "swiglu":
         extra["shared_inner_dim"] = 128
-    cfg = _cpu_cfg(grid_size=(16,), gate_mode=gate, expert=expert, expert_bias_update_rate=1e-3, failure_rate=0.1,
-                   trainer_microbatches=2, routed_scaling_factor=2.5, router_score=score, n_group=4, topk_group=2,
-                   **UN, **extra)
+    cfg = cpu_cfg(grid_size=(16,), gate_mode=gate, expert=expert, expert_bias_update_rate=1e-3, failure_rate=0.1,
+                  trainer_microbatches=2, routed_scaling_factor=2.5, router_score=score, n_group=4, topk_group=2,
+                  **UN, **extra)
     for path in ("small", "big"):
         E.DMoEConfig(**{**cfg.__dict__, "expert_path": path})
     E.DMoEConfig(**{**cfg.__dict__, "update_every_steps": 2})
@@ -194,7 +179,7 @@ def test_gate_backward_formula_equals_float64_autograd(grid):
 def test_cpu_layer_gate_gradient_against_the_formula():
     torch.manual_seed(0)
     grid = (4, 4)
-    layer = E.FusedDMoE(_cpu_cfg(grid_size=grid, k=2, routed_scaling_factor=2.0, **UN)).train()
+    layer = E.FusedDMoE(cpu_cfg(grid_size=grid, k=2, routed_scaling_factor=2.0, **UN)).train()
     layer.alive_ref = (torch.arange(16) % 5 != 3).to(torch.uint8)
     x = torch.randn(32, 64)
     logits = layer.gate_logits(x, layer.proj).detach().requires_grad_(True)
@@ -218,8 +203,8 @@ def test_cpu_layer_gate_gradient_against_the_formula():
 # ======================================================================================================== CPU: trainer
 def _switch_run(norm, steps=5):
     torch.manual_seed(0)
-    cfg = _cpu_cfg(grid_size=(8,), k=1, gate_mode="product_key", tokens_per_rank=64, weight_decay=0.0,
-                   norm_topk_prob=norm)
+    cfg = cpu_cfg(grid_size=(8,), k=1, gate_mode="product_key", tokens_per_rank=64, weight_decay=0.0,
+                  norm_topk_prob=norm)
     t = DMoETrainer(cfg)
     gen = torch.Generator().manual_seed(1)
     gate0 = [p.detach().clone() for p in t.model.blocks[0].proj.parameters()]
@@ -241,16 +226,16 @@ def test_checkpoints_load_across_the_setting(one_thread):
     gen = torch.Generator().manual_seed(4)
     xs = [torch.randn(64, 16, generator=gen) for _ in range(4)]
     ys = [torch.randint(0, 10, (64,), generator=gen) for _ in range(4)]
-    a = DMoETrainer(_cpu_cfg(num_layers=2, **UN))
+    a = DMoETrainer(cpu_cfg(num_layers=2, **UN))
     for x, y in zip(xs[:2], ys[:2]):
         a.train_step(x, y)
     state = a.state_dict()
-    plain = DMoETrainer(_cpu_cfg(num_layers=2))
+    plain = DMoETrainer(cpu_cfg(num_layers=2))
     assert set(state["trainer"]) == set(plain.state_dict()["trainer"])
     plain.load_state_dict(state)
     for ba, bb in zip(a.model.blocks, plain.model.blocks):
         assert torch.equal(ba.proj.weight, bb.proj.weight) and torch.equal(ba.shard.p, bb.shard.p)
-    back = DMoETrainer(_cpu_cfg(num_layers=2, **UN))
+    back = DMoETrainer(cpu_cfg(num_layers=2, **UN))
     back.load_state_dict(plain.state_dict())
     la = [a.train_step(x, y) for x, y in zip(xs[2:], ys[2:])]
     lb = [back.train_step(x, y) for x, y in zip(xs[2:], ys[2:])]
@@ -258,34 +243,6 @@ def test_checkpoints_load_across_the_setting(one_thread):
 
 
 # ======================================================================================================== GPU
-@pytest.fixture(scope="module")
-def step_counters():
-    """zeroed step counters for this module's direct gate calls; whatever was installed before is put back"""
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    prev = lib.lah_get_epoch_base()
-    ctr = torch.zeros(4, dtype=torch.int32, device="cuda")
-    yield ctr
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev))
-
-
-def _run_gate(logits, grid, k, *, alive, rate, bias, score="softmax", scale=1.0, norm=True, n_group=1, topk_group=1):
-    B = logits.shape[0]
-    idx = torch.full((B * k,), 12345, dtype=torch.int32, device="cuda")
-    pos, w = torch.full_like(idx, 12345), torch.full((B * k,), 7.0, device="cuda")
-    sig = torch.full((B * k,), 7.0, device="cuda") if score == "sigmoid" else None
-    lse = torch.full((B,), 7.0, device="cuda") if score == "softmax" and not norm else None
-    counts = torch.zeros(math.prod(grid), dtype=torch.int32, device="cuda")
-    K.gate_topk(logits, grid, k, alive=alive, failure_rate=rate, seed=99, token_offset=0, idx=idx, w=w, pos=pos,
-                counts=counts, bias=bias, score=score, scale=scale, sig=sig, norm=norm, lse=lse, n_group=n_group,
-                topk_group=topk_group)
-    torch.cuda.synchronize()
-    return idx.view(B, k), w.view(B, k), pos.view(B, k), counts, sig, lse
-
-
 def _grouping(E_):
     g = next(d for d in (8, 5, 4, 3, 2) if E_ % d == 0)
     return g, max(1, g // 2)
@@ -295,8 +252,6 @@ def _grouping(E_):
 @pytest.mark.parametrize("B", [0, 1, 257, 4096])
 @pytest.mark.parametrize("grid", [(64,), (256,), (8, 8), (64, 64), (4096,), (3, 5, 7)])
 def test_gate_against_the_normalised_kernel_and_the_oracle(step_counters, grid, B):
-    K.set_step_counters(step_counters)
-    step_counters.zero_()
     E_ = math.prod(grid)
     gen = torch.Generator(device="cuda").manual_seed(B * 3 + E_)
     if len(grid) <= 2:
@@ -311,8 +266,8 @@ def test_gate_against_the_normalised_kernel_and_the_oracle(step_counters, grid, 
         for score in ("softmax", "sigmoid"):
             for b, (ng, tg) in ((None, (1, 1)), (bias, (1, 1)), (None, (G, M)), (bias, (G, M))):
                 kw = dict(alive=alive, rate=0.1, bias=b, score=score, n_group=ng, topk_group=tg)
-                idx, w, pos, counts, sig, lse = _run_gate(logits, grid, k, scale=c, norm=False, **kw)
-                nidx, _, npos, ncounts, nsig, _ = _run_gate(logits, grid, k, scale=c if score == "sigmoid" else 1.0,
+                idx, w, pos, counts, sig, lse = run_gate(logits, grid, k, scale=c, norm=False, **kw)
+                nidx, _, npos, ncounts, nsig, _ = run_gate(logits, grid, k, scale=c if score == "sigmoid" else 1.0,
                                                            **kw)
                 assert torch.equal(idx, nidx) and torch.equal(pos, npos) and torch.equal(counts, ncounts), (k, score)
                 if sig is not None:
@@ -359,34 +314,12 @@ def test_wrappers_refuse_bad_arguments_before_launching(step_counters):
     assert native.launches() == before
 
 
-@pytest.fixture(scope="module")
-def world1():
-    """a world-1 symmetric heap made directly (no EngineContext) with one receive region, for gate_bwd"""
-    from lah_b200.parallel.symmetric import SymmetricHeap
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    lib = K._lib()
-    lib.lah_get_epoch_base.restype = ctypes.c_void_p
-    prev_ctr = lib.lah_get_epoch_base()
-    heap = SymmetricHeap(64 << 20)
-    region, region_off = heap.alloc((48 << 20,), torch.uint8)
-    w = SimpleNamespace(heap=heap, region=region, region_off=region_off,
-                        step_ctr=torch.zeros(4, dtype=torch.int32, device="cuda"))
-    yield w
-    torch.cuda.synchronize()
-    lib.lah_set_step_counters(ctypes.c_void_p(prev_ctr))
-    heap.close()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("score", ["softmax", "sigmoid"])
 @pytest.mark.parametrize("k", [1, 4, 8])
 @pytest.mark.parametrize("grid,H", [((64,), 256), ((4, 4), 512), ((2, 32), 1024), ((3, 5, 7), 512), ((256,), 1024),
                                     ((64, 64), 512)])
-def test_gate_bwd_against_the_float64_formula(world1, grid, H, k, score):
-    K.set_peers(world1.heap.peer_bases, 0)
-    K.set_multicast(0)
-    K.set_step_counters(world1.step_ctr)
+def test_gate_bwd_against_the_float64_formula(rt, grid, H, k, score):
     gen = torch.Generator().manual_seed(k * H + len(grid))
     B, E_, c = 257, math.prod(grid), 2.5
     logits = torch.randn(B, sum(grid), generator=gen) * 2
@@ -403,7 +336,7 @@ def test_gate_bwd_against_the_float64_formula(world1, grid, H, k, score):
     pair_row = torch.randperm(R, generator=gen)[: B * k].view(B, k)
     pair_row[torch.rand(B, k, generator=gen) < 0.05] = -1   # pairs that scatter_rows dropped
     pair_row = torch.where(valid, pair_row, torch.full_like(pair_row, -1))
-    yo = world1.region[: R * H * 2].view(torch.bfloat16).view(R, H)
+    yo = rt.region[: R * H * 2].view(torch.bfloat16).view(R, H)
     yo.copy_(torch.randn(R, H, generator=gen).to(torch.bfloat16))
     g = torch.randn(B, H, generator=gen).to(torch.bfloat16)
     g[5] = 0                                                  # sum w dw = 0: no gradient at all
@@ -420,7 +353,7 @@ def test_gate_bwd_against_the_float64_formula(world1, grid, H, k, score):
     dl = torch.full((B, sum(grid)), 5.0, device="cuda")
     kw = dict(lse=K.softmax_lse_ref(scores, alive).float().cuda(), alive=alive.cuda(), logits=logits.cuda()) \
         if score == "softmax" else dict(score="sigmoid", sig=sg.float().flatten().cuda())
-    K.gate_bwd(world1.region_off, g.cuda(), idx.flatten().to(torch.int32).cuda(),
+    K.gate_bwd(rt.region_off, g.cuda(), idx.flatten().to(torch.int32).cuda(),
                pair_row.flatten().to(torch.int32).cuda(), w.flatten().cuda(), dl, k, E_, grid, scale=c, norm=False,
                **kw)
     torch.cuda.synchronize()
@@ -429,55 +362,22 @@ def test_gate_bwd_against_the_float64_formula(world1, grid, H, k, score):
     err = float((dl - ref).abs().max() / terms.clamp_min(1e-30))
     assert err < 1e-4, err
     dl2 = torch.full((B, sum(grid)), 5.0, device="cuda")   # deterministic: the same bits again
-    K.gate_bwd(world1.region_off, g.cuda(), idx.flatten().to(torch.int32).cuda(),
+    K.gate_bwd(rt.region_off, g.cuda(), idx.flatten().to(torch.int32).cuda(),
                pair_row.flatten().to(torch.int32).cuda(), w.flatten().cuda(), dl2, k, E_, grid, scale=c, norm=False,
                **kw)
     torch.cuda.synchronize()
     assert torch.equal(dl2.cpu().double(), dl)
 
 
-def _rel(a, b):
-    a, b = a.detach().float(), b.detach().float()
-    return float((a - b).norm() / b.norm().clamp_min(1e-12))
-
-
-def _layer_against_the_oracle(cfg):
-    ctx = E.EngineContext(cfg)
-    try:
-        layer = E.FusedDMoE(cfg, ctx).cuda().train()
-        oracle = E.FusedDMoE(cfg, device=torch.device("cuda")).cuda().train()
-        oracle.ref_emulate_bf16 = True
-        with torch.no_grad():
-            oracle.load_state_dict(layer.state_dict())
-            oracle.shard.p.copy_(layer.shard.p[:oracle.shard.p.numel()])
-        B = 512
-        x = torch.randn(B, cfg.hidden, device="cuda").to(torch.bfloat16)
-        gy = torch.randn(B, cfg.hidden, device="cuda").to(torch.bfloat16)
-        logits = layer.gate_logits(x, layer.proj).detach()
-        lg = logits.clone().requires_grad_(True)
-        y = E._FusedDMoEFunction.apply(x, lg, layer)
-        y.backward(gy)
-        torch.cuda.synchronize()
-        ctx.check_status()
-        lr_ = logits.clone().requires_grad_(True)
-        yr = oracle._forward_ref(x.float(), lr_, emulate_bf16=True)
-        yr.backward(gy.float())
-        ridx, rw = K.gate_topk_ref(logits, cfg.grid_size, cfg.k, alive=ctx.alive, score=cfg.router_score,
-                                   scale=cfg.routed_scaling_factor, n_group=cfg.n_group, topk_group=cfg.topk_group,
-                                   norm=False)
-        got = layer.ws.idx[:B * cfg.k].view(B, cfg.k).long()
-        same = (got == ridx).all(1)
-        assert int((~same).sum()) <= 2, int((~same).sum())
-        gw = layer.ws.w[:B * cfg.k].view(B, cfg.k)
-        assert float(((gw - rw).abs() / rw.abs().clamp_min(1e-30))[same].max()) < 1e-5
-        if layer.dense_gate:
-            rz = K.softmax_lse_ref(K.product_key_scores(logits.double(), cfg.grid_size), ctx.alive)
-            assert float((layer.ws.lse[:B].double() - rz).abs().max()) < 1e-5 * float(rz.abs().max())
-        if layer.router_loss is not None:
-            torch.testing.assert_close(layer.router_loss, oracle.router_loss, rtol=1e-3, atol=1e-6)
-        assert _rel(y, yr) < 2e-2 and _rel(lg.grad, lr_.grad) < 5e-2, (_rel(y, yr), _rel(lg.grad, lr_.grad))
-    finally:
-        ctx.close()
+def _check(r):
+    """the unnormalised weights of the tokens routed alike, the dense gate's log-partition, and the router losses"""
+    cfg, B = r.layer.cfg, r.idx.shape[0]
+    assert float(((r.w - r.rw).abs() / r.rw.abs().clamp_min(1e-30))[r.same].max()) < 1e-5
+    if r.layer.dense_gate:
+        rz = K.softmax_lse_ref(K.product_key_scores(r.logits.double(), cfg.grid_size), r.ctx.alive)
+        assert float((r.layer.ws.lse[:B].double() - rz).abs().max()) < 1e-5 * float(rz.abs().max())
+    if r.layer.router_loss is not None:
+        torch.testing.assert_close(r.layer.router_loss, r.oracle.router_loss, rtol=1e-3, atol=1e-6)
 
 
 @pytest.mark.gpu
@@ -490,7 +390,7 @@ def test_layer_against_the_cpu_oracle(path, expert, gate, score):
     grid = (16,) if gate == "emulator" else (4, 4)
     cfg = E.DMoEConfig(hidden=512, grid_size=grid, k=4, num_layers=1, tokens_per_rank=512, expert=expert,
                        expert_path=path, gate_mode=gate, routed_scaling_factor=2.5, router_score=score, **UN)
-    _layer_against_the_oracle(cfg)
+    layer_against_the_oracle(cfg, max_mismatch=2, check=_check)
 
 
 @pytest.mark.gpu
@@ -500,7 +400,7 @@ def test_switch_shaped_layer_against_the_cpu_oracle(path):
     torch.manual_seed(5)
     cfg = E.DMoEConfig(hidden=512, grid_size=(8, 8), k=1, num_layers=1, tokens_per_rank=512, expert_path=path,
                        router_aux_loss_coef=1e-2, **UN)
-    _layer_against_the_oracle(cfg)
+    layer_against_the_oracle(cfg, max_mismatch=2, check=_check)
 
 
 @pytest.mark.gpu
@@ -511,7 +411,7 @@ def test_deepseek_v2_shaped_layer_against_the_cpu_oracle(path):
     cfg = E.DMoEConfig(hidden=512, grid_size=(8, 8), k=6, num_layers=1, tokens_per_rank=512, expert="swiglu",
                        inner_dim=256, shared_inner_dim=512, expert_path=path, n_group=8, topk_group=3,
                        routed_scaling_factor=16.0, router_aux_loss_coef=1e-2, **UN)
-    _layer_against_the_oracle(cfg)
+    layer_against_the_oracle(cfg, max_mismatch=2, check=_check)
 
 
 @pytest.mark.gpu
